@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the semseg training hot path (BASELINE.json metric: PSPNet50 473x473 training images/sec).
 
-    python bench.py --gpus N --steps K --warmup W            # B200-native arm (this repository)
+    python bench.py --gpus N --steps K --warmup W            # native arm (this repository)
     python bench.py --impl reference --gpus N ...            # reference arm: the reference's OWN modules
                                                              # (baseline/_ref/model/pspnet.py) on the host cores
 
@@ -45,16 +45,24 @@ def parse():
     ap.add_argument("--parity-mode-multi", action="store_true", help="also time the bf16x3 leg when --gpus > 1")
     ap.add_argument("--optimizer", default="torch", choices=["torch", "fused"],
                     help="torch.optim.SGD (the reference's, tool/train.py:140) or semseg_b200.optim.FusedSGD (one launch)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (prediction, losses) as DIR/<name>.npy")
     return ap.parse_args()
+
+
+# H100 SXM data sheet (700 W card): dense BF16 tensor rate and HBM3 bandwidth; used where no measured peaks are given
+H100_BF16_TFLOPS, H100_HBM_GBS = 989.0, 3350.0
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(bf16_tflops=d.get("bf16_tflops", 1590.0), bf16_tflops_sustained=d.get("bf16_tflops_sustained",
-                    1400.0), hbm_gbs=d.get("hbm_gbs", 6650.0), source="measured (MEASURED_PEAKS.json)")
-    return dict(bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, hbm_gbs=6650.0, source="fallback")
+        return dict(bf16_tflops=d.get("bf16_tflops", H100_BF16_TFLOPS), bf16_tflops_sustained=d.get(
+                    "bf16_tflops_sustained", H100_BF16_TFLOPS), hbm_gbs=d.get("hbm_gbs", H100_HBM_GBS),
+                    source="measured (MEASURED_PEAKS.json)")
+    return dict(bf16_tflops=H100_BF16_TFLOPS, bf16_tflops_sustained=H100_BF16_TFLOPS, hbm_gbs=H100_HBM_GBS,
+                source="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
@@ -104,6 +112,26 @@ class ClockSampler(threading.Thread):
                 "samples": len(s)}
 
 
+def dump_outputs(outdir, arrays, budget=64 << 20):
+    """Writes each array as outdir/<name>.npy in float32 (float64 stays float64). Arrays that would take the total past
+    `budget` bytes are replaced by a fixed, seeded sample of their flattened elements (name + "_sample", with the
+    sampled flat indices as name + "_sample_idx")."""
+    import numpy as np
+    os.makedirs(outdir, exist_ok=True)
+    used = 0
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        if used + a.nbytes > budget:
+            k = max(1, min(a.size, (budget - used) // (2 * a.itemsize + 8) if budget > used else 1))
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=k, replace=False))
+            np.save(os.path.join(outdir, name + "_sample_idx.npy"), idx.astype(np.float64))
+            a, name = a.reshape(-1)[idx], name + "_sample"
+            used += idx.nbytes
+        np.save(os.path.join(outdir, name + ".npy"), a)
+        used += a.nbytes
+
+
 def synth_batch(n, size, classes, seed):
     import torch
     g = torch.Generator().manual_seed(seed)
@@ -130,17 +158,7 @@ REF_DIR = os.path.join(ROOT, "baseline", "_ref")
 
 
 def reference_available():
-    """The unmodified reference tree under baseline/_ref (baseline/install_reference.py; git-ignored, travels with the
-    snapshot). In the build container it is (re)created from /root/reference on demand."""
-    if not os.path.isdir(os.path.join(REF_DIR, "model")):
-        try:
-            sys.path.insert(0, os.path.join(ROOT, "baseline"))
-            import install_reference
-            install_reference.install()
-        except Exception:      # noqa: BLE001
-            pass
-        finally:
-            sys.path.pop(0)
+    """The unmodified reference tree under baseline/_ref (git-ignored; put there by baseline/install_reference.py)."""
     return os.path.isdir(os.path.join(REF_DIR, "model"))
 
 
@@ -247,7 +265,7 @@ def run_reference_arm(args):
     print(json.dumps(line), flush=True)
 
 
-# ---------------------------------------------------------------------------------------------------- B200 arm
+# ---------------------------------------------------------------------------------------------------- native arm
 def run_b200_arm(args):
     import torch
     import torch.distributed as dist
@@ -285,12 +303,15 @@ def run_b200_arm(args):
     x_dev, y_dev = x_host.to(dev), y_host.to(dev)
     h2d = x_host.numel() * 4 + y_host.numel() * 8
 
+    last = {}
+
     def step(inp, tgt):
-        _, main_loss, aux_loss = model(inp, tgt)
+        out, main_loss, aux_loss = model(inp, tgt)
         loss = main_loss + 0.4 * aux_loss
         opt.zero_grad()
         loss.backward()
         opt.step()
+        last.update(prediction=out, main_loss=main_loss, aux_loss=aux_loss, loss=loss)
         return loss
 
     def step_e2e():
@@ -327,6 +348,8 @@ def run_b200_arm(args):
     l0 = _lib.launch_count()
     ms_dev = timed(lambda: step(x_dev, y_dev), args.steps)
     launches = _lib.launch_count() - l0
+    if args.dump_outputs and rank == 0:     # before any further step overwrites the (graph-static) outputs
+        dump_outputs(args.dump_outputs, {k: v.detach().float().cpu().numpy() for k, v in last.items()})
     graphed = graphs.launches_per_step(inner)
     if graphed:                      # kernels replayed from the captured step graphs are not counted by the library
         launches += graphed * args.steps
@@ -374,7 +397,7 @@ def run_b200_arm(args):
             ops.conv_fprop(xa, pw.wf, 512, taps, stats=True)
         ts = []
         for _ in range(10):
-            flush.zero_()                       # flush the 126 MB L2 between timed launches
+            flush.zero_()                       # flush the 50 MB L2 between timed launches
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
             ops.conv_fprop(xa, pw.wf, 512, taps, stats=True)
@@ -387,14 +410,8 @@ def run_b200_arm(args):
         roof = {"bound": "tensor", "kernel": "conv_igemm_kernel<256> (cls 3x3 4096->512 fprop, bs%d %dx%d)" % (
                     args.batch, fmap, fmap), "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
                 "frac": ach / pk["bf16_tflops"],
-                # dram__bytes_read.sum + dram__bytes_write.sum of this kernel at this shape from the committed
-                # `ncu --set full` capture of the final build (profiles/r1_ncu_full_final_key_metrics.csv, first row):
-                # 738.1 MB + 72.5 MB per launch; the algorithmic bytes are 510 MB in + 59 MB out.
-                "traffic": 810.6e6 if (args.batch, fmap) == (16, 60) else None, "traffic_unit": "bytes/launch",
-                "traffic_source": "ncu --set full capture of round 1 (profiles/r1_ncu_full_final_key_metrics.csv); the "
-                                  "bf16 instantiation of this kernel and its tiling are unchanged in round 2",
-                "ms_per_launch": t_k, "peak_source": pk["source"] +
-                " burst bf16 (kernel timed alone)"}
+                "ms_per_launch": t_k, "peak_source": pk["source"] + " dense bf16 (kernel timed alone)",
+                "gpu": torch.cuda.get_device_name(dev)}
         del xa, w, pw, flush
 
     if world > 1:
@@ -415,7 +432,7 @@ def run_b200_arm(args):
         "parity_mode": parity,
         "config": {"workload": workload_name(args),
                    "global_batch": args.batch * world, "parallelism": "dp%d" % world,
-                   "l2": "inputs larger than L2: each step streams > 10 GB of activations through the 126 MB L2",
+                   "l2": "inputs larger than L2: each step streams > 10 GB of activations through the 50 MB L2",
                    "optimizer": "%s, momentum 0.9 wd 1e-4, 8 param groups" % (
                        "torch.optim.SGD" if args.optimizer == "torch" else "semseg_b200.optim.FusedSGD (one launch)"),
                    "sync_bn": world > 1,

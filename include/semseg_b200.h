@@ -4,7 +4,7 @@
  * Plain pointers and sizes only: no ATen / pybind types cross this boundary. Every entry point
  * takes device pointers, a cudaStream_t passed as void*, returns 0 on success or a negative
  * SEMSEG_E_* code, and never throws; semseg_last_error() returns the message of the last failure
- * on the calling thread. All kernels are sm_100a-only; there is no CPU fallback behind this ABI.
+ * on the calling thread. All kernels are sm_90a-only; there is no CPU fallback behind this ABI.
  *
  * What each group replaces in the reference (paths relative to the hszhao/semseg tree):
  *   - semseg_psamask_*        : lib/psa/src/gpu/operator.h:3-4 (psamask_forward_cuda / psamask_backward_cuda,
@@ -76,7 +76,7 @@ int semseg_psa_attend_bwd_attn(int psa_type, const float* attn, int a_pitch, con
                                int mH, int mW, int C, float scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Implicit-GEMM convolution on tcgen05 tensor cores (bf16 operands, fp32 accumulation in TMEM).
+ * Implicit-GEMM convolution on wgmma tensor cores (bf16 operands, fp32 accumulation in registers).
  *
  * One descriptor drives fprop and dgrad (dgrad = fprop of dY with the transposed/flipped packed
  * weights). The output pixel grid is [N, H, W]; tap t reads input pixel

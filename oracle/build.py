@@ -6,7 +6,7 @@
                   torch.utils.cpp_extension (the files include <torch/torch.h>, so torch's headers are needed;
                   no other external dependency, no build system of the reference is run).
   build_ref_gpu(): likewise lib/psa/src/gpu/{operator.cpp,psamask_cuda.cu} -> oracle/_ref/psamask_ref_gpu.so (nvcc
-                  cross-compiles for sm_100 without a GPU): the checker of tests/test_validate_path_gpu.py and the
+                  cross-compiles for sm_90 without a GPU): the checker of tests/test_validate_path_gpu.py and the
                   baseline of tools/bench_psamask.py.
 """
 import os
@@ -48,7 +48,7 @@ def build_ref(verbose=False):
 
 def build_ref_gpu(verbose=False):
     """The reference's own CUDA extension (lib/psa/src/gpu/{operator.cpp,psamask_cuda.cu} — "the kernel the rewrite must
-    beat", SURVEY.md §2.1) cross-compiled for sm_100 where the sources lie, into oracle/_ref/psamask_ref_gpu*.so. Used
+    beat", SURVEY.md §2.1) cross-compiled for sm_90 where the sources lie, into oracle/_ref/psamask_ref_gpu*.so. Used
     by tools/bench_psamask.py (a same-box timing of stock vs rewritten kernel) and tests/test_validate_path_gpu.py (bit
     equality). None when /root/reference is absent."""
     gpu_dir = os.path.join(REFERENCE, "lib", "psa", "src", "gpu")
@@ -63,7 +63,7 @@ def build_ref_gpu(verbose=False):
     if found() or not os.path.isdir(gpu_dir):
         return found()
     os.makedirs(ref_dir, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     from torch.utils.cpp_extension import load
     load(name="psamask_ref_gpu",
          sources=[os.path.join(gpu_dir, "operator.cpp"), os.path.join(gpu_dir, "psamask_cuda.cu")],

@@ -1,3 +1,3 @@
-"""semseg_b200 — B200-native (sm_100a) implementation of the dense-prediction training hot path of
+"""semseg_b200 — H100-native (sm_90a) implementation of the dense-prediction training hot path of
 hszhao/semseg: PSPNet / PSANet on a dilated ResNet, hand-written CUDA behind a C-ABI (include/semseg_b200.h)."""
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-"""Build libsemseg_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libsemseg_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 The library has no torch / pybind dependency: it is compiled straight from semseg_b200/csrc/*.cu and
 loaded through ctypes (semseg_b200/_lib.py). nvcc cross-compiles without a GPU, so this runs on the
@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(OUT_DIR, "libsemseg_b200.so")
 BUILD_DIR = os.path.join(HERE, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -76,7 +76,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

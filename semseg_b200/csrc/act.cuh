@@ -3,7 +3,7 @@
 //   plain : one bf16 NHWC tensor (the speed configuration, "bf16").
 //   split : two bf16 NHWC planes (hi, lo) with the same pitch whose fp32 sum is the value: hi = bf16(v),
 //           lo = bf16(v - hi) -> 16 mantissa bits. The convolution kernels consume the planes as extra K segments
-//           (x_hi*w_hi + x_lo*w_hi + x_hi*w_lo, fp32 accumulation in TMEM: the error-compensated "bf16x3" operand
+//           (x_hi*w_hi + x_lo*w_hi + x_hi*w_lo, fp32 accumulation in registers: the error-compensated "bf16x3" operand
 //           mode, SURVEY.md §7 hard part 1), which is what lets the path meet north_star's 1e-3 / exact-argmax
 //           parity with the fp32 reference (model/resnet.py:63-92 computes in fp32 / TF32).
 //

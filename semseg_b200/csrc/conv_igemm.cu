@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution (fprop and dgrad) for NHWC bf16 activations on tcgen05 tensor cores.
+// Implicit-GEMM convolution (fprop and dgrad) for NHWC bf16 activations on sm_90a tensor cores (wgmma).
 //
 //   out[p, co] = sum_t sum_ci x[p + off(t), ci] * w[t][co][ci]
 //
@@ -7,17 +7,14 @@
 //
 // Replaces the cuDNN convolutions behind nn.Conv2d in the reference (model/resnet.py:63-69,
 // model/pspnet.py:49-58,65-69,73-77). One persistent CTA per SM, warp-specialised:
-//   warp 0   : TMA producer   — A tile = 4-D box [64 ch, bw, bh, 1] at the tap-shifted pixel
-//                               (TMA zero-fills the halo), B tile = 3-D box [64, BLOCK_N, 1] of the
-//                               packed weights; both land in 128B-swizzled shared memory.
-//   warp 1   : MMA issuer     — one elected thread issues tcgen05.mma (M=128, N=BLOCK_N, K=16),
-//                               accumulators live in TMEM (2 stages so the epilogue overlaps the next tile).
-//   warps 2-5: epilogue       — tcgen05.ld -> registers -> (affine / ReLU / residual) -> bf16 ->
-//   (+ 6-9)                     swizzled smem -> TMA store; running BatchNorm statistics (sum, sum of squares,
-//                               count per channel) of the stored bf16 values, one row per TMEM lane quarter.
-//                               With kEpiGroups = 2 a second warpgroup takes every other 64-column chunk of the
-//                               tile (own staging buffer, own named barrier): the 1x1 convs with wide outputs are
-//                               epilogue-bound and a single warp per scheduler cannot hide its own latencies.
+//   warpgroup 0   : TMA producer (one elected thread) — A tile = 4-D box [64 ch, bw, bh, 1] at the tap-shifted pixel
+//                   (TMA zero-fills the halo), B tile = 3-D box [64, BLOCK_N, 1] of the packed weights; both land in
+//                   128B-swizzled shared memory.
+//   warpgroups 1-2: MMA + epilogue — warpgroup w issues wgmma (M=64, N=BLOCK_N, K=16) on pixel rows [64w, 64w+64) of
+//                   the tile into fp32 register accumulators, then runs the epilogue straight from the registers:
+//                   (affine / ReLU / residual) -> bf16 -> swizzled smem -> TMA store; running BatchNorm statistics
+//                   (sum, sum of squares, count per channel) of the stored bf16 values, one statistics row per
+//                   32 pixel rows of the tile.
 #include "host_common.h"
 #include "ptx.cuh"
 
@@ -25,8 +22,8 @@ namespace sb {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 bytes = one swizzle span
-constexpr int kEpiGroupThreads = 128;  // one epilogue warpgroup = 4 warps = the 4 TMEM lane quarters
-constexpr int conv_threads(int epi_groups) { return 64 + epi_groups * kEpiGroupThreads; }
+constexpr int kConvThreads = 384;   // producer warpgroup + two MMA / epilogue warpgroups
+constexpr int kConsumerThreads = 256;
 constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KB
 constexpr int kStageOutBytes = kBlockM * 64 * 2;    // 16 KB epilogue staging chunk (64 columns)
 constexpr int kMiscBytes = 2048;
@@ -36,11 +33,7 @@ struct ConvCfg {
   static constexpr int kBTileBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = kATileBytes + kBTileBytes;
   static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128 ? 6 : 8);
-  static constexpr int kTmemCols = 2 * BLOCK_N;  // two accumulator stages
   static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kStageOutBytes + kMiscBytes + 1024;
-  // CTA-pair mode: each CTA stages its own 128 pixel rows of A and HALF of the weight rows -> smaller stages, more of them
-  static constexpr int kPairStageBytes = kATileBytes + kBTileBytes / 2;
-  static constexpr int kPairStages = (kStages * kStageBytes) / kPairStageBytes;
 };
 
 struct ConvKParams {
@@ -61,67 +54,45 @@ struct ConvKParams {
   int nseg;  // operand segments per K block: 1 = bf16, 3 = bf16x3 (x_hi*w_hi, x_lo*w_hi, x_hi*w_lo)
   // K slicing (F32 epilogue only): work item = (pixel tile, channel tile, K slice); slice s accumulates K blocks
   // [s*kb_per_slice, (s+1)*kb_per_slice) and writes its fp32 partial to out_f32 + s*slice_stride. Bounds the length of
-  // one tensor-core accumulation chain: tcgen05 accumulates in fp32 with truncation, a bias of ~2^-24 per MMA step
-  // towards zero (tools/probe_accum.py), negligible for bf16 but not at the 1e-5 level the bf16x3 mode works at.
+  // one tensor-core accumulation chain: the tensor core accumulates in fp32 with truncation, a bias of ~2^-24 per MMA
+  // step towards zero, negligible for bf16 but not at the 1e-5 level the bf16x3 mode works at.
   int k_slices, kb_per_slice;
   long long slice_stride;
   float* out_f32;
   int out_pitch;
-  float* stats_partial;  // [gridDim.x * 4][3][Cout]: per epilogue warp (sum, sum of squares, count) per channel
+  float* stats_partial;  // [gridDim.x * 4][3][Cout]: per 32 pixel rows of the tile (sum, sum of squares, count)
 };
 
-// kCluster (CTA pair, tcgen05 cta_group::2): two CTAs of a cluster own two neighbouring pixel tiles of the SAME channel
-// block and execute ONE M=256 x N=BLOCK_N MMA per K step, issued by the leader CTA. Each CTA stages only its own 128
-// pixel rows of A and HALF of the weight rows (the tensor core reads the other half from the peer's shared memory), so
-// the operand bytes that cross L2->SM per FLOP drop by a third (16 KB + 16 KB instead of 16 KB + 32 KB per K block at
-// BLOCK_N=256) and the freed smem buys more pipeline stages. TMA completions of both CTAs are credited to the leader's
-// full barrier; the leader's tcgen05.commit is multicast to both CTAs' empty / tmem_full barriers; the peer's epilogue
-// hands its accumulator stage back by arriving on the leader's tmem_empty barrier.
-//
 // kSplit (bf16x3 operand mode, activations stored as hi/lo bf16 planes — act.cuh): every K block is issued three times,
-// (x_hi, w_hi), (x_lo, w_hi), (x_hi, w_lo), into the same fp32 TMEM accumulator; the producer just picks the hi or lo
-// tensor map per segment, the MMA warp is unchanged. The epilogue splits its fp32 result into (hi, lo) again and stores
+// (x_hi, w_hi), (x_lo, w_hi), (x_hi, w_lo), into the same fp32 accumulator; the producer just picks the hi or lo
+// tensor map per segment, the MMA loop is unchanged. The epilogue splits its fp32 result into (hi, lo) again and stores
 // both planes (two staging tiles, two TMA stores); BatchNorm statistics are taken from hi + lo.
-template <int BLOCK_N, bool kCluster, int kEpiGroups, bool kSplit>
-__global__ void __launch_bounds__(conv_threads(kEpiGroups), 1)
+template <int BLOCK_N, bool kSplit>
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA_lo,
                   const __grid_constant__ CUtensorMap tmB_lo, const __grid_constant__ CUtensorMap tmC_lo,
                   const ConvKParams p) {
-  static_assert(!kSplit || kEpiGroups == 1, "split storage uses both staging buffers of the single epilogue group");
   using Cfg = ConvCfg<BLOCK_N>;
-  constexpr int kNumThreads = conv_threads(kEpiGroups);
-  constexpr int kEpiThreads = kEpiGroups * kEpiGroupThreads;
-  static_assert(kEpiGroups == 1 || kEpiGroups == 2, "one or two epilogue warpgroups");
-  constexpr int kStages = kCluster ? Cfg::kPairStages : Cfg::kStages;
-  constexpr int kStageBytes = kCluster ? Cfg::kPairStageBytes : Cfg::kStageBytes;
-  const uint32_t cta_rank = kCluster ? cluster_ctarank() : 0u;
-  const bool is_leader = cta_rank == 0;
-  // Work items: (pixel tile, channel tile) or, clustered, (pair of pixel tiles, channel tile) per cluster.
-  const int item_first = kCluster ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int item_step = kCluster ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  const int num_items = (kCluster ? ((p.num_m_tiles + 1) >> 1) : p.num_m_tiles) * p.n_tiles * p.k_slices;
-  auto decode_item = [&](int item, int& m_tile, int& n_tile, int& k_slice) -> bool {
+  constexpr int kStages = Cfg::kStages;
+  constexpr int kStageBytes = Cfg::kStageBytes;
+  constexpr int kAcc = BLOCK_N / 2;   // fp32 accumulator registers per thread
+  const int num_items = p.num_m_tiles * p.n_tiles * p.k_slices;
+  auto decode_item = [&](int item, int& m_tile, int& n_tile, int& k_slice) {
     k_slice = item % p.k_slices;
     item /= p.k_slices;
     n_tile = item % p.n_tiles;
-    const int mi = item / p.n_tiles;
-    const int m_raw = kCluster ? 2 * mi + static_cast<int>(cta_rank) : mi;
-    m_tile = m_raw < p.num_m_tiles ? m_raw : p.num_m_tiles - 1;  // odd tail: the second CTA shadows the last tile
-    return m_raw < p.num_m_tiles;
+    m_tile = item / p.n_tiles;
   };
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* stage_base = smem;
-  uint8_t* out_stage = smem + Cfg::kStages * Cfg::kStageBytes;  // 2 x 16 KB (same offset in both modes)
+  uint8_t* out_stage = smem + kStages * kStageBytes;  // 2 x 16 KB
   uint8_t* misc = out_stage + 2 * kStageOutBytes;
   static_assert(kStages <= 16, "barrier area sized for <= 16 stages");
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(misc);
   uint64_t* empty_bar = full_bar + 16;
-  uint64_t* tmem_full = empty_bar + 16;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -131,9 +102,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     kblk0 = k_slice * p.kb_per_slice;
     kblk1 = min(kblk0 + p.kb_per_slice, total_kblk);
   };
-  const uint32_t a_bytes = static_cast<uint32_t>(p.bh * p.bw) * 128u;
-  // bytes credited to a full barrier per stage: own A + whole B, or (pair mode, leader's barrier) both A tiles + both B halves
-  const uint32_t stage_tx = (kCluster ? 2u * a_bytes : a_bytes) + static_cast<uint32_t>(Cfg::kBTileBytes);
+  const uint32_t stage_tx = static_cast<uint32_t>(p.bh * p.bw) * 128u + static_cast<uint32_t>(Cfg::kBTileBytes);
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -146,33 +115,22 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kCluster ? 2 * kEpiThreads : kEpiThreads);  // pair: both CTAs' epilogues
+      mbar_init(&empty_bar[i], kConsumerThreads);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (kCluster) tmem_alloc_2sm<Cfg::kTmemCols>(tmem_ptr);
-    else tmem_alloc<Cfg::kTmemCols>(tmem_ptr);
-  }
-  if (p.stats_partial != nullptr) {  // four statistics rows per CTA: one per epilogue warp (32 accumulator rows each)
+  if (p.stats_partial != nullptr) {  // four statistics rows per CTA: one per 32 pixel rows of the tile
     float* row = p.stats_partial + static_cast<size_t>(blockIdx.x) * 4 * 3 * p.Cout;
-    for (int i = threadIdx.x; i < 4 * 3 * p.Cout; i += kNumThreads) row[i] = 0.f;
+    for (int i = threadIdx.x; i < 4 * 3 * p.Cout; i += kConvThreads) row[i] = 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  if (kCluster) cluster_sync_all();  // both CTAs' barriers are initialised before any remote arrive / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================================================================== TMA producer
-    if (elect_one()) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       int it = 0;
-      for (int item = item_first; item < num_items; item += item_step) {
+      for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
         int m_tile, n_tile, k_slice, kblk0, kblk1;
         decode_item(item, m_tile, n_tile, k_slice);
         slice_range(k_slice, kblk0, kblk1);
@@ -194,173 +152,108 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const CUtensorMap* mB = (kSplit && seg == 2) ? &tmB_lo : &tmB;
           uint8_t* a_dst = stage_base + s * kStageBytes;
           uint8_t* b_dst = a_dst + kATileBytes;
-          if (kCluster) {
-            // both CTAs' loads complete on the LEADER's full barrier; only the leader arms it
-            const uint32_t lead_bar = mapa_u32(&full_bar[s], 0);
-            if (is_leader) mbar_expect_tx(&full_bar[s], stage_tx);
-            tma_load_4d_2sm(a_dst, mA, lead_bar, cb * kBlockK, w0 + p.dw[t], h0 + p.dh[t],
-                            img * p.img_mul + p.img_add[t]);
-            tma_load_3d_2sm(b_dst, mB, lead_bar, cb * kBlockK, n0 + static_cast<int>(cta_rank) * (BLOCK_N / 2),
-                            p.wtap[t]);
-          } else {
-            mbar_expect_tx(&full_bar[s], stage_tx);
-            tma_load_4d(a_dst, mA, &full_bar[s], cb * kBlockK, w0 + p.dw[t], h0 + p.dh[t],
-                        img * p.img_mul + p.img_add[t]);
-            // 3-D weights [taps][rows][cols]: coordinates (k, row, tap)
-            asm volatile(
-                "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-                "%5}], [%2];" ::"r"(smem_u32(b_dst)),
-                "l"(reinterpret_cast<uint64_t>(mB)), "r"(smem_u32(&full_bar[s])), "r"(cb * kBlockK), "r"(n0),
-                "r"(p.wtap[t])
-                : "memory");
-          }
+          mbar_expect_tx(&full_bar[s], stage_tx);
+          tma_load_4d(a_dst, mA, &full_bar[s], cb * kBlockK, w0 + p.dw[t], h0 + p.dh[t],
+                      img * p.img_mul + p.img_add[t]);
+          // 3-D weights [taps][rows][cols]: coordinates (k, row, tap)
+          tma_load_3d(b_dst, mB, &full_bar[s], cb * kBlockK, n0, p.wtap[t]);
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (pair mode: leader CTA only)
-    if ((!kCluster || is_leader) && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(kCluster ? 2 * kBlockM : kBlockM, BLOCK_N, 0, 0);
-      int it = 0;
-      int tile_iter = 0;
-      for (int item = item_first; item < num_items; item += item_step, ++tile_iter) {
-        const int as = tile_iter & 1;
-        const uint32_t apar = (tile_iter >> 1) & 1;
-        mbar_wait(&tmem_empty[as], apar ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * BLOCK_N);
-        int kblk0, kblk1;
-        slice_range((item % p.k_slices), kblk0, kblk1);
-        const int num_kb = (kblk1 - kblk0) * nseg;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t par = (it / kStages) & 1;
-          mbar_wait(&full_bar[s], par);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(stage_base + s * kStageBytes);
-          const uint32_t b_addr = a_addr + kATileBytes;
-          const uint64_t adesc = make_smem_desc_sw128(a_addr, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(b_addr, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            // advance 32 bytes (16 bf16) along K inside the 128-byte swizzle span
-            if (kCluster)
-              umma_bf16_2sm(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2), idesc,
-                            (kb > 0 || k > 0) ? 1u : 0u);
-            else
-              umma_bf16(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2), idesc,
-                        (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          // frees the smem stage once these MMAs have read it (clustered: in both CTAs, the peer multicasts into it)
-          if (kCluster) umma_commit_2sm_mcast(&empty_bar[s], static_cast<uint16_t>(3));
-          else umma_commit(&empty_bar[s]);
-        }
-        // accumulator complete (pair mode: each CTA's epilogue waits on its own tmem_full barrier)
-        if (kCluster) umma_commit_2sm_mcast(&tmem_full[as], static_cast<uint16_t>(3));
-        else umma_commit(&tmem_full[as]);
       }
     }
   } else {
-    // ===================================================================== epilogue (warps 2..5 and, two groups, 6..9)
-    const int g = warp & 3;             // TMEM lane quarter this warp may access (hardware rule: warp id % 4)
-    const int row = g * 32 + lane;      // accumulator row == pixel within the tile
-    const int grp = (warp - 2) >> 2;    // epilogue warpgroup: chunks grp, grp + kEpiGroups, ... of every tile
-    const int et = ((warp - 2) & 3) * 32 + lane;  // 0..127 inside the group
-    const uint32_t bar_id = 1u + static_cast<uint32_t>(grp);
-    int tile_iter = 0;
+    // ===================================================================== MMA + epilogue (warpgroups 1, 2)
+    setmaxnreg_inc<232>();
+    const int ct = threadIdx.x - 128;      // 0..255
+    const int wg = ct >> 7;                // pixel rows [64*wg, 64*wg + 64) of the tile
+    const int wq = (ct >> 5) & 3;          // warp inside the warpgroup
+    const int r_base = wg * 64 + wq * 16 + (lane >> 2);   // accumulator rows r_base and r_base + 8
+    const int cq = 2 * (lane & 3);         // first of the thread's column pair inside every 8 columns
+    int it = 0;
     int store_buf = 0;
-    for (int item = item_first; item < num_items; item += item_step, ++tile_iter) {
-      int m_tile, n_tile, k_slice;
-      const bool tile_live = decode_item(item, m_tile, n_tile, k_slice);
-      if (!tile_live) {  // shadow tile of an odd tail: keep the TMEM handshake, store nothing
-        const int as_ = tile_iter & 1;
-        mbar_wait(&tmem_full[as_], (tile_iter >> 1) & 1);
-        tc_fence_after();
-        tc_fence_before();
-        if (kCluster) mbar_arrive_cluster(mapa_u32(&tmem_empty[as_], 0));
-        else mbar_arrive(&tmem_empty[as_]);
-        continue;
+    float acc[kAcc];
+    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
+      int m_tile, n_tile, k_slice, kblk0, kblk1;
+      decode_item(item, m_tile, n_tile, k_slice);
+      slice_range(k_slice, kblk0, kblk1);
+      const int num_kb = (kblk1 - kblk0) * nseg;
+      // ---- main loop: one wgmma batch (K = 64) per stage; a stage is released once the next batch was issued and
+      // the one reading it has completed
+      int prev_s = -1;
+#pragma unroll
+      for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        const int s = it % kStages;
+        const uint32_t par = (it / kStages) & 1;
+        mbar_wait(&full_bar[s], par);
+        const uint32_t a_addr = smem_u32(stage_base + s * kStageBytes) + static_cast<uint32_t>(wg * 64 * 128);
+        const uint32_t b_addr = smem_u32(stage_base + s * kStageBytes + kATileBytes);
+        const uint64_t adesc = make_wgmma_desc_sw128(a_addr, 16, 1024);
+        const uint64_t bdesc = make_wgmma_desc_sw128(b_addr, 16, 1024);
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k)   // advance 32 bytes (16 bf16) along K inside the 128-byte swizzle span
+          wgmma_bf16<BLOCK_N, 0, 0>(acc, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
+                                    (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        wgmma_fence_operand(acc);
+        if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
       }
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+
+      // ---- epilogue
       const int tiles_per_img = p.tiles_h * p.tiles_w;
       const int img = m_tile / tiles_per_img;
       const int rem = m_tile - img * tiles_per_img;
       const int h0 = (rem / p.tiles_w) * p.bh;
       const int w0 = (rem % p.tiles_w) * p.bw;
       const int n0 = n_tile * BLOCK_N;
-      const int hi = row / p.bw;
-      const int wi = row - hi * p.bw;
-      const bool row_valid = (row < p.bh * p.bw) && (h0 + hi < p.H) && (w0 + wi < p.W);
-      const long long pix = (static_cast<long long>(img) * p.H + (h0 + hi)) * p.W + (w0 + wi);
-      const uint32_t row_msk = __ballot_sync(0xffffffffu, row_valid);  // valid rows of this warp's 32-row group
-      const int as = tile_iter & 1;
-      const uint32_t apar = (tile_iter >> 1) & 1;
-      mbar_wait(&tmem_full[as], apar);
-      tc_fence_after();
-
+      auto row_ok = [&](int r) {
+        const int hi = r / p.bw, wi = r - (r / p.bw) * p.bw;
+        return (r < p.bh * p.bw) && (h0 + hi < p.H) && (w0 + wi < p.W);
+      };
+      auto row_pix = [&](int r) {
+        const int hi = r / p.bw, wi = r - hi * p.bw;
+        return (static_cast<long long>(img) * p.H + (h0 + hi)) * p.W + (w0 + wi);
+      };
+      bool rv[2];
+      long long pix[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        rv[i] = row_ok(r_base + 8 * i);
+        pix[i] = row_pix(r_base + 8 * i);
+      }
       constexpr int kChunks = BLOCK_N / 64;
-#pragma unroll 1
-      for (int ch = grp; ch < kChunks; ch += kEpiGroups) {
+#pragma unroll
+      for (int ch = 0; ch < kChunks; ++ch) {
         const int c0 = n0 + ch * 64;  // first output channel of this chunk
         if (c0 >= p.Cout) break;      // (uniform) nothing to write for padded columns
-        // Prefetch this CTA's running statistics for the chunk's columns now; the read-modify-write below then
-        // does not expose the global-memory latency in the epilogue's critical path.
-        const bool do_stats = p.stats_partial != nullptr && p.epi_mode == SEMSEG_EPI_RAW;
-        float st_old[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        float* st_dst = nullptr;
-        if (do_stats) {  // every epilogue warp owns statistics row (blockIdx.x*4 + g); lane = column pair
-          st_dst = p.stats_partial + (static_cast<size_t>(blockIdx.x) * 4 + g) * 3 * p.Cout + c0 + 2 * lane;
-          st_old[0] = st_dst[0];
-          st_old[1] = st_dst[1];
-          st_old[2] = st_dst[p.Cout];
-          st_old[3] = st_dst[p.Cout + 1];
-          st_old[4] = st_dst[2 * p.Cout];
-          st_old[5] = st_dst[2 * p.Cout + 1];
-        }
-        // Residual operand (AFFINE mode): issue the row's eight 16-byte loads before the TMEM loads so their latency
-        // overlaps with tcgen05.ld instead of sitting in front of the first use.
-        uint4 rres[8];
-        const bool has_res = p.epi_mode == SEMSEG_EPI_AFFINE && p.residual != nullptr && row_valid;
-        if (has_res && !kSplit) {
-          const uint4* rp = reinterpret_cast<const uint4*>(p.residual + pix * p.res_pitch + c0);
-#pragma unroll
-          for (int j8 = 0; j8 < 8; ++j8) rres[j8] = rp[j8];
-        }
-        uint32_t v[2][32];
-        const uint32_t taddr =
-            tmem_base + (static_cast<uint32_t>(g * 32) << 16) + static_cast<uint32_t>(as * BLOCK_N + ch * 64);
-        tmem_ld_32x32(taddr, v[0]);
-        tmem_ld_32x32(taddr + 32, v[1]);
-        tmem_ld_wait();
+        float* a = acc + ch * 32;     // this chunk's 32 registers: a[4j + 2i + e] = (row r_base + 8i, col 8j + cq + e)
 
         if (p.epi_mode == SEMSEG_EPI_F32) {
-          if (row_valid) {
-            float* orow = p.out_f32 + k_slice * p.slice_stride + pix * p.out_pitch;
-            const bool bias = p.shift != nullptr && k_slice == 0;
-            if (c0 + 64 <= p.Cout && (p.out_pitch & 3) == 0) {   // whole chunk inside: 16-byte stores
+          const bool bias = p.shift != nullptr && k_slice == 0;
+          const bool pairs = (p.out_pitch & 1) == 0;
 #pragma unroll
-              for (int j4 = 0; j4 < 16; ++j4) {
-                float4 o;
-                o.x = __uint_as_float(v[j4 >> 3][(4 * j4 + 0) & 31]);
-                o.y = __uint_as_float(v[j4 >> 3][(4 * j4 + 1) & 31]);
-                o.z = __uint_as_float(v[j4 >> 3][(4 * j4 + 2) & 31]);
-                o.w = __uint_as_float(v[j4 >> 3][(4 * j4 + 3) & 31]);
+          for (int i = 0; i < 2; ++i) {
+            if (!rv[i]) continue;
+            float* orow = p.out_f32 + k_slice * p.slice_stride + pix[i] * p.out_pitch;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int c = c0 + 8 * j + cq;
+              float v0 = a[4 * j + 2 * i], v1 = a[4 * j + 2 * i + 1];
+              if (pairs && c + 1 < p.Cout) {
                 if (bias) {
-                  o.x += __ldg(p.shift + c0 + 4 * j4);
-                  o.y += __ldg(p.shift + c0 + 4 * j4 + 1);
-                  o.z += __ldg(p.shift + c0 + 4 * j4 + 2);
-                  o.w += __ldg(p.shift + c0 + 4 * j4 + 3);
+                  v0 += __ldg(p.shift + c);
+                  v1 += __ldg(p.shift + c + 1);
                 }
-                *reinterpret_cast<float4*>(orow + c0 + 4 * j4) = o;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 64; ++j) {
-                const int c = c0 + j;
-                if (c < p.Cout) {
-                  float a = __uint_as_float(v[j >> 5][j & 31]);
-                  if (bias) a += __ldg(p.shift + c);
-                  orow[c] = a;
-                }
+                *reinterpret_cast<float2*>(orow + c) = make_float2(v0, v1);
+              } else {
+                if (c < p.Cout) orow[c] = bias ? v0 + __ldg(p.shift + c) : v0;
+                if (c + 1 < p.Cout) orow[c + 1] = bias ? v1 + __ldg(p.shift + c + 1) : v1;
               }
             }
           }
@@ -368,94 +261,86 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
 
         if (p.epi_mode == SEMSEG_EPI_AFFINE) {
+          const bool has_res = p.residual != nullptr;
 #pragma unroll
-          for (int j8 = 0; j8 < 8; ++j8) {
-            float r[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            if (has_res) {
-              if constexpr (kSplit) {   // hi + lo planes, loaded here (no prefetch: register budget)
-                const long long ro = pix * p.res_pitch + c0 + j8 * 8;
-                const uint4 rh = *reinterpret_cast<const uint4*>(p.residual + ro);
-                const uint4 rl = *reinterpret_cast<const uint4*>(p.residual_lo + ro);
-                const __nv_bfloat162* ph = reinterpret_cast<const __nv_bfloat162*>(&rh);
-                const __nv_bfloat162* pl = reinterpret_cast<const __nv_bfloat162*>(&rl);
+          for (int j = 0; j < 8; ++j) {
+            const int c = c0 + 8 * j + cq;
+            const float sc0 = p.scale ? __ldg(p.scale + c) : 1.f, sc1 = p.scale ? __ldg(p.scale + c + 1) : 1.f;
+            const float sh0 = p.shift ? __ldg(p.shift + c) : 0.f, sh1 = p.shift ? __ldg(p.shift + c + 1) : 0.f;
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 fh = __bfloat1622float2(ph[q]);
-                  const float2 fl = __bfloat1622float2(pl[q]);
-                  r[2 * q] = fh.x + fl.x;
-                  r[2 * q + 1] = fh.y + fl.y;
+            for (int i = 0; i < 2; ++i) {
+              float r0 = 0.f, r1 = 0.f;
+              if (has_res && rv[i]) {
+                const long long ro = pix[i] * p.res_pitch + c;
+                float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.residual + ro));
+                if constexpr (kSplit) {
+                  const float2 fl = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.residual_lo + ro));
+                  f.x += fl.x;
+                  f.y += fl.y;
                 }
-              } else {
-                const uint4 rv = rres[j8];
-                const __nv_bfloat162* rp = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 f = __bfloat1622float2(rp[q]);
-                  r[2 * q] = f.x;
-                  r[2 * q + 1] = f.y;
-                }
+                r0 = f.x;
+                r1 = f.y;
               }
-            }
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int j = j8 * 8 + q;
-              const int c = c0 + j;
-              float a = __uint_as_float(v[j >> 5][j & 31]);
-              const float sc = p.scale ? __ldg(p.scale + c) : 1.f;
-              const float sh = p.shift ? __ldg(p.shift + c) : 0.f;
-              a = fmaf(a, sc, sh) + r[q];
-              if (p.relu) a = fmaxf(a, 0.f);
-              v[j >> 5][j & 31] = __float_as_uint(a);
+              float v0 = fmaf(a[4 * j + 2 * i], sc0, sh0) + r0;
+              float v1 = fmaf(a[4 * j + 2 * i + 1], sc1, sh1) + r1;
+              if (p.relu) {
+                v0 = fmaxf(v0, 0.f);
+                v1 = fmaxf(v1, 0.f);
+              }
+              a[4 * j + 2 * i] = v0;
+              a[4 * j + 2 * i + 1] = v1;
             }
           }
         }
 
-        // registers -> bf16 -> 128B-swizzled staging tile (row = pixel, 64 channels = 128 bytes)
-        // one group: two staging buffers used alternately; two groups: one buffer each
-        // split storage: buffer 0 = hi plane tile, buffer 1 = lo plane tile
-        uint8_t* obuf = out_stage + (kSplit ? 0 : (kEpiGroups == 1 ? store_buf : grp)) * kStageOutBytes;
-        if (et == 0) tma_store_wait_read<((kEpiGroups == 1 && !kSplit) ? 1 : 0)>();  // the store(s) that last read the buffer(s) drained
-        named_bar_sync(bar_id, kEpiGroupThreads);
+        // registers -> bf16 -> 128B-swizzled staging tile (row = pixel, 64 channels = 128 bytes); the two staging
+        // buffers are used alternately (split storage: buffer 0 = hi plane tile, buffer 1 = lo plane tile)
+        uint8_t* obuf = out_stage + (kSplit ? 0 : store_buf) * kStageOutBytes;
+        if (ct == 0) tma_store_wait_read<(kSplit ? 0 : 1)>();  // the store(s) that last read the buffer(s) drained
+        named_bar_sync(1, kConsumerThreads);
 #pragma unroll
-        for (int j8 = 0; j8 < 8; ++j8) {
-          uint4 o;
-          const int b = j8 * 8;
-          o.x = pack_bf16x2(__uint_as_float(v[b >> 5][(b + 0) & 31]), __uint_as_float(v[b >> 5][(b + 1) & 31]));
-          o.y = pack_bf16x2(__uint_as_float(v[b >> 5][(b + 2) & 31]), __uint_as_float(v[b >> 5][(b + 3) & 31]));
-          o.z = pack_bf16x2(__uint_as_float(v[b >> 5][(b + 4) & 31]), __uint_as_float(v[b >> 5][(b + 5) & 31]));
-          o.w = pack_bf16x2(__uint_as_float(v[b >> 5][(b + 6) & 31]), __uint_as_float(v[b >> 5][(b + 7) & 31]));
-          *reinterpret_cast<uint4*>(obuf + row * 128 + ((j8 ^ (row & 7)) << 4)) = o;
-          if constexpr (kSplit) {   // lo = value - float(hi), staged in the second buffer
-            const __nv_bfloat162* hp = reinterpret_cast<const __nv_bfloat162*>(&o);
-            float l[8];
+        for (int j = 0; j < 8; ++j) {
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 hf = __bfloat1622float2(hp[q]);
-              l[2 * q] = __uint_as_float(v[b >> 5][(b + 2 * q) & 31]) - hf.x;
-              l[2 * q + 1] = __uint_as_float(v[b >> 5][(b + 2 * q + 1) & 31]) - hf.y;
+          for (int i = 0; i < 2; ++i) {
+            const int r = r_base + 8 * i;
+            const float v0 = a[4 * j + 2 * i], v1 = a[4 * j + 2 * i + 1];
+            const uint32_t h = pack_bf16x2(v0, v1);
+            const int off = r * 128 + ((j ^ (r & 7)) << 4) + cq * 2;
+            *reinterpret_cast<uint32_t*>(obuf + off) = h;
+            if constexpr (kSplit) {   // lo = value - float(hi), staged in the second buffer
+              const float2 hf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&h));
+              *reinterpret_cast<uint32_t*>(obuf + kStageOutBytes + off) = pack_bf16x2(v0 - hf.x, v1 - hf.y);
             }
-            uint4 ol;
-            ol.x = pack_bf16x2(l[0], l[1]);
-            ol.y = pack_bf16x2(l[2], l[3]);
-            ol.z = pack_bf16x2(l[4], l[5]);
-            ol.w = pack_bf16x2(l[6], l[7]);
-            *reinterpret_cast<uint4*>(obuf + kStageOutBytes + row * 128 + ((j8 ^ (row & 7)) << 4)) = ol;
           }
         }
         fence_proxy_async_smem();
-        if (do_stats) {
-          // Per-column statistics of the bf16 values just staged (exactly what BN-apply will read back). Each warp
-          // reduces the 32 rows it wrote itself (only a __syncwarp away), lane = column pair (one 4-byte word,
-          // conflict-free), one pass of sum and sum of squares, then a read-modify-write of the warp's own running
-          // (sum, sum of squares, count) row in global memory: no cross-warp traffic, fixed order -> deterministic.
-          __syncwarp();
+        named_bar_sync(1, kConsumerThreads);
+        if (ct == 0) {
+          tma_store_4d(&tmC, obuf, c0, w0, h0, img);
+          if (kSplit) tma_store_4d(&tmC_lo, obuf + kStageOutBytes, c0, w0, h0, img);
+          tma_store_commit();
+        }
+        if (p.stats_partial != nullptr && p.epi_mode == SEMSEG_EPI_RAW && wg == (ch & 1)) {
+          // Per-column statistics of the bf16 values just staged (exactly what BN-apply will read back). Warp g of the
+          // warpgroup whose turn it is reduces pixel rows [32g, 32g + 32), lane = column pair (one 4-byte word,
+          // conflict-free), one pass of sum and sum of squares, then a read-modify-write of the CTA's statistics row g
+          // in global memory: no cross-warp traffic, fixed order -> deterministic.
+          const int g = wq;
+          float* st_dst = p.stats_partial + (static_cast<size_t>(blockIdx.x) * 4 + g) * 3 * p.Cout + c0 + 2 * lane;
+          float st_old[6];
+          st_old[0] = st_dst[0];
+          st_old[1] = st_dst[1];
+          st_old[2] = st_dst[p.Cout];
+          st_old[3] = st_dst[p.Cout + 1];
+          st_old[4] = st_dst[2 * p.Cout];
+          st_old[5] = st_dst[2 * p.Cout + 1];
+          const uint32_t row_msk = __ballot_sync(0xffffffffu, row_ok(g * 32 + lane));
           float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
           const uint8_t* base = obuf + (lane & 3) * 4;
           const int chunk16 = lane >> 2;
           auto add_row = [&](int rr, int sw) {  // sw = rr & 7 (the row's swizzle phase)
-            const __nv_bfloat162 bv =
-                *reinterpret_cast<const __nv_bfloat162*>(base + rr * 128 + ((chunk16 ^ sw) << 4));
-            float2 f = __bfloat1622float2(bv);
+            float2 f = __bfloat1622float2(
+                *reinterpret_cast<const __nv_bfloat162*>(base + rr * 128 + ((chunk16 ^ sw) << 4)));
             if constexpr (kSplit) {
               const float2 fl = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(
                   base + kStageOutBytes + rr * 128 + ((chunk16 ^ sw) << 4)));
@@ -491,115 +376,46 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           st_dst[2 * p.Cout] = st_old[4] + nt;
           st_dst[2 * p.Cout + 1] = st_old[5] + nt;
         }
-        named_bar_sync(bar_id, kEpiGroupThreads);
-        if (et == 0) {
-          tma_store_4d(&tmC, obuf, c0, w0, h0, img);
-          if (kSplit) tma_store_4d(&tmC_lo, obuf + kStageOutBytes, c0, w0, h0, img);
-          tma_store_commit();
-        }
         store_buf ^= 1;
       }
-      // all TMEM reads of this accumulator stage are done -> hand it back to the (leader's) MMA warp
-      tc_fence_before();
-      if (kCluster) mbar_arrive_cluster(mapa_u32(&tmem_empty[as], 0));
-      else mbar_arrive(&tmem_empty[as]);
     }
-    if (et == 0) tma_store_wait_all<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (kCluster) cluster_sync_all();  // the peer may still signal my barriers until it is done as well
-  if (warp == 1) {
-    tc_fence_after();
-    if (kCluster) tmem_dealloc_2sm<Cfg::kTmemCols>(tmem_base);
-    else tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+    if (ct == 0) tma_store_wait_all<0>();
   }
 }
 
-static bool cluster_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEMSEG_B200_CLUSTER");
-    v = (e && e[0] == '0') ? 0 : 1;  // CTA-pair mode by default (validated on B200); SEMSEG_B200_CLUSTER=0 disables
-  }
-  return v != 0;
-}
-
-// Grid (= rows of the statistics buffer) and whether the clustered variant is used.
-static int conv_grid(int num_m_tiles, int n_tiles, bool* clustered) {
+// Grid (= 1/4 of the rows of the statistics buffer): one persistent CTA per SM at most.
+static int conv_grid(int num_m_tiles, int n_tiles) {
   const int sms = num_sms();
-  const bool cl = cluster_enabled() && num_m_tiles >= 2;
-  *clustered = cl;
-  if (!cl) {
-    const long long tiles = static_cast<long long>(num_m_tiles) * n_tiles;
-    return static_cast<int>(tiles < sms ? tiles : sms);
-  }
-  const long long items = static_cast<long long>((num_m_tiles + 1) / 2) * n_tiles;  // one per cluster
-  const long long max_clusters = sms / 2;
-  return static_cast<int>(2 * (items < max_clusters ? items : max_clusters));
-}
-
-// Two epilogue warpgroups by default for tiles with >= 2 column chunks (SEMSEG_B200_EPI_GROUPS=1 keeps one).
-static int epi_groups_wanted() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEMSEG_B200_EPI_GROUPS");
-    v = (e && e[0] == '1') ? 1 : 2;
-  }
-  return v;
+  const long long tiles = static_cast<long long>(num_m_tiles) * n_tiles;
+  return static_cast<int>(tiles < sms ? tiles : sms);
 }
 
 struct ConvMaps {
   CUtensorMap a, b, c, a_lo, b_lo, c_lo;
 };
 
-template <int BLOCK_N, int kEpiGroups, bool kSplit>
-static int launch_conv_g(const ConvMaps& tm, const ConvKParams& kp, bool clustered, int grid, cudaStream_t stream) {
+template <int BLOCK_N>
+static int launch_conv(const ConvMaps& tm, const ConvKParams& kp, bool split, int grid, cudaStream_t stream) {
   using Cfg = ConvCfg<BLOCK_N>;
   // the opt-in to > 48 KB of dynamic shared memory is per device: set it once for every device this process uses
   static std::atomic<bool> attr_set[64];
   int dev = 0;
   SB_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, false, kEpiGroups, kSplit>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, true, kEpiGroups, kSplit>,
-                                 cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 Cfg::kSmemBytes));
+    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 Cfg::kSmemBytes));
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
-  constexpr int kThreads = conv_threads(kEpiGroups);
-  if (!clustered) {
-    conv_igemm_kernel<BLOCK_N, false, kEpiGroups, kSplit><<<grid, kThreads, Cfg::kSmemBytes, stream>>>(
-        tm.a, tm.b, tm.c, tm.a_lo, tm.b_lo, tm.c_lo, kp);
-  } else {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    SB_CUDA(cudaLaunchKernelEx(&cfg, conv_igemm_kernel<BLOCK_N, true, kEpiGroups, kSplit>, tm.a, tm.b, tm.c, tm.a_lo,
-                               tm.b_lo, tm.c_lo, kp));
-  }
+  if (split)
+    conv_igemm_kernel<BLOCK_N, true><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(tm.a, tm.b, tm.c, tm.a_lo,
+                                                                                      tm.b_lo, tm.c_lo, kp);
+  else
+    conv_igemm_kernel<BLOCK_N, false><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(tm.a, tm.b, tm.c, tm.a_lo,
+                                                                                       tm.b_lo, tm.c_lo, kp);
   SB_LAUNCHED();
   return SEMSEG_OK;
-}
-
-template <int BLOCK_N>
-static int launch_conv(const ConvMaps& tm, const ConvKParams& kp, bool split, bool clustered, int grid,
-                       cudaStream_t stream) {
-  if (split) return launch_conv_g<BLOCK_N, 1, true>(tm, kp, clustered, grid, stream);
-  if constexpr (BLOCK_N >= 128) {
-    if (epi_groups_wanted() == 2) return launch_conv_g<BLOCK_N, 2, false>(tm, kp, clustered, grid, stream);
-  }
-  return launch_conv_g<BLOCK_N, 1, false>(tm, kp, clustered, grid, stream);
 }
 
 }  // namespace sb
@@ -622,8 +438,8 @@ extern "C" int semseg_conv_stats_rows(int N, int H, int W, int Cout) {
   if (N <= 0 || H <= 0 || W <= 0 || Cout <= 0) return SEMSEG_E_INVALID;
   int bh, bw;
   sb::choose_box(H, W, sb::kBlockM, &bh, &bw);
-  bool clustered;  // four statistics rows per CTA (one per epilogue warp)
-  return 4 * sb::conv_grid(N * sb::cdiv(H, bh) * sb::cdiv(W, bw), sb::cdiv(Cout, conv_block_n(Cout)), &clustered);
+  // four statistics rows per CTA (one per 32 pixel rows of the tile)
+  return 4 * sb::conv_grid(N * sb::cdiv(H, bh) * sb::cdiv(W, bw), sb::cdiv(Cout, conv_block_n(Cout)));
 }
 
 extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
@@ -683,8 +499,7 @@ extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
                  kp.taps * kp.k_chunks, kp.k_slices);
     kp.slice_stride = d->slice_stride;
   }
-  bool clustered = false;
-  const int grid = conv_grid(kp.num_m_tiles, kp.n_tiles * kp.k_slices, &clustered);
+  const int grid = conv_grid(kp.num_m_tiles, kp.n_tiles * kp.k_slices);
 
   // A: input activations [Nin][Hin][Win][x_pitch] viewed as (C, W, H, N)
   ConvMaps tm;
@@ -701,8 +516,7 @@ extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
   {
     uint64_t dims[3] = {(uint64_t)d->w_cols, (uint64_t)d->w_rows, (uint64_t)d->n_wtaps};
     uint64_t str[2] = {(uint64_t)d->w_cols * 2, (uint64_t)d->w_cols * 2 * d->w_rows};
-    // clustered: each CTA loads (and multicasts) half of the weight rows of the tile
-    uint32_t box[3] = {(uint32_t)kBlockK, (uint32_t)(clustered ? block_n / 2 : block_n), 1};
+    uint32_t box[3] = {(uint32_t)kBlockK, (uint32_t)block_n, 1};
     int r = encode_tmap_bf16(&tm.b, d->w, 3, dims, str, box);
     if (r) return r;
     tm.b_lo = tm.b;
@@ -731,8 +545,8 @@ extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
     if (split && (r = encode_tmap_bf16(&tm.c_lo, d->y_lo, 4, dims, str, box))) return r;
   }
   switch (block_n) {
-    case 256: return launch_conv<256>(tm, kp, split, clustered, grid, stream);
-    case 128: return launch_conv<128>(tm, kp, split, clustered, grid, stream);
-    default: return launch_conv<64>(tm, kp, split, clustered, grid, stream);
+    case 256: return launch_conv<256>(tm, kp, split, grid, stream);
+    case 128: return launch_conv<128>(tm, kp, split, grid, stream);
+    default: return launch_conv<64>(tm, kp, split, grid, stream);
   }
 }

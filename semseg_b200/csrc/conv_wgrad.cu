@@ -1,4 +1,4 @@
-// Weight-gradient implicit GEMM on tcgen05:
+// Weight-gradient implicit GEMM on sm_90a tensor cores (wgmma):
 //
 //   dw[t][co][ci] = sum_p dy[p, co] * x[p + off(t), ci]
 //
@@ -11,13 +11,15 @@
 // Work unit = (split, tap, co-tile, ci-tile); a split owns a contiguous range of pixel boxes.
 // K block = one pixel box of <= 64 pixels; the smem rows a box does not cover are zeroed once at kernel
 // start and never written again, so they contribute exact zeros.
+// Warpgroup 0 is the TMA producer; warpgroup 1 + w (w = 0, 1) owns output channels [64w, 64w + 64) of the co tile:
+// wgmma M = 64 x N = BLOCK_N into fp32 registers, then fp32 partials straight from the registers to global memory.
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace sb {
 
-constexpr int kWgThreads = 192;
-constexpr int kWgEpiThreads = 128;
+constexpr int kWgThreads = 384;
+constexpr int kWgConsumerThreads = 256;
 constexpr int kWgBoxPixels = 64;
 constexpr int kWgBoxBytes = kWgBoxPixels * 128;  // one 64-channel x 64-pixel box
 constexpr int kWgABoxes = 2;                      // 128 Cout channels
@@ -28,61 +30,44 @@ struct WgCfg {
   static constexpr int kBBoxes = BN / 64;
   static constexpr int kStageBytes = (kWgABoxes + kBBoxes) * kWgBoxBytes;  // 48 / 32 / 24 KB
   static constexpr int kStages = BN == 256 ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int kTmemCols = 2 * BN;
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 1024;
-  // CTA-pair mode (cta_group::2, M = 256 output channels over two CTAs): each CTA stages its own 128 dy channels and
-  // half of the x channels of the tile.
-  static constexpr int kPairBBoxes = BN / 128;
-  static constexpr int kPairStageBytes = (kWgABoxes + kPairBBoxes) * kWgBoxBytes;
-  static constexpr int kPairStages = (kStages * kStageBytes) / kPairStageBytes;
 };
 
 struct WgradKParams {
   int N, H, W, Cin, Cout, taps;
   int bh, bw, tiles_h, tiles_w, num_boxes;
-  int co_tiles, ci_tiles, n_splits, boxes_per_split, block_n, pair;
+  int co_tiles, ci_tiles, n_splits, boxes_per_split, block_n;
   // Multi-tap units for narrow inputs (Cin <= 128, 3x3): the 256-wide N tile holds `tu` taps x (cin_boxes*64) channels,
   // so the dy tile is loaded once for `tu` taps instead of once per tap (the narrow layers are L2->SM bound).
   int tu, cin_boxes, unit_taps, oob_img;
   int dh[SEMSEG_MAX_TAPS], dw[SEMSEG_MAX_TAPS], img_add[SEMSEG_MAX_TAPS];
   int img_mul;
-  int nseg;    // 1 = bf16 operands; 3 = bf16x3 (dy_hi*x_hi, dy_lo*x_hi, dy_hi*x_lo accumulated in TMEM)
+  int nseg;    // 1 = bf16 operands; 3 = bf16x3 (dy_hi*x_hi, dy_lo*x_hi, dy_hi*x_lo accumulated in registers)
   float* out;  // [n_splits][taps][Cout][Cin]
 };
 
-// kPair: two CTAs of a cluster compute one 256(co) x BN(ci) tile with cta_group::2 MMAs (see conv_igemm.cu): the
-// leader issues the MMAs, both CTAs' TMA loads complete on the leader's full barrier, commits are multicast.
-template <int kWgBlockN, bool kPair>
+template <int kWgBlockN>
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX,
                   const __grid_constant__ CUtensorMap tmDY_lo, const __grid_constant__ CUtensorMap tmX_lo,
                   const WgradKParams p) {
-  constexpr int kWgBBoxes = kPair ? WgCfg<kWgBlockN>::kPairBBoxes : WgCfg<kWgBlockN>::kBBoxes;
-  constexpr int kWgStageBytes = kPair ? WgCfg<kWgBlockN>::kPairStageBytes : WgCfg<kWgBlockN>::kStageBytes;
-  constexpr int kWgStages = kPair ? WgCfg<kWgBlockN>::kPairStages : WgCfg<kWgBlockN>::kStages;
-  constexpr int kWgTmemCols = WgCfg<kWgBlockN>::kTmemCols;
+  constexpr int kWgBBoxes = WgCfg<kWgBlockN>::kBBoxes;
+  constexpr int kWgStageBytes = WgCfg<kWgBlockN>::kStageBytes;
+  constexpr int kWgStages = WgCfg<kWgBlockN>::kStages;
+  constexpr int kAcc = kWgBlockN / 2;
   static_assert(kWgStages <= 16, "barrier area sized for <= 16 stages");
-  const uint32_t cta_rank = kPair ? cluster_ctarank() : 0u;
-  const bool is_leader = cta_rank == 0;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* misc = smem + kWgStages * kWgStageBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(misc);
   uint64_t* empty_bar = full_bar + 16;
-  uint64_t* tmem_full = empty_bar + 16;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // pair mode: p.co_tiles counts 256-channel tiles (one per cluster); this CTA owns the 128-channel half `cta_rank`
   const int units_per_split = p.unit_taps * p.co_tiles * p.ci_tiles;
   const int num_units = units_per_split * p.n_splits;
-  const int unit_first = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int unit_step = kPair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
   const uint32_t box_bytes = static_cast<uint32_t>(p.bh * p.bw) * 128u;
-  // bytes credited to a full barrier per stage (pair: both CTAs' loads land on the leader's barrier)
-  const uint32_t stage_tx = box_bytes * (kWgABoxes + kWgBBoxes) * (kPair ? 2u : 1u);
+  const uint32_t stage_tx = box_bytes * (kWgABoxes + kWgBBoxes);   // bytes credited to a full barrier per stage
 
   // Zero all operand stages once: rows beyond the pixel box stay zero for the whole kernel.
   {
@@ -101,39 +86,27 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     }
     for (int i = 0; i < kWgStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kPair ? 2 * kWgEpiThreads : kWgEpiThreads);
+      mbar_init(&empty_bar[i], kWgConsumerThreads);
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    if (kPair) tmem_alloc_2sm<kWgTmemCols>(tmem_ptr);
-    else tmem_alloc<kWgTmemCols>(tmem_ptr);
-  }
-  tc_fence_before();
   __syncthreads();
-  if (kPair) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   // unit -> (split, tap, co_tile, ci_tile); ci fastest so concurrent CTAs share the dy boxes in L2
   auto decode = [&](int unit, int& split, int& tap, int& co_t, int& ci_t) {
     ci_t = unit % p.ci_tiles;
     int r = unit / p.ci_tiles;
     co_t = r % p.co_tiles;
-    if (kPair) co_t = 2 * co_t + static_cast<int>(cta_rank);  // my 128-channel half of the 256-channel tile
     r /= p.co_tiles;
     tap = r % p.unit_taps;   // tap, or tap group when p.tu > 1
     split = r / p.unit_taps;
   };
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       int it = 0;
-      for (int unit = unit_first; unit < num_units; unit += unit_step) {
+      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         int split, tap, co_t, ci_t;
         decode(unit, split, tap, co_t, ci_t);
         const int b0 = split * p.boxes_per_split;
@@ -152,144 +125,96 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
           const int h0 = (rem / p.tiles_w) * p.bh;
           const int w0 = (rem % p.tiles_w) * p.bw;
           uint8_t* st = smem + s * kWgStageBytes;
-          if (kPair) {
-            const uint32_t lead_bar = mapa_u32(&full_bar[s], 0);
-            if (is_leader) mbar_expect_tx(&full_bar[s], stage_tx);
+          mbar_expect_tx(&full_bar[s], stage_tx);
 #pragma unroll
-            for (int i = 0; i < kWgABoxes; ++i)
-              tma_load_4d_2sm(st + i * kWgBoxBytes, mDY, lead_bar, co_t * 128 + i * 64, w0, h0, img);
+          for (int i = 0; i < kWgABoxes; ++i)
+            tma_load_4d(st + i * kWgBoxBytes, mDY, &full_bar[s], co_t * 128 + i * 64, w0, h0, img);
+          if (p.tu > 1) {
+#pragma unroll
+            for (int i = 0; i < kWgBBoxes; ++i) {   // box i = (tap of the group, 64-channel block)
+              const int ti = tap * p.tu + i / p.cin_boxes;
+              const bool live = ti < p.taps;        // dead taps of the last group: fully out-of-range box -> zeros
+              const int tt = live ? ti : 0;
+              tma_load_4d(st + (kWgABoxes + i) * kWgBoxBytes, mX, &full_bar[s], (i % p.cin_boxes) * 64,
+                          w0 + p.dw[tt], h0 + p.dh[tt], live ? img * p.img_mul + p.img_add[tt] : p.oob_img);
+            }
+          } else {
 #pragma unroll
             for (int i = 0; i < kWgBBoxes; ++i)
-              tma_load_4d_2sm(st + (kWgABoxes + i) * kWgBoxBytes, mX, lead_bar,
-                              ci_t * kWgBlockN + static_cast<int>(cta_rank) * (kWgBlockN / 2) + i * 64,
-                              w0 + p.dw[tap], h0 + p.dh[tap], img * p.img_mul + p.img_add[tap]);
-          } else {
-            mbar_expect_tx(&full_bar[s], stage_tx);
-#pragma unroll
-            for (int i = 0; i < kWgABoxes; ++i)
-              tma_load_4d(st + i * kWgBoxBytes, mDY, &full_bar[s], co_t * 128 + i * 64, w0, h0, img);
-            if (p.tu > 1) {
-#pragma unroll
-              for (int i = 0; i < kWgBBoxes; ++i) {   // box i = (tap of the group, 64-channel block)
-                const int ti = tap * p.tu + i / p.cin_boxes;
-                const bool live = ti < p.taps;        // dead taps of the last group: fully out-of-range box -> zeros
-                const int tt = live ? ti : 0;
-                tma_load_4d(st + (kWgABoxes + i) * kWgBoxBytes, mX, &full_bar[s], (i % p.cin_boxes) * 64,
-                            w0 + p.dw[tt], h0 + p.dh[tt], live ? img * p.img_mul + p.img_add[tt] : p.oob_img);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < kWgBBoxes; ++i)
-                tma_load_4d(st + (kWgABoxes + i) * kWgBoxBytes, mX, &full_bar[s], ci_t * kWgBlockN + i * 64,
-                            w0 + p.dw[tap], h0 + p.dh[tap], img * p.img_mul + p.img_add[tap]);
-            }
+              tma_load_4d(st + (kWgABoxes + i) * kWgBoxBytes, mX, &full_bar[s], ci_t * kWgBlockN + i * 64,
+                          w0 + p.dw[tap], h0 + p.dh[tap], img * p.img_mul + p.img_add[tap]);
           }
         }
-      }
-    }
-  } else if (warp == 1) {
-    if ((!kPair || is_leader) && elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(kPair ? 256 : 128, kWgBlockN, 1, 1);  // A and B MN-major
-      int it = 0;
-      int unit_iter = 0;
-      for (int unit = unit_first; unit < num_units; unit += unit_step, ++unit_iter) {
-        int split, tap, co_t, ci_t;
-        decode(unit, split, tap, co_t, ci_t);
-        const int b0 = split * p.boxes_per_split;
-        const int b1 = min(b0 + p.boxes_per_split, p.num_boxes);
-        const int as = unit_iter & 1;
-        const uint32_t apar = (unit_iter >> 1) & 1;
-        mbar_wait(&tmem_empty[as], apar ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * kWgBlockN);
-        for (int b = b0 * p.nseg; b < b1 * p.nseg; ++b, ++it) {
-          const int s = it % kWgStages;
-          const uint32_t par = (it / kWgStages) & 1;
-          mbar_wait(&full_bar[s], par);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * kWgStageBytes);
-          const uint32_t b_addr = a_addr + kWgABoxes * kWgBoxBytes;
-          // MN-major SW128: LBO = next 64-channel box, SBO = next 8 pixels (1024 B)
-          const uint64_t adesc = make_smem_desc_sw128(a_addr, kWgBoxBytes, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(b_addr, kWgBoxBytes, 1024);
-#pragma unroll
-          for (int k = 0; k < kWgBoxPixels / 16; ++k) {
-            // 16 pixels along K = 2048 bytes -> +128 in 16-byte units
-            if (kPair)
-              umma_bf16_2sm(d_tmem, adesc + static_cast<uint64_t>(k * 128), bdesc + static_cast<uint64_t>(k * 128),
-                            idesc, (b > b0 * p.nseg || k > 0) ? 1u : 0u);
-            else
-              umma_bf16(d_tmem, adesc + static_cast<uint64_t>(k * 128), bdesc + static_cast<uint64_t>(k * 128), idesc,
-                        (b > b0 * p.nseg || k > 0) ? 1u : 0u);
-          }
-          if (kPair) umma_commit_2sm_mcast(&empty_bar[s], static_cast<uint16_t>(3));
-          else umma_commit(&empty_bar[s]);
-        }
-        if (kPair) umma_commit_2sm_mcast(&tmem_full[as], static_cast<uint16_t>(3));
-        else umma_commit(&tmem_full[as]);
       }
     }
   } else {
-    const int g = warp & 3;
-    const int row = g * 32 + lane;  // Cout index within the tile
-    int unit_iter = 0;
-    for (int unit = unit_first; unit < num_units; unit += unit_step, ++unit_iter) {
+    setmaxnreg_inc<232>();
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7;                 // dy box (64 output channels) of this warpgroup
+    const int wq = (ct >> 5) & 3;
+    const int cq = 2 * (lane & 3);
+    float acc[kAcc];
+    int it = 0;
+    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
       int split, tap, co_t, ci_t;
       decode(unit, split, tap, co_t, ci_t);
-      const int as = unit_iter & 1;
-      const uint32_t apar = (unit_iter >> 1) & 1;
-      mbar_wait(&tmem_full[as], apar);
-      tc_fence_after();
-      const int co = co_t * 128 + row;
+      const int b0 = split * p.boxes_per_split;
+      const int b1 = min(b0 + p.boxes_per_split, p.num_boxes);
+#pragma unroll
+      for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+      int prev_s = -1;
+      for (int b = b0 * p.nseg; b < b1 * p.nseg; ++b, ++it) {
+        const int s = it % kWgStages;
+        const uint32_t par = (it / kWgStages) & 1;
+        mbar_wait(&full_bar[s], par);
+        const uint32_t st = smem_u32(smem + s * kWgStageBytes);
+        // MN-major SW128: LBO = next 64-channel box, SBO = next 8 pixels (1024 B)
+        const uint64_t adesc = make_wgmma_desc_sw128(st + wg * kWgBoxBytes, kWgBoxBytes, 1024);
+        const uint64_t bdesc = make_wgmma_desc_sw128(st + kWgABoxes * kWgBoxBytes, kWgBoxBytes, 1024);
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kWgBoxPixels / 16; ++k)   // 16 pixels along K = 2048 bytes -> +128 in 16-byte units
+          wgmma_bf16<kWgBlockN, 1, 1>(acc, adesc + static_cast<uint64_t>(k * 128),
+                                      bdesc + static_cast<uint64_t>(k * 128), (b > b0 * p.nseg || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        wgmma_fence_operand(acc);
+        if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+        prev_s = s;
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+
       const int ci0 = ci_t * kWgBlockN;
-#pragma unroll 1
-      for (int ch = 0; ch < kWgBlockN / 32; ++ch) {
-        // destination of this 32-column block: (tap, first input channel)
-        int tap_o = tap, ci_o = ci0 + ch * 32;
-        if (p.tu > 1) {
-          const int box = ch >> 1;
-          tap_o = tap * p.tu + box / p.cin_boxes;
-          ci_o = (box % p.cin_boxes) * 64 + (ch & 1) * 32;
-          if (tap_o >= p.taps) continue;
-        }
-        if (ci_o >= p.Cin) {
-          if (p.tu > 1) continue;
-          break;
-        }
-        uint32_t v[32];
-        const uint32_t taddr =
-            tmem_base + (static_cast<uint32_t>(g * 32) << 16) + static_cast<uint32_t>(as * kWgBlockN + ch * 32);
-        tmem_ld_32x32(taddr, v);
-        tmem_ld_wait();
-        if (co < p.Cout) {
-          float* orow = p.out + ((static_cast<size_t>(split) * p.taps + tap_o) * p.Cout + co) * p.Cin + ci_o;
-          if (ci_o + 32 <= p.Cin && (p.Cin & 3) == 0) {
+      const bool pairs = (p.Cin & 1) == 0;
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              float4 f = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]),
-                                     __uint_as_float(v[4 * q + 2]), __uint_as_float(v[4 * q + 3]));
-              *reinterpret_cast<float4*>(orow + 4 * q) = f;
-            }
+      for (int i = 0; i < 2; ++i) {
+        const int co = co_t * 128 + wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
+        if (co >= p.Cout) continue;
+#pragma unroll
+        for (int j = 0; j < kWgBlockN / 8; ++j) {
+          const int col = 8 * j + cq;          // column of the N tile (even)
+          int tap_o = tap, ci = ci0 + col;
+          if (p.tu > 1) {                      // destination of the column: (tap of the group, input channel)
+            const int box = col >> 6;
+            tap_o = tap * p.tu + box / p.cin_boxes;
+            ci = (box % p.cin_boxes) * 64 + (col & 63);
+            if (tap_o >= p.taps) continue;
+          }
+          if (ci >= p.Cin) continue;
+          float* o = p.out + ((static_cast<size_t>(split) * p.taps + tap_o) * p.Cout + co) * p.Cin + ci;
+          const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+          if (pairs && ci + 1 < p.Cin) {
+            *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
           } else {
-#pragma unroll
-            for (int q = 0; q < 32; ++q)
-              if (ci_o + q < p.Cin) orow[q] = __uint_as_float(v[q]);
+            o[0] = v0;
+            if (ci + 1 < p.Cin) o[1] = v1;
           }
         }
       }
-      tc_fence_before();
-      if (kPair) mbar_arrive_cluster(mapa_u32(&tmem_empty[as], 0));
-      else mbar_arrive(&tmem_empty[as]);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (kPair) cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    if (kPair) tmem_dealloc_2sm<kWgTmemCols>(tmem_base);
-    else tmem_dealloc<kWgTmemCols>(tmem_base);
   }
 }
 
@@ -362,16 +287,7 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, int n_splits
   }
 }
 
-static bool wgrad_pair_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEMSEG_B200_CLUSTER");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
-template <int BN, bool kPair>
+template <int BN>
 static int launch_wgrad(const CUtensorMap& tmDY, const CUtensorMap& tmX, const CUtensorMap& tmDY_lo,
                         const CUtensorMap& tmX_lo, const WgradKParams& kp, int grid, cudaStream_t stream) {
   // per-device opt-in to > 48 KB dynamic shared memory (see conv_igemm.cu)
@@ -379,27 +295,11 @@ static int launch_wgrad(const CUtensorMap& tmDY, const CUtensorMap& tmX, const C
   int dev = 0;
   SB_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-    SB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<BN, kPair>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  WgCfg<BN>::kSmemBytes));
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
-  if (!kPair) {
-    conv_wgrad_kernel<BN, false><<<grid, kWgThreads, WgCfg<BN>::kSmemBytes, stream>>>(tmDY, tmX, tmDY_lo, tmX_lo, kp);
-  } else {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kWgThreads);
-    cfg.dynamicSmemBytes = WgCfg<BN>::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    SB_CUDA(cudaLaunchKernelEx(&cfg, conv_wgrad_kernel<BN, true>, tmDY, tmX, tmDY_lo, tmX_lo, kp));
-  }
+  conv_wgrad_kernel<BN><<<grid, kWgThreads, WgCfg<BN>::kSmemBytes, stream>>>(tmDY, tmX, tmDY_lo, tmX_lo, kp);
   return SEMSEG_OK;
 }
 
@@ -412,14 +312,11 @@ static void wgrad_geometry(const semseg_wgrad_desc* d, WgradKParams* kp) {
   kp->co_tiles = cdiv(d->Cout, 128);
   kp->block_n = d->Cin > 128 ? 256 : (d->Cin > 64 ? 128 : 64);
   kp->ci_tiles = cdiv(d->Cin, kp->block_n);
-  // CTA-pair mode needs two 128-channel dy tiles per cluster and a >= 128-channel x tile to halve
-  kp->pair = (wgrad_pair_enabled() && d->Cout > 128 && kp->block_n >= 128) ? 1 : 0;
-  if (kp->pair) kp->co_tiles = cdiv(d->Cout, 256);
   kp->tu = 1;
   kp->cin_boxes = cdiv(d->Cin, 64);
   kp->unit_taps = d->taps;
   kp->oob_img = d->Nin;
-  if (!kp->pair && d->taps > 1 && d->Cin <= 128) {   // narrow 3x3: several taps share one dy tile (N tile = 256)
+  if (d->taps > 1 && d->Cin <= 128) {   // narrow 3x3: several taps share one dy tile (N tile = 256)
     kp->tu = 4 / kp->cin_boxes;
     kp->unit_taps = cdiv(d->taps, kp->tu);
     kp->block_n = 256;
@@ -428,10 +325,9 @@ static void wgrad_geometry(const semseg_wgrad_desc* d, WgradKParams* kp) {
   const int units = kp->unit_taps * kp->co_tiles * kp->ci_tiles;
   int splits = d->n_splits;
   if (splits <= 0) {
-    // Split-K factor: the work units (units x splits) run on `slots` CTAs (clusters in pair mode) in whole rounds, so
-    // the last round should be (nearly) full — 9 taps x 17 splits = 153 units on 74 clusters is 3 rounds at 69 %, x 16 is
-    // 2 rounds at 97 % — while every unit keeps enough K blocks to amortise its pipeline fill / TMEM drain (~8 blocks).
-    const int slots = num_sms() / (kp->pair ? 2 : 1);
+    // Split-K factor: the work units (units x splits) run on `slots` CTAs in whole rounds, so the last round should be
+    // (nearly) full, while every unit keeps enough K blocks to amortise its pipeline fill / drain (~8 blocks).
+    const int slots = num_sms();
     const int max_by_k = kp->num_boxes / 16 > 0 ? kp->num_boxes / 16 : 1;
     const int max_s = max_by_k < 64 ? max_by_k : 64;
     double best = -1.0;
@@ -448,8 +344,8 @@ static void wgrad_geometry(const semseg_wgrad_desc* d, WgradKParams* kp) {
     }
     if (d->x_lo != nullptr) {
       // bf16x3: bound one accumulation chain to 21 pixel boxes (21 x 4 MMA steps x 3 segments = 252 steps): the tensor
-      // core's fp32 accumulation truncates (~2^-24 per step towards zero, tools/probe_accum.py); the fixed-order fp32
-      // reduction of the split partials rounds to nearest.
+      // core's fp32 accumulation truncates (~2^-24 per step towards zero); the fixed-order fp32 reduction of the split
+      // partials rounds to nearest.
       const int need = cdiv(kp->num_boxes, 21);
       if (splits < need) splits = need;
     }
@@ -513,18 +409,11 @@ extern "C" int semseg_conv_wgrad(const semseg_wgrad_desc* d, void* stream_) {
   }
   const int units = kp.unit_taps * kp.co_tiles * kp.ci_tiles * kp.n_splits;
   int rc = SEMSEG_OK;
-  if (kp.pair) {
-    const int max_clusters = num_sms() / 2;
-    const int grid = 2 * (units < max_clusters ? units : max_clusters);
-    rc = kp.block_n == 256 ? launch_wgrad<256, true>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream)
-                           : launch_wgrad<128, true>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream);
-  } else {
-    const int grid = units < num_sms() ? units : num_sms();
-    switch (kp.block_n) {
-      case 256: rc = launch_wgrad<256, false>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream); break;
-      case 128: rc = launch_wgrad<128, false>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream); break;
-      default: rc = launch_wgrad<64, false>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream); break;
-    }
+  const int grid = units < num_sms() ? units : num_sms();
+  switch (kp.block_n) {
+    case 256: rc = launch_wgrad<256>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream); break;
+    case 128: rc = launch_wgrad<128>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream); break;
+    default: rc = launch_wgrad<64>(tmDY, tmX, tmDY_lo, tmX_lo, kp, grid, stream); break;
   }
   if (rc) return rc;
   SB_LAUNCHED();

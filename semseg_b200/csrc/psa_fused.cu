@@ -15,13 +15,14 @@
 //   kStatsRow : the softmax statistics (max, 1/sum) of element (row, k) belong to the row (else to k)
 //     forward  collect: (1,1)   forward distribute: (0,1)   dfeat collect: (0,0)   dfeat distribute: (1,0)
 //
-// CTA = 128 rows (whole grid rows of the HxW map: 4 x 30 = 120 live rows for the shipped 30x30 geometry).
-//   warp 0      : TMA producer of the B operand: feat/dout K blocks [64 pixels x 512 channels] bf16 as eight
-//                 [64 ch, 64 px] boxes = MN-major SWIZZLE_128B operand (exactly the wgrad kernel's operand form)
-//   warp 1      : tcgen05.mma issuer: D[128 x 512 fp32, all 512 TMEM columns] += P[128 x 64] * B[64 x 512]
-//   warps 2..9  : (a) softmax statistics of the CTA's rows (forward), (b) per K block: gather 128 x 64 logits, exp,
-//                 normalise, bf16 -> K-major SWIZZLE_128B A-operand stage in shared memory, (c) epilogue: TMEM -> scale
-//                 -> bf16 (or hi/lo pair) -> global.
+// CTA = a run of <= 64 consecutive pixel positions (rows) of one image. 64 rows x 512 fp32 accumulator columns is half
+// of the register file, so the tile is 64 rows rather than 128.
+//   warpgroup 0    : TMA producer of the B operand (one elected thread): feat/dout K blocks [64 pixels x 512 channels]
+//                    bf16 as eight [64 ch, 64 px] boxes = MN-major SWIZZLE_128B operand (the wgrad kernel's operand form)
+//   warpgroups 1-2 : (a) softmax statistics of the CTA's rows (forward), (b) per K block: gather 64 x 64 logits, exp,
+//                    normalise, bf16 -> K-major SWIZZLE_128B A-operand stage in shared memory, then warpgroup w issues
+//                    wgmma D[64 x 256 fp32 registers] += P[64 x 64] * B[64 x columns 256w..256w+255],
+//                    (c) epilogue: registers -> scale -> bf16 (or hi/lo pair) -> global.
 // bf16x3 (split feat / out): the K loop runs three times (P_hi*B_hi, P_lo*B_hi, P_hi*B_lo) into the same accumulator.
 #include "host_common.h"
 #include "ptx.cuh"
@@ -29,16 +30,16 @@
 
 namespace sb {
 
-constexpr int kPfRows = 128;
+constexpr int kPfRows = 64;
 constexpr int kPfK = 64;
 constexpr int kPfC = 512;                         // channels of feat / out (mid_channels of the PSA module)
 constexpr int kPfBoxBytes = kPfK * 128;           // one [64 ch, 64 px] box
 constexpr int kPfBBytes = (kPfC / 64) * kPfBoxBytes;   // 64 KB
-constexpr int kPfABytes = kPfRows * 128;          // 16 KB
+constexpr int kPfABytes = kPfRows * 128;          // 8 KB
 constexpr int kPfStageBytes = kPfABytes + kPfBBytes;
 constexpr int kPfStages = 2;
-constexpr int kPfWorkers = 256;                   // warps 2..9
-constexpr int kPfThreads = 64 + kPfWorkers;
+constexpr int kPfWorkers = 256;                   // warpgroups 1, 2
+constexpr int kPfThreads = 128 + kPfWorkers;
 constexpr int kPfMisc = 256 + 2 * kPfRows * 4 + 2 * 8 * kPfRows * 4;   // barriers, row stats, per-warp partial stats
 constexpr int kPfSmem = kPfStages * kPfStageBytes + kPfMisc + 1024;
 
@@ -49,7 +50,7 @@ struct PsaFusedParams {
   __nv_bfloat16* out_lo;
   int out_pitch;
   int N, H, W, mH, mW, a_pitch;
-  int rows_per_tile;    // grid rows per CTA tile: 128 / W
+  int tile_rows;        // pixel positions per CTA tile (<= kPfRows)
   int tiles_per_img;
   int nseg;             // 1 (bf16) or 3 (bf16x3)
   float scale;          // 1 / normalization_factor
@@ -69,19 +70,16 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* misc = smem + kPfStages * kPfStageBytes;
   uint64_t* full_b = reinterpret_cast<uint64_t*>(misc);       // TMA bytes of the B tile landed
-  uint64_t* full_a = full_b + kPfStages;                      // all workers wrote the P tile
-  uint64_t* empty = full_a + kPfStages;                       // MMAs that read the stage completed
-  uint64_t* tmem_full = empty + kPfStages;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
-  float* s_m = reinterpret_cast<float*>(misc + 256);          // [128] row max
-  float* s_inv = s_m + kPfRows;                               // [128] row 1/sum
+  uint64_t* empty = full_b + kPfStages;                       // MMAs that read the stage completed
+  float* s_m = reinterpret_cast<float*>(misc + 256);          // [64] row max
+  float* s_inv = s_m + kPfRows;                               // [64] row 1/sum
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x / p.tiles_per_img;
   const int tile = blockIdx.x - n * p.tiles_per_img;
   const int Q = p.H * p.W;
-  const int row_i0 = tile * p.rows_per_tile;                              // first grid row of this tile
-  const int live_rows = min(p.rows_per_tile, p.H - row_i0) * p.W;         // rows of the tile that exist
+  const int pos0 = tile * p.tile_rows;                                   // first pixel position of this tile
+  const int live_rows = min(p.tile_rows, Q - pos0);                      // rows of the tile that exist
   const int hh = (p.mH - 1) / 2, hw = (p.mW - 1) / 2;
   const int num_kb = (Q + kPfK - 1) / kPfK;
   const int total_kb = num_kb * p.nseg;
@@ -93,27 +91,22 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
     if (p.nseg > 1) tma_prefetch_desc(&tmB_lo);
     for (int i = 0; i < kPfStages; ++i) {
       mbar_init(&full_b[i], 1);
-      mbar_init(&full_a[i], kPfWorkers);
-      mbar_init(&empty[i], 1);
+      mbar_init(&empty[i], kPfWorkers);
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  // rows of the 128-row A tile that do not exist in this CTA's tile stay zero for the whole kernel
+  // rows of the 64-row A tile that do not exist in this CTA's tile stay zero for the whole kernel
   for (int s = 0; s < kPfStages; ++s) {
     uint4* a4 = reinterpret_cast<uint4*>(smem + s * kPfStageBytes);
     for (int i = threadIdx.x; i < kPfABytes / 16; i += kPfThreads) a4[i] = make_uint4(0, 0, 0, 0);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================================================================== TMA producer (B operand)
-    if (elect_one()) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       for (int it = 0; it < total_kb; ++it) {
         const int s = it % kPfStages;
         const uint32_t par = (it / kPfStages) & 1;
@@ -123,199 +116,176 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
         uint8_t* dst = smem + s * kPfStageBytes + kPfABytes;
         mbar_expect_tx(&full_b[s], kPfBBytes);
 #pragma unroll
-        for (int bx = 0; bx < kPfC / 64; ++bx) {
-          asm volatile(
-              "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-              "[%2];" ::"r"(smem_u32(dst + bx * kPfBoxBytes)),
-              "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(&full_b[s])), "r"(bx * 64), "r"(kb * kPfK), "r"(n)
-              : "memory");
-        }
+        for (int bx = 0; bx < kPfC / 64; ++bx) tma_load_3d(dst + bx * kPfBoxBytes, m, &full_b[s], bx * 64, kb * kPfK, n);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(kPfRows, 256, 0, 1);   // A K-major, B MN-major
-      for (int it = 0; it < total_kb; ++it) {
-        const int s = it % kPfStages;
-        const uint32_t par = (it / kPfStages) & 1;
-        mbar_wait(&full_b[s], par);
-        mbar_wait(&full_a[s], par);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * kPfStageBytes);
-        const uint32_t b_addr = a_addr + kPfABytes;
-        const uint64_t adesc = make_smem_desc_sw128(a_addr, 16, 1024);
+    return;
+  }
+  // ===================================================================== workers: statistics, P tiles, MMA, epilogue
+  setmaxnreg_inc<232>();
+  const int wt = threadIdx.x - 128;         // 0..255
+  const int ww = wt >> 5;                    // worker warp 0..7
+  // ---- (a) softmax statistics of the tile's rows (forward kernels)
+  if (kStatsRow) {
+    if (kRowOwner) {
+      // collect: row = target, its own attention vector, contiguous along the source column -> one warp per row
+      for (int r = ww; r < kPfRows; r += kPfWorkers / 32) {
+        float m = -INFINITY, sum = 0.f;
+        if (r < live_rows) {
+          const int own = pos0 + r, ri = own / p.W, rj = own - ri * p.W;
+          for (int q = lane; q < Q; q += 32) m = fmaxf(m, pf_logit(An, p.a_pitch, own, ri, rj, q / p.W, q % p.W, hh, hw, p.mH, p.mW));
 #pragma unroll
-        for (int nh = 0; nh < 2; ++nh) {
-          const uint64_t bdesc = make_smem_desc_sw128(b_addr + nh * 4 * kPfBoxBytes, kPfBoxBytes, 1024);
+          for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+          for (int q = lane; q < Q; q += 32)
+            sum += __expf(pf_logit(An, p.a_pitch, own, ri, rj, q / p.W, q % p.W, hh, hw, p.mH, p.mW) - m);
 #pragma unroll
-          for (int k = 0; k < kPfK / 16; ++k)
-            umma_bf16(tmem_base + nh * 256, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 128),
-                      idesc, (it > 0 || k > 0) ? 1u : 0u);
+          for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+          if (lane == 0) stats_n[own] = make_float2(m, 1.f / sum);
         }
-        umma_commit(&empty[s]);
-      }
-      umma_commit(tmem_full);
-    }
-  } else {
-    // ===================================================================== workers: statistics, P tiles, epilogue
-    const int wt = threadIdx.x - 64;          // 0..255
-    const int ww = wt >> 5;                    // worker warp 0..7
-    // ---- (a) softmax statistics of the tile's rows (forward kernels)
-    if (kStatsRow) {
-      if (kRowOwner) {
-        // collect: row = target, its own attention vector, contiguous along the source column -> one warp per row
-        for (int r = ww; r < kPfRows; r += kPfWorkers / 32) {
-          float m = -INFINITY, sum = 0.f;
-          if (r < live_rows) {
-            const int ri = row_i0 + r / p.W, rj = r % p.W, own = ri * p.W + rj;
-            for (int q = lane; q < Q; q += 32) m = fmaxf(m, pf_logit(An, p.a_pitch, own, ri, rj, q / p.W, q % p.W, hh, hw, p.mH, p.mW));
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-            for (int q = lane; q < Q; q += 32)
-              sum += __expf(pf_logit(An, p.a_pitch, own, ri, rj, q / p.W, q % p.W, hh, hw, p.mH, p.mW) - m);
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-            if (lane == 0) stats_n[own] = make_float2(m, 1.f / sum);
-          }
-          if (lane == 0) {
-            s_m[r] = m;
-            s_inv[r] = (r < live_rows) ? 1.f / sum : 0.f;
-          }
-        }
-      } else {
-        // distribute: row = target, one entry of every source vector; consecutive rows read consecutive addresses ->
-        // lanes along rows, the sources split over the 8 worker warps (online softmax), partials merged through smem
-        float* pm = reinterpret_cast<float*>(misc + 256 + 2 * kPfRows * 4);   // [8][128] partial max
-        float* ps = pm + 8 * kPfRows;                                           // [8][128] partial sum
-        const int q_per = (Q + 7) / 8, q0 = ww * q_per, q1 = min(Q, q0 + q_per);
-        for (int r = lane; r < kPfRows; r += 32) {
-          float m = -INFINITY, sum = 0.f;
-          if (r < live_rows) {
-            const int ri = row_i0 + r / p.W, rj = r % p.W;
-            for (int q = q0; q < q1; ++q) {
-              const float l = pf_logit(An, p.a_pitch, q, q / p.W, q % p.W, ri, rj, hh, hw, p.mH, p.mW);
-              const float mn = fmaxf(m, l);
-              sum = sum * __expf(m - mn) + __expf(l - mn);
-              m = mn;
-            }
-          }
-          pm[ww * kPfRows + r] = m;
-          ps[ww * kPfRows + r] = sum;
-        }
-        named_bar_sync(1, kPfWorkers);
-        if (wt < kPfRows) {
-          const int r = wt;
-          float m = -INFINITY, sum = 0.f;
-          if (r < live_rows) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) m = fmaxf(m, pm[k * kPfRows + r]);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const float mk = pm[k * kPfRows + r];
-              if (mk > -INFINITY) sum += ps[k * kPfRows + r] * __expf(mk - m);
-            }
-            const int ri = row_i0 + r / p.W, rj = r % p.W;
-            stats_n[ri * p.W + rj] = make_float2(m, 1.f / sum);
-          }
+        if (lane == 0) {
           s_m[r] = m;
           s_inv[r] = (r < live_rows) ? 1.f / sum : 0.f;
         }
       }
+    } else {
+      // distribute: row = target, one entry of every source vector; consecutive rows read consecutive addresses ->
+      // lanes along rows, the sources split over the 8 worker warps (online softmax), partials merged through smem
+      float* pm = reinterpret_cast<float*>(misc + 256 + 2 * kPfRows * 4);   // [8][64] partial max
+      float* ps = pm + 8 * kPfRows;                                           // [8][64] partial sum
+      const int q_per = (Q + 7) / 8, q0 = ww * q_per, q1 = min(Q, q0 + q_per);
+      for (int r = lane; r < kPfRows; r += 32) {
+        float m = -INFINITY, sum = 0.f;
+        if (r < live_rows) {
+          const int pos = pos0 + r, ri = pos / p.W, rj = pos - ri * p.W;
+          for (int q = q0; q < q1; ++q) {
+            const float l = pf_logit(An, p.a_pitch, q, q / p.W, q % p.W, ri, rj, hh, hw, p.mH, p.mW);
+            const float mn = fmaxf(m, l);
+            sum = sum * __expf(m - mn) + __expf(l - mn);
+            m = mn;
+          }
+        }
+        pm[ww * kPfRows + r] = m;
+        ps[ww * kPfRows + r] = sum;
+      }
       named_bar_sync(1, kPfWorkers);
-    }
-    // ---- (b) P tiles
-    for (int it = 0; it < total_kb; ++it) {
-      const int s = it % kPfStages;
-      const uint32_t par = (it / kPfStages) & 1;
-      const int seg = it / num_kb, kb = it - seg * num_kb;
-      mbar_wait(&empty[s], par ^ 1);
-      uint8_t* a_st = smem + s * kPfStageBytes;
-      const bool want_lo = seg == 1;
-      if (kRowOwner) {
-        // the row pixel owns the attention vector -> addresses are contiguous along k: one warp per (row, 32-column
-        // half), lanes along k; the live (row, half) items are dealt round-robin to the 8 worker warps
-        // [forward collect, dfeat distribute]
-        for (int item = ww; item < 2 * live_rows; item += kPfWorkers / 32) {
-          const int r = item >> 1, half = item & 1;
-          const int ri = row_i0 + r / p.W, rj = r % p.W, rpos = ri * p.W + rj;
-          const int kl = half * 32 + lane, q = kb * kPfK + kl;
-          float pv = 0.f;
-          if (q < Q) {
-            const int qi = q / p.W, qj = q - qi * p.W;
-            const float l = pf_logit(An, p.a_pitch, rpos, ri, rj, qi, qj, hh, hw, p.mH, p.mW);
-            if (kStatsRow) {
-              pv = __expf(l - s_m[r]) * s_inv[r];
-            } else {
-              const float2 st = stats_n[q];
-              pv = __expf(l - st.x) * st.y;
-            }
-          }
-          __nv_bfloat16 hi = __float2bfloat16_rn(pv);
-          if (want_lo) hi = __float2bfloat16_rn(pv - __bfloat162float(hi));
-          *reinterpret_cast<__nv_bfloat16*>(a_st + r * 128 + (((kl >> 3) ^ (r & 7)) << 4) + (kl & 7) * 2) = hi;
-        }
-      } else {
-        // the k pixel owns the vector -> addresses are contiguous along the row index: lanes along rows; the
-        // (32-row group, k column) items are dealt round-robin to the 8 worker warps  [forward distribute, dfeat collect]
-        const int row_groups = (live_rows + 31) >> 5;
-        for (int item = ww; item < row_groups * kPfK; item += kPfWorkers / 32) {
-          const int rg = item % row_groups, kl = item / row_groups;
-          const int r = rg * 32 + lane, q = kb * kPfK + kl;
-          if (r >= live_rows) continue;
-          float pv = 0.f;
-          if (q < Q) {
-            const int ri = row_i0 + r / p.W, rj = r % p.W;
-            const int qi = q / p.W, qj = q - qi * p.W;
-            const float l = pf_logit(An, p.a_pitch, q, qi, qj, ri, rj, hh, hw, p.mH, p.mW);
-            if (kStatsRow) {
-              pv = __expf(l - s_m[r]) * s_inv[r];
-            } else {
-              const float2 st = stats_n[q];
-              pv = __expf(l - st.x) * st.y;
-            }
-          }
-          __nv_bfloat16 hi = __float2bfloat16_rn(pv);
-          if (want_lo) hi = __float2bfloat16_rn(pv - __bfloat162float(hi));
-          *reinterpret_cast<__nv_bfloat16*>(a_st + r * 128 + (((kl >> 3) ^ (r & 7)) << 4) + (kl & 7) * 2) = hi;
-        }
-      }
-      fence_proxy_async_smem();
-      mbar_arrive(&full_a[s]);
-    }
-    // ---- (c) epilogue: TMEM -> registers -> scale -> bf16 (hi/lo) -> global
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-    const int g = warp & 3;                    // TMEM lane quarter of this warp (hardware rule: warp id % 4)
-    const int chalf = (warp - 2) >> 2;         // 0: columns 0..255, 1: 256..511
-    const int r = g * 32 + lane;
-    const bool r_ok = r < live_rows;
-    const long long orow = (static_cast<long long>(n) * Q + static_cast<long long>(row_i0) * p.W + r) * p.out_pitch;
-#pragma unroll 1
-    for (int ch = 0; ch < 4; ++ch) {
-      uint32_t v[2][32];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(g * 32) << 16) + static_cast<uint32_t>(chalf * 256 + ch * 64);
-      tmem_ld_32x32(taddr, v[0]);
-      tmem_ld_32x32(taddr + 32, v[1]);
-      tmem_ld_wait();
-      if (r_ok) {
+      if (wt < kPfRows) {
+        const int r = wt;
+        float m = -INFINITY, sum = 0.f;
+        if (r < live_rows) {
 #pragma unroll
-        for (int j8 = 0; j8 < 8; ++j8) {
-          float f[8];
+          for (int k = 0; k < 8; ++k) m = fmaxf(m, pm[k * kPfRows + r]);
 #pragma unroll
-          for (int q = 0; q < 8; ++q) f[q] = __uint_as_float(v[(j8 * 8 + q) >> 5][(j8 * 8 + q) & 31]) * p.scale;
-          const long long o = orow + chalf * 256 + ch * 64 + j8 * 8;
-          if (p.out_lo) act_st8<true>(p.out, p.out_lo, o, f);
-          else act_st8<false>(p.out, nullptr, o, f);
+          for (int k = 0; k < 8; ++k) {
+            const float mk = pm[k * kPfRows + r];
+            if (mk > -INFINITY) sum += ps[k * kPfRows + r] * __expf(mk - m);
+          }
+          stats_n[pos0 + r] = make_float2(m, 1.f / sum);
         }
+        s_m[r] = m;
+        s_inv[r] = (r < live_rows) ? 1.f / sum : 0.f;
       }
     }
-    tc_fence_before();
+    named_bar_sync(1, kPfWorkers);
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
+  // ---- (b) P tiles and MMAs
+  const int wg = wt >> 7;                    // accumulator columns [256 wg, 256 wg + 256)
+  float acc[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  int prev_s = -1;
+  for (int it = 0; it < total_kb; ++it) {
+    const int s = it % kPfStages;
+    const uint32_t par = (it / kPfStages) & 1;
+    const int seg = it / num_kb, kb = it - seg * num_kb;
+    mbar_wait(&empty[s], par ^ 1);
+    uint8_t* a_st = smem + s * kPfStageBytes;
+    const bool want_lo = seg == 1;
+    if (kRowOwner) {
+      // the row pixel owns the attention vector -> addresses are contiguous along k: one warp per (row, 32-column
+      // half), lanes along k; the live (row, half) items are dealt round-robin to the 8 worker warps
+      // [forward collect, dfeat distribute]
+      for (int item = ww; item < 2 * live_rows; item += kPfWorkers / 32) {
+        const int r = item >> 1, half = item & 1;
+        const int rpos = pos0 + r, ri = rpos / p.W, rj = rpos - ri * p.W;
+        const int kl = half * 32 + lane, q = kb * kPfK + kl;
+        float pv = 0.f;
+        if (q < Q) {
+          const int qi = q / p.W, qj = q - qi * p.W;
+          const float l = pf_logit(An, p.a_pitch, rpos, ri, rj, qi, qj, hh, hw, p.mH, p.mW);
+          if (kStatsRow) {
+            pv = __expf(l - s_m[r]) * s_inv[r];
+          } else {
+            const float2 st = stats_n[q];
+            pv = __expf(l - st.x) * st.y;
+          }
+        }
+        __nv_bfloat16 hi = __float2bfloat16_rn(pv);
+        if (want_lo) hi = __float2bfloat16_rn(pv - __bfloat162float(hi));
+        *reinterpret_cast<__nv_bfloat16*>(a_st + r * 128 + (((kl >> 3) ^ (r & 7)) << 4) + (kl & 7) * 2) = hi;
+      }
+    } else {
+      // the k pixel owns the vector -> addresses are contiguous along the row index: lanes along rows; the
+      // (32-row group, k column) items are dealt round-robin to the 8 worker warps  [forward distribute, dfeat collect]
+      const int row_groups = (live_rows + 31) >> 5;
+      for (int item = ww; item < row_groups * kPfK; item += kPfWorkers / 32) {
+        const int rg = item % row_groups, kl = item / row_groups;
+        const int r = rg * 32 + lane, q = kb * kPfK + kl;
+        if (r >= live_rows) continue;
+        float pv = 0.f;
+        if (q < Q) {
+          const int pos = pos0 + r, ri = pos / p.W, rj = pos - ri * p.W;
+          const int qi = q / p.W, qj = q - qi * p.W;
+          const float l = pf_logit(An, p.a_pitch, q, qi, qj, ri, rj, hh, hw, p.mH, p.mW);
+          if (kStatsRow) {
+            pv = __expf(l - s_m[r]) * s_inv[r];
+          } else {
+            const float2 st = stats_n[q];
+            pv = __expf(l - st.x) * st.y;
+          }
+        }
+        __nv_bfloat16 hi = __float2bfloat16_rn(pv);
+        if (want_lo) hi = __float2bfloat16_rn(pv - __bfloat162float(hi));
+        *reinterpret_cast<__nv_bfloat16*>(a_st + r * 128 + (((kl >> 3) ^ (r & 7)) << 4) + (kl & 7) * 2) = hi;
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1, kPfWorkers);           // the whole P tile is in shared memory
+    mbar_wait(&full_b[s], par);
+    const uint32_t a_addr = smem_u32(a_st);
+    const uint64_t adesc = make_wgmma_desc_sw128(a_addr, 16, 1024);
+    const uint64_t bdesc = make_wgmma_desc_sw128(a_addr + kPfABytes + wg * 4 * kPfBoxBytes, kPfBoxBytes, 1024);
+    wgmma_fence_operand(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kPfK / 16; ++k)
+      wgmma_bf16<256, 0, 1>(acc, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 128),
+                            (it > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_fence_operand(acc);
+    if (prev_s >= 0) mbar_arrive(&empty[prev_s]);
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+  // ---- (c) epilogue: registers -> scale -> bf16 (hi/lo) -> global
+  const int wq = (wt >> 5) & 3;
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int r = wq * 16 + (lane >> 2) + 8 * i;
+    if (r >= live_rows) continue;
+    const long long orow = (static_cast<long long>(n) * Q + pos0 + r) * p.out_pitch + wg * 256 + cq;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const float v0 = acc[4 * j + 2 * i] * p.scale, v1 = acc[4 * j + 2 * i + 1] * p.scale;
+      const uint32_t h = pack_bf16x2(v0, v1);
+      *reinterpret_cast<uint32_t*>(p.out + orow + 8 * j) = h;
+      if (p.out_lo) {
+        const float2 hf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&h));
+        *reinterpret_cast<uint32_t*>(p.out_lo + orow + 8 * j) = pack_bf16x2(v0 - hf.x, v1 - hf.y);
+      }
+    }
   }
 }
 
@@ -335,6 +305,13 @@ static int launch_attend(const CUtensorMap& tmB, const CUtensorMap& tmB_lo, cons
   return SEMSEG_OK;
 }
 
+// Pixel positions per CTA tile: `max_rows`, fewer when that leaves SMs idle (`blocks_per_tile` CTAs share a tile).
+static int psa_tile_rows(int N, int Q, int max_rows, int blocks_per_tile) {
+  const long long want = static_cast<long long>(N) * Q * blocks_per_tile / num_sms();
+  if (want >= max_rows) return max_rows;
+  return want < 8 ? 8 : static_cast<int>(want);
+}
+
 }  // namespace sb
 
 // mode 0: out = P * feat (forward; writes stats)      mode 1: dfeat = P^T * dout (backward; reads stats)
@@ -348,7 +325,7 @@ extern "C" int semseg_psa_attend(int mode, int psa_type, const float* attn, int 
   SB_CHECK_ARG(psa_type == 0 || psa_type == 1, "psa_attend: psa_type must be 0 (collect) or 1 (distribute)");
   SB_CHECK_ARG(mH > 0 && mW > 0 && (mH & 1) && (mW & 1) && a_pitch >= mH * mW, "psa_attend: bad mask geometry");
   SB_CHECK_ARG(C == kPfC, "psa_attend: feature width must be %d (got %d)", kPfC, C);
-  SB_CHECK_ARG(W <= kPfRows, "psa_attend: feature maps wider than %d are not supported", kPfRows);
+  SB_CHECK_ARG(W <= 128, "psa_attend: feature maps wider than %d are not supported", 128);
   SB_CHECK_ARG(feat_pitch % 8 == 0 && out_pitch % 8 == 0 && feat_pitch >= C && out_pitch >= C, "psa_attend: bad pitch");
   SB_CHECK_ARG((feat_lo != nullptr) == (out_lo != nullptr), "psa_attend: feat and out must use the same storage form");
   PsaFusedParams p;
@@ -356,15 +333,10 @@ extern "C" int semseg_psa_attend(int mode, int psa_type, const float* attn, int 
   p.A = attn; p.stats = reinterpret_cast<float2*>(stats);
   p.out = static_cast<__nv_bfloat16*>(out); p.out_lo = static_cast<__nv_bfloat16*>(out_lo); p.out_pitch = out_pitch;
   p.N = N; p.H = H; p.W = W; p.mH = mH; p.mW = mW; p.a_pitch = a_pitch;
-  // grid rows per CTA: at most 128 / W, fewer when that leaves SMs idle (the tensor-core work is negligible, the
-  // per-row gather / exp work of the workers is what takes the time)
-  p.rows_per_tile = kPfRows / W;
-  {
-    const int want = (N * H) / num_sms();
-    const int rpt = want < 1 ? 1 : want;
-    if (rpt < p.rows_per_tile) p.rows_per_tile = rpt;
-  }
-  p.tiles_per_img = cdiv(H, p.rows_per_tile);
+  // the tensor-core work is negligible, the per-row gather / exp work of the workers is what takes the time: tiles
+  // shrink below 64 rows when 64 would leave SMs idle
+  p.tile_rows = psa_tile_rows(N, H * W, kPfRows, 1);
+  p.tiles_per_img = cdiv(H * W, p.tile_rows);
   p.nseg = feat_lo ? 3 : 1;
   p.scale = scale;
   CUtensorMap tmB, tmB_lo;
@@ -387,13 +359,14 @@ extern "C" int semseg_psa_attend(int mode, int psa_type, const float* attn, int 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Attention-logit gradient of the fused op (the softmax backward, flash-attention style: nothing [HW x HW] is stored):
-//   dP[t, s] = scale * sum_c dout[t, c] * feat[s, c]                       (GEMM on tcgen05: M = targets, N = sources, K = C)
+//   dP[t, s] = scale * sum_c dout[t, c] * feat[s, c]                       (GEMM on wgmma: M = targets, N = sources, K = C)
 //   D[t]     = sum_c dout[t, c] * out[t, c]            (= sum_s P[t, s] * dP[t, s])
 //   dL[t, s] = P[t, s] * (dP[t, s] - D[t])             P recomputed from the logits and the saved (max, 1/sum)
 //   dA[owner][idx(other - owner)] = dL[t, s]           owner = t (collect) or s (distribute); dA is zero elsewhere (caller
 //                                                      zero-fills it: 74 % of a full 59x59 mask never receives gradient)
-// CTA = 128 target rows; 4 source blocks of 256 (two TMEM accumulator stages: the epilogue of block j overlaps the MMAs of
-// block j+1); operands K-major from TMA ([64 c, 128 rows] of dout, [64 c, 256 rows] of feat), 4-stage ring.
+// CTA = <= 128 consecutive target positions x one block of 256 sources; warpgroup 0 = TMA producer, warpgroup 1 + w
+// computes targets [64w, 64w + 64) with wgmma into registers; operands K-major from TMA ([64 c, 128 rows] of dout,
+// [64 c, 256 rows] of feat), 4-stage ring.
 namespace sb {
 
 constexpr int kPgBlockN = 256;
@@ -401,7 +374,7 @@ constexpr int kPgABytes = 128 * 128;             // [128 rows][64 c] bf16
 constexpr int kPgBBytes = kPgBlockN * 128;       // [256 rows][64 c]
 constexpr int kPgStageBytes = kPgABytes + kPgBBytes;   // 48 KB
 constexpr int kPgStages = 4;
-constexpr int kPgThreads = 64 + 256;
+constexpr int kPgThreads = 384;
 constexpr int kPgSmem = kPgStages * kPgStageBytes + 1024 + 1024;
 
 struct PsaGradParams {
@@ -414,7 +387,7 @@ struct PsaGradParams {
   const __nv_bfloat16* out_lo;
   int dout_pitch, out_pitch;
   int N, H, W, mH, mW, a_pitch, C;
-  int rows_per_tile, tiles_per_img, nseg;
+  int tile_rows, tiles_per_img, nseg;
   float scale;
 };
 
@@ -428,22 +401,18 @@ psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_cons
   uint8_t* misc = smem + kPgStages * kPgStageBytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(misc);
   uint64_t* empty = full + kPgStages;
-  uint64_t* tmem_full = empty + kPgStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x / p.tiles_per_img;
   const int tile = blockIdx.x - n * p.tiles_per_img;
   const int Q = p.H * p.W;
-  const int row_i0 = tile * p.rows_per_tile;
-  const int q_row0 = row_i0 * p.W;                                       // first target position of the tile
-  const int live_rows = min(p.rows_per_tile, p.H - row_i0) * p.W;
+  const int q_row0 = tile * p.tile_rows;                                 // first target position of the tile
+  const int live_rows = min(p.tile_rows, Q - q_row0);
   const int hh = (p.mH - 1) / 2, hw = (p.mW - 1) / 2;
   const int k_blocks = p.C / 64;
   // one 256-source block per CTA (blockIdx.y): the per-element epilogue (recompute P, scatter) dominates, so the source
   // blocks of a target tile run on different SMs
-  const int nb_first = blockIdx.y, nb_last = blockIdx.y + 1;
+  const int nb = blockIdx.y;
   const int per_nb = k_blocks * p.nseg;
 
   if (warp == 0 && lane == 0) {
@@ -451,86 +420,54 @@ psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_cons
     tma_prefetch_desc(&tmF);
     for (int i = 0; i < kPgStages; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 256);
+      mbar_init(&empty[i], 256);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    if (elect_one()) {
-      int it = 0;
-      for (int nb = nb_first; nb < nb_last; ++nb) {
-        for (int kk = 0; kk < per_nb; ++kk, ++it) {
-          const int s = it % kPgStages;
-          const uint32_t par = (it / kPgStages) & 1;
-          mbar_wait(&empty[s], par ^ 1);
-          const int seg = kk / k_blocks, kb = kk - seg * k_blocks;   // 0: do_hi*f_hi, 1: do_lo*f_hi, 2: do_hi*f_lo
-          const CUtensorMap* mA = seg == 1 ? &tmDO_lo : &tmDO;
-          const CUtensorMap* mB = seg == 2 ? &tmF_lo : &tmF;
-          uint8_t* a_dst = smem + s * kPgStageBytes;
-          mbar_expect_tx(&full[s], kPgStageBytes);
-          asm volatile(
-              "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-              "[%2];" ::"r"(smem_u32(a_dst)),
-              "l"(reinterpret_cast<uint64_t>(mA)), "r"(smem_u32(&full[s])), "r"(kb * 64), "r"(q_row0), "r"(n)
-              : "memory");
-          asm volatile(
-              "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], "
-              "[%2];" ::"r"(smem_u32(a_dst + kPgABytes)),
-              "l"(reinterpret_cast<uint64_t>(mB)), "r"(smem_u32(&full[s])), "r"(kb * 64), "r"(nb * kPgBlockN), "r"(n)
-              : "memory");
-        }
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      for (int kk = 0; kk < per_nb; ++kk) {
+        const int s = kk % kPgStages;
+        const uint32_t par = (kk / kPgStages) & 1;
+        mbar_wait(&empty[s], par ^ 1);
+        const int seg = kk / k_blocks, kb = kk - seg * k_blocks;   // 0: do_hi*f_hi, 1: do_lo*f_hi, 2: do_hi*f_lo
+        const CUtensorMap* mA = seg == 1 ? &tmDO_lo : &tmDO;
+        const CUtensorMap* mB = seg == 2 ? &tmF_lo : &tmF;
+        uint8_t* a_dst = smem + s * kPgStageBytes;
+        mbar_expect_tx(&full[s], kPgStageBytes);
+        tma_load_3d(a_dst, mA, &full[s], kb * 64, q_row0, n);
+        tma_load_3d(a_dst + kPgABytes, mB, &full[s], kb * 64, nb * kPgBlockN, n);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc_bf16(128, kPgBlockN, 0, 0);   // both operands K-major
-      int it = 0;
-      for (int nb = nb_first; nb < nb_last; ++nb) {
-        const int as = (nb - nb_first) & 1;
-        mbar_wait(&tmem_empty[as], (((nb - nb_first) >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(as * kPgBlockN);
-        for (int kk = 0; kk < per_nb; ++kk, ++it) {
-          const int s = it % kPgStages;
-          const uint32_t par = (it / kPgStages) & 1;
-          mbar_wait(&full[s], par);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * kPgStageBytes);
-          const uint64_t adesc = make_smem_desc_sw128(a_addr, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(a_addr + kPgABytes, 16, 1024);
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int ct = threadIdx.x - 128;
+  const int wg = ct >> 7, wq = (ct >> 5) & 3;
+  const int cq = 2 * (lane & 3);
+  const float* An = p.A + static_cast<size_t>(n) * Q * p.a_pitch;
+  float* dAn = p.dA + static_cast<size_t>(n) * Q * p.a_pitch;
+  // the thread's two target rows r = 64 wg + 16 wq + lane / 4 + 8 i; D[t] = <dout[t, :], out[t, :]> (the four lanes
+  // that share a row take a quarter of the channels each) and the row's softmax statistics
+  bool r_ok[2];
+  int tpos[2];
+  float D[2], rm[2], rinv[2];
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(d_tmem, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2), idesc,
-                      (kk > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty[s]);
-        }
-        umma_commit(&tmem_full[as]);
-      }
-    }
-  } else {
-    const int g = warp & 3;
-    const int chalf = (warp - 2) >> 2;          // columns [chalf*128, +128) of every 256-source block
-    const int r = g * 32 + lane;
-    const bool r_ok = r < live_rows;
-    const int ti = row_i0 + r / p.W, tj = r % p.W, tpos = ti * p.W + tj;
-    const float* An = p.A + static_cast<size_t>(n) * Q * p.a_pitch;
-    float* dAn = p.dA + static_cast<size_t>(n) * Q * p.a_pitch;
-    // D[t] = <dout[t, :], out[t, :]> and the row's softmax statistics
-    float D = 0.f, rm = 0.f, rinv = 0.f;
-    if (r_ok) {
-      const long long o1 = (static_cast<long long>(n) * Q + tpos) * p.dout_pitch;
-      const long long o2 = (static_cast<long long>(n) * Q + tpos) * p.out_pitch;
-      for (int c = 0; c < p.C; c += 8) {
+  for (int i = 0; i < 2; ++i) {
+    const int r = wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
+    r_ok[i] = r < live_rows;
+    tpos[i] = q_row0 + (r_ok[i] ? r : 0);
+    float d = 0.f;
+    rm[i] = 0.f;
+    rinv[i] = 0.f;
+    if (r_ok[i]) {
+      const long long o1 = (static_cast<long long>(n) * Q + tpos[i]) * p.dout_pitch;
+      const long long o2 = (static_cast<long long>(n) * Q + tpos[i]) * p.out_pitch;
+      const int cpl = p.C / 4;
+      for (int c = (lane & 3) * cpl; c < (lane & 3) * cpl + cpl; c += 8) {
         float a[8], b[8];
         if (p.dout_lo) {
           act_ld8<true>(p.dout, p.dout_lo, o1 + c, a);
@@ -540,50 +477,64 @@ psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_cons
           act_ld8<false>(p.out, nullptr, o2 + c, b);
         }
 #pragma unroll
-        for (int q = 0; q < 8; ++q) D = fmaf(a[q], b[q], D);
+        for (int q = 0; q < 8; ++q) d = fmaf(a[q], b[q], d);
       }
-      const float2 st = p.stats[static_cast<size_t>(n) * Q + tpos];
-      rm = st.x;
-      rinv = st.y;
+      const float2 st = p.stats[static_cast<size_t>(n) * Q + tpos[i]];
+      rm[i] = st.x;
+      rinv[i] = st.y;
     }
-    for (int nb = nb_first; nb < nb_last; ++nb) {
-      const int as = (nb - nb_first) & 1;
-      mbar_wait(&tmem_full[as], ((nb - nb_first) >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(g * 32) << 16) +
-                               static_cast<uint32_t>(as * kPgBlockN + chalf * 128 + ch * 32);
-        tmem_ld_32x32(taddr, v);
-        tmem_ld_wait();
-        if (r_ok) {
-          const int s0 = nb * kPgBlockN + chalf * 128 + ch * 32;
+    d += __shfl_xor_sync(0xffffffffu, d, 1);
+    d += __shfl_xor_sync(0xffffffffu, d, 2);
+    D[i] = d;
+  }
+
+  float acc[128];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int s = s0 + j;
-            if (s >= Q) continue;
-            const int si = s / p.W, sj = s - si * p.W;
-            // owner / other of the attention entry
-            const int oi = kCollect ? ti : si, oj = kCollect ? tj : sj, own = kCollect ? tpos : s;
-            const int a = (kCollect ? si : ti) - oi + hh, b = (kCollect ? sj : tj) - oj + hw;
-            if (a >= 0 && a < p.mH && b >= 0 && b < p.mW) {
-              const size_t off = static_cast<size_t>(own) * p.a_pitch + a * p.mW + b;
-              const float pv = __expf(__ldg(An + off) - rm) * rinv;
-              dAn[off] = pv * (p.scale * __uint_as_float(v[j]) - D);
-            }
-          }
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  int prev_s = -1;
+  for (int kk = 0; kk < per_nb; ++kk) {
+    const int s = kk % kPgStages;
+    const uint32_t par = (kk / kPgStages) & 1;
+    mbar_wait(&full[s], par);
+    const uint32_t a_addr = smem_u32(smem + s * kPgStageBytes);
+    const uint64_t adesc = make_wgmma_desc_sw128(a_addr + wg * 64 * 128, 16, 1024);
+    const uint64_t bdesc = make_wgmma_desc_sw128(a_addr + kPgABytes, 16, 1024);
+    wgmma_fence_operand(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_bf16<kPgBlockN, 0, 0>(acc, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
+                                  (kk > 0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_fence_operand(acc);
+    if (prev_s >= 0) mbar_arrive(&empty[prev_s]);
+    prev_s = s;
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    if (!r_ok[i]) continue;
+    const int tp = tpos[i], ti = tp / p.W, tj = tp - ti * p.W;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int s = nb * kPgBlockN + 8 * j + cq + e;
+        if (s >= Q) continue;
+        const int si = s / p.W, sj = s - si * p.W;
+        // owner / other of the attention entry
+        const int oi = kCollect ? ti : si, oj = kCollect ? tj : sj, own = kCollect ? tp : s;
+        const int a = (kCollect ? si : ti) - oi + hh, b = (kCollect ? sj : tj) - oj + hw;
+        if (a >= 0 && a < p.mH && b >= 0 && b < p.mW) {
+          const size_t off = static_cast<size_t>(own) * p.a_pitch + a * p.mW + b;
+          const float pv = __expf(__ldg(An + off) - rm[i]) * rinv[i];
+          dAn[off] = pv * (p.scale * acc[4 * j + 2 * i + e] - D[i]);
         }
       }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[as]);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -627,13 +578,8 @@ extern "C" int semseg_psa_attend_bwd_attn(int psa_type, const float* attn, int a
   p.out = static_cast<const __nv_bfloat16*>(out); p.out_lo = static_cast<const __nv_bfloat16*>(out_lo);
   p.dout_pitch = dout_pitch; p.out_pitch = out_pitch;
   p.N = N; p.H = H; p.W = W; p.mH = mH; p.mW = mW; p.a_pitch = a_pitch; p.C = C;
-  p.rows_per_tile = 128 / W;
-  {
-    const int want = (N * H * cdiv(H * W, kPgBlockN)) / num_sms();     // keep every SM busy (rows <-> epilogue threads)
-    const int rpt = want < 1 ? 1 : want;
-    if (rpt < p.rows_per_tile) p.rows_per_tile = rpt;
-  }
-  p.tiles_per_img = cdiv(H, p.rows_per_tile);
+  p.tile_rows = psa_tile_rows(N, H * W, 128, cdiv(H * W, kPgBlockN));   // keep every SM busy
+  p.tiles_per_img = cdiv(H * W, p.tile_rows);
   p.nseg = split ? 3 : 1;
   p.scale = scale;
   // the caller's dattn must be zero where no gradient lands

@@ -347,7 +347,7 @@ def _is_native_conv(conv, cin):
 
 
 def _require_native(conv, cin):
-    """There is exactly one backend: a convolution the sm_100a kernel does not cover is an error, never a library
+    """There is exactly one backend: a convolution the sm_90a kernel does not cover is an error, never a library
     (cuDNN) fallback. Every convolution of PSPNet / PSANet (model/resnet.py, model/pspnet.py, model/psanet.py) is covered."""
     if not _is_native_conv(conv, cin):
         raise NotImplementedError(

@@ -11,7 +11,7 @@ from ._lib import ConvDesc, WgradDesc, EPI_RAW, EPI_AFFINE, EPI_F32, MAX_TAPS
 
 
 # bf16x3: K blocks (64-channel block x tap) one tensor-core accumulation chain may span (8 x 4 x 3 = 96 MMA steps; the
-# truncating fp32 accumulation of tcgen05 loses ~2^-24 per step towards zero, tools/probe_accum.py)
+# truncating fp32 accumulation of the tensor core loses ~2^-24 per step towards zero, tools/probe_accum.py)
 X3_MAX_KBLOCKS = 8
 
 _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)

@@ -3,7 +3,7 @@
   "bf16"    single-pass bf16 conv operands, bf16 activation storage: the speed configuration.
   "bf16x3"  error-compensated operands: activations and packed weights are stored as (hi, lo) bf16 pairs
             (16 mantissa bits) and every convolution accumulates x_hi*w_hi + x_lo*w_hi + x_hi*w_lo in fp32 on the
-            same tcgen05 kernel (three K segments per block). This is the mode that meets north_star's parity bar
+            same wgmma kernel (three K segments per block). This is the mode that meets north_star's parity bar
             (eval logits within 1e-3 of the fp32 reference, identical argmax) — the reference itself computes in
             fp32 (CPU) / TF32 (cuDNN default), model/resnet.py:63-92.
 

@@ -1,5 +1,5 @@
 """psa_mask (collect / distribute) autograd op: drop-in for lib.psa.functional.psa_mask
-(lib/psa/functional.py:4-5, lib/psa/functions/psamask.py:6-39) on the sm_100a kernel."""
+(lib/psa/functional.py:4-5, lib/psa/functions/psamask.py:6-39) on the sm_90a kernel."""
 import torch
 from torch.autograd import Function
 

@@ -1,6 +1,6 @@
 """PSPNet, drop-in for the reference's model/pspnet.py (same constructor / forward signatures, same child
 module names and state_dict keys, same return values — model/pspnet.py:29-105), executed on NHWC bf16
-activations by the sm_100a kernels behind semseg_b200/functional.py.
+activations by the sm_90a kernels behind semseg_b200/functional.py.
 """
 import torch
 from torch import nn

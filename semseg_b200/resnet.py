@@ -6,7 +6,7 @@ state_dict keys (real nn.Conv2d / nn.BatchNorm2d children, so nn.SyncBatchNorm.c
 DDP keep working, tool/train.py:141-157). Modules are constructed in the reference's order
 (model/resnet.py:100-128), so a given torch.manual_seed yields bit-identical initial weights.
 
-What differs is the execution: `forward_nhwc` runs on NHWC bf16 activations through the sm_100a kernels
+What differs is the execution: `forward_nhwc` runs on NHWC bf16 activations through the sm_90a kernels
 (semseg_b200/functional.py); the nn.Conv2d / nn.BatchNorm2d children are parameter holders whose own
 forward is never called. `BasicBlock` / resnet18/34 are unreachable from PSPNet/PSANet
 (model/pspnet.py:32) and are not provided.

@@ -1,5 +1,6 @@
 """CPU tier: pin the oracle (oracle/) against the reference — golden fixtures made from the real reference
-(tests/golden/make_golden.py) and, when built, the reference's own compiled psamask extension (oracle/_ref)."""
+(tests/golden/make_golden.py, tests/golden/make_psamask_digests.py) and, when built, the reference's own compiled
+psamask extension (oracle/_ref)."""
 import hashlib
 import json
 import os
@@ -10,7 +11,7 @@ import torch
 
 import oracle
 from oracle import torch_oracle
-from tests import util
+from tests import psamask_cases, util
 
 CASES = [(2, 4, 5, 7, 9), (1, 6, 7, 5, 3), (2, 5, 5, 9, 9), (1, 30, 30, 59, 59)]
 
@@ -32,21 +33,23 @@ def test_psamask_oracle_matches_reference_goldens(golden_dir):
                 assert np.array_equal(din, g[key + "/din"])
 
 
-def test_psamask_oracle_matches_compiled_reference():
+def test_psamask_oracle_matches_compiled_reference(golden_dir):
+    """The reference's own compiled CPU psamask (lib/psa/src/cpu): its output digests on these seeded inputs are stored in
+    tests/golden/psamask_ref_digests.json; where oracle/_ref holds the compiled extension it is compared live as well."""
+    dig = json.load(open(os.path.join(golden_dir, "psamask_ref_digests.json")))["cpu"]
     ref = oracle.ref_psamask_module()
-    if ref is None:
-        pytest.skip("oracle/_ref not built (reference tree absent)")
-    rng = np.random.default_rng(11)
-    for (n, h, w, mh, mw) in CASES + [(1, 3, 9, 5, 17), (1, 1, 1, 1, 1)]:
-        for t in (0, 1):
-            x = rng.standard_normal((n, mh * mw, h, w)).astype(np.float32)
-            out = torch.zeros(n, h * w, h, w)
-            ref.psamask_forward(t, torch.from_numpy(x), out, n, h, w, mh, mw, (mh - 1) // 2, (mw - 1) // 2)
-            assert np.array_equal(oracle.psamask_fwd(x, t, mh, mw), out.numpy())
-            g = rng.standard_normal((n, h * w, h, w)).astype(np.float32)
+    for key, t, (n, h, w, mh, mw), x, g in psamask_cases.cpu_cases():
+        out = oracle.psamask_fwd(x, t, mh, mw)
+        din = oracle.psamask_bwd(g, t, mh, mw)
+        assert hashlib.sha256(out.tobytes()).hexdigest() == dig[key]["out"], key
+        assert hashlib.sha256(din.tobytes()).hexdigest() == dig[key]["din"], key
+        if ref is not None:
+            o = torch.zeros(n, h * w, h, w)
+            ref.psamask_forward(t, torch.from_numpy(x), o, n, h, w, mh, mw, (mh - 1) // 2, (mw - 1) // 2)
+            assert np.array_equal(out, o.numpy())
             gi = torch.zeros(n, mh * mw, h, w)
             ref.psamask_backward(t, torch.from_numpy(g), gi, n, h, w, mh, mw, (mh - 1) // 2, (mw - 1) // 2)
-            assert np.array_equal(oracle.psamask_bwd(g, t, mh, mw), gi.numpy())
+            assert np.array_equal(din, gi.numpy())
 
 
 def test_psamask_torch_restatement_matches_c_oracle():

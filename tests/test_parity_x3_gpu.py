@@ -10,12 +10,11 @@ and much tighter bounds at kernel and block level where nothing amplifies a roun
   * networks: eval logits rel-L2 <= 1e-4 (north_star asks 1e-3), ZERO argmax flips at every pixel whose fp32 top-1/top-2
     margin exceeds twice the largest logit error; train-step losses to 1e-4.
 
-What "bit-exact argmax" can mean on 447 458 pixels was measured on the B200 (tools/probe_x3_floor.py,
-profiles/r2_x3_floor_probe.txt): the fp32 oracle against ITSELF with another cuDNN algorithm (channels_last) already differs
-in 2 pixels (rel-L2 1.8e-6) — the reference is not bit-exact against itself; the fp32 oracle with every conv operand rounded
-to 16 mantissa bits and EXACT fp32 accumulation (the best any hi/lo bf16 scheme can do) differs in 15 pixels (rel-L2 1.2e-5);
-all of them are near-ties (top-2 margin < 1e-3 of |logit|). The raw flip count is therefore asserted against that measured
-floor (<= 64 of ~440k pixels, i.e. 1.5e-4 of the pixels; single-pass bf16 flips 2.8 %), the margin-aware count against 0.
+What "bit-exact argmax" can mean on 447 458 pixels is measured by tools/probe_x3_floor.py: the fp32 oracle against ITSELF
+with another cuDNN algorithm (channels_last) already differs in a few near-tie pixels — the reference is not bit-exact
+against itself — and so does the fp32 oracle with every conv operand rounded to 16 mantissa bits and EXACT fp32
+accumulation (the best any hi/lo bf16 scheme can do). The raw flip count is therefore asserted against a floor
+(<= 64 of ~440k pixels, i.e. 1.5e-4 of the pixels), the margin-aware count against 0.
 
 The reference arithmetic is fp32 (model/resnet.py:63-92, model/pspnet.py:80-105); the oracle is oracle/torch_oracle.py
 (pinned to the reference's own outputs in tests/test_oracle_cpu.py) running fp32 on the GPU with TF32 disabled.

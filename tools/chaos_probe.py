@@ -1,7 +1,7 @@
 """How sensitive are train-mode gradients of a random-init PSPNet50 to a tiny input perturbation?
 
 Control experiment behind the parity tolerances (DESIGN.md §4): the same probe is run on the fp32 oracle (pure
-PyTorch, TF32 off) and on the B200 path. If the *oracle's own* gradients decorrelate under a 1e-3 input
+PyTorch, TF32 off) and on the native path. If the *oracle's own* gradients decorrelate under a 1e-3 input
 perturbation, element-wise end-to-end gradient parity between any two implementations that differ by rounding is not
 a meaningful test, and parity has to be asserted per kernel / per block instead.
 """

@@ -1,4 +1,4 @@
-"""Accumulation-error probe: tcgen05 fp32 accumulation (TMEM) vs an fp64 reference on bf16-exact operands, as a function
+"""Accumulation-error probe: tensor-core fp32 accumulation vs an fp64 reference on bf16-exact operands, as a function
 of the number of sequential MMA steps (K / 16). Output feeds DESIGN.md §4 (why long-K convs are K-sliced in bf16x3)."""
 import os
 import sys
@@ -22,5 +22,5 @@ for cin, k in [(64, 1), (256, 1), (1024, 1), (4096, 1), (512, 3), (4096, 3)]:
         e = ((y.double() - ref).norm() / ref.norm()).item()
         e32 = ((ref32.double() - ref).norm() / ref.norm()).item()
         bias = ((y.double() - ref) * ref.sign()).sum().item() / ref.abs().sum().item()
-        print("K=%6d steps=%5d %s: tcgen05 rel %.2e (signed bias %.2e) | cuDNN fp32 rel %.2e" %
+        print("K=%6d steps=%5d %s: tensor core rel %.2e (signed bias %.2e) | cuDNN fp32 rel %.2e" %
               (cin * k * k, cin * k * k // 16, "pos" if positive else "rnd", e, bias, e32), flush=True)
