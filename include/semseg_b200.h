@@ -19,6 +19,11 @@
  *   - semseg_ppm_* / pool     : model/pspnet.py:12-26 (AdaptiveAvgPool2d, bilinear upsample, concat),
  *                               nn.MaxPool2d at model/resnet.py:115.
  *   - semseg_upsample_ce_*    : F.interpolate + CrossEntropyLoss + argmax, model/pspnet.py:94-103.
+ *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
+ *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
+ *                               (tool/test.py:139-141), the overlap accumulation and normalisation
+ *                               (tool/test.py:163-176) and the per-scale resize into the running total
+ *                               (tool/test.py:177, 202).
  *
  * Activations are NHWC bf16 in HBM; "pitch" arguments are the distance between consecutive pixels in
  * elements (>= channels; lets a kernel read/write a channel slice of a wider concat buffer).
@@ -356,6 +361,28 @@ long long semseg_upsample_ce_bwd_workspace_floats(int N, int Ho, int w, int C);
 int semseg_upsample_ce_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                            int Ho, int Wo, int ignore_index, const float* lse, const float* loss_info,
                            const float* grad_out, float* workspace, float* dlogits, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Sliding-window evaluation after the network (semseg_b200/inference.py, exact=False). No tensor cores, no atomics.
+ *   window_scores     : logits fp32 NHWC [G (+G mirrored crops when flip), h, w, C] (pitch >= C; with flip, images
+ *                       G..2G-1 are the mirrors of 0..G-1) -> out fp32 [G, C, crop_h, crop_w] (contiguous) =
+ *                       softmax over C of the x8 bilinear (align_corners=True) upsample, averaged with the mirrored
+ *                       crop's scores as (p + p_mirror) * 0.5 when flip. Requires crop = 8(h-1)+1 x 8(w-1)+1 and
+ *                       C <= 256. The upsampled logits are never stored.
+ *   window_accumulate : scores fp32 [ny*nx, C, crop_h, crop_w] of a scale's crop grid in row-major order, crop origins
+ *                       ys[ny] / xs[nx] (host arrays, at most 256 each: ascending, first 0, last full - crop, gaps <=
+ *                       crop) on the padded [full_h, full_w] image -> canvas fp64 [C, img_h, img_w] = the un-padded
+ *                       window at (top, left) of the fp64 sum of the covering crops' scores in grid order, divided by
+ *                       their count. Every element written once; bit-identical to the sequential accumulation.
+ *   window_resize_add : total fp64 [C, Ho, Wo] += bilinear resize (align_corners=False, half-pixel centres, fp64 as
+ *                       ATen's upsample_bilinear2d) of canvas fp64 [C, Hi, Wi].
+ */
+int semseg_window_scores(const float* logits, int pitch, int G, int h, int w, int C, int flip, float* out, int crop_h,
+                         int crop_w, void* stream);
+int semseg_window_accumulate(const float* scores, int C, int crop_h, int crop_w, const int* ys, int ny, const int* xs,
+                             int nx, int full_h, int full_w, int top, int left, int img_h, int img_w, double* canvas,
+                             void* stream);
+int semseg_window_resize_add(const double* canvas, int C, int Hi, int Wi, double* total, int Ho, int Wo, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Step glue: per-class intersection / union / target areas (util/util.py:55-67, called at tool/train.py:286,375).

@@ -156,6 +156,10 @@ SIGNATURES = {
     "semseg_upsample_ce_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp,
                                        c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                         c_int, c_int, c_int, c_vp, c_vp]),
+    "semseg_window_resize_add": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
 }
 
 _lib = None

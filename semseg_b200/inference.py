@@ -14,6 +14,11 @@ accumulation / normalisation by the overlap count stay on the device. Two ways t
     the sum over scales and the argmax also run on the device; only the result crosses PCIe. At 1024x2048 x 19 classes
     the host steps of the reference procedure (float64 [h, w, classes] arrays through cv2 and numpy) cost several times
     the network itself. Scores agree with the exact path to ~1e-7.
+    When the model is this package's PSPNet / PSANet (eval mode, CUDA, zoom factor 8, crop = 8(h'-1)+1, at most 256
+    classes) everything after the network runs on the native kernels of csrc/window.cu: one kernel turns the 1/8
+    resolution logits of a batch into flip-averaged softmax scores (the upsampled [2G, classes, crop, crop] logits never
+    exist), one gathers a scale's crops into its overlap-normalised fp64 canvas (bit-identical to the ATen loop), and
+    one resizes the canvas and adds it into the running total. Any other model runs the ATen steps below.
 `net_process` / `scale_process` keep the reference's signatures and return types (and the exact arithmetic);
 `SlidingWindowPredictor` is the object form that also covers the per-image scale loop.
 
@@ -26,6 +31,8 @@ import cv2
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+from . import ops
 
 __all__ = ["crop_origins", "scaled_size", "net_process", "scale_process", "SlidingWindowPredictor"]
 
@@ -48,6 +55,20 @@ def scaled_size(h, w, long_size):
 def _model_device(model):
     p = next(iter(model.parameters()), None)
     return p.device if p is not None else torch.device("cpu")
+
+
+def _native_net(model, classes, crop_h, crop_w, device):
+    """The semseg_b200 PSPNet / PSANet behind `model` when its scores can be finished by csrc/window.cu, else None."""
+    from .psanet import PSANet
+    from .pspnet import PSPNet
+    if isinstance(model, torch.nn.DataParallel):
+        if len(model.device_ids) > 1:
+            return None
+        model = model.module
+    if not (type(model) in (PSPNet, PSANet) and not model.training and device.type == "cuda"
+            and model.zoom_factor == 8 and (crop_h - 1) % 8 == 0 and (crop_w - 1) % 8 == 0 and classes <= 256):
+        return None
+    return model
 
 
 class SlidingWindowPredictor:
@@ -74,9 +95,21 @@ class SlidingWindowPredictor:
             t = t / torch.tensor(self.std, dtype=torch.float32, device=self.device).view(3, 1, 1)
         return t.contiguous()
 
-    def _scores(self, crops):
-        """[G, 3, ch, cw] normalised crops -> [G, classes, ch, cw] flip-averaged softmax scores (fp32)."""
+    def _scores(self, crops, net=None):
+        """[G, 3, ch, cw] normalised crops -> [G, classes, ch, cw] flip-averaged softmax scores (fp32). With `net` (see
+        _native_net) the scores kernel writes each batch's scores straight into the result from the 1/8-resolution
+        logits."""
         per_call = self.max_batch // 2 if self.flip else self.max_batch
+        if net is not None:
+            out = torch.empty((crops.shape[0], self.classes) + tuple(crops.shape[2:]), dtype=torch.float32,
+                              device=crops.device)
+            with torch.no_grad():
+                for g0 in range(0, crops.shape[0], per_call):
+                    part = crops[g0:g0 + per_call]
+                    logits = net._eval_logits_nhwc(torch.cat([part, part.flip(3)], 0) if self.flip else part)
+                    self.forward_calls += 1
+                    ops.window_scores(logits, self.flip, out[g0:g0 + part.shape[0]])
+            return out
         outs = []
         with torch.no_grad():
             for g0 in range(0, crops.shape[0], per_call):
@@ -94,9 +127,10 @@ class SlidingWindowPredictor:
         return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
 
     # ------------------------------------------------------------------------------------------- one scale
-    def _scale_canvas(self, image):
+    def _scale_canvas(self, image, net=None):
         """Overlap-normalised scores of one rescaled image, un-padded: float64 [classes, img_h, img_w] on the device
-        (tool/test.py:148-176: padding, crop grid, accumulation in grid order, division by the crop count)."""
+        (tool/test.py:148-176: padding, crop grid, accumulation in grid order, division by the crop count). With `net`
+        the scores and the accumulation run on the native kernels (contiguous result, same bits as the loop)."""
         ch, cw = self.crop_h, self.crop_w
         img_h, img_w = image.shape[:2]
         extra_h, extra_w = max(ch - img_h, 0), max(cw - img_w, 0)
@@ -105,11 +139,13 @@ class SlidingWindowPredictor:
             image = cv2.copyMakeBorder(image, top, extra_h - top, left, extra_w - left, cv2.BORDER_CONSTANT,
                                        value=self.mean)
         full_h, full_w = image.shape[:2]
-        windows = [(y0, x0) for y0 in crop_origins(full_h, ch, self.stride_rate)
-                   for x0 in crop_origins(full_w, cw, self.stride_rate)]
+        ys, xs = crop_origins(full_h, ch, self.stride_rate), crop_origins(full_w, cw, self.stride_rate)
+        windows = [(y0, x0) for y0 in ys for x0 in xs]
         x = self._normalised(image)
         crops = torch.stack([x[:, y0:y0 + ch, x0:x0 + cw] for y0, x0 in windows], 0)
-        scores = self._scores(crops)
+        scores = self._scores(crops, net)
+        if net is not None:
+            return ops.window_accumulate(scores, ys, xs, (full_h, full_w), top, left, (img_h, img_w))
         canvas = torch.zeros((self.classes, full_h, full_w), dtype=torch.float64, device=self.device)
         hits = np.zeros((full_h, full_w), dtype=np.float64)
         for k, (y0, x0) in enumerate(windows):          # grid order = the reference's accumulation order
@@ -144,10 +180,16 @@ class SlidingWindowPredictor:
         h, w = image.shape[:2]
         total = np.zeros((h, w, self.classes), dtype=np.float64) if exact else \
             torch.zeros((self.classes, h, w), dtype=torch.float64, device=self.device)
+        net = None if exact else _native_net(self.model, self.classes, self.crop_h, self.crop_w, self.device)
         for s in scales:
             new_h, new_w = scaled_size(h, w, round(s * base_size))
             resized = cv2.resize(image, (new_w, new_h), interpolation=cv2.INTER_LINEAR)
-            total += self.scale(resized, h, w) if exact else self.scale_on_device(resized, h, w)
+            if exact:
+                total += self.scale(resized, h, w)
+            elif net is not None:
+                ops.window_resize_add(self._scale_canvas(resized, net), total)     # resize + add in one pass
+            else:
+                total += self.scale_on_device(resized, h, w)
         total /= len(scales)
         if exact:
             return total, np.argmax(total, axis=2)

@@ -652,6 +652,59 @@ def upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_out):
     return dl
 
 
+# ------------------------------------------------------------------------------------------------ sliding-window evaluation
+def window_scores(logits, flip, out):
+    """fp32 NHWC logits [G (+G mirrored crops when flip), h, w, C] -> flip-averaged softmax scores written into `out`,
+    a contiguous fp32 [G, C, 8(h-1)+1, 8(w-1)+1] tensor (typically a slice of a scale's score buffer)."""
+    _require_cuda(logits, out)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(3) == 1
+    n, h, w, c = logits.shape
+    pitch = logits.stride(2)
+    assert logits.stride(1) == w * pitch and logits.stride(0) == h * logits.stride(1), "logits must be pixel-contiguous"
+    g = n // 2 if flip else n
+    assert not flip or n % 2 == 0, "flip needs the crops followed by their mirrors"
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and tuple(out.shape[:2]) == (g, c)
+    _lib.check(lib.semseg_window_scores(_ptr(logits), pitch, g, h, w, c, int(bool(flip)), _ptr(out), out.shape[2],
+                                        out.shape[3], _stream()), "semseg_window_scores")
+    return out
+
+
+def _int_array(vals):
+    return (ctypes.c_int * len(vals))(*[int(v) for v in vals])
+
+
+def window_accumulate(scores, ys, xs, full_size, top, left, img_size):
+    """Overlap-normalised fp64 canvas [C, img_h, img_w] of a scale: scores fp32 [len(ys)*len(xs), C, crop_h, crop_w] of
+    the crop grid (row-major), crop origins ys / xs on the padded image of size full_size, un-padded window at
+    (top, left) of size img_size."""
+    _require_cuda(scores)
+    lib = _lib.load()
+    assert scores.dtype == torch.float32 and scores.is_contiguous() and scores.dim() == 4
+    k, c, ch, cw = scores.shape
+    assert k == len(ys) * len(xs), "one score map per crop of the grid"
+    img_h, img_w = img_size
+    canvas = torch.empty((c, img_h, img_w), dtype=torch.float64, device=scores.device)
+    _lib.check(lib.semseg_window_accumulate(_ptr(scores), c, ch, cw, _int_array(ys), len(ys), _int_array(xs), len(xs),
+                                            full_size[0], full_size[1], top, left, img_h, img_w, _ptr(canvas),
+                                            _stream()), "semseg_window_accumulate")
+    return canvas
+
+
+def window_resize_add(canvas, total):
+    """total fp64 [C, H, W] += bilinear resize (align_corners=False) of canvas fp64 [C, h, w] to H x W; in place."""
+    _require_cuda(canvas, total)
+    lib = _lib.load()
+    assert canvas.dtype == torch.float64 and total.dtype == torch.float64
+    assert canvas.is_contiguous() and total.is_contiguous() and canvas.dim() == 3 and total.dim() == 3
+    assert canvas.shape[0] == total.shape[0], "canvas and total must have the same classes"
+    c, hi, wi = canvas.shape
+    _, ho, wo = total.shape
+    _lib.check(lib.semseg_window_resize_add(_ptr(canvas), c, hi, wi, _ptr(total), ho, wo, _stream()),
+               "semseg_window_resize_add")
+    return total
+
+
 # ------------------------------------------------------------------------------------------------ pyramid pooling
 def _bin_args(bins, tensors):
     """(bins[], hi pointers[], lo pointers[] or NULL, nb)"""

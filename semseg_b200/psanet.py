@@ -196,18 +196,7 @@ class PSANet(nn.Module):
         if self.training and torch.is_grad_enabled():
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
-        t = SF.to_nhwc_bf16(x)
-        t = self.layer0.forward_nhwc(t)
-        t = self.layer1.forward_nhwc(t)
-        t = graphs.note_boundary(self.layer2.forward_nhwc(t))     # where a captured backward is cut in two
-        t_tmp = self.layer3.forward_nhwc(t)
-        t_aux = None
-        if self.training:       # layer3's output feeds layer4 and the aux head: explicit fan-out (native gradient add)
-            t_tmp, t_aux = SF.fork(t_tmp, 2)
-        t = self.layer4.forward_nhwc(t_tmp)
-        if self.use_psa:
-            t = self.psa.forward_nhwc(t)
-        logits = head_forward_nhwc(self.cls, t)
+        logits, t_aux = self._logits_nhwc(x)
 
         if self.training:
             aux_logits = head_forward_nhwc(self.aux, t_aux)
@@ -226,3 +215,25 @@ class PSANet(nn.Module):
             if self.zoom_factor != 1:
                 x = F.interpolate(x, size=(h, w), mode='bilinear', align_corners=True)
             return x
+
+    def _logits_nhwc(self, x):
+        """fp32 NHWC classifier logits [N, h', w', classes] before the final upsample, and in training mode layer3's
+        output for the aux head (None in eval mode)."""
+        t = SF.to_nhwc_bf16(x)
+        t = self.layer0.forward_nhwc(t)
+        t = self.layer1.forward_nhwc(t)
+        t = graphs.note_boundary(self.layer2.forward_nhwc(t))     # where a captured backward is cut in two
+        t_tmp = self.layer3.forward_nhwc(t)
+        t_aux = None
+        if self.training:       # layer3's output feeds layer4 and the aux head: explicit fan-out (native gradient add)
+            t_tmp, t_aux = SF.fork(t_tmp, 2)
+        t = self.layer4.forward_nhwc(t_tmp)
+        if self.use_psa:
+            t = self.psa.forward_nhwc(t)
+        return head_forward_nhwc(self.cls, t), t_aux
+
+    def _eval_logits_nhwc(self, x):
+        """The eval forward up to the classifier: fp32 NHWC logits [N, h', w', classes]. The sliding-window engine
+        (inference.py) upsamples, scores and flip-averages them in one native kernel."""
+        assert not self.training, "_eval_logits_nhwc is the eval-mode forward"
+        return self._logits_nhwc(x)[0]
