@@ -288,6 +288,18 @@ int semseg_bn_bwd_apply(const void* dy, const void* dy_lo, int dy_pitch, const v
                         const float* scale_shift, const float* sums, float count, int M, int C, int relu, void* dx,
                         void* dx_lo, int dx_pitch, void* dres, void* dres_lo, int dres_pitch, float* dgamma_dbeta,
                         void* stream);
+/* Frozen BatchNorm backward (BN normalised with its running statistics inside a network that trains), one pass.
+ *   scale = gamma/sqrt(running_var+eps), shift = beta - running_mean*scale (gamma / beta may be NULL: 1 / 0);
+ *   dz = dy * (y > 0 if relu); d_raw = dz*scale; dres (optional) = dz;
+ *   sums [2][C] (optional) = (sum dz, sum dz*xhat) = (dbeta, dgamma), xhat = (raw - running_mean)/sqrt(running_var+eps),
+ *   reduced in a fixed order (deterministic) through `workspace` (semseg_bn_workspace_floats(M, C) floats).
+ *   The mask comes from y, or — relu with y == NULL, valid when the forward had no residual — from
+ *   fma(raw, scale, shift) > 0. raw == NULL: the sum dz*xhat row is zero. sums == NULL: no reduction, no workspace. */
+int semseg_bn_bwd_frozen(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo, int y_pitch,
+                         const void* raw, const void* raw_lo, int raw_pitch, const float* gamma, const float* beta,
+                         const float* running_mean, const float* running_var, float eps, int M, int C, int relu,
+                         void* d_raw, void* d_raw_lo, int d_raw_pitch, void* dres, void* dres_lo, int dres_pitch,
+                         float* workspace, long long workspace_floats, float* sums, void* stream);
 /* out = a + b (merges gradient branches; split-aware, unlike an elementwise add of the two planes). */
 int semseg_add_act(const void* a, const void* a_lo, int a_pitch, const void* b, const void* b_lo, int b_pitch,
                    void* out, void* out_lo, int out_pitch, int M, int C, void* stream);

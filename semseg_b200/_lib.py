@@ -133,6 +133,9 @@ SIGNATURES = {
                                      c_int, c_vp, c_ll, c_vp, c_vp]),
     "semseg_bn_bwd_apply": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
                                     c_f, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp]),
+    "semseg_bn_bwd_frozen": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
+                                     c_f, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_ll, c_vp,
+                                     c_vp]),
     "semseg_add_act": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_int, c_vp]),
     "semseg_scale_nc": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp]),
     "semseg_f32_to_act": (c_int, [c_vp, c_int, c_vp, c_vp, c_int, c_ll, c_int, c_int, c_vp]),

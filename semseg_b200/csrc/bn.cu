@@ -273,15 +273,25 @@ __global__ void bn_finalize_kernel(const float* __restrict__ rs, int R, int C, c
   }
 }
 
+// Running-statistics folding of channel c: invstd, scale = gamma*invstd, shift = beta - mean*scale. Shared by the eval
+// fold and the frozen-BN backward, so that the backward's ReLU mask fma(raw, scale, shift) > 0 sees the forward's bits.
+__device__ __forceinline__ void fold_running(const float* __restrict__ gamma, const float* __restrict__ beta,
+                                             const float* __restrict__ rm, const float* __restrict__ rv, float eps, int c,
+                                             float& invstd, float& sc, float& sh) {
+  invstd = rsqrtf(rv[c] + eps);
+  sc = (gamma ? gamma[c] : 1.f) * invstd;
+  sh = (beta ? beta[c] : 0.f) - rm[c] * sc;
+}
+
 __global__ void bn_fold_eval_kernel(const float* __restrict__ gamma, const float* __restrict__ beta,
                                     const float* __restrict__ rm, const float* __restrict__ rv, float eps, int C,
                                     float* __restrict__ scale_shift) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float invstd = rsqrtf(rv[c] + eps);
-  const float sc = (gamma ? gamma[c] : 1.f) * invstd;
+  float invstd, sc, sh;
+  fold_running(gamma, beta, rm, rv, eps, c, invstd, sc, sh);
   scale_shift[c] = sc;
-  scale_shift[C + c] = (beta ? beta[c] : 0.f) - rm[c] * sc;
+  scale_shift[C + c] = sh;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -566,6 +576,113 @@ __global__ void bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dy, const 
     act_ld8<S>(x, x_lo, p * x_pitch + c0, xv);
     if (mask_from_y) act_ld8<S>(y, y_lo, p * y_pitch + c0, yv);
     finish(d, xv, yv, p);
+  }
+}
+
+// Frozen BatchNorm backward (eval-mode BN inside a network that trains): the forward normalised with the running
+// statistics, so nothing global is needed before d_raw and the whole backward is ONE pass. With dz = dy * (y > 0 if relu):
+//   d_raw = dz * scale, dres = dz (optional), and per-chunk partials of (sum dz, sum dz*xhat), xhat = (raw - mean)*invstd,
+// in the bn_bwd_reduce workspace layout (bn_bwd_reduce_final_kernel finishes them in a fixed order). The ReLU mask comes
+// from y, or — y == nullptr, forward without residual — from fma(raw, scale, shift) > 0 like bn_bwd_reduce_kernel.
+// part == nullptr: no sums. raw == nullptr: the dz*xhat row is zero. block = 8 channel groups x 32 pixel lanes.
+template <bool S>
+__global__ void __launch_bounds__(256, 2)
+bn_bwd_frozen_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ dy_lo, int dy_pitch,
+                     const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ y_lo, int y_pitch,
+                     const __nv_bfloat16* __restrict__ raw, const __nv_bfloat16* __restrict__ raw_lo, int raw_pitch,
+                     const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ rm,
+                     const float* __restrict__ rv, float eps, int M, int C, int relu, int rows_per_chunk,
+                     __nv_bfloat16* __restrict__ d_raw, __nv_bfloat16* __restrict__ d_raw_lo, int d_raw_pitch,
+                     __nv_bfloat16* __restrict__ dres, __nv_bfloat16* __restrict__ dres_lo, int dres_pitch,
+                     float* __restrict__ part) {
+  __shared__ float s_a[32][65];
+  __shared__ float s_b[32][65];
+  const int gl = threadIdx.x & 7;
+  const int pl = threadIdx.x >> 3;
+  const int c0 = blockIdx.x * 64 + gl * 8;
+  const int chunk = blockIdx.y;
+  const int r0 = chunk * rows_per_chunk;
+  const int r1 = min(M, r0 + rows_per_chunk);
+  const bool active = c0 < C;
+  float a[8] = {0, 0, 0, 0, 0, 0, 0, 0}, b[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (active) {
+    float mean[8], invstd[8], sc[8], sh[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      fold_running(gamma, beta, rm, rv, eps, c0 + q, invstd[q], sc[q], sh[q]);
+      mean[q] = rm[c0 + q];
+    }
+    const bool mask_from_y = relu && y != nullptr;
+    const bool mask_from_x = relu && y == nullptr;
+    const bool load_x = raw != nullptr && (mask_from_x || part != nullptr);
+    constexpr int U = S ? 2 : 4;  // rows in flight per thread
+    auto finish = [&](float (&d)[8], const float (&xv)[8], const float (&yv)[8], long long rr) {
+      if (mask_from_y) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+          if (!(yv[q] > 0.f)) d[q] = 0.f;
+      } else if (mask_from_x) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+          if (!(fmaf(xv[q], sc[q], sh[q]) > 0.f)) d[q] = 0.f;
+      }
+      if (dres) act_st8<S>(dres, dres_lo, rr * dres_pitch + c0, d);
+      float o[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        a[q] += d[q];
+        if (load_x) b[q] = fmaf(d[q], (xv[q] - mean[q]) * invstd[q], b[q]);
+        o[q] = d[q] * sc[q];
+      }
+      act_st8<S>(d_raw, d_raw_lo, rr * d_raw_pitch + c0, o);
+    };
+    int r = r0 + pl;
+    for (; r + (U - 1) * 32 < r1; r += U * 32) {
+      Raw8<S> dv[U], xr[U], yr[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) dv[u] = act_ldraw<S>(dy, dy_lo, static_cast<long long>(r + u * 32) * dy_pitch + c0);
+      if (load_x) {
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+          xr[u] = act_ldraw<S>(raw, raw_lo, static_cast<long long>(r + u * 32) * raw_pitch + c0);
+      }
+      if (mask_from_y) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) yr[u] = act_ldraw<S>(y, y_lo, static_cast<long long>(r + u * 32) * y_pitch + c0);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        float d[8], xv[8] = {0, 0, 0, 0, 0, 0, 0, 0}, yv[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        act_unpack<S>(dv[u], d);
+        if (load_x) act_unpack<S>(xr[u], xv);
+        if (mask_from_y) act_unpack<S>(yr[u], yv);
+        finish(d, xv, yv, r + u * 32);
+      }
+    }
+    for (; r < r1; r += 32) {
+      float d[8], xv[8] = {0, 0, 0, 0, 0, 0, 0, 0}, yv[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      act_ld8<S>(dy, dy_lo, static_cast<long long>(r) * dy_pitch + c0, d);
+      if (load_x) act_ld8<S>(raw, raw_lo, static_cast<long long>(r) * raw_pitch + c0, xv);
+      if (mask_from_y) act_ld8<S>(y, y_lo, static_cast<long long>(r) * y_pitch + c0, yv);
+      finish(d, xv, yv, r);
+    }
+  }
+  if (part == nullptr) return;  // uniform over the grid: no thread is left waiting at the barrier
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    s_a[pl][gl * 8 + q] = a[q];
+    s_b[pl][gl * 8 + q] = b[q];
+  }
+  __syncthreads();
+  if (pl < 2 && active) {
+    // pl 0 reduces the dz sums, pl 1 the dz*xhat sums (same order as bn_bwd_reduce_kernel)
+    float(*src)[65] = pl == 0 ? s_a : s_b;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      float t = 0.f;
+      for (int i = 0; i < 32; ++i) t += src[i][gl * 8 + q];
+      if (c0 + q < C) part[(static_cast<size_t>(chunk) * 2 + pl) * C + c0 + q] = t;
+    }
   }
 }
 
@@ -1034,6 +1151,46 @@ extern "C" int semseg_bn_bwd_apply(const void* dy, const void* dy_lo, int dy_pit
                              static_cast<bf16*>(dx_lo), dx_pitch, static_cast<bf16*>(dres),
                              static_cast<bf16*>(dres_lo), dres_pitch, dgamma_dbeta));
   SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" int semseg_bn_bwd_frozen(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo,
+                                    int y_pitch, const void* raw, const void* raw_lo, int raw_pitch, const float* gamma,
+                                    const float* beta, const float* running_mean, const float* running_var, float eps,
+                                    int M, int C, int relu, void* d_raw, void* d_raw_lo, int d_raw_pitch, void* dres,
+                                    void* dres_lo, int dres_pitch, float* workspace, long long workspace_floats,
+                                    float* sums, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SB_CHECK_ARG(dy && d_raw && running_mean && running_var, "bn_bwd_frozen: null dy, d_raw or running statistics");
+  SB_CHECK_ARG(M > 0 && C > 0 && C % 8 == 0, "bn_bwd_frozen: need M > 0 and C > 0, C %% 8 == 0 (M %d, C %d)", M, C);
+  SB_CHECK_ARG(!relu || y || raw, "bn_bwd_frozen: relu needs y or raw for the mask");
+  const bool use_y = relu && y, use_raw = raw != nullptr;
+  SB_CHECK_ARG(dy_pitch >= C && dy_pitch % 8 == 0 && d_raw_pitch >= C && d_raw_pitch % 8 == 0 &&
+                   (!use_y || (y_pitch >= C && y_pitch % 8 == 0)) &&
+                   (!use_raw || (raw_pitch >= C && raw_pitch % 8 == 0)) &&
+                   (!dres || (dres_pitch >= C && dres_pitch % 8 == 0)),
+               "bn_bwd_frozen: pitches must be multiples of 8 and at least C");
+  SB_CHECK_ARG(!sums || (workspace && workspace_floats >= semseg_bn_workspace_floats(M, C)),
+               "bn_bwd_frozen: sums need a workspace of semseg_bn_workspace_floats(M, C) floats");
+  const bool split = dy_lo != nullptr;
+  SB_CHECK_ARG((d_raw_lo != nullptr) == split && (!use_y || (y_lo != nullptr) == split) &&
+                   (!use_raw || (raw_lo != nullptr) == split) && (!dres || (dres_lo != nullptr) == split),
+               "bn_bwd_frozen: all tensors must use the same storage form (plain or split)");
+  const int rows = chunk_rows(M);
+  const int chunks = cdiv(M, rows);
+  dim3 grid(cdiv(C, 64), chunks);
+  SB_ACT_DISPATCH(split, bn_bwd_frozen_kernel<kS><<<grid, 256, 0, stream>>>(
+                             static_cast<const bf16*>(dy), static_cast<const bf16*>(dy_lo), dy_pitch,
+                             static_cast<const bf16*>(use_y ? y : nullptr), static_cast<const bf16*>(y_lo), y_pitch,
+                             static_cast<const bf16*>(raw), static_cast<const bf16*>(raw_lo), raw_pitch, gamma, beta,
+                             running_mean, running_var, eps, M, C, relu, rows, static_cast<bf16*>(d_raw),
+                             static_cast<bf16*>(d_raw_lo), d_raw_pitch, static_cast<bf16*>(dres),
+                             static_cast<bf16*>(dres_lo), dres_pitch, sums ? workspace : nullptr));
+  SB_LAUNCHED();
+  if (sums) {
+    bn_bwd_reduce_final_kernel<<<cdiv(2 * C, 32), 1024, 0, stream>>>(workspace, chunks, C, sums);
+    SB_LAUNCHED();
+  }
   return SEMSEG_OK;
 }
 

@@ -9,7 +9,16 @@ conv + BatchNorm(train) + ReLU (+ residual) is three launches forward:
 because training-mode BN needs the batch (and, under SyncBN, cross-rank) statistics of the complete conv
 output before anything can be normalised (model/resnet.py:77-83). In eval mode the BN folds into the conv
 epilogue and the whole thing is a single kernel.
+
+Frozen BatchNorm — a BN layer in eval mode inside a network that trains (`model.train()`, then `.eval()` on the BN
+layers) — normalises with its running statistics, leaves them untouched and still passes gradients: its forward is the
+eval kernel (or conv + apply when gamma needs a gradient) and its backward one pass (ops.bn_bwd_frozen). `_bn_mode` is
+the one place that decides which of the three forms a stage takes.
 """
+import contextlib
+import functools
+import threading
+
 import torch
 import torch.distributed as dist
 import torch.nn as nn
@@ -95,6 +104,45 @@ def prepack(model, force=False):
         c.__dict__["_sb_pack"] = (k, pw)
 
 
+# Whether the network being run is in training mode, per thread (nn.DataParallel replicas run in threads,
+# tool/train.py:159). Set by the forward of PSPNet / PSANet and of the modules that can be run on their own.
+_net = threading.local()
+
+
+@contextlib.contextmanager
+def network_mode(training):
+    """Runs the enclosed forward as part of a network in training mode (True) or not (False) on this thread."""
+    prev = getattr(_net, "training", False)
+    _net.training = bool(training)
+    try:
+        yield
+    finally:
+        _net.training = prev
+
+
+def network_forward(fn):
+    """Decorator of a module's forward: the module is the network being run, in its own training mode."""
+    @functools.wraps(fn)
+    def forward(self, *args, **kwargs):
+        with network_mode(self.training):
+            return fn(self, *args, **kwargs)
+    return forward
+
+
+def _bn_mode(bn, *inputs):
+    """How a conv + `bn` stage runs, given the tensors its gradients would flow to (None entries allowed):
+      "batch"  : batch statistics (BN in training mode, or without running statistics), running statistics updated;
+      "frozen" : running statistics, differentiable — BN in eval mode, the network in training mode, autograd enabled,
+                 and some input needs a gradient;
+      "eval"   : the folded single kernel, detached (model.eval(), torch.no_grad(), or nothing needs a gradient)."""
+    if bn.training or bn.running_mean is None:
+        return "batch"
+    if (torch.is_grad_enabled() and getattr(_net, "training", False) and
+            any(t is not None and t.requires_grad for t in inputs)):
+        return "frozen"
+    return "eval"
+
+
 def _sync_group(bn):
     """Process group when `bn` is a SyncBatchNorm that must synchronise, else None."""
     if isinstance(bn, nn.SyncBatchNorm) and dist.is_available() and dist.is_initialized():
@@ -156,12 +204,17 @@ def _bn_backward(ctx_pg, world, dy, y, raw, mi, gamma, relu, want_dres, ss=None)
 class _CbaState:
     """What one conv+BN(+residual)(+ReLU) stage keeps for its backward pass."""
     __slots__ = ("xin", "raw", "y", "mi", "gamma", "ss", "pw", "k", "dil", "stride", "relu", "pg", "world",
-                 "in_shape", "has_res")
+                 "in_shape", "has_res", "frozen", "beta", "rm", "rv", "eps", "want_g", "want_b")
 
 
-def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True):
+def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True, frozen=False):
     """conv (1x1 / 3x3; stride 1 with any dilation, or stride 2) + training BatchNorm + optional residual + ReLU.
     Returns (y, state). Three launches: conv_fprop (raw + per-CTA statistics) -> finalise (+ SyncBN exchange) -> apply.
+
+    frozen=True: BatchNorm with its running statistics (see _bn_mode) — no statistics, no SyncBN exchange, running
+    statistics and num_batches_tracked untouched. When gamma needs no gradient the forward is the eval kernel (conv +
+    folded BN + residual + ReLU in one launch) and only x and y are kept; otherwise conv (raw) -> apply with the folded
+    scale / shift, and raw is kept for dgamma's x-hat.
 
     Stride-2 convs (stem conv1, layer2.0 conv2 / downsample — model/resnet.py:108,130-137) run on the same
     stride-1 tensor-core kernel through a 2x2 phase decomposition of the input (ops.space_to_phases): tap (r, s)
@@ -183,6 +236,26 @@ def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True):
         t2 = ops.conv_taps_s2(k, n)
         taps, img_add = [t[:3] for t in t2], [t[3] for t in t2]
         out_nhw = (n, (h - 1) // 2 + 1, (w - 1) // 2 + 1)
+    if frozen:
+        ss = ops.bn_fold_eval(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+        want_g = bn.weight is not None and bn.weight.requires_grad
+        if want_g:
+            raw, _ = ops.conv_fprop(xin, wf, pw.cout, taps, img_add=img_add, out_nhw=out_nhw)
+            y = ops.bn_apply(raw, ss, residual=residual, relu=relu, out=out)
+        else:
+            raw = None
+            y, _ = ops.conv_fprop(xin, wf, pw.cout, taps, epi=EPI_AFFINE, relu=relu, scale=ss[0], shift=ss[1],
+                                  residual=residual, out=out, img_add=img_add, out_nhw=out_nhw)
+        st = _CbaState()
+        # ReLU mask for backward: recomputed from raw when there is raw and no residual, else the saved output
+        need_y = relu and (residual is not None or raw is None)
+        st.xin, st.raw, st.y, st.mi, st.ss = xin, raw, (y if need_y else None), None, None
+        st.frozen, st.gamma, st.beta, st.eps = True, bn.weight, bn.bias, bn.eps
+        st.rm, st.rv = bn.running_mean, bn.running_var
+        st.want_g, st.want_b = want_g, bn.bias is not None and bn.bias.requires_grad
+        st.pw, st.k, st.dil, st.stride, st.relu, st.pg, st.world = pw, k, dil, stride, relu, None, 1
+        st.in_shape, st.has_res = (n, h, w, cx), residual is not None
+        return y, st
     raw, sp = ops.conv_fprop(xin, wf, pw.cout, taps, stats=True, img_add=img_add, out_nhw=out_nhw)
     pg = _sync_group(bn)
     track = bn.track_running_stats and bn.running_mean is not None
@@ -205,6 +278,7 @@ def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True):
     st = _CbaState()
     # ReLU mask for backward: with a residual it needs the saved output, otherwise it is recomputed from raw
     need_y = relu and residual is not None
+    st.frozen = False
     st.xin, st.raw, st.y, st.mi, st.gamma = xin, raw, (y if need_y else None), mi, bn.weight
     st.ss = ss if (relu and not need_y) else None
     st.pw, st.k, st.dil, st.stride, st.relu, st.pg, st.world = pw, k, dil, stride, relu, pg, world
@@ -217,8 +291,18 @@ def cba_backward(st, dy, need_dx=True, need_dw=True, need_dres=False, dx_add=Non
     dx inside the dgrad epilogue (AFFINE mode with a residual operand) — this is how gradient fan-in is fused."""
     pw = st.pw
     n, h, w, cx = st.in_shape
-    d_raw, dres, dgamma, dbeta = _bn_backward(st.pg, st.world, dy, st.y, st.raw, st.mi, st.gamma, st.relu,
-                                              st.has_res and need_dres, st.ss)
+    if st.frozen:
+        if not (need_dx or need_dw or (st.has_res and need_dres) or st.want_g or st.want_b):
+            return None, None, None, None, None
+        # one pass: d_raw = dz*scale (+ dres = dz) and, when gamma / beta need them, the deterministic channel sums
+        d_raw, dres, sums = ops.bn_bwd_frozen(dy if dy.is_contiguous() else dy.contiguous(), st.y, st.raw, st.gamma,
+                                              st.beta, st.rm, st.rv, st.eps, st.relu,
+                                              want_dres=st.has_res and need_dres, want_sums=st.want_g or st.want_b)
+        dgamma = sums[1] if st.want_g else None
+        dbeta = sums[0] if st.want_b else None
+    else:
+        d_raw, dres, dgamma, dbeta = _bn_backward(st.pg, st.world, dy, st.y, st.raw, st.mi, st.gamma, st.relu,
+                                                  st.has_res and need_dres, st.ss)
     dx = dw = None
     if st.stride == 0:      # patch form of the stem conv (no input gradient by construction)
         if need_dx:
@@ -265,8 +349,8 @@ class _ConvBnAct(torch.autograd.Function):
     """Autograd wrapper of one cba_forward / cba_backward stage."""
 
     @staticmethod
-    def forward(ctx, x, weight, gamma, beta, residual, conv, bn, relu, out):
-        y, st = cba_forward(x, conv, bn, relu, residual, out, input_needs_grad=ctx.needs_input_grad[0])
+    def forward(ctx, x, weight, gamma, beta, residual, conv, bn, relu, out, frozen):
+        y, st = cba_forward(x, conv, bn, relu, residual, out, input_needs_grad=ctx.needs_input_grad[0], frozen=frozen)
         ctx.st = st
         if out is not None:
             ctx.mark_dirty(out)
@@ -277,24 +361,24 @@ class _ConvBnAct(torch.autograd.Function):
         ni = ctx.needs_input_grad
         dx, dw, dgamma, dbeta, dres = cba_backward(ctx.st, dy, need_dx=ni[0], need_dw=ni[1], need_dres=ni[4])
         ctx.st = None
-        return dx, dw, dgamma, dbeta, dres, None, None, None, None
+        return dx, dw, dgamma, dbeta, dres, None, None, None, None, None
 
 
 class _BottleneckFn(torch.autograd.Function):
     """A whole Bottleneck (model/resnet.py:74-94) as one autograd node: conv1-bn1-relu, conv2-bn2-relu, conv3-bn3,
     (+ downsample conv-bn), residual add, relu. Besides saving three autograd nodes per block, the backward pass
     fuses the gradient fan-in (dx = dgrad(conv1) + d(residual branch)) into the dgrad epilogue instead of a separate
-    elementwise add."""
+    elementwise add. `frozen` holds one flag per BatchNorm (bn1, bn2, bn3, downsample): frozen or batch statistics."""
 
     @staticmethod
-    def forward(ctx, x, blk, *params):
-        y1, s1 = cba_forward(x, blk.conv1, blk.bn1, True, None)
-        y2, s2 = cba_forward(y1, blk.conv2, blk.bn2, True, None)
+    def forward(ctx, x, blk, frozen, *params):
+        y1, s1 = cba_forward(x, blk.conv1, blk.bn1, True, None, frozen=frozen[0])
+        y2, s2 = cba_forward(y1, blk.conv2, blk.bn2, True, None, frozen=frozen[1])
         if blk.downsample is not None:
-            res, sd = cba_forward(x, blk.downsample[0], blk.downsample[1], False, None)
+            res, sd = cba_forward(x, blk.downsample[0], blk.downsample[1], False, None, frozen=frozen[3])
         else:
             res, sd = x, None
-        y3, s3 = cba_forward(y2, blk.conv3, blk.bn3, True, res)
+        y3, s3 = cba_forward(y2, blk.conv3, blk.bn3, True, res, frozen=frozen[2])
         ctx.states = (s1, s2, s3, sd)
         return y3
 
@@ -302,34 +386,39 @@ class _BottleneckFn(torch.autograd.Function):
     def backward(ctx, dy):
         s1, s2, s3, sd = ctx.states
         ctx.states = None
-        need_dx = ctx.needs_input_grad[0]
-        d2, dw3, dg3, db3, dres = cba_backward(s3, dy, need_dres=True)
-        d1, dw2, dg2, db2, _ = cba_backward(s2, d2)
+        ni = ctx.needs_input_grad      # x, blk, frozen, then (conv weight, gamma, beta) per stage from index 3
+        need_dx = ni[0]
+        d2, dw3, dg3, db3, dres = cba_backward(s3, dy, need_dw=ni[9], need_dres=True)
+        d1, dw2, dg2, db2, _ = cba_backward(s2, d2, need_dw=ni[6])
         grads_ds = ()
         if sd is not None:
-            dxd, dwd, dgd, dbd, _ = cba_backward(sd, dres, need_dx=need_dx)
+            dxd, dwd, dgd, dbd, _ = cba_backward(sd, dres, need_dx=need_dx, need_dw=ni[12])
             dres_to_x = dxd
             grads_ds = (dwd, dgd, dbd)
         else:
             dres_to_x = dres
-        dx, dw1, dg1, db1, _ = cba_backward(s1, d1, need_dx=need_dx, dx_add=dres_to_x if need_dx else None)
-        return (dx, None, dw1, dg1, db1, dw2, dg2, db2, dw3, dg3, db3) + grads_ds
+        dx, dw1, dg1, db1, _ = cba_backward(s1, d1, need_dx=need_dx, need_dw=ni[3],
+                                            dx_add=dres_to_x if need_dx else None)
+        return (dx, None, None, dw1, dg1, db1, dw2, dg2, db2, dw3, dg3, db3) + grads_ds
 
 
 def bottleneck(x, blk):
-    """Fused Bottleneck when every stage is covered by the native kernels in training mode, else stage by stage."""
+    """Fused Bottleneck when every stage is covered by the native kernels and each BatchNorm uses batch statistics or is
+    frozen (see _bn_mode), else stage by stage."""
     convs = [blk.conv1, blk.conv2, blk.conv3] + ([blk.downsample[0]] if blk.downsample is not None else [])
     bns = [blk.bn1, blk.bn2, blk.bn3] + ([blk.downsample[1]] if blk.downsample is not None else [])
     cins = [x.shape[-1], blk.conv1.out_channels, blk.conv2.out_channels, x.shape[-1]]
-    fused = (torch.is_grad_enabled() and all(b.training or b.running_mean is None for b in bns) and
+    params = [blk.conv1.weight, blk.bn1.weight, blk.bn1.bias, blk.conv2.weight, blk.bn2.weight, blk.bn2.bias,
+              blk.conv3.weight, blk.bn3.weight, blk.bn3.bias]
+    if blk.downsample is not None:
+        params += [blk.downsample[0].weight, blk.downsample[1].weight, blk.downsample[1].bias]
+    modes = [_bn_mode(b, x, *params) for b in bns]     # one autograd node: any gradient runs through every stage
+    fused = (torch.is_grad_enabled() and "eval" not in modes and
              all(_is_native_conv(c, ci) for c, ci in zip(convs, cins)) and
              (blk.downsample is None or len(blk.downsample) == 2))
     if fused:
-        params = [blk.conv1.weight, blk.bn1.weight, blk.bn1.bias, blk.conv2.weight, blk.bn2.weight, blk.bn2.bias,
-                  blk.conv3.weight, blk.bn3.weight, blk.bn3.bias]
-        if blk.downsample is not None:
-            params += [blk.downsample[0].weight, blk.downsample[1].weight, blk.downsample[1].bias]
-        return _BottleneckFn.apply(x, blk, *params)
+        frozen = tuple(m == "frozen" for m in modes) + (False,) * (4 - len(modes))
+        return _BottleneckFn.apply(x, blk, frozen, *params)
     y = conv_bn_act(x, blk.conv1, blk.bn1, relu=True)
     y = conv_bn_act(y, blk.conv2, blk.bn2, relu=True)
     residual = conv_bn_act(x, blk.downsample[0], blk.downsample[1], relu=False) if blk.downsample is not None else x
@@ -357,14 +446,16 @@ def _require_native(conv, cin):
 
 
 def conv_bn_act(x, conv, bn, relu=True, residual=None, out=None):
-    """NHWC activation -> NHWC activation: conv -> BatchNorm -> (+residual) -> (ReLU), training or eval semantics of `bn`."""
-    use_batch_stats = bn.training or (bn.running_mean is None)
+    """NHWC activation -> NHWC activation: conv -> BatchNorm -> (+residual) -> (ReLU), training, frozen or eval
+    semantics of `bn` (see _bn_mode)."""
+    mode = _bn_mode(bn, x, conv.weight, bn.weight, bn.bias, residual)
     _require_native(conv, x.shape[-1])
-    if use_batch_stats:
-        return _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, residual, conv, bn, relu, out)
+    if mode != "eval":
+        return _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, residual, conv, bn, relu, out, mode == "frozen")
     # Eval-mode BatchNorm: conv + folded BN + residual + ReLU are ONE kernel. It has no backward: the reference's
     # validate() (tool/train.py:353-359) calls model.eval()(input) without torch.no_grad() and never back-propagates,
     # so the result is returned detached (a later .backward() through it raises torch's usual "does not require grad").
+    # A frozen BatchNorm of a training network takes this path only when nothing of the stage needs a gradient.
     ss = ops.bn_fold_eval(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
     split = ops.is_split(x)
     with torch.no_grad():

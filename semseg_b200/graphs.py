@@ -251,8 +251,11 @@ def train_step(model, impl, x, y):
     # the graphs address the parameters' storage directly: a parameter that was re-allocated since the capture
     # (model.to(...), a swapped nn.Parameter) must not hit a stale graph, so the storage addresses are part of the key
     ptrs = tuple(p.data_ptr() for p in model.parameters() if p.requires_grad)
+    # BatchNorm modes (batch statistics or frozen) decide which kernels the step runs: freezing or unfreezing a layer
+    # after a capture must capture again, not replay the old step
+    bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
-           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1)
+           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes)
     st = steps.get(key)
     if st is None:
         st = steps[key] = _Step(key)

@@ -567,6 +567,30 @@ def bn_bwd_apply(dy, y, x, mean_invstd, gamma, sums, count, relu, want_dres=Fals
     return dx, dres, dgb
 
 
+def bn_bwd_frozen(dy, y, raw, gamma, beta, running_mean, running_var, eps, relu, want_dres=False, want_sums=True):
+    """Backward of BatchNorm normalised with its running statistics (+ residual) (+ ReLU), one pass.
+    The ReLU mask comes from `y`, or from `raw` when `y` is None (forward without residual). Returns
+    (d_raw, dres or None, sums [2][C] = (dbeta, dgamma) or None); with `raw` None, the dgamma row is zero."""
+    lib = _lib.load()
+    n, h, w, c, dp = _nhwc_meta(dy)
+    yp = _nhwc_meta(y)[4] if y is not None else 0
+    rp = _nhwc_meta(raw)[4] if raw is not None else 0
+    _same_form(dy, y, raw)
+    split = is_split(dy)
+    m = n * h * w
+    d_raw = empty_act((n, h, w, c), split, dy.device)
+    dres = empty_act((n, h, w, c), split, dy.device) if want_dres else None
+    ws, nf, sums = None, 0, None
+    if want_sums:
+        ws, nf = bn_workspace(m, c, dy.device)
+        sums = torch.empty((2, c), dtype=torch.float32, device=dy.device)
+    _lib.check(lib.semseg_bn_bwd_frozen(_ptr(dy), _lo(dy), dp, _ptr(y), _lo(y), yp, _ptr(raw), _lo(raw), rp,
+                                        _ptr(gamma), _ptr(beta), _ptr(running_mean), _ptr(running_var), float(eps), m,
+                                        c, int(bool(relu)), _ptr(d_raw), _lo(d_raw), c, _ptr(dres), _lo(dres), c,
+                                        _ptr(ws), nf, _ptr(sums), _stream()), "semseg_bn_bwd_frozen")
+    return d_raw, dres, sums
+
+
 def add_act(a, b, out=None):
     """a + b of two activations (either storage form; a split-aware add, unlike adding the planes)."""
     lib = _lib.load()

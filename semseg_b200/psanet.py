@@ -117,6 +117,7 @@ class PSA(nn.Module):
             t = _interp_nhwc(t, (h, w))
         return torch.cat((out, t), -1)
 
+    @SF.network_forward
     def forward(self, x):
         return SF.to_nchw_f32(self.forward_nhwc(SF.to_nhwc_bf16(x)))
 
@@ -188,6 +189,7 @@ class PSANet(nn.Module):
                 return out
         return self._forward_impl(x, y)
 
+    @SF.network_forward
     def _forward_impl(self, x, y=None):
         x_size = x.size()
         h = int((x_size[2] - 1) / 8 * self.zoom_factor + 1)

@@ -39,6 +39,7 @@ class PPM(nn.Module):
         feats = [SF.conv_bn_act(p, f[1], f[2], relu=True) for p, f in zip(pooled, self.features)]
         return SF.ppm_upsample_concat(x, feats, bins, link)      # one launch: upsample x4 + concat, written in place
 
+    @SF.network_forward
     def forward(self, x):
         return SF.to_nchw_f32(self.forward_nhwc(SF.to_nhwc_bf16(x)))
 
@@ -124,6 +125,7 @@ class PSPNet(nn.Module):
                 return out
         return self._forward_impl(x, y)
 
+    @SF.network_forward
     def _forward_impl(self, x, y=None):
         x_size = x.size()
         h = int((x_size[2] - 1) / 8 * self.zoom_factor + 1)

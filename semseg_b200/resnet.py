@@ -31,6 +31,7 @@ class NHWCSequential(nn.Sequential):
             x = m.forward_nhwc(x)
         return x
 
+    @SF.network_forward
     def forward(self, x):
         # standalone use with an fp32 NCHW tensor (the reference's calling convention)
         return SF.to_nchw_f32(self.forward_nhwc(SF.to_nhwc_bf16(x)))
@@ -55,6 +56,7 @@ class Bottleneck(nn.Module):
     def forward_nhwc(self, x):
         return SF.bottleneck(x, self)
 
+    @SF.network_forward
     def forward(self, x):
         return SF.to_nchw_f32(self.forward_nhwc(SF.to_nhwc_bf16(x)))
 
@@ -117,6 +119,7 @@ class ResNet(nn.Module):
         return Stem(self.conv1, self.bn1, self.relu, self.conv2, self.bn2, self.relu, self.conv3, self.bn3,
                     self.relu, self.maxpool)
 
+    @SF.network_forward
     def forward(self, x):
         # ImageNet-classification forward of the reference (model/resnet.py:147-164); not on the segmentation path.
         y = self.stem().forward_nhwc(SF.to_nhwc_bf16(x))
