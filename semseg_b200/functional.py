@@ -159,105 +159,9 @@ def _bn_momentum(bn):
     return bn.momentum
 
 
-def _finalize_stats(stats, bn, pg, count_batches=True):
-    """stats [3][C] local (mean, M2, count) -> (mean_invstd, scale_shift, world). Updates running stats."""
-    world = 1
-    if pg is not None:
-        world = dist.get_world_size(pg)
-        stats = gather_rank_stats(stats, pg)
-    track = bn.track_running_stats and bn.running_mean is not None
-    mom = _bn_momentum(bn) if track else 0.0
-    mi, ss = ops.bn_finalize(stats, bn.weight, bn.bias, bn.eps, mom, bn.running_mean if track else None,
-                             bn.running_var if track else None)
-    if count_batches and track and bn.num_batches_tracked is not None:
-        bn.num_batches_tracked.add_(1)
-    return mi, ss, world
-
-
-def _bn_backward(ctx_pg, world, dy, y, raw, mi, gamma, relu, want_dres, ss=None):
-    """Shared BN(+ReLU) backward: returns (d_raw, dres, dgamma, dbeta). The ReLU mask comes from the saved output `y`,
-    or — when `y` is None and `ss` (scale/shift) is given, i.e. no residual — is recomputed from `raw` (saves one
-    tensor read in each of the two passes)."""
-    n, h, w, c = raw.shape[-4:]
-    if not dy.is_contiguous():
-        dy = dy.contiguous()
-    px = p2p.get_exchange(ctx_pg) if ctx_pg is not None else None
-    if px is not None and 2 * c <= p2p.SLOT_FLOATS:
-        # cross-rank sum over NVLink peer memory inside the reduction kernel (no NCCL call)
-        local, sums = ops.bn_bwd_reduce_p2p(dy, y if relu else None, raw, mi, relu, ss if y is None else None, px)
-        dbeta, dgamma = local[0], local[1]
-    else:
-        sums = ops.bn_bwd_reduce(dy, y if relu else None, raw, mi, relu, scale_shift=ss if y is None else None)
-        dbeta, dgamma = sums[0], sums[1]
-        if ctx_pg is not None:
-            dbeta, dgamma = dbeta.clone(), dgamma.clone()  # local sums feed dgamma/dbeta (DDP averages them)
-            dist.all_reduce(sums, group=ctx_pg)
-    # under SyncBN the per-channel sample count is the one the forward exchange measured (mi row 2): exact also when the
-    # ranks hold different numbers of pixels, like torch.nn.SyncBatchNorm's gathered counts
-    count = float(n * h * w) if world == 1 else 0.0
-    d_raw, dres, _ = ops.bn_bwd_apply(dy, y if relu else None, raw, mi, gamma, sums, count, relu, want_dres=want_dres,
-                                      scale_shift=ss if y is None else None)
-    return d_raw, dres, dgamma, dbeta
-
-
-# ------------------------------------------------------------------------------------------------ conv+bn+act
-class _CbaState:
-    """What one conv+BN(+residual)(+ReLU) stage keeps for its backward pass."""
-    __slots__ = ("xin", "raw", "y", "mi", "gamma", "ss", "pw", "k", "dil", "stride", "relu", "pg", "world",
-                 "in_shape", "has_res", "frozen", "beta", "rm", "rv", "eps", "want_g", "want_b")
-
-
-def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True, frozen=False):
-    """conv (1x1 / 3x3; stride 1 with any dilation, or stride 2) + training BatchNorm + optional residual + ReLU.
-    Returns (y, state). Three launches: conv_fprop (raw + per-CTA statistics) -> finalise (+ SyncBN exchange) -> apply.
-
-    frozen=True: BatchNorm with its running statistics (see _bn_mode) — no statistics, no SyncBN exchange, running
-    statistics and num_batches_tracked untouched. When gamma needs no gradient the forward is the eval kernel (conv +
-    folded BN + residual + ReLU in one launch) and only x and y are kept; otherwise conv (raw) -> apply with the folded
-    scale / shift, and raw is kept for dgamma's x-hat.
-
-    Stride-2 convs (stem conv1, layer2.0 conv2 / downsample — model/resnet.py:108,130-137) run on the same
-    stride-1 tensor-core kernel through a 2x2 phase decomposition of the input (ops.space_to_phases): tap (r, s)
-    reads phase ((r+1)&1, (s+1)&1) shifted by -1 or 0; dgrad is one small conv per phase, wgrad reads the phases."""
-    split = ops.is_split(x)
-    pw = packed(conv, split=split)
-    k, dil, stride = conv.kernel_size[0], conv.dilation[0], conv.stride[0]
-    n, h, w, cx = x.shape[-4:]
-    wf = pw.wf
-    if stride == 1:
-        xin, img_add, out_nhw = x, None, None
-        taps = ops.conv_taps(k, dil)
-    elif not input_needs_grad and _is_patch_conv(conv, x):
-        # stem conv: one 1x1 conv over 27-value input patches instead of 9 taps of a 3(->64)-channel K block
-        xin, img_add, out_nhw = ops.im2col3x3s2(x, conv.in_channels), None, None
-        taps, wf, stride = ops.conv_taps(1, 1), packed_patches(conv, split), 0    # stride 0 marks the patch form
-    else:
-        xin = ops.space_to_phases(x)                     # [4N, Hh, Wh, C]
-        t2 = ops.conv_taps_s2(k, n)
-        taps, img_add = [t[:3] for t in t2], [t[3] for t in t2]
-        out_nhw = (n, (h - 1) // 2 + 1, (w - 1) // 2 + 1)
-    if frozen:
-        ss = ops.bn_fold_eval(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
-        want_g = bn.weight is not None and bn.weight.requires_grad
-        if want_g:
-            raw, _ = ops.conv_fprop(xin, wf, pw.cout, taps, img_add=img_add, out_nhw=out_nhw)
-            y = ops.bn_apply(raw, ss, residual=residual, relu=relu, out=out)
-        else:
-            raw = None
-            y, _ = ops.conv_fprop(xin, wf, pw.cout, taps, epi=EPI_AFFINE, relu=relu, scale=ss[0], shift=ss[1],
-                                  residual=residual, out=out, img_add=img_add, out_nhw=out_nhw)
-        st = _CbaState()
-        # ReLU mask for backward: recomputed from raw when there is raw and no residual, else the saved output
-        need_y = relu and (residual is not None or raw is None)
-        st.xin, st.raw, st.y, st.mi, st.ss = xin, raw, (y if need_y else None), None, None
-        st.frozen, st.gamma, st.beta, st.eps = True, bn.weight, bn.bias, bn.eps
-        st.rm, st.rv = bn.running_mean, bn.running_var
-        st.want_g, st.want_b = want_g, bn.bias is not None and bn.bias.requires_grad
-        st.pw, st.k, st.dil, st.stride, st.relu, st.pg, st.world = pw, k, dil, stride, relu, None, 1
-        st.in_shape, st.has_res = (n, h, w, cx), residual is not None
-        return y, st
-    raw, sp = ops.conv_fprop(xin, wf, pw.cout, taps, stats=True, img_add=img_add, out_nhw=out_nhw)
-    pg = _sync_group(bn)
+def _batch_stats(sp, bn, pg):
+    """Per-CTA statistics partials of the conv output -> (mean_invstd, scale_shift) of the batch, over every rank of
+    `pg` under SyncBN. Updates the running statistics and num_batches_tracked like nn.BatchNorm in training mode."""
     track = bn.track_running_stats and bn.running_mean is not None
     mom = _bn_momentum(bn) if track else 0.0
     rm, rv = (bn.running_mean, bn.running_var) if track else (None, None)
@@ -265,83 +169,172 @@ def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True, fr
     if pg is None:
         # single rank: merge the per-CTA partials and finalise in one launch
         mi, ss = ops.bn_finalize_partials(sp, bn.weight, bn.bias, bn.eps, mom, rm, rv)
-        world = 1
-    elif px is not None and 3 * pw.cout <= p2p.SLOT_FLOATS:
+    elif px is not None and 3 * sp.shape[-1] <= p2p.SLOT_FLOATS:
         # SyncBN: statistics exchanged over NVLink peer memory inside the finalise kernel (no NCCL call)
         mi, ss = ops.bn_finalize_p2p(sp, bn.weight, bn.bias, bn.eps, mom, rm, rv, px)
-        world = px.world
     else:
-        mi, ss, world = _finalize_stats(ops.bn_merge_partials(sp), bn, pg, count_batches=False)
+        # SyncBN over NCCL: every rank's local (mean, M2, count), then one finalise
+        mi, ss = ops.bn_finalize(gather_rank_stats(ops.bn_merge_partials(sp), pg), bn.weight, bn.bias, bn.eps, mom,
+                                 rm, rv)
     if track and bn.num_batches_tracked is not None:
         bn.num_batches_tracked.add_(1)
-    y = ops.bn_apply(raw, ss, residual=residual, relu=relu, out=out)
+    return mi, ss
+
+
+def _bn_backward(pg, dy, y, raw, mi, gamma, relu, want_dres, ss=None):
+    """Shared BN(+ReLU) backward: returns (d_raw, dres, dgamma, dbeta). The ReLU mask comes from the saved output `y`,
+    or — when `y` is None and `ss` (scale/shift) is given, i.e. no residual — is recomputed from `raw` (saves one
+    tensor read in each of the two passes)."""
+    n, h, w, c = raw.shape[-4:]
+    if not dy.is_contiguous():
+        dy = dy.contiguous()
+    px = p2p.get_exchange(pg) if pg is not None else None
+    if px is not None and 2 * c <= p2p.SLOT_FLOATS:
+        # cross-rank sum over NVLink peer memory inside the reduction kernel (no NCCL call)
+        local, sums = ops.bn_bwd_reduce_p2p(dy, y if relu else None, raw, mi, relu, ss if y is None else None, px)
+        dbeta, dgamma = local[0], local[1]
+    else:
+        sums = ops.bn_bwd_reduce(dy, y if relu else None, raw, mi, relu, scale_shift=ss if y is None else None)
+        dbeta, dgamma = sums[0], sums[1]
+        if pg is not None:
+            dbeta, dgamma = dbeta.clone(), dgamma.clone()  # local sums feed dgamma/dbeta (DDP averages them)
+            dist.all_reduce(sums, group=pg)
+    # under SyncBN the per-channel sample count is the one the forward exchange measured (mi row 2): exact also when the
+    # ranks hold different numbers of pixels, like torch.nn.SyncBatchNorm's gathered counts
+    count = float(n * h * w) if pg is None else 0.0
+    d_raw, dres, _ = ops.bn_bwd_apply(dy, y if relu else None, raw, mi, gamma, sums, count, relu, want_dres=want_dres,
+                                      scale_shift=ss if y is None else None)
+    return d_raw, dres, dgamma, dbeta
+
+
+# ------------------------------------------------------------------------------------------------ conv+bn+act
+class _ConvForm:
+    """How the conv of one stage runs on the stride-1 tensor-core kernel, chosen once from (conv, x, input_needs_grad,
+    BatchNorm mode). It owns the input transform, the taps and the weight slab, and the fprop / dgrad / wgrad of its form:
+      "direct" : stride 1, any dilation.
+      "phases" : stride 2 (stem conv1, layer2.0 conv2 / downsample — model/resnet.py:108,130-137) through a 2x2 phase
+                 decomposition of the input (space_to_phases): tap (r, s) reads phase ((r+1)&1, (s+1)&1) shifted by
+                 -1 or 0; dgrad is one small conv per phase, wgrad reads the phases.
+      "patches": the 3-channel stride-2 stem conv on an input that needs no gradient: one 1x1 conv over 27-value input
+                 patches (ops.im2col3x3s2) instead of 9 taps of a 3(->64)-channel K block. No dgrad. Eval mode always
+                 takes the phase form: the patch form sums in another order, so its output bits differ."""
+    __slots__ = ("kind", "pw", "wf", "xin", "taps", "img_add", "out_nhw", "in_shape")
+
+    def __init__(self, conv, x, input_needs_grad, mode):
+        split = ops.is_split(x)
+        self.pw = packed(conv, need_dgrad=mode != "eval", split=split)
+        self.wf, self.img_add, self.out_nhw = self.pw.wf, None, None
+        self.in_shape = tuple(x.shape[-4:])
+        n, h, w, _ = self.in_shape
+        k = conv.kernel_size[0]
+        if conv.stride[0] == 1:
+            self.kind, self.xin, self.taps = "direct", x, ops.conv_taps(k, conv.dilation[0])
+        elif mode != "eval" and not input_needs_grad and _is_patch_conv(conv, x):
+            self.kind, self.xin = "patches", ops.im2col3x3s2(x, conv.in_channels)
+            self.taps, self.wf = ops.conv_taps(1, 1), packed_patches(conv, split)
+        else:
+            self.kind, self.xin = "phases", ops.space_to_phases(x)          # [4N, Hh, Wh, C]
+            t2 = ops.conv_taps_s2(k, n)
+            self.taps, self.img_add = [t[:3] for t in t2], [t[3] for t in t2]
+            self.out_nhw = (n, (h - 1) // 2 + 1, (w - 1) // 2 + 1)
+
+    def fprop(self, **kw):
+        """The conv on the transformed input; `kw` are ops.conv_fprop's epilogue / statistics / output options."""
+        return ops.conv_fprop(self.xin, self.wf, self.pw.cout, self.taps, img_add=self.img_add, out_nhw=self.out_nhw,
+                              **kw)
+
+    def dgrad(self, d_raw, dx_add=None):
+        """Input gradient from the conv output's gradient `d_raw`. `dx_add` (same shape as dx) is summed into dx — in
+        the dgrad epilogue (AFFINE mode with a residual operand) for the direct form: this is how gradient fan-in is
+        fused."""
+        if self.kind == "patches":
+            raise RuntimeError("semseg_b200: the patch form of the stem conv was chosen but dx is requested")
+        pw = self.pw
+        n, h, w, _ = self.in_shape
+        mirrored = [(-dh, -dw, wt) for dh, dw, wt in self.taps]       # taps of the transposed conv
+        if self.kind == "direct":
+            dx, _ = ops.conv_fprop(d_raw, pw.wd, pw.cin, mirrored, epi=EPI_RAW if dx_add is None else EPI_AFFINE,
+                                   residual=dx_add)
+            return dx
+        if pw.cin % 64 != 0:
+            raise NotImplementedError("semseg_b200: input gradient of a stride-2 conv needs Cin % 64 == 0")
+        hh, wh = self.xin.shape[-3], self.xin.shape[-2]
+        dxp = ops.empty_act((4 * n, hh, wh, pw.cin), ops.is_split(d_raw), d_raw.device)
+        for q in range(4):
+            sub = [t for t, a in zip(mirrored, self.img_add) if a == q * n]      # the taps that read phase q
+            part = ops.act_batch_slice(dxp, q * n, (q + 1) * n)
+            if sub:
+                ops.conv_fprop(d_raw, pw.wd, pw.cin, sub, out=part, out_nhw=(n, hh, wh))
+            else:
+                part.zero_()
+        dx = ops.phases_to_space(dxp, n, h, w)
+        return dx if dx_add is None else ops.add_act(dx, dx_add)
+
+    def wgrad(self, d_raw):
+        """Weight gradient, fp32 OIHW like conv.weight."""
+        pw = self.pw
+        # the kernel reduces over every channel of the tensor it reads: 32 patch columns, or Cin padded to 8 (stem)
+        dw = ops.conv_wgrad(self.xin, d_raw, self.xin.shape[-1], pw.cout, self.taps, img_add=self.img_add)
+        if self.kind == "patches":          # [Cout, 32, 1, 1]: column (r*3+s)*Cin + c holds weight[:, c, r, s]
+            return dw[:, :9 * pw.cin, 0, 0].reshape(pw.cout, 3, 3, pw.cin).permute(0, 3, 1, 2).contiguous()
+        return dw[:, :pw.cin].contiguous() if dw.shape[1] != pw.cin else dw
+
+
+class _CbaState:
+    """What one conv+BN(+residual)(+ReLU) stage keeps for its backward pass."""
+    __slots__ = ("form", "bn", "frozen", "relu", "has_res", "raw", "y", "mi", "ss", "pg")
+
+
+def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True, mode="batch"):
+    """conv (1x1 / 3x3; stride 1 with any dilation, or stride 2; see _ConvForm) + BatchNorm in `mode` (see _bn_mode)
+    + optional residual + ReLU. Returns (y, state for cba_backward).
+      "batch" : three launches: conv (raw + per-CTA statistics) -> finalise (+ SyncBN exchange) -> apply.
+      "frozen": running statistics — no statistics, no SyncBN exchange, running statistics and num_batches_tracked
+                untouched. When gamma needs a gradient: conv (raw) -> apply with the folded scale / shift, and raw is
+                kept for dgamma's x-hat; otherwise the eval kernel, and only x and y are kept.
+      "eval"  : the eval kernel: conv + folded BN + residual + ReLU in one launch."""
+    form = _ConvForm(conv, x, input_needs_grad, mode)
+    raw = mi = pg = None
+    if mode == "batch":
+        raw, sp = form.fprop(stats=True)
+        pg = _sync_group(bn)
+        mi, ss = _batch_stats(sp, bn, pg)
+    else:
+        ss = ops.bn_fold_eval(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+        if mode == "frozen" and bn.weight is not None and bn.weight.requires_grad:
+            raw, _ = form.fprop()
+    if raw is not None:
+        y = ops.bn_apply(raw, ss, residual=residual, relu=relu, out=out)
+    else:
+        y, _ = form.fprop(epi=EPI_AFFINE, relu=relu, scale=ss[0], shift=ss[1], residual=residual, out=out)
     st = _CbaState()
-    # ReLU mask for backward: with a residual it needs the saved output, otherwise it is recomputed from raw
-    need_y = relu and residual is not None
-    st.frozen = False
-    st.xin, st.raw, st.y, st.mi, st.gamma = xin, raw, (y if need_y else None), mi, bn.weight
-    st.ss = ss if (relu and not need_y) else None
-    st.pw, st.k, st.dil, st.stride, st.relu, st.pg, st.world = pw, k, dil, stride, relu, pg, world
-    st.in_shape, st.has_res = (n, h, w, cx), residual is not None
+    # ReLU mask for backward: recomputed from raw when there is raw and no residual, else the saved output
+    need_y = relu and (residual is not None or raw is None)
+    st.form, st.bn, st.frozen, st.relu, st.has_res = form, bn, mode != "batch", relu, residual is not None
+    st.raw, st.y, st.mi, st.pg = raw, (y if need_y else None), mi, pg
+    st.ss = ss if (mode == "batch" and relu and not need_y) else None     # the frozen backward derives its own
     return y, st
 
 
 def cba_backward(st, dy, need_dx=True, need_dw=True, need_dres=False, dx_add=None):
     """Backward of cba_forward: returns (dx, dw, dgamma, dbeta, dres). `dx_add` (same shape as dx) is summed into
-    dx inside the dgrad epilogue (AFFINE mode with a residual operand) — this is how gradient fan-in is fused."""
-    pw = st.pw
-    n, h, w, cx = st.in_shape
+    dx (see _ConvForm.dgrad)."""
+    bn = st.bn
+    want_dres = st.has_res and need_dres
     if st.frozen:
-        if not (need_dx or need_dw or (st.has_res and need_dres) or st.want_g or st.want_b):
+        want_g, want_b = st.raw is not None, bn.bias is not None and bn.bias.requires_grad
+        if not (need_dx or need_dw or want_dres or want_g or want_b):
             return None, None, None, None, None
         # one pass: d_raw = dz*scale (+ dres = dz) and, when gamma / beta need them, the deterministic channel sums
-        d_raw, dres, sums = ops.bn_bwd_frozen(dy if dy.is_contiguous() else dy.contiguous(), st.y, st.raw, st.gamma,
-                                              st.beta, st.rm, st.rv, st.eps, st.relu,
-                                              want_dres=st.has_res and need_dres, want_sums=st.want_g or st.want_b)
-        dgamma = sums[1] if st.want_g else None
-        dbeta = sums[0] if st.want_b else None
+        d_raw, dres, sums = ops.bn_bwd_frozen(dy if dy.is_contiguous() else dy.contiguous(), st.y, st.raw, bn.weight,
+                                              bn.bias, bn.running_mean, bn.running_var, bn.eps, st.relu,
+                                              want_dres=want_dres, want_sums=want_g or want_b)
+        dgamma = sums[1] if want_g else None
+        dbeta = sums[0] if want_b else None
     else:
-        d_raw, dres, dgamma, dbeta = _bn_backward(st.pg, st.world, dy, st.y, st.raw, st.mi, st.gamma, st.relu,
-                                                  st.has_res and need_dres, st.ss)
-    dx = dw = None
-    if st.stride == 0:      # patch form of the stem conv (no input gradient by construction)
-        if need_dx:
-            raise RuntimeError("semseg_b200: the patch form of the stem conv was chosen but dx is requested")
-        if need_dw:
-            cin = pw.cin
-            dwp = ops.conv_wgrad(st.xin, d_raw, 32, pw.cout, ops.conv_taps(1, 1))          # [Cout, 32, 1, 1]
-            dw = dwp[:, :9 * cin, 0, 0].reshape(pw.cout, 3, 3, cin).permute(0, 3, 1, 2).contiguous()
-        return dx, dw, dgamma, dbeta, dres
-    if st.stride == 1:
-        if need_dx:
-            if dx_add is not None:
-                dx, _ = ops.conv_fprop(d_raw, pw.wd, pw.cin, ops.conv_taps(st.k, st.dil, transpose=True),
-                                       epi=EPI_AFFINE, residual=dx_add)
-            else:
-                dx, _ = ops.conv_fprop(d_raw, pw.wd, pw.cin, ops.conv_taps(st.k, st.dil, transpose=True))
-        if need_dw:
-            dw = ops.conv_wgrad(st.xin, d_raw, cx, pw.cout, ops.conv_taps(st.k, st.dil))
-    else:
-        t2 = ops.conv_taps_s2(st.k, n)
-        if need_dx:
-            if pw.cin % 64 != 0:
-                raise NotImplementedError("semseg_b200: input gradient of a stride-2 conv needs Cin % 64 == 0")
-            hh, wh = st.xin.shape[-3], st.xin.shape[-2]
-            dxp = ops.empty_act((4 * n, hh, wh, pw.cin), ops.is_split(d_raw), dy.device)
-            for q in range(4):
-                sub = [(-t[0], -t[1], t[2]) for t in t2 if t[4] == (q >> 1, q & 1)]
-                part = ops.act_batch_slice(dxp, q * n, (q + 1) * n)
-                if sub:      # dx of phase q: conv of d_raw with the taps that read this phase (mirrored shifts)
-                    ops.conv_fprop(d_raw, pw.wd, pw.cin, sub, out=part, out_nhw=(n, hh, wh))
-                else:
-                    part.zero_()
-            dx = ops.phases_to_space(dxp, n, h, w)
-            if dx_add is not None:
-                dx = ops.add_act(dx, dx_add)
-        if need_dw:
-            dw = ops.conv_wgrad(st.xin, d_raw, cx, pw.cout, [t[:2] for t in t2], img_add=[t[3] for t in t2])
-    if dw is not None and cx != pw.cin and st.stride != 0:
-        dw = dw[:, :pw.cin].contiguous()          # input channels were zero-padded to a multiple of 8 (stem)
+        d_raw, dres, dgamma, dbeta = _bn_backward(st.pg, dy, st.y, st.raw, st.mi, bn.weight, st.relu, want_dres, st.ss)
+    dx = st.form.dgrad(d_raw, dx_add) if need_dx else None
+    dw = st.form.wgrad(d_raw) if need_dw else None
     return dx, dw, dgamma, dbeta, dres
 
 
@@ -350,7 +343,8 @@ class _ConvBnAct(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, residual, conv, bn, relu, out, frozen):
-        y, st = cba_forward(x, conv, bn, relu, residual, out, input_needs_grad=ctx.needs_input_grad[0], frozen=frozen)
+        y, st = cba_forward(x, conv, bn, relu, residual, out, input_needs_grad=ctx.needs_input_grad[0],
+                            mode="frozen" if frozen else "batch")
         ctx.st = st
         if out is not None:
             ctx.mark_dirty(out)
@@ -372,13 +366,14 @@ class _BottleneckFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, blk, frozen, *params):
-        y1, s1 = cba_forward(x, blk.conv1, blk.bn1, True, None, frozen=frozen[0])
-        y2, s2 = cba_forward(y1, blk.conv2, blk.bn2, True, None, frozen=frozen[1])
+        m1, m2, m3, md = ("frozen" if f else "batch" for f in frozen)
+        y1, s1 = cba_forward(x, blk.conv1, blk.bn1, True, None, mode=m1)
+        y2, s2 = cba_forward(y1, blk.conv2, blk.bn2, True, None, mode=m2)
         if blk.downsample is not None:
-            res, sd = cba_forward(x, blk.downsample[0], blk.downsample[1], False, None, frozen=frozen[3])
+            res, sd = cba_forward(x, blk.downsample[0], blk.downsample[1], False, None, mode=md)
         else:
             res, sd = x, None
-        y3, s3 = cba_forward(y2, blk.conv3, blk.bn3, True, res, frozen=frozen[2])
+        y3, s3 = cba_forward(y2, blk.conv3, blk.bn3, True, res, mode=m3)
         ctx.states = (s1, s2, s3, sd)
         return y3
 
@@ -456,20 +451,7 @@ def conv_bn_act(x, conv, bn, relu=True, residual=None, out=None):
     # validate() (tool/train.py:353-359) calls model.eval()(input) without torch.no_grad() and never back-propagates,
     # so the result is returned detached (a later .backward() through it raises torch's usual "does not require grad").
     # A frozen BatchNorm of a training network takes this path only when nothing of the stage needs a gradient.
-    ss = ops.bn_fold_eval(bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
-    split = ops.is_split(x)
-    with torch.no_grad():
-        pw = packed(conv, need_dgrad=False, split=split)
-        if conv.stride == (1, 1):
-            y, _ = ops.conv_fprop(x, pw.wf, pw.cout, ops.conv_taps(conv.kernel_size[0], conv.dilation[0]),
-                                  epi=EPI_AFFINE, relu=relu, scale=ss[0], shift=ss[1], residual=residual, out=out)
-        else:
-            n, h, w, _ = x.shape[-4:]
-            t2 = ops.conv_taps_s2(conv.kernel_size[0], n)
-            y, _ = ops.conv_fprop(ops.space_to_phases(x), pw.wf, pw.cout, [t[:3] for t in t2], epi=EPI_AFFINE,
-                                  relu=relu, scale=ss[0], shift=ss[1], residual=residual, out=out,
-                                  img_add=[t[3] for t in t2], out_nhw=(n, (h - 1) // 2 + 1, (w - 1) // 2 + 1))
-    return y
+    return cba_forward(x, conv, bn, relu, residual, out, mode="eval")[0]
 
 
 # ------------------------------------------------------------------------------------------------ classifier

@@ -59,16 +59,17 @@ def upsample_logits(logits_nhwc, size, zoom_factor):
     return x
 
 
-class PSPNet(nn.Module):
-    def __init__(self, layers=50, bins=(1, 2, 3, 6), dropout=0.1, classes=2, zoom_factor=8, use_ppm=True,
-                 criterion=nn.CrossEntropyLoss(ignore_index=255), pretrained=True):
-        super(PSPNet, self).__init__()
+class _SegNet(nn.Module):
+    """The network body PSPNet and PSANet share (model/pspnet.py:29-105, model/psanet.py:101-179): the dilated ResNet,
+    a context module between layer4 and `cls`, the `cls` / `aux` heads and the forward. `context` is None or
+    (attribute name, factory called with the feature width); the subclass applies the module in `_context_nhwc`."""
+
+    def __init__(self, layers, dropout, classes, zoom_factor, criterion, pretrained, context):
+        super(_SegNet, self).__init__()
         assert layers in [50, 101, 152]
-        assert 2048 % len(bins) == 0
         assert classes > 1
         assert zoom_factor in [1, 2, 4, 8]
         self.zoom_factor = zoom_factor
-        self.use_ppm = use_ppm
         self.criterion = criterion
 
         if layers == 50:
@@ -93,8 +94,9 @@ class PSPNet(nn.Module):
                 m.stride = (1, 1)
 
         fea_dim = 2048
-        if use_ppm:
-            self.ppm = PPM(fea_dim, int(fea_dim / len(bins)), bins)
+        if context is not None:
+            name, make = context
+            setattr(self, name, make(fea_dim))       # built here: construction order decides the initial weights
             fea_dim *= 2
         self.cls = nn.Sequential(
             nn.Conv2d(fea_dim, 512, kernel_size=3, padding=1, bias=False),
@@ -166,12 +168,22 @@ class PSPNet(nn.Module):
         if self.training:       # layer3's output feeds layer4 and the aux head: explicit fan-out (native gradient add)
             t_tmp, t_aux = SF.fork(t_tmp, 2)
         t = self.layer4.forward_nhwc(t_tmp)
-        if self.use_ppm:
-            t = self.ppm.forward_nhwc(t)
-        return head_forward_nhwc(self.cls, t), t_aux
+        return head_forward_nhwc(self.cls, self._context_nhwc(t)), t_aux
 
     def _eval_logits_nhwc(self, x):
         """The eval forward up to the classifier: fp32 NHWC logits [N, h', w', classes]. The sliding-window engine
         (inference.py) upsamples, scores and flip-averages them in one native kernel."""
         assert not self.training, "_eval_logits_nhwc is the eval-mode forward"
         return self._logits_nhwc(x)[0]
+
+
+class PSPNet(_SegNet):
+    def __init__(self, layers=50, bins=(1, 2, 3, 6), dropout=0.1, classes=2, zoom_factor=8, use_ppm=True,
+                 criterion=nn.CrossEntropyLoss(ignore_index=255), pretrained=True):
+        assert 2048 % len(bins) == 0
+        super(PSPNet, self).__init__(layers, dropout, classes, zoom_factor, criterion, pretrained,
+                                     ("ppm", lambda dim: PPM(dim, int(dim / len(bins)), bins)) if use_ppm else None)
+        self.use_ppm = use_ppm
+
+    def _context_nhwc(self, t):
+        return self.ppm.forward_nhwc(t) if self.use_ppm else t
