@@ -1244,6 +1244,10 @@ extern "C" int semseg_conv_splitk_finish(const float* partial, int k_slices, lon
   SB_CHECK_ARG(part_pitch % 4 == 0 && part_pitch >= C && slice_stride % 4 == 0 && y_pitch % 8 == 0 &&
                    (!residual || res_pitch % 8 == 0),
                "conv_splitk_finish: pitches must keep 16-byte alignment");
+  SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(partial) | reinterpret_cast<uintptr_t>(y) |
+                 reinterpret_cast<uintptr_t>(y_lo) | reinterpret_cast<uintptr_t>(residual) |
+                 reinterpret_cast<uintptr_t>(residual_lo)) & 15) == 0,
+               "conv_splitk_finish: partial, y and residual must be 16-byte aligned");
   SB_CHECK_ARG(epi_mode == SEMSEG_EPI_RAW || epi_mode == SEMSEG_EPI_AFFINE, "conv_splitk_finish: RAW or AFFINE only");
   SB_CHECK_ARG(!stats_partial || epi_mode == SEMSEG_EPI_RAW, "conv_splitk_finish: statistics only in RAW mode");
   const bool split = y_lo != nullptr;

@@ -236,7 +236,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
         if (p.epi_mode == SEMSEG_EPI_F32) {
           const bool bias = p.shift != nullptr && k_slice == 0;
-          const bool pairs = (p.out_pitch & 1) == 0;
+          // float2 stores need 8-byte alignment: an even pitch and slice stride, and an output that starts on an even
+          // float (out_f32 may be a channel slice of a wider buffer at any offset)
+          const bool pairs = ((p.out_pitch | p.slice_stride) & 1) == 0 &&
+                             (reinterpret_cast<uintptr_t>(p.out_f32) & 7) == 0;
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
             if (!rv[i]) continue;
@@ -534,7 +537,10 @@ extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
     SB_CHECK_ARG(d->y != nullptr, "conv: null y");
     SB_CHECK_ARG(d->Cout % 64 == 0, "conv: bf16 epilogue needs Cout %% 64 == 0 (got %d)", d->Cout);
     SB_CHECK_ARG(d->y_pitch % 8 == 0 && d->y_pitch >= d->Cout, "conv: bad y_pitch %d", d->y_pitch);
-    if (d->residual) SB_CHECK_ARG(d->res_pitch % 8 == 0, "conv: res_pitch must be a multiple of 8");
+    if (d->residual)   // the epilogue reads the residual as bf16 pairs
+      SB_CHECK_ARG(d->res_pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(d->residual) & 3) == 0 &&
+                       (reinterpret_cast<uintptr_t>(d->residual_lo) & 3) == 0,
+                   "conv: res_pitch must be a multiple of 8 and the residual 4-byte aligned");
     uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N};
     uint64_t str[3] = {(uint64_t)d->y_pitch * 2, (uint64_t)d->y_pitch * 2 * d->W,
                        (uint64_t)d->y_pitch * 2 * d->W * d->H};
