@@ -227,11 +227,7 @@ int semseg_phases_to_space(const void* xp, int N, int H, int W, int C, void* x, 
  */
 /* Merge the conv epilogue's per-CTA partials [rows][3][C] (Chan) into per-channel (mean, M2, count): out_stats [3][C]. */
 int semseg_bn_merge_partials(const float* stats_partial, int rows, int C, float* out_stats, void* stream);
-/* Per-channel statistics of an arbitrary NHWC bf16 tensor [M pixels][C] (used where the producer is not the
- * conv kernel): out_stats [3][C] = (mean, M2, count). */
-int semseg_bn_stats(const void* x, int M, int C, int pitch, float* workspace, long long workspace_floats,
-                    float* out_stats, void* stream);
-/* Scratch floats the two-stage reductions (bn_stats, bn_bwd_reduce) need for an [M][C] tensor. */
+/* Scratch floats of the two-stage backward reductions (bn_bwd_reduce, bn_bwd_frozen) for an [M][C] tensor. */
 long long semseg_bn_workspace_floats(int M, int C);
 /* Merge R rank-stat blocks [R][3][C] (R = 1 without SyncBN) and finalise:
  *   mean_invstd [3][C] = (mean, 1/sqrt(var+eps), total samples per channel over all ranks — every finalize entry point
@@ -240,31 +236,22 @@ long long semseg_bn_workspace_floats(int M, int C);
 int semseg_bn_finalize(const float* rank_stats, int R, int C, const float* gamma, const float* beta, float eps,
                        float momentum, float* running_mean, float* running_var, float* mean_invstd,
                        float* scale_shift, void* stream);
-/* Single-rank fast path: semseg_bn_merge_partials + semseg_bn_finalize (R = 1) in one launch. */
-int semseg_bn_finalize_partials(const float* stats_partial, int rows, int C, const float* gamma, const float* beta, float eps, float momentum,
-                                float* running_mean, float* running_var, float* mean_invstd, float* scale_shift,
-                                void* stream);
-/* SyncBatchNorm exchange over NVLink peer memory instead of NCCL (one kernel per exchange). peer_bufs[world] /
- * peer_flags[world] are device pointers into every rank's symmetric (peer-mapped) allocation: a zero-initialised buffer
- * of n_slots*world*slot_floats 8-byte words (every value travels as one {fp32, sequence number} word that the sender
- * stores into sub-block `rank` of the slot in every peer's buffer; the receiver polls its own memory: flag-in-data, no
- * fences) and a uint32 flag array [n_slots][world] (unused by this protocol, kept for ABI stability); `counter` is a zeroed local uint32;
- * `slot` must be unique per exchange within a step and the sequence number strictly increasing per step (same on every
- * rank): it is `seq`, or — when seq_ptr is non-NULL — the uint32 read from that device address when the kernel runs (a
- * device-resident step counter, so that a captured CUDA graph with baked-in slots can be replayed).
- *   finalize_p2p   : per-CTA conv partials -> exchange (mean, M2, n) -> cross-rank merge in rank order -> finalise.
- *   bwd_reduce_p2p : local [sum dz, sum dz*xhat] -> sums_local; exchanged and added in rank order -> sums_total. */
-int semseg_bn_finalize_p2p(const float* stats_partial, int rows, int C, const float* gamma, const float* beta,
-                           float eps, float momentum, float* running_mean, float* running_var, float* mean_invstd,
-                           float* scale_shift, void* const* peer_bufs, void* const* peer_flags, void* counter,
-                           int world, int rank, int slot, int slot_floats, unsigned seq, const void* seq_ptr,
-                           void* stream);
-int semseg_bn_bwd_reduce_p2p(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo,
-                             int y_pitch, const void* x, const void* x_lo, int x_pitch, const float* mean_invstd,
-                             const float* scale_shift, int M, int C, int relu, float* workspace,
-                             long long workspace_floats, float* sums_local, float* sums_total,
-                             void* const* peer_bufs, void* const* peer_flags, void* counter, int world, int rank,
-                             int slot, int slot_floats, unsigned seq, const void* seq_ptr, void* stream);
+/* Peer exchange (SyncBatchNorm over NVLink peer memory instead of NCCL, inside the kernel): the arguments
+ * (peer_bufs, world, rank, slot, slot_floats, seq_ptr) that semseg_bn_finalize_partials and semseg_bn_bwd_reduce take.
+ * peer_bufs == NULL: a single rank, and the other five are ignored. Otherwise peer_bufs[world] (world <= 8, rank < world)
+ * are device pointers into every rank's symmetric (peer-mapped) allocation: a zero-initialised buffer of
+ * n_slots*world*slot_floats 8-byte words. Every value travels as one {fp32, sequence number} word that the sender stores
+ * into sub-block `rank` of the slot in every peer's buffer; the receiver polls its own memory (flag-in-data, no fences).
+ * `slot` must be unique per exchange within a step; the sequence number is the uint32 read from the device address
+ * seq_ptr when the kernel runs, strictly increasing per step and the same on every rank (a device-resident step
+ * counter, so that a captured CUDA graph with baked-in slots can be replayed). */
+/* Merge the per-CTA conv partials [rows][3][C] and finalise in one launch, like semseg_bn_merge_partials +
+ * semseg_bn_finalize (R = 1). With peers, this rank's (mean, M2, n) [3][C] (3*C <= slot_floats) is exchanged and the
+ * ranks' moments are merged in rank order before the finalise; every rank computes the same bits. */
+int semseg_bn_finalize_partials(const float* stats_partial, int rows, int C, const float* gamma, const float* beta,
+                                float eps, float momentum, float* running_mean, float* running_var, float* mean_invstd,
+                                float* scale_shift, void* const* peer_bufs, int world, int rank, int slot,
+                                int slot_floats, const void* seq_ptr, void* stream);
 /* Eval-mode folding: scale = gamma/sqrt(var+eps), shift = beta - mean*scale. */
 int semseg_bn_fold_eval(const float* gamma, const float* beta, const float* running_mean,
                         const float* running_var, float eps, int C, float* scale_shift, void* stream);
@@ -273,12 +260,15 @@ int semseg_bn_apply(const void* x, const void* x_lo, int x_pitch, const float* s
                     const void* residual_lo, int res_pitch, void* y, void* y_lo, int y_pitch, int M, int C, int relu,
                     void* stream);
 /* Backward reduce: with dz = dy * (y > 0 if relu) and xhat = (x - mean)*invstd,
- *   sums [2][C] = (sum dz, sum dz*xhat). y may be NULL when relu == 0; when relu != 0 and y == NULL the mask is
- *   recomputed as fma(x, scale, shift) > 0 from scale_shift [2][C] (valid when the forward had no residual). */
+ *   sums [2][C] = this rank's (sum dz, sum dz*xhat). y may be NULL when relu == 0; when relu != 0 and y == NULL the mask
+ *   is recomputed as fma(x, scale, shift) > 0 from scale_shift [2][C] (valid when the forward had no residual).
+ *   With peers (see the peer exchange above; 2*C <= slot_floats), sums_total [2][C] = the sums added over the ranks in
+ *   rank order; without, sums_total may be NULL and is not written. */
 int semseg_bn_bwd_reduce(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo, int y_pitch,
                          const void* x, const void* x_lo, int x_pitch, const float* mean_invstd,
                          const float* scale_shift, int M, int C, int relu, float* workspace,
-                         long long workspace_floats, float* sums, void* stream);
+                         long long workspace_floats, float* sums, float* sums_total, void* const* peer_bufs,
+                         int world, int rank, int slot, int slot_floats, const void* seq_ptr, void* stream);
 /* Backward apply: dx = gamma*invstd*(dz - sum_dz/count - xhat*sum_dzxhat/count);
  *   dres (optional) = dz; dgamma = sum_dzxhat, dbeta = sum_dz written to dgamma_dbeta [2][C].
  *   count = total number of samples per channel across all ranks; count <= 0 takes it from mean_invstd row 2 (what

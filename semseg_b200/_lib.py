@@ -117,20 +117,15 @@ SIGNATURES = {
     "semseg_space_to_phases": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_phases_to_space": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_bn_merge_partials": (c_int, [c_vp, c_int, c_int, c_vp, c_vp]),
-    "semseg_bn_stats": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_ll, c_vp, c_vp]),
     "semseg_bn_workspace_floats": (c_ll, [c_int, c_int]),
     "semseg_bn_finalize": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "semseg_bn_finalize_partials": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "semseg_bn_finalize_p2p": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
-                                       c_vp, c_int, c_int, c_int, c_int, ctypes.c_uint, c_vp, c_vp]),
-    "semseg_bn_bwd_reduce_p2p": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int,
-                                         c_int, c_int, c_vp, c_ll, c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int,
-                                         c_int, ctypes.c_uint, c_vp, c_vp]),
+    "semseg_bn_finalize_partials": (c_int, [c_vp, c_int, c_int, c_vp, c_vp, c_f, c_f, c_vp, c_vp, c_vp, c_vp,
+                                            c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_bn_fold_eval": (c_int, [c_vp, c_vp, c_vp, c_vp, c_f, c_int, c_vp, c_vp]),
     "semseg_bn_apply": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int, c_int, c_int,
                                 c_vp]),
     "semseg_bn_bwd_reduce": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_int,
-                                     c_int, c_vp, c_ll, c_vp, c_vp]),
+                                     c_int, c_vp, c_ll, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_bn_bwd_apply": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,
                                     c_f, c_int, c_int, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp]),
     "semseg_bn_bwd_frozen": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_vp,

@@ -23,39 +23,6 @@ __device__ __forceinline__ Moments merge(const Moments& a, const Moments& b) {
   return r;
 }
 
-// ------------------------------------------------------------------------------------------------
-// partials [T][2][C] (sum, M2 about the tile mean) + counts [T]  ->  out [3][C] (mean, M2, count)
-// block = 32 channels x 32 tile lanes.
-__global__ void __launch_bounds__(1024) bn_merge_partials_kernel(const float* __restrict__ part, const float* __restrict__ cnt, int T, int C,
-                                         float* __restrict__ out) {
-  __shared__ Moments sm[32][33];
-  const int cl = threadIdx.x & 31;
-  const int tl = threadIdx.x >> 5;
-  const int c = blockIdx.x * 32 + cl;
-  Moments acc = {0.f, 0.f, 0.f};
-  if (c < C) {
-    for (int t = tl; t < T; t += 32) {
-      const float n = cnt[t];
-      if (n > 0.f) {
-        Moments m;
-        m.n = n;
-        m.mean = part[(static_cast<size_t>(t) * 2) * C + c] / n;
-        m.m2 = part[(static_cast<size_t>(t) * 2 + 1) * C + c];
-        acc = merge(acc, m);
-      }
-    }
-  }
-  sm[tl][cl] = acc;
-  __syncthreads();
-  if (tl == 0 && c < C) {
-    Moments r = sm[0][cl];
-    for (int i = 1; i < 32; ++i) r = merge(r, sm[i][cl]);
-    out[c] = r.mean;
-    out[C + c] = r.m2;
-    out[2 * C + c] = r.n;
-  }
-}
-
 // The conv epilogue's statistics buffer is [rows][3][C] = (sum, sum of squares, count) per epilogue warp.
 
 // Block-wide merge of the conv statistics rows for CH channels starting at c0. A block is 1024 threads = CH channels x
@@ -124,9 +91,28 @@ __device__ __forceinline__ Moments block_conv_moments(const float* __restrict__ 
   return r;  // valid in lane 0 of warps 0..CH-1
 }
 
-// Channels per block such that a layer needs at most 128 blocks (one wave; the peer-exchange kernels additionally
-// need all of their blocks co-resident because they spin on the peers' flags).
+// Channels per block such that a layer needs at most 128 blocks (one wave). The peer exchange does not rely on that:
+// its blocks only wait for words the peers push, which needs none of this GPU's SMs (st_ll / ld_ll below).
 static int stats_group_channels(int C) { return C <= 1024 ? 8 : (C <= 2048 ? 16 : 32); }
+
+// Launch helper: KERNEL<kCH> with kCH = stats_group_channels(C) channels per block.
+#define SB_STATS_GROUP_DISPATCH(C, ...)  \
+  do {                                   \
+    switch (stats_group_channels(C)) {   \
+      case 8: {                          \
+        constexpr int kCH = 8;           \
+        __VA_ARGS__;                     \
+      } break;                           \
+      case 16: {                         \
+        constexpr int kCH = 16;          \
+        __VA_ARGS__;                     \
+      } break;                           \
+      default: {                         \
+        constexpr int kCH = 32;          \
+        __VA_ARGS__;                     \
+      } break;                           \
+    }                                    \
+  } while (0)
 
 template <int CH>
 __global__ void __launch_bounds__(1024) bn_merge_conv_partials_kernel(const float* __restrict__ part, int T, int C,
@@ -142,105 +128,104 @@ __global__ void __launch_bounds__(1024) bn_merge_conv_partials_kernel(const floa
 }
 
 // ------------------------------------------------------------------------------------------------
-// Single-rank fast path: merge the per-tile partials AND finalise in one launch (no SyncBN exchange needed).
-template <int CH>
+// SyncBatchNorm statistics exchange over NVLink peer memory (torch symmetric memory): fused into the finalise and the
+// backward's final reduction (their PEER form), no NCCL call, no stream hop; the protocol is described at st_ll / ld_ll
+// below. The cross-rank merge is done in rank order on every rank, so all ranks compute bit-identical statistics.
+// Kernels take it as a `const __grid_constant__` parameter: buf[p] with a run-time p is then read from the parameter
+// bank instead of from a copy of the whole struct in local memory.
+struct PeerArgs {
+  float* buf[8];        // peer-mapped data buffers (buf[rank] is local): 8-byte {value, seq} words, [slot][src rank][slot_floats]
+  int world, rank, slot, slot_floats;
+  const unsigned* seq_ptr;  // device-resident step counter = the sequence number of this exchange (read at run time, so
+                            // a captured CUDA graph with the slot baked in can be replayed)
+  long long timeout_ticks;
+};
+
+// Exchange protocol ("LL", flag-in-data): a value travels as ONE 8-byte word {fp32 bits, sequence number}. The sender
+// stores the word straight into sub-block `rank` of the slot in EVERY peer's buffer (posted NVLink stores); the receiver
+// polls the word in its OWN memory until the sequence number matches. 8-byte stores are single transactions, so there is
+// no separate flag, no system-scope fence, no cross-block counter: every thread that finishes a channel exchanges that
+// channel on its own, the latency is one NVLink store, and a block only ever waits for data that peers push without
+// needing any of this GPU's SMs (no co-residency requirement, nothing an NCCL kernel sharing the SMs can dead-lock with).
+// A peer that never arrives trips the watchdog (default 10 minutes, SEMSEG_B200_P2P_TIMEOUT_S) instead of hanging the GPU.
+__device__ __forceinline__ void st_ll(unsigned long long* p, float v, unsigned seq) {
+  const unsigned long long w = (static_cast<unsigned long long>(seq) << 32) | __float_as_uint(v);
+  asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
+}
+__device__ __forceinline__ float ld_ll(const unsigned long long* p, unsigned seq, const PeerArgs& pa, int peer) {
+  unsigned long long w;
+  const long long t0 = clock64();
+  for (;;) {
+    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(w) : "l"(p) : "memory");
+    if (static_cast<unsigned>(w >> 32) == seq) break;
+    if (clock64() - t0 > pa.timeout_ticks) {
+      printf("semseg_b200: SyncBN peer exchange timed out (rank %d waiting for rank %d, slot %d, seq %u)\n", pa.rank, peer,
+             pa.slot, seq);
+      __trap();
+    }
+  }
+  return __uint_as_float(static_cast<unsigned>(w & 0xffffffffu));
+}
+
+// Finalise channel c from its moments over all ranks: mean_invstd [3][C] = (mean, invstd, samples per channel over all
+// ranks — the backward's 1/count), scale_shift [2][C] = (gamma*invstd, beta - mean*scale), and the running statistics
+// (momentum, unbiased variance) when given. Every finalise kernel ends here, so equal moments give equal bits.
+__device__ __forceinline__ void finalize_channel(const Moments& r, int c, int C, const float* __restrict__ gamma,
+                                                 const float* __restrict__ beta, float eps, float momentum,
+                                                 float* __restrict__ running_mean, float* __restrict__ running_var,
+                                                 float* __restrict__ mean_invstd, float* __restrict__ scale_shift) {
+  const float var = r.n > 0.f ? r.m2 / r.n : 0.f;
+  const float invstd = rsqrtf(var + eps);
+  mean_invstd[c] = r.mean;
+  mean_invstd[C + c] = invstd;
+  mean_invstd[2 * C + c] = r.n;
+  const float sc = (gamma ? gamma[c] : 1.f) * invstd;
+  scale_shift[c] = sc;
+  scale_shift[C + c] = (beta ? beta[c] : 0.f) - r.mean * sc;
+  if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * r.mean;
+  if (running_var) {
+    const float unb = r.n > 1.f ? r.m2 / (r.n - 1.f) : var;
+    running_var[c] = (1.f - momentum) * running_var[c] + momentum * unb;
+  }
+}
+
+// Merge this rank's conv partials and finalise in one launch. PEER: exchange the channel's (mean, M2, n) with every
+// rank and merge the ranks' moments in rank order before finalising.
+template <int CH, bool PEER>
 __global__ void __launch_bounds__(1024) bn_finalize_partials_kernel(const float* __restrict__ part, int T, int C,
                                             const float* __restrict__ gamma, const float* __restrict__ beta,
                                             float eps, float momentum, float* __restrict__ running_mean,
                                             float* __restrict__ running_var, float* __restrict__ mean_invstd,
-                                            float* __restrict__ scale_shift) {
+                                            float* __restrict__ scale_shift, const __grid_constant__ PeerArgs pa) {
   __shared__ Moments sm[32][CH + 1];
-  const Moments r = block_conv_moments<CH>(part, T, C, blockIdx.x * CH, sm);
+  Moments r = block_conv_moments<CH>(part, T, C, blockIdx.x * CH, sm);
   const int c = blockIdx.x * CH + (threadIdx.x >> 5);
-  if ((threadIdx.x & 31) == 0 && (threadIdx.x >> 5) < CH && c < C) {
-    const float var = r.n > 0.f ? r.m2 / r.n : 0.f;
-    const float invstd = rsqrtf(var + eps);
-    mean_invstd[c] = r.mean;
-    mean_invstd[C + c] = invstd;
-    mean_invstd[2 * C + c] = r.n;     // samples per channel over all ranks (the backward's 1/count)
-    const float sc = (gamma ? gamma[c] : 1.f) * invstd;
-    scale_shift[c] = sc;
-    scale_shift[C + c] = (beta ? beta[c] : 0.f) - r.mean * sc;
-    if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * r.mean;
-    if (running_var) {
-      const float unb = r.n > 1.f ? r.m2 / (r.n - 1.f) : var;
-      running_var[c] = (1.f - momentum) * running_var[c] + momentum * unb;
+  if (!((threadIdx.x & 31) == 0 && (threadIdx.x >> 5) < CH && c < C)) return;   // this thread finishes channel c
+  if constexpr (PEER) {
+    const unsigned seq = *pa.seq_ptr;
+    const size_t slot0 = static_cast<size_t>(pa.slot) * pa.world * pa.slot_floats;
+    const size_t off = slot0 + static_cast<size_t>(pa.rank) * pa.slot_floats;
+    for (int p = 0; p < pa.world; ++p) {
+      unsigned long long* dst = reinterpret_cast<unsigned long long*>(pa.buf[p]) + off;
+      st_ll(dst + c, r.mean, seq);
+      st_ll(dst + C + c, r.m2, seq);
+      st_ll(dst + 2 * C + c, r.n, seq);
+    }
+    r = Moments{0.f, 0.f, 0.f};
+    for (int p = 0; p < pa.world; ++p) {
+      const unsigned long long* b = reinterpret_cast<const unsigned long long*>(pa.buf[pa.rank]) + slot0 +
+                                    static_cast<size_t>(p) * pa.slot_floats;
+      Moments m;
+      m.mean = ld_ll(b + c, seq, pa, p);
+      m.m2 = ld_ll(b + C + c, seq, pa, p);
+      m.n = ld_ll(b + 2 * C + c, seq, pa, p);
+      r = merge(r, m);
     }
   }
+  finalize_channel(r, c, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift);
 }
 
-// ------------------------------------------------------------------------------------------------
-// Generic per-chunk statistics of x [M][pitch] (bf16): chunk = rows_per_chunk pixels.
-// block = 8 channel-groups (8 ch each = 64 channels) x 32 pixel lanes; grid = (C/64 ceil, chunks).
-__global__ void bn_chunk_stats_kernel(const __nv_bfloat16* __restrict__ x, int M, int C, int pitch,
-                                      int rows_per_chunk, float* __restrict__ part, float* __restrict__ cnt) {
-  __shared__ float s_sum[32][65];
-  const int gl = threadIdx.x & 7;   // channel group within block
-  const int pl = threadIdx.x >> 3;  // pixel lane 0..31
-  const int c0 = blockIdx.x * 64 + gl * 8;
-  const int chunk = blockIdx.y;
-  const int r0 = chunk * rows_per_chunk;
-  const int r1 = min(M, r0 + rows_per_chunk);
-  const bool active = c0 < C;
-  float s[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  if (active) {
-    for (int r = r0 + pl; r < r1; r += 32) {
-      const uint4 v = *reinterpret_cast<const uint4*>(x + static_cast<size_t>(r) * pitch + c0);
-      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float2 f = __bfloat1622float2(h[q]);
-        s[2 * q] += f.x;
-        s[2 * q + 1] += f.y;
-      }
-    }
-  }
-#pragma unroll
-  for (int q = 0; q < 8; ++q) s_sum[pl][gl * 8 + q] = s[q];
-  __syncthreads();
-  const float n = static_cast<float>(r1 - r0);
-  float mean[8];
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    float t = 0.f;
-    for (int i = 0; i < 32; ++i) t += s_sum[i][gl * 8 + q];
-    mean[q] = t / n;
-    s[q] = t;  // total sum
-  }
-  __syncthreads();
-  float m2[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  if (active) {
-    for (int r = r0 + pl; r < r1; r += 32) {
-      const uint4 v = *reinterpret_cast<const uint4*>(x + static_cast<size_t>(r) * pitch + c0);
-      const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float2 f = __bfloat1622float2(h[q]);
-        const float d0 = f.x - mean[2 * q], d1 = f.y - mean[2 * q + 1];
-        m2[2 * q] = fmaf(d0, d0, m2[2 * q]);
-        m2[2 * q + 1] = fmaf(d1, d1, m2[2 * q + 1]);
-      }
-    }
-  }
-#pragma unroll
-  for (int q = 0; q < 8; ++q) s_sum[pl][gl * 8 + q] = m2[q];
-  __syncthreads();
-  if (pl == 0 && active) {
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      float t = 0.f;
-      for (int i = 0; i < 32; ++i) t += s_sum[i][gl * 8 + q];
-      if (c0 + q < C) {
-        part[(static_cast<size_t>(chunk) * 2) * C + c0 + q] = s[q];
-        part[(static_cast<size_t>(chunk) * 2 + 1) * C + c0 + q] = t;
-      }
-    }
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) cnt[chunk] = n;
-}
-
-// ------------------------------------------------------------------------------------------------
-// rank_stats [R][3][C] -> mean_invstd [2][C], scale_shift [2][C], running stats update.
+// NCCL form: rank_stats [R][3][C] (every rank's merged conv partials, gathered) -> merged in rank order, finalised.
 __global__ void bn_finalize_kernel(const float* __restrict__ rs, int R, int C, const float* __restrict__ gamma,
                                    const float* __restrict__ beta, float eps, float momentum,
                                    float* __restrict__ running_mean, float* __restrict__ running_var,
@@ -256,21 +241,7 @@ __global__ void bn_finalize_kernel(const float* __restrict__ rs, int R, int C, c
     m.n = b[2 * C + c];
     acc = merge(acc, m);
   }
-  const float var = acc.n > 0.f ? acc.m2 / acc.n : 0.f;
-  const float invstd = rsqrtf(var + eps);
-  mean_invstd[c] = acc.mean;
-  mean_invstd[C + c] = invstd;
-  mean_invstd[2 * C + c] = acc.n;
-  const float g = gamma ? gamma[c] : 1.f;
-  const float bt = beta ? beta[c] : 0.f;
-  const float sc = g * invstd;
-  scale_shift[c] = sc;
-  scale_shift[C + c] = bt - acc.mean * sc;
-  if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * acc.mean;
-  if (running_var) {
-    const float unb = acc.n > 1.f ? acc.m2 / (acc.n - 1.f) : var;
-    running_var[c] = (1.f - momentum) * running_var[c] + momentum * unb;
-  }
+  finalize_channel(acc, c, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift);
 }
 
 // Running-statistics folding of channel c: invstd, scale = gamma*invstd, shift = beta - mean*scale. Shared by the eval
@@ -463,9 +434,12 @@ __global__ void bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dy, const
   }
 }
 
-// stage 2: sums[2][C] = sum over chunks (fixed order).
+// stage 2: sums[2][C] = sum over chunks (fixed order). PEER: also exchange this rank's sums with every rank and add
+// them in rank order into sums_total[2][C] (sums, the local ones, feed dgamma/dbeta, which DDP averages later).
+template <bool PEER>
 __global__ void __launch_bounds__(1024) bn_bwd_reduce_final_kernel(const float* __restrict__ part, int chunks, int C,
-                                           float* __restrict__ sums) {
+                                           float* __restrict__ sums, float* __restrict__ sums_total,
+                                           const __grid_constant__ PeerArgs pa) {
   __shared__ float sm[32][33];
   const int cl = threadIdx.x & 31;
   const int tl = threadIdx.x >> 5;
@@ -487,10 +461,20 @@ __global__ void __launch_bounds__(1024) bn_bwd_reduce_final_kernel(const float* 
   }
   sm[tl][cl] = acc;
   __syncthreads();
-  if (tl == 0 && idx < 2 * C) {
+  if (!(tl == 0 && idx < 2 * C)) return;
+  float own = 0.f;
+  for (int i = 0; i < 32; ++i) own += sm[i][cl];
+  sums[idx] = own;
+  if constexpr (PEER) {
+    const unsigned seq = *pa.seq_ptr;
+    const size_t slot0 = static_cast<size_t>(pa.slot) * pa.world * pa.slot_floats;
+    const size_t off = slot0 + static_cast<size_t>(pa.rank) * pa.slot_floats + idx;
+    for (int p = 0; p < pa.world; ++p) st_ll(reinterpret_cast<unsigned long long*>(pa.buf[p]) + off, own, seq);
     float r = 0.f;
-    for (int i = 0; i < 32; ++i) r += sm[i][cl];
-    sums[idx] = r;
+    for (int p = 0; p < pa.world; ++p)
+      r += ld_ll(reinterpret_cast<const unsigned long long*>(pa.buf[pa.rank]) + slot0 + static_cast<size_t>(p) * pa.slot_floats + idx,
+                 seq, pa, p);
+    sums_total[idx] = r;
   }
 }
 
@@ -839,134 +823,6 @@ __global__ void act_to_f32_kernel(const __nv_bfloat16* __restrict__ in, const __
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// SyncBatchNorm statistics exchange over NVLink peer memory (torch symmetric memory): one kernel per exchange, no NCCL
-// call, no stream hop; the protocol is described at st_ll / ld_ll below. The cross-rank merge is done in rank order on
-// every rank, so all ranks compute bit-identical statistics.
-struct PeerArgs {
-  float* buf[8];        // peer-mapped data buffers (buf[rank] is local): 8-byte {value, seq} words, [slot][src rank][slot_floats]
-  unsigned* flags[8];   // (unused by the LL protocol; kept in the ABI)
-  unsigned* counter;    // (unused by the LL protocol)
-  int world, rank, slot, slot_floats;
-  unsigned seq;         // sequence number of this exchange: the value of *seq_ptr when seq_ptr is given, else `seq`
-  const unsigned* seq_ptr;  // device-resident step counter (lets a captured CUDA graph be replayed: the slot is baked
-                            // into the graph, the sequence number is read at run time)
-  long long timeout_ticks;
-};
-
-// Exchange protocol ("LL", flag-in-data): a value travels as ONE 8-byte word {fp32 bits, sequence number}. The sender
-// stores the word straight into sub-block `rank` of the slot in EVERY peer's buffer (posted NVLink stores); the receiver
-// polls the word in its OWN memory until the sequence number matches. 8-byte stores are single transactions, so there is
-// no separate flag, no system-scope fence, no cross-block counter: every thread that finishes a channel exchanges that
-// channel on its own, the latency is one NVLink store, and a block only ever waits for data that peers push without
-// needing any of this GPU's SMs (no co-residency requirement, nothing an NCCL kernel sharing the SMs can dead-lock with).
-// A peer that never arrives trips the watchdog (default 10 minutes, SEMSEG_B200_P2P_TIMEOUT_S) instead of hanging the GPU.
-__device__ __forceinline__ void st_ll(unsigned long long* p, float v, unsigned seq) {
-  const unsigned long long w = (static_cast<unsigned long long>(seq) << 32) | __float_as_uint(v);
-  asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
-}
-__device__ __forceinline__ float ld_ll(const unsigned long long* p, unsigned seq, const PeerArgs& pa, int peer) {
-  unsigned long long w;
-  const long long t0 = clock64();
-  for (;;) {
-    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(w) : "l"(p) : "memory");
-    if (static_cast<unsigned>(w >> 32) == seq) break;
-    if (clock64() - t0 > pa.timeout_ticks) {
-      printf("semseg_b200: SyncBN peer exchange timed out (rank %d waiting for rank %d, slot %d, seq %u)\n", pa.rank, peer,
-             pa.slot, seq);
-      __trap();
-    }
-  }
-  return __uint_as_float(static_cast<unsigned>(w & 0xffffffffu));
-}
-
-// Forward: merge this rank's conv partials, exchange (mean, M2, n), merge over ranks in rank order, finalise.
-template <int CH>
-__global__ void __launch_bounds__(1024) bn_finalize_p2p_kernel(const float* __restrict__ part, int T, int C, const float* __restrict__ gamma,
-                                       const float* __restrict__ beta, float eps, float momentum,
-                                       float* __restrict__ running_mean, float* __restrict__ running_var,
-                                       float* __restrict__ mean_invstd, float* __restrict__ scale_shift, PeerArgs pa) {
-  __shared__ Moments sm[32][CH + 1];
-  const Moments own_m = block_conv_moments<CH>(part, T, C, blockIdx.x * CH, sm);
-  const int c = blockIdx.x * CH + (threadIdx.x >> 5);
-  if (!((threadIdx.x & 31) == 0 && (threadIdx.x >> 5) < CH && c < C)) return;   // this thread finishes channel c
-  const unsigned seq = pa.seq_ptr ? *pa.seq_ptr : pa.seq;
-  const size_t slot0 = static_cast<size_t>(pa.slot) * pa.world * pa.slot_floats;
-  {
-    const size_t off = slot0 + static_cast<size_t>(pa.rank) * pa.slot_floats;
-    for (int p = 0; p < pa.world; ++p) {
-      unsigned long long* dst = reinterpret_cast<unsigned long long*>(pa.buf[p]) + off;
-      st_ll(dst + c, own_m.mean, seq);
-      st_ll(dst + C + c, own_m.m2, seq);
-      st_ll(dst + 2 * C + c, own_m.n, seq);
-    }
-  }
-  Moments r = {0.f, 0.f, 0.f};
-  for (int p = 0; p < pa.world; ++p) {
-    const unsigned long long* b = reinterpret_cast<const unsigned long long*>(pa.buf[pa.rank]) + slot0 +
-                                  static_cast<size_t>(p) * pa.slot_floats;
-    Moments m;
-    m.mean = ld_ll(b + c, seq, pa, p);
-    m.m2 = ld_ll(b + C + c, seq, pa, p);
-    m.n = ld_ll(b + 2 * C + c, seq, pa, p);
-    r = merge(r, m);
-  }
-  const float var = r.n > 0.f ? r.m2 / r.n : 0.f;
-  const float invstd = rsqrtf(var + eps);
-  mean_invstd[c] = r.mean;
-  mean_invstd[C + c] = invstd;
-  mean_invstd[2 * C + c] = r.n;     // samples per channel over all ranks (the backward's 1/count)
-  const float sc = (gamma ? gamma[c] : 1.f) * invstd;
-  scale_shift[c] = sc;
-  scale_shift[C + c] = (beta ? beta[c] : 0.f) - r.mean * sc;
-  if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * r.mean;
-  if (running_var) {
-    const float unb = r.n > 1.f ? r.m2 / (r.n - 1.f) : var;
-    running_var[c] = (1.f - momentum) * running_var[c] + momentum * unb;
-  }
-}
-
-// Backward: finish the local chunk reduction, exchange [sum dz, sum dz*xhat], add over ranks in rank order.
-//   sums_local [2][C] (feeds dgamma/dbeta, averaged later by DDP), sums_total [2][C] (feeds dx).
-__global__ void __launch_bounds__(1024) bn_bwd_reduce_final_p2p_kernel(const float* __restrict__ part, int chunks, int C,
-                                               float* __restrict__ sums_local, float* __restrict__ sums_total,
-                                               PeerArgs pa) {
-  __shared__ float sm[32][33];
-  const int cl = threadIdx.x & 31;
-  const int tl = threadIdx.x >> 5;
-  const int idx = blockIdx.x * 32 + cl;  // over 2*C
-  float acc = 0.f;
-  if (idx < 2 * C) {
-    const int which = idx / C, c = idx - which * C;
-    constexpr int U = 8;
-    for (int t0 = tl; t0 < chunks; t0 += 32 * U) {
-      float v[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int t = t0 + 32 * u;
-        v[u] = t < chunks ? part[(static_cast<size_t>(t) * 2 + which) * C + c] : 0.f;
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) acc += v[u];
-    }
-  }
-  sm[tl][cl] = acc;
-  __syncthreads();
-  if (!(tl == 0 && idx < 2 * C)) return;
-  float own = 0.f;
-  for (int i = 0; i < 32; ++i) own += sm[i][cl];
-  sums_local[idx] = own;
-  const unsigned seq = pa.seq_ptr ? *pa.seq_ptr : pa.seq;
-  const size_t slot0 = static_cast<size_t>(pa.slot) * pa.world * pa.slot_floats;
-  const size_t off = slot0 + static_cast<size_t>(pa.rank) * pa.slot_floats + idx;
-  for (int p = 0; p < pa.world; ++p) st_ll(reinterpret_cast<unsigned long long*>(pa.buf[p]) + off, own, seq);
-  float r = 0.f;
-  for (int p = 0; p < pa.world; ++p)
-    r += ld_ll(reinterpret_cast<const unsigned long long*>(pa.buf[pa.rank]) + slot0 + static_cast<size_t>(p) * pa.slot_floats + idx,
-               seq, pa, p);
-  sums_total[idx] = r;
-}
-
 static int ew_grid(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
   const long long cap = static_cast<long long>(num_sms()) * 16;
@@ -1000,51 +856,63 @@ extern "C" long long semseg_bn_workspace_floats(int M, int C) {
   if (M <= 0 || C <= 0) return 0;
   const int rows = chunk_rows(M);
   const long long chunks = cdiv(M, rows);
-  return chunks * 2 * C + chunks + 3LL * C;
+  return chunks * 2 * C;
+}
+
+// The exchange arguments of semseg_bn_finalize_partials / semseg_bn_bwd_reduce with a peer table: `need_floats` words
+// of this rank's block must fit in a slot.
+static int fill_peer_args(sb::PeerArgs* pa, void* const* peer_bufs, int world, int rank, int slot, int slot_floats,
+                          const void* seq_ptr, int need_floats) {
+  SB_CHECK_ARG(world >= 1 && world <= 8 && rank >= 0 && rank < world, "p2p: world %d rank %d unsupported", world, rank);
+  SB_CHECK_ARG(slot >= 0 && need_floats <= slot_floats, "p2p: slot too small (%d > %d floats)", need_floats,
+               slot_floats);
+  SB_CHECK_ARG(seq_ptr, "p2p: null sequence-number pointer");
+  for (int i = 0; i < world; ++i) {
+    SB_CHECK_ARG(peer_bufs[i], "p2p: null peer pointer %d", i);
+    pa->buf[i] = static_cast<float*>(peer_bufs[i]);
+  }
+  pa->world = world;
+  pa->rank = rank;
+  pa->slot = slot;
+  pa->slot_floats = slot_floats;
+  pa->seq_ptr = static_cast<const unsigned*>(seq_ptr);
+  static long long ticks = 0;
+  if (ticks == 0) {
+    const char* e = getenv("SEMSEG_B200_P2P_TIMEOUT_S");
+    double sec = e ? atof(e) : 600.0;
+    if (!(sec > 0.0)) sec = 600.0;
+    ticks = static_cast<long long>(sec * 2.0e9);
+  }
+  pa->timeout_ticks = ticks;
+  return SEMSEG_OK;
 }
 
 extern "C" int semseg_bn_merge_partials(const float* stats_partial, int rows, int C, float* out_stats, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SB_CHECK_ARG(stats_partial && out_stats && rows > 0 && C > 0, "bn_merge_partials: bad args");
-  switch (stats_group_channels(C)) {
-    case 8: bn_merge_conv_partials_kernel<8><<<cdiv(C, 8), 1024, 0, stream>>>(stats_partial, rows, C, out_stats); break;
-    case 16: bn_merge_conv_partials_kernel<16><<<cdiv(C, 16), 1024, 0, stream>>>(stats_partial, rows, C, out_stats); break;
-    default: bn_merge_conv_partials_kernel<32><<<cdiv(C, 32), 1024, 0, stream>>>(stats_partial, rows, C, out_stats); break;
-  }
+  SB_STATS_GROUP_DISPATCH(C, bn_merge_conv_partials_kernel<kCH><<<cdiv(C, kCH), 1024, 0, stream>>>(stats_partial, rows,
+                                                                                                   C, out_stats));
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
 
-extern "C" int semseg_bn_finalize_partials(const float* stats_partial, int num_tiles, int C,
-                                           const float* gamma, const float* beta, float eps, float momentum,
-                                           float* running_mean, float* running_var, float* mean_invstd,
-                                           float* scale_shift, void* stream_) {
+extern "C" int semseg_bn_finalize_partials(const float* stats_partial, int rows, int C, const float* gamma,
+                                           const float* beta, float eps, float momentum, float* running_mean,
+                                           float* running_var, float* mean_invstd, float* scale_shift,
+                                           void* const* peer_bufs, int world, int rank, int slot, int slot_floats,
+                                           const void* seq_ptr, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(stats_partial && mean_invstd && scale_shift && num_tiles > 0 && C > 0,
-               "bn_finalize_partials: bad args");
-  switch (stats_group_channels(C)) {
-    case 8: bn_finalize_partials_kernel<8><<<cdiv(C, 8), 1024, 0, stream>>>(stats_partial, num_tiles, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift); break;
-    case 16: bn_finalize_partials_kernel<16><<<cdiv(C, 16), 1024, 0, stream>>>(stats_partial, num_tiles, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift); break;
-    default: bn_finalize_partials_kernel<32><<<cdiv(C, 32), 1024, 0, stream>>>(stats_partial, num_tiles, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift); break;
+  SB_CHECK_ARG(stats_partial && mean_invstd && scale_shift && rows > 0 && C > 0, "bn_finalize_partials: bad args");
+  sb::PeerArgs pa = {};
+  if (peer_bufs) {
+    const int r = fill_peer_args(&pa, peer_bufs, world, rank, slot, slot_floats, seq_ptr, 3 * C);
+    if (r) return r;
   }
-  SB_LAUNCHED();
-  return SEMSEG_OK;
-}
-
-extern "C" int semseg_bn_stats(const void* x, int M, int C, int pitch, float* workspace, long long workspace_floats,
-                               float* out_stats, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(x && workspace && out_stats && M > 0 && C > 0, "bn_stats: bad args");
-  SB_CHECK_ARG(C % 8 == 0 && pitch % 8 == 0 && pitch >= C, "bn_stats: C/pitch must be multiples of 8");
-  SB_CHECK_ARG(workspace_floats >= semseg_bn_workspace_floats(M, C), "bn_stats: workspace too small");
-  const int rows = chunk_rows(M);
-  const int chunks = cdiv(M, rows);
-  float* part = workspace;
-  float* cnt = workspace + static_cast<size_t>(chunks) * 2 * C;
-  dim3 grid(cdiv(C, 64), chunks);
-  bn_chunk_stats_kernel<<<grid, 256, 0, stream>>>(static_cast<const bf16*>(x), M, C, pitch, rows, part, cnt);
-  SB_LAUNCHED();
-  bn_merge_partials_kernel<<<cdiv(C, 32), 1024, 0, stream>>>(part, cnt, chunks, C, out_stats);
+  SB_STATS_GROUP_DISPATCH(C, {
+    auto kernel = peer_bufs ? bn_finalize_partials_kernel<kCH, true> : bn_finalize_partials_kernel<kCH, false>;
+    kernel<<<cdiv(C, kCH), 1024, 0, stream>>>(stats_partial, rows, C, gamma, beta, eps, momentum, running_mean,
+                                             running_var, mean_invstd, scale_shift, pa);
+  });
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
@@ -1089,12 +957,27 @@ extern "C" int semseg_bn_apply(const void* x, const void* x_lo, int x_pitch, con
   return SEMSEG_OK;
 }
 
-static int launch_bwd_reduce(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo,
-                             int y_pitch, const void* x, const void* x_lo, int x_pitch, const float* mean_invstd,
-                             const float* scale_shift, int M, int C, int relu, float* workspace, cudaStream_t stream) {
+extern "C" int semseg_bn_bwd_reduce(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo,
+                                    int y_pitch, const void* x, const void* x_lo, int x_pitch,
+                                    const float* mean_invstd, const float* scale_shift, int M, int C, int relu,
+                                    float* workspace, long long workspace_floats, float* sums, float* sums_total,
+                                    void* const* peer_bufs, int world, int rank, int slot, int slot_floats,
+                                    const void* seq_ptr, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SB_CHECK_ARG(dy && x && mean_invstd && workspace && sums && M > 0 && C > 0, "bn_bwd_reduce: bad args");
+  SB_CHECK_ARG(!relu || y || scale_shift, "bn_bwd_reduce: relu needs y or scale_shift");
+  SB_CHECK_ARG(C % 8 == 0 && dy_pitch % 8 == 0 && x_pitch % 8 == 0 && (!(relu && y) || y_pitch % 8 == 0),
+               "bn_bwd_reduce: channels and pitches must be multiples of 8");
+  SB_CHECK_ARG(workspace_floats >= semseg_bn_workspace_floats(M, C), "bn_bwd_reduce: workspace too small");
   const bool split = dy_lo != nullptr;
   SB_CHECK_ARG((x_lo != nullptr) == split && (!(relu && y) || (y_lo != nullptr) == split),
                "bn_bwd_reduce: all tensors must use the same storage form (plain or split)");
+  sb::PeerArgs pa = {};
+  if (peer_bufs) {
+    SB_CHECK_ARG(sums_total, "bn_bwd_reduce: the peer exchange needs sums_total");
+    const int r = fill_peer_args(&pa, peer_bufs, world, rank, slot, slot_floats, seq_ptr, 2 * C);
+    if (r) return r;
+  }
   const int rows = chunk_rows(M);
   const int chunks = cdiv(M, rows);
   dim3 grid(cdiv(C, 64), chunks);
@@ -1104,23 +987,8 @@ static int launch_bwd_reduce(const void* dy, const void* dy_lo, int dy_pitch, co
                              static_cast<const bf16*>(x), static_cast<const bf16*>(x_lo), x_pitch, mean_invstd,
                              scale_shift, M, C, relu, rows, workspace));
   SB_LAUNCHED();
-  return SEMSEG_OK;
-}
-
-extern "C" int semseg_bn_bwd_reduce(const void* dy, const void* dy_lo, int dy_pitch, const void* y, const void* y_lo,
-                                    int y_pitch, const void* x, const void* x_lo, int x_pitch,
-                                    const float* mean_invstd, const float* scale_shift, int M, int C, int relu,
-                                    float* workspace, long long workspace_floats, float* sums, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(dy && x && mean_invstd && workspace && sums && M > 0 && C > 0, "bn_bwd_reduce: bad args");
-  SB_CHECK_ARG(!relu || y || scale_shift, "bn_bwd_reduce: relu needs y or scale_shift");
-  SB_CHECK_ARG(C % 8 == 0 && dy_pitch % 8 == 0 && x_pitch % 8 == 0 && (!(relu && y) || y_pitch % 8 == 0),
-               "bn_bwd_reduce: channels and pitches must be multiples of 8");
-  SB_CHECK_ARG(workspace_floats >= semseg_bn_workspace_floats(M, C), "bn_bwd_reduce: workspace too small");
-  int r = launch_bwd_reduce(dy, dy_lo, dy_pitch, y, y_lo, y_pitch, x, x_lo, x_pitch, mean_invstd, scale_shift, M, C,
-                            relu, workspace, stream);
-  if (r) return r;
-  bn_bwd_reduce_final_kernel<<<cdiv(2 * C, 32), 1024, 0, stream>>>(workspace, cdiv(M, chunk_rows(M)), C, sums);
+  auto final_kernel = peer_bufs ? bn_bwd_reduce_final_kernel<true> : bn_bwd_reduce_final_kernel<false>;
+  final_kernel<<<cdiv(2 * C, 32), 1024, 0, stream>>>(workspace, chunks, C, sums, sums_total, pa);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
@@ -1188,7 +1056,8 @@ extern "C" int semseg_bn_bwd_frozen(const void* dy, const void* dy_lo, int dy_pi
                              static_cast<bf16*>(dres_lo), dres_pitch, sums ? workspace : nullptr));
   SB_LAUNCHED();
   if (sums) {
-    bn_bwd_reduce_final_kernel<<<cdiv(2 * C, 32), 1024, 0, stream>>>(workspace, chunks, C, sums);
+    bn_bwd_reduce_final_kernel<false><<<cdiv(2 * C, 32), 1024, 0, stream>>>(workspace, chunks, C, sums, nullptr,
+                                                                         sb::PeerArgs{});
     SB_LAUNCHED();
   }
   return SEMSEG_OK;
@@ -1286,81 +1155,6 @@ extern "C" int semseg_act_to_f32(const void* in, const void* in_lo, int in_pitch
   SB_ACT_DISPATCH(in_lo != nullptr, act_to_f32_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                                         static_cast<const bf16*>(in), static_cast<const bf16*>(in_lo), in_pitch, out,
                                         out_pitch, M, C));
-  SB_LAUNCHED();
-  return SEMSEG_OK;
-}
-
-static int fill_peer_args(sb::PeerArgs* pa, void* const* peer_bufs, void* const* peer_flags, void* counter, int world,
-                          int rank, int slot, int slot_floats, unsigned seq, const void* seq_ptr, int need_floats) {
-  SB_CHECK_ARG(peer_bufs && peer_flags && counter, "p2p: null peer tables");
-  SB_CHECK_ARG(world >= 1 && world <= 8 && rank >= 0 && rank < world, "p2p: world %d rank %d unsupported", world, rank);
-  SB_CHECK_ARG(slot >= 0 && need_floats <= slot_floats, "p2p: slot too small (%d > %d floats)", need_floats,
-               slot_floats);
-  for (int i = 0; i < world; ++i) {
-    SB_CHECK_ARG(peer_bufs[i] && peer_flags[i], "p2p: null peer pointer %d", i);
-    pa->buf[i] = static_cast<float*>(peer_bufs[i]);
-    pa->flags[i] = static_cast<unsigned*>(peer_flags[i]);
-  }
-  pa->counter = static_cast<unsigned*>(counter);
-  pa->world = world;
-  pa->rank = rank;
-  pa->slot = slot;
-  pa->slot_floats = slot_floats;
-  pa->seq = seq;
-  pa->seq_ptr = static_cast<const unsigned*>(seq_ptr);
-  static long long ticks = 0;
-  if (ticks == 0) {
-    const char* e = getenv("SEMSEG_B200_P2P_TIMEOUT_S");
-    double sec = e ? atof(e) : 600.0;
-    if (!(sec > 0.0)) sec = 600.0;
-    ticks = static_cast<long long>(sec * 2.0e9);
-  }
-  pa->timeout_ticks = ticks;
-  return SEMSEG_OK;
-}
-
-extern "C" int semseg_bn_finalize_p2p(const float* stats_partial, int rows, int C, const float* gamma,
-                                      const float* beta, float eps, float momentum, float* running_mean,
-                                      float* running_var, float* mean_invstd, float* scale_shift,
-                                      void* const* peer_bufs, void* const* peer_flags, void* counter, int world,
-                                      int rank, int slot, int slot_floats, unsigned seq, const void* seq_ptr,
-                                      void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(stats_partial && mean_invstd && scale_shift && rows > 0 && C > 0, "bn_finalize_p2p: bad args");
-  sb::PeerArgs pa;
-  int r = fill_peer_args(&pa, peer_bufs, peer_flags, counter, world, rank, slot, slot_floats, seq, seq_ptr, 3 * C);
-  if (r) return r;
-  switch (stats_group_channels(C)) {
-    case 8: bn_finalize_p2p_kernel<8><<<cdiv(C, 8), 1024, 0, stream>>>(stats_partial, rows, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift, pa); break;
-    case 16: bn_finalize_p2p_kernel<16><<<cdiv(C, 16), 1024, 0, stream>>>(stats_partial, rows, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift, pa); break;
-    default: bn_finalize_p2p_kernel<32><<<cdiv(C, 32), 1024, 0, stream>>>(stats_partial, rows, C, gamma, beta, eps, momentum, running_mean, running_var, mean_invstd, scale_shift, pa); break;
-  }
-  SB_LAUNCHED();
-  return SEMSEG_OK;
-}
-
-extern "C" int semseg_bn_bwd_reduce_p2p(const void* dy, const void* dy_lo, int dy_pitch, const void* y,
-                                        const void* y_lo, int y_pitch, const void* x, const void* x_lo, int x_pitch,
-                                        const float* mean_invstd, const float* scale_shift, int M, int C, int relu,
-                                        float* workspace, long long workspace_floats, float* sums_local,
-                                        float* sums_total, void* const* peer_bufs, void* const* peer_flags,
-                                        void* counter, int world, int rank, int slot, int slot_floats, unsigned seq,
-                                        const void* seq_ptr, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(dy && x && mean_invstd && workspace && sums_local && sums_total && M > 0 && C > 0,
-               "bn_bwd_reduce_p2p: bad args");
-  SB_CHECK_ARG(!relu || y || scale_shift, "bn_bwd_reduce_p2p: relu needs y or scale_shift");
-  SB_CHECK_ARG(C % 8 == 0 && dy_pitch % 8 == 0 && x_pitch % 8 == 0 && (!(relu && y) || y_pitch % 8 == 0),
-               "bn_bwd_reduce_p2p: channels and pitches must be multiples of 8");
-  SB_CHECK_ARG(workspace_floats >= semseg_bn_workspace_floats(M, C), "bn_bwd_reduce_p2p: workspace too small");
-  sb::PeerArgs pa;
-  int r = fill_peer_args(&pa, peer_bufs, peer_flags, counter, world, rank, slot, slot_floats, seq, seq_ptr, 2 * C);
-  if (r) return r;
-  r = launch_bwd_reduce(dy, dy_lo, dy_pitch, y, y_lo, y_pitch, x, x_lo, x_pitch, mean_invstd, scale_shift, M, C, relu,
-                        workspace, stream);
-  if (r) return r;
-  bn_bwd_reduce_final_p2p_kernel<<<cdiv(2 * C, 32), 1024, 0, stream>>>(workspace, cdiv(M, chunk_rows(M)), C,
-                                                                      sums_local, sums_total, pa);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }

@@ -166,12 +166,10 @@ def _batch_stats(sp, bn, pg):
     mom = _bn_momentum(bn) if track else 0.0
     rm, rv = (bn.running_mean, bn.running_var) if track else (None, None)
     px = p2p.get_exchange(pg) if pg is not None else None
-    if pg is None:
-        # single rank: merge the per-CTA partials and finalise in one launch
-        mi, ss = ops.bn_finalize_partials(sp, bn.weight, bn.bias, bn.eps, mom, rm, rv)
-    elif px is not None and 3 * sp.shape[-1] <= p2p.SLOT_FLOATS:
-        # SyncBN: statistics exchanged over NVLink peer memory inside the finalise kernel (no NCCL call)
-        mi, ss = ops.bn_finalize_p2p(sp, bn.weight, bn.bias, bn.eps, mom, rm, rv, px)
+    if pg is None or (px is not None and 3 * sp.shape[-1] <= p2p.SLOT_FLOATS):
+        # merge the per-CTA partials and finalise in one launch; under SyncBN the statistics are exchanged over NVLink
+        # peer memory inside that kernel (no NCCL call)
+        mi, ss = ops.bn_finalize_partials(sp, bn.weight, bn.bias, bn.eps, mom, rm, rv, px=px)
     else:
         # SyncBN over NCCL: every rank's local (mean, M2, count), then one finalise
         mi, ss = ops.bn_finalize(gather_rank_stats(ops.bn_merge_partials(sp), pg), bn.weight, bn.bias, bn.eps, mom,
@@ -189,16 +187,14 @@ def _bn_backward(pg, dy, y, raw, mi, gamma, relu, want_dres, ss=None):
     if not dy.is_contiguous():
         dy = dy.contiguous()
     px = p2p.get_exchange(pg) if pg is not None else None
-    if px is not None and 2 * c <= p2p.SLOT_FLOATS:
-        # cross-rank sum over NVLink peer memory inside the reduction kernel (no NCCL call)
-        local, sums = ops.bn_bwd_reduce_p2p(dy, y if relu else None, raw, mi, relu, ss if y is None else None, px)
-        dbeta, dgamma = local[0], local[1]
+    if pg is None or (px is not None and 2 * c <= p2p.SLOT_FLOATS):
+        # under SyncBN the cross-rank sum is taken over NVLink peer memory inside the reduction kernel (no NCCL call)
+        local, sums = ops.bn_bwd_reduce(dy, y if relu else None, raw, mi, relu, ss if y is None else None, px=px)
     else:
-        sums = ops.bn_bwd_reduce(dy, y if relu else None, raw, mi, relu, scale_shift=ss if y is None else None)
-        dbeta, dgamma = sums[0], sums[1]
-        if pg is not None:
-            dbeta, dgamma = dbeta.clone(), dgamma.clone()  # local sums feed dgamma/dbeta (DDP averages them)
-            dist.all_reduce(sums, group=pg)
+        local, sums = ops.bn_bwd_reduce(dy, y if relu else None, raw, mi, relu, ss if y is None else None)
+        local = local.clone()                   # local sums feed dgamma/dbeta (DDP averages them)
+        dist.all_reduce(sums, group=pg)
+    dbeta, dgamma = local[0], local[1]
     # under SyncBN the per-channel sample count is the one the forward exchange measured (mi row 2): exact also when the
     # ranks hold different numbers of pixels, like torch.nn.SyncBatchNorm's gathered counts
     count = float(n * h * w) if pg is None else 0.0

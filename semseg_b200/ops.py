@@ -7,6 +7,7 @@ import ctypes
 import torch
 
 from . import _lib
+from . import p2p
 from ._lib import ConvDesc, WgradDesc, EPI_RAW, EPI_AFFINE, EPI_F32, MAX_TAPS
 
 
@@ -466,18 +467,6 @@ def bn_merge_partials(stats_partial):
     return out
 
 
-def bn_stats(x):
-    """(mean, M2, count) [3][C] of an NHWC bf16 tensor."""
-    _require_cuda(x)
-    lib = _lib.load()
-    n, h, w, c, p = _nhwc_meta(x)
-    m = n * h * w
-    ws, nf = bn_workspace(m, c, x.device)
-    out = torch.empty((3, c), dtype=torch.float32, device=x.device)
-    _lib.check(lib.semseg_bn_stats(_ptr(x), m, c, p, _ptr(ws), nf, _ptr(out), _stream()), "semseg_bn_stats")
-    return out
-
-
 def bn_finalize(rank_stats, gamma, beta, eps, momentum, running_mean, running_var):
     """rank_stats [R][3][C] -> (mean_invstd [2][C], scale_shift [2][C]); updates running stats in place."""
     lib = _lib.load()
@@ -493,15 +482,25 @@ def bn_finalize(rank_stats, gamma, beta, eps, momentum, running_mean, running_va
     return mi, ss
 
 
-def bn_finalize_partials(stats_partial, gamma, beta, eps, momentum, running_mean, running_var):
-    """Per-tile conv partials -> (mean_invstd, scale_shift) in one launch (single-rank BatchNorm)."""
+def _peer_args(px):
+    """(peer_bufs, world, rank, slot, slot_floats, seq_ptr) of the statistics entry points: the next exchange of the
+    NVLink peer exchange `px` (p2p.PeerExchange), or a single rank (NULL peer table) when `px` is None."""
+    if px is None:
+        return None, 1, 0, 0, 0, None
+    return px.data_ptrs, px.world, px.rank, px.next(), p2p.SLOT_FLOATS, _ptr(px.step)
+
+
+def bn_finalize_partials(stats_partial, gamma, beta, eps, momentum, running_mean, running_var, px=None):
+    """Per-tile conv partials -> (mean_invstd, scale_shift) in one launch; with `px` the statistics of every rank, exchanged
+    inside the kernel over peer memory (SyncBN)."""
     lib = _lib.load()
     t, _, c = stats_partial.shape
     buf = torch.empty((5, c), dtype=torch.float32, device=stats_partial.device)
     mi, ss = buf[:3], buf[3:]                               # (mean, invstd, total count), (scale, shift)
     _lib.check(lib.semseg_bn_finalize_partials(_ptr(stats_partial), t, c, _ptr(gamma), _ptr(beta),
                                                float(eps), float(momentum), _ptr(running_mean), _ptr(running_var),
-                                               _ptr(mi), _ptr(ss), _stream()), "semseg_bn_finalize_partials")
+                                               _ptr(mi), _ptr(ss), *_peer_args(px), _stream()),
+               "semseg_bn_finalize_partials")
     return mi, ss
 
 
@@ -533,20 +532,23 @@ def bn_apply(x, scale_shift, residual=None, relu=True, out=None):
     return out
 
 
-def bn_bwd_reduce(dy, y, x, mean_invstd, relu, scale_shift=None):
+def bn_bwd_reduce(dy, y, x, mean_invstd, relu, scale_shift=None, px=None):
+    """-> (sums_local [2][C], sums_total [2][C]) = (sum dz, sum dz*xhat) of this rank and over all ranks, added inside
+    the kernel over peer memory when `px` is given; without `px` both are the same tensor."""
     lib = _lib.load()
     n, h, w, c, dp = _nhwc_meta(dy)
     _, _, _, _, xp = _nhwc_meta(x)
     yp = _nhwc_meta(y)[4] if y is not None else 0
     m = n * h * w
     ws, nf = bn_workspace(m, c, dy.device)
-    sums = torch.empty((2, c), dtype=torch.float32, device=dy.device)
+    out = torch.empty((2 if px is not None else 1, 2, c), dtype=torch.float32, device=dy.device)
+    local, total = out[0], out[-1]
     _same_form(dy, y, x)
     _lib.check(lib.semseg_bn_bwd_reduce(_ptr(dy), _lo(dy), dp, _ptr(y), _lo(y), yp, _ptr(x), _lo(x), xp,
                                         _ptr(mean_invstd), _ptr(scale_shift), m, c, int(bool(relu)), _ptr(ws), nf,
-                                        _ptr(sums), _stream()),
+                                        _ptr(local), _ptr(total), *_peer_args(px), _stream()),
                "semseg_bn_bwd_reduce")
-    return sums
+    return local, total
 
 
 def bn_bwd_apply(dy, y, x, mean_invstd, gamma, sums, count, relu, want_dres=False, scale_shift=None):
@@ -834,40 +836,3 @@ def maxpool3x3s2_bwd(argcode, dy, in_shape):
     _lib.check(lib.semseg_maxpool3x3s2_bwd(_ptr(argcode), _ptr(dy), _lo(dy), _ptr(dx), _lo(dx), n, h, w, c,
                                            _stream()), "semseg_maxpool3x3s2_bwd")
     return dx
-
-
-# ------------------------------------------------------------------------------------------------ SyncBN over NVLink
-def bn_finalize_p2p(stats_partial, gamma, beta, eps, momentum, running_mean, running_var, px):
-    """Like bn_finalize_partials, with the cross-rank exchange done inside the kernel over peer memory (px)."""
-    lib = _lib.load()
-    t, _, c = stats_partial.shape
-    buf = torch.empty((5, c), dtype=torch.float32, device=stats_partial.device)
-    mi, ss = buf[:3], buf[3:]
-    slot, seq = px.next()
-    _lib.check(lib.semseg_bn_finalize_p2p(_ptr(stats_partial), t, c, _ptr(gamma), _ptr(beta), float(eps),
-                                          float(momentum), _ptr(running_mean), _ptr(running_var), _ptr(mi), _ptr(ss),
-                                          px.data_ptrs, px.flag_ptrs, _ptr(px.counter), px.world, px.rank, slot,
-                                          int(__import__("semseg_b200.p2p", fromlist=["x"]).SLOT_FLOATS), seq,
-                                          _ptr(px.step), _stream()), "semseg_bn_finalize_p2p")
-    return mi, ss
-
-
-def bn_bwd_reduce_p2p(dy, y, x, mean_invstd, relu, scale_shift, px):
-    """-> (sums_local [2][C], sums_total [2][C]) with the all-reduce done over peer memory."""
-    lib = _lib.load()
-    n, h, w, c, dp = _nhwc_meta(dy)
-    _, _, _, _, xp = _nhwc_meta(x)
-    yp = _nhwc_meta(y)[4] if y is not None else 0
-    m = n * h * w
-    ws, nf = bn_workspace(m, c, dy.device)
-    out = torch.empty((2, 2, c), dtype=torch.float32, device=dy.device)
-    slot, seq = px.next()
-    _same_form(dy, y, x)
-    _lib.check(lib.semseg_bn_bwd_reduce_p2p(_ptr(dy), _lo(dy), dp, _ptr(y), _lo(y), yp, _ptr(x), _lo(x), xp,
-                                            _ptr(mean_invstd),
-                                            _ptr(scale_shift), m, c, int(bool(relu)), _ptr(ws), nf, _ptr(out[0]),
-                                            _ptr(out[1]), px.data_ptrs, px.flag_ptrs, _ptr(px.counter), px.world,
-                                            px.rank, slot,
-                                            int(__import__("semseg_b200.p2p", fromlist=["x"]).SLOT_FLOATS), seq,
-                                            _ptr(px.step), _stream()), "semseg_bn_bwd_reduce_p2p")
-    return out[0], out[1]

@@ -1,9 +1,10 @@
 """SyncBatchNorm statistics exchange over NVLink peer memory (torch symmetric memory).
 
 One process per GPU; every rank allocates the same symmetric buffer, `rendezvous` maps all peers' buffers into this
-process, and the exchange kernels (csrc/bn.cu: bn_finalize_p2p, bn_bwd_reduce_p2p) push every value as one 8-byte
-{value, sequence number} word into every peer's buffer and poll their own memory for the peers' words (flag-in-data, no
-fences, no counters) — all over NVLink — one kernel per BatchNorm exchange instead of merge-kernel + NCCL collective + finalise-kernel.
+process, and the exchange kernels (csrc/bn.cu: the peer forms of bn_finalize_partials and bn_bwd_reduce_final) push
+every value as one 8-byte {value, sequence number} word into every peer's buffer and poll their own memory for the peers'
+words (flag-in-data, no fences, no counters) — all over NVLink — one kernel per BatchNorm exchange instead of
+merge-kernel + NCCL collective + finalise-kernel.
 If symmetric memory cannot be set up (no P2P access, single process, SEMSEG_B200_SYNCBN=nccl) the callers use the
 NCCL path (torch.distributed all_gather / all_reduce); both paths compute the same statistics.
 """
@@ -27,22 +28,17 @@ class PeerExchange:
         if self.world > 8:
             raise RuntimeError("peer exchange supports up to 8 ranks (one NVSwitch domain)")
         dev = torch.device("cuda", torch.cuda.current_device())
-        flag_words = N_SLOTS * self.world
         # data words are 8 bytes ({fp32 value, sequence number}): two fp32 elements per word
-        self.buf = symm_mem.empty(flag_words + 2 * N_SLOTS * self.world * SLOT_FLOATS, dtype=torch.float32, device=dev)
+        self.buf = symm_mem.empty(2 * N_SLOTS * self.world * SLOT_FLOATS, dtype=torch.float32, device=dev)
         self.buf.zero_()
         self.handle = symm_mem.rendezvous(self.buf, pg)
-        ptrs = [int(p) for p in self.handle.buffer_ptrs]
-        self.flag_ptrs = (ctypes.c_void_p * self.world)(*ptrs)
-        assert (4 * flag_words) % 8 == 0
-        self.data_ptrs = (ctypes.c_void_p * self.world)(*[p + 4 * flag_words for p in ptrs])
-        self.counter = torch.zeros((1,), dtype=torch.int32, device=dev)
+        self.data_ptrs = (ctypes.c_void_p * self.world)(*[int(p) for p in self.handle.buffer_ptrs])
         # Device-resident step counter = the sequence number of every exchange of the current step. The kernels read it
         # when they run, so a training step captured in a CUDA graph (slots baked in) can be replayed: the graph only
         # has to contain the increment (begin_step) once per step.
         self.step = torch.ones((1,), dtype=torch.int32, device=dev)
         torch.cuda.synchronize()
-        self.handle.barrier()           # every rank's flags are zero before the first exchange
+        self.handle.barrier()           # every rank's buffer is zero before the first exchange
         torch.cuda.synchronize()
         self.calls = 0
 
@@ -56,13 +52,13 @@ class PeerExchange:
             self.calls = 0
 
     def next(self):
-        """(slot, seq) of the next exchange: identical on every rank because all ranks run the same op sequence.
-        seq = 0 tells the kernel to take the sequence number from the device-resident step counter."""
+        """Slot of the next exchange: identical on every rank because all ranks run the same op sequence. The kernel
+        takes the sequence number from the device-resident step counter."""
         if self.calls >= N_SLOTS:       # more exchanges than slots without a begin_step(): open a new epoch
             self.begin_step()
         k = self.calls
         self.calls += 1
-        return k, 0
+        return k
 
 
 def get_exchange(pg):

@@ -39,7 +39,7 @@ def test_no_undeclared_exports():
 def test_ctypes_binding_covers_header():
     assert sorted(_lib.SIGNATURES) == header_symbols()
     lib = _lib.load()
-    assert lib.semseg_abi_version() == 1
+    assert lib.semseg_abi_version() == 2
     assert lib.semseg_launch_count() == 0 or lib.semseg_launch_count() > 0
 
 
@@ -153,3 +153,36 @@ def test_round2_entry_points_validate_before_any_cuda_call():
     # bf16x3 accumulation-chain planning is pure host arithmetic: K blocks = taps * Cin / 64, at most 8 per slice
     assert lib.semseg_conv_k_slices(4096, 9, 8) == 72 and lib.semseg_conv_k_slices(64, 1, 8) == 1
     assert lib.semseg_conv_k_slices(256, 9, 8) == 5 and lib.semseg_conv_splitk_rows(4) >= 1
+
+
+def test_peer_exchange_arguments_validated_before_any_cuda_call():
+    """The SyncBN peer-exchange arguments (peer_bufs, world, rank, slot, slot_floats, seq_ptr) of both statistics entry
+    points go through one check: a bad world, rank, slot size or peer pointer is SEMSEG_E_INVALID with a message, before
+    anything is launched (no GPU here)."""
+    lib = _lib.load()
+    P = ctypes.c_void_p(16)
+    c = 64
+    peers = (ctypes.c_void_p * 8)(*([16] * 8))
+    holey = (ctypes.c_void_p * 2)(16, None)
+    nf = lib.semseg_bn_workspace_floats(64, c)
+    assert nf > 0
+
+    def finalize(bufs, world, rank, slot_floats, seq_ptr=P):
+        # semseg_bn_finalize_partials(stats_partial, rows, C, gamma, beta, eps, momentum, running_mean, running_var,
+        #                             mean_invstd, scale_shift, peer_bufs, world, rank, slot, slot_floats, seq_ptr, stream)
+        return lib.semseg_bn_finalize_partials(P, 4, c, None, None, 1e-5, 0.1, None, None, P, P, bufs, world, rank, 0,
+                                               slot_floats, seq_ptr, None)
+
+    def bwd_reduce(bufs, world, rank, slot_floats, seq_ptr=P):
+        # semseg_bn_bwd_reduce(dy, dy_lo, dy_pitch, y, y_lo, y_pitch, x, x_lo, x_pitch, mean_invstd, scale_shift, M, C,
+        #                      relu, workspace, workspace_floats, sums, sums_total, peer_bufs, world, rank, slot,
+        #                      slot_floats, seq_ptr, stream)
+        return lib.semseg_bn_bwd_reduce(P, None, c, None, None, 0, P, None, c, P, None, 64, c, 0, P, nf, P, P, bufs,
+                                        world, rank, 0, slot_floats, seq_ptr, None)
+
+    for call, need in ((finalize, 3 * c), (bwd_reduce, 2 * c)):
+        assert call(peers, 9, 0, need) == -1 and b"world 9" in lib.semseg_last_error()
+        assert call(peers, 2, 2, need) == -1 and b"rank 2" in lib.semseg_last_error()
+        assert call(peers, 2, 0, need - 1) == -1 and b"slot too small" in lib.semseg_last_error()
+        assert call(holey, 2, 0, need) == -1 and b"null peer pointer 1" in lib.semseg_last_error()
+        assert call(peers, 2, 0, need, None) == -1 and b"sequence" in lib.semseg_last_error()

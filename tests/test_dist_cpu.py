@@ -56,8 +56,8 @@ def test_syncbn_stats_exchange_and_timing_reduce_world2():
 
 
 def test_peer_exchange_slot_sequence_and_nccl_override(monkeypatch):
-    """Host logic of the NVLink peer exchange: (slot, seq) advance identically on every rank and a slot is only
-    reused with a strictly larger sequence number; SEMSEG_B200_SYNCBN=nccl disables the peer path."""
+    """Host logic of the NVLink peer exchange: slots advance identically on every rank and a slot is only reused with a
+    strictly larger sequence number (the step counter); SEMSEG_B200_SYNCBN=nccl disables the peer path."""
     from semseg_b200 import p2p
 
     class Fake(p2p.PeerExchange):
@@ -69,10 +69,9 @@ def test_peer_exchange_slot_sequence_and_nccl_override(monkeypatch):
     for k in range(3 * p2p.N_SLOTS + 5):
         if k % 200 == 199:          # a training forward opens a new epoch on every rank at the same point
             a.begin_step(), b.begin_step()
-        sa, sb_ = a.next(), b.next()
-        assert sa == sb_ and int(a.step) == int(b.step)
-        slot, seq = sa
-        assert 0 <= slot < p2p.N_SLOTS and seq == 0     # seq 0: the kernel reads the step counter
+        slot = a.next()
+        assert slot == b.next() and int(a.step) == int(b.step)
+        assert 0 <= slot < p2p.N_SLOTS
         assert int(a.step) > seen.get(slot, 0)          # a slot is only reused under a larger sequence number
         seen[slot] = int(a.step)
     assert p2p.SLOT_FLOATS >= 3 * 2048          # widest BatchNorm on the path (layer4 / PSA proj: 2048 channels)

@@ -151,7 +151,7 @@ def test_bn_and_elementwise_kernels_split_vs_torch():
     y = ops.bn_apply(x, ss, residual=res, relu=True)
     assert util.rel_l2(_f32(y), yr.permute(0, 2, 3, 1)) < 2e-5
     yr.backward(_f32(dy).permute(0, 3, 1, 2))
-    sums = ops.bn_bwd_reduce(dy, y, x, mi, True)
+    _, sums = ops.bn_bwd_reduce(dy, y, x, mi, True)
     dx, dres, dgb = ops.bn_bwd_apply(dy, y, x, mi, gamma, sums, float(n * h * w), True, want_dres=True)
     assert util.rel_l2(_f32(dx), xf.grad.permute(0, 2, 3, 1)) < 5e-5
     assert util.rel_l2(_f32(dres), rf.grad.permute(0, 2, 3, 1)) < 2e-5

@@ -190,7 +190,9 @@ def check_bn():
     beta = torch.randn((C,), device="cuda", generator=g)
     rm = torch.zeros(C, device="cuda")
     rv = torch.ones(C, device="cuda")
-    st = ops.bn_stats(x)
+    v = x.float().reshape(-1, C)      # fp32 moments of x: (mean, M2, count)
+    st = torch.stack([v.mean(0), v.var(0, unbiased=False) * v.shape[0], torch.full((C,), float(v.shape[0]),
+                                                                                   device="cuda")])
     mi, ss = ops.bn_finalize(st, gamma, beta, 1e-5, 0.1, rm, rv)
     res = torch.randn((N, H, W, C), device="cuda", generator=g).to(torch.bfloat16)
     y = ops.bn_apply(x, ss, residual=res, relu=True)
@@ -209,7 +211,7 @@ def check_bn():
     mask = (y.float() > 0).permute(0, 3, 1, 2)
     pre = torch.nn.functional.batch_norm(xf, None, None, gm, bt, True, 0.1, 1e-5) + rf
     (pre * mask * dy.float().permute(0, 3, 1, 2)).sum().backward()
-    sums = ops.bn_bwd_reduce(dy, y, x, mi, True)
+    _, sums = ops.bn_bwd_reduce(dy, y, x, mi, True)
     dx, dres, dgb = ops.bn_bwd_apply(dy, y, x, mi, gamma, sums, float(N * H * W), True, want_dres=True)
     ok &= _report("bn bwd dx", dx, xf.grad.permute(0, 2, 3, 1), 1e-2)
     ok &= _report("bn bwd dres", dres, rf.grad.permute(0, 2, 3, 1), 1e-2)
