@@ -124,7 +124,7 @@ typedef struct semseg_conv_desc {
   float* stats_partial;
   /* bf16x3 operand mode (split storage): lo planes of x / y / residual (same shapes and pitches as the hi planes);
    * all NULL for plain bf16. With x_lo set, w must hold the lo slab directly behind the hi slab (w_split != 0,
-   * semseg_pack_weights(..., split = 1)) and every K block is accumulated as x_hi*w_hi + x_lo*w_hi + x_hi*w_lo;
+   * semseg_pack_item.split != 0) and every K block is accumulated as x_hi*w_hi + x_lo*w_hi + x_hi*w_lo;
    * statistics are those of hi + lo. */
   const void* x_lo;
   void* y_lo;
@@ -179,25 +179,23 @@ int semseg_conv_wgrad(const semseg_wgrad_desc* d, void* stream);
 int semseg_wgrad_reduce(const float* dw_partial, int n_splits, int taps, int Cout, int Cin, float* dw_oihw,
                         int accumulate, void* stream);
 
-/* Weight packing: fp32 OIHW [Cout][Cin][taps] ->
- *   wf bf16 [taps][rows_f][cols_f]  (wf[t][co][ci], zero padded)   — fprop B operand
- *   wd bf16 [taps][rows_d][cols_d]  (wd[t][ci][co], zero padded)   — dgrad B operand
- * Either output may be NULL. */
-int semseg_pack_weights(const float* w_oihw, int Cout, int Cin, int taps, void* wf, int rows_f, int cols_f,
-                        void* wd, int rows_d, int cols_d, int split, void* stream);
-
-/* The same packing for every conv of a model in one launch (torch re-packs after each optimizer step; 2 x 63 small
- * launches per step for PSPNet50 otherwise). `items` is an array in DEVICE memory, sorted by tile0; an item's tiles are
- * its 32 x 32 (co, ci) blocks: tiles_ci = ceil(cols_f / 32) per row of ceil(cols_d / 32) rows. wf is
- * [taps][Cout][cols_f], wd is [taps][Cin][cols_d] (cols_* = Cin / Cout rounded up to 8, zero padded); either may be NULL. */
+/* Weight packing: fp32 OIHW [Cout][Cin][taps] -> the bf16 operand slabs of the conv kernels, for every conv of a model
+ * in one launch (torch re-packs after each optimizer step). `items` is an array in DEVICE memory, sorted by tile0; an
+ * item's tiles are its 32 x 32 (co, ci) blocks: tiles_ci = ceil(cols_f / 32) per row of ceil(cols_d / 32) rows.
+ *   wf bf16 [taps][Cout][cols_f]  (wf[t][co][ci], zero padded)   — fprop B operand
+ *   wd bf16 [taps][Cin][cols_d]   (wd[t][ci][co], zero padded)   — dgrad B operand
+ *   wp bf16 [Cout][32]            (wp[co][t*Cin + ci], columns 9*Cin..31 zero; taps == 9 and Cin <= 3 only) — the stem
+ *                                 conv as a 1x1 conv over semseg_im2col3x3s2 patches
+ * cols_* = Cin / Cout rounded up to 8; wd and wp may be NULL. */
 typedef struct semseg_pack_item {
   const float* w;
   void* wf;
   void* wd;
+  void* wp;
   int Cout, Cin, taps;
   int cols_f, cols_d;
   int tile0, tiles_ci;
-  int split; /* != 0: lo slabs follow the hi slabs (wf + taps*Cout*cols_f, wd + taps*Cin*cols_d) */
+  int split; /* != 0: lo slabs follow the hi slabs (wf + taps*Cout*cols_f, wd + taps*Cin*cols_d, wp + Cout*32) */
 } semseg_pack_item;
 int semseg_pack_weights_multi(const semseg_pack_item* items_dev, int n_items, int n_tiles, int max_taps, void* stream);
 

@@ -23,7 +23,7 @@ I9 = c_i32 * MAX_TAPS
 class PackItem(ctypes.Structure):
     """struct semseg_pack_item (include/semseg_b200.h)."""
     _fields_ = [
-        ("w", c_vp), ("wf", c_vp), ("wd", c_vp),
+        ("w", c_vp), ("wf", c_vp), ("wd", c_vp), ("wp", c_vp),
         ("Cout", c_i32), ("Cin", c_i32), ("taps", c_i32),
         ("cols_f", c_i32), ("cols_d", c_i32),
         ("tile0", c_i32), ("tiles_ci", c_i32),
@@ -105,7 +105,6 @@ SIGNATURES = {
     "semseg_conv_wgrad_splits": (c_int, [ctypes.POINTER(WgradDesc)]),
     "semseg_conv_wgrad": (c_int, [ctypes.POINTER(WgradDesc), c_vp]),
     "semseg_wgrad_reduce": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_vp]),
-    "semseg_pack_weights": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp]),
     "semseg_pack_weights_multi": (c_int, [c_vp, c_int, c_int, c_int, c_vp]),
     "semseg_sgd_chunk_elems": (c_int, []),
     "semseg_sgd_multi": (c_int, [c_vp, c_vp, c_int, c_int, ctypes.POINTER(SgdHyper), c_vp]),

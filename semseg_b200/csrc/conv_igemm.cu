@@ -523,7 +523,7 @@ extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
     int r = encode_tmap_bf16(&tm.b, d->w, 3, dims, str, box);
     if (r) return r;
     tm.b_lo = tm.b;
-    if (split) {   // the lo slab follows the hi slab (semseg_pack_weights with split != 0)
+    if (split) {   // the lo slab follows the hi slab (semseg_pack_item.split != 0)
       const __nv_bfloat16* w_lo =
           static_cast<const __nv_bfloat16*>(d->w) + static_cast<size_t>(d->n_wtaps) * d->w_rows * d->w_cols;
       if ((r = encode_tmap_bf16(&tm.b_lo, w_lo, 3, dims, str, box))) return r;

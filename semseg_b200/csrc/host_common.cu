@@ -113,5 +113,5 @@ void choose_box(int H, int W, int max_pixels, int* bh_out, int* bw_out) {
 }  // namespace sb
 
 extern "C" const char* semseg_last_error(void) { return sb::g_err; }
-extern "C" int semseg_abi_version(void) { return 2; }
+extern "C" int semseg_abi_version(void) { return 3; }
 extern "C" long long semseg_launch_count(void) { return sb::g_launches.load(); }

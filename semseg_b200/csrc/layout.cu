@@ -58,53 +58,19 @@ __global__ void nhwc_to_nchw_kernel(const TIn* __restrict__ in, const TIn* __res
   }
 }
 
-// w[co][ci][t] fp32 -> wf[t][co][ci] bf16 (rows_f x cols_f, zero padded). One thread per output element.
-// split != 0: the lo slab (bf16(v - hi)) is written directly behind the hi slab.
-__global__ void pack_wf_kernel(const float* __restrict__ w, int Cout, int Cin, int taps, __nv_bfloat16* __restrict__ wf,
-                               int rows, int cols, int split) {
-  const size_t total = static_cast<size_t>(taps) * rows * cols;
-  for (size_t idx = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
-       idx += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int ci = static_cast<int>(idx % cols);
-    const size_t r = idx / cols;
-    const int co = static_cast<int>(r % rows);
-    const int t = static_cast<int>(r / rows);
-    float v = 0.f;
-    if (co < Cout && ci < Cin) v = w[(static_cast<size_t>(co) * Cin + ci) * taps + t];
-    const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-    wf[idx] = hi;
-    if (split) wf[total + idx] = __float2bfloat16_rn(v - __bfloat162float(hi));
-  }
+// dst[o] = bf16(v) (round to nearest); split != 0: dst[lo + o] = bf16(v - hi), the lo slab behind the hi slab.
+__device__ __forceinline__ void store_hi_lo(__nv_bfloat16* dst, size_t o, size_t lo, float v, int split) {
+  const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+  dst[o] = hi;
+  if (split) dst[lo + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
 }
 
-// w[co][ci][t] fp32 -> wd[t][ci][co] bf16 via a 32x32 smem transpose of the (co, ci) plane per tap.
-__global__ void pack_wd_kernel(const float* __restrict__ w, int Cout, int Cin, int taps, __nv_bfloat16* __restrict__ wd,
-                               int rows, int cols, int split) {
-  __shared__ float tile[32][33];
-  const int t = blockIdx.z;
-  const int ci0 = blockIdx.x * 32, co0 = blockIdx.y * 32;
-  for (int r = threadIdx.y; r < 32; r += blockDim.y) {
-    const int co = co0 + r, ci = ci0 + threadIdx.x;
-    tile[r][threadIdx.x] = (co < Cout && ci < Cin) ? w[(static_cast<size_t>(co) * Cin + ci) * taps + t] : 0.f;
-  }
-  __syncthreads();
-  for (int r = threadIdx.y; r < 32; r += blockDim.y) {
-    const int ci = ci0 + r, co = co0 + threadIdx.x;
-    if (ci < rows && co < cols) {
-      const float v = tile[threadIdx.x][r];
-      const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-      const size_t o = (static_cast<size_t>(t) * rows + ci) * cols + co;
-      wd[o] = hi;
-      if (split) wd[static_cast<size_t>(gridDim.z) * rows * cols + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
-    }
-  }
-}
-
-// All conv weights of a model in ONE launch (the per-layer kernels above are launch-latency bound: 2 x 63 launches of
-// 2-3 us per step for PSPNet50). A block owns one 32 (co) x 32 (ci) tile of one layer with all of its taps: the fp32
+// Every operand slab of every conv of a model in ONE launch (per-layer packing would be 2 x 63 launch-latency-bound
+// launches per step for PSPNet50). A block owns one 32 (co) x 32 (ci) tile of one layer with all of its taps: the fp32
 // OIHW rows are read once (32*taps contiguous floats per output channel), parked in shared memory, and written out as
-// both bf16 operand slabs (wf[t][co][ci] and wd[t][ci][co], zero padded to the slab widths). items[] lives in device
-// memory and is sorted by tile0; the block finds its layer by binary search.
+// the bf16 operand slabs the item asks for, zero padded to the slab widths: wf[t][co][ci], wd[t][ci][co] and the stem's
+// patch slab wp[co][t*Cin + ci] (Cin <= 3, so the one ci0 == 0 tile of a row holds all 9*Cin values). items[] lives in
+// device memory and is sorted by tile0; the block finds its layer by binary search.
 __global__ void __launch_bounds__(256) pack_multi_kernel(const semseg_pack_item* __restrict__ items, int n_items) {
   extern __shared__ float pk_tile[];  // [32][32 * taps + 1]
   __shared__ int s_item;
@@ -132,28 +98,32 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const semseg_pack_item*
   const int total = taps * 1024;
   if (it.wf) {
     __nv_bfloat16* wf = static_cast<__nv_bfloat16*>(it.wf);
+    const size_t lo = static_cast<size_t>(taps) * it.Cout * it.cols_f;
     for (int idx = threadIdx.x; idx < total; idx += 256) {
       const int ci_l = idx & 31, co_l = (idx >> 5) & 31, t = idx >> 10;
-      if (co_l < nco && ci0 + ci_l < it.cols_f) {
-        const float v = pk_tile[co_l * pitch + ci_l * taps + t];
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        const size_t o = (static_cast<size_t>(t) * it.Cout + co0 + co_l) * it.cols_f + ci0 + ci_l;
-        wf[o] = hi;
-        if (it.split) wf[static_cast<size_t>(taps) * it.Cout * it.cols_f + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
-      }
+      if (co_l < nco && ci0 + ci_l < it.cols_f)
+        store_hi_lo(wf, (static_cast<size_t>(t) * it.Cout + co0 + co_l) * it.cols_f + ci0 + ci_l, lo,
+                    pk_tile[co_l * pitch + ci_l * taps + t], it.split);
     }
   }
   if (it.wd) {
     __nv_bfloat16* wd = static_cast<__nv_bfloat16*>(it.wd);
+    const size_t lo = static_cast<size_t>(taps) * it.Cin * it.cols_d;
     for (int idx = threadIdx.x; idx < total; idx += 256) {
       const int co_l = idx & 31, ci_l = (idx >> 5) & 31, t = idx >> 10;
-      if (ci_l < nci && co0 + co_l < it.cols_d) {
-        const float v = pk_tile[co_l * pitch + ci_l * taps + t];
-        const __nv_bfloat16 hi = __float2bfloat16_rn(v);
-        const size_t o = (static_cast<size_t>(t) * it.Cin + ci0 + ci_l) * it.cols_d + co0 + co_l;
-        wd[o] = hi;
-        if (it.split) wd[static_cast<size_t>(taps) * it.Cin * it.cols_d + o] = __float2bfloat16_rn(v - __bfloat162float(hi));
-      }
+      if (ci_l < nci && co0 + co_l < it.cols_d)
+        store_hi_lo(wd, (static_cast<size_t>(t) * it.Cin + ci0 + ci_l) * it.cols_d + co0 + co_l, lo,
+                    pk_tile[co_l * pitch + ci_l * taps + t], it.split);
+    }
+  }
+  if (it.wp && ci0 == 0) {
+    __nv_bfloat16* wp = static_cast<__nv_bfloat16*>(it.wp);
+    const int real = taps * it.Cin;   // columns real..31 are zero
+    for (int idx = threadIdx.x; idx < 1024; idx += 256) {
+      const int col = idx & 31, co_l = idx >> 5;
+      if (co_l < nco)
+        store_hi_lo(wp, static_cast<size_t>(co0 + co_l) * 32 + col, static_cast<size_t>(it.Cout) * 32,
+                    col < real ? pk_tile[co_l * pitch + (col % it.Cin) * taps + col / it.Cin] : 0.f, it.split);
     }
   }
 }
@@ -267,31 +237,6 @@ extern "C" int semseg_phases_to_space(const void* xp, int N, int H, int W, int C
   phases_to_space_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(static_cast<const bf16*>(xp), N, H, W, C,
                                                                            Hh, Wh, static_cast<bf16*>(x));
   SB_LAUNCHED();
-  return SEMSEG_OK;
-}
-
-extern "C" int semseg_pack_weights(const float* w_oihw, int Cout, int Cin, int taps, void* wf, int rows_f, int cols_f,
-                                   void* wd, int rows_d, int cols_d, int split, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(w_oihw && Cout > 0 && Cin > 0 && taps > 0 && taps <= SEMSEG_MAX_TAPS, "pack_weights: bad args");
-  if (wf) {
-    SB_CHECK_ARG(rows_f >= Cout && cols_f >= Cin && cols_f % 8 == 0, "pack_weights: bad wf dims %d x %d", rows_f,
-                 cols_f);
-    const size_t total = static_cast<size_t>(taps) * rows_f * cols_f;
-    size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
-    pack_wf_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(w_oihw, Cout, Cin, taps, static_cast<bf16*>(wf),
-                                                                     rows_f, cols_f, split);
-    SB_LAUNCHED();
-  }
-  if (wd) {
-    SB_CHECK_ARG(rows_d >= Cin && cols_d >= Cout && cols_d % 8 == 0, "pack_weights: bad wd dims %d x %d", rows_d,
-                 cols_d);
-    dim3 grid(cdiv(rows_d, 32), cdiv(cols_d, 32), taps);
-    pack_wd_kernel<<<grid, dim3(32, 8), 0, stream>>>(w_oihw, Cout, Cin, taps, static_cast<bf16*>(wd), rows_d, cols_d,
-                                                     split);
-    SB_LAUNCHED();
-  }
   return SEMSEG_OK;
 }
 

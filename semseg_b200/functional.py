@@ -33,9 +33,10 @@ from .ops import EPI_RAW, EPI_AFFINE, EPI_F32
 
 # ------------------------------------------------------------------------------------------------ helpers
 def packed(conv, need_dgrad=True, split=False):
-    """bf16 operand slabs of conv.weight (hi + lo slabs when split), re-packed only when the parameter changed
-    (optimizer step / load). The cache key is (parameter version, storage pointer): in-place edits through `.data`
-    do not bump the version — call `invalidate_packs(model)` after such an edit."""
+    """bf16 operand slabs of conv.weight (hi + lo slabs when split; also the patch slab of a stem conv), re-packed only
+    when the parameter changed (optimizer step / load). The cache key is (parameter version, storage pointer): in-place
+    edits through `.data` do not bump the version — call `invalidate_packs(model)` after such an edit. A miss refreshes
+    the conv's own one-conv plan, which is rebuilt only for a new storage, storage form or first need of dgrad slabs."""
     w = conv.weight
     key = (w._version, w.data_ptr(), need_dgrad, split)
     cache = conv.__dict__.get("_sb_pack")
@@ -43,8 +44,15 @@ def packed(conv, need_dgrad=True, split=False):
         return cache[1]
     if cache is not None and cache[0][:2] == key[:2] and cache[0][3] == split and cache[0][2]:
         return cache[1]                       # a pack with dgrad slabs also serves a forward-only request
-    pw = ops.pack_weights(w, need_dgrad=need_dgrad, split=split)
-    conv.__dict__["_sb_pack"] = (key, pw)
+    plan = conv.__dict__.get("_sb_conv_plan")
+    if plan is None or not plan.valid_for([w], split) or (need_dgrad and plan.packs[0].wd is None):
+        wc = w.detach()
+        plan = ops.WeightPackPlan([wc if wc.is_contiguous() else wc.contiguous()], split, dgrad=need_dgrad,
+                                  patches=[_is_patch_conv(conv)])
+        conv.__dict__["_sb_conv_plan"] = plan
+    plan.refresh()
+    pw = plan.packs[0]
+    conv.__dict__["_sb_pack"] = (key[:2] + (pw.wd is not None, split), pw)
     return pw
 
 
@@ -53,38 +61,19 @@ def invalidate_packs(model):
     bump the version counter the cache is keyed on)."""
     for m in model.modules():
         m.__dict__.pop("_sb_pack", None)
-        m.__dict__.pop("_sb_pack_patches", None)
     model.__dict__.pop("_sb_pack_plan", None)
 
 
-def packed_patches(conv, split=False):
-    """Operand slab of the stem conv in its patch form (ops.im2col3x3s2): wf [1][Cout][32] with column
-    (r*3+s)*Cin + c = weight[:, c, r, s], zero padded ([2][1][Cout][32] = hi, lo slabs when split); re-made only when the
-    parameter changed."""
-    w = conv.weight
-    key = (w._version, w.data_ptr(), "patches", split)
-    cache = conv.__dict__.get("_sb_pack_patches")
-    if cache is not None and cache[0] == key:
-        return cache[1]
-    cout, cin = w.shape[0], w.shape[1]
-    flat = torch.zeros((1, cout, 32), dtype=torch.float32, device=w.device)
-    flat[0, :, :9 * cin] = w.detach().permute(0, 2, 3, 1).reshape(cout, 9 * cin)
-    hi = flat.to(torch.bfloat16)
-    wf = torch.stack([hi, (flat - hi.float()).to(torch.bfloat16)], 0) if split else hi
-    conv.__dict__["_sb_pack_patches"] = (key, wf)
-    return wf
-
-
-def _is_patch_conv(conv, x):
-    """The 3-channel stride-2 stem conv (model/resnet.py:106-108) on an input that needs no gradient."""
+def _is_patch_conv(conv):
+    """The 3-channel stride-2 stem conv (model/resnet.py:106-108), which can run as a 1x1 conv over input patches."""
     return (conv.kernel_size == (3, 3) and conv.stride == (2, 2) and conv.dilation == (1, 1) and conv.padding == (1, 1)
-            and conv.in_channels <= 3 and conv.groups == 1 and x.shape[-1] >= 4)
+            and conv.in_channels <= 3 and conv.groups == 1)
 
 
 def prepack(model, force=False):
     """Refresh the operand slabs of every native conv of `model` in one launch when its weights changed (call at the top
     of a training forward; force=True while the step is being captured into a CUDA graph, so that the re-pack is part
-    of every replay). Convs keep working without it: `packed` falls back to the per-layer kernels."""
+    of every replay). Convs keep working without it: `packed` re-packs each conv through its own one-conv plan."""
     convs = [m for m in model.modules() if isinstance(m, nn.Conv2d) and m.weight.is_cuda and
              m.weight.dtype == torch.float32 and m.weight.is_contiguous() and m.kernel_size[0] == m.kernel_size[1] and
              m.kernel_size[0] * m.kernel_size[1] <= ops.MAX_TAPS]
@@ -97,7 +86,7 @@ def prepack(model, force=False):
     plan = model.__dict__.get("_sb_pack_plan")
     weights = [c.weight.detach() for c in convs]
     if plan is None or not plan.valid_for(weights, split):
-        plan = ops.WeightPackPlan(weights, split)
+        plan = ops.WeightPackPlan(weights, split, patches=[_is_patch_conv(c) for c in convs])
         model.__dict__["_sb_pack_plan"] = plan
     plan.refresh()
     for c, k, pw in zip(convs, keys, plan.packs):
@@ -225,9 +214,9 @@ class _ConvForm:
         k = conv.kernel_size[0]
         if conv.stride[0] == 1:
             self.kind, self.xin, self.taps = "direct", x, ops.conv_taps(k, conv.dilation[0])
-        elif mode != "eval" and not input_needs_grad and _is_patch_conv(conv, x):
+        elif mode != "eval" and not input_needs_grad and _is_patch_conv(conv) and x.shape[-1] >= 4:
             self.kind, self.xin = "patches", ops.im2col3x3s2(x, conv.in_channels)
-            self.taps, self.wf = ops.conv_taps(1, 1), packed_patches(conv, split)
+            self.taps, self.wf = ops.conv_taps(1, 1), self.pw.wp
         else:
             self.kind, self.xin = "phases", ops.space_to_phases(x)          # [4N, Hh, Wh, C]
             t2 = ops.conv_taps_s2(k, n)

@@ -205,7 +205,8 @@ def _capture(model, impl, st, x, y):
         head_ids = set()
         if t_mid is not None and os.environ.get("SEMSEG_B200_GRAPH_SEGMENTS", "2") != "1":
             for name in getattr(model, "_sb_head_modules", ()):
-                head_ids.update(id(q) for q in getattr(model, name).parameters())
+                # the proxies only: a frozen parameter has none and must not be counted into the head
+                head_ids.update(id(q) for q in getattr(model, name).parameters() if q.requires_grad)
         if head_ids:
             # parameters reordered: head (before the boundary) first, tail after
             order = [k for k, q in enumerate(proxies) if id(q) in head_ids] + \
@@ -234,9 +235,6 @@ def _capture(model, impl, st, x, y):
     del proxies
     # the graphs reference the persistent weight slabs: keep their owner alive as long as the graphs
     st.keep = model.__dict__.get("_sb_pack_plan")
-    # per-conv pack caches were keyed on the proxies' version counters during capture: forget them
-    for mod in model.modules():
-        mod.__dict__.pop("_sb_pack_patches", None)
     torch.cuda.synchronize()
 
 

@@ -148,12 +148,14 @@ def psa_attend_bwd_attn(attn, stats, feat, out, dout, psa_type, mask_h, mask_w, 
 
 # ------------------------------------------------------------------------------------------------ weights
 class PackedWeight:
-    """bf16 operand slabs of one conv weight: wf [taps][Cout][Cin_p] (fprop), wd [taps][Cin][Cout_p] (dgrad); with
-    split=True each is [2][taps][rows][cols] = the hi slab followed by the lo slab (bf16x3 operand mode)."""
-    __slots__ = ("wf", "wd", "cout", "cin", "taps", "ksize", "split")
+    """bf16 operand slabs of one conv weight: wf [taps][Cout][Cin_p] (fprop), wd [taps][Cin][Cout_p] (dgrad) or None,
+    wp [1][Cout][32] or None (the stem conv as a 1x1 conv over im2col3x3s2 patches: column t*Cin + c holds tap t of
+    input channel c); with split=True each is [2][...] = the hi slab followed by the lo slab (bf16x3 operand mode)."""
+    __slots__ = ("wf", "wd", "wp", "cout", "cin", "taps", "ksize", "split")
 
-    def __init__(self, wf, wd, cout, cin, taps, ksize, split=False):
-        self.wf, self.wd, self.cout, self.cin, self.taps, self.ksize, self.split = wf, wd, cout, cin, taps, ksize, split
+    def __init__(self, wf, wd, wp, cout, cin, taps, ksize, split=False):
+        self.wf, self.wd, self.wp = wf, wd, wp
+        self.cout, self.cin, self.taps, self.ksize, self.split = cout, cin, taps, ksize, split
 
 
 def _slab(taps, rows, cols, split, device):
@@ -161,35 +163,22 @@ def _slab(taps, rows, cols, split, device):
 
 
 def pack_weights(w, need_dgrad=True, split=False):
-    """w: fp32 OIHW parameter -> PackedWeight (one fused launch pair)."""
-    _require_cuda(w)
-    lib = _lib.load()
+    """w: fp32 OIHW parameter -> PackedWeight (a one-conv WeightPackPlan, packed once)."""
     w = w.detach()
-    assert w.dtype == torch.float32 and w.dim() == 4
-    if not w.is_contiguous():
-        w = w.contiguous()
-    cout, cin, kh, kw = w.shape
-    assert kh == kw
-    taps = kh * kw
-    cin_p, cout_p = round_up(cin, 8), round_up(cout, 8)
-    wf = _slab(taps, cout, cin_p, split, w.device)
-    wd = _slab(taps, cin, cout_p, split, w.device) if need_dgrad else None
-    _lib.check(lib.semseg_pack_weights(_ptr(w), cout, cin, taps, _ptr(wf), cout, cin_p, _ptr(wd),
-                                       cin if need_dgrad else 0, cout_p if need_dgrad else 0, int(bool(split)),
-                                       _stream()),
-               "semseg_pack_weights")
-    return PackedWeight(wf, wd, cout, cin, taps, kh, bool(split))
+    plan = WeightPackPlan([w if w.is_contiguous() else w.contiguous()], split, dgrad=need_dgrad)
+    plan.refresh()
+    return plan.packs[0]
 
 
 class WeightPackPlan:
     """Persistent bf16 operand slabs for a list of conv weights, refreshed in ONE launch (semseg_pack_weights_multi).
 
     The fp32 OIHW parameters stay the masters (optimizer / DDP / checkpoints); after an optimizer step every conv of the
-    model needs new slabs, which costs 2 launches per conv on the per-layer path. The plan owns one (wf, wd) pair per
-    conv and a device-side item table; `refresh()` re-packs all of them into the same buffers."""
+    model needs new slabs. The plan owns the slabs of every conv (wf; wd when `dgrad`; wp where `patches[k]`) and a
+    device-side item table; `refresh()` re-packs all of them into the same buffers. Building a plan uploads the table,
+    so it cannot be done while a CUDA graph is being captured; refreshing can."""
 
-    def __init__(self, weights, split=False):
-        import ctypes
+    def __init__(self, weights, split=False, dgrad=True, patches=None):
         _require_cuda(*weights)
         self.split = bool(split)
         self.weights = [w for w in weights]
@@ -201,13 +190,15 @@ class WeightPackPlan:
             assert w.dtype == torch.float32 and w.dim() == 4 and w.is_contiguous() and w.shape[2] == w.shape[3]
             cout, cin, kh, _ = w.shape
             taps = kh * kh
-            assert taps <= MAX_TAPS
+            patch = bool(patches and patches[k])
+            assert taps <= MAX_TAPS and (not patch or (taps == 9 and cin <= 3))
             cin_p, cout_p = round_up(cin, 8), round_up(cout, 8)
             wf = _slab(taps, cout, cin_p, self.split, w.device)
-            wd = _slab(taps, cin, cout_p, self.split, w.device)
-            self.packs.append(PackedWeight(wf, wd, cout, cin, taps, kh, self.split))
+            wd = _slab(taps, cin, cout_p, self.split, w.device) if dgrad else None
+            wp = _slab(1, cout, 32, self.split, w.device) if patch else None
+            self.packs.append(PackedWeight(wf, wd, wp, cout, cin, taps, kh, self.split))
             it = items[k]
-            it.w, it.wf, it.wd = w.data_ptr(), wf.data_ptr(), wd.data_ptr()
+            it.w, it.wf, it.wd, it.wp = w.data_ptr(), wf.data_ptr(), _ptr(wd).value, _ptr(wp).value
             it.Cout, it.Cin, it.taps, it.cols_f, it.cols_d = cout, cin, taps, cin_p, cout_p
             it.tile0, it.tiles_ci, it.split = tile0, (cin_p + 31) // 32, int(self.split)
             tile0 += it.tiles_ci * ((cout_p + 31) // 32)

@@ -39,7 +39,7 @@ def test_no_undeclared_exports():
 def test_ctypes_binding_covers_header():
     assert sorted(_lib.SIGNATURES) == header_symbols()
     lib = _lib.load()
-    assert lib.semseg_abi_version() == 2
+    assert lib.semseg_abi_version() == 3
     assert lib.semseg_launch_count() == 0 or lib.semseg_launch_count() > 0
 
 
@@ -51,8 +51,9 @@ def test_struct_layout_matches_header():
 #include "semseg_b200.h"
 #include <stddef.h>
 int main(void) {
-  printf("%zu %zu %zu %zu %zu %zu\n", sizeof(semseg_conv_desc), sizeof(semseg_wgrad_desc), sizeof(semseg_pack_item),
-         offsetof(semseg_pack_item, Cout), offsetof(semseg_pack_item, tile0), offsetof(semseg_pack_item, tiles_ci));
+  printf("%zu %zu %zu %zu %zu %zu %zu\n", sizeof(semseg_conv_desc), sizeof(semseg_wgrad_desc), sizeof(semseg_pack_item),
+         offsetof(semseg_pack_item, wp), offsetof(semseg_pack_item, Cout), offsetof(semseg_pack_item, tile0),
+         offsetof(semseg_pack_item, tiles_ci));
   return 0;
 }
 '''
@@ -61,13 +62,13 @@ int main(void) {
         open(c, "w").write(prog)
         exe = os.path.join(d, "t")
         subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
-        a, b, c, o_cout, o_tile0, o_tiles = map(int, subprocess.check_output([exe]).split())
+        a, b, c, o_wp, o_cout, o_tile0, o_tiles = map(int, subprocess.check_output([exe]).split())
     assert a == ctypes.sizeof(_lib.ConvDesc)
     assert b == ctypes.sizeof(_lib.WgradDesc)
     # the item table of semseg_pack_weights_multi is built by ctypes and read by the device code
     assert c == ctypes.sizeof(_lib.PackItem)
-    assert (o_cout, o_tile0, o_tiles) == (_lib.PackItem.Cout.offset, _lib.PackItem.tile0.offset,
-                                          _lib.PackItem.tiles_ci.offset)
+    assert (o_wp, o_cout, o_tile0, o_tiles) == (_lib.PackItem.wp.offset, _lib.PackItem.Cout.offset,
+                                                _lib.PackItem.tile0.offset, _lib.PackItem.tiles_ci.offset)
 
 
 def test_invalid_arguments_return_error_codes_without_gpu():
@@ -85,6 +86,7 @@ def test_invalid_arguments_return_error_codes_without_gpu():
     assert lib.semseg_im2col3x3s2(ctypes.c_void_p(16), 8, 1, 9, 9, 4, ctypes.c_void_p(16), None) == -1
     assert b"im2col3x3s2" in lib.semseg_last_error()
     assert lib.semseg_pack_weights_multi(None, 1, 1, 9, None) == -1
+    assert not hasattr(lib, "semseg_pack_weights")          # the one-launch packing is the only packing entry point
 
 
 def test_round2_struct_layouts_match_header():

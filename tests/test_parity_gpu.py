@@ -173,25 +173,58 @@ def test_conv_epilogues():
     assert bool((buf[..., :256] == 0).all())
 
 
+def _slabs_ref(w, split, patches):
+    """torch restatement of the operand slab layouts of fp32 OIHW `w`: wf[t][co][ci] and wd[t][ci][co] zero padded to
+    widths rounded up to 8, wp[0][co][t*Cin + ci] zero padded to 32 columns (None unless `patches`); each as bf16, or as
+    [2][...] = (hi, lo) with hi = bf16(v) and lo = bf16(v - hi) when `split`."""
+    cout, cin, k, _ = w.shape
+    taps = k * k
+    wt = w.reshape(cout, cin, taps)
+    wf = torch.zeros((taps, cout, (cin + 7) // 8 * 8), device=w.device)
+    wf[:, :, :cin] = wt.permute(2, 0, 1)
+    wd = torch.zeros((taps, cin, (cout + 7) // 8 * 8), device=w.device)
+    wd[:, :, :cout] = wt.permute(2, 1, 0)
+    wp = None
+    if patches:
+        wp = torch.zeros((1, cout, 32), device=w.device)
+        wp[0, :, :taps * cin] = wt.permute(0, 2, 1).reshape(cout, taps * cin)
+
+    def bf16(v):
+        if v is None:
+            return None
+        hi = v.to(torch.bfloat16)
+        return torch.stack([hi, (v - hi.float()).to(torch.bfloat16)]) if split else hi
+    return bf16(wf), bf16(wd), bf16(wp)
+
+
 def test_pack_weights_multi_matches_per_layer_pack():
-    """One-launch packing of a whole list of conv weights == the per-layer kernels, bit for bit (incl. zero padding of
-    Cin = 3 -> 8 and Cout = 150 -> 152), and again after an in-place update of the masters."""
+    """One-launch packing of a list of conv weights == a torch restatement of the slab layouts, bit for bit, in bf16 and
+    bf16x3: wf, wd (or none), the stem's patch slab wp, zero padding of Cin = 3 -> 8 and Cout = 150 -> 152, hi and lo
+    slabs; again after an in-place update of the masters; the per-layer ops.pack_weights gives the same slabs."""
     from semseg_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(11)
     shapes = [(64, 3, 3), (64, 64, 3), (256, 64, 1), (150, 512, 1), (512, 4096, 3), (40, 24, 3), (2048, 512, 1)]
     ws = [torch.randn((co, ci, k, k), device="cuda", generator=g) for co, ci, k in shapes]
-    plan = ops.WeightPackPlan(ws)
-    for rnd in range(2):
-        for pk in plan.packs:                      # poison: every element must be rewritten
-            pk.wf.fill_(7.0)
-            pk.wd.fill_(7.0)
-        plan.refresh()
-        for w, pk in zip(ws, plan.packs):
-            ref = ops.pack_weights(w)
-            assert torch.equal(pk.wf, ref.wf) and torch.equal(pk.wd, ref.wd), tuple(w.shape)
-        for w in ws:
-            w.mul_(0.5).add_(0.01)
-    assert plan.valid_for(ws) and not plan.valid_for(ws[:-1])
+    patches = [sh == (64, 3, 3) for sh in shapes]
+    for split, dgrad in ((False, True), (False, False), (True, True), (True, False)):
+        plan = ops.WeightPackPlan(ws, split, dgrad=dgrad, patches=patches)
+        for rnd in range(2):
+            for pk in plan.packs:                      # poison: every element must be rewritten
+                for t in (pk.wf, pk.wd, pk.wp):
+                    if t is not None:
+                        t.fill_(7.0)
+            plan.refresh()
+            for w, pk, patch in zip(ws, plan.packs, patches):
+                wf, wd, wp = _slabs_ref(w, split, patch)
+                what = (tuple(w.shape), split, dgrad, rnd)
+                assert torch.equal(pk.wf, wf), what
+                assert torch.equal(pk.wd, wd) if dgrad else pk.wd is None, what
+                assert torch.equal(pk.wp, wp) if patch else pk.wp is None, what
+                one = ops.pack_weights(w, need_dgrad=dgrad, split=split)
+                assert torch.equal(one.wf, pk.wf) and (torch.equal(one.wd, pk.wd) if dgrad else one.wd is None), what
+            for w in ws:
+                w.mul_(0.5).add_(0.01)
+        assert plan.valid_for(ws, split) and not plan.valid_for(ws[:-1], split) and not plan.valid_for(ws, not split)
 
 
 def test_bn_kernels_vs_torch():
