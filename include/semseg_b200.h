@@ -344,7 +344,8 @@ int semseg_resize_bilinear_bwd(const void* dy, const void* dy_lo, int dy_pitch, 
                                int Wo, void* dx, void* dx_lo, int dx_pitch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused logit upsample (bilinear, align_corners=True, x8) + cross-entropy (ignore_index, mean over valid
+ * Fused logit upsample (bilinear, align_corners=True, x8; the zoom entry points below take zoom 1, 2, 4 or 8) +
+ * cross-entropy (ignore_index, mean over valid
  * pixels) + argmax: F.interpolate + CrossEntropyLoss + max(1) of model/pspnet.py:94-103 without the
  * [N, classes, Ho, Wo] tensor. Requires Ho = 8(h-1)+1, Wo = 8(w-1)+1 (zoom_factor 8), classes <= 256.
  *   logits fp32 NHWC [N,h,w,C] (pitch), target int64 [N,Ho,Wo].
@@ -361,6 +362,18 @@ long long semseg_upsample_ce_bwd_workspace_floats(int N, int Ho, int w, int C);
 int semseg_upsample_ce_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                            int Ho, int Wo, int ignore_index, const float* lse, const float* loss_info,
                            const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* The same at zoom factor `zoom` in {1, 2, 4, 8}: requires Ho = zoom(h-1)+1, Wo = zoom(w-1)+1 (zoom 1: no
+ * interpolation, plain cross-entropy + argmax of the logits). The forward workspace holds 2 floats per forward CTA,
+ * N * ((Ho-1)/zoom+1) * ceil(Wo/128) CTAs; the backward one [N][(Ho-1)/zoom+1][2][w][C] floats. The workspace functions
+ * return -1 for a zoom outside {1, 2, 4, 8}. Zoom 8 is exactly the entry points above. */
+long long semseg_upsample_ce_zoom_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_ce_zoom_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                int Ho, int Wo, int zoom, int ignore_index, float* workspace, float* loss_out,
+                                int64_t* argmax, float* lse, void* stream);
+long long semseg_upsample_ce_zoom_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_zoom_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* loss_info,
+                                const float* grad_out, float* workspace, float* dlogits, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sliding-window evaluation after the network (semseg_b200/inference.py, exact=False). No tensor cores, no atomics.

@@ -1,15 +1,19 @@
-// Fused logit upsample (bilinear, align_corners=True, x8) + cross-entropy(ignore_index) + argmax.
+// Fused logit upsample (bilinear, align_corners=True, xZ for zoom_factor Z in {1, 2, 4, 8}) + cross-entropy(ignore_index)
+// + argmax.
 //
 // Replaces F.interpolate -> CrossEntropyLoss -> max(1) at model/pspnet.py:94-103 (same in model/psanet.py:168-177),
-// which materialise an [N, classes, H, W] fp32 tensor (2.15 GB at bs16 / 150 classes / 473x473) and stream it
+// which materialise an [N, classes, H, W] fp32 tensor (2.15 GB at bs16 / 150 classes / 473x473, zoom 8) and stream it
 // ~9 times per head. Here the low-resolution logits (fp32 NHWC, a few MB, L2 resident) are staged in shared
 // memory and every output pixel's class vector is interpolated on the fly; the only full-resolution tensors
 // are the int64 argmax and an fp32 log-sum-exp map kept for the backward pass.
 //
-// The kernels require Ho = 8*(h-1)+1 and Wo = 8*(w-1)+1 (zoom_factor 8, every shipped config): then the
-// align_corners scale (h-1)/(Ho-1) is exactly 1/8, source index = x >> 3 and the weights are (x & 7)/8 — the same
-// fp32 values ATen computes. Interpolation order follows ATen's upsample_bilinear2d:
+// The kernels are templated on the zoom factor Z and require Ho = Z*(h-1)+1 and Wo = Z*(w-1)+1. For a power-of-two Z
+// the align_corners scale (h-1)/(Ho-1) is exactly 1/Z in fp32, so the source index is x / Z and the weights (x % Z)/Z
+// are exact — the same fp32 values ATen computes. Interpolation order follows ATen's upsample_bilinear2d:
 //   v = l0h*(l0w*v00 + l1w*v01) + l1h*(l0w*v10 + l1w*v11).
+// Z = 1 is plain cross-entropy + argmax + lse on the NHWC logits (model/pspnet.py:94 skips the interpolation): one node
+// row is staged and v is the logit itself. Every shipped config uses Z = 8; the Z = 8 instance is the kernel the
+// original x8-only entry points ran, instruction for instruction.
 //
 // Backward is a deterministic, separable gather (rows kernel + cols kernel, see below). No atomics, every dlogits
 // element is written exactly once.
@@ -27,26 +31,49 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr int kFwdCols = 128;                    // output columns per CTA (one per thread)
-constexpr int kFwdNodes = kFwdCols / 8 + 1;      // low-res node columns a CTA touches
 
-// One CTA per (128 output columns, low-res interval row i0, image); a thread owns one output column and the 8
+// Compile-time geometry of zoom factor Z (a power of two): source index x >> kShift, fraction (x & kMask) * kStep.
+template <int Z>
+struct Zoom {
+  static_assert(Z == 1 || Z == 2 || Z == 4 || Z == 8, "zoom factor must be 1, 2, 4 or 8");
+  static constexpr int kShift = Z == 1 ? 0 : Z == 2 ? 1 : Z == 4 ? 2 : 3;
+  static constexpr int kMask = Z - 1;
+  static constexpr float kStep = 1.f / Z;                 // exact: Z is a power of two
+  static constexpr int kNodes = kFwdCols / Z + 1;         // low-res node columns a forward CTA touches
+  static constexpr int kNodeRows = Z == 1 ? 1 : 2;        // node rows a forward CTA stages (Z = 1: no vertical lerp)
+};
+
+// Output row r of an interval from its horizontally interpolated node rows, compile-time row weights r/Z.
+template <int Z>
+__device__ __forceinline__ float row_lerp(float top, float bot, int r) {
+  if constexpr (Z == 1) {
+    return top;
+  } else {
+    return (1.f - Zoom<Z>::kStep * r) * top + (Zoom<Z>::kStep * r) * bot;
+  }
+}
+
+// One CTA per (128 output columns, low-res interval row i0, image); a thread owns one output column and the Z
 // output rows of the interval. Per class the horizontal interpolation of the two node rows (top, bot) is done once
-// and shared by the 8 rows (v = l0h*top + l1h*bot with compile-time row weights), so a pixel-class costs ~5
+// and shared by the Z rows (v = l0h*top + l1h*bot with compile-time row weights), so at Z = 8 a pixel-class costs ~5
 // instructions per pass instead of a full 4-tap interpolation. Two passes over the classes: max/argmax, then
 // sum of exp2 — one MUFU per pixel-class, no rescaling branches.
+template <int Z>
 __global__ void __launch_bounds__(kFwdCols)
 upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
                        const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                        float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out) {
-  extern __shared__ float S[];  // [2][kFwdNodes][Cs]; Cs odd -> the 4-5 node columns a warp reads hit distinct banks
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs]; Cs odd -> the node columns a warp reads hit distinct banks
   __shared__ float red_loss[kFwdCols / 32];
   __shared__ float red_cnt[kFwdCols / 32];
   const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
   const int i1 = min(i0 + 1, h - 1);
-  const int j_base = x0 >> 3;
+  const int j_base = x0 >> G::kShift;
   const int nj = min(kFwdNodes, w - j_base);
   const int tid = threadIdx.x;
-  for (int idx = tid; idx < 2 * nj * C; idx += kFwdCols) {
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
     const int c = idx % C;
     const int node = idx / C;
     const int jj = node % nj, rr = node / nj;
@@ -56,62 +83,63 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
   __syncthreads();
   float loss = 0.f, cnt = 0.f;
   const int x = x0 + tid;
-  const int rows = min(8, Ho - 8 * i0);  // 8, or 1 for the last node row (Ho = 8(h-1)+1)
+  const int rows = min(Z, Ho - Z * i0);  // Z, or 1 for the last node row (Ho = Z(h-1)+1)
   if (x < Wo) {
-    const int j0 = x >> 3;
+    const int j0 = x >> G::kShift;
     const int j1 = min(j0 + 1, w - 1);
-    const float l1w = static_cast<float>(x & 7) * 0.125f, l0w = 1.f - l1w;
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
     const float* A = S + (j0 - j_base) * Cs;   // node (i0, j0)
     const float* B = S + (j1 - j_base) * Cs;   // node (i0, j1)
-    const float* Cc = A + kFwdNodes * Cs;      // node (i1, j0)
+    const float* Cc = A + kFwdNodes * Cs;      // node (i1, j0); not staged (and not read) at Z = 1
     const float* D = B + kFwdNodes * Cs;       // node (i1, j1)
-    float m[8], sum[8];
-    int am[8];
+    float m[Z], sum[Z];
+    int am[Z];
 #pragma unroll
-    for (int r = 0; r < 8; ++r) {
+    for (int r = 0; r < Z; ++r) {
       m[r] = -INFINITY;
       am[r] = 0;
       sum[r] = 0.f;
     }
 #pragma unroll 2
     for (int c = 0; c < C; ++c) {
-      const float top = l0w * A[c] + l1w * B[c];
-      const float bot = l0w * Cc[c] + l1w * D[c];
+      // the interval's two horizontally interpolated node rows (Z = 1: the logit itself)
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
 #pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        const float v = (1.f - 0.125f * r) * top + (0.125f * r) * bot;
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
         if (v > m[r]) {
           m[r] = v;
           am[r] = c;
         }
       }
     }
-    float m2[8];
+    float m2[Z];
 #pragma unroll
-    for (int r = 0; r < 8; ++r) m2[r] = m[r] * kLog2e;
+    for (int r = 0; r < Z; ++r) m2[r] = m[r] * kLog2e;
 #pragma unroll 2
     for (int c = 0; c < C; ++c) {
-      const float top = l0w * A[c] + l1w * B[c];
-      const float bot = l0w * Cc[c] + l1w * D[c];
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
 #pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        const float v = (1.f - 0.125f * r) * top + (0.125f * r) * bot;
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
         sum[r] += ex2_approx(fmaf(v, kLog2e, -m2[r]));
       }
     }
 #pragma unroll
-    for (int r = 0; r < 8; ++r) {
+    for (int r = 0; r < Z; ++r) {
       if (r < rows) {
-        const size_t pix = (static_cast<size_t>(n) * Ho + (8 * i0 + r)) * Wo + x;
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
         const long long t = target[pix];
         const float lse = m[r] + __logf(sum[r]);
         if (argmax_out) argmax_out[pix] = am[r];
         lse_out[pix] = lse;
         if (t != ignore_index && t >= 0 && t < C) {
           const int tc = static_cast<int>(t);
-          const float top = l0w * A[tc] + l1w * B[tc];
-          const float bot = l0w * Cc[tc] + l1w * D[tc];
-          const float vt = (1.f - 0.125f * r) * top + (0.125f * r) * bot;
+          const float top = Z == 1 ? A[tc] : l0w * A[tc] + l1w * B[tc];
+          const float bot = Z == 1 ? 0.f : l0w * Cc[tc] + l1w * D[tc];
+          const float vt = row_lerp<Z>(top, bot, r);
           loss += lse - vt;
           cnt += 1.f;
         }
@@ -170,26 +198,29 @@ __global__ void upsample_ce_reduce_kernel(const float* __restrict__ partial, int
 //   dL[i,j,c] = gs * sum_y wy(y,i) * sum_x wx(x,j) * g[y,x,c].
 // Phase 1 (rows): one CTA per (image, low-res interval row i0), one thread per class. The thread walks x = 0..Wo-1
 // with the four node values of its class in registers; per column the horizontal interpolation (top, bot) is shared
-// by the interval's 8 output rows and the rows are folded immediately with their compile-time vertical weights, so a
-// pixel-class costs ~10 instructions and one MUFU. (lse*log2e, target) of the 8 rows are staged in shared memory as
+// by the interval's Z output rows and the rows are folded immediately with their compile-time vertical weights, so at
+// Z = 8 a pixel-class costs ~10 instructions and one MUFU. (lse*log2e, target) of the Z rows are staged in shared memory as
 // one 8-byte word per pixel and read as warp-uniform broadcasts. Output: T2[n][i0][s][j][c], s = 0: the interval's
-// contribution to node row i0, s = 1: to node row i0+1 (fp32 workspace, 68 MB at bs16 / 150 classes).
+// contribution to node row i0, s = 1: to node row i0+1 (fp32 workspace, 68 MB at bs16 / 150 classes; at Z = 1 slot 1
+// is all zeros).
 // Phase 2 (cols): dL[i] = gs * (T2[i][0] + T2[i-1][1]).
 struct __align__(8) PixInfo {
   float lse2;  // log-sum-exp * log2(e)
   int t;       // target class, -1 = ignored
 };
 
+template <int Z>
 __global__ void __launch_bounds__(256)
 upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
                             const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                             const float* __restrict__ lse, float* __restrict__ T2) {
-  extern __shared__ PixInfo s_pix[];  // [8][Wo]
+  using G = Zoom<Z>;
+  extern __shared__ PixInfo s_pix[];  // [Z][Wo]
   const int i0 = blockIdx.x, n = blockIdx.y;
   const int i1 = min(i0 + 1, h - 1);
-  const int rows = min(8, Ho - 8 * i0);
+  const int rows = min(Z, Ho - Z * i0);
   for (int r = 0; r < rows; ++r) {
-    const size_t rowbase = (static_cast<size_t>(n) * Ho + (8 * i0 + r)) * Wo;
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
     for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
       const long long t = target[rowbase + x];
       PixInfo pi;
@@ -214,23 +245,23 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
     nb = L0[static_cast<size_t>(jn) * pitch];          // prefetch the next interval's right column
     nd = L1[static_cast<size_t>(jn) * pitch];
     float accL0 = 0.f, accR0 = 0.f, accL1 = 0.f, accR1 = 0.f;
-    const int xb = j0 * 8;
-    const int nx = min(8, Wo - xb);   // 8, or 1 for the last node column
-    if (rows == 8 && nx == 8) {
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);   // Z, or 1 for the last node column
+    if (rows == Z && nx == Z) {
 #pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const float l1w = 0.125f * k, l0w = 1.f - l1w;
+      for (int k = 0; k < Z; ++k) {
+        const float l1w = G::kStep * k, l0w = 1.f - l1w;
         const float top = l0w * a + l1w * b;
         const float bot = l0w * cc + l1w * d;
         float g0 = 0.f, g1 = 0.f;
 #pragma unroll
-        for (int r = 0; r < 8; ++r) {
+        for (int r = 0; r < Z; ++r) {
           const PixInfo pi = s_pix[r * Wo + xb + k];
           if (pi.t < 0) continue;  // warp-uniform
-          const float v = (1.f - 0.125f * r) * top + (0.125f * r) * bot;
+          const float v = row_lerp<Z>(top, bot, r);
           const float g = ex2_approx(fmaf(v, kLog2e, -pi.lse2)) - (c == pi.t ? 1.f : 0.f);
-          g0 = fmaf(1.f - 0.125f * r, g, g0);
-          g1 = fmaf(0.125f * r, g, g1);
+          g0 = fmaf(1.f - G::kStep * r, g, g0);
+          g1 = fmaf(G::kStep * r, g, g1);
         }
         accL0 = fmaf(l0w, g0, accL0);
         accR0 = fmaf(l1w, g0, accR0);
@@ -239,14 +270,14 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
       }
     } else {
       for (int k = 0; k < nx; ++k) {
-        const float l1w = 0.125f * k, l0w = 1.f - l1w;
+        const float l1w = G::kStep * k, l0w = 1.f - l1w;
         const float top = l0w * a + l1w * b;
         const float bot = l0w * cc + l1w * d;
         float g0 = 0.f, g1 = 0.f;
         for (int r = 0; r < rows; ++r) {
           const PixInfo pi = s_pix[r * Wo + xb + k];
           if (pi.t < 0) continue;
-          const float l1h = 0.125f * r, l0h = 1.f - l1h;
+          const float l1h = G::kStep * r, l0h = 1.f - l1h;
           const float v = l0h * top + l1h * bot;
           const float g = ex2_approx(fmaf(v, kLog2e, -pi.lse2)) - (c == pi.t ? 1.f : 0.f);
           g0 = fmaf(l0h, g, g0);
@@ -288,30 +319,52 @@ upsample_ce_bwd_cols_kernel(const float* __restrict__ T2, int N, int h, int w, i
 
 using namespace sb;
 
-static int check_tail(const void* logits, int pitch, int N, int h, int w, int C, const void* target, int Ho, int Wo) {
+static bool valid_zoom(int zoom) { return zoom == 1 || zoom == 2 || zoom == 4 || zoom == 8; }
+
+static int check_tail(const void* logits, int pitch, int N, int h, int w, int C, const void* target, int Ho, int Wo,
+                      int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce: zoom %d is not one of 1, 2, 4, 8", zoom);
   SB_CHECK_ARG(logits && target, "upsample_ce: null pointer");
   SB_CHECK_ARG(N > 0 && h > 1 && w > 1 && C > 1 && C <= kMaxClasses && pitch >= C, "upsample_ce: bad sizes (C<=%d)",
                kMaxClasses);
-  SB_CHECK_ARG(Ho == 8 * (h - 1) + 1 && Wo == 8 * (w - 1) + 1,
-               "upsample_ce: fused kernel needs Ho=8(h-1)+1, Wo=8(w-1)+1 (got %dx%d -> %dx%d)", h, w, Ho, Wo);
+  SB_CHECK_ARG(Ho == zoom * (h - 1) + 1 && Wo == zoom * (w - 1) + 1,
+               "upsample_ce: fused kernel needs Ho=%d(h-1)+1, Wo=%d(w-1)+1 (got %dx%d -> %dx%d)", zoom, zoom, h, w, Ho,
+               Wo);
   return SEMSEG_OK;
 }
 
-extern "C" long long semseg_upsample_ce_workspace_floats(int N, int Ho, int Wo) {
-  return 2LL * N * ((Ho - 1) / 8 + 1) * cdiv(Wo, kFwdCols);  // (loss, count) per forward CTA
+// The opt-in to more than 48 KB of dynamic shared memory is per device (nn.DataParallel replicas run the same kernels on
+// several devices, from several threads): made once for every device this process uses, to the kernel's largest size,
+// before the first launch on that device that needs it.
+template <typename Kernel>
+static int opt_in_smem(Kernel kernel, std::atomic<bool>* attr_set, int max_bytes) {
+  int dev = 0;
+  SB_CUDA(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
+    SB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_bytes));
+    if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
+  }
+  return SEMSEG_OK;
 }
 
-extern "C" int semseg_upsample_ce_fwd(const float* logits, int pitch, int N, int h, int w, int C,
-                                      const int64_t* target, int Ho, int Wo, int ignore_index, float* workspace,
-                                      float* loss_out, int64_t* argmax, float* lse, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo);
-  if (r) return r;
-  SB_CHECK_ARG(workspace && loss_out && lse, "upsample_ce_fwd: null output");
+constexpr size_t kSmemDefault = 48 * 1024;
+constexpr size_t kBwdSmemMax = 160 * 1024;   // staged (lse, target) words of the backward's Z output rows
+
+template <int Z>
+static int launch_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
+                      int ignore_index, float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                      cudaStream_t stream) {
   dim3 grid(cdiv(Wo, kFwdCols), h, N);
   const int Cs = C | 1;
-  const size_t smem = static_cast<size_t>(2) * kFwdNodes * Cs * sizeof(float);
-  upsample_ce_fwd_kernel<<<grid, kFwdCols, smem, stream>>>(
+  // at most 2 * 65 * 257 floats (Z = 2, 256 classes); above 48 KB only at Z <= 4 (Z = 1 and 2 with 150 classes: 78 KB)
+  constexpr size_t kMaxSmem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_ce_fwd_kernel<Z><<<grid, kFwdCols, smem, stream>>>(
       logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, workspace,
       reinterpret_cast<long long*>(argmax), lse);
   SB_LAUNCHED();
@@ -320,30 +373,96 @@ extern "C" int semseg_upsample_ce_fwd(const float* logits, int pitch, int N, int
   return SEMSEG_OK;
 }
 
+template <int Z>
+static int launch_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
+                      int ignore_index, const float* lse, const float* loss_info, const float* grad_out,
+                      float* workspace, float* dlogits, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(PixInfo);
+  SB_CHECK_ARG(smem <= kBwdSmemMax, "upsample_ce_bwd: output width %d too large for the staged rows", Wo);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_bwd_rows_kernel<Z>, attr_set, static_cast<int>(kBwdSmemMax));
+    if (r) return r;
+  }
+  upsample_ce_bwd_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, workspace);
+  SB_LAUNCHED();
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_zoom_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce: zoom %d is not one of 1, 2, 4, 8", zoom);
+  return 2LL * N * ((Ho - 1) / zoom + 1) * cdiv(Wo, kFwdCols);  // (loss, count) per forward CTA
+}
+
+extern "C" int semseg_upsample_ce_zoom_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                           const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                           float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                           void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse, "upsample_ce_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out, argmax,
+                                 lse, stream);
+    case 2: return launch_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out, argmax,
+                                 lse, stream);
+    case 4: return launch_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out, argmax,
+                                 lse, stream);
+    default: return launch_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out, argmax,
+                                  lse, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_zoom_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce: zoom %d is not one of 1, 2, 4, 8", zoom);
+  return 2LL * N * ((Ho - 1) / zoom + 1) * w * C;  // T2[N][h][2][w][C]
+}
+
+extern "C" int semseg_upsample_ce_zoom_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                           const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                           const float* lse, const float* loss_info, const float* grad_out,
+                                           float* workspace, float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  SB_CHECK_ARG(lse && loss_info && grad_out && dlogits && workspace, "upsample_ce_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
+                                 workspace, dlogits, stream);
+    case 2: return launch_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
+                                 workspace, dlogits, stream);
+    case 4: return launch_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
+                                 workspace, dlogits, stream);
+    default: return launch_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
+                                  workspace, dlogits, stream);
+  }
+}
+
+// The x8 entry points (zoom_factor 8, every shipped config): the Z = 8 instances above.
+extern "C" long long semseg_upsample_ce_workspace_floats(int N, int Ho, int Wo) {
+  return semseg_upsample_ce_zoom_workspace_floats(N, Ho, Wo, 8);
+}
+
+extern "C" int semseg_upsample_ce_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                      const int64_t* target, int Ho, int Wo, int ignore_index, float* workspace,
+                                      float* loss_out, int64_t* argmax, float* lse, void* stream_) {
+  return semseg_upsample_ce_zoom_fwd(logits, pitch, N, h, w, C, target, Ho, Wo, 8, ignore_index, workspace, loss_out,
+                                     argmax, lse, stream_);
+}
+
 extern "C" long long semseg_upsample_ce_bwd_workspace_floats(int N, int Ho, int w, int C) {
-  return 2LL * N * ((Ho - 1) / 8 + 1) * w * C;  // T2[N][h][2][w][C]
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, 8);
 }
 
 extern "C" int semseg_upsample_ce_bwd(const float* logits, int pitch, int N, int h, int w, int C,
                                       const int64_t* target, int Ho, int Wo, int ignore_index, const float* lse,
                                       const float* loss_info, const float* grad_out, float* workspace,
                                       float* dlogits, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo);
-  if (r) return r;
-  SB_CHECK_ARG(lse && loss_info && grad_out && dlogits && workspace, "upsample_ce_bwd: null pointer");
-  const int threads = (C + 31) / 32 * 32;
-  const size_t smem = static_cast<size_t>(8) * Wo * sizeof(PixInfo);
-  SB_CHECK_ARG(smem <= 160 * 1024, "upsample_ce_bwd: output width %d too large for the staged rows", Wo);
-  static size_t smem_attr = 48 * 1024;
-  if (smem > smem_attr) {
-    SB_CUDA(cudaFuncSetAttribute(upsample_ce_bwd_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    smem_attr = 160 * 1024;
-  }
-  upsample_ce_bwd_rows_kernel<<<dim3(h, N), threads, smem, stream>>>(
-      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, workspace);
-  SB_LAUNCHED();
-  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out, dlogits);
-  SB_LAUNCHED();
-  return SEMSEG_OK;
+  return semseg_upsample_ce_zoom_bwd(logits, pitch, N, h, w, C, target, Ho, Wo, 8, ignore_index, lse, loss_info,
+                                     grad_out, workspace, dlogits, stream_);
 }

@@ -10,6 +10,10 @@
 //   v = l0h*(l0w*v00 + l1w*v01) + l1h*(l0w*v10 + l1w*v11).
 // The mirrored crop's logits are interpolated in their own coordinates at x' = crop-1-x (= F.interpolate of the
 // flipped batch followed by .flip(3)); the two softmaxes are averaged as (p + p_mirror) * 0.5.
+// The kernel serves every zoom factor of the network: its input is always the 1/8-resolution logits. At zoom Z < 8 the
+// reference upsamples them xZ (the module output) and then x(8/Z) to the crop; one x8 upsample is the same function,
+// because the xZ grid nests in the x8 grid (align_corners), the xZ result is bilinear on each of its cells, and bilinear
+// interpolation of a bilinear function is exact. The two differ only by fp32 rounding.
 //
 // semseg_window_accumulate: a gather. Every pixel of the un-padded canvas sums in fp64 the scores of the crops that
 // cover it in grid (row-major) order, starting from 0.0, and divides by their count: the same fp64 operations in the

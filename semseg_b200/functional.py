@@ -480,39 +480,44 @@ def conv_bias_f32(x, conv):
 
 # ------------------------------------------------------------------------------------------------ fused tail
 class _UpsampleCE(torch.autograd.Function):
-    """bilinear x8 upsample (align_corners) + CrossEntropyLoss(ignore_index, mean) + argmax in one kernel each way
-    (model/pspnet.py:94-103) — the [N, classes, H, W] logits tensor is never materialised."""
+    """bilinear xZ upsample (align_corners; Z = zoom_factor in {1, 2, 4, 8}, none at 1) + CrossEntropyLoss(ignore_index,
+    mean) + argmax in one kernel each way (model/pspnet.py:94-103) — the [N, classes, H, W] logits tensor is never
+    materialised."""
 
     @staticmethod
-    def forward(ctx, logits, target, ignore_index):
-        info, amax, lse = ops.upsample_ce_fwd(logits, target, ignore_index)
+    def forward(ctx, logits, target, ignore_index, zoom):
+        info, amax, lse = ops.upsample_ce_fwd(logits, target, ignore_index, zoom=zoom)
         ctx.save_for_backward(logits, target, lse, info)
-        ctx.ignore_index = ignore_index
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
         ctx.mark_non_differentiable(amax)
         return info[0], amax
 
     @staticmethod
     def backward(ctx, grad_loss, _grad_amax):
         logits, target, lse, info = ctx.saved_tensors
-        return ops.upsample_ce_bwd(logits, target, ctx.ignore_index, lse, info, grad_loss), None, None
+        return ops.upsample_ce_bwd(logits, target, ctx.ignore_index, lse, info, grad_loss, zoom=ctx.zoom), None, None, None
 
 
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
-    """The fused kernel implements exactly nn.CrossEntropyLoss(ignore_index=k) with default options at zoom 8.
+    """The fused kernel implements exactly nn.CrossEntropyLoss(ignore_index=k) with default options, at every zoom factor
+    of the model (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if not (type(criterion) is nn.CrossEntropyLoss and criterion.weight is None and criterion.reduction == 'mean'
-            and getattr(criterion, 'label_smoothing', 0.0) == 0.0 and zoom_factor == 8 and target is not None
-            and target.dtype == torch.int64 and target.dim() == 3):
+            and getattr(criterion, 'label_smoothing', 0.0) == 0.0 and zoom_factor in (1, 2, 4, 8)
+            and target is not None and target.dtype == torch.int64 and target.dim() == 3):
         return False
     if logits is None:
-        return target.shape[1] == x_size[2] and target.shape[2] == x_size[3]
-    return (logits.shape[-1] <= 256 and target.shape[1] == 8 * (logits.shape[1] - 1) + 1
-            and target.shape[2] == 8 * (logits.shape[2] - 1) + 1)
+        h, w = (x_size[2] - 1) // 8 + 1, (x_size[3] - 1) // 8 + 1      # the network's output stride is 8
+    else:
+        if logits.shape[-1] > 256:
+            return False
+        h, w = logits.shape[1], logits.shape[2]
+    return target.shape[1] == zoom_factor * (h - 1) + 1 and target.shape[2] == zoom_factor * (w - 1) + 1
 
 
-def upsample_ce(logits, target, ignore_index):
-    """-> (mean CE loss scalar, argmax int64 [N,H,W])."""
-    return _UpsampleCE.apply(logits, target.contiguous(), ignore_index)
+def upsample_ce(logits, target, ignore_index, zoom=8):
+    """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1."""
+    return _UpsampleCE.apply(logits, target.contiguous(), ignore_index, int(zoom))
 
 
 # ------------------------------------------------------------------------------------------------ pyramid pooling

@@ -14,11 +14,15 @@ accumulation / normalisation by the overlap count stay on the device. Two ways t
     the sum over scales and the argmax also run on the device; only the result crosses PCIe. At 1024x2048 x 19 classes
     the host steps of the reference procedure (float64 [h, w, classes] arrays through cv2 and numpy) cost several times
     the network itself. Scores agree with the exact path to ~1e-7.
-    When the model is this package's PSPNet / PSANet (eval mode, CUDA, zoom factor 8, crop = 8(h'-1)+1, at most 256
-    classes) everything after the network runs on the native kernels of csrc/window.cu: one kernel turns the 1/8
+    When the model is this package's PSPNet / PSANet (eval mode, CUDA, crop = 8(h'-1)+1, at most 256 classes, any zoom
+    factor) everything after the network runs on the native kernels of csrc/window.cu: one kernel turns the 1/8
     resolution logits of a batch into flip-averaged softmax scores (the upsampled [2G, classes, crop, crop] logits never
     exist), one gathers a scale's crops into its overlap-normalised fp64 canvas (bit-identical to the ATen loop), and
     one resizes the canvas and adds it into the running total. Any other model runs the ATen steps below.
+    At zoom factor Z < 8 the model's output is the logits upsampled xZ, and the ATen steps upsample that again by 8/Z
+    to the crop. The native kernel upsamples the 1/8-resolution logits x8 straight to the crop instead. The two are
+    equal up to fp32 rounding: the xZ grid nests in the x8 grid (align_corners), the xZ result is bilinear on every
+    cell of its grid, and bilinear interpolation reproduces a bilinear function exactly.
 `net_process` / `scale_process` keep the reference's signatures and return types (and the exact arithmetic);
 `SlidingWindowPredictor` is the object form that also covers the per-image scale loop.
 
@@ -65,8 +69,9 @@ def _native_net(model, classes, crop_h, crop_w, device):
         if len(model.device_ids) > 1:
             return None
         model = model.module
+    # any zoom factor: the scores kernel upsamples the 1/8-resolution logits x8 (see the module docstring)
     if not (type(model) in (PSPNet, PSANet) and not model.training and device.type == "cuda"
-            and model.zoom_factor == 8 and (crop_h - 1) % 8 == 0 and (crop_w - 1) % 8 == 0 and classes <= 256):
+            and (crop_h - 1) % 8 == 0 and (crop_w - 1) % 8 == 0 and classes <= 256):
         return None
     return model
 

@@ -635,37 +635,41 @@ def act_to_f32(x):
 
 
 # ------------------------------------------------------------------------------------------------ fused tail
-def upsample_ce_fwd(logits, target, ignore_index, want_argmax=True):
-    """logits fp32 NHWC [N,h,w,C], target int64 [N,Ho,Wo] -> (loss_info [2] = (mean CE, count), argmax, lse)."""
+def upsample_ce_fwd(logits, target, ignore_index, want_argmax=True, zoom=8):
+    """logits fp32 NHWC [N,h,w,C], target int64 [N,Ho,Wo] with Ho = zoom*(h-1)+1, Wo = zoom*(w-1)+1 (zoom 1, 2, 4 or 8)
+    -> (loss_info [2] = (mean CE, count), argmax, lse)."""
     _require_cuda(logits, target)
     lib = _lib.load()
     assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
     assert target.dtype == torch.int64 and target.is_contiguous()
     n, h, w, c = logits.shape
     _, ho, wo = target.shape
-    nws = int(lib.semseg_upsample_ce_workspace_floats(n, ho, wo))
+    nws = int(lib.semseg_upsample_ce_zoom_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_zoom_workspace_floats")
     ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
     info = torch.empty((2,), dtype=torch.float32, device=logits.device)
     amax = torch.empty((n, ho, wo), dtype=torch.int64, device=logits.device) if want_argmax else None
     lse = torch.empty((n, ho, wo), dtype=torch.float32, device=logits.device)
-    _lib.check(lib.semseg_upsample_ce_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
-                                          int(ignore_index), _ptr(ws), _ptr(info), _ptr(amax), _ptr(lse), _stream()),
-               "semseg_upsample_ce_fwd")
+    _lib.check(lib.semseg_upsample_ce_zoom_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                               int(zoom), int(ignore_index), _ptr(ws), _ptr(info), _ptr(amax),
+                                               _ptr(lse), _stream()),
+               "semseg_upsample_ce_zoom_fwd")
     return info, amax, lse
 
 
-def upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_out):
+def upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_out, zoom=8):
     lib = _lib.load()
     n, h, w, c = logits.shape
     _, ho, wo = target.shape
     dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
-    ws = torch.empty((int(lib.semseg_upsample_ce_bwd_workspace_floats(n, ho, w, c)),), dtype=torch.float32,
-                     device=logits.device)
+    nws = int(lib.semseg_upsample_ce_zoom_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_zoom_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
     g = grad_out.reshape(1).float().contiguous()
-    _lib.check(lib.semseg_upsample_ce_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
-                                          int(ignore_index), _ptr(lse), _ptr(info), _ptr(g), _ptr(ws), _ptr(dl),
-                                          _stream()),
-               "semseg_upsample_ce_bwd")
+    _lib.check(lib.semseg_upsample_ce_zoom_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                               int(zoom), int(ignore_index), _ptr(lse), _ptr(info), _ptr(g), _ptr(ws),
+                                               _ptr(dl), _stream()),
+               "semseg_upsample_ce_zoom_bwd")
     return dl
 
 
