@@ -80,6 +80,23 @@ int semseg_psa_attend_bwd_attn(int psa_type, const float* attn, int a_pitch, con
                                const void* dout, const void* dout_lo, int dout_pitch, float* dattn, int N, int H, int W,
                                int mH, int mW, int C, float scale, void* stream);
 
+/* The same two operations for every option of the reference's PSA module (model/psanet.py:76-84). `form` is a bit mask:
+ *   SEMSEG_PSA_DENSE      compact=True: mH*mW == H*W and a_pitch >= H*W; the owner's attention vector is indexed by the
+ *                         other pixel's flat position (collect: L[t,s] = attn[t][s], distribute: L[t,s] = attn[s][t]);
+ *                         every element of dattn is written from it. Without the bit: the odd mH x mW window above.
+ *   SEMSEG_PSA_NO_SOFTMAX psa_softmax=False: P = L. stats may be NULL and are neither written nor read; in the logit
+ *                         gradient dattn = scale * dout . feat^T scattered back, and out / out_lo may be NULL.
+ * form 0 is semseg_psa_attend / semseg_psa_attend_bwd_attn, bit for bit. */
+#define SEMSEG_PSA_DENSE 1
+#define SEMSEG_PSA_NO_SOFTMAX 2
+int semseg_psa_attend_ex(int mode, int psa_type, int form, const float* attn, int a_pitch, const void* feat,
+                         const void* feat_lo, int feat_pitch, float* stats, void* out, void* out_lo, int out_pitch, int N,
+                         int H, int W, int mH, int mW, int C, float scale, void* stream);
+int semseg_psa_attend_bwd_attn_ex(int psa_type, int form, const float* attn, int a_pitch, const float* stats,
+                                  const void* feat, const void* feat_lo, int feat_pitch, const void* out,
+                                  const void* out_lo, int out_pitch, const void* dout, const void* dout_lo, int dout_pitch,
+                                  float* dattn, int N, int H, int W, int mH, int mW, int C, float scale, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Implicit-GEMM convolution on wgmma tensor cores (bf16 operands, fp32 accumulation in registers).
  *

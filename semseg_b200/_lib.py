@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libsemseg_b200.so")
 
 MAX_TAPS = 9
 EPI_RAW, EPI_AFFINE, EPI_F32 = 0, 1, 2
+PSA_DENSE, PSA_NO_SOFTMAX = 1, 2          # form bits of semseg_psa_attend_ex / semseg_psa_attend_bwd_attn_ex
 
 c_int = ctypes.c_int
 c_i32 = ctypes.c_int32
@@ -96,6 +97,11 @@ SIGNATURES = {
                                   c_int, c_int, c_int, c_int, c_f, c_vp]),
     "semseg_psa_attend_bwd_attn": (c_int, [c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp,
                                            c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_f, c_vp]),
+    "semseg_psa_attend_ex": (c_int, [c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int,
+                                     c_int, c_int, c_int, c_int, c_int, c_int, c_f, c_vp]),
+    "semseg_psa_attend_bwd_attn_ex": (c_int, [c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_vp, c_vp, c_int,
+                                              c_vp, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_f,
+                                              c_vp]),
     "semseg_conv_stats_rows": (c_int, [c_int, c_int, c_int, c_int]),
     "semseg_conv_k_slices": (c_int, [c_int, c_int, c_int]),
     "semseg_conv_splitk_rows": (c_int, [c_int]),

@@ -7,6 +7,10 @@
 //   distribute (psa_type 1): L[t, s] = A[s, idx(t - s)]   (one entry of every SOURCE pixel's vector)
 //   idx(d) = (d.y + hh) * mW + (d.x + hw); positions outside the mask window contribute logit 0 (the reference zero-fills
 //   psa_mask's output BEFORE the softmax, lib/psa/functions/psamask.py:17).
+// Two more forms of the same gather (template parameters; the window + softmax instances are the original kernels):
+//   dense (compact=True, model/psanet.py:76-79): mH*mW == HW and the owner's vector is indexed by the other pixel's flat
+//     position, L[t, s] = A[t, s] (collect) or A[s, t] (distribute: the reference's view(n,hw,hw).transpose(1,2));
+//   no softmax (psa_softmax=False): P = L, no statistics are computed or read.
 // A = attention logits fp32 NHWC [N, HW, a_pitch] straight from the 1x1 conv's F32 epilogue (no NCHW copy).
 //
 // One kernel template covers the forward aggregation AND the feature gradient of the backward pass, which is the same
@@ -56,13 +60,17 @@ struct PsaFusedParams {
   float scale;          // 1 / normalization_factor
 };
 
+// logit of attention element (own, other): window form = the owner's mask entry at offset other - own, zero outside the
+// window; dense form = the owner's entry at the other pixel's flat position `oth`
+template <bool kDense>
 __device__ __forceinline__ float pf_logit(const float* __restrict__ An, int a_pitch, int own, int own_i, int own_j,
-                                          int oth_i, int oth_j, int hh, int hw, int mH, int mW) {
+                                          int oth, int oth_i, int oth_j, int hh, int hw, int mH, int mW) {
+  if (kDense) return __ldg(An + static_cast<size_t>(own) * a_pitch + oth);
   const int a = oth_i - own_i + hh, b = oth_j - own_j + hw;
   return (a >= 0 && a < mH && b >= 0 && b < mW) ? __ldg(An + static_cast<size_t>(own) * a_pitch + a * mW + b) : 0.f;
 }
 
-template <bool kRowOwner, bool kStatsRow>
+template <bool kRowOwner, bool kStatsRow, bool kDense, bool kSoftmax>
 __global__ void __launch_bounds__(kPfThreads, 1)
 psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmB_lo,
                   const PsaFusedParams p) {
@@ -126,18 +134,19 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
   const int wt = threadIdx.x - 128;         // 0..255
   const int ww = wt >> 5;                    // worker warp 0..7
   // ---- (a) softmax statistics of the tile's rows (forward kernels)
-  if (kStatsRow) {
+  if (kSoftmax && kStatsRow) {
     if (kRowOwner) {
       // collect: row = target, its own attention vector, contiguous along the source column -> one warp per row
       for (int r = ww; r < kPfRows; r += kPfWorkers / 32) {
         float m = -INFINITY, sum = 0.f;
         if (r < live_rows) {
           const int own = pos0 + r, ri = own / p.W, rj = own - ri * p.W;
-          for (int q = lane; q < Q; q += 32) m = fmaxf(m, pf_logit(An, p.a_pitch, own, ri, rj, q / p.W, q % p.W, hh, hw, p.mH, p.mW));
+          for (int q = lane; q < Q; q += 32)
+            m = fmaxf(m, pf_logit<kDense>(An, p.a_pitch, own, ri, rj, q, q / p.W, q % p.W, hh, hw, p.mH, p.mW));
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
           for (int q = lane; q < Q; q += 32)
-            sum += __expf(pf_logit(An, p.a_pitch, own, ri, rj, q / p.W, q % p.W, hh, hw, p.mH, p.mW) - m);
+            sum += __expf(pf_logit<kDense>(An, p.a_pitch, own, ri, rj, q, q / p.W, q % p.W, hh, hw, p.mH, p.mW) - m);
 #pragma unroll
           for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
           if (lane == 0) stats_n[own] = make_float2(m, 1.f / sum);
@@ -158,7 +167,7 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
         if (r < live_rows) {
           const int pos = pos0 + r, ri = pos / p.W, rj = pos - ri * p.W;
           for (int q = q0; q < q1; ++q) {
-            const float l = pf_logit(An, p.a_pitch, q, q / p.W, q % p.W, ri, rj, hh, hw, p.mH, p.mW);
+            const float l = pf_logit<kDense>(An, p.a_pitch, q, q / p.W, q % p.W, pos, ri, rj, hh, hw, p.mH, p.mW);
             const float mn = fmaxf(m, l);
             sum = sum * __expf(m - mn) + __expf(l - mn);
             m = mn;
@@ -211,8 +220,10 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
         float pv = 0.f;
         if (q < Q) {
           const int qi = q / p.W, qj = q - qi * p.W;
-          const float l = pf_logit(An, p.a_pitch, rpos, ri, rj, qi, qj, hh, hw, p.mH, p.mW);
-          if (kStatsRow) {
+          const float l = pf_logit<kDense>(An, p.a_pitch, rpos, ri, rj, q, qi, qj, hh, hw, p.mH, p.mW);
+          if (!kSoftmax) {
+            pv = l;
+          } else if (kStatsRow) {
             pv = __expf(l - s_m[r]) * s_inv[r];
           } else {
             const float2 st = stats_n[q];
@@ -235,8 +246,10 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
         if (q < Q) {
           const int pos = pos0 + r, ri = pos / p.W, rj = pos - ri * p.W;
           const int qi = q / p.W, qj = q - qi * p.W;
-          const float l = pf_logit(An, p.a_pitch, q, qi, qj, ri, rj, hh, hw, p.mH, p.mW);
-          if (kStatsRow) {
+          const float l = pf_logit<kDense>(An, p.a_pitch, q, qi, qj, pos, ri, rj, hh, hw, p.mH, p.mW);
+          if (!kSoftmax) {
+            pv = l;
+          } else if (kStatsRow) {
             pv = __expf(l - s_m[r]) * s_inv[r];
           } else {
             const float2 st = stats_n[q];
@@ -289,20 +302,34 @@ psa_attend_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant
   }
 }
 
-template <bool kRowOwner, bool kStatsRow>
+template <bool kRowOwner, bool kStatsRow, bool kDense, bool kSoftmax>
 static int launch_attend(const CUtensorMap& tmB, const CUtensorMap& tmB_lo, const PsaFusedParams& p, int grid,
                          cudaStream_t stream) {
   static std::atomic<bool> attr_set[64];
+  const auto kernel = psa_attend_kernel<kRowOwner, kStatsRow, kDense, kSoftmax>;
   int dev = 0;
   SB_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-    SB_CUDA(cudaFuncSetAttribute(psa_attend_kernel<kRowOwner, kStatsRow>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kPfSmem));
+    SB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPfSmem));
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
-  psa_attend_kernel<kRowOwner, kStatsRow><<<grid, kPfThreads, kPfSmem, stream>>>(tmB, tmB_lo, p);
+  kernel<<<grid, kPfThreads, kPfSmem, stream>>>(tmB, tmB_lo, p);
   SB_LAUNCHED();
   return SEMSEG_OK;
+}
+
+// (row owner, stats on row): forward collect (1,1), forward distribute (0,1), dfeat collect (0,0), dfeat distribute (1,0).
+// Without softmax there are no statistics, so only the owner side differs between the four.
+template <bool kDense, bool kSoftmax>
+static int launch_attend_form(int mode, int psa_type, const CUtensorMap& tmB, const CUtensorMap& tmB_lo,
+                              const PsaFusedParams& p, int grid, cudaStream_t stream) {
+  if (!kSoftmax)
+    return (mode == 0) == (psa_type == 0) ? launch_attend<true, false, kDense, false>(tmB, tmB_lo, p, grid, stream)
+                                          : launch_attend<false, false, kDense, false>(tmB, tmB_lo, p, grid, stream);
+  if (mode == 0) return psa_type == 0 ? launch_attend<true, true, kDense, true>(tmB, tmB_lo, p, grid, stream)
+                                      : launch_attend<false, true, kDense, true>(tmB, tmB_lo, p, grid, stream);
+  return psa_type == 0 ? launch_attend<false, false, kDense, true>(tmB, tmB_lo, p, grid, stream)
+                       : launch_attend<true, false, kDense, true>(tmB, tmB_lo, p, grid, stream);
 }
 
 // Pixel positions per CTA tile: `max_rows`, fewer when that leaves SMs idle (`blocks_per_tile` CTAs share a tile).
@@ -314,16 +341,40 @@ static int psa_tile_rows(int N, int Q, int max_rows, int blocks_per_tile) {
 
 }  // namespace sb
 
+namespace sb {
+
+// form bits of the _ex entry points: the mask form and the softmax switch shared by the forward and backward checks
+static int check_psa_form(const char* fn, int form, int H, int W, int mH, int mW, int a_pitch, bool has_stats) {
+  SB_CHECK_ARG((form & ~(SEMSEG_PSA_DENSE | SEMSEG_PSA_NO_SOFTMAX)) == 0, "%s: unknown form bits 0x%x", fn, form);
+  if (form & SEMSEG_PSA_DENSE)
+    SB_CHECK_ARG(mH > 0 && mW > 0 && mH * mW == H * W && a_pitch >= H * W,
+                 "%s: bad mask geometry: the dense form needs mH*mW == H*W (%d x %d for %d x %d) and a_pitch >= H*W", fn,
+                 mH, mW, H, W);
+  else
+    SB_CHECK_ARG(mH > 0 && mW > 0 && (mH & 1) && (mW & 1) && a_pitch >= mH * mW, "%s: bad mask geometry", fn);
+  SB_CHECK_ARG(has_stats || (form & SEMSEG_PSA_NO_SOFTMAX), "%s: stats are required with softmax", fn);
+  return SEMSEG_OK;
+}
+
+}  // namespace sb
+
 // mode 0: out = P * feat (forward; writes stats)      mode 1: dfeat = P^T * dout (backward; reads stats)
 extern "C" int semseg_psa_attend(int mode, int psa_type, const float* attn, int a_pitch, const void* feat,
                                  const void* feat_lo, int feat_pitch, float* stats, void* out, void* out_lo, int out_pitch,
                                  int N, int H, int W, int mH, int mW, int C, float scale, void* stream_) {
+  return semseg_psa_attend_ex(mode, psa_type, 0, attn, a_pitch, feat, feat_lo, feat_pitch, stats, out, out_lo, out_pitch,
+                              N, H, W, mH, mW, C, scale, stream_);
+}
+
+extern "C" int semseg_psa_attend_ex(int mode, int psa_type, int form, const float* attn, int a_pitch, const void* feat,
+                                    const void* feat_lo, int feat_pitch, float* stats, void* out, void* out_lo,
+                                    int out_pitch, int N, int H, int W, int mH, int mW, int C, float scale, void* stream_) {
   using namespace sb;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(attn && feat && stats && out && N > 0 && H > 0 && W > 0, "psa_attend: bad args");
+  SB_CHECK_ARG(attn && feat && out && N > 0 && H > 0 && W > 0, "psa_attend: bad args");
   SB_CHECK_ARG(mode == 0 || mode == 1, "psa_attend: mode must be 0 (forward) or 1 (feature gradient)");
   SB_CHECK_ARG(psa_type == 0 || psa_type == 1, "psa_attend: psa_type must be 0 (collect) or 1 (distribute)");
-  SB_CHECK_ARG(mH > 0 && mW > 0 && (mH & 1) && (mW & 1) && a_pitch >= mH * mW, "psa_attend: bad mask geometry");
+  if (const int r = check_psa_form("psa_attend", form, H, W, mH, mW, a_pitch, stats != nullptr)) return r;
   SB_CHECK_ARG(C == kPfC, "psa_attend: feature width must be %d (got %d)", kPfC, C);
   SB_CHECK_ARG(W <= 128, "psa_attend: feature maps wider than %d are not supported", 128);
   SB_CHECK_ARG(feat_pitch % 8 == 0 && out_pitch % 8 == 0 && feat_pitch >= C && out_pitch >= C, "psa_attend: bad pitch");
@@ -350,11 +401,12 @@ extern "C" int semseg_psa_attend(int mode, int psa_type, const float* attn, int 
     if (feat_lo && (r = encode_tmap_bf16(&tmB_lo, feat_lo, 3, dims, str, box))) return r;
   }
   const int grid = N * p.tiles_per_img;
-  // (row owner, stats on row): forward collect (1,1), forward distribute (0,1), dfeat collect (0,0), dfeat distribute (1,0)
-  if (mode == 0) return psa_type == 0 ? launch_attend<true, true>(tmB, tmB_lo, p, grid, stream)
-                                      : launch_attend<false, true>(tmB, tmB_lo, p, grid, stream);
-  return psa_type == 0 ? launch_attend<false, false>(tmB, tmB_lo, p, grid, stream)
-                       : launch_attend<true, false>(tmB, tmB_lo, p, grid, stream);
+  switch (form) {
+    case 0: return launch_attend_form<false, true>(mode, psa_type, tmB, tmB_lo, p, grid, stream);
+    case SEMSEG_PSA_DENSE: return launch_attend_form<true, true>(mode, psa_type, tmB, tmB_lo, p, grid, stream);
+    case SEMSEG_PSA_NO_SOFTMAX: return launch_attend_form<false, false>(mode, psa_type, tmB, tmB_lo, p, grid, stream);
+    default: return launch_attend_form<true, false>(mode, psa_type, tmB, tmB_lo, p, grid, stream);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -364,6 +416,8 @@ extern "C" int semseg_psa_attend(int mode, int psa_type, const float* attn, int 
 //   dL[t, s] = P[t, s] * (dP[t, s] - D[t])             P recomputed from the logits and the saved (max, 1/sum)
 //   dA[owner][idx(other - owner)] = dL[t, s]           owner = t (collect) or s (distribute); dA is zero elsewhere (caller
 //                                                      zero-fills it: 74 % of a full 59x59 mask never receives gradient)
+// Dense form: dA[owner][other] = dL[t, s], every entry is written. Without softmax: dL[t, s] = dP[t, s], so D, out and the
+// statistics are not read.
 // CTA = <= 128 consecutive target positions x one block of 256 sources; warpgroup 0 = TMA producer, warpgroup 1 + w
 // computes targets [64w, 64w + 64) with wgmma into registers; operands K-major from TMA ([64 c, 128 rows] of dout,
 // [64 c, 256 rows] of feat), 4-stage ring.
@@ -391,7 +445,7 @@ struct PsaGradParams {
   float scale;
 };
 
-template <bool kCollect>
+template <bool kCollect, bool kDense, bool kSoftmax>
 __global__ void __launch_bounds__(kPgThreads, 1)
 psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDO_lo,
                      const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmF_lo,
@@ -463,7 +517,7 @@ psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_cons
     float d = 0.f;
     rm[i] = 0.f;
     rinv[i] = 0.f;
-    if (r_ok[i]) {
+    if (kSoftmax && r_ok[i]) {
       const long long o1 = (static_cast<long long>(n) * Q + tpos[i]) * p.dout_pitch;
       const long long o2 = (static_cast<long long>(n) * Q + tpos[i]) * p.out_pitch;
       const int cpl = p.C / 4;
@@ -483,8 +537,10 @@ psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_cons
       rm[i] = st.x;
       rinv[i] = st.y;
     }
-    d += __shfl_xor_sync(0xffffffffu, d, 1);
-    d += __shfl_xor_sync(0xffffffffu, d, 2);
+    if (kSoftmax) {
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+    }
     D[i] = d;
   }
 
@@ -528,30 +584,43 @@ psa_attn_grad_kernel(const __grid_constant__ CUtensorMap tmDO, const __grid_cons
         // owner / other of the attention entry
         const int oi = kCollect ? ti : si, oj = kCollect ? tj : sj, own = kCollect ? tp : s;
         const int a = (kCollect ? si : ti) - oi + hh, b = (kCollect ? sj : tj) - oj + hw;
-        if (a >= 0 && a < p.mH && b >= 0 && b < p.mW) {
-          const size_t off = static_cast<size_t>(own) * p.a_pitch + a * p.mW + b;
-          const float pv = __expf(__ldg(An + off) - rm[i]) * rinv[i];
-          dAn[off] = pv * (p.scale * acc[4 * j + 2 * i + e] - D[i]);
+        if (kDense || (a >= 0 && a < p.mH && b >= 0 && b < p.mW)) {
+          const size_t off = kDense ? static_cast<size_t>(own) * p.a_pitch + (kCollect ? s : tp)
+                                    : static_cast<size_t>(own) * p.a_pitch + a * p.mW + b;
+          if (kSoftmax) {
+            const float pv = __expf(__ldg(An + off) - rm[i]) * rinv[i];
+            dAn[off] = pv * (p.scale * acc[4 * j + 2 * i + e] - D[i]);
+          } else {
+            dAn[off] = p.scale * acc[4 * j + 2 * i + e];
+          }
         }
       }
     }
   }
 }
 
-template <bool kCollect>
+template <bool kCollect, bool kDense, bool kSoftmax>
 static int launch_attn_grad(const CUtensorMap& a, const CUtensorMap& al, const CUtensorMap& b, const CUtensorMap& bl,
                             const PsaGradParams& p, int grid, cudaStream_t stream) {
   static std::atomic<bool> attr_set[64];
+  const auto kernel = psa_attn_grad_kernel<kCollect, kDense, kSoftmax>;
   int dev = 0;
   SB_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-    SB_CUDA(cudaFuncSetAttribute(psa_attn_grad_kernel<kCollect>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPgSmem));
+    SB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPgSmem));
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
   const dim3 g(grid, cdiv(p.H * p.W, kPgBlockN));
-  psa_attn_grad_kernel<kCollect><<<g, kPgThreads, kPgSmem, stream>>>(a, al, b, bl, p);
+  kernel<<<g, kPgThreads, kPgSmem, stream>>>(a, al, b, bl, p);
   SB_LAUNCHED();
   return SEMSEG_OK;
+}
+
+template <bool kDense, bool kSoftmax>
+static int launch_attn_grad_form(int psa_type, const CUtensorMap& a, const CUtensorMap& al, const CUtensorMap& b,
+                                 const CUtensorMap& bl, const PsaGradParams& p, int grid, cudaStream_t stream) {
+  return psa_type == 0 ? launch_attn_grad<true, kDense, kSoftmax>(a, al, b, bl, p, grid, stream)
+                       : launch_attn_grad<false, kDense, kSoftmax>(a, al, b, bl, p, grid, stream);
 }
 
 }  // namespace sb
@@ -561,15 +630,26 @@ extern "C" int semseg_psa_attend_bwd_attn(int psa_type, const float* attn, int a
                                           const void* out_lo, int out_pitch, const void* dout, const void* dout_lo,
                                           int dout_pitch, float* dattn, int N, int H, int W, int mH, int mW, int C,
                                           float scale, void* stream_) {
+  return semseg_psa_attend_bwd_attn_ex(psa_type, 0, attn, a_pitch, stats, feat, feat_lo, feat_pitch, out, out_lo,
+                                       out_pitch, dout, dout_lo, dout_pitch, dattn, N, H, W, mH, mW, C, scale, stream_);
+}
+
+extern "C" int semseg_psa_attend_bwd_attn_ex(int psa_type, int form, const float* attn, int a_pitch, const float* stats,
+                                             const void* feat, const void* feat_lo, int feat_pitch, const void* out,
+                                             const void* out_lo, int out_pitch, const void* dout, const void* dout_lo,
+                                             int dout_pitch, float* dattn, int N, int H, int W, int mH, int mW, int C,
+                                             float scale, void* stream_) {
   using namespace sb;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(attn && stats && feat && out && dout && dattn && N > 0 && H > 0 && W > 0, "psa_attend_bwd_attn: bad args");
+  const bool softmax = !(form & SEMSEG_PSA_NO_SOFTMAX);
+  SB_CHECK_ARG(attn && feat && dout && dattn && N > 0 && H > 0 && W > 0, "psa_attend_bwd_attn: bad args");
   SB_CHECK_ARG(psa_type == 0 || psa_type == 1, "psa_attend_bwd_attn: psa_type must be 0 or 1");
-  SB_CHECK_ARG(mH > 0 && mW > 0 && (mH & 1) && (mW & 1) && a_pitch >= mH * mW, "psa_attend_bwd_attn: bad mask geometry");
+  if (const int r = check_psa_form("psa_attend_bwd_attn", form, H, W, mH, mW, a_pitch, stats != nullptr)) return r;
+  SB_CHECK_ARG(out || !softmax, "psa_attend_bwd_attn: out is required with softmax");
   SB_CHECK_ARG(C > 0 && C % 64 == 0 && W <= 128, "psa_attend_bwd_attn: C %% 64 == 0 and W <= 128 required");
   SB_CHECK_ARG(feat_pitch % 8 == 0 && out_pitch % 8 == 0 && dout_pitch % 8 == 0, "psa_attend_bwd_attn: bad pitch");
   const bool split = feat_lo != nullptr;
-  SB_CHECK_ARG((out_lo != nullptr) == split && (dout_lo != nullptr) == split,
+  SB_CHECK_ARG(((out_lo != nullptr) == split || (!softmax && !out)) && (dout_lo != nullptr) == split,
                "psa_attend_bwd_attn: all activations must use the same storage form");
   PsaGradParams p;
   memset(&p, 0, sizeof(p));
@@ -582,8 +662,10 @@ extern "C" int semseg_psa_attend_bwd_attn(int psa_type, const float* attn, int a
   p.tiles_per_img = cdiv(H * W, p.tile_rows);
   p.nseg = split ? 3 : 1;
   p.scale = scale;
-  // the caller's dattn must be zero where no gradient lands
-  SB_CUDA(cudaMemsetAsync(dattn, 0, sizeof(float) * static_cast<size_t>(N) * H * W * a_pitch, stream));
+  // the caller's dattn must be zero where no gradient lands: outside the mask windows, and in the dense form the padding
+  // columns of a pitch wider than H*W
+  if (!(form & SEMSEG_PSA_DENSE) || a_pitch != H * W)
+    SB_CUDA(cudaMemsetAsync(dattn, 0, sizeof(float) * static_cast<size_t>(N) * H * W * a_pitch, stream));
   CUtensorMap tmDO, tmDO_lo, tmF, tmF_lo;
   {
     uint64_t dims[3] = {(uint64_t)C, (uint64_t)H * W, (uint64_t)N};
@@ -604,6 +686,11 @@ extern "C" int semseg_psa_attend_bwd_attn(int psa_type, const float* attn, int a
     if (split && (r = encode_tmap_bf16(&tmF_lo, feat_lo, 3, dims, str, box))) return r;
   }
   const int grid = N * p.tiles_per_img;
-  return psa_type == 0 ? launch_attn_grad<true>(tmDO, tmDO_lo, tmF, tmF_lo, p, grid, stream)
-                       : launch_attn_grad<false>(tmDO, tmDO_lo, tmF, tmF_lo, p, grid, stream);
+  switch (form) {
+    case 0: return launch_attn_grad_form<false, true>(psa_type, tmDO, tmDO_lo, tmF, tmF_lo, p, grid, stream);
+    case SEMSEG_PSA_DENSE: return launch_attn_grad_form<true, true>(psa_type, tmDO, tmDO_lo, tmF, tmF_lo, p, grid, stream);
+    case SEMSEG_PSA_NO_SOFTMAX:
+      return launch_attn_grad_form<false, false>(psa_type, tmDO, tmDO_lo, tmF, tmF_lo, p, grid, stream);
+    default: return launch_attn_grad_form<true, false>(psa_type, tmDO, tmDO_lo, tmF, tmF_lo, p, grid, stream);
+  }
 }

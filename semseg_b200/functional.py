@@ -585,38 +585,50 @@ def ppm_link():
 
 # ------------------------------------------------------------------------------------------------ fused PSA attention
 class _PSAAttend(torch.autograd.Function):
-    """psa_mask -> softmax over the source positions -> aggregation bmm -> 1/normalization_factor (model/psanet.py:81-91)
-    as one kernel each way; nothing [HW x HW] is written to HBM (the backward recomputes the probabilities from the
-    logits and the saved per-target (max, 1/sum))."""
+    """psa_mask (or the compact mode's dense view) -> softmax over the source positions (or none) -> aggregation bmm ->
+    1/normalization_factor (model/psanet.py:76-91) as one kernel each way; nothing [HW x HW] is written to HBM (with
+    softmax the backward recomputes the probabilities from the logits and the saved per-target (max, 1/sum); without it
+    the probabilities are the logits, and neither the statistics nor the output are kept)."""
 
     @staticmethod
-    def forward(ctx, attn, feat, psa_type, mask_h, mask_w, scale):
-        out, stats = ops.psa_attend(attn, feat, psa_type, mask_h, mask_w, scale)
-        ctx.save_for_backward(attn, feat, out, stats)
-        ctx.cfg = (psa_type, mask_h, mask_w, scale)
+    def forward(ctx, attn, feat, psa_type, mask_h, mask_w, scale, compact, softmax):
+        out, stats = ops.psa_attend(attn, feat, psa_type, mask_h, mask_w, scale, compact=compact, softmax=softmax)
+        if softmax:
+            ctx.save_for_backward(attn, feat, out, stats)
+        else:
+            ctx.save_for_backward(attn, feat)
+        ctx.cfg = (psa_type, mask_h, mask_w, scale, compact, softmax)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        attn, feat, out, stats = ctx.saved_tensors
-        psa_type, mask_h, mask_w, scale = ctx.cfg
+        psa_type, mask_h, mask_w, scale, compact, softmax = ctx.cfg
+        attn, feat, out, stats = ctx.saved_tensors + (None, None) * (not softmax)
         if not dout.is_contiguous():
             dout = dout.contiguous()
+        form = dict(compact=compact, softmax=softmax)
         dattn = dfeat = None
         if ctx.needs_input_grad[1]:
-            dfeat, _ = ops.psa_attend(attn, dout, psa_type, mask_h, mask_w, scale, stats=stats, mode=1)
+            dfeat, _ = ops.psa_attend(attn, dout, psa_type, mask_h, mask_w, scale, stats=stats, mode=1, **form)
         if ctx.needs_input_grad[0]:
-            dattn = ops.psa_attend_bwd_attn(attn, stats, feat, out, dout, psa_type, mask_h, mask_w, scale)
-        return dattn, dfeat, None, None, None, None
+            dattn = ops.psa_attend_bwd_attn(attn, stats, feat, out, dout, psa_type, mask_h, mask_w, scale, **form)
+        return dattn, dfeat, None, None, None, None, None, None
 
 
-def psa_attend(attn, feat, psa_type, mask_h, mask_w, scale):
-    """attn fp32 NHWC [N,h,w,mask_h*mask_w], feat NHWC activation [N,h,w,512] -> aggregated features [N,h,w,512]."""
-    return _PSAAttend.apply(attn.contiguous(), feat, psa_type, mask_h, mask_w, scale)
+def psa_attend(attn, feat, psa_type, mask_h, mask_w, scale, compact=False, softmax=True):
+    """attn fp32 NHWC [N,h,w,mask_h*mask_w], feat NHWC activation [N,h,w,512] -> aggregated features [N,h,w,512].
+    compact: the dense form of the reference's compact mode (mask_h*mask_w == h*w); softmax: its psa_softmax."""
+    return _PSAAttend.apply(attn.contiguous(), feat, psa_type, mask_h, mask_w, scale, compact, softmax)
 
 
-def psa_attend_supported(feat, mask_h, mask_w):
-    return feat.shape[-1] == 512 and feat.shape[-2] <= 128 and mask_h % 2 == 1 and mask_w % 2 == 1
+def psa_attend_supported(feat, mask_h, mask_w, compact=False):
+    """Whether the fused kernels cover this geometry: 512 channels, at most 128 columns, and odd masks (window form) or a
+    mask of exactly h*w entries (compact mode's dense form)."""
+    if feat.shape[-1] != 512 or feat.shape[-2] > 128:
+        return False
+    if compact:
+        return mask_h * mask_w == feat.shape[-3] * feat.shape[-2]
+    return mask_h % 2 == 1 and mask_w % 2 == 1
 
 
 # ------------------------------------------------------------------------------------------------ bilinear resize

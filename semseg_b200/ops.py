@@ -113,35 +113,43 @@ def psamask_bwd(grad_out, psa_type, mask_h, mask_w):
 
 
 # ------------------------------------------------------------------------------------------------ fused PSA attention
-def psa_attend(attn, feat, psa_type, mask_h, mask_w, scale, stats=None, mode=0):
+def _psa_form(compact, softmax):
+    return (_lib.PSA_DENSE if compact else 0) | (0 if softmax else _lib.PSA_NO_SOFTMAX)
+
+
+def psa_attend(attn, feat, psa_type, mask_h, mask_w, scale, stats=None, mode=0, compact=False, softmax=True):
     """mode 0: (out, stats) = fused mask-gather -> softmax -> aggregation (model/psanet.py:81-91) of the fp32 NHWC logits
     `attn` [N,h,w,>=mask_h*mask_w] and the NHWC activation `feat` [N,h,w,512]; mode 1: the feature gradient (pass dout as
-    `feat` and the forward's `stats`)."""
+    `feat` and the forward's `stats`). compact: the dense mask form (mask_h*mask_w == h*w, model/psanet.py:76-79);
+    softmax=False: P = the gathered logits, and stats is None."""
     _require_cuda(attn, feat)
     lib = _lib.load()
     assert attn.dtype == torch.float32 and attn.dim() == 4 and attn.is_contiguous()
     n, h, w, c, fp = _nhwc_meta(feat)
     assert tuple(attn.shape[:3]) == (n, h, w) and attn.shape[3] >= mask_h * mask_w
     out = empty_act((n, h, w, c), is_split(feat), feat.device)
-    if stats is None:
+    if stats is None and softmax:
         assert mode == 0
         stats = torch.empty((n, h * w, 2), dtype=torch.float32, device=feat.device)
-    _lib.check(lib.semseg_psa_attend(mode, psa_type, _ptr(attn), attn.shape[3], _ptr(feat), _lo(feat), fp, _ptr(stats),
-                                     _ptr(out), _lo(out), c, n, h, w, mask_h, mask_w, c, float(scale), _stream()),
+    _lib.check(lib.semseg_psa_attend_ex(mode, psa_type, _psa_form(compact, softmax), _ptr(attn), attn.shape[3], _ptr(feat),
+                                        _lo(feat), fp, _ptr(stats), _ptr(out), _lo(out), c, n, h, w, mask_h, mask_w, c,
+                                        float(scale), _stream()),
                "semseg_psa_attend")
     return out, stats
 
 
-def psa_attend_bwd_attn(attn, stats, feat, out, dout, psa_type, mask_h, mask_w, scale):
-    """Gradient of psa_attend w.r.t. the attention logits (same shape as attn, zero outside the mask windows)."""
+def psa_attend_bwd_attn(attn, stats, feat, out, dout, psa_type, mask_h, mask_w, scale, compact=False, softmax=True):
+    """Gradient of psa_attend w.r.t. the attention logits (same shape as attn, zero outside the mask windows). Without
+    softmax, stats and out are not read and may be None."""
     lib = _lib.load()
     n, h, w, c, fp = _nhwc_meta(feat)
-    op, dp = _nhwc_meta(out)[4], _nhwc_meta(dout)[4]
+    op, dp = (_nhwc_meta(out)[4] if out is not None else c), _nhwc_meta(dout)[4]
     _same_form(feat, out, dout)
     dattn = torch.empty_like(attn)
-    _lib.check(lib.semseg_psa_attend_bwd_attn(psa_type, _ptr(attn), attn.shape[3], _ptr(stats), _ptr(feat), _lo(feat), fp,
-                                              _ptr(out), _lo(out), op, _ptr(dout), _lo(dout), dp, _ptr(dattn), n, h, w,
-                                              mask_h, mask_w, c, float(scale), _stream()),
+    _lib.check(lib.semseg_psa_attend_bwd_attn_ex(psa_type, _psa_form(compact, softmax), _ptr(attn), attn.shape[3],
+                                                 _ptr(stats), _ptr(feat), _lo(feat), fp, _ptr(out), _lo(out), op,
+                                                 _ptr(dout), _lo(dout), dp, _ptr(dattn), n, h, w, mask_h, mask_w, c,
+                                                 float(scale), _stream()),
                "semseg_psa_attend_bwd_attn")
     return dattn
 

@@ -79,11 +79,14 @@ class PSA(nn.Module):
         t, t_agg = SF.fork(t, 2)                              # t feeds the attention convs and the aggregation
         a = SF.conv_bn_act(t, attention[0], attention[1], relu=True)
         y = SF.conv_bias_f32(a, attention[3])                 # fp32 NHWC [n,h,w,mask_h*mask_w]
-        if (self.psa_softmax and not self.compact and SF.psa_attend_supported(t_agg, self.mask_h, self.mask_w)
+        if (SF.psa_attend_supported(t_agg, self.mask_h, self.mask_w, self.compact)
                 and os.environ.get("SEMSEG_B200_PSA_FUSED", "1") != "0"):
-            # one kernel: mask gather -> softmax over the h*w source positions -> aggregation -> 1/normalization_factor
-            # (model/psanet.py:81-91); the [n, hw, hw] attention map is never written to HBM
-            return SF.psa_attend(y, t_agg, mask_type, self.mask_h, self.mask_w, 1.0 / self.normalization_factor), (h, w)
+            # one kernel: mask gather (compact: the dense view) -> softmax over the h*w source positions (unless
+            # psa_softmax is off) -> aggregation -> 1/normalization_factor (model/psanet.py:76-91); the [n, hw, hw]
+            # attention map is never written to HBM. A compact mask that does not match the feature map falls through to
+            # the composition below, which rejects it as the reference does.
+            return SF.psa_attend(y, t_agg, mask_type, self.mask_h, self.mask_w, 1.0 / self.normalization_factor,
+                                 self.compact, self.psa_softmax), (h, w)
         y = y.permute(0, 3, 1, 2).contiguous()                # NCHW fp32, the layout psa_mask is defined on
         if self.compact:
             if mask_type == 1:
