@@ -231,6 +231,17 @@ int semseg_nhwc_f32_to_nchw_f32(const float* in, float* out, int N, int C, int H
  *   out is [N, (H-1)/2+1, (W-1)/2+1, 32] bf16. x is NHWC bf16 with x_pitch >= 4 (the first Cin channels are read). */
 int semseg_im2col3x3s2(const void* x, int x_pitch, int N, int H, int W, int Cin, void* out, void* stream);
 
+/* Input gradient of that stem conv (the adjoint of semseg_im2col3x3s2 + the patch-slab product), fp32 NCHW:
+ *   dx[n, c, y, x] = sum_{(r, s, ho, wo): 2ho-1+r = y, 2wo-1+s = x} sum_k dy[n, ho, wo, k] * w[k, c, r, s]
+ * dy     : bf16 NHWC [N, Ho, Wo, >= Cout] with dy_pitch (a multiple of 8, 16-byte aligned); dy_lo its lo plane in
+ *          bf16x3 (same pitch), else NULL
+ * wp     : the patch slab bf16 [Cout][32], column (r*3+s)*Cin + c = w[:, c, r, s]; with wp_split = 1 its lo slab follows
+ *          (required exactly when dy_lo is given: the three products hi*hi + lo*hi + hi*lo)
+ * dx_nchw: fp32 [N, Cin, H, W], every element written; Ho = (H-1)/2+1, Wo = (W-1)/2+1, 1 <= Cin <= 3, Cout = 64.
+ * Deterministic: fp32 accumulation in a fixed order, no atomics. */
+int semseg_stem_dgrad3x3s2(const void* dy, const void* dy_lo, int dy_pitch, int N, int Ho, int Wo, int H, int W, int Cin,
+                           int Cout, const void* wp, int wp_split, float* dx_nchw, void* stream);
+
 /* 2x2 phase decomposition used to run stride-2 convolutions (model/resnet.py:108 conv1, layer2.0 conv2 and
  * downsample) on the stride-1 tensor-core kernel:
  *   xp [4][N][Hh][Wh][C], Hh = (H+1)/2:  xp[ph*2+pw][n][i][j] = x[n][2i+ph][2j+pw] (zero outside x). */

@@ -116,6 +116,8 @@ SIGNATURES = {
     "semseg_sgd_multi": (c_int, [c_vp, c_vp, c_int, c_int, ctypes.POINTER(SgdHyper), c_vp]),
     "semseg_iou_hist": (c_int, [c_vp, c_vp, ctypes.c_longlong, c_int, ctypes.c_longlong, c_int, c_vp, c_vp]),
     "semseg_im2col3x3s2": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
+    "semseg_stem_dgrad3x3s2": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int,
+                                       c_vp, c_vp]),
     "semseg_nchw_f32_to_nhwc_bf16": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "semseg_nhwc_bf16_to_nchw_f32": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "semseg_nhwc_f32_to_nchw_f32": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),

@@ -164,6 +164,115 @@ __global__ void __launch_bounds__(256) im2col3x3s2_kernel(const __nv_bfloat16* _
   }
 }
 
+// Input gradient of the stem conv (the adjoint of im2col3x3s2 + the patch-slab product), written as fp32 NCHW:
+//   dx[n, c, y, x] = sum over (r, s, ho, wo) with 2ho-1+r = y, 2wo-1+s = x of  sum_k dy[n, ho, wo, k] * w[k, c, r, s]
+// A thread owns the 2x2 input pixels (2i..2i+1, 2j..2j+1), which only the four conv-output pixels (i..i+1, j..j+1)
+// reach, each through its own taps:
+//   dy(i, j)    : (2i, 2j) tap 4, (2i, 2j+1) tap 5, (2i+1, 2j) tap 7, (2i+1, 2j+1) tap 8
+//   dy(i, j+1)  : (2i, 2j+1) tap 3, (2i+1, 2j+1) tap 6
+//   dy(i+1, j)  : (2i+1, 2j) tap 1, (2i+1, 2j+1) tap 2
+//   dy(i+1, j+1): (2i+1, 2j+1) tap 0
+// so all 9 taps are used once per k. The weights w[k][tap][c] (fp32 copies of the bf16 slab values, lo slab behind) sit
+// in shared memory as one float4 per (k, tap) and are read warp-uniformly (broadcast). bf16x3 sums the conv kernels'
+// three products hi*hi + lo*hi + hi*lo. Each output is one fp32 chain in a fixed order (k ascending, then the dy pixel,
+// then the product): deterministic, no atomics.
+constexpr int kStemCout = 64;
+
+template <int CIN, bool SPLIT>
+__global__ void __launch_bounds__(256) stem_dgrad3x3s2_kernel(const __nv_bfloat16* __restrict__ dy,
+                                                              const __nv_bfloat16* __restrict__ dy_lo, int pitch, int N,
+                                                              int H, int W, int Ho, int Wo,
+                                                              const __nv_bfloat16* __restrict__ wp,
+                                                              float* __restrict__ dx) {
+  __shared__ float4 ws[SPLIT ? 2 : 1][kStemCout * 9];
+  for (int e = threadIdx.x; e < kStemCout * 9; e += blockDim.x) {
+    const int k = e / 9, t = e % 9;
+#pragma unroll
+    for (int part = 0; part < (SPLIT ? 2 : 1); ++part) {
+      const __nv_bfloat16* row = wp + static_cast<size_t>(part) * kStemCout * 32 + k * 32 + t * CIN;
+      float v[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+      for (int c = 0; c < CIN; ++c) v[c] = __bfloat162float(row[c]);
+      ws[part][e] = make_float4(v[0], v[1], v[2], 0.f);
+    }
+  }
+  __syncthreads();
+  const size_t plane = static_cast<size_t>(H) * W;
+  const long long total = static_cast<long long>(N) * Ho * Wo;
+  for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int j = static_cast<int>(idx % Wo);
+    const int i = static_cast<int>((idx / Wo) % Ho);
+    const int n = static_cast<int>(idx / (static_cast<long long>(Wo) * Ho));
+    // the four dy pixels (i, j), (i, j+1), (i+1, j), (i+1, j+1); those outside the conv output contribute zero
+    const bool ok[4] = {true, j + 1 < Wo, i + 1 < Ho, i + 1 < Ho && j + 1 < Wo};
+    size_t off[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      off[q] = ((static_cast<size_t>(n) * Ho + i + (q >> 1)) * Wo + j + (q & 1)) * pitch;
+    float acc[4][CIN];
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+#pragma unroll
+      for (int c = 0; c < CIN; ++c) acc[p][c] = 0.f;
+    for (int k0 = 0; k0 < kStemCout; k0 += 8) {
+      float dh[4][8], dl[4][8];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        uint4 hv = make_uint4(0, 0, 0, 0), lv = make_uint4(0, 0, 0, 0);
+        if (ok[q]) {
+          hv = __ldg(reinterpret_cast<const uint4*>(dy + off[q] + k0));
+          if (SPLIT) lv = __ldg(reinterpret_cast<const uint4*>(dy_lo + off[q] + k0));
+        }
+        const __nv_bfloat16* hb = reinterpret_cast<const __nv_bfloat16*>(&hv);
+        const __nv_bfloat16* lb = reinterpret_cast<const __nv_bfloat16*>(&lv);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          dh[q][e] = __bfloat162float(hb[e]);
+          dl[q][e] = SPLIT ? __bfloat162float(lb[e]) : 0.f;
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int k = k0 + e;
+        // (dy pixel q, output pixel p, tap t) in the order the chains are summed
+        constexpr int kq[9] = {0, 0, 0, 0, 1, 1, 2, 2, 3};
+        constexpr int kp[9] = {0, 1, 2, 3, 1, 3, 2, 3, 3};
+        constexpr int kt[9] = {4, 5, 7, 8, 3, 6, 1, 2, 0};
+#pragma unroll
+        for (int u = 0; u < 9; ++u) {
+          const float4 wh = ws[0][k * 9 + kt[u]];
+          const float whc[3] = {wh.x, wh.y, wh.z};
+          float wlc[3] = {0.f, 0.f, 0.f};
+          if (SPLIT) {
+            const float4 wl = ws[SPLIT ? 1 : 0][k * 9 + kt[u]];
+            wlc[0] = wl.x; wlc[1] = wl.y; wlc[2] = wl.z;
+          }
+#pragma unroll
+          for (int c = 0; c < CIN; ++c) {
+            float a = fmaf(dh[kq[u]][e], whc[c], acc[kp[u]][c]);
+            if (SPLIT) {
+              a = fmaf(dl[kq[u]][e], whc[c], a);
+              a = fmaf(dh[kq[u]][e], wlc[c], a);
+            }
+            acc[kp[u]][c] = a;
+          }
+        }
+      }
+    }
+    const int y0 = 2 * i, x0 = 2 * j;
+#pragma unroll
+    for (int c = 0; c < CIN; ++c) {
+      float* base = dx + (static_cast<size_t>(n) * CIN + c) * plane;
+#pragma unroll
+      for (int p = 0; p < 4; ++p) {
+        const int y = y0 + (p >> 1), x = x0 + (p & 1);
+        if (y < H && x < W) base[static_cast<size_t>(y) * W + x] = acc[p][c];
+      }
+    }
+  }
+}
+
 // Stride-2 convolutions run on the stride-1 tensor-core kernel through a 2x2 phase decomposition:
 //   xp[(ph*2+pw)*N + n][i][j][c] = x[n][2i+ph][2j+pw][c]   (zero where 2i+ph >= H or 2j+pw >= W)
 // so tap (r, s) of a stride-2 conv reads phase ((r+1)&1, (s+1)&1) at a shift of -1 or 0.
@@ -251,6 +360,41 @@ extern "C" int semseg_im2col3x3s2(const void* x, int x_pitch, int N, int H, int 
   if (blocks > 148 * 16) blocks = 148 * 16;
   sb::im2col3x3s2_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(static_cast<const bf16*>(x), x_pitch, N, H, W,
                                                                            Cin, Ho, Wo, static_cast<bf16*>(out));
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" int semseg_stem_dgrad3x3s2(const void* dy, const void* dy_lo, int dy_pitch, int N, int Ho, int Wo, int H,
+                                      int W, int Cin, int Cout, const void* wp, int wp_split, float* dx_nchw,
+                                      void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SB_CHECK_ARG(dy && wp && dx_nchw, "stem_dgrad3x3s2: null pointer (dy, wp and dx are required)");
+  SB_CHECK_ARG(Cin >= 1 && Cin <= 3, "stem_dgrad3x3s2: needs 1..3 input channels (got Cin=%d)", Cin);
+  SB_CHECK_ARG(Cout == kStemCout, "stem_dgrad3x3s2: needs Cout=%d (got %d)", kStemCout, Cout);
+  SB_CHECK_ARG(N > 0 && H > 0 && W > 0 && Ho == (H - 1) / 2 + 1 && Wo == (W - 1) / 2 + 1,
+               "stem_dgrad3x3s2: Ho=(H-1)/2+1 and Wo=(W-1)/2+1 required (got N=%d H=%d W=%d Ho=%d Wo=%d)", N, H, W, Ho,
+               Wo);
+  SB_CHECK_ARG(dy_pitch >= Cout && dy_pitch % 8 == 0,
+               "stem_dgrad3x3s2: dy pitch must be >= Cout and a multiple of 8 (got %d)", dy_pitch);
+  SB_CHECK_ARG(wp_split == 0 || wp_split == 1, "stem_dgrad3x3s2: wp_split must be 0 or 1 (got %d)", wp_split);
+  SB_CHECK_ARG((dy_lo != nullptr) == (wp_split == 1),
+               "stem_dgrad3x3s2: dy_lo and a split weight slab go together (bf16x3), got dy_lo=%s wp_split=%d",
+               dy_lo ? "set" : "null", wp_split);
+  SB_CHECK_ARG(reinterpret_cast<uintptr_t>(dy) % 16 == 0 && reinterpret_cast<uintptr_t>(dy_lo) % 16 == 0,
+               "stem_dgrad3x3s2: dy and dy_lo must be 16-byte aligned");
+  const long long total = static_cast<long long>(N) * Ho * Wo;
+  long long blocks = (total + 255) / 256;
+  if (blocks > 148 * 16) blocks = 148 * 16;
+  const dim3 grid(static_cast<unsigned>(blocks));
+  const bf16 *d = static_cast<const bf16*>(dy), *dl = static_cast<const bf16*>(dy_lo), *w = static_cast<const bf16*>(wp);
+#define SB_STEM_DGRAD(CIN, SPLIT) \
+  sb::stem_dgrad3x3s2_kernel<CIN, SPLIT><<<grid, 256, 0, stream>>>(d, dl, dy_pitch, N, H, W, Ho, Wo, w, dx_nchw)
+  if (wp_split) {
+    if (Cin == 1) SB_STEM_DGRAD(1, true); else if (Cin == 2) SB_STEM_DGRAD(2, true); else SB_STEM_DGRAD(3, true);
+  } else {
+    if (Cin == 1) SB_STEM_DGRAD(1, false); else if (Cin == 2) SB_STEM_DGRAD(2, false); else SB_STEM_DGRAD(3, false);
+  }
+#undef SB_STEM_DGRAD
   SB_LAUNCHED();
   return SEMSEG_OK;
 }

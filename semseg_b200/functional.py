@@ -99,36 +99,50 @@ _net = threading.local()
 
 
 @contextlib.contextmanager
-def network_mode(training):
-    """Runs the enclosed forward as part of a network in training mode (True) or not (False) on this thread."""
-    prev = getattr(_net, "training", False)
-    _net.training = bool(training)
+def network_mode(training, input_grad=True):
+    """Runs the enclosed forward as part of a network in training mode (True) or not (False) on this thread.
+    `input_grad`: whether the network's input needs a gradient (see _bn_mode)."""
+    prev = getattr(_net, "training", False), getattr(_net, "input_grad", True)
+    _net.training, _net.input_grad = bool(training), bool(input_grad)
     try:
         yield
     finally:
-        _net.training = prev
+        _net.training, _net.input_grad = prev
 
 
 def network_forward(fn):
-    """Decorator of a module's forward: the module is the network being run, in its own training mode."""
+    """Decorator of a module's forward(x, ...): the module is the network being run, in its own training mode."""
     @functools.wraps(fn)
     def forward(self, *args, **kwargs):
-        with network_mode(self.training):
+        x = args[0] if args else kwargs.get("x")
+        with network_mode(self.training, torch.is_tensor(x) and x.requires_grad):
             return fn(self, *args, **kwargs)
     return forward
 
 
-def _bn_mode(bn, *inputs):
-    """How a conv + `bn` stage runs, given the tensors its gradients would flow to (None entries allowed):
+def _needs_grad(ts):
+    return any(t is not None and t.requires_grad for t in ts)
+
+
+def _bn_mode(bn, acts, params=()):
+    """How a conv + `bn` stage runs, given the tensors its gradients would flow to (None entries allowed): its activation
+    inputs `acts` (x, the residual) and its parameters `params`:
       "batch"  : batch statistics (BN in training mode, or without running statistics), running statistics updated;
-      "frozen" : running statistics, differentiable — BN in eval mode, the network in training mode, autograd enabled,
-                 and some input needs a gradient;
-      "eval"   : the folded single kernel, detached (model.eval(), torch.no_grad(), or nothing needs a gradient)."""
+      "frozen" : running statistics, differentiable — BN in eval mode, autograd enabled, and either the network in
+                 training mode with some input or parameter needing a gradient, or the network in eval mode, its input
+                 needing a gradient and an activation input of the stage needing one (input gradients of an eval
+                 network: saliency, adversarial attacks);
+      "eval"   : the folded single kernel, detached (model.eval() on an input that needs no gradient — the reference's
+                 validate(), where activations may still need a gradient through a parameter such as PSA's attention
+                 conv — torch.no_grad(), or nothing needs a gradient)."""
     if bn.training or bn.running_mean is None:
         return "batch"
-    if (torch.is_grad_enabled() and getattr(_net, "training", False) and
-            any(t is not None and t.requires_grad for t in inputs)):
-        return "frozen"
+    if torch.is_grad_enabled():
+        if getattr(_net, "training", False):
+            if _needs_grad(acts) or _needs_grad(params):
+                return "frozen"
+        elif getattr(_net, "input_grad", True) and _needs_grad(acts):
+            return "frozen"
     return "eval"
 
 
@@ -201,15 +215,18 @@ class _ConvForm:
                  decomposition of the input (space_to_phases): tap (r, s) reads phase ((r+1)&1, (s+1)&1) shifted by
                  -1 or 0; dgrad is one small conv per phase, wgrad reads the phases.
       "patches": the 3-channel stride-2 stem conv on an input that needs no gradient: one 1x1 conv over 27-value input
-                 patches (ops.im2col3x3s2) instead of 9 taps of a 3(->64)-channel K block. No dgrad. Eval mode always
-                 takes the phase form: the patch form sums in another order, so its output bits differ."""
-    __slots__ = ("kind", "pw", "wf", "xin", "taps", "img_add", "out_nhw", "in_shape")
+                 patches (ops.im2col3x3s2) instead of 9 taps of a 3(->64)-channel K block. Eval mode always takes the
+                 phase form: the patch form sums in another order, so its output bits differ.
+    The stem conv's input gradient, whichever form ran forward, is one CUDA-core kernel over the patch slab
+    (ops.stem_dgrad3x3s2), written as fp32 NCHW."""
+    __slots__ = ("kind", "pw", "wf", "xin", "taps", "img_add", "out_nhw", "in_shape", "stem")
 
     def __init__(self, conv, x, input_needs_grad, mode):
         split = ops.is_split(x)
         self.pw = packed(conv, need_dgrad=mode != "eval", split=split)
         self.wf, self.img_add, self.out_nhw = self.pw.wf, None, None
         self.in_shape = tuple(x.shape[-4:])
+        self.stem = _is_patch_conv(conv) and conv.out_channels == 64
         n, h, w, _ = self.in_shape
         k = conv.kernel_size[0]
         if conv.stride[0] == 1:
@@ -228,14 +245,21 @@ class _ConvForm:
         return ops.conv_fprop(self.xin, self.wf, self.pw.cout, self.taps, img_add=self.img_add, out_nhw=self.out_nhw,
                               **kw)
 
-    def dgrad(self, d_raw, dx_add=None):
+    def dgrad(self, d_raw, dx_add=None, nchw=False):
         """Input gradient from the conv output's gradient `d_raw`. `dx_add` (same shape as dx) is summed into dx — in
         the dgrad epilogue (AFFINE mode with a residual operand) for the direct form: this is how gradient fan-in is
-        fused."""
-        if self.kind == "patches":
-            raise RuntimeError("semseg_b200: the patch form of the stem conv was chosen but dx is requested")
+        fused. nchw=True (stem conv only, no `dx_add`): the fp32 NCHW gradient of the module input, as the kernel
+        writes it."""
         pw = self.pw
-        n, h, w, _ = self.in_shape
+        n, h, w, c = self.in_shape
+        if self.stem:
+            dx = ops.stem_dgrad3x3s2(d_raw, pw.wp, pw.cin, h, w)
+            if nchw:
+                assert dx_add is None
+                return dx
+            dx = ops.f32_to_act(dx.permute(0, 2, 3, 1).contiguous(), ops.is_split(d_raw), pad_to=c)
+            return dx if dx_add is None else ops.add_act(dx, dx_add)
+        assert not nchw, "only the stem conv writes an NCHW input gradient"
         mirrored = [(-dh, -dw, wt) for dh, dw, wt in self.taps]       # taps of the transposed conv
         if self.kind == "direct":
             dx, _ = ops.conv_fprop(d_raw, pw.wd, pw.cin, mirrored, epi=EPI_RAW if dx_add is None else EPI_AFFINE,
@@ -301,9 +325,9 @@ def cba_forward(x, conv, bn, relu, residual, out=None, input_needs_grad=True, mo
     return y, st
 
 
-def cba_backward(st, dy, need_dx=True, need_dw=True, need_dres=False, dx_add=None):
+def cba_backward(st, dy, need_dx=True, need_dw=True, need_dres=False, dx_add=None, dx_nchw=False):
     """Backward of cba_forward: returns (dx, dw, dgamma, dbeta, dres). `dx_add` (same shape as dx) is summed into
-    dx (see _ConvForm.dgrad)."""
+    dx; dx_nchw: the stem conv's dx as fp32 NCHW (see _ConvForm.dgrad)."""
     bn = st.bn
     want_dres = st.has_res and need_dres
     if st.frozen:
@@ -318,17 +342,20 @@ def cba_backward(st, dy, need_dx=True, need_dw=True, need_dres=False, dx_add=Non
         dbeta = sums[0] if want_b else None
     else:
         d_raw, dres, dgamma, dbeta = _bn_backward(st.pg, dy, st.y, st.raw, st.mi, bn.weight, st.relu, want_dres, st.ss)
-    dx = st.form.dgrad(d_raw, dx_add) if need_dx else None
+    dx = st.form.dgrad(d_raw, dx_add, nchw=dx_nchw) if need_dx else None
     dw = st.form.wgrad(d_raw) if need_dw else None
     return dx, dw, dgamma, dbeta, dres
 
 
 class _ConvBnAct(torch.autograd.Function):
-    """Autograd wrapper of one cba_forward / cba_backward stage."""
+    """Autograd wrapper of one cba_forward / cba_backward stage. `x` is an activation, or — for the stem conv — the
+    module's fp32 NCHW input, converted here and given its gradient straight from the stem dgrad kernel."""
 
     @staticmethod
     def forward(ctx, x, weight, gamma, beta, residual, conv, bn, relu, out, frozen):
-        y, st = cba_forward(x, conv, bn, relu, residual, out, input_needs_grad=ctx.needs_input_grad[0],
+        ctx.nchw = x.dtype != torch.bfloat16
+        xa = ops.nchw_to_nhwc_bf16(x.contiguous().float(), split=precision.split_enabled()) if ctx.nchw else x
+        y, st = cba_forward(xa, conv, bn, relu, residual, out, input_needs_grad=ctx.needs_input_grad[0],
                             mode="frozen" if frozen else "batch")
         ctx.st = st
         if out is not None:
@@ -338,7 +365,8 @@ class _ConvBnAct(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         ni = ctx.needs_input_grad
-        dx, dw, dgamma, dbeta, dres = cba_backward(ctx.st, dy, need_dx=ni[0], need_dw=ni[1], need_dres=ni[4])
+        dx, dw, dgamma, dbeta, dres = cba_backward(ctx.st, dy, need_dx=ni[0], need_dw=ni[1], need_dres=ni[4],
+                                                   dx_nchw=ctx.nchw)
         ctx.st = None
         return dx, dw, dgamma, dbeta, dres, None, None, None, None, None
 
@@ -392,7 +420,7 @@ def bottleneck(x, blk):
               blk.conv3.weight, blk.bn3.weight, blk.bn3.bias]
     if blk.downsample is not None:
         params += [blk.downsample[0].weight, blk.downsample[1].weight, blk.downsample[1].bias]
-    modes = [_bn_mode(b, x, *params) for b in bns]     # one autograd node: any gradient runs through every stage
+    modes = [_bn_mode(b, (x,), params) for b in bns]   # one autograd node: any gradient runs through every stage
     fused = (torch.is_grad_enabled() and "eval" not in modes and
              all(_is_native_conv(c, ci) for c, ci in zip(convs, cins)) and
              (blk.downsample is None or len(blk.downsample) == 2))
@@ -428,15 +456,26 @@ def _require_native(conv, cin):
 def conv_bn_act(x, conv, bn, relu=True, residual=None, out=None):
     """NHWC activation -> NHWC activation: conv -> BatchNorm -> (+residual) -> (ReLU), training, frozen or eval
     semantics of `bn` (see _bn_mode)."""
-    mode = _bn_mode(bn, x, conv.weight, bn.weight, bn.bias, residual)
+    mode = _bn_mode(bn, (x, residual), (conv.weight, bn.weight, bn.bias))
     _require_native(conv, x.shape[-1])
     if mode != "eval":
         return _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, residual, conv, bn, relu, out, mode == "frozen")
     # Eval-mode BatchNorm: conv + folded BN + residual + ReLU are ONE kernel. It has no backward: the reference's
     # validate() (tool/train.py:353-359) calls model.eval()(input) without torch.no_grad() and never back-propagates,
     # so the result is returned detached (a later .backward() through it raises torch's usual "does not require grad").
-    # A frozen BatchNorm of a training network takes this path only when nothing of the stage needs a gradient.
+    # A frozen BatchNorm takes this path only when nothing of the stage needs a gradient (see _bn_mode).
     return cba_forward(x, conv, bn, relu, residual, out, mode="eval")[0]
+
+
+def stem_conv_bn_act(x, conv, bn, relu=True):
+    """The module's fp32 NCHW input -> first stem stage (3-channel stride-2 conv -> BatchNorm -> ReLU), NHWC activation.
+    When `x` needs a gradient, the input conversion is part of the stage's autograd node and x.grad comes as fp32 NCHW
+    straight from the stem dgrad kernel; otherwise this is conv_bn_act(to_nhwc_bf16(x)), the patch form in training."""
+    if not (torch.is_grad_enabled() and x.requires_grad):
+        return conv_bn_act(to_nhwc_bf16(x), conv, bn, relu=relu)
+    mode = _bn_mode(bn, (x,), (conv.weight, bn.weight, bn.bias))
+    _require_native(conv, ops.round_up(x.shape[1], 8))
+    return _ConvBnAct.apply(x, conv.weight, bn.weight, bn.bias, None, conv, bn, relu, None, mode == "frozen")
 
 
 # ------------------------------------------------------------------------------------------------ classifier
@@ -651,9 +690,26 @@ def resize_bilinear(x, size):
 
 
 # ------------------------------------------------------------------------------------------------ misc NHWC ops
+class _NCHWToAct(torch.autograd.Function):
+    """fp32 NCHW -> activation (differentiable): the gradient goes back as fp32 NCHW through the split-aware
+    transpose, the padding channels dropped."""
+
+    @staticmethod
+    def forward(ctx, x, split):
+        ctx.c = x.shape[1]
+        return ops.nchw_to_nhwc_bf16(x.contiguous().float(), split=split)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return ops.nhwc_bf16_to_nchw((dy if dy.is_contiguous() else dy.contiguous())[..., :ctx.c]), None
+
+
 def to_nhwc_bf16(x_nchw):
     """fp32 NCHW module input -> NHWC activation (channels padded to a multiple of 8 with zeros) in the storage form of
-    the current precision mode (precision.py): plain bf16, or (hi, lo) bf16 planes for bf16x3."""
+    the current precision mode (precision.py): plain bf16, or (hi, lo) bf16 planes for bf16x3. Differentiable when
+    the input needs a gradient."""
+    if torch.is_grad_enabled() and x_nchw.requires_grad:
+        return _NCHWToAct.apply(x_nchw, precision.split_enabled())
     return ops.nchw_to_nhwc_bf16(x_nchw.contiguous().float(), split=precision.split_enabled())
 
 

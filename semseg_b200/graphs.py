@@ -6,7 +6,8 @@ DistributedDataParallel every host hiccup turns into a cross-rank wait inside th
 eager steps with the same input shape, `model(x, y)` in training mode therefore captures
 
     forward  : module input -> (argmax, main_loss, aux_loss)              [one graph]
-    backward : d(main_loss, aux_loss)/d(parameters) via torch.autograd.grad [one graph]
+    backward : d(main_loss, aux_loss)/d(parameters, and the input when it needs a gradient) via torch.autograd.grad
+                                                                            [one graph]
 
 into two CUDA graphs (the same kernels, in the same order, on the same stream) and replays them from ONE autograd node
 whose inputs are the module's parameters: `loss.backward()`, DDP's gradient hooks, `optimizer.step()` and checkpoints see
@@ -57,10 +58,10 @@ def note_boundary(t):
 
 class _Step:
     __slots__ = ("key", "calls", "failed", "fwd", "bwd", "bwd2", "x", "y", "pred", "main", "aux", "g_main", "g_aux",
-                 "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches")
+                 "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot")
 
     def __init__(self, key):
-        self.key, self.calls, self.failed, self.fwd = key, 0, False, None
+        self.key, self.calls, self.failed, self.fwd, self.dx_slot = key, 0, False, None, False
 
 
 def _set_grad_outputs(st, g_main, g_aux):
@@ -114,7 +115,15 @@ class _Replay(torch.autograd.Function):
         st = ctx.st
         _set_grad_outputs(st, g_main, g_aux)
         st.bwd.replay()
-        return (None, None, None) + _fresh(st.grads)
+        return _with_dx(st, _fresh(st.grads))
+
+
+def _with_dx(st, gs):
+    """(None, dx, None) + parameter gradients from the gradients `gs` a backward graph produced, the input gradient last
+    when the step was captured with an input that needs one."""
+    if st.dx_slot:
+        return (None, gs[-1], None) + gs[:-1]
+    return (None, None, None) + gs
 
 
 class _ReplayHead(torch.autograd.Function):
@@ -135,7 +144,7 @@ class _ReplayHead(torch.autograd.Function):
         if d_mid.data_ptr() != st.d_mid.data_ptr():
             st.d_mid.copy_(d_mid)
         st.bwd2.replay()
-        return (None, None, None) + _fresh(st.grads2)
+        return _with_dx(st, _fresh(st.grads2))
 
 
 class _ReplayTail(torch.autograd.Function):
@@ -183,7 +192,7 @@ def _capture(model, impl, st, x, y):
                 slots.append((mod, name, prm))
     st.params = [prm for _, _, prm in slots]
     st.x, st.y = torch.empty_like(x), torch.empty_like(y)
-    st.x.copy_(x)
+    st.x.copy_(x.detach())
     st.y.copy_(y)
     torch.cuda.synchronize()
     st.pool = torch.cuda.graph_pool_handle()
@@ -192,6 +201,11 @@ def _capture(model, impl, st, x, y):
     global _boundary
     _capturing, _boundary = True, None
     proxies = []
+    # an input that needs a gradient is captured as a leaf aliasing st.x; its gradient is the last one the backward
+    # graph (the second one in the two-segment form) produces
+    st.dx_slot = x.requires_grad
+    x_in = st.x.detach().requires_grad_(True) if st.dx_slot else st.x
+    x_leaf = [x_in] if st.dx_slot else []
     try:
         for mod, name, prm in slots:
             q = prm.detach().requires_grad_(True)      # same storage, new leaf
@@ -199,7 +213,7 @@ def _capture(model, impl, st, x, y):
             proxies.append(q)
         with torch.cuda.graph(st.fwd, pool=st.pool, capture_error_mode="thread_local"):
             with torch.enable_grad():
-                st.pred, st.main, st.aux = impl(st.x, st.y)
+                st.pred, st.main, st.aux = impl(x_in, st.y)
         st.g_main, st.g_aux = torch.ones_like(st.main), torch.ones_like(st.aux)
         t_mid = _boundary
         head_ids = set()
@@ -220,11 +234,12 @@ def _capture(model, impl, st, x, y):
             st.d_mid, st.grads = gs[0], gs[1:]
             st.bwd2 = torch.cuda.CUDAGraph()
             with torch.cuda.graph(st.bwd2, pool=st.pool, capture_error_mode="thread_local"):
-                st.grads2 = torch.autograd.grad((t_mid,), prox_head, (st.d_mid,), allow_unused=True)
+                st.grads2 = torch.autograd.grad((t_mid,), prox_head + x_leaf, (st.d_mid,), allow_unused=True)
             st.t_mid, st.n_tail = t_mid.detach(), len(prox_tail)
         else:
             with torch.cuda.graph(st.bwd, pool=st.pool, capture_error_mode="thread_local"):
-                st.grads = torch.autograd.grad((st.main, st.aux), proxies, (st.g_main, st.g_aux), allow_unused=True)
+                st.grads = torch.autograd.grad((st.main, st.aux), proxies + x_leaf, (st.g_main, st.g_aux),
+                                               allow_unused=True)
     finally:
         _capturing, _boundary = False, None
         for mod, name, prm in slots:
@@ -232,7 +247,7 @@ def _capture(model, impl, st, x, y):
     st.launches = _lib.launch_count() - l0          # native kernels per replayed step (forward + backward graphs)
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
-    del proxies
+    del proxies, x_in, x_leaf
     # the graphs reference the persistent weight slabs: keep their owner alive as long as the graphs
     st.keep = model.__dict__.get("_sb_pack_plan")
     torch.cuda.synchronize()
@@ -252,8 +267,11 @@ def train_step(model, impl, x, y):
     # BatchNorm modes (batch statistics or frozen) decide which kernels the step runs: freezing or unfreezing a layer
     # after a capture must capture again, not replay the old step
     bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
+    # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
-           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes)
+           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad)
+    if x.requires_grad and x.dtype != torch.float32:
+        return None                           # the captured input gradient is handed out in the parameters' fp32 buffer
     st = steps.get(key)
     if st is None:
         st = steps[key] = _Step(key)

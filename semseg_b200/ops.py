@@ -282,6 +282,22 @@ def im2col3x3s2(x, cin):
     return out
 
 
+def stem_dgrad3x3s2(dy, wp, cin, h, w):
+    """Input gradient of the stem conv (3x3 / stride 2 / pad 1, `cin` <= 3 channels) as fp32 NCHW [N, cin, h, w], from
+    the conv output's gradient `dy` (activation [N, Ho, Wo, 64], either storage form) and the patch slab `wp` of
+    PackedWeight (split exactly when dy is: bf16x3)."""
+    _require_cuda(dy, wp)
+    lib = _lib.load()
+    n, ho, wo, cout, p = _nhwc_meta(dy)
+    split = is_split(dy)
+    assert wp.dtype == torch.bfloat16 and wp.is_contiguous() and wp.dim() == (4 if split else 3), \
+        "the patch slab must be [1][Cout][32] (plain) or [2][1][Cout][32] (split), in dy's storage form"
+    dx = torch.empty((n, cin, h, w), dtype=torch.float32, device=dy.device)
+    _lib.check(lib.semseg_stem_dgrad3x3s2(_ptr(dy), _lo(dy), p, n, ho, wo, h, w, int(cin), cout, _ptr(wp), int(split),
+                                          _ptr(dx), _stream()), "semseg_stem_dgrad3x3s2")
+    return dx
+
+
 def space_to_phases(x):
     """x [N,H,W,C] bf16 -> [4N, (H+1)//2, (W+1)//2, C] (phase-major)."""
     _require_cuda(x)

@@ -159,8 +159,7 @@ class _SegNet(nn.Module):
     def _logits_nhwc(self, x):
         """fp32 NHWC classifier logits [N, h', w', classes] before the final upsample, and in training mode layer3's
         output for the aux head (None in eval mode)."""
-        t = SF.to_nhwc_bf16(x)
-        t = self.layer0.forward_nhwc(t)
+        t = self.layer0.forward_nchw(x)          # x.grad, when asked for, straight from the stem dgrad kernel
         t = self.layer1.forward_nhwc(t)
         t = graphs.note_boundary(self.layer2.forward_nhwc(t))     # where a captured backward is cut in two
         t_tmp = self.layer3.forward_nhwc(t)

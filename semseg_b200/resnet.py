@@ -66,10 +66,20 @@ class Stem(NHWCSequential):
     (model/pspnet.py:46) so state_dict keys are layer0.0.weight, layer0.1.weight, ..."""
 
     def forward_nhwc(self, x):
-        x = SF.conv_bn_act(x, self[0], self[1], relu=True)
+        return self._rest(SF.conv_bn_act(x, self[0], self[1], relu=True))
+
+    def forward_nchw(self, x):
+        """fp32 NCHW module input -> NHWC activation; when x needs a gradient it comes from the stem dgrad kernel."""
+        return self._rest(SF.stem_conv_bn_act(x, self[0], self[1], relu=True))
+
+    def _rest(self, x):
         x = SF.conv_bn_act(x, self[3], self[4], relu=True)
         x = SF.conv_bn_act(x, self[6], self[7], relu=True)
         return SF.maxpool_nhwc(x, self[9])
+
+    @SF.network_forward
+    def forward(self, x):
+        return SF.to_nchw_f32(self.forward_nchw(x))
 
 
 class ResNet(nn.Module):
@@ -122,7 +132,7 @@ class ResNet(nn.Module):
     @SF.network_forward
     def forward(self, x):
         # ImageNet-classification forward of the reference (model/resnet.py:147-164); not on the segmentation path.
-        y = self.stem().forward_nhwc(SF.to_nhwc_bf16(x))
+        y = self.stem().forward_nchw(x)
         for layer in (self.layer1, self.layer2, self.layer3, self.layer4):
             y = layer.forward_nhwc(y)
         y = SF.to_nchw_f32(y)
