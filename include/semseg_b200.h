@@ -19,6 +19,7 @@
  *   - semseg_ppm_* / pool     : model/pspnet.py:12-26 (AdaptiveAvgPool2d, bilinear upsample, concat),
  *                               nn.MaxPool2d at model/resnet.py:115.
  *   - semseg_upsample_ce_*    : F.interpolate + CrossEntropyLoss + argmax, model/pspnet.py:94-103.
+ *                               semseg_upsample_ce_ohem_*: the same with an OHEM cross-entropy criterion.
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -402,6 +403,26 @@ long long semseg_upsample_ce_zoom_bwd_workspace_floats(int N, int Ho, int w, int
 int semseg_upsample_ce_zoom_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                                 int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* loss_info,
                                 const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* OHEM cross-entropy (semseg_b200/losses.py OhemCrossEntropyLoss) on the same fused upsample at zoom `zoom`: with
+ * p_t = softmax(v)[target] and nll = -log_softmax(v)[target] per valid pixel (target != ignore_index, 0 <= target < C),
+ * k = min(min_kept, n_v - 1) over the n_v valid pixels, thr = max(thresh, k-th smallest p_t (0-based)), the loss is the
+ * mean nll over the kept pixels, p_t < thr; 0 (and a zero gradient) when none is kept. Requires 0 <= thresh <= 1,
+ * min_kept >= 0. The selection is exact and runs on the device (no host synchronisation; graph-capturable).
+ *   fwd: loss_out[0] = mean nll over the kept pixels, loss_out[1] = kept count; argmax (or NULL) and lse as above;
+ *        pt, nll fp32 [N,Ho,Wo] (pt = -1, nll = 0 where the pixel is not valid); thr fp32 [1] = the threshold.
+ *        workspace: semseg_upsample_ce_ohem_workspace_floats() floats.
+ *   bwd: dlogits as above, with every pixel whose pt is not below *thr treated as ignored (the forward's kept set);
+ *        workspace: semseg_upsample_ce_ohem_bwd_workspace_floats() floats (the same as the zoom backward's). */
+long long semseg_upsample_ce_ohem_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_ce_ohem_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                int Ho, int Wo, int zoom, int ignore_index, float thresh, int min_kept,
+                                float* workspace, float* loss_out, int64_t* argmax, float* lse, float* pt, float* nll,
+                                float* thr, void* stream);
+long long semseg_upsample_ce_ohem_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_ohem_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* pt,
+                                const float* thr, const float* loss_info, const float* grad_out, float* workspace,
+                                float* dlogits, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sliding-window evaluation after the network (semseg_b200/inference.py, exact=False). No tensor cores, no atomics.

@@ -167,6 +167,12 @@ SIGNATURES = {
     "semseg_upsample_ce_zoom_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_zoom_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_ohem_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_ohem_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                            c_f, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_ohem_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_ohem_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                            c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
     "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_vp, c_vp]),

@@ -17,6 +17,11 @@
 //
 // Backward is a deterministic, separable gather (rows kernel + cols kernel, see below). No atomics, every dlogits
 // element is written exactly once.
+//
+// Online hard-pixel mining (OHEM cross-entropy, semseg_b200/losses.py) runs on the same kernels in a compile-time form
+// (kOhem): the forward also writes each pixel's target probability p_t and nll and leaves the loss to a masked reduce;
+// a radix select over the p_t bit patterns finds the k-th smallest p_t on the device; the backward treats every pixel
+// with p_t >= threshold as ignored. The kOhem = false instances are the plain cross-entropy kernels, unchanged.
 #include "host_common.h"
 
 namespace sb {
@@ -31,6 +36,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr int kFwdCols = 128;                    // output columns per CTA (one per thread)
+constexpr float kInvalidPt = -1.f;               // p_t of a pixel that is ignored or whose target is out of range
 
 // Compile-time geometry of zoom factor Z (a power of two): source index x >> kShift, fraction (x & kMask) * kStep.
 template <int Z>
@@ -58,11 +64,14 @@ __device__ __forceinline__ float row_lerp(float top, float bot, int r) {
 // and shared by the Z rows (v = l0h*top + l1h*bot with compile-time row weights), so at Z = 8 a pixel-class costs ~5
 // instructions per pass instead of a full 4-tap interpolation. Two passes over the classes: max/argmax, then
 // sum of exp2 — one MUFU per pixel-class, no rescaling branches.
-template <int Z>
+// kOhem: no loss partials; per pixel p_t = exp(v_t - lse) and nll = lse - v_t instead (kInvalidPt / 0 where the target
+// is ignored or out of range). The OHEM-only arguments come last, so the plain instances keep their parameter layout.
+template <int Z, bool kOhem>
 __global__ void __launch_bounds__(kFwdCols)
 upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
                        const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
-                       float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out) {
+                       float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out,
+                       float* __restrict__ pt_out, float* __restrict__ nll_out) {
   using G = Zoom<Z>;
   constexpr int kFwdNodes = G::kNodes;
   extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs]; Cs odd -> the node columns a warp reads hit distinct banks
@@ -140,31 +149,41 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
           const float top = Z == 1 ? A[tc] : l0w * A[tc] + l1w * B[tc];
           const float bot = Z == 1 ? 0.f : l0w * Cc[tc] + l1w * D[tc];
           const float vt = row_lerp<Z>(top, bot, r);
-          loss += lse - vt;
-          cnt += 1.f;
+          if constexpr (kOhem) {
+            pt_out[pix] = expf(vt - lse);
+            nll_out[pix] = lse - vt;
+          } else {
+            loss += lse - vt;
+            cnt += 1.f;
+          }
+        } else if constexpr (kOhem) {
+          pt_out[pix] = kInvalidPt;
+          nll_out[pix] = 0.f;
         }
       }
     }
   }
-  // deterministic block reduction -> one partial per CTA
-  for (int o = 16; o > 0; o >>= 1) {
-    loss += __shfl_xor_sync(0xffffffffu, loss, o);
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-  }
-  if ((tid & 31) == 0) {
-    red_loss[tid >> 5] = loss;
-    red_cnt[tid >> 5] = cnt;
-  }
-  __syncthreads();
-  if (tid == 0) {
-    float l = 0.f, k = 0.f;
-    for (int i = 0; i < kFwdCols / 32; ++i) {
-      l += red_loss[i];
-      k += red_cnt[i];
+  if constexpr (!kOhem) {
+    // deterministic block reduction -> one partial per CTA
+    for (int o = 16; o > 0; o >>= 1) {
+      loss += __shfl_xor_sync(0xffffffffu, loss, o);
+      cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
     }
-    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    partial[2 * b] = l;
-    partial[2 * b + 1] = k;
+    if ((tid & 31) == 0) {
+      red_loss[tid >> 5] = loss;
+      red_cnt[tid >> 5] = cnt;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      float l = 0.f, k = 0.f;
+      for (int i = 0; i < kFwdCols / 32; ++i) {
+        l += red_loss[i];
+        k += red_cnt[i];
+      }
+      const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+      partial[2 * b] = l;
+      partial[2 * b + 1] = k;
+    }
   }
 }
 
@@ -193,6 +212,118 @@ __global__ void upsample_ce_reduce_kernel(const float* __restrict__ partial, int
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- OHEM selection
+// The k-th smallest p_t over the valid pixels, exactly: a radix select over the fp32 bit patterns (non-negative floats
+// order like their uint32 patterns), four passes of 8 bits from the top. Each pass histograms the digit of the pixels
+// whose higher digits equal the prefix found so far (integer counts: the result does not depend on the order of the
+// atomics), then one CTA picks the digit that holds the k-th value. Device state only: no host synchronisation, so the
+// whole selection is captured into a CUDA graph with the step. Workspace words (zeroed before the first pass):
+constexpr int kSelPrefix = 0;     // digits found so far
+constexpr int kSelK = 1;          // rank of the wanted value among the pixels matching the prefix
+constexpr int kSelValid = 2;      // number of valid pixels n_v (pass 0)
+constexpr int kSelHist = 4;       // [4 passes][256] counts
+constexpr int kSelWords = kSelHist + 4 * 256;
+constexpr int kSelThreads = 256;
+
+__global__ void __launch_bounds__(kSelThreads)
+ohem_hist_kernel(const float* __restrict__ pt, long long M, int pass, unsigned* __restrict__ sel) {
+  __shared__ unsigned hist[256];
+  hist[threadIdx.x] = 0;
+  __syncthreads();
+  const int shift = 24 - 8 * pass;
+  const unsigned hi_mask = pass == 0 ? 0u : 0xffffffffu << (shift + 8);
+  const unsigned prefix = sel[kSelPrefix];
+  const int lane = threadIdx.x & 31;
+  // base is CTA-uniform: every lane of a warp runs every iteration (the warp-aggregated add below needs all 32)
+  for (long long base = static_cast<long long>(blockIdx.x) * kSelThreads; base < M;
+       base += static_cast<long long>(gridDim.x) * kSelThreads) {
+    const long long i = base + threadIdx.x;
+    unsigned d = 0xffffffffu;
+    if (i < M) {
+      const float p = pt[i];
+      const unsigned u = __float_as_uint(p);
+      if (p >= 0.f && (u & hi_mask) == prefix) d = (u >> shift) & 255u;
+    }
+    // confident pixels share a few digits (every p_t in [0.5, 1] has top byte 0x3f): one add per distinct digit
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    if (d != 0xffffffffu && lane == __ffs(peers) - 1) atomicAdd(&hist[d], static_cast<unsigned>(__popc(peers)));
+  }
+  __syncthreads();
+  if (hist[threadIdx.x]) atomicAdd(&sel[kSelHist + pass * 256 + threadIdx.x], hist[threadIdx.x]);
+}
+
+// One CTA: pass 0 counts n_v and sets k = min(min_kept, n_v - 1); every pass appends the digit whose bin holds rank k.
+// After the last pass the prefix is the k-th smallest p_t and thr = max(thresh, it) (thresh when no pixel is valid).
+__global__ void __launch_bounds__(kSelThreads)
+ohem_select_kernel(unsigned* __restrict__ sel, int pass, float thresh, int min_kept, float* __restrict__ thr) {
+  __shared__ unsigned cnt[256];
+  cnt[threadIdx.x] = sel[kSelHist + pass * 256 + threadIdx.x];
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  unsigned k, prefix;
+  if (pass == 0) {
+    unsigned nv = 0;
+    for (int b = 0; b < 256; ++b) nv += cnt[b];
+    sel[kSelValid] = nv;
+    k = nv == 0 ? 0u : min(static_cast<unsigned>(min_kept), nv - 1u);
+    prefix = 0;
+  } else {
+    k = sel[kSelK];
+    prefix = sel[kSelPrefix];
+  }
+  unsigned d = 0;
+  for (; d < 255; ++d) {
+    if (k < cnt[d]) break;
+    k -= cnt[d];
+  }
+  prefix |= d << (24 - 8 * pass);
+  sel[kSelK] = k;
+  sel[kSelPrefix] = prefix;
+  if (pass == 3) thr[0] = sel[kSelValid] ? fmaxf(thresh, __uint_as_float(prefix)) : thresh;
+}
+
+// Kept pixels (p_t >= 0, i.e. valid, and p_t < thr): one (sum of nll, count) partial per kMaskPix pixels, fixed order;
+// upsample_ce_reduce_kernel turns them into (mean, kept count).
+constexpr int kMaskPix = 4096;
+
+__global__ void __launch_bounds__(kSelThreads)
+ohem_masked_sum_kernel(const float* __restrict__ pt, const float* __restrict__ nll, long long M,
+                       const float* __restrict__ thr, float* __restrict__ partial) {
+  __shared__ float red_loss[kSelThreads / 32];
+  __shared__ float red_cnt[kSelThreads / 32];
+  const float t = thr[0];
+  const long long base = static_cast<long long>(blockIdx.x) * kMaskPix;
+  float loss = 0.f, cnt = 0.f;
+  for (int j = threadIdx.x; j < kMaskPix; j += kSelThreads) {
+    const long long i = base + j;
+    if (i < M) {
+      const float p = pt[i];
+      if (p >= 0.f && p < t) {
+        loss += nll[i];
+        cnt += 1.f;
+      }
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    red_loss[threadIdx.x >> 5] = loss;
+    red_cnt[threadIdx.x >> 5] = cnt;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float l = 0.f, k = 0.f;
+    for (int i = 0; i < kSelThreads / 32; ++i) {
+      l += red_loss[i];
+      k += red_cnt[i];
+    }
+    partial[2 * blockIdx.x] = l;
+    partial[2 * blockIdx.x + 1] = k;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------- backward
 // Separable, deterministic, no atomics. With g[y,x,c] = softmax_{y,x}[c] - [c == t_{y,x}] (0 for ignored pixels):
 //   dL[i,j,c] = gs * sum_y wy(y,i) * sum_x wx(x,j) * g[y,x,c].
@@ -204,27 +335,35 @@ __global__ void upsample_ce_reduce_kernel(const float* __restrict__ partial, int
 // contribution to node row i0, s = 1: to node row i0+1 (fp32 workspace, 68 MB at bs16 / 150 classes; at Z = 1 slot 1
 // is all zeros).
 // Phase 2 (cols): dL[i] = gs * (T2[i][0] + T2[i-1][1]).
+// kOhem: a pixel is also ignored when its stored p_t is not below the device threshold, the forward's kept set bit for
+// bit; the cols kernel then divides by the kept count in loss_info[1].
 struct __align__(8) PixInfo {
   float lse2;  // log-sum-exp * log2(e)
   int t;       // target class, -1 = ignored
 };
 
-template <int Z>
+template <int Z, bool kOhem>
 __global__ void __launch_bounds__(256)
 upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
                             const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
-                            const float* __restrict__ lse, float* __restrict__ T2) {
+                            const float* __restrict__ lse, float* __restrict__ T2, const float* __restrict__ pt,
+                            const float* __restrict__ thr) {
   using G = Zoom<Z>;
   extern __shared__ PixInfo s_pix[];  // [Z][Wo]
   const int i0 = blockIdx.x, n = blockIdx.y;
   const int i1 = min(i0 + 1, h - 1);
   const int rows = min(Z, Ho - Z * i0);
+  float thr_v = 0.f;
+  if constexpr (kOhem) thr_v = thr[0];
   for (int r = 0; r < rows; ++r) {
     const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
     for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
       const long long t = target[rowbase + x];
       PixInfo pi;
       pi.t = (t == ignore_index || t < 0 || t >= C) ? -1 : static_cast<int>(t);
+      if constexpr (kOhem) {
+        if (!(pt[rowbase + x] < thr_v)) pi.t = -1;
+      }
       pi.lse2 = lse[rowbase + x] * kLog2e;
       s_pix[r * Wo + x] = pi;
     }
@@ -350,10 +489,12 @@ static int opt_in_smem(Kernel kernel, std::atomic<bool>* attr_set, int max_bytes
 constexpr size_t kSmemDefault = 48 * 1024;
 constexpr size_t kBwdSmemMax = 160 * 1024;   // staged (lse, target) words of the backward's Z output rows
 
-template <int Z>
-static int launch_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
-                      int ignore_index, float* workspace, float* loss_out, int64_t* argmax, float* lse,
-                      cudaStream_t stream) {
+static int fwd_ctas(int N, int h, int Wo) { return cdiv(Wo, kFwdCols) * h * N; }
+
+template <int Z, bool kOhem>
+static int launch_fwd_kernel(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                             int Wo, int ignore_index, float* partial, int64_t* argmax, float* lse, float* pt,
+                             float* nll, cudaStream_t stream) {
   dim3 grid(cdiv(Wo, kFwdCols), h, N);
   const int Cs = C | 1;
   // at most 2 * 65 * 257 floats (Z = 2, 256 classes); above 48 KB only at Z <= 4 (Z = 1 and 2 with 150 classes: 78 KB)
@@ -361,32 +502,73 @@ static int launch_fwd(const float* logits, int pitch, int N, int h, int w, int C
   const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
   static std::atomic<bool> attr_set[64];
   if (smem > kSmemDefault) {
-    int r = opt_in_smem(upsample_ce_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    int r = opt_in_smem(upsample_ce_fwd_kernel<Z, kOhem>, attr_set, static_cast<int>(kMaxSmem));
     if (r) return r;
   }
-  upsample_ce_fwd_kernel<Z><<<grid, kFwdCols, smem, stream>>>(
-      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, workspace,
-      reinterpret_cast<long long*>(argmax), lse);
-  SB_LAUNCHED();
-  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, static_cast<int>(grid.x * grid.y * grid.z), loss_out);
+  upsample_ce_fwd_kernel<Z, kOhem><<<grid, kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, partial,
+      reinterpret_cast<long long*>(argmax), lse, pt, nll);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
 
 template <int Z>
+static int launch_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
+                      int ignore_index, float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                      cudaStream_t stream) {
+  int r = launch_fwd_kernel<Z, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, argmax, lse,
+                                      nullptr, nullptr, stream);
+  if (r) return r;
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+static long long ohem_hist_ctas(long long M) { return std::min<long long>((M + kSelThreads - 1) / kSelThreads, 8LL * num_sms()); }
+static long long ohem_mask_ctas(long long M) { return (M + kMaskPix - 1) / kMaskPix; }
+
+// Workspace: kSelWords selection words, then (loss, count) per masked-reduce CTA.
+template <int Z>
+static int launch_ohem_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                           int Wo, int ignore_index, float thresh, int min_kept, float* workspace, float* loss_out,
+                           int64_t* argmax, float* lse, float* pt, float* nll, float* thr, cudaStream_t stream) {
+  const long long M = static_cast<long long>(N) * Ho * Wo;
+  unsigned* sel = reinterpret_cast<unsigned*>(workspace);
+  float* partial = workspace + kSelWords;
+  SB_CUDA(cudaMemsetAsync(sel, 0, kSelWords * sizeof(unsigned), stream));
+  int r = launch_fwd_kernel<Z, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, nullptr, argmax, lse, pt,
+                                     nll, stream);
+  if (r) return r;
+  const int hist_ctas = static_cast<int>(ohem_hist_ctas(M));
+  for (int pass = 0; pass < 4; ++pass) {
+    ohem_hist_kernel<<<hist_ctas, kSelThreads, 0, stream>>>(pt, M, pass, sel);
+    SB_LAUNCHED();
+    ohem_select_kernel<<<1, kSelThreads, 0, stream>>>(sel, pass, thresh, min_kept, thr);
+    SB_LAUNCHED();
+  }
+  const int mask_ctas = static_cast<int>(ohem_mask_ctas(M));
+  ohem_masked_sum_kernel<<<mask_ctas, kSelThreads, 0, stream>>>(pt, nll, M, thr, partial);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(partial, mask_ctas, loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z, bool kOhem>
 static int launch_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
                       int ignore_index, const float* lse, const float* loss_info, const float* grad_out,
-                      float* workspace, float* dlogits, cudaStream_t stream) {
+                      float* workspace, float* dlogits, const float* pt, const float* thr, cudaStream_t stream) {
   const int threads = (C + 31) / 32 * 32;
   const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(PixInfo);
   SB_CHECK_ARG(smem <= kBwdSmemMax, "upsample_ce_bwd: output width %d too large for the staged rows", Wo);
   static std::atomic<bool> attr_set[64];
   if (smem > kSmemDefault) {
-    int r = opt_in_smem(upsample_ce_bwd_rows_kernel<Z>, attr_set, static_cast<int>(kBwdSmemMax));
+    int r = opt_in_smem(upsample_ce_bwd_rows_kernel<Z, kOhem>, attr_set, static_cast<int>(kBwdSmemMax));
     if (r) return r;
   }
-  upsample_ce_bwd_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(
-      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, workspace);
+  upsample_ce_bwd_rows_kernel<Z, kOhem><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, workspace, pt,
+      thr);
   SB_LAUNCHED();
   upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out, dlogits);
   SB_LAUNCHED();
@@ -432,14 +614,74 @@ extern "C" int semseg_upsample_ce_zoom_bwd(const float* logits, int pitch, int N
   if (r) return r;
   SB_CHECK_ARG(lse && loss_info && grad_out && dlogits && workspace, "upsample_ce_bwd: null pointer");
   switch (zoom) {
-    case 1: return launch_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
-                                 workspace, dlogits, stream);
-    case 2: return launch_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
-                                 workspace, dlogits, stream);
-    case 4: return launch_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
-                                 workspace, dlogits, stream);
-    default: return launch_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info, grad_out,
-                                  workspace, dlogits, stream);
+    case 1: return launch_bwd<1, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                        grad_out, workspace, dlogits, nullptr, nullptr, stream);
+    case 2: return launch_bwd<2, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                        grad_out, workspace, dlogits, nullptr, nullptr, stream);
+    case 4: return launch_bwd<4, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                        grad_out, workspace, dlogits, nullptr, nullptr, stream);
+    default: return launch_bwd<8, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                         grad_out, workspace, dlogits, nullptr, nullptr, stream);
+  }
+}
+
+// OHEM cross-entropy at zoom factor `zoom`: the kOhem instances, the selection and the masked reduce.
+static int check_ohem(float thresh, int min_kept) {
+  SB_CHECK_ARG(thresh >= 0.f && thresh <= 1.f, "upsample_ce_ohem: thresh %g is not in [0, 1]", thresh);
+  SB_CHECK_ARG(min_kept >= 0, "upsample_ce_ohem: min_kept %d is negative", min_kept);
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_ohem_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_ohem: zoom %d is not one of 1, 2, 4, 8", zoom);
+  return kSelWords + 2LL * ohem_mask_ctas(static_cast<long long>(N) * Ho * Wo);
+}
+
+extern "C" int semseg_upsample_ce_ohem_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                           const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                           float thresh, int min_kept, float* workspace, float* loss_out,
+                                           int64_t* argmax, float* lse, float* pt, float* nll, float* thr,
+                                           void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_ohem(thresh, min_kept);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && pt && nll && thr, "upsample_ce_ohem_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_ohem_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                      workspace, loss_out, argmax, lse, pt, nll, thr, stream);
+    case 2: return launch_ohem_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                      workspace, loss_out, argmax, lse, pt, nll, thr, stream);
+    case 4: return launch_ohem_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                      workspace, loss_out, argmax, lse, pt, nll, thr, stream);
+    default: return launch_ohem_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                       workspace, loss_out, argmax, lse, pt, nll, thr, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_ohem_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_ce_ohem_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                           const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                           const float* lse, const float* pt, const float* thr,
+                                           const float* loss_info, const float* grad_out, float* workspace,
+                                           float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  SB_CHECK_ARG(lse && pt && thr && loss_info && grad_out && dlogits && workspace, "upsample_ce_ohem_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_bwd<1, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                       grad_out, workspace, dlogits, pt, thr, stream);
+    case 2: return launch_bwd<2, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                       grad_out, workspace, dlogits, pt, thr, stream);
+    case 4: return launch_bwd<4, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                       grad_out, workspace, dlogits, pt, thr, stream);
+    default: return launch_bwd<8, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                        grad_out, workspace, dlogits, pt, thr, stream);
   }
 }
 

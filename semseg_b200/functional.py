@@ -24,6 +24,7 @@ import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F
 
+from . import losses
 from . import ops
 from . import p2p
 from . import precision
@@ -537,12 +538,34 @@ class _UpsampleCE(torch.autograd.Function):
         return ops.upsample_ce_bwd(logits, target, ctx.ignore_index, lse, info, grad_loss, zoom=ctx.zoom), None, None, None
 
 
+class _UpsampleCEOhem(torch.autograd.Function):
+    """The fused tail with the OHEM cross-entropy of losses.OhemCrossEntropyLoss: the forward also keeps each pixel's
+    p_t and the device threshold, and the backward trains exactly the pixels the forward kept."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, thresh, min_kept):
+        info, amax, lse, pt, _nll, thr = ops.upsample_ce_ohem_fwd(logits, target, ignore_index, thresh, min_kept,
+                                                                  zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, pt, thr, info)
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, pt, thr, info = ctx.saved_tensors
+        dl = ops.upsample_ce_ohem_bwd(logits, target, ctx.ignore_index, lse, pt, thr, info, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None
+
+
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
-    """The fused kernel implements exactly nn.CrossEntropyLoss(ignore_index=k) with default options, at every zoom factor
-    of the model (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits.
+    """The fused kernel implements exactly nn.CrossEntropyLoss(ignore_index=k) with default options and
+    losses.OhemCrossEntropyLoss, at every zoom factor of the model (1, 2, 4, 8) with the target at the zoomed size
+    zoom*(h'-1)+1 of the 1/8-resolution logits.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
-    if not (type(criterion) is nn.CrossEntropyLoss and criterion.weight is None and criterion.reduction == 'mean'
-            and getattr(criterion, 'label_smoothing', 0.0) == 0.0 and zoom_factor in (1, 2, 4, 8)
+    plain_ce = (type(criterion) is nn.CrossEntropyLoss and criterion.weight is None and criterion.reduction == 'mean'
+                and getattr(criterion, 'label_smoothing', 0.0) == 0.0)
+    if not ((plain_ce or type(criterion) is losses.OhemCrossEntropyLoss) and zoom_factor in (1, 2, 4, 8)
             and target is not None and target.dtype == torch.int64 and target.dim() == 3):
         return False
     if logits is None:
@@ -554,8 +577,12 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     return target.shape[1] == zoom_factor * (h - 1) + 1 and target.shape[2] == zoom_factor * (w - 1) + 1
 
 
-def upsample_ce(logits, target, ignore_index, zoom=8):
-    """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1."""
+def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None):
+    """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
+    losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index)."""
+    if isinstance(criterion, losses.OhemCrossEntropyLoss):
+        return _UpsampleCEOhem.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.thresh,
+                                     criterion.min_kept)
     return _UpsampleCE.apply(logits, target.contiguous(), ignore_index, int(zoom))
 
 

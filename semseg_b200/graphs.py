@@ -17,7 +17,8 @@ step counter incremented inside the graph — csrc/bn.cu st_ll / ld_ll) and drop
 
 Limits (same as torch.cuda.make_graphed_callables): a second training forward before the backward of the first one
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
-The NCCL fallback of the SyncBN exchange and non-default criteria are not captured (such models simply stay eager).
+The NCCL fallback of the SyncBN exchange and criteria other than the default and OHEM cross-entropy are not captured
+(such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -268,8 +269,12 @@ def train_step(model, impl, x, y):
     # after a capture must capture again, not replay the old step
     bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
     # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
+    # the criterion's options are launch arguments baked into the graph: a changed thresh or ignore_index captures anew
+    crit = getattr(model, "criterion", None)
+    crit_key = (type(crit),) + tuple(getattr(crit, a, None) for a in ("ignore_index", "thresh", "min_kept"))
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
-           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad)
+           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad,
+           crit_key)
     if x.requires_grad and x.dtype != torch.float32:
         return None                           # the captured input gradient is handed out in the parameters' fp32 buffer
     st = steps.get(key)

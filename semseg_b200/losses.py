@@ -1,0 +1,59 @@
+"""Loss modules the networks accept as `criterion` besides nn.CrossEntropyLoss.
+
+OhemCrossEntropyLoss is online hard-pixel mining: only the pixels the network is least sure of are trained on. With
+the network's fused tail (functional.upsample_ce) it runs inside the same kernels as the default loss, graphed at every
+zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
+zoom-1 form of those kernels on an NHWC copy of the logits.
+"""
+import torch
+from torch import nn
+
+
+class OhemCrossEntropyLoss(nn.Module):
+    """Pixel OHEM cross-entropy, the sort-based definition of the HRNet / OCR code bases, for logits [N, C, H, W] and
+    target [N, H, W]:
+
+        valid = target != ignore_index and 0 <= target < C     (other out-of-range targets are skipped)
+        p_t   = softmax(logits)[target],  nll = -log_softmax(logits)[target]        per valid pixel
+        k     = min(min_kept, n_valid - 1)
+        thr   = max(thresh, k-th smallest p_t over the valid pixels (0-based))
+        kept  = valid and p_t < thr                                                  (strict)
+        loss  = mean of nll over the kept pixels
+
+    With no valid or no kept pixel the loss is 0 and every gradient is 0 (the fused tail's convention; torch's mean over
+    nothing would be nan). The selection is exact: the k-th value is found by a radix select on the device, without a
+    host synchronisation. Under DistributedDataParallel each rank mines its own pixels.
+
+    CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
+
+    def __init__(self, ignore_index=255, thresh=0.7, min_kept=100000):
+        super(OhemCrossEntropyLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        if isinstance(min_kept, bool) or not isinstance(min_kept, int):
+            raise TypeError("min_kept must be an int, got %r" % (min_kept,))
+        thresh = float(thresh)
+        if not 0.0 <= thresh <= 1.0:
+            raise ValueError("thresh must lie in [0, 1], got %r" % thresh)
+        if not 0 <= min_kept < 2 ** 31:
+            raise ValueError("min_kept must be a non-negative 32-bit int, got %r" % min_kept)
+        self.ignore_index, self.thresh, self.min_kept = ignore_index, thresh, min_kept
+
+    def extra_repr(self):
+        return "ignore_index=%d, thresh=%g, min_kept=%d" % (self.ignore_index, self.thresh, self.min_kept)
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        if logits.dim() != 4 or target.dim() != 3 or target.shape != logits.shape[:1] + logits.shape[2:]:
+            raise ValueError("OhemCrossEntropyLoss: logits [N, C, H, W] and target [N, H, W] expected, got %s and %s" %
+                             (tuple(logits.shape), tuple(target.shape)))
+        if logits.shape[1] > 256:
+            raise ValueError("OhemCrossEntropyLoss: at most 256 classes (got %d); no fallback" % logits.shape[1])
+        if not (logits.is_cuda and target.is_cuda):
+            raise RuntimeError("OhemCrossEntropyLoss runs on the native CUDA kernels only (no CPU fallback); got %s, %s"
+                               % (logits.device, target.device))
+        if logits.dtype != torch.float32 or target.dtype != torch.int64:
+            raise TypeError("OhemCrossEntropyLoss: fp32 logits and int64 target expected, got %s and %s" %
+                            (logits.dtype, target.dtype))
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss

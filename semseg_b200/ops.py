@@ -697,6 +697,48 @@ def upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_out, zoom=8):
     return dl
 
 
+def upsample_ce_ohem_fwd(logits, target, ignore_index, thresh, min_kept, want_argmax=True, zoom=8):
+    """OHEM cross-entropy on the fused tail (semseg_b200/losses.py states the contract); arguments as upsample_ce_fwd
+    -> (loss_info [2] = (mean nll over the kept pixels, kept count), argmax, lse, p_t, nll, thr [1]). p_t / nll fp32
+    [N,Ho,Wo], p_t = -1 where the pixel is not valid."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_ohem_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_ohem_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    thr = torch.empty((1,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse, pt, nll = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(3))
+    _lib.check(lib.semseg_upsample_ce_ohem_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                               int(zoom), int(ignore_index), float(thresh), int(min_kept), _ptr(ws),
+                                               _ptr(info), _ptr(amax), _ptr(lse), _ptr(pt), _ptr(nll), _ptr(thr),
+                                               _stream()),
+               "semseg_upsample_ce_ohem_fwd")
+    return info, amax, lse, pt, nll, thr
+
+
+def upsample_ce_ohem_bwd(logits, target, ignore_index, lse, pt, thr, info, grad_out, zoom=8):
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_ohem_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_ohem_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_ohem_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                               int(zoom), int(ignore_index), _ptr(lse), _ptr(pt), _ptr(thr), _ptr(info),
+                                               _ptr(g), _ptr(ws), _ptr(dl), _stream()),
+               "semseg_upsample_ce_ohem_bwd")
+    return dl
+
+
 # ------------------------------------------------------------------------------------------------ sliding-window evaluation
 def window_scores(logits, flip, out):
     """fp32 NHWC logits [G (+G mirrored crops when flip), h, w, C] -> flip-averaged softmax scores written into `out`,

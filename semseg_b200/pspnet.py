@@ -142,8 +142,10 @@ class _SegNet(nn.Module):
             aux_logits = head_forward_nhwc(self.aux, t_aux)
             if SF.fused_tail_supported(self.criterion, logits, y, self.zoom_factor):
                 # upsample + cross-entropy + argmax fused: [N, classes, H, W] never exists (model/pspnet.py:94-103)
-                main_loss, pred = SF.upsample_ce(logits, y, self.criterion.ignore_index, self.zoom_factor)
-                aux_loss, _ = SF.upsample_ce(aux_logits, y, self.criterion.ignore_index, self.zoom_factor)
+                main_loss, pred = SF.upsample_ce(logits, y, self.criterion.ignore_index, self.zoom_factor,
+                                                 criterion=self.criterion)
+                aux_loss, _ = SF.upsample_ce(aux_logits, y, self.criterion.ignore_index, self.zoom_factor,
+                                             criterion=self.criterion)
                 return pred, main_loss, aux_loss
             x = upsample_logits(logits, (h, w), self.zoom_factor)
             aux = upsample_logits(aux_logits, (h, w), self.zoom_factor)
