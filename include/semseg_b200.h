@@ -20,6 +20,7 @@
  *                               nn.MaxPool2d at model/resnet.py:115.
  *   - semseg_upsample_ce_*    : F.interpolate + CrossEntropyLoss + argmax, model/pspnet.py:94-103.
  *                               semseg_upsample_ce_ohem_*: the same with an OHEM cross-entropy criterion.
+ *                               semseg_upsample_ce_{,ohem_}weighted_*: class weights / label smoothing.
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -423,6 +424,40 @@ int semseg_upsample_ce_ohem_bwd(const float* logits, int pitch, int N, int h, in
                                 int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* pt,
                                 const float* thr, const float* loss_info, const float* grad_out, float* workspace,
                                 float* dlogits, void* stream);
+/* Class-weighted and label-smoothed cross-entropy (nn.CrossEntropyLoss(weight, ignore_index, reduction='mean',
+ * label_smoothing)) on the same fused upsample at zoom `zoom`. class_weight fp32 [C] on the device (NULL = all ones;
+ * read at every launch, so a CUDA graph sees in-place edits), label_smoothing eps in [0, 1]. With w_t the weight of a
+ * valid pixel's target, W = sum_c w_c and lse = logsumexp_c v_c:
+ *   loss_pix = (1-eps) w_t (lse - v_t) + (eps/C) sum_c w_c (lse - v_c),  loss = sum over valid pixels / D, D = sum w_t;
+ * loss 0 and an exactly zero gradient when D = 0 (where torch gives nan). Out-of-range targets are ignored.
+ *   fwd: loss_out[0] = loss, loss_out[1] = D; argmax (or NULL) and lse as above; workspace:
+ *        semseg_upsample_ce_weighted_workspace_floats() floats (the zoom forward's).
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits; workspace:
+ *        semseg_upsample_ce_weighted_bwd_workspace_floats() floats (the zoom backward's). Same width limit as the zoom
+ *        backward.
+ * Weighted OHEM (losses.OhemCrossEntropyLoss(weight=...)): the OHEM entry points with nll = w_t (lse - v_t); the
+ * selection on p_t is unweighted and the loss is the plain mean of w_t * nll over the kept pixels. Workspaces are the
+ * OHEM ones. All of these reject a bad shape, zoom, option or null output before any CUDA call. */
+long long semseg_upsample_ce_weighted_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_ce_weighted_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                    int Ho, int Wo, int zoom, int ignore_index, const float* class_weight,
+                                    float label_smoothing, float* workspace, float* loss_out, int64_t* argmax,
+                                    float* lse, void* stream);
+long long semseg_upsample_ce_weighted_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_weighted_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                    int Ho, int Wo, int zoom, int ignore_index, const float* class_weight,
+                                    float label_smoothing, const float* lse, const float* loss_info,
+                                    const float* grad_out, float* workspace, float* dlogits, void* stream);
+int semseg_upsample_ce_ohem_weighted_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                         const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                         float thresh, int min_kept, const float* class_weight, float* workspace,
+                                         float* loss_out, int64_t* argmax, float* lse, float* pt, float* nll,
+                                         float* thr, void* stream);
+int semseg_upsample_ce_ohem_weighted_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                         const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                         const float* class_weight, const float* lse, const float* pt,
+                                         const float* thr, const float* loss_info, const float* grad_out,
+                                         float* workspace, float* dlogits, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sliding-window evaluation after the network (semseg_b200/inference.py, exact=False). No tensor cores, no atomics.

@@ -173,6 +173,18 @@ SIGNATURES = {
     "semseg_upsample_ce_ohem_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_ohem_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_weighted_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_weighted_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
+                                                c_int, c_vp, c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_weighted_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_weighted_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
+                                                c_int, c_vp, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_ohem_weighted_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,
+                                                     c_int, c_int, c_f, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                     c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_ohem_weighted_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,
+                                                     c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                     c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
     "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_vp, c_vp]),

@@ -22,6 +22,15 @@
 // (kOhem): the forward also writes each pixel's target probability p_t and nll and leaves the loss to a masked reduce;
 // a radix select over the p_t bit patterns finds the k-th smallest p_t on the device; the backward treats every pixel
 // with p_t >= threshold as ignored. The kOhem = false instances are the plain cross-entropy kernels, unchanged.
+//
+// Class weights and label smoothing (nn.CrossEntropyLoss(weight, label_smoothing)) are a second compile-time flag,
+// kWeighted. With w the class weights (all ones when none are given), W = sum_c w_c, eps the smoothing and a valid
+// pixel's lse = logsumexp_c v_c:
+//   loss_pix = (1-eps) w_t (lse - v_t) + (eps/C) sum_c w_c (lse - v_c),   loss = sum loss_pix / D,   D = sum w_t
+//   dloss_pix/dv_c = p_c ((1-eps) w_t + (eps/C) W) - [c = t] (1-eps) w_t - (eps/C) w_c
+// and loss 0 with an exactly zero gradient when D = 0. Weighted OHEM (kOhem and kWeighted) writes nll = w_t (lse - v_t)
+// and scales the pixel's gradient by w_t; its selection and mean over the kept pixels are the OHEM ones. The
+// kWeighted = false instances are unchanged.
 #include "host_common.h"
 
 namespace sb {
@@ -59,6 +68,19 @@ __device__ __forceinline__ float row_lerp(float top, float bot, int r) {
   }
 }
 
+// The C class weights (1 where class_weight is NULL) into s_w[0..C-1] and, after the caller's next __syncthreads(),
+// their sum W in s_w[C]: warp 0 sums in a fixed order, so every CTA gets the same bits. Needs blockDim.x >= 32.
+__device__ __forceinline__ void stage_class_weights(const float* __restrict__ class_weight, int C, float* s_w) {
+  for (int c = threadIdx.x; c < C; c += blockDim.x) s_w[c] = class_weight ? class_weight[c] : 1.f;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float a = 0.f;
+    for (int c = threadIdx.x; c < C; c += 32) a += s_w[c];
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (threadIdx.x == 0) s_w[C] = a;
+  }
+}
+
 // One CTA per (128 output columns, low-res interval row i0, image); a thread owns one output column and the Z
 // output rows of the interval. Per class the horizontal interpolation of the two node rows (top, bot) is done once
 // and shared by the Z rows (v = l0h*top + l1h*bot with compile-time row weights), so at Z = 8 a pixel-class costs ~5
@@ -66,14 +88,19 @@ __device__ __forceinline__ float row_lerp(float top, float bot, int r) {
 // sum of exp2 — one MUFU per pixel-class, no rescaling branches.
 // kOhem: no loss partials; per pixel p_t = exp(v_t - lse) and nll = lse - v_t instead (kInvalidPt / 0 where the target
 // is ignored or out of range). The OHEM-only arguments come last, so the plain instances keep their parameter layout.
-template <int Z, bool kOhem>
+// kWeighted without kOhem: the partials are (sum of loss_pix, sum of w_t); the class weights and W are staged after the
+// node rows and the second class pass also sums w_c (m - v_c) per output row (m: the row's max, so no term cancels).
+// kWeighted with kOhem: nll = w_t (lse - v_t). The weighted-only arguments come after the OHEM ones.
+template <int Z, bool kOhem, bool kWeighted = false>
 __global__ void __launch_bounds__(kFwdCols)
 upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
                        const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                        float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out,
-                       float* __restrict__ pt_out, float* __restrict__ nll_out) {
+                       float* __restrict__ pt_out, float* __restrict__ nll_out,
+                       const float* __restrict__ class_weight = nullptr, float smoothing = 0.f) {
   using G = Zoom<Z>;
   constexpr int kFwdNodes = G::kNodes;
+  constexpr bool kWeightedCE = kWeighted && !kOhem;
   extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs]; Cs odd -> the node columns a warp reads hit distinct banks
   __shared__ float red_loss[kFwdCols / 32];
   __shared__ float red_cnt[kFwdCols / 32];
@@ -82,6 +109,7 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
   const int j_base = x0 >> G::kShift;
   const int nj = min(kFwdNodes, w - j_base);
   const int tid = threadIdx.x;
+  float* s_w = S + G::kNodeRows * kFwdNodes * Cs;  // kWeightedCE: [C] class weights, then W
   for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
     const int c = idx % C;
     const int node = idx / C;
@@ -89,6 +117,7 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
     S[(rr * kFwdNodes + jj) * Cs + c] =
         logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
   }
+  if constexpr (kWeightedCE) stage_class_weights(class_weight, C, s_w);
   __syncthreads();
   float loss = 0.f, cnt = 0.f;
   const int x = x0 + tid;
@@ -123,9 +152,12 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
         }
       }
     }
-    float m2[Z];
+    float m2[Z], sw[Z];  // sw: kWeightedCE, sum_c w_c (m - v_c)
 #pragma unroll
-    for (int r = 0; r < Z; ++r) m2[r] = m[r] * kLog2e;
+    for (int r = 0; r < Z; ++r) {
+      m2[r] = m[r] * kLog2e;
+      sw[r] = 0.f;
+    }
 #pragma unroll 2
     for (int c = 0; c < C; ++c) {
       const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
@@ -134,6 +166,7 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
       for (int r = 0; r < Z; ++r) {
         const float v = row_lerp<Z>(top, bot, r);
         sum[r] += ex2_approx(fmaf(v, kLog2e, -m2[r]));
+        if constexpr (kWeightedCE) sw[r] = fmaf(s_w[c], m[r] - v, sw[r]);
       }
     }
 #pragma unroll
@@ -151,7 +184,14 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
           const float vt = row_lerp<Z>(top, bot, r);
           if constexpr (kOhem) {
             pt_out[pix] = expf(vt - lse);
-            nll_out[pix] = lse - vt;
+            nll_out[pix] = kWeighted ? (class_weight ? class_weight[tc] : 1.f) * (lse - vt) : lse - vt;
+          } else if constexpr (kWeightedCE) {
+            // sum_c w_c (lse - v_c) = W (lse - m) + sum_c w_c (m - v_c): two non-negative terms for positive weights.
+            // lse - m rather than a second __logf(sum): lse keeps the plain kernel's bits
+            const float wt = s_w[tc];
+            const float smooth = fmaf(s_w[C], lse - m[r], sw[r]);
+            loss += fmaf((1.f - smoothing) * wt, lse - vt, (smoothing / C) * smooth);
+            cnt += wt;
           } else {
             loss += lse - vt;
             cnt += 1.f;
@@ -188,6 +228,9 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
 }
 
 // loss_out[0] = sum / max(count, 1) (mean over non-ignored pixels), loss_out[1] = count. Fixed summation order.
+// kWeightedMean: the second partial is D = sum of w_t, and loss_out[0] = sum / D, 0 when D = 0 (the sum need not be 0
+// then: label smoothing still scores the pixels of zero-weight classes).
+template <bool kWeightedMean = false>
 __global__ void upsample_ce_reduce_kernel(const float* __restrict__ partial, int nblocks, float* __restrict__ loss_out) {
   __shared__ double sl[256];
   __shared__ double sc[256];
@@ -207,7 +250,11 @@ __global__ void upsample_ce_reduce_kernel(const float* __restrict__ partial, int
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    loss_out[0] = static_cast<float>(sl[0] / (sc[0] > 0.0 ? sc[0] : 1.0));
+    if constexpr (kWeightedMean) {
+      loss_out[0] = sc[0] != 0.0 ? static_cast<float>(sl[0] / sc[0]) : 0.f;
+    } else {
+      loss_out[0] = static_cast<float>(sl[0] / (sc[0] > 0.0 ? sc[0] : 1.0));
+    }
     loss_out[1] = static_cast<float>(sc[0]);
   }
 }
@@ -337,22 +384,42 @@ ohem_masked_sum_kernel(const float* __restrict__ pt, const float* __restrict__ n
 // Phase 2 (cols): dL[i] = gs * (T2[i][0] + T2[i-1][1]).
 // kOhem: a pixel is also ignored when its stored p_t is not below the device threshold, the forward's kept set bit for
 // bit; the cols kernel then divides by the kept count in loss_info[1].
+// kWeighted: the class weights and W are staged after the pixel words (the width limit of the staged rows is the plain
+// one); a thread's own w_c is a register, a pixel's w_t a warp-uniform read of the table. g above becomes
+// p_c ((1-eps) w_t + (eps/C) W) - [c = t] (1-eps) w_t - (eps/C) w_c, or w_t (p_c - [c = t]) with kOhem, and the
+// weighted cols kernel divides by D = loss_info[1] (0 when D = 0).
 struct __align__(8) PixInfo {
   float lse2;  // log-sum-exp * log2(e)
   int t;       // target class, -1 = ignored
 };
 
-template <int Z, bool kOhem>
+// One pixel-class term g of the backward (see above) from p = softmax_c at the pixel.
+template <bool kOhem, bool kWeighted>
+__device__ __forceinline__ float pix_grad(float p, int c, int t, const float* s_w, float k1, float k2, float gam) {
+  if constexpr (!kWeighted) {
+    return p - (c == t ? 1.f : 0.f);
+  } else if constexpr (kOhem) {
+    return s_w[t] * (p - (c == t ? 1.f : 0.f));
+  } else {
+    const float beta = k1 * s_w[t];
+    return fmaf(p, beta + k2, -(c == t ? beta + gam : gam));
+  }
+}
+
+template <int Z, bool kOhem, bool kWeighted = false>
 __global__ void __launch_bounds__(256)
 upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
                             const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                             const float* __restrict__ lse, float* __restrict__ T2, const float* __restrict__ pt,
-                            const float* __restrict__ thr) {
+                            const float* __restrict__ thr, const float* __restrict__ class_weight = nullptr,
+                            float smoothing = 0.f) {
   using G = Zoom<Z>;
   extern __shared__ PixInfo s_pix[];  // [Z][Wo]
   const int i0 = blockIdx.x, n = blockIdx.y;
   const int i1 = min(i0 + 1, h - 1);
   const int rows = min(Z, Ho - Z * i0);
+  float* s_w = reinterpret_cast<float*>(s_pix + Z * Wo);   // kWeighted: [C] class weights, then W
+  if constexpr (kWeighted) stage_class_weights(class_weight, C, s_w);
   float thr_v = 0.f;
   if constexpr (kOhem) thr_v = thr[0];
   for (int r = 0; r < rows; ++r) {
@@ -371,6 +438,12 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
   __syncthreads();
   const int c = threadIdx.x;
   if (c >= C) return;
+  float k1 = 0.f, k2 = 0.f, gam = 0.f;  // kWeighted, not kOhem: 1-eps, (eps/C) W, (eps/C) w_c
+  if constexpr (kWeighted && !kOhem) {
+    k1 = 1.f - smoothing;
+    k2 = (smoothing / C) * s_w[C];
+    gam = (smoothing / C) * s_w[c];
+  }
   const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
   const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
   float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
@@ -398,7 +471,8 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
           const PixInfo pi = s_pix[r * Wo + xb + k];
           if (pi.t < 0) continue;  // warp-uniform
           const float v = row_lerp<Z>(top, bot, r);
-          const float g = ex2_approx(fmaf(v, kLog2e, -pi.lse2)) - (c == pi.t ? 1.f : 0.f);
+          const float g =
+              pix_grad<kOhem, kWeighted>(ex2_approx(fmaf(v, kLog2e, -pi.lse2)), c, pi.t, s_w, k1, k2, gam);
           g0 = fmaf(1.f - G::kStep * r, g, g0);
           g1 = fmaf(G::kStep * r, g, g1);
         }
@@ -418,7 +492,8 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
           if (pi.t < 0) continue;
           const float l1h = G::kStep * r, l0h = 1.f - l1h;
           const float v = l0h * top + l1h * bot;
-          const float g = ex2_approx(fmaf(v, kLog2e, -pi.lse2)) - (c == pi.t ? 1.f : 0.f);
+          const float g =
+              pix_grad<kOhem, kWeighted>(ex2_approx(fmaf(v, kLog2e, -pi.lse2)), c, pi.t, s_w, k1, k2, gam);
           g0 = fmaf(l0h, g, g0);
           g1 = fmaf(l1h, g, g1);
         }
@@ -437,13 +512,19 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
   }
 }
 
+template <bool kWeightedMean = false>
 __global__ void __launch_bounds__(256)
 upsample_ce_bwd_cols_kernel(const float* __restrict__ T2, int N, int h, int w, int C,
                             const float* __restrict__ loss_info, const float* __restrict__ grad_out,
                             float* __restrict__ dlogits) {
   const int i = blockIdx.x, n = blockIdx.y;
   const float cntv = loss_info[1];
-  const float gs = grad_out[0] / (cntv > 0.f ? cntv : 1.f);
+  float gs;
+  if constexpr (kWeightedMean) {
+    gs = cntv != 0.f ? grad_out[0] / cntv : 0.f;   // D = sum of w_t; T2 need not be 0 when D = 0
+  } else {
+    gs = grad_out[0] / (cntv > 0.f ? cntv : 1.f);
+  }
   const int wc = w * C;
   const float* own = T2 + ((static_cast<size_t>(n) * h + i) * 2 + 0) * wc;                 // interval i, top slot
   const float* prev = i > 0 ? T2 + ((static_cast<size_t>(n) * h + (i - 1)) * 2 + 1) * wc : nullptr;  // interval i-1, bottom
@@ -491,35 +572,40 @@ constexpr size_t kBwdSmemMax = 160 * 1024;   // staged (lse, target) words of th
 
 static int fwd_ctas(int N, int h, int Wo) { return cdiv(Wo, kFwdCols) * h * N; }
 
-template <int Z, bool kOhem>
+template <int Z, bool kOhem, bool kWeighted = false>
 static int launch_fwd_kernel(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
                              int Wo, int ignore_index, float* partial, int64_t* argmax, float* lse, float* pt,
-                             float* nll, cudaStream_t stream) {
+                             float* nll, cudaStream_t stream, const float* class_weight = nullptr,
+                             float smoothing = 0.f) {
   dim3 grid(cdiv(Wo, kFwdCols), h, N);
   const int Cs = C | 1;
+  // the weighted cross-entropy form stages the C class weights and W after the node rows
+  constexpr size_t kWeightFloats = kWeighted && !kOhem ? kMaxClasses + 1 : 0;
+  const size_t weight_floats = kWeighted && !kOhem ? C + 1 : 0;
   // at most 2 * 65 * 257 floats (Z = 2, 256 classes); above 48 KB only at Z <= 4 (Z = 1 and 2 with 150 classes: 78 KB)
-  constexpr size_t kMaxSmem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
-  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  constexpr size_t kMaxSmem =
+      (static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) + kWeightFloats) * sizeof(float);
+  const size_t smem = (static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs + weight_floats) * sizeof(float);
   static std::atomic<bool> attr_set[64];
   if (smem > kSmemDefault) {
-    int r = opt_in_smem(upsample_ce_fwd_kernel<Z, kOhem>, attr_set, static_cast<int>(kMaxSmem));
+    int r = opt_in_smem(upsample_ce_fwd_kernel<Z, kOhem, kWeighted>, attr_set, static_cast<int>(kMaxSmem));
     if (r) return r;
   }
-  upsample_ce_fwd_kernel<Z, kOhem><<<grid, kFwdCols, smem, stream>>>(
+  upsample_ce_fwd_kernel<Z, kOhem, kWeighted><<<grid, kFwdCols, smem, stream>>>(
       logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, partial,
-      reinterpret_cast<long long*>(argmax), lse, pt, nll);
+      reinterpret_cast<long long*>(argmax), lse, pt, nll, class_weight, smoothing);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
 
-template <int Z>
+template <int Z, bool kWeighted = false>
 static int launch_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
                       int ignore_index, float* workspace, float* loss_out, int64_t* argmax, float* lse,
-                      cudaStream_t stream) {
-  int r = launch_fwd_kernel<Z, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, argmax, lse,
-                                      nullptr, nullptr, stream);
+                      cudaStream_t stream, const float* class_weight = nullptr, float smoothing = 0.f) {
+  int r = launch_fwd_kernel<Z, false, kWeighted>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace,
+                                                 argmax, lse, nullptr, nullptr, stream, class_weight, smoothing);
   if (r) return r;
-  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
+  upsample_ce_reduce_kernel<kWeighted><<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
@@ -528,16 +614,17 @@ static long long ohem_hist_ctas(long long M) { return std::min<long long>((M + k
 static long long ohem_mask_ctas(long long M) { return (M + kMaskPix - 1) / kMaskPix; }
 
 // Workspace: kSelWords selection words, then (loss, count) per masked-reduce CTA.
-template <int Z>
+template <int Z, bool kWeighted = false>
 static int launch_ohem_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
                            int Wo, int ignore_index, float thresh, int min_kept, float* workspace, float* loss_out,
-                           int64_t* argmax, float* lse, float* pt, float* nll, float* thr, cudaStream_t stream) {
+                           int64_t* argmax, float* lse, float* pt, float* nll, float* thr, cudaStream_t stream,
+                           const float* class_weight = nullptr) {
   const long long M = static_cast<long long>(N) * Ho * Wo;
   unsigned* sel = reinterpret_cast<unsigned*>(workspace);
   float* partial = workspace + kSelWords;
   SB_CUDA(cudaMemsetAsync(sel, 0, kSelWords * sizeof(unsigned), stream));
-  int r = launch_fwd_kernel<Z, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, nullptr, argmax, lse, pt,
-                                     nll, stream);
+  int r = launch_fwd_kernel<Z, true, kWeighted>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, nullptr,
+                                                argmax, lse, pt, nll, stream, class_weight);
   if (r) return r;
   const int hist_ctas = static_cast<int>(ohem_hist_ctas(M));
   for (int pass = 0; pass < 4; ++pass) {
@@ -554,23 +641,29 @@ static int launch_ohem_fwd(const float* logits, int pitch, int N, int h, int w, 
   return SEMSEG_OK;
 }
 
-template <int Z, bool kOhem>
+template <int Z, bool kOhem, bool kWeighted = false>
 static int launch_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho, int Wo,
                       int ignore_index, const float* lse, const float* loss_info, const float* grad_out,
-                      float* workspace, float* dlogits, const float* pt, const float* thr, cudaStream_t stream) {
+                      float* workspace, float* dlogits, const float* pt, const float* thr, cudaStream_t stream,
+                      const float* class_weight = nullptr, float smoothing = 0.f) {
   const int threads = (C + 31) / 32 * 32;
   const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(PixInfo);
   SB_CHECK_ARG(smem <= kBwdSmemMax, "upsample_ce_bwd: output width %d too large for the staged rows", Wo);
+  // the weighted forms stage the class weights and W after the pixel words: the width limit stays the plain one
+  constexpr size_t kWeightBytes = kWeighted ? (kMaxClasses + 1) * sizeof(float) : 0;
+  const size_t smem_all = smem + (kWeighted ? (C + 1) * sizeof(float) : 0);
   static std::atomic<bool> attr_set[64];
-  if (smem > kSmemDefault) {
-    int r = opt_in_smem(upsample_ce_bwd_rows_kernel<Z, kOhem>, attr_set, static_cast<int>(kBwdSmemMax));
+  if (smem_all > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_bwd_rows_kernel<Z, kOhem, kWeighted>, attr_set,
+                        static_cast<int>(kBwdSmemMax + kWeightBytes));
     if (r) return r;
   }
-  upsample_ce_bwd_rows_kernel<Z, kOhem><<<dim3(h, N), threads, smem, stream>>>(
+  upsample_ce_bwd_rows_kernel<Z, kOhem, kWeighted><<<dim3(h, N), threads, smem_all, stream>>>(
       logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, workspace, pt,
-      thr);
+      thr, class_weight, smoothing);
   SB_LAUNCHED();
-  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out, dlogits);
+  upsample_ce_bwd_cols_kernel<kWeighted && !kOhem><<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info,
+                                                                                  grad_out, dlogits);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
@@ -682,6 +775,118 @@ extern "C" int semseg_upsample_ce_ohem_bwd(const float* logits, int pitch, int N
                                        grad_out, workspace, dlogits, pt, thr, stream);
     default: return launch_bwd<8, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
                                         grad_out, workspace, dlogits, pt, thr, stream);
+  }
+}
+
+// Class-weighted and label-smoothed cross-entropy at zoom factor `zoom`: the kWeighted instances. class_weight NULL =
+// all ones.
+static int check_smoothing(float label_smoothing) {
+  SB_CHECK_ARG(label_smoothing >= 0.f && label_smoothing <= 1.f,
+               "upsample_ce_weighted: label_smoothing %g is not in [0, 1]", label_smoothing);
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_weighted_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  return semseg_upsample_ce_zoom_workspace_floats(N, Ho, Wo, zoom);
+}
+
+extern "C" int semseg_upsample_ce_weighted_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                               const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                               const float* class_weight, float label_smoothing, float* workspace,
+                                               float* loss_out, int64_t* argmax, float* lse, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_smoothing(label_smoothing);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse, "upsample_ce_weighted_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_fwd<1, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                       argmax, lse, stream, class_weight, label_smoothing);
+    case 2: return launch_fwd<2, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                       argmax, lse, stream, class_weight, label_smoothing);
+    case 4: return launch_fwd<4, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                       argmax, lse, stream, class_weight, label_smoothing);
+    default: return launch_fwd<8, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                        argmax, lse, stream, class_weight, label_smoothing);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_weighted_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_ce_weighted_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                               const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                               const float* class_weight, float label_smoothing, const float* lse,
+                                               const float* loss_info, const float* grad_out, float* workspace,
+                                               float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_smoothing(label_smoothing);
+  if (r) return r;
+  SB_CHECK_ARG(lse && loss_info && grad_out && dlogits && workspace, "upsample_ce_weighted_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_bwd<1, false, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                              grad_out, workspace, dlogits, nullptr, nullptr, stream, class_weight,
+                                              label_smoothing);
+    case 2: return launch_bwd<2, false, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                              grad_out, workspace, dlogits, nullptr, nullptr, stream, class_weight,
+                                              label_smoothing);
+    case 4: return launch_bwd<4, false, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                              grad_out, workspace, dlogits, nullptr, nullptr, stream, class_weight,
+                                              label_smoothing);
+    default: return launch_bwd<8, false, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse,
+                                               loss_info, grad_out, workspace, dlogits, nullptr, nullptr, stream,
+                                               class_weight, label_smoothing);
+  }
+}
+
+// Weighted OHEM: the OHEM entry points with nll = w_t (lse - v_t) and each kept pixel's gradient scaled by w_t. The
+// workspaces are the OHEM ones.
+extern "C" int semseg_upsample_ce_ohem_weighted_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                                    const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                                    float thresh, int min_kept, const float* class_weight,
+                                                    float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                                    float* pt, float* nll, float* thr, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_ohem(thresh, min_kept);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && pt && nll && thr, "upsample_ce_ohem_weighted_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_ohem_fwd<1, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                            workspace, loss_out, argmax, lse, pt, nll, thr, stream, class_weight);
+    case 2: return launch_ohem_fwd<2, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                            workspace, loss_out, argmax, lse, pt, nll, thr, stream, class_weight);
+    case 4: return launch_ohem_fwd<4, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                            workspace, loss_out, argmax, lse, pt, nll, thr, stream, class_weight);
+    default: return launch_ohem_fwd<8, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, thresh, min_kept,
+                                             workspace, loss_out, argmax, lse, pt, nll, thr, stream, class_weight);
+  }
+}
+
+extern "C" int semseg_upsample_ce_ohem_weighted_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                                    const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                                    const float* class_weight, const float* lse, const float* pt,
+                                                    const float* thr, const float* loss_info, const float* grad_out,
+                                                    float* workspace, float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  SB_CHECK_ARG(lse && pt && thr && loss_info && grad_out && dlogits && workspace,
+               "upsample_ce_ohem_weighted_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_bwd<1, true, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                             grad_out, workspace, dlogits, pt, thr, stream, class_weight);
+    case 2: return launch_bwd<2, true, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                             grad_out, workspace, dlogits, pt, thr, stream, class_weight);
+    case 4: return launch_bwd<4, true, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                             grad_out, workspace, dlogits, pt, thr, stream, class_weight);
+    default: return launch_bwd<8, true, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
+                                              grad_out, workspace, dlogits, pt, thr, stream, class_weight);
   }
 }
 

@@ -538,35 +538,77 @@ class _UpsampleCE(torch.autograd.Function):
         return ops.upsample_ce_bwd(logits, target, ctx.ignore_index, lse, info, grad_loss, zoom=ctx.zoom), None, None, None
 
 
-class _UpsampleCEOhem(torch.autograd.Function):
-    """The fused tail with the OHEM cross-entropy of losses.OhemCrossEntropyLoss: the forward also keeps each pixel's
-    p_t and the device threshold, and the backward trains exactly the pixels the forward kept."""
+class _UpsampleCEWeighted(torch.autograd.Function):
+    """The fused tail with nn.CrossEntropyLoss(weight, label_smoothing): loss = sum of the valid pixels' smoothed,
+    weighted losses / D, D = sum of their target weights; 0 with a zero gradient when D = 0. The class weights are
+    read on the device at every launch (a CUDA-graph replay sees in-place edits) and get no gradient, as in torch."""
 
     @staticmethod
-    def forward(ctx, logits, target, ignore_index, zoom, thresh, min_kept):
+    def forward(ctx, logits, target, ignore_index, zoom, weight, label_smoothing):
+        info, amax, lse = ops.upsample_ce_weighted_fwd(logits, target, ignore_index, weight, label_smoothing,
+                                                       zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, info, weight)
+        ctx.ignore_index, ctx.zoom, ctx.label_smoothing = ignore_index, zoom, label_smoothing
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, info, weight = ctx.saved_tensors
+        dl = ops.upsample_ce_weighted_bwd(logits, target, ctx.ignore_index, weight, ctx.label_smoothing, lse, info,
+                                          grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None
+
+
+class _UpsampleCEOhem(torch.autograd.Function):
+    """The fused tail with the OHEM cross-entropy of losses.OhemCrossEntropyLoss: the forward also keeps each pixel's
+    p_t and the device threshold, and the backward trains exactly the pixels the forward kept. With class weights the
+    loss is the mean of w_t * nll over the kept pixels (the selection stays unweighted)."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, thresh, min_kept, weight=None):
         info, amax, lse, pt, _nll, thr = ops.upsample_ce_ohem_fwd(logits, target, ignore_index, thresh, min_kept,
-                                                                  zoom=zoom)
-        ctx.save_for_backward(logits, target, lse, pt, thr, info)
+                                                                  zoom=zoom, weight=weight)
+        ctx.save_for_backward(logits, target, lse, pt, thr, info, weight)
         ctx.ignore_index, ctx.zoom = ignore_index, zoom
         ctx.mark_non_differentiable(amax)
         return info[0], amax
 
     @staticmethod
     def backward(ctx, grad_loss, _grad_amax):
-        logits, target, lse, pt, thr, info = ctx.saved_tensors
-        dl = ops.upsample_ce_ohem_bwd(logits, target, ctx.ignore_index, lse, pt, thr, info, grad_loss, zoom=ctx.zoom)
-        return dl, None, None, None, None, None
+        logits, target, lse, pt, thr, info, weight = ctx.saved_tensors
+        dl = ops.upsample_ce_ohem_bwd(logits, target, ctx.ignore_index, lse, pt, thr, info, grad_loss, zoom=ctx.zoom,
+                                      weight=weight)
+        return dl, None, None, None, None, None, None
+
+
+def _class_weight_supported(weight, target, classes):
+    """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
+    length `classes` when that is known)."""
+    if weight is None:
+        return True
+    return (torch.is_tensor(weight) and weight.dtype == torch.float32 and weight.dim() == 1 and weight.is_contiguous()
+            and weight.is_cuda and weight.device == target.device and (classes is None or weight.numel() == classes))
 
 
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
-    """The fused kernel implements exactly nn.CrossEntropyLoss(ignore_index=k) with default options and
-    losses.OhemCrossEntropyLoss, at every zoom factor of the model (1, 2, 4, 8) with the target at the zoomed size
-    zoom*(h'-1)+1 of the 1/8-resolution logits.
+    """The fused kernel implements exactly nn.CrossEntropyLoss(weight, ignore_index=k, reduction='mean',
+    label_smoothing) and losses.OhemCrossEntropyLoss (with or without class weights), at every zoom factor of the model
+    (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits. The weighted / smoothed
+    forms need the target on a CUDA device and class weights as a contiguous fp32 [classes] tensor on that device; any
+    other weight, another reduction, and any subclass keep the ATen tail.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
-    plain_ce = (type(criterion) is nn.CrossEntropyLoss and criterion.weight is None and criterion.reduction == 'mean'
-                and getattr(criterion, 'label_smoothing', 0.0) == 0.0)
-    if not ((plain_ce or type(criterion) is losses.OhemCrossEntropyLoss) and zoom_factor in (1, 2, 4, 8)
+    if type(criterion) is nn.CrossEntropyLoss:
+        eps = getattr(criterion, 'label_smoothing', 0.0)
+        plain = criterion.weight is None and eps == 0.0
+        ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
+              (plain or (target is not None and target.is_cuda)))
+    else:
+        ok = type(criterion) is losses.OhemCrossEntropyLoss
+    if not (ok and zoom_factor in (1, 2, 4, 8)
             and target is not None and target.dtype == torch.int64 and target.dim() == 3):
+        return False
+    if not _class_weight_supported(criterion.weight, target, None if logits is None else logits.shape[-1]):
         return False
     if logits is None:
         h, w = (x_size[2] - 1) // 8 + 1, (x_size[3] - 1) // 8 + 1      # the network's output stride is 8
@@ -579,10 +621,19 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
 
 def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None):
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
-    losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index)."""
+    losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
+    weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean.
+    The default criterion runs the plain kernels."""
     if isinstance(criterion, losses.OhemCrossEntropyLoss):
+        if criterion.weight is None:
+            return _UpsampleCEOhem.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                         criterion.thresh, criterion.min_kept)
         return _UpsampleCEOhem.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.thresh,
-                                     criterion.min_kept)
+                                     criterion.min_kept, criterion.weight)
+    if isinstance(criterion, nn.CrossEntropyLoss) and (criterion.weight is not None or
+                                                       getattr(criterion, 'label_smoothing', 0.0) != 0.0):
+        return _UpsampleCEWeighted.apply(logits, target.contiguous(), ignore_index, int(zoom), criterion.weight,
+                                         float(criterion.label_smoothing))
     return _UpsampleCE.apply(logits, target.contiguous(), ignore_index, int(zoom))
 
 

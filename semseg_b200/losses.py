@@ -24,9 +24,15 @@ class OhemCrossEntropyLoss(nn.Module):
     nothing would be nan). The selection is exact: the k-th value is found by a radix select on the device, without a
     host synchronisation. Under DistributedDataParallel each rank mines its own pixels.
 
+    `weight` (a 1-D float tensor of one weight per class, as nn.CrossEntropyLoss's) weights each kept pixel's nll by its
+    target class's weight, as HRNet's OhemCrossEntropy does: the selection on p_t is unchanged and unweighted, and the
+    loss is the plain mean of w_t * nll over the kept pixels (not divided by the sum of the weights). It is registered
+    as a buffer like nn.CrossEntropyLoss's (moved by .cuda() / .to(), saved in the state_dict); without it there is no
+    buffer. The native tail needs it contiguous fp32 on the logits' device.
+
     CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
 
-    def __init__(self, ignore_index=255, thresh=0.7, min_kept=100000):
+    def __init__(self, ignore_index=255, thresh=0.7, min_kept=100000, weight=None):
         super(OhemCrossEntropyLoss, self).__init__()
         if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
             raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
@@ -37,10 +43,17 @@ class OhemCrossEntropyLoss(nn.Module):
             raise ValueError("thresh must lie in [0, 1], got %r" % thresh)
         if not 0 <= min_kept < 2 ** 31:
             raise ValueError("min_kept must be a non-negative 32-bit int, got %r" % min_kept)
+        if weight is not None:
+            if not torch.is_tensor(weight) or not weight.is_floating_point():
+                raise TypeError("weight must be a floating-point tensor or None, got %r" % (weight,))
+            if weight.dim() != 1 or weight.numel() == 0:
+                raise ValueError("weight must be 1-D with one entry per class, got shape %s" % (tuple(weight.shape),))
         self.ignore_index, self.thresh, self.min_kept = ignore_index, thresh, min_kept
+        self.register_buffer("weight", weight)
 
     def extra_repr(self):
-        return "ignore_index=%d, thresh=%g, min_kept=%d" % (self.ignore_index, self.thresh, self.min_kept)
+        s = "ignore_index=%d, thresh=%g, min_kept=%d" % (self.ignore_index, self.thresh, self.min_kept)
+        return s if self.weight is None else s + ", weight=[%d]" % self.weight.numel()
 
     def forward(self, logits, target):
         from . import functional as SF
@@ -55,5 +68,10 @@ class OhemCrossEntropyLoss(nn.Module):
         if logits.dtype != torch.float32 or target.dtype != torch.int64:
             raise TypeError("OhemCrossEntropyLoss: fp32 logits and int64 target expected, got %s and %s" %
                             (logits.dtype, target.dtype))
+        w = self.weight
+        if w is not None and not (w.numel() == logits.shape[1] and w.dtype == torch.float32 and w.is_contiguous()
+                                  and w.device == logits.device):
+            raise ValueError("OhemCrossEntropyLoss: weight must be contiguous fp32 [%d] on %s (no fallback), got %s "
+                             "[%d] on %s" % (logits.shape[1], logits.device, w.dtype, w.numel(), w.device))
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
         return loss

@@ -697,14 +697,67 @@ def upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_out, zoom=8):
     return dl
 
 
-def upsample_ce_ohem_fwd(logits, target, ignore_index, thresh, min_kept, want_argmax=True, zoom=8):
-    """OHEM cross-entropy on the fused tail (semseg_b200/losses.py states the contract); arguments as upsample_ce_fwd
-    -> (loss_info [2] = (mean nll over the kept pixels, kept count), argmax, lse, p_t, nll, thr [1]). p_t / nll fp32
-    [N,Ho,Wo], p_t = -1 where the pixel is not valid."""
+def _check_class_weight(weight, logits):
+    """A class-weight tensor the weighted tail kernels read: None, or fp32 contiguous [C] on the logits' device."""
+    if weight is None:
+        return
+    c = logits.shape[-1]
+    if not (weight.dtype == torch.float32 and weight.dim() == 1 and weight.is_contiguous() and weight.numel() == c
+            and weight.device == logits.device):
+        raise ValueError("semseg_b200: class weights must be a contiguous fp32 [%d] tensor on %s, got %s %s on %s" %
+                         (c, logits.device, weight.dtype, tuple(weight.shape), weight.device))
+
+
+def upsample_ce_weighted_fwd(logits, target, ignore_index, weight, label_smoothing, want_argmax=True, zoom=8):
+    """Class-weighted, label-smoothed cross-entropy on the fused tail (include/semseg_b200.h states the contract):
+    arguments as upsample_ce_fwd plus `weight` (fp32 [C] or None = all ones) and `label_smoothing` in [0, 1]
+    -> (loss_info [2] = (loss, D = sum of the valid pixels' target weights), argmax, lse)."""
     _require_cuda(logits, target)
     lib = _lib.load()
     assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
     assert target.dtype == torch.int64 and target.is_contiguous()
+    _check_class_weight(weight, logits)
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_weighted_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_weighted_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    info = torch.empty((2,), dtype=torch.float32, device=logits.device)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=logits.device) if want_argmax else None
+    lse = torch.empty((n, ho, wo), dtype=torch.float32, device=logits.device)
+    _lib.check(lib.semseg_upsample_ce_weighted_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                   int(zoom), int(ignore_index), _ptr(weight), float(label_smoothing),
+                                                   _ptr(ws), _ptr(info), _ptr(amax), _ptr(lse), _stream()),
+               "semseg_upsample_ce_weighted_fwd")
+    return info, amax, lse
+
+
+def upsample_ce_weighted_bwd(logits, target, ignore_index, weight, label_smoothing, lse, info, grad_out, zoom=8):
+    lib = _lib.load()
+    _check_class_weight(weight, logits)
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_weighted_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_weighted_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_weighted_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                   int(zoom), int(ignore_index), _ptr(weight), float(label_smoothing),
+                                                   _ptr(lse), _ptr(info), _ptr(g), _ptr(ws), _ptr(dl), _stream()),
+               "semseg_upsample_ce_weighted_bwd")
+    return dl
+
+
+def upsample_ce_ohem_fwd(logits, target, ignore_index, thresh, min_kept, want_argmax=True, zoom=8, weight=None):
+    """OHEM cross-entropy on the fused tail (semseg_b200/losses.py states the contract); arguments as upsample_ce_fwd
+    -> (loss_info [2] = (mean nll over the kept pixels, kept count), argmax, lse, p_t, nll, thr [1]). p_t / nll fp32
+    [N,Ho,Wo], p_t = -1 where the pixel is not valid. `weight` (fp32 [C]): the weighted form, nll = w_t * nll."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    _check_class_weight(weight, logits)
     n, h, w, c = logits.shape
     _, ho, wo = target.shape
     nws = int(lib.semseg_upsample_ce_ohem_workspace_floats(n, ho, wo, int(zoom)))
@@ -715,16 +768,20 @@ def upsample_ce_ohem_fwd(logits, target, ignore_index, thresh, min_kept, want_ar
     thr = torch.empty((1,), dtype=torch.float32, device=dev)
     amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
     lse, pt, nll = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(3))
-    _lib.check(lib.semseg_upsample_ce_ohem_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
-                                               int(zoom), int(ignore_index), float(thresh), int(min_kept), _ptr(ws),
-                                               _ptr(info), _ptr(amax), _ptr(lse), _ptr(pt), _ptr(nll), _ptr(thr),
-                                               _stream()),
-               "semseg_upsample_ce_ohem_fwd")
+    head = (_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo, int(zoom), int(ignore_index),
+            float(thresh), int(min_kept))
+    outs = (_ptr(ws), _ptr(info), _ptr(amax), _ptr(lse), _ptr(pt), _ptr(nll), _ptr(thr), _stream())
+    if weight is None:
+        _lib.check(lib.semseg_upsample_ce_ohem_fwd(*head, *outs), "semseg_upsample_ce_ohem_fwd")
+    else:
+        _lib.check(lib.semseg_upsample_ce_ohem_weighted_fwd(*head, _ptr(weight), *outs),
+                   "semseg_upsample_ce_ohem_weighted_fwd")
     return info, amax, lse, pt, nll, thr
 
 
-def upsample_ce_ohem_bwd(logits, target, ignore_index, lse, pt, thr, info, grad_out, zoom=8):
+def upsample_ce_ohem_bwd(logits, target, ignore_index, lse, pt, thr, info, grad_out, zoom=8, weight=None):
     lib = _lib.load()
+    _check_class_weight(weight, logits)
     n, h, w, c = logits.shape
     _, ho, wo = target.shape
     dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
@@ -732,10 +789,13 @@ def upsample_ce_ohem_bwd(logits, target, ignore_index, lse, pt, thr, info, grad_
     _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_ohem_bwd_workspace_floats")
     ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
     g = grad_out.reshape(1).float().contiguous()
-    _lib.check(lib.semseg_upsample_ce_ohem_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
-                                               int(zoom), int(ignore_index), _ptr(lse), _ptr(pt), _ptr(thr), _ptr(info),
-                                               _ptr(g), _ptr(ws), _ptr(dl), _stream()),
-               "semseg_upsample_ce_ohem_bwd")
+    head = (_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo, int(zoom), int(ignore_index))
+    tail = (_ptr(lse), _ptr(pt), _ptr(thr), _ptr(info), _ptr(g), _ptr(ws), _ptr(dl), _stream())
+    if weight is None:
+        _lib.check(lib.semseg_upsample_ce_ohem_bwd(*head, *tail), "semseg_upsample_ce_ohem_bwd")
+    else:
+        _lib.check(lib.semseg_upsample_ce_ohem_weighted_bwd(*head, _ptr(weight), *tail),
+                   "semseg_upsample_ce_ohem_weighted_bwd")
     return dl
 
 
