@@ -26,6 +26,7 @@
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
  *                               (tool/test.py:163-176) and the per-scale resize into the running total
  *                               (tool/test.py:177, 202).
+ *   - semseg_augment          : tool/train.py:194-212's transform chains (util/transform.py), one launch per batch.
  *
  * Activations are NHWC bf16 in HBM; "pitch" arguments are the distance between consecutive pixels in
  * elements (>= channels; lets a kernel read/write a channel slice of a wider concat buffer).
@@ -517,6 +518,34 @@ typedef struct semseg_sgd_hyper {
 int semseg_sgd_chunk_elems(void);
 int semseg_sgd_multi(const semseg_sgd_item* items_dev, const void* grad_ptrs_dev, int n_items, int n_chunks,
                      const semseg_sgd_hyper* hyper, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Training-batch augmentation: tool/train.py:194-201's RandScale -> RandRotate -> RandomGaussianBlur ->
+ * RandomHorizontalFlip -> Crop -> ToTensor -> Normalize (util/transform.py) with the parameters drawn on the host, in
+ * ONE launch over decoded uint8 images. `data` holds every sample's uint8 RGB HWC image and uint8 HW label at the byte
+ * offsets of its descriptor. Per output pixel: crop/pad -> flip -> 5x5 Gaussian (reflect-101 at the rotated image's
+ * edges) -> cv2's fixed-point warpAffine (AB_BITS 10, border = mean / ignore_label) -> cv2's resize (INTER_LINEAR image,
+ * INTER_NEAREST label) of the source; a stage whose flag is off (or rh,rw == h,w for the resize) is skipped. Nothing at
+ * resized or rotated resolution is written. Outputs: out_img fp32 [N,3,crop_h,crop_w] = (v - mean[c]) / std[c],
+ * out_lab int64 [N,crop_h,crop_w]. desc_host (validated before any CUDA call) and desc_dev hold the same n entries.
+ * Validation mode is the same call with every stage off and centred offsets.
+ */
+typedef struct semseg_augment_desc {
+  long long img_off;   /* byte offset of the uint8 RGB HWC image in data */
+  long long lab_off;   /* byte offset of the uint8 HW label in data */
+  int h, w;            /* source size */
+  int rh, rw;          /* resized size; equal to (h, w) = cv2's copy, no interpolation */
+  double scale_y;      /* 1 / fy: source step per resized pixel (cv2's scale_y) */
+  double scale_x;      /* 1 / fx */
+  double m[6];         /* inverse affine map resized <- rotated, row-major 2x3 (cv2.invertAffineTransform) */
+  int rotate, blur, flip;
+  int pad_top, pad_left;   /* leading padding: max(crop - resized, 0) / 2 */
+  int off_y, off_x;        /* crop offsets in the padded frame */
+  int reserved;
+} semseg_augment_desc;
+int semseg_augment(const void* data, long long data_bytes, const semseg_augment_desc* desc_host,
+                   const semseg_augment_desc* desc_dev, int n, int crop_h, int crop_w, const float* mean3,
+                   const float* std3, int ignore_label, float* out_img, long long* out_lab, void* stream);
 
 #ifdef __cplusplus
 }

@@ -85,6 +85,14 @@ class WgradDesc(ctypes.Structure):
     ]
 
 
+class AugmentDesc(ctypes.Structure):
+    """struct semseg_augment_desc (include/semseg_b200.h): one sample of semseg_augment."""
+    _fields_ = [("img_off", c_ll), ("lab_off", c_ll), ("h", c_i32), ("w", c_i32), ("rh", c_i32), ("rw", c_i32),
+                ("scale_y", ctypes.c_double), ("scale_x", ctypes.c_double), ("m", ctypes.c_double * 6),
+                ("rotate", c_i32), ("blur", c_i32), ("flip", c_i32), ("pad_top", c_i32), ("pad_left", c_i32),
+                ("off_y", c_i32), ("off_x", c_i32), ("reserved", c_i32)]
+
+
 # name -> (restype, argtypes); must list every symbol include/semseg_b200.h declares
 # (tests/test_abi.py parses the header and checks both directions).
 SIGNATURES = {
@@ -189,6 +197,8 @@ SIGNATURES = {
     "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_window_resize_add": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    "semseg_augment": (c_int, [c_vp, c_ll, ctypes.POINTER(AugmentDesc), c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int,
+                               c_vp, c_vp, c_vp]),
 }
 
 _lib = None

@@ -957,3 +957,20 @@ def maxpool3x3s2_bwd(argcode, dy, in_shape):
     _lib.check(lib.semseg_maxpool3x3s2_bwd(_ptr(argcode), _ptr(dy), _lo(dy), _ptr(dx), _lo(dx), n, h, w, c,
                                            _stream()), "semseg_maxpool3x3s2_bwd")
     return dx
+
+
+# ------------------------------------------------------------------------------------------------ batch augmentation
+def augment(data, descs, descs_dev, crop_h, crop_w, mean, std, ignore_label):
+    """One semseg_augment launch. `data`: uint8 CUDA buffer of every sample's image and label; `descs`: ctypes array of
+    AugmentDesc (validated on the host); `descs_dev`: the same bytes on the device. -> (fp32 [N,3,ch,cw], int64
+    [N,ch,cw])."""
+    _require_cuda(data, descs_dev)
+    lib = _lib.load()
+    assert data.dtype == torch.uint8 and data.is_contiguous()
+    n = len(descs)
+    img = torch.empty((n, 3, crop_h, crop_w), dtype=torch.float32, device=data.device)
+    lab = torch.empty((n, crop_h, crop_w), dtype=torch.int64, device=data.device)
+    m3, s3 = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
+    _lib.check(lib.semseg_augment(_ptr(data), data.numel(), descs, _ptr(descs_dev), n, crop_h, crop_w, m3, s3,
+                                  ignore_label, _ptr(img), _ptr(lab), _stream()), "semseg_augment")
+    return img, lab
