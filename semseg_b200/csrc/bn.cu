@@ -3,6 +3,8 @@
 // formula in a fixed order, so results are run-to-run deterministic.
 // Mirrors nn.BatchNorm2d / nn.SyncBatchNorm + ReLU + residual add as used at model/resnet.py:77-92
 // (biased variance for normalisation, unbiased for running_var, eps 1e-5, momentum 0.1).
+#include <initializer_list>
+
 #include "host_common.h"
 #include "ptx.cuh"
 #include "act.cuh"
@@ -887,6 +889,26 @@ static int fill_peer_args(sb::PeerArgs* pa, void* const* peer_bufs, int world, i
   return SEMSEG_OK;
 }
 
+// An activation operand of the 16-byte vector kernels (act_ldraw / act_st8): hi and lo bases, pitch in elements.
+struct VecAct {
+  const void* hi;
+  const void* lo;
+  int pitch;
+};
+
+// Rejects before launch an operand those kernels would access out of line: a hi or lo base that is not 16-byte aligned
+// (a channel slice starting at a channel that is not a multiple of 8), or a pitch below C (rows that overlap). Operands
+// the kernel does not touch are passed with hi == nullptr and skipped.
+static int check_vec_acts(const char* fn, int C, std::initializer_list<VecAct> acts) {
+  for (const VecAct& a : acts) {
+    if (!a.hi) continue;
+    SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.hi) | reinterpret_cast<uintptr_t>(a.lo)) & 15) == 0,
+                 "%s: activation base %p (lo %p) is not 16-byte aligned", fn, a.hi, a.lo);
+    SB_CHECK_ARG(a.pitch >= C, "%s: pitch %d is smaller than C = %d", fn, a.pitch, C);
+  }
+  return SEMSEG_OK;
+}
+
 extern "C" int semseg_bn_merge_partials(const float* stats_partial, int rows, int C, float* out_stats, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SB_CHECK_ARG(stats_partial && out_stats && rows > 0 && C > 0, "bn_merge_partials: bad args");
@@ -947,6 +969,9 @@ extern "C" int semseg_bn_apply(const void* x, const void* x_lo, int x_pitch, con
   const bool split = x_lo != nullptr;
   SB_CHECK_ARG((y_lo != nullptr) == split && (!residual || (residual_lo != nullptr) == split),
                "bn_apply: all tensors must use the same storage form (plain or split)");
+  if (const int r = check_vec_acts("bn_apply", C, {{x, x_lo, x_pitch}, {residual, residual_lo, res_pitch},
+                                                   {y, y_lo, y_pitch}}))
+    return r;
   const long long total = static_cast<long long>(M) * (C / 8);
   const int grid = ew_grid_fixed_channels(total, 256, C / 8);
   SB_ACT_DISPATCH(split, bn_apply_kernel<kS><<<grid, 256, 0, stream>>>(
@@ -972,6 +997,9 @@ extern "C" int semseg_bn_bwd_reduce(const void* dy, const void* dy_lo, int dy_pi
   const bool split = dy_lo != nullptr;
   SB_CHECK_ARG((x_lo != nullptr) == split && (!(relu && y) || (y_lo != nullptr) == split),
                "bn_bwd_reduce: all tensors must use the same storage form (plain or split)");
+  if (const int r = check_vec_acts("bn_bwd_reduce", C, {{dy, dy_lo, dy_pitch}, {x, x_lo, x_pitch},
+                                                        {relu ? y : nullptr, y_lo, y_pitch}}))
+    return r;
   sb::PeerArgs pa = {};
   if (peer_bufs) {
     SB_CHECK_ARG(sums_total, "bn_bwd_reduce: the peer exchange needs sums_total");
@@ -1009,6 +1037,10 @@ extern "C" int semseg_bn_bwd_apply(const void* dy, const void* dy_lo, int dy_pit
   SB_CHECK_ARG((x_lo != nullptr) == split && (dx_lo != nullptr) == split &&
                    (!(relu && y) || (y_lo != nullptr) == split) && (!dres || (dres_lo != nullptr) == split),
                "bn_bwd_apply: all tensors must use the same storage form (plain or split)");
+  if (const int r = check_vec_acts("bn_bwd_apply", C, {{dy, dy_lo, dy_pitch}, {x, x_lo, x_pitch},
+                                                       {relu ? y : nullptr, y_lo, y_pitch}, {dx, dx_lo, dx_pitch},
+                                                       {dres, dres_lo, dres_pitch}}))
+    return r;
   const long long total = static_cast<long long>(M) * (C / 8);
   const int grid = ew_grid_fixed_channels(total, 256, C / 8);
   SB_ACT_DISPATCH(split, bn_bwd_apply_kernel<kS><<<grid, 256, 0, stream>>>(
@@ -1044,6 +1076,10 @@ extern "C" int semseg_bn_bwd_frozen(const void* dy, const void* dy_lo, int dy_pi
   SB_CHECK_ARG((d_raw_lo != nullptr) == split && (!use_y || (y_lo != nullptr) == split) &&
                    (!use_raw || (raw_lo != nullptr) == split) && (!dres || (dres_lo != nullptr) == split),
                "bn_bwd_frozen: all tensors must use the same storage form (plain or split)");
+  if (const int r = check_vec_acts("bn_bwd_frozen", C, {{dy, dy_lo, dy_pitch}, {use_y ? y : nullptr, y_lo, y_pitch},
+                                                        {raw, raw_lo, raw_pitch}, {d_raw, d_raw_lo, d_raw_pitch},
+                                                        {dres, dres_lo, dres_pitch}}))
+    return r;
   const int rows = chunk_rows(M);
   const int chunks = cdiv(M, rows);
   dim3 grid(cdiv(C, 64), chunks);
@@ -1072,6 +1108,8 @@ extern "C" int semseg_add_act(const void* a, const void* a_lo, int a_pitch, cons
   const bool split = a_lo != nullptr;
   SB_CHECK_ARG((b_lo != nullptr) == split && (out_lo != nullptr) == split,
                "add_act: all tensors must use the same storage form (plain or split)");
+  if (const int r = check_vec_acts("add_act", C, {{a, a_lo, a_pitch}, {b, b_lo, b_pitch}, {out, out_lo, out_pitch}}))
+    return r;
   const long long total = static_cast<long long>(M) * (C / 8);
   SB_ACT_DISPATCH(split, add_act_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                              static_cast<const bf16*>(a), static_cast<const bf16*>(a_lo), a_pitch,
@@ -1088,6 +1126,8 @@ extern "C" int semseg_scale_nc(const void* x, const void* x_lo, int x_pitch, con
                "scale_nc: bad args");
   const bool split = x_lo != nullptr;
   SB_CHECK_ARG((out_lo != nullptr) == split, "scale_nc: input and output must use the same storage form");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(scale) & 15) == 0, "scale_nc: scale %p is not 16-byte aligned", scale);
+  if (const int r = check_vec_acts("scale_nc", C, {{x, x_lo, x_pitch}, {out, out_lo, out_pitch}})) return r;
   const long long total = static_cast<long long>(N) * HW * (C / 8);
   SB_ACT_DISPATCH(split, scale_nc_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                              static_cast<const bf16*>(x), static_cast<const bf16*>(x_lo), x_pitch, scale,
@@ -1135,9 +1175,9 @@ extern "C" int semseg_conv_splitk_finish(const float* partial, int k_slices, lon
 extern "C" int semseg_f32_to_act(const float* in, int in_pitch, void* out, void* out_lo, int out_pitch, long long M,
                                  int C, int Cp, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(in && out && M > 0 && C > 0 && Cp >= C && Cp % 8 == 0 && out_pitch % 8 == 0 && out_pitch >= Cp &&
-                   in_pitch >= C,
+  SB_CHECK_ARG(in && out && M > 0 && C > 0 && Cp >= C && Cp % 8 == 0 && out_pitch % 8 == 0 && in_pitch >= C,
                "f32_to_act: bad args");
+  if (const int r = check_vec_acts("f32_to_act", Cp, {{out, out_lo, out_pitch}})) return r;
   const long long total = M * (Cp / 8);
   SB_ACT_DISPATCH(out_lo != nullptr, f32_to_act_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                                          in, in_pitch, static_cast<bf16*>(out), static_cast<bf16*>(out_lo), out_pitch,
@@ -1151,6 +1191,7 @@ extern "C" int semseg_act_to_f32(const void* in, const void* in_lo, int in_pitch
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SB_CHECK_ARG(in && out && M > 0 && C > 0 && C % 8 == 0 && in_pitch % 8 == 0 && out_pitch >= C,
                "act_to_f32: bad args");
+  if (const int r = check_vec_acts("act_to_f32", C, {{in, in_lo, in_pitch}})) return r;
   const long long total = M * (C / 8);
   SB_ACT_DISPATCH(in_lo != nullptr, act_to_f32_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                                         static_cast<const bf16*>(in), static_cast<const bf16*>(in_lo), in_pitch, out,

@@ -219,7 +219,8 @@ def ratio(out, ref, s, r_out, steps):
     term."""
     err = (out - ref).abs()
     if r_out == R_BF16:
-        half = torch.where(out != 0, torch.exp2(torch.floor(torch.log2(out.abs().clamp_min(1e-300))) - 8), 0.0)
+        # floor(log2|out|) = frexp exponent - 1, exactly (a device log2 may land just below the integer at 2^k)
+        half = torch.where(out != 0, torch.ldexp(torch.ones_like(out), torch.frexp(out)[1] - 9), 0.0)
         err = (err - half).clamp_min(0.0)
         bound = steps * U * s
     else:
