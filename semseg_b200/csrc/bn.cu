@@ -889,26 +889,6 @@ static int fill_peer_args(sb::PeerArgs* pa, void* const* peer_bufs, int world, i
   return SEMSEG_OK;
 }
 
-// An activation operand of the 16-byte vector kernels (act_ldraw / act_st8): hi and lo bases, pitch in elements.
-struct VecAct {
-  const void* hi;
-  const void* lo;
-  int pitch;
-};
-
-// Rejects before launch an operand those kernels would access out of line: a hi or lo base that is not 16-byte aligned
-// (a channel slice starting at a channel that is not a multiple of 8), or a pitch below C (rows that overlap). Operands
-// the kernel does not touch are passed with hi == nullptr and skipped.
-static int check_vec_acts(const char* fn, int C, std::initializer_list<VecAct> acts) {
-  for (const VecAct& a : acts) {
-    if (!a.hi) continue;
-    SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.hi) | reinterpret_cast<uintptr_t>(a.lo)) & 15) == 0,
-                 "%s: activation base %p (lo %p) is not 16-byte aligned", fn, a.hi, a.lo);
-    SB_CHECK_ARG(a.pitch >= C, "%s: pitch %d is smaller than C = %d", fn, a.pitch, C);
-  }
-  return SEMSEG_OK;
-}
-
 extern "C" int semseg_bn_merge_partials(const float* stats_partial, int rows, int C, float* out_stats, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SB_CHECK_ARG(stats_partial && out_stats && rows > 0 && C > 0, "bn_merge_partials: bad args");

@@ -30,6 +30,16 @@ int num_sms() {
   return cached[dev];
 }
 
+int check_vec_acts(const char* fn, int C, std::initializer_list<VecAct> acts, int align) {
+  for (const VecAct& a : acts) {
+    if (!a.hi) continue;
+    SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.hi) | reinterpret_cast<uintptr_t>(a.lo)) & (align - 1)) == 0,
+                 "%s: activation base %p (lo %p) is not %d-byte aligned", fn, a.hi, a.lo, align);
+    SB_CHECK_ARG(a.pitch >= C, "%s: pitch %d is smaller than C = %d", fn, a.pitch, C);
+  }
+  return SEMSEG_OK;
+}
+
 static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
   static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
   static std::once_flag once;

@@ -7,6 +7,7 @@
 #include <stdio.h>
 
 #include <atomic>
+#include <initializer_list>
 
 #include "../../include/semseg_b200.h"
 
@@ -53,5 +54,18 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
 void choose_box(int H, int W, int max_pixels, int* bh, int* bw);
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// An activation operand of a kernel that accesses it in vector pieces (act_ld8 / act_st8, uint4, uint2): hi and lo
+// bases, pitch in elements.
+struct VecAct {
+  const void* hi;
+  const void* lo;
+  int pitch;
+};
+
+// Rejects before launch an operand such a kernel would access out of line: a hi or lo base that is not `align`-byte
+// aligned (16 for 8-channel bf16 vectors: a channel slice starting at a channel that is not a multiple of 8), or a pitch
+// below C (rows that overlap). Operands the kernel does not touch are passed with hi == nullptr and skipped.
+int check_vec_acts(const char* fn, int C, std::initializer_list<VecAct> acts, int align = 16);
 
 }  // namespace sb

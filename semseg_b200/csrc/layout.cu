@@ -326,6 +326,7 @@ extern "C" int semseg_space_to_phases(const void* x, int x_pitch, int N, int H, 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SB_CHECK_ARG(x && xp && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && x_pitch % 8 == 0,
                "space_to_phases: bad args");
+  if (const int r = check_vec_acts("space_to_phases", C, {{x, nullptr, x_pitch}, {xp, nullptr, C}})) return r;
   const int Hh = (H + 1) / 2, Wh = (W + 1) / 2;
   const long long total = 4LL * N * Hh * Wh * (C / 8);
   long long blocks = (total + 255) / 256;
@@ -339,6 +340,7 @@ extern "C" int semseg_space_to_phases(const void* x, int x_pitch, int N, int H, 
 extern "C" int semseg_phases_to_space(const void* xp, int N, int H, int W, int C, void* x, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   SB_CHECK_ARG(x && xp && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "phases_to_space: bad args");
+  if (const int r = check_vec_acts("phases_to_space", C, {{xp, nullptr, C}, {x, nullptr, C}})) return r;
   const int Hh = (H + 1) / 2, Wh = (W + 1) / 2;
   const long long total = static_cast<long long>(N) * H * W * (C / 8);
   long long blocks = (total + 255) / 256;
@@ -354,6 +356,9 @@ extern "C" int semseg_im2col3x3s2(const void* x, int x_pitch, int N, int H, int 
   SB_CHECK_ARG(x && out && N > 0 && H > 0 && W > 0 && Cin >= 1 && Cin <= 3 && x_pitch >= 4 && x_pitch % 4 == 0,
                "im2col3x3s2: needs 1..3 input channels in a pitch that is a multiple of 4 (got Cin=%d pitch=%d)", Cin,
                x_pitch);
+  // one uint2 (4 channels) per input pixel, 16-byte stores of 32 patch values
+  if (const int r = check_vec_acts("im2col3x3s2", Cin, {{x, nullptr, x_pitch}}, 8)) return r;
+  if (const int r = check_vec_acts("im2col3x3s2", 0, {{out, nullptr, 32}})) return r;
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
   const long long total = static_cast<long long>(N) * Ho * Wo;
   long long blocks = (total + 255) / 256;

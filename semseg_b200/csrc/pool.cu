@@ -1,6 +1,7 @@
 // MaxPool2d(kernel 3, stride 2, padding 1) on NHWC bf16 (model/resnet.py:115, used as layer0[9]).
 // Forward: one thread per (output pixel, 8 channels); it also records the window position (0..8) of the arg-max
-// (first maximum in row-major window order, the tie rule of ATen's max_pool2d_with_indices) as one byte per element.
+// (first maximum in row-major window order, the tie rule of ATen's max_pool2d_with_indices; NaN propagates and the last
+// NaN of the window is recorded, as in ATen) as one byte per element.
 // Backward is a deterministic gather: every input pixel checks the (up to four) windows that contain it and sums the
 // dy of those whose recorded arg-max is this pixel. No atomics, every dx element written once.
 #include "host_common.h"
@@ -41,7 +42,9 @@ __global__ void maxpool3x3s2_fwd_kernel(const __nv_bfloat16* __restrict__ x, con
         act_ld8<S>(x, x_lo, ((static_cast<long long>(n) * H + h) * W + w) * C + c0, f);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
-          if (f[q] > m[q] || code[q] == 255u) {  // first maximum in row-major window order (ATen's tie rule)
+          // ATen's rule: the first maximum in row-major window order, but the last NaN (a NaN always replaces the
+          // running maximum; an all -inf window keeps its first in-bounds tap)
+          if (f[q] > m[q] || isnan(f[q]) || code[q] == 255u) {
             m[q] = f[q];
             code[q] = static_cast<unsigned>(kh * 3 + kw);
           }
@@ -108,8 +111,10 @@ using namespace sb;
 extern "C" int semseg_maxpool3x3s2_fwd(const void* x, const void* x_lo, void* y, void* y_lo, void* argcode, int N,
                                        int H, int W, int C, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(x && y && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "maxpool_fwd: bad args");
-  SB_CHECK_ARG((x_lo != nullptr) == (y_lo != nullptr), "maxpool_fwd: input and output must use the same storage form");
+  SB_CHECK_ARG(x && y && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "maxpool3x3s2_fwd: bad args");
+  SB_CHECK_ARG((x_lo != nullptr) == (y_lo != nullptr), "maxpool3x3s2_fwd: input and output must use the same storage form");
+  if (const int r = check_vec_acts("maxpool3x3s2_fwd", C, {{x, x_lo, C}, {y, y_lo, C}})) return r;
+  if (const int r = check_vec_acts("maxpool3x3s2_fwd", C, {{argcode, nullptr, C}}, 8)) return r;  // uint2 stores
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
   const long long total = static_cast<long long>(N) * Ho * Wo * (C / 8);
   typedef __nv_bfloat16 bf16;
@@ -124,8 +129,10 @@ extern "C" int semseg_maxpool3x3s2_fwd(const void* x, const void* x_lo, void* y,
 extern "C" int semseg_maxpool3x3s2_bwd(const void* argcode, const void* dy, const void* dy_lo, void* dx, void* dx_lo,
                                        int N, int H, int W, int C, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(argcode && dy && dx && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "maxpool_bwd: bad args");
-  SB_CHECK_ARG((dy_lo != nullptr) == (dx_lo != nullptr), "maxpool_bwd: dy and dx must use the same storage form");
+  SB_CHECK_ARG(argcode && dy && dx && N > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "maxpool3x3s2_bwd: bad args");
+  SB_CHECK_ARG((dy_lo != nullptr) == (dx_lo != nullptr), "maxpool3x3s2_bwd: dy and dx must use the same storage form");
+  if (const int r = check_vec_acts("maxpool3x3s2_bwd", C, {{dy, dy_lo, C}, {dx, dx_lo, C}})) return r;
+  if (const int r = check_vec_acts("maxpool3x3s2_bwd", C, {{argcode, nullptr, C}}, 8)) return r;  // uint2 loads
   const int Ho = (H + 2 - 3) / 2 + 1, Wo = (W + 2 - 3) / 2 + 1;
   const long long total = static_cast<long long>(N) * H * W * (C / 8);
   typedef __nv_bfloat16 bf16;

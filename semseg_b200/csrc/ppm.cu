@@ -66,8 +66,26 @@ ppm_pool_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __rest
   }
 }
 
-// dx[n,h,w,c] = sum over bins, over cells whose window contains (h,w): dpooled[n,cell,c] / window_size.
-// One warp per pixel: the (cell, 1/window) list of the pixel is derived once, then the lanes sweep the channels.
+// Windows of one bin along one dimension of extent L that contain coordinate x: window i spans [floor(i*L/b),
+// ceil((i+1)*L/b)), both ends non-decreasing in i, so they are the contiguous range [lo, hi]. lo = floor(x*b/L) always
+// contains x (x < (lo+1)*L/b), and so does every later window that starts at or before x. While b <= L a coordinate lies
+// in at most 2 windows; when the bin is larger than the map, in about b/L + 1.
+__device__ __forceinline__ void ppm_window_range(int x, int L, int b, int& lo, int& hi) {
+  lo = (x * b) / L;
+  hi = lo;
+  while (hi + 1 < b && ((hi + 1) * L) / b <= x) ++hi;
+}
+
+__device__ __forceinline__ int ppm_window_size(int i, int L, int b) {
+  return ((i + 1) * L + b - 1) / b - (i * L) / b;
+}
+
+// dx[n,h,w,c] = add[n,h,w,c] + sum over bins, over cells whose window contains (h,w): dpooled[n,cell,c] / window_size,
+// in the fixed order add, bins ascending, ci ascending, cj ascending, one fmaf each with the window's fl(1/size).
+// One warp per pixel: the pixel's windows are the ranges [ci_lo, ci_hi] x [cj_lo, cj_hi] of every bin, derived once;
+// then the lanes sweep the channels. Up to kMaxCells windows (every pixel while no bin is larger than the map) are listed
+// as (cell, 1/size) first, so the channel loop streams through the list and its loads overlap; a pixel with more windows
+// walks the ranges in the channel loop instead, in the same order, so both forms give the same bits.
 template <bool S>
 __global__ void __launch_bounds__(256)
 ppm_pool_bwd_kernel(__nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dx_lo, int pitch,
@@ -76,46 +94,66 @@ ppm_pool_bwd_kernel(__nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ 
   const int lane = threadIdx.x & 31;
   const long long npix = static_cast<long long>(N) * H * W;
   const int groups = C >> 3;
-  constexpr int kMaxCells = 4 * kMaxBins;  // up to 2x2 overlapping windows per bin
+  constexpr int kMaxCells = 4 * kMaxBins;
   for (long long p = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); p < npix;
        p += static_cast<long long>(gridDim.x) * (blockDim.x >> 5)) {
     const int wx = static_cast<int>(p % W);
     const int hh = static_cast<int>((p / W) % H);
     const int n = static_cast<int>(p / (static_cast<long long>(W) * H));
-    const __nv_bfloat16* src[kMaxCells];
-    const __nv_bfloat16* src_lo[kMaxCells];
-    float inv[kMaxCells];
-    int cnt = 0;
+    int4 rng[kMaxBins];  // (ci_lo, ci_hi, cj_lo, cj_hi) per bin
+    int total = 0;
     for (int k = 0; k < bs.nb; ++k) {
-      const int b = bs.b[k];
-      const __nv_bfloat16* dp = static_cast<const __nv_bfloat16*>(bs.ptr[k]) + static_cast<size_t>(n) * b * b * C;
-      const __nv_bfloat16* dp_lo =
-          S ? static_cast<const __nv_bfloat16*>(bs.ptr_lo[k]) + static_cast<size_t>(n) * b * b * C : nullptr;
-      for (int ci = (hh * b) / H; ci < b; ++ci) {
-        const int hs = (ci * H) / b, he = ((ci + 1) * H + b - 1) / b;
-        if (hs > hh) break;
-        if (hh >= he) continue;
-        for (int cj = (wx * b) / W; cj < b; ++cj) {
-          const int ws = (cj * W) / b, we = ((cj + 1) * W + b - 1) / b;
-          if (ws > wx) break;
-          if (wx >= we) continue;
-          if (cnt < kMaxCells) {
-            src[cnt] = dp + static_cast<size_t>(ci * b + cj) * C;
-            src_lo[cnt] = S ? dp_lo + static_cast<size_t>(ci * b + cj) * C : nullptr;
-            inv[cnt] = 1.f / static_cast<float>((he - hs) * (we - ws));
+      ppm_window_range(hh, H, bs.b[k], rng[k].x, rng[k].y);
+      ppm_window_range(wx, W, bs.b[k], rng[k].z, rng[k].w);
+      total += (rng[k].y - rng[k].x + 1) * (rng[k].w - rng[k].z + 1);
+    }
+    if (total <= kMaxCells) {
+      const __nv_bfloat16* src[kMaxCells];
+      const __nv_bfloat16* src_lo[kMaxCells];
+      float inv[kMaxCells];
+      int cnt = 0;
+      for (int k = 0; k < bs.nb; ++k) {
+        const int b = bs.b[k];
+        const size_t base = static_cast<size_t>(n) * b * b * C;
+        for (int ci = rng[k].x; ci <= rng[k].y; ++ci) {
+          for (int cj = rng[k].z; cj <= rng[k].w; ++cj) {
+            const size_t off = base + static_cast<size_t>(ci * b + cj) * C;
+            src[cnt] = static_cast<const __nv_bfloat16*>(bs.ptr[k]) + off;
+            src_lo[cnt] = S ? static_cast<const __nv_bfloat16*>(bs.ptr_lo[k]) + off : nullptr;
+            inv[cnt] = 1.f / static_cast<float>(ppm_window_size(ci, H, b) * ppm_window_size(cj, W, b));
             ++cnt;
           }
         }
       }
+      for (int g = lane; g < groups; g += 32) {
+        float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        if (add) act_ld8<S>(add, add_lo, p * add_pitch + g * 8, acc);  // the other gradient branch of x (identity part of the concat)
+        for (int i = 0; i < cnt; ++i) {
+          float f[8];
+          act_ld8<S>(src[i], src_lo[i], g * 8, f);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) acc[q] = fmaf(f[q], inv[i], acc[q]);
+        }
+        act_st8<S>(dx, dx_lo, p * pitch + g * 8, acc);
+      }
+      continue;
     }
     for (int g = lane; g < groups; g += 32) {
       float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      if (add) act_ld8<S>(add, add_lo, p * add_pitch + g * 8, acc);  // the other gradient branch of x (identity part of the concat)
-      for (int i = 0; i < cnt; ++i) {
-        float f[8];
-        act_ld8<S>(src[i], src_lo[i], g * 8, f);
+      if (add) act_ld8<S>(add, add_lo, p * add_pitch + g * 8, acc);
+      for (int k = 0; k < bs.nb; ++k) {
+        const int b = bs.b[k];
+        const size_t base = static_cast<size_t>(n) * b * b * C + g * 8;
+        for (int ci = rng[k].x; ci <= rng[k].y; ++ci) {
+          for (int cj = rng[k].z; cj <= rng[k].w; ++cj) {
+            const float inv = 1.f / static_cast<float>(ppm_window_size(ci, H, b) * ppm_window_size(cj, W, b));
+            float f[8];
+            act_ld8<S>(static_cast<const __nv_bfloat16*>(bs.ptr[k]), static_cast<const __nv_bfloat16*>(bs.ptr_lo[k]),
+                       base + static_cast<size_t>(ci * b + cj) * C, f);
 #pragma unroll
-        for (int q = 0; q < 8; ++q) acc[q] = fmaf(f[q], inv[i], acc[q]);
+            for (int q = 0; q < 8; ++q) acc[q] = fmaf(f[q], inv, acc[q]);
+          }
+        }
       }
       act_st8<S>(dx, dx_lo, p * pitch + g * 8, acc);
     }
@@ -244,6 +282,13 @@ static int make_binset(const int* bins, void* const* ptrs, void* const* ptrs_lo,
   return SEMSEG_OK;
 }
 
+// The per-bin tensors are dense [N][b][b][C] and accessed in 8-channel vectors: their bases must be 16-byte aligned.
+static int check_bins(const char* fn, const BinSet& bs) {
+  for (int k = 0; k < bs.nb; ++k)
+    if (const int r = check_vec_acts(fn, 0, {{bs.ptr[k], bs.ptr_lo[k], 0}})) return r;
+  return SEMSEG_OK;
+}
+
 static int ew_blocks(long long total) {
   long long b = (total + 255) / 256;
   const long long cap = static_cast<long long>(num_sms()) * 16;
@@ -263,6 +308,8 @@ extern "C" int semseg_ppm_pool(const void* x, const void* x_lo, int x_pitch, int
   BinSet bs;
   int r = make_binset(bins, pooled, pooled_lo, nb, &bs);
   if (r) return r;
+  if ((r = check_vec_acts("ppm_pool", C, {{x, x_lo, x_pitch}}))) return r;
+  if ((r = check_bins("ppm_pool", bs))) return r;
   dim3 grid(N * bs.cell_off[nb], cdiv(C, 64));
   SB_ACT_DISPATCH(x_lo != nullptr, ppm_pool_kernel<kS><<<grid, 256, 0, stream>>>(
                                        static_cast<const bf16*>(x), static_cast<const bf16*>(x_lo), x_pitch, N, H, W, C,
@@ -283,6 +330,8 @@ extern "C" int semseg_ppm_pool_bwd(void* const* dpooled, void* const* dpooled_lo
   BinSet bs;
   int r = make_binset(bins, dpooled, dpooled_lo, nb, &bs);
   if (r) return r;
+  if ((r = check_vec_acts("ppm_pool_bwd", C, {{dx, dx_lo, dx_pitch}, {add, add_lo, add_pitch}}))) return r;
+  if ((r = check_bins("ppm_pool_bwd", bs))) return r;
   const long long warps = static_cast<long long>(N) * H * W;
   SB_ACT_DISPATCH(split, ppm_pool_bwd_kernel<kS><<<ew_blocks(warps * 32), 256, 0, stream>>>(
                              static_cast<bf16*>(dx), static_cast<bf16*>(dx_lo), dx_pitch, static_cast<const bf16*>(add),
@@ -304,6 +353,8 @@ extern "C" int semseg_ppm_upsample_concat(const void* x, const void* x_lo, int x
   BinSet bs;
   int r = make_binset(bins, feats, feats_lo, nb, &bs);
   if (r) return r;
+  if ((r = check_vec_acts("ppm_upsample_concat", C, {{x, x_lo, x_pitch}, {out, out_lo, out_pitch}}))) return r;
+  if ((r = check_bins("ppm_upsample_concat", bs))) return r;
   const long long total = static_cast<long long>(N) * H * W * (C / 8 + nb * (Cr / 8));
   SB_ACT_DISPATCH(split, ppm_upsample_concat_kernel<kS><<<ew_blocks(total), 256, 0, stream>>>(
                              static_cast<const bf16*>(x), static_cast<const bf16*>(x_lo), x_pitch, N, H, W, C, Cr, bs,
@@ -316,13 +367,17 @@ extern "C" int semseg_ppm_upsample_bwd(const void* dout, const void* dout_lo, in
                                        void* const* dfeats, void* const* dfeats_lo, const int* bins, int nb, int N,
                                        int H, int W, int Cr, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(dout && N > 0 && H > 0 && W > 0 && Cr % 8 == 0 && dout_pitch % 8 == 0 && c_off % 8 == 0,
+  SB_CHECK_ARG(dout && N > 0 && H > 0 && W > 0 && Cr % 8 == 0 && dout_pitch % 8 == 0 && c_off % 8 == 0 && c_off >= 0,
                "ppm_upsample_bwd: bad args");
   SB_CHECK_ARG((dout_lo != nullptr) == (dfeats_lo != nullptr),
                "ppm_upsample_bwd: all tensors must use the same storage form");
   BinSet bs;
   int r = make_binset(bins, dfeats, dfeats_lo, nb, &bs);
   if (r) return r;
+  SB_CHECK_ARG(static_cast<long long>(c_off) + static_cast<long long>(nb) * Cr <= dout_pitch,
+               "ppm_upsample_bwd: channels c_off + nb*Cr = %d + %d*%d exceed the pitch %d", c_off, nb, Cr, dout_pitch);
+  if ((r = check_vec_acts("ppm_upsample_bwd", 0, {{dout, dout_lo, dout_pitch}}))) return r;
+  if ((r = check_bins("ppm_upsample_bwd", bs))) return r;
   dim3 grid(N * bs.cell_off[nb], cdiv(Cr, 64));
   SB_ACT_DISPATCH(dout_lo != nullptr, ppm_upsample_bwd_kernel<kS><<<grid, 256, 0, stream>>>(
                                           static_cast<const bf16*>(dout), static_cast<const bf16*>(dout_lo), dout_pitch,

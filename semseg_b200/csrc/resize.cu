@@ -120,6 +120,7 @@ extern "C" int semseg_resize_bilinear_fwd(const void* x, const void* x_lo, int x
                    y_pitch % 8 == 0,
                "resize_bilinear_fwd: bad args");
   SB_CHECK_ARG((x_lo != nullptr) == (y_lo != nullptr), "resize_bilinear_fwd: x and y must use the same storage form");
+  if (const int r = check_vec_acts("resize_bilinear_fwd", C, {{x, x_lo, x_pitch}, {y, y_lo, y_pitch}})) return r;
   const long long total = static_cast<long long>(N) * Ho * Wo * (C / 8);
   SB_ACT_DISPATCH(x_lo != nullptr, resize_bilinear_fwd_kernel<kS><<<rs_blocks(total), 256, 0, stream>>>(
                                        static_cast<const bf16*>(x), static_cast<const bf16*>(x_lo), x_pitch, N, Hi, Wi, C,
@@ -135,6 +136,7 @@ extern "C" int semseg_resize_bilinear_bwd(const void* dy, const void* dy_lo, int
                    dx_pitch % 8 == 0,
                "resize_bilinear_bwd: bad args");
   SB_CHECK_ARG((dy_lo != nullptr) == (dx_lo != nullptr), "resize_bilinear_bwd: dy and dx must use the same storage form");
+  if (const int r = check_vec_acts("resize_bilinear_bwd", C, {{dy, dy_lo, dy_pitch}, {dx, dx_lo, dx_pitch}})) return r;
   const long long total = static_cast<long long>(N) * Hi * Wi * (C / 8);
   SB_ACT_DISPATCH(dy_lo != nullptr, resize_bilinear_bwd_kernel<kS><<<rs_blocks(total), 256, 0, stream>>>(
                                         static_cast<const bf16*>(dy), static_cast<const bf16*>(dy_lo), dy_pitch, N, Hi, Wi,

@@ -141,7 +141,8 @@ def test_round2_entry_points_validate_before_any_cuda_call():
     assert b"psa_attend_bwd_attn" in err()
     assert lib.semseg_resize_bilinear_fwd(None, None, 64, 1, 4, 4, 64, 8, 8, P, None, 64, None) == -1
     assert b"resize_bilinear_fwd" in err()
-    assert lib.semseg_resize_bilinear_fwd(P, None, 60, 1, 4, 4, 64, 8, 8, P, None, 64, None) == -1       # pitch < C
+    assert lib.semseg_resize_bilinear_fwd(P, None, 56, 1, 4, 4, 64, 8, 8, P, None, 64, None) == -1       # pitch < C
+    assert b"pitch 56 is smaller than C = 64" in err()
     assert lib.semseg_resize_bilinear_bwd(P, P, 64, 1, 4, 4, 64, 8, 8, P, None, 64, None) == -1
     assert b"same storage form" in err()
     h = _lib.SgdHyper()
