@@ -343,8 +343,12 @@ static int psa_tile_rows(int N, int Q, int max_rows, int blocks_per_tile) {
 
 namespace sb {
 
-// form bits of the _ex entry points: the mask form and the softmax switch shared by the forward and backward checks
-static int check_psa_form(const char* fn, int form, int H, int W, int mH, int mW, int a_pitch, bool has_stats) {
+// form bits of the _ex entry points: the mask form and the softmax switch shared by the forward and backward checks.
+// Both kernels read (and the forward writes) stats as float2.
+static int check_psa_form(const char* fn, int form, int H, int W, int mH, int mW, int a_pitch, const float* stats) {
+  const bool has_stats = stats != nullptr;
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(stats) & 7) == 0, "%s: stats %p is not 8-byte aligned", fn,
+               static_cast<const void*>(stats));
   SB_CHECK_ARG((form & ~(SEMSEG_PSA_DENSE | SEMSEG_PSA_NO_SOFTMAX)) == 0, "%s: unknown form bits 0x%x", fn, form);
   if (form & SEMSEG_PSA_DENSE)
     SB_CHECK_ARG(mH > 0 && mW > 0 && mH * mW == H * W && a_pitch >= H * W,
@@ -374,11 +378,14 @@ extern "C" int semseg_psa_attend_ex(int mode, int psa_type, int form, const floa
   SB_CHECK_ARG(attn && feat && out && N > 0 && H > 0 && W > 0, "psa_attend: bad args");
   SB_CHECK_ARG(mode == 0 || mode == 1, "psa_attend: mode must be 0 (forward) or 1 (feature gradient)");
   SB_CHECK_ARG(psa_type == 0 || psa_type == 1, "psa_attend: psa_type must be 0 (collect) or 1 (distribute)");
-  if (const int r = check_psa_form("psa_attend", form, H, W, mH, mW, a_pitch, stats != nullptr)) return r;
+  if (const int r = check_psa_form("psa_attend", form, H, W, mH, mW, a_pitch, stats)) return r;
   SB_CHECK_ARG(C == kPfC, "psa_attend: feature width must be %d (got %d)", kPfC, C);
   SB_CHECK_ARG(W <= 128, "psa_attend: feature maps wider than %d are not supported", 128);
   SB_CHECK_ARG(feat_pitch % 8 == 0 && out_pitch % 8 == 0 && feat_pitch >= C && out_pitch >= C, "psa_attend: bad pitch");
   SB_CHECK_ARG((feat_lo != nullptr) == (out_lo != nullptr), "psa_attend: feat and out must use the same storage form");
+  // feat through TMA (16-byte global addresses), out stored as bf16 pairs
+  if (const int r = check_vec_acts("psa_attend", C, {{feat, feat_lo, feat_pitch}})) return r;
+  if (const int r = check_vec_acts("psa_attend", C, {{out, out_lo, out_pitch}}, 4)) return r;
   PsaFusedParams p;
   memset(&p, 0, sizeof(p));
   p.A = attn; p.stats = reinterpret_cast<float2*>(stats);
@@ -644,13 +651,18 @@ extern "C" int semseg_psa_attend_bwd_attn_ex(int psa_type, int form, const float
   const bool softmax = !(form & SEMSEG_PSA_NO_SOFTMAX);
   SB_CHECK_ARG(attn && feat && dout && dattn && N > 0 && H > 0 && W > 0, "psa_attend_bwd_attn: bad args");
   SB_CHECK_ARG(psa_type == 0 || psa_type == 1, "psa_attend_bwd_attn: psa_type must be 0 or 1");
-  if (const int r = check_psa_form("psa_attend_bwd_attn", form, H, W, mH, mW, a_pitch, stats != nullptr)) return r;
+  if (const int r = check_psa_form("psa_attend_bwd_attn", form, H, W, mH, mW, a_pitch, stats)) return r;
   SB_CHECK_ARG(out || !softmax, "psa_attend_bwd_attn: out is required with softmax");
   SB_CHECK_ARG(C > 0 && C % 64 == 0 && W <= 128, "psa_attend_bwd_attn: C %% 64 == 0 and W <= 128 required");
   SB_CHECK_ARG(feat_pitch % 8 == 0 && out_pitch % 8 == 0 && dout_pitch % 8 == 0, "psa_attend_bwd_attn: bad pitch");
   const bool split = feat_lo != nullptr;
   SB_CHECK_ARG(((out_lo != nullptr) == split || (!softmax && !out)) && (dout_lo != nullptr) == split,
                "psa_attend_bwd_attn: all activations must use the same storage form");
+  // feat and dout through TMA, dout and out (read only with softmax) as 16-byte vectors in the D term: every check
+  // comes before the dattn memset, so a rejected call makes no CUDA call
+  if (const int r = check_vec_acts("psa_attend_bwd_attn", C, {{feat, feat_lo, feat_pitch}, {dout, dout_lo, dout_pitch},
+                                                              {softmax ? out : nullptr, out_lo, out_pitch}}))
+    return r;
   PsaGradParams p;
   memset(&p, 0, sizeof(p));
   p.A = attn; p.stats = reinterpret_cast<const float2*>(stats); p.dA = dattn;
