@@ -21,6 +21,7 @@
  *   - semseg_upsample_ce_*    : F.interpolate + CrossEntropyLoss + argmax, model/pspnet.py:94-103.
  *                               semseg_upsample_ce_ohem_*: the same with an OHEM cross-entropy criterion.
  *                               semseg_upsample_ce_{,ohem_}weighted_*: class weights / label smoothing.
+ *                               semseg_upsample_ce_dice_*: soft Dice loss, alone or plus cross-entropy.
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -459,6 +460,29 @@ int semseg_upsample_ce_ohem_weighted_bwd(const float* logits, int pitch, int N, 
                                          const float* class_weight, const float* lse, const float* pt,
                                          const float* thr, const float* loss_info, const float* grad_out,
                                          float* workspace, float* dlogits, void* stream);
+/* Soft Dice loss, alone or plus cross-entropy (semseg_b200/losses.py DiceLoss), on the same fused upsample at zoom
+ * `zoom`. With p = softmax(v) and sums over every valid pixel (target != ignore_index, 0 <= target < C) of every image:
+ *   n_c = #{t = c},  I_c = sum p_c [t = c],  S_c = sum p_c + n_c,  dice_c = (2 I_c + smooth) / max(S_c + smooth, eps)
+ *   loss = (1/C) sum_{c: n_c > 0} (1 - dice_c) + ce_weight * CE,   CE = mean over the valid pixels of lse - v_t
+ * loss 0 and an exactly zero gradient when no pixel is valid. smooth, eps, ce_weight finite and >= 0. The staged rows
+ * take 12 bytes per pixel: Wo <= 229376 / (12 zoom), i.e. 2389 at zoom 8; a wider target is rejected before any launch.
+ *   fwd: loss_out[0] = loss, loss_out[1] = number of valid pixels; argmax (or NULL) and lse as the zoom forward's
+ *        (the same bits); table fp32 [5C+2] = alpha[C], beta[C], I[C], S[C], n[C], ce_weight / n_valid, 1 (the
+ *        gradient coefficients and the per-class statistics, written on the device: graph-capturable);
+ *        workspace: semseg_upsample_ce_dice_workspace_floats() floats, 8-byte aligned.
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits from the forward's lse and table; workspace:
+ *        semseg_upsample_ce_dice_bwd_workspace_floats() floats.
+ * Both reject a bad shape, zoom, option, width or null output before any CUDA call; the workspace functions return -1
+ * for a zoom outside {1, 2, 4, 8}. */
+long long semseg_upsample_ce_dice_workspace_floats(int N, int Ho, int Wo, int C, int zoom);
+int semseg_upsample_ce_dice_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                int Ho, int Wo, int zoom, int ignore_index, float smooth, float eps, float ce_weight,
+                                float* workspace, float* loss_out, int64_t* argmax, float* lse, float* table,
+                                void* stream);
+long long semseg_upsample_ce_dice_bwd_workspace_floats(int N, int Ho, int Wo, int w, int C, int zoom);
+int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* table,
+                                const float* grad_out, float* workspace, float* dlogits, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sliding-window evaluation after the network (semseg_b200/inference.py, exact=False). No tensor cores, no atomics.

@@ -31,6 +31,11 @@
 // and loss 0 with an exactly zero gradient when D = 0. Weighted OHEM (kOhem and kWeighted) writes nll = w_t (lse - v_t)
 // and scales the pixel's gradient by w_t; its selection and mean over the kept pixels are the OHEM ones. The
 // kWeighted = false instances are unchanged.
+//
+// The soft Dice loss, alone or plus cross-entropy, runs the plain forward instance and its own statistics, reduce and
+// gradient kernels (see "Dice" below); no existing instance changes.
+#include <cmath>
+
 #include "host_common.h"
 
 namespace sb {
@@ -535,6 +540,298 @@ upsample_ce_bwd_cols_kernel(const float* __restrict__ T2, int N, int h, int w, i
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- Dice
+// Soft Dice loss (segmentation_models_pytorch's multiclass DiceLoss from logits, with ignore_index), alone or plus
+// ce_weight * cross-entropy, summed over every pixel of every image of the call. With p = softmax(v), valid pixels i:
+//   n_c = #{t_i = c},  I_c = sum p_ic [t_i = c],  S_c = sum p_ic + n_c,  D_c = max(S_c + smooth, eps)
+//   L = (1/C) sum_{c: n_c > 0} (1 - (2 I_c + smooth) / D_c) + ce_weight * CE
+//   dL/dv_ic = p_ic (beta_c + lam - G_i) - [c = t_i] (p_ic alpha_c + lam),   G_i = sum_c p_ic beta_c - p_it alpha_t
+//   alpha_c = 2 m_c / (C D_c),  beta_c = m_c (2 I_c + smooth) / (C D_c^2) (0 where D_c is the clamp eps),
+//   m_c = [n_c > 0],  lam = ce_weight / n_valid
+// A pixel's gradient depends on sums over the whole call, so the criterion is a chain of passes:
+//   forward : the plain forward instance (lse, argmax, CE partials: lse and argmax are the plain tail's bits), the
+//             statistics pass (rows layout, one thread per class: (sum p, sum p at the target, n) per (interval, image)
+//             and class, no cross-thread reduction), a per-class fp64 reduce in a fixed order (the (I, S, n) and
+//             alpha / beta tables), and a one-CTA reduce of the loss;
+//   backward: G_i in the forward's thread-per-pixel layout, the rows kernel with (lse, t, G) staged per pixel, and the
+//             plain cols kernel (which divides by table[5C+1] = 1).
+// Device table, 5C + 2 floats: alpha[C], beta[C], I[C], S[C], n[C], lam, 1.
+struct DicePix {
+  float lse2;  // log-sum-exp * log2(e)
+  int t;       // target class, -1 = ignored
+  float g;     // G_i (backward only)
+};
+constexpr int kDiceWords = 5;   // alpha, beta, I, S, n
+
+// One interval (Z columns of Z rows; fewer at the last node row / column when !kFull) of the Dice rows kernel for
+// class c. kGrad: acc = the (left, right) x (top, bottom node row) gradient sums as in upsample_ce_bwd_rows_kernel;
+// else acc = (sum p, sum p at the target, target count).
+template <int Z, bool kGrad, bool kFull>
+__device__ __forceinline__ void dice_interval(const DicePix* s, int Wo, int xb, int rows, int nx, int c, float a,
+                                              float b, float cc, float d, float ac, float bl, float lam, float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const DicePix pi = s[r * Wo + xb + k];
+      if (pi.t < 0) continue;  // warp-uniform
+      const float v = row_lerp<Z>(top, bot, r);
+      const float p = ex2_approx(fmaf(v, kLog2e, -pi.lse2));
+      if constexpr (kGrad) {
+        const float q = p * (bl - pi.g);
+        const float g = c == pi.t ? q - fmaf(p, ac, lam) : q;
+        g0 = fmaf(1.f - G::kStep * r, g, g0);
+        g1 = fmaf(G::kStep * r, g, g1);
+      } else {
+        acc[0] += p;
+        if (c == pi.t) {
+          acc[1] += p;
+          acc[2] += 1.f;
+        }
+      }
+    }
+    if constexpr (kGrad) {
+      acc[0] = fmaf(l0w, g0, acc[0]);
+      acc[1] = fmaf(l1w, g0, acc[1]);
+      acc[2] = fmaf(l0w, g1, acc[2]);
+      acc[3] = fmaf(l1w, g1, acc[3]);
+    }
+  }
+}
+
+// Rows layout of upsample_ce_bwd_rows_kernel: one CTA per (low-res interval row i0, image), one thread per class,
+// (lse, target[, G]) of the interval's Z output rows staged as one 12-byte word per pixel.
+// !kGrad (statistics): out = partial[n][i0][3][C] = (sum p, sum p at the target, n) over the interval's valid pixels;
+// each thread sums an interval column in fp32 and the columns in fp64, so a partial is rounded once.
+// kGrad: out = T2 as in upsample_ce_bwd_rows_kernel, of the Dice (+ CE) gradient; gmap = G_i, table = the Dice table.
+template <int Z, bool kGrad>
+__global__ void __launch_bounds__(256)
+upsample_ce_dice_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
+                             const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                             const float* __restrict__ lse, const float* __restrict__ gmap,
+                             const float* __restrict__ table, float* __restrict__ out) {
+  extern __shared__ DicePix s_dpix[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const long long t = target[rowbase + x];
+      DicePix pi;
+      pi.t = (t == ignore_index || t < 0 || t >= C) ? -1 : static_cast<int>(t);
+      pi.lse2 = lse[rowbase + x] * kLog2e;
+      pi.g = kGrad ? gmap[rowbase + x] : 0.f;
+      s_dpix[r * Wo + x] = pi;
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  float ac = 0.f, bl = 0.f, lam = 0.f;  // kGrad: alpha_c, beta_c + lam, lam
+  if constexpr (kGrad) {
+    ac = table[c];
+    lam = table[kDiceWords * C];
+    bl = table[C + c] + lam;
+  }
+  const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
+  const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
+  float* T0 = out + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;   // kGrad
+  float* T1 = out + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  float a = L0[0], cc = L1[0];
+  float nb = L0[static_cast<size_t>(min(1, w - 1)) * pitch], nd = L1[static_cast<size_t>(min(1, w - 1)) * pitch];
+  float carry0 = 0.f, carry1 = 0.f;
+  double sp = 0.0, si = 0.0, sn = 0.0;  // !kGrad
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd;
+    const int jn = min(j0 + 2, w - 1);
+    nb = L0[static_cast<size_t>(jn) * pitch];
+    nd = L1[static_cast<size_t>(jn) * pitch];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      dice_interval<Z, kGrad, true>(s_dpix, Wo, xb, rows, nx, c, a, b, cc, d, ac, bl, lam, acc);
+    } else {
+      dice_interval<Z, kGrad, false>(s_dpix, Wo, xb, rows, nx, c, a, b, cc, d, ac, bl, lam, acc);
+    }
+    if constexpr (kGrad) {
+      T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+      T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+      carry0 = acc[1];
+      carry1 = acc[3];
+    } else {
+      sp += acc[0];
+      si += acc[1];
+      sn += acc[2];
+    }
+    a = b;
+    cc = d;
+  }
+  if constexpr (!kGrad) {
+    float* P = out + (static_cast<size_t>(n) * h + i0) * 3 * C + c;
+    P[0] = static_cast<float>(sp);
+    P[C] = static_cast<float>(si);
+    P[2 * C] = static_cast<float>(sn);
+  }
+}
+
+// One CTA per class: the class's statistics partials summed in fp64 in a fixed order, then its table entries and its
+// loss term 1 - dice_c (0 for an absent class) into terms[c].
+__global__ void __launch_bounds__(256)
+dice_class_reduce_kernel(const float* __restrict__ partial, int nparts, int C, float smooth, float eps,
+                         float* __restrict__ table, double* __restrict__ terms) {
+  __shared__ double red[3][256];
+  const int c = blockIdx.x;
+  double sp = 0.0, si = 0.0, sn = 0.0;
+  for (int i = threadIdx.x; i < nparts; i += 256) {
+    const float* P = partial + static_cast<size_t>(i) * 3 * C + c;
+    sp += P[0];
+    si += P[C];
+    sn += P[2 * C];
+  }
+  red[0][threadIdx.x] = sp;
+  red[1][threadIdx.x] = si;
+  red[2][threadIdx.x] = sn;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      red[0][threadIdx.x] += red[0][threadIdx.x + o];
+      red[1][threadIdx.x] += red[1][threadIdx.x + o];
+      red[2][threadIdx.x] += red[2][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double I = red[1][0], nc = red[2][0];
+    const double S = red[0][0] + nc;
+    const double num = 2.0 * I + smooth;
+    const double D = fmax(S + smooth, static_cast<double>(eps));
+    double alpha = 0.0, beta = 0.0, term = 0.0;
+    if (nc > 0.0) {
+      term = 1.0 - num / D;
+      alpha = 2.0 / (C * D);
+      beta = S + smooth < eps ? 0.0 : num / (C * D * D);   // a clamped denominator does not depend on p
+    }
+    table[c] = static_cast<float>(alpha);
+    table[C + c] = static_cast<float>(beta);
+    table[2 * C + c] = static_cast<float>(I);
+    table[3 * C + c] = static_cast<float>(S);
+    table[4 * C + c] = static_cast<float>(nc);
+    terms[c] = term;
+  }
+}
+
+// One CTA: CE = (sum of the forward's CE partials) / n_valid and sum_c terms[c], both in fp64 in a fixed order ->
+// loss_out = (L, n_valid), table[5C] = lam, table[5C+1] = 1.
+__global__ void __launch_bounds__(256)
+dice_loss_kernel(const float* __restrict__ ce_partial, int nblocks, const double* __restrict__ terms, int C,
+                 float ce_weight, float* __restrict__ loss_out, float* __restrict__ table) {
+  __shared__ double sl[256];
+  __shared__ double sc[256];
+  __shared__ double st[256];
+  double l = 0.0, k = 0.0;
+  for (int i = threadIdx.x; i < nblocks; i += 256) {
+    l += ce_partial[2 * i];
+    k += ce_partial[2 * i + 1];
+  }
+  sl[threadIdx.x] = l;
+  sc[threadIdx.x] = k;
+  st[threadIdx.x] = threadIdx.x < C ? terms[threadIdx.x] : 0.0;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      sl[threadIdx.x] += sl[threadIdx.x + o];
+      sc[threadIdx.x] += sc[threadIdx.x + o];
+      st[threadIdx.x] += st[threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double nv = sc[0];
+    const double ce = nv > 0.0 ? sl[0] / nv : 0.0;
+    loss_out[0] = static_cast<float>(st[0] / C + static_cast<double>(ce_weight) * ce);
+    loss_out[1] = static_cast<float>(nv);
+    table[kDiceWords * C] = nv > 0.0 ? static_cast<float>(ce_weight / nv) : 0.f;
+    table[kDiceWords * C + 1] = 1.f;
+  }
+}
+
+// G_i = sum_c p_ic beta_c - p_it alpha_t per valid pixel (0 elsewhere), in the forward's layout: one CTA per (128
+// output columns, interval row, image), one thread per output column and its Z rows, the node rows and the alpha /
+// beta tables staged in shared memory.
+template <int Z>
+__global__ void __launch_bounds__(kFwdCols)
+upsample_ce_dice_g_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
+                          const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                          const float* __restrict__ lse, const float* __restrict__ table, float* __restrict__ gmap) {
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs], then alpha[C], beta[C]
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kFwdNodes, w - j_base);
+  const int tid = threadIdx.x;
+  float* s_ab = S + G::kNodeRows * kFwdNodes * Cs;
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * kFwdNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
+  }
+  for (int c = tid; c < 2 * C; c += kFwdCols) s_ab[c] = table[c];
+  __syncthreads();
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x >= Wo) return;
+  const int j0 = x >> G::kShift;
+  const int j1 = min(j0 + 1, w - 1);
+  const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+  const float* A = S + (j0 - j_base) * Cs;
+  const float* B = S + (j1 - j_base) * Cs;
+  const float* Cc = A + kFwdNodes * Cs;
+  const float* D = B + kFwdNodes * Cs;
+  float lse2[Z], g[Z];
+#pragma unroll
+  for (int r = 0; r < Z; ++r) {
+    g[r] = 0.f;
+    lse2[r] = r < rows ? lse[(static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x] * kLog2e : 0.f;
+  }
+#pragma unroll 2
+  for (int c = 0; c < C; ++c) {
+    const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+    const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+    const float beta = s_ab[C + c];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) g[r] = fmaf(ex2_approx(fmaf(row_lerp<Z>(top, bot, r), kLog2e, -lse2[r])), beta, g[r]);
+  }
+#pragma unroll
+  for (int r = 0; r < Z; ++r) {
+    if (r < rows) {
+      const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+      const long long t = target[pix];
+      float gv = 0.f;
+      if (t != ignore_index && t >= 0 && t < C) {
+        const int tc = static_cast<int>(t);
+        const float top = Z == 1 ? A[tc] : l0w * A[tc] + l1w * B[tc];
+        const float bot = Z == 1 ? 0.f : l0w * Cc[tc] + l1w * D[tc];
+        const float pt = ex2_approx(fmaf(row_lerp<Z>(top, bot, r), kLog2e, -lse2[r]));
+        gv = fmaf(-pt, s_ab[tc], g[r]);
+      }
+      gmap[pix] = gv;
+    }
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -887,6 +1184,154 @@ extern "C" int semseg_upsample_ce_ohem_weighted_bwd(const float* logits, int pit
                                              grad_out, workspace, dlogits, pt, thr, stream, class_weight);
     default: return launch_bwd<8, true, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, loss_info,
                                               grad_out, workspace, dlogits, pt, thr, stream, class_weight);
+  }
+}
+
+// Dice loss (+ ce_weight * CE) at zoom factor `zoom`. The rows kernels stage 12 bytes per pixel of the interval's Z
+// output rows in at most 224 KB of shared memory: Wo <= 2389 at zoom 8 (the plain form's 8-byte words allow 2560).
+constexpr size_t kDiceSmemMax = 224 * 1024;
+
+static int check_dice(int zoom, int Wo, float smooth, float eps, float ce_weight) {
+  SB_CHECK_ARG(std::isfinite(smooth) && smooth >= 0.f, "upsample_ce_dice: smooth %g is not finite and >= 0", smooth);
+  SB_CHECK_ARG(std::isfinite(eps) && eps >= 0.f, "upsample_ce_dice: eps %g is not finite and >= 0", eps);
+  SB_CHECK_ARG(std::isfinite(ce_weight) && ce_weight >= 0.f, "upsample_ce_dice: ce_weight %g is not finite and >= 0",
+               ce_weight);
+  const size_t max_wo = kDiceSmemMax / (static_cast<size_t>(zoom) * sizeof(DicePix));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_ce_dice: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+template <int Z, bool kGrad>
+static int launch_dice_rows(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                            int Wo, int ignore_index, const float* lse, const float* gmap, const float* table,
+                            float* out, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(DicePix);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_dice_rows_kernel<Z, kGrad>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  upsample_ce_dice_rows_kernel<Z, kGrad><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, gmap, table,
+      out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+// Forward workspace: the CE partials (2 per forward CTA), the statistics partials [N][h][3][C], then (8-byte aligned)
+// the C fp64 loss terms.
+static long long dice_terms_offset(int N, int h, int Wo, int C) {
+  const long long f = 2LL * fwd_ctas(N, h, Wo) + 3LL * N * h * C;
+  return (f + 1) & ~1LL;
+}
+
+template <int Z>
+static int launch_dice_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                           int Wo, int ignore_index, float smooth, float eps, float ce_weight, float* workspace,
+                           float* loss_out, int64_t* argmax, float* lse, float* table, cudaStream_t stream) {
+  const int ctas = fwd_ctas(N, h, Wo);
+  float* stats = workspace + 2LL * ctas;
+  double* terms = reinterpret_cast<double*>(workspace + dice_terms_offset(N, h, Wo, C));
+  int r = launch_fwd_kernel<Z, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, argmax, lse,
+                                      nullptr, nullptr, stream);
+  if (r) return r;
+  r = launch_dice_rows<Z, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, nullptr, nullptr, stats,
+                                 stream);
+  if (r) return r;
+  dice_class_reduce_kernel<<<C, 256, 0, stream>>>(stats, N * h, C, smooth, eps, table, terms);
+  SB_LAUNCHED();
+  dice_loss_kernel<<<1, 256, 0, stream>>>(workspace, ctas, terms, C, ce_weight, loss_out, table);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+// Backward workspace: T2 [N][h][2][w][C] of the rows kernel, then the G map [N][Ho][Wo].
+template <int Z>
+static int launch_dice_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                           int Wo, int ignore_index, const float* lse, const float* table, const float* grad_out,
+                           float* workspace, float* dlogits, cudaStream_t stream) {
+  float* gmap = workspace + 2LL * N * h * w * C;
+  const int Cs = C | 1;
+  const size_t smem = (static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs + 2 * C) * sizeof(float);
+  constexpr size_t kMaxSmem =
+      (static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) + 2 * kMaxClasses) * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_dice_g_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_ce_dice_g_kernel<Z><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, table,
+      gmap);
+  SB_LAUNCHED();
+  int r = launch_dice_rows<Z, true>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, gmap, table,
+                                    workspace, stream);
+  if (r) return r;
+  // table[5C + 1] = 1: the plain cols kernel's count, so dlogits = grad_out[0] * T2 sums
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, table + kDiceWords * C, grad_out,
+                                                             dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_dice_workspace_floats(int N, int Ho, int Wo, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_dice: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && C > 0, "upsample_ce_dice: bad sizes");
+  return dice_terms_offset(N, (Ho - 1) / zoom + 1, Wo, C) + 2LL * C;
+}
+
+extern "C" int semseg_upsample_ce_dice_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                           const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                           float smooth, float eps, float ce_weight, float* workspace,
+                                           float* loss_out, int64_t* argmax, float* lse, float* table,
+                                           void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_dice(zoom, Wo, smooth, eps, ce_weight);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && table, "upsample_ce_dice_fwd: null output");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "upsample_ce_dice_fwd: workspace not 8-byte aligned");
+  switch (zoom) {
+    case 1: return launch_dice_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, smooth, eps, ce_weight,
+                                      workspace, loss_out, argmax, lse, table, stream);
+    case 2: return launch_dice_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, smooth, eps, ce_weight,
+                                      workspace, loss_out, argmax, lse, table, stream);
+    case 4: return launch_dice_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, smooth, eps, ce_weight,
+                                      workspace, loss_out, argmax, lse, table, stream);
+    default: return launch_dice_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, smooth, eps,
+                                       ce_weight, workspace, loss_out, argmax, lse, table, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_dice_bwd_workspace_floats(int N, int Ho, int Wo, int w, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_dice: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && w > 0 && C > 0, "upsample_ce_dice: bad sizes");
+  return 2LL * N * ((Ho - 1) / zoom + 1) * w * C + static_cast<long long>(N) * Ho * Wo;
+}
+
+extern "C" int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                           const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                           const float* lse, const float* table, const float* grad_out,
+                                           float* workspace, float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_dice(zoom, Wo, 0.f, 0.f, 0.f);
+  if (r) return r;
+  SB_CHECK_ARG(lse && table && grad_out && workspace && dlogits, "upsample_ce_dice_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_dice_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
+                                      workspace, dlogits, stream);
+    case 2: return launch_dice_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
+                                      workspace, dlogits, stream);
+    case 4: return launch_dice_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
+                                      workspace, dlogits, stream);
+    default: return launch_dice_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
+                                       workspace, dlogits, stream);
   }
 }
 

@@ -582,6 +582,26 @@ class _UpsampleCEOhem(torch.autograd.Function):
         return dl, None, None, None, None, None, None
 
 
+class _UpsampleCEDice(torch.autograd.Function):
+    """The fused tail with losses.DiceLoss: soft Dice over every pixel of the call, plus ce_weight * CE. The forward
+    keeps the per-class gradient table it reduced on the device; the backward needs nothing else from the host."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, smooth, eps, ce_weight):
+        info, amax, lse, table = ops.upsample_ce_dice_fwd(logits, target, ignore_index, smooth, eps, ce_weight,
+                                                          zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, table)
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, table = ctx.saved_tensors
+        dl = ops.upsample_ce_dice_bwd(logits, target, ctx.ignore_index, lse, table, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None, None
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""
@@ -591,24 +611,34 @@ def _class_weight_supported(weight, target, classes):
             and weight.is_cuda and weight.device == target.device and (classes is None or weight.numel() == classes))
 
 
+# The Dice rows kernels stage 12 bytes per pixel of an interval's Z output rows in at most 224 KB of shared memory
+# (csrc/tail.cu kDiceSmemMax): Wo <= 2389 at zoom 8.
+_DICE_PIXEL_BYTES, _DICE_STAGE_BYTES = 12, 224 * 1024
+
+
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     """The fused kernel implements exactly nn.CrossEntropyLoss(weight, ignore_index=k, reduction='mean',
-    label_smoothing) and losses.OhemCrossEntropyLoss (with or without class weights), at every zoom factor of the model
-    (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits. The weighted / smoothed
-    forms need the target on a CUDA device and class weights as a contiguous fp32 [classes] tensor on that device; any
-    other weight, another reduction, and any subclass keep the ATen tail.
+    label_smoothing), losses.OhemCrossEntropyLoss (with or without class weights) and losses.DiceLoss, at every zoom
+    factor of the model (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits. The
+    weighted / smoothed forms need the target on a CUDA device and class weights as a contiguous fp32 [classes] tensor
+    on that device; any other weight, another reduction, and any subclass keep the ATen tail. DiceLoss also needs the
+    target no wider than its kernels stage (2389 columns at zoom 8).
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is nn.CrossEntropyLoss:
         eps = getattr(criterion, 'label_smoothing', 0.0)
         plain = criterion.weight is None and eps == 0.0
         ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
               (plain or (target is not None and target.is_cuda)))
+    elif type(criterion) is losses.DiceLoss:
+        ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
+              _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     else:
         ok = type(criterion) is losses.OhemCrossEntropyLoss
     if not (ok and zoom_factor in (1, 2, 4, 8)
             and target is not None and target.dtype == torch.int64 and target.dim() == 3):
         return False
-    if not _class_weight_supported(criterion.weight, target, None if logits is None else logits.shape[-1]):
+    if not _class_weight_supported(getattr(criterion, "weight", None), target,
+                                   None if logits is None else logits.shape[-1]):
         return False
     if logits is None:
         h, w = (x_size[2] - 1) // 8 + 1, (x_size[3] - 1) // 8 + 1      # the network's output stride is 8
@@ -622,8 +652,11 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
 def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None):
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
-    weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean.
-    The default criterion runs the plain kernels."""
+    weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
+    with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index). The default criterion runs the plain kernels."""
+    if isinstance(criterion, losses.DiceLoss):
+        return _UpsampleCEDice.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.smooth,
+                                     criterion.eps, criterion.ce_weight)
     if isinstance(criterion, losses.OhemCrossEntropyLoss):
         if criterion.weight is None:
             return _UpsampleCEOhem.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),

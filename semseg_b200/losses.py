@@ -3,8 +3,11 @@
 OhemCrossEntropyLoss is online hard-pixel mining: only the pixels the network is least sure of are trained on. With
 the network's fused tail (functional.upsample_ce) it runs inside the same kernels as the default loss, graphed at every
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
-zoom-1 form of those kernels on an NHWC copy of the logits.
+zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
+runs the same way.
 """
+import math
+
 import torch
 from torch import nn
 
@@ -73,5 +76,63 @@ class OhemCrossEntropyLoss(nn.Module):
                                   and w.device == logits.device):
             raise ValueError("OhemCrossEntropyLoss: weight must be contiguous fp32 [%d] on %s (no fallback), got %s "
                              "[%d] on %s" % (logits.shape[1], logits.device, w.dtype, w.numel(), w.device))
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+def _non_negative(name, v):
+    if isinstance(v, bool) or not isinstance(v, (int, float)):
+        raise TypeError("%s must be a number, got %r" % (name, v))
+    v = float(v)
+    if not (math.isfinite(v) and v >= 0.0):
+        raise ValueError("%s must be finite and >= 0, got %r" % (name, v))
+    return v
+
+
+class DiceLoss(nn.Module):
+    """Soft Dice loss from logits, optionally plus cross-entropy, for logits [N, C, H, W] and target [N, H, W]:
+
+        valid  = target != ignore_index and 0 <= target < C     (other out-of-range targets are skipped)
+        p      = softmax(logits) over C
+        n_c    = #{valid pixels with target c},  I_c = sum over valid pixels of p_c [target = c]
+        S_c    = sum over valid pixels of p_c, plus n_c
+        dice_c = (2 I_c + smooth) / max(S_c + smooth, eps)
+        loss   = (1/C) sum over the classes with n_c > 0 of (1 - dice_c) + ce_weight * CE
+
+    CE is the mean cross-entropy over the valid pixels. The sums run over every pixel of every image of the call (per
+    rank under DistributedDataParallel). Classes without a pixel add 0 but still count in 1/C. With no valid pixel the
+    loss is 0 and every gradient is 0. This is segmentation_models_pytorch's DiceLoss(mode='multiclass',
+    from_logits=True, smooth, eps, ignore_index), plus the CE term.
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, graphed at every zoom
+    factor; called as a module (validate()) it runs their zoom-1 form on an NHWC copy of the logits. CUDA fp32 logits
+    with at most 256 classes only: there is no CPU or library fallback."""
+
+    def __init__(self, ignore_index=255, smooth=0.0, eps=1e-7, ce_weight=0.0):
+        super(DiceLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        self.ignore_index = ignore_index
+        self.smooth = _non_negative("smooth", smooth)
+        self.eps = _non_negative("eps", eps)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+
+    def extra_repr(self):
+        return "ignore_index=%d, smooth=%g, eps=%g, ce_weight=%g" % (self.ignore_index, self.smooth, self.eps,
+                                                                      self.ce_weight)
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        if logits.dim() != 4 or target.dim() != 3 or target.shape != logits.shape[:1] + logits.shape[2:]:
+            raise ValueError("DiceLoss: logits [N, C, H, W] and target [N, H, W] expected, got %s and %s" %
+                             (tuple(logits.shape), tuple(target.shape)))
+        if logits.shape[1] > 256:
+            raise ValueError("DiceLoss: at most 256 classes (got %d); no fallback" % logits.shape[1])
+        if not (logits.is_cuda and target.is_cuda):
+            raise RuntimeError("DiceLoss runs on the native CUDA kernels only (no CPU fallback); got %s, %s"
+                               % (logits.device, target.device))
+        if logits.dtype != torch.float32 or target.dtype != torch.int64:
+            raise TypeError("DiceLoss: fp32 logits and int64 target expected, got %s and %s" %
+                            (logits.dtype, target.dtype))
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
         return loss

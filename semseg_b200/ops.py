@@ -799,6 +799,48 @@ def upsample_ce_ohem_bwd(logits, target, ignore_index, lse, pt, thr, info, grad_
     return dl
 
 
+def upsample_ce_dice_fwd(logits, target, ignore_index, smooth, eps, ce_weight, want_argmax=True, zoom=8):
+    """Soft Dice loss (+ ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract); arguments as
+    upsample_ce_fwd plus the Dice options -> (loss_info [2] = (loss, valid count), argmax, lse, table [5C+2] =
+    (alpha, beta, I, S, n per class, ce_weight / n_valid, 1))."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_dice_workspace_floats(n, ho, wo, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_dice_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    table = torch.empty((5 * c + 2,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse = torch.empty((n, ho, wo), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_upsample_ce_dice_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                               int(zoom), int(ignore_index), float(smooth), float(eps),
+                                               float(ce_weight), _ptr(ws), _ptr(info), _ptr(amax), _ptr(lse),
+                                               _ptr(table), _stream()),
+               "semseg_upsample_ce_dice_fwd")
+    return info, amax, lse, table
+
+
+def upsample_ce_dice_bwd(logits, target, ignore_index, lse, table, grad_out, zoom=8):
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_dice_bwd_workspace_floats(n, ho, wo, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_dice_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_dice_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                               int(zoom), int(ignore_index), _ptr(lse), _ptr(table), _ptr(g), _ptr(ws),
+                                               _ptr(dl), _stream()),
+               "semseg_upsample_ce_dice_bwd")
+    return dl
+
+
 # ------------------------------------------------------------------------------------------------ sliding-window evaluation
 def window_scores(logits, flip, out):
     """fp32 NHWC logits [G (+G mirrored crops when flip), h, w, C] -> flip-averaged softmax scores written into `out`,
