@@ -22,6 +22,8 @@
  *                               semseg_upsample_ce_ohem_*: the same with an OHEM cross-entropy criterion.
  *                               semseg_upsample_ce_{,ohem_}weighted_*: class weights / label smoothing.
  *                               semseg_upsample_ce_dice_*: soft Dice loss, alone or plus cross-entropy.
+ *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
+ *                               semseg_segsort_u32_pairs (segmented stable radix sort).
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -483,6 +485,46 @@ long long semseg_upsample_ce_dice_bwd_workspace_floats(int N, int Ho, int Wo, in
 int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                                 int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* table,
                                 const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Lovász-Softmax loss (Berman et al., CVPR 2018), alone or plus cross-entropy (semseg_b200/losses.py
+ * LovaszSoftmaxLoss), on the same fused upsample at zoom `zoom`. p = softmax(v) as the Dice passes compute it. A segment
+ * is one class over every valid pixel of the call (per_image = 0, S = C segments of L = N*Ho*Wo pixels) or one (image,
+ * class) pair (per_image = 1, S = N*C, L = Ho*Wo). Per segment, fg_i = [t_i = c], e_i = |fg_i - p_ic| (fp32),
+ * G = sum fg_i, the valid pixels sorted by e descending with ties by flat pixel index n*Ho*Wo + y*Wo + x ascending:
+ *   J_k = 1 - (G - A_k) / (G + B_k)  (A_k, B_k: fg / bg pixels among the first k; integer counts, fp64 J),  J_0 = 0
+ *   loss_seg = sum_k e_(k) (J_k - J_{k-1})
+ * classes_all = 0 ('present') averages over the segments with G > 0, classes_all = 1 over every segment of a scope
+ * (call or image) with a valid pixel; per_image averages the images' means over all N images. Plus ce_weight * CE (the
+ * mean over the call's valid pixels); loss 0 and an exactly zero gradient when no pixel is valid. The gradient holds the
+ * sort order fixed: gamma_ic = w_seg g_k sign(p_ic - fg_i) (sign(0) = 0),
+ *   dL/dv_ic = p_ic (gamma_ic - sum_c' p_ic' gamma_ic') + (ce_weight / n_valid) (p_ic - fg_i).
+ * Wo has the Dice limit (2389 at zoom 8) and N*Ho*Wo < 2^31; a bad shape, option or width is rejected before any launch.
+ *   fwd: loss_out[0] = loss, loss_out[1] = number of valid pixels; argmax (or NULL) and lse as the zoom forward's
+ *        (the same bits); gamma fp32 [N*Ho*Wo*C + 2] = w_seg g_k per pixel and class ([pixel][class], unsigned: the
+ *        backward applies the sign), then ce_weight / n_valid and 1; keep it for the backward.
+ *        workspace: semseg_upsample_ce_lovasz_workspace_floats() floats, 8-byte aligned, about (16 S L + 1 KB * S *
+ *        ceil(L / 4096)) bytes. After the call its words [0, S*L) hold each considered segment's sorted keys
+ *        (0x7FFFFFFF - bits(e), 0xFFFFFFFF for invalid pixels, which sort last) and [S*L, 2*S*L) their payloads
+ *        ((pixel index << 1) | fg); the segments of skipped (not considered) scopes are not written.
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits from the forward's lse and gamma; workspace:
+ *        semseg_upsample_ce_lovasz_bwd_workspace_floats() floats.
+ * The workspace functions return -1 for a bad zoom, size or per_image. */
+long long semseg_upsample_ce_lovasz_workspace_floats(int N, int Ho, int Wo, int C, int zoom, int per_image);
+int semseg_upsample_ce_lovasz_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                  int Ho, int Wo, int zoom, int ignore_index, int classes_all, int per_image,
+                                  float ce_weight, float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                  float* gamma, void* stream);
+long long semseg_upsample_ce_lovasz_bwd_workspace_floats(int N, int Ho, int Wo, int w, int C, int zoom);
+int semseg_upsample_ce_lovasz_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                  int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* gamma,
+                                  const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Segmented stable radix sort (csrc/segsort.cu): S segments of L (uint32 key, uint32 payload) pairs, [S][L], each sorted
+ * in place by key ascending, equal keys in input order. keys_alt / vals_alt: scratch of the same size. skip: NULL, or
+ * int [S] on the device, a non-zero entry leaves that segment untouched. workspace:
+ * semseg_segsort_u32_pairs_workspace_bytes() bytes = 1 KB * S * ceil(L / 4096). No host synchronisation, fixed launch
+ * geometry (graph-capturable), deterministic. 0 < L < 2^31; the workspace function returns -1 for bad sizes. */
+long long semseg_segsort_u32_pairs_workspace_bytes(int S, long long L);
+int semseg_segsort_u32_pairs(unsigned* keys, unsigned* vals, unsigned* keys_alt, unsigned* vals_alt, int S,
+                             long long L, const int* skip, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Sliding-window evaluation after the network (semseg_b200/inference.py, exact=False). No tensor cores, no atomics.

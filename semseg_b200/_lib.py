@@ -199,6 +199,14 @@ SIGNATURES = {
     "semseg_upsample_ce_dice_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_dice_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_lovasz_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_lovasz_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
+                                              c_int, c_int, c_int, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_lovasz_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_lovasz_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
+                                              c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_segsort_u32_pairs_workspace_bytes": (c_ll, [c_int, c_ll]),
+    "semseg_segsort_u32_pairs": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_ll, c_vp, c_vp, c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
     "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_vp, c_vp]),

@@ -34,6 +34,10 @@
 //
 // The soft Dice loss, alone or plus cross-entropy, runs the plain forward instance and its own statistics, reduce and
 // gradient kernels (see "Dice" below); no existing instance changes.
+//
+// The Lovász-Softmax loss, alone or plus cross-entropy, runs the plain forward instance, a key pass, the segmented stable
+// radix sort of csrc/segsort.cu and its own scan and gradient kernels (see "Lovász-Softmax" below); no existing
+// instance changes.
 #include <cmath>
 
 #include "host_common.h"
@@ -832,6 +836,464 @@ upsample_ce_dice_g_kernel(const float* __restrict__ logits, int pitch, int N, in
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- Lovász-Softmax
+// Lovász-Softmax (Berman, Triki, Blaschko, CVPR 2018), alone or plus ce_weight * cross-entropy. A segment is one class
+// over every valid pixel of the call, or one (image, class) pair with per_image. Per segment, with fg_i = [t_i = c],
+// e_i = |fg_i - p_ic| (fp32), G = sum fg_i and the valid pixels sorted by e descending, ties by flat pixel index:
+//   A_k, B_k = fg / bg counts among the first k,  J_k = 1 - (G - A_k) / (G + B_k),  J_0 = 0,  g_k = J_k - J_{k-1}
+//   loss_seg = sum_k e_(k) g_k,   loss = sum_seg w_seg loss_seg + ce_weight * CE
+// w_seg is 1 / (number of segments considered) (per_image: 1 / (N * the image's count)); 'present' considers the
+// segments with G > 0, 'all' every segment of a scope that has a valid pixel. With the sort order held fixed:
+//   gamma_ic = w_seg g_k sign(p_ic - fg_i),  Gamma_i = sum_c p_ic gamma_ic
+//   dL/dv_ic = p_ic (gamma_ic - Gamma_i) + lam (p_ic - fg_i),  lam = ce_weight / n_valid
+// Every pass computes p_ic the same way, the interpolation spelled out in explicit fmas (lovasz_v), so the key pass,
+// the Gamma pass and the rows kernel see the same bits and agree on every sign, zeros included.
+//   forward : the plain forward instance (lse, argmax, CE partials); a target histogram per image; one CTA turns it into
+//             the per-segment (skip, G, w) table; the key pass writes key = 0x7FFFFFFF - bits(e) (0xFFFFFFFF for an
+//             invalid pixel, sorted last) and payload = (pixel index << 1) | fg for each considered segment, in pixel
+//             order; the segmented stable radix sort (csrc/segsort.cu); per sorted tile the fg count, a per-segment
+//             scan of those counts, and the gradient pass (J_k in fp64 from integer counts, fp64 partials of e g_k,
+//             and the scatter of w_seg g_k into the kept gamma map [P][C]); one CTA reduces the loss in a fixed order.
+//   backward: Gamma_i (one warp per pixel, the sign applied from p), the rows kernel with (lse, t, Gamma) staged per
+//             pixel and gamma read per pixel-class, then the plain cols kernel.
+constexpr int kLovThreads = 256;
+constexpr int kLovItems = 16;
+constexpr int kLovTile = kLovThreads * kLovItems;   // sorted pairs per CTA of the scan passes
+constexpr unsigned kLovInvalidKey = 0xFFFFFFFFu;
+
+// The interpolated logit of output pixel (row r, column k) of an interval from its four node values.
+template <int Z>
+__device__ __forceinline__ float lovasz_h(float a, float b, int k) {
+  if constexpr (Z == 1) {
+    return a;
+  } else {
+    const float l1 = Zoom<Z>::kStep * k;
+    return fmaf(1.f - l1, a, __fmul_rn(l1, b));
+  }
+}
+template <int Z>
+__device__ __forceinline__ float lovasz_v(float top, float bot, int r) {
+  if constexpr (Z == 1) {
+    return top;
+  } else {
+    const float l1 = Zoom<Z>::kStep * r;
+    return fmaf(1.f - l1, top, __fmul_rn(l1, bot));
+  }
+}
+__device__ __forceinline__ float lovasz_sign(float p, float fg) { return p > fg ? 1.f : p < fg ? -1.f : 0.f; }
+
+// Valid pixels per (image, class) and per image: hist[n][C + 1] (zeroed by the caller; integer atomics).
+__global__ void __launch_bounds__(256)
+lovasz_target_hist_kernel(const long long* __restrict__ target, int HW, int C, int ignore_index,
+                          int* __restrict__ hist) {
+  __shared__ int s[kMaxClasses + 1];
+  const int n = blockIdx.y;
+  for (int c = threadIdx.x; c <= C; c += 256) s[c] = 0;
+  __syncthreads();
+  const long long* T = target + static_cast<size_t>(n) * HW;
+  const int base = blockIdx.x * kLovTile;
+  const int end = min(base + kLovTile, HW);
+  for (int i = base + threadIdx.x; i < end; i += 256) {
+    const long long t = T[i];
+    if (t != ignore_index && t >= 0 && t < C) {
+      atomicAdd(&s[t], 1);
+      atomicAdd(&s[C], 1);
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c <= C; c += 256)
+    if (s[c]) atomicAdd(&hist[n * (C + 1) + c], s[c]);
+}
+
+// One CTA, one thread per class: skip[seg], G[seg], w[seg] of every segment (seg = c, or n * C + c with per_image).
+__global__ void __launch_bounds__(kMaxClasses)
+lovasz_segments_kernel(const int* __restrict__ hist, int N, int C, int classes_all, int per_image,
+                       int* __restrict__ skip, int* __restrict__ seg_g, double* __restrict__ seg_w) {
+  const int c = threadIdx.x;
+  const bool cls = c < C;
+  if (!per_image) {
+    int g = 0, nv = 0;
+    for (int n = 0; n < N; ++n) {
+      if (cls) g += hist[n * (C + 1) + c];
+      nv += hist[n * (C + 1) + C];
+    }
+    const int cnt = classes_all ? (nv > 0 ? C : 0) : __syncthreads_count(cls && g > 0);
+    const bool considered = classes_all ? nv > 0 : g > 0;
+    if (cls) {
+      skip[c] = !considered;
+      seg_g[c] = g;
+      seg_w[c] = considered ? 1.0 / cnt : 0.0;
+    }
+    return;
+  }
+  for (int n = 0; n < N; ++n) {
+    const int g = cls ? hist[n * (C + 1) + c] : 0;
+    const int nv = hist[n * (C + 1) + C];
+    const int cnt = classes_all ? (nv > 0 ? C : 0) : __syncthreads_count(g > 0);
+    const bool considered = classes_all ? nv > 0 : g > 0;
+    if (cls) {
+      skip[n * C + c] = !considered;
+      seg_g[n * C + c] = g;
+      seg_w[n * C + c] = considered ? 1.0 / (static_cast<double>(N) * cnt) : 0.0;
+    }
+  }
+}
+
+// Forward layout (one CTA per 128 output columns, interval row, image; one thread per column and its Z rows): for every
+// considered segment, each pixel's sort key and payload at its position in the segment (pixel order).
+template <int Z>
+__global__ void __launch_bounds__(kFwdCols)
+lovasz_key_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
+                  const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                  const float* __restrict__ lse, int per_image, const int* __restrict__ skip,
+                  unsigned* __restrict__ keys, unsigned* __restrict__ vals) {
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs], then the skip flags of the image's C segments
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kFwdNodes, w - j_base);
+  const int tid = threadIdx.x;
+  int* s_skip = reinterpret_cast<int*>(S + G::kNodeRows * kFwdNodes * Cs);
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * kFwdNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
+  }
+  for (int c = tid; c < C; c += kFwdCols) s_skip[c] = skip[per_image ? n * C + c : c];
+  __syncthreads();
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x >= Wo) return;
+  const int j0 = x >> G::kShift;
+  const int j1 = min(j0 + 1, w - 1);
+  const int k = x & G::kMask;
+  const float* A = S + (j0 - j_base) * Cs;
+  const float* B = S + (j1 - j_base) * Cs;
+  const float* Cc = A + kFwdNodes * Cs;
+  const float* D = B + kFwdNodes * Cs;
+  const size_t L = per_image ? static_cast<size_t>(Ho) * Wo : static_cast<size_t>(N) * Ho * Wo;
+  float lse2[Z];
+  int t[Z];
+  unsigned pix[Z];
+#pragma unroll
+  for (int r = 0; r < Z; ++r) {
+    const size_t p = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+    pix[r] = static_cast<unsigned>(p);
+    t[r] = -1;
+    lse2[r] = 0.f;
+    if (r < rows) {
+      const long long tv = target[p];
+      t[r] = (tv == ignore_index || tv < 0 || tv >= C) ? -1 : static_cast<int>(tv);
+      lse2[r] = lse[p] * kLog2e;
+    }
+  }
+  const size_t local0 = per_image ? static_cast<size_t>(Z * i0) * Wo + x : pix[0];
+  for (int c = 0; c < C; ++c) {
+    if (s_skip[c]) continue;   // CTA-uniform
+    const float top = lovasz_h<Z>(A[c], B[c], k);
+    const float bot = Z == 1 ? 0.f : lovasz_h<Z>(Cc[c], D[c], k);
+    const size_t seg = per_image ? static_cast<size_t>(n) * C + c : c;
+    unsigned* K = keys + seg * L + local0;
+    unsigned* V = vals + seg * L + local0;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const float p = ex2_approx(fmaf(lovasz_v<Z>(top, bot, r), kLog2e, -lse2[r]));
+        const bool fg = t[r] == c;
+        const float e = fabsf((fg ? 1.f : 0.f) - p);
+        K[static_cast<size_t>(r) * Wo] = t[r] < 0 ? kLovInvalidKey : 0x7FFFFFFFu - __float_as_uint(e);
+        V[static_cast<size_t>(r) * Wo] = (pix[r] << 1) | (fg ? 1u : 0u);
+      }
+    }
+  }
+}
+
+// Block-wide exclusive scan of one value per thread (kLovThreads threads); returns the thread's prefix and, through
+// total, the block's sum. Integer adds: the order does not matter.
+__device__ __forceinline__ unsigned lovasz_block_scan(unsigned v, unsigned* total) {
+  __shared__ unsigned ws[kLovThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned inc = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += u;
+  }
+  if (lane == 31) ws[warp] = inc;
+  __syncthreads();
+  unsigned before = 0, all = 0;
+  for (int i = 0; i < kLovThreads / 32; ++i) {
+    if (i < warp) before += ws[i];
+    all += ws[i];
+  }
+  __syncthreads();
+  *total = all;
+  return before + inc - v;
+}
+
+// fg pairs per sorted tile -> fgcnt[seg][tile].
+__global__ void __launch_bounds__(kLovThreads)
+lovasz_fgcount_kernel(const unsigned* __restrict__ vals, int L, int nt, const int* __restrict__ skip,
+                      unsigned* __restrict__ fgcnt) {
+  const int seg = blockIdx.x / nt, tile = blockIdx.x % nt;
+  if (skip[seg]) return;
+  const unsigned* V = vals + static_cast<size_t>(seg) * L;
+  const int base = tile * kLovTile, end = min(base + kLovTile, L);
+  unsigned cnt = 0;
+  for (int i = base + threadIdx.x; i < end; i += kLovThreads) cnt += V[i] & 1u;
+  unsigned total;
+  lovasz_block_scan(cnt, &total);
+  if (threadIdx.x == 0) fgcnt[blockIdx.x] = total;
+}
+
+// One CTA per segment: the exclusive scan of its tiles' fg counts, in place.
+__global__ void __launch_bounds__(kLovThreads)
+lovasz_fgscan_kernel(unsigned* __restrict__ fgcnt, int nt, const int* __restrict__ skip) {
+  const int seg = blockIdx.x;
+  if (skip[seg]) return;
+  unsigned* F = fgcnt + static_cast<size_t>(seg) * nt;
+  const int chunk = (nt + kLovThreads - 1) / kLovThreads;
+  const int b = min(static_cast<int>(threadIdx.x) * chunk, nt), e = min(b + chunk, nt);
+  unsigned s = 0;
+  for (int i = b; i < e; ++i) s += F[i];
+  unsigned total;
+  unsigned run = lovasz_block_scan(s, &total);
+  for (int i = b; i < e; ++i) {
+    const unsigned c = F[i];
+    F[i] = run;
+    run += c;
+  }
+}
+
+// One CTA per (segment, sorted tile); thread t owns the tile's pairs t*kLovItems .. +kLovItems-1 (staged through
+// shared memory, one padding word per 32). Writes gamma[pix][c] = w_seg g_k for the valid pairs and the tile's fp64
+// partial of sum e g_k (a fixed-order reduction) to partial[seg][tile].
+__global__ void __launch_bounds__(kLovThreads)
+lovasz_grad_kernel(const unsigned* __restrict__ keys, const unsigned* __restrict__ vals, int L, int nt, int C,
+                   int per_image, const int* __restrict__ skip, const int* __restrict__ seg_g,
+                   const double* __restrict__ seg_w, const unsigned* __restrict__ fgbase, float* __restrict__ gamma,
+                   double* __restrict__ partial) {
+  __shared__ unsigned sk[kLovTile + kLovTile / 32];
+  __shared__ unsigned sv[kLovTile + kLovTile / 32];
+  __shared__ double red[kLovThreads / 32];
+  const int seg = blockIdx.x / nt, tile = blockIdx.x % nt;
+  if (skip[seg]) return;
+  const size_t off = static_cast<size_t>(seg) * L;
+  const int base = tile * kLovTile;
+  const int n = min(kLovTile, L - base);
+  for (int i = threadIdx.x; i < kLovTile; i += kLovThreads) {
+    sk[i + (i >> 5)] = i < n ? keys[off + base + i] : kLovInvalidKey;
+    sv[i + (i >> 5)] = i < n ? vals[off + base + i] : 0u;
+  }
+  __syncthreads();
+  const int i0 = threadIdx.x * kLovItems;
+  unsigned cnt = 0;
+#pragma unroll
+  for (int j = 0; j < kLovItems; ++j) cnt += sv[i0 + j + ((i0 + j) >> 5)] & 1u;
+  unsigned total;
+  unsigned a = fgbase[blockIdx.x] + lovasz_block_scan(cnt, &total);   // fg pairs before this thread's first
+  const double g_all = seg_g[seg], wv = seg_w[seg];
+  const int c = per_image ? seg % C : seg;
+  double acc = 0.0;
+  for (int j = 0; j < kLovItems; ++j) {
+    const int i = i0 + j;
+    const unsigned key = sk[i + (i >> 5)];
+    if (key == kLovInvalidKey) break;   // invalid pixels (and the tile's tail) sort last
+    const unsigned v = sv[i + (i >> 5)];
+    const unsigned fg = v & 1u;
+    const double k = static_cast<double>(base + i + 1);   // rank in the segment, 1-based
+    const double a1 = a + fg;
+    const double jk = 1.0 - (g_all - a1) / (g_all + (k - a1));
+    const double jp = k == 1.0 ? 0.0 : 1.0 - (g_all - a) / (g_all + (k - 1.0 - a));
+    const double gk = jk - jp;
+    acc += static_cast<double>(__uint_as_float(0x7FFFFFFFu - key)) * gk;
+    gamma[static_cast<size_t>(v >> 1) * C + c] = static_cast<float>(wv * gk);
+    a += fg;
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int i = 0; i < kLovThreads / 32; ++i) s += red[i];
+    partial[blockIdx.x] = s;
+  }
+}
+
+// One CTA: CE = (sum of the forward's CE partials) / n_valid and sum over the considered segments' tiles of
+// w_seg * partial, both fp64 in a fixed order -> loss_out = (L, n_valid), tail = (lam, 1).
+__global__ void __launch_bounds__(256)
+lovasz_loss_kernel(const float* __restrict__ ce_partial, int nblocks, const double* __restrict__ partial, int S, int nt,
+                   const int* __restrict__ skip, const double* __restrict__ seg_w, float ce_weight,
+                   float* __restrict__ loss_out, float* __restrict__ tail) {
+  __shared__ double sl[256];
+  __shared__ double sc[256];
+  __shared__ double st[256];
+  double l = 0.0, k = 0.0, t = 0.0;
+  for (int i = threadIdx.x; i < nblocks; i += 256) {
+    l += ce_partial[2 * i];
+    k += ce_partial[2 * i + 1];
+  }
+  const long long m = static_cast<long long>(S) * nt;
+  for (long long i = threadIdx.x; i < m; i += 256) {
+    const int seg = static_cast<int>(i / nt);
+    if (!skip[seg]) t += seg_w[seg] * partial[i];
+  }
+  sl[threadIdx.x] = l;
+  sc[threadIdx.x] = k;
+  st[threadIdx.x] = t;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      sl[threadIdx.x] += sl[threadIdx.x + o];
+      sc[threadIdx.x] += sc[threadIdx.x + o];
+      st[threadIdx.x] += st[threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double nv = sc[0];
+    const double ce = nv > 0.0 ? sl[0] / nv : 0.0;
+    loss_out[0] = static_cast<float>(st[0] + static_cast<double>(ce_weight) * ce);
+    loss_out[1] = static_cast<float>(nv);
+    tail[0] = nv > 0.0 ? static_cast<float>(ce_weight / nv) : 0.f;
+    tail[1] = 1.f;
+  }
+}
+
+// Gamma_i = sum_c p_ic gamma_ic, one warp per output pixel (0 for an invalid pixel): the lanes read the pixel's four
+// node vectors and its gamma row across the classes, a fixed shuffle tree sums them.
+template <int Z>
+__global__ void __launch_bounds__(256)
+lovasz_gamma_sum_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
+                        const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                        const float* __restrict__ lse, const float* __restrict__ gamma, float* __restrict__ gmap) {
+  using G = Zoom<Z>;
+  const long long P = static_cast<long long>(N) * Ho * Wo;
+  const long long pix = static_cast<long long>(blockIdx.x) * (256 / 32) + (threadIdx.x >> 5);
+  if (pix >= P) return;
+  const int lane = threadIdx.x & 31;
+  const int x = static_cast<int>(pix % Wo);
+  const long long ny = pix / Wo;
+  const int y = static_cast<int>(ny % Ho), n = static_cast<int>(ny / Ho);
+  const long long tv = target[pix];
+  if (tv == ignore_index || tv < 0 || tv >= C) {
+    if (lane == 0) gmap[pix] = 0.f;
+    return;
+  }
+  const int t = static_cast<int>(tv);
+  const int i0 = y >> G::kShift, r = y & G::kMask, j0 = x >> G::kShift, k = x & G::kMask;
+  const int i1 = min(i0 + 1, h - 1), j1 = min(j0 + 1, w - 1);
+  const float* A = logits + ((static_cast<size_t>(n) * h + i0) * w + j0) * pitch;
+  const float* B = logits + ((static_cast<size_t>(n) * h + i0) * w + j1) * pitch;
+  const float* Cc = logits + ((static_cast<size_t>(n) * h + i1) * w + j0) * pitch;
+  const float* D = logits + ((static_cast<size_t>(n) * h + i1) * w + j1) * pitch;
+  const float lse2 = lse[pix] * kLog2e;
+  const float* gr = gamma + static_cast<size_t>(pix) * C;
+  float s = 0.f;
+  for (int c = lane; c < C; c += 32) {
+    const float top = lovasz_h<Z>(A[c], B[c], k);
+    const float bot = Z == 1 ? 0.f : lovasz_h<Z>(Cc[c], D[c], k);
+    const float p = ex2_approx(fmaf(lovasz_v<Z>(top, bot, r), kLog2e, -lse2));
+    s = fmaf(p, gr[c] * lovasz_sign(p, c == t ? 1.f : 0.f), s);
+  }
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) gmap[pix] = s;
+}
+
+// One interval of the Lovász rows kernel for class c (the Dice rows kernel's layout and folding):
+// g = p (gamma sign - Gamma) + lam (p - fg) per valid pixel.
+template <int Z, bool kFull>
+__device__ __forceinline__ void lovasz_interval(const DicePix* s, const float* __restrict__ gam_row, int Wo, int C,
+                                                int xb, int rows, int nx, int c, float a, float b, float cc, float d,
+                                                float lam, float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float top = lovasz_h<Z>(a, b, k);
+    const float bot = Z == 1 ? 0.f : lovasz_h<Z>(cc, d, k);
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const DicePix pi = s[r * Wo + xb + k];
+      if (pi.t < 0) continue;  // warp-uniform
+      const float p = ex2_approx(fmaf(lovasz_v<Z>(top, bot, r), kLog2e, -pi.lse2));
+      const float fg = c == pi.t ? 1.f : 0.f;
+      const float gm = gam_row[(static_cast<size_t>(r) * Wo + xb + k) * C] * lovasz_sign(p, fg);
+      const float g = fmaf(p, gm - pi.g, lam * (p - fg));
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+// The rows kernel of the Lovász backward: one CTA per (interval row, image), one thread per class, (lse, t, Gamma)
+// of the interval's Z output rows staged as one 12-byte word per pixel -> T2 as upsample_ce_bwd_rows_kernel's.
+template <int Z>
+__global__ void __launch_bounds__(256)
+lovasz_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
+                   const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                   const float* __restrict__ lse, const float* __restrict__ gmap, const float* __restrict__ gamma,
+                   float* __restrict__ T2) {
+  extern __shared__ DicePix s_lpix[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const long long t = target[rowbase + x];
+      DicePix pi;
+      pi.t = (t == ignore_index || t < 0 || t >= C) ? -1 : static_cast<int>(t);
+      pi.lse2 = lse[rowbase + x] * kLog2e;
+      pi.g = gmap[rowbase + x];
+      s_lpix[r * Wo + x] = pi;
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const float lam = gamma[static_cast<size_t>(N) * Ho * Wo * C];
+  const float* gam_row = gamma + (static_cast<size_t>(n) * Ho + Z * i0) * Wo * C + c;
+  const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
+  const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  float a = L0[0], cc = L1[0];
+  float nb = L0[static_cast<size_t>(min(1, w - 1)) * pitch], nd = L1[static_cast<size_t>(min(1, w - 1)) * pitch];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd;
+    const int jn = min(j0 + 2, w - 1);
+    nb = L0[static_cast<size_t>(jn) * pitch];
+    nd = L1[static_cast<size_t>(jn) * pitch];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      lovasz_interval<Z, true>(s_lpix, gam_row, Wo, C, xb, rows, nx, c, a, b, cc, d, lam, acc);
+    } else {
+      lovasz_interval<Z, false>(s_lpix, gam_row, Wo, C, xb, rows, nx, c, a, b, cc, d, lam, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -1332,6 +1794,190 @@ extern "C" int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N
                                       workspace, dlogits, stream);
     default: return launch_dice_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
                                        workspace, dlogits, stream);
+  }
+}
+
+// Lovász-Softmax (+ ce_weight * CE) at zoom factor `zoom`. The rows kernel stages the Dice rows kernel's 12-byte words:
+// the Dice width limit. Payloads hold the flat pixel index in 31 bits: N * Ho * Wo < 2^31.
+static int check_lovasz(int N, int Ho, int Wo, int C, int zoom, int classes_all, int per_image, float ce_weight) {
+  SB_CHECK_ARG(classes_all == 0 || classes_all == 1, "upsample_ce_lovasz: classes_all %d is not 0 or 1", classes_all);
+  SB_CHECK_ARG(per_image == 0 || per_image == 1, "upsample_ce_lovasz: per_image %d is not 0 or 1", per_image);
+  SB_CHECK_ARG(static_cast<long long>(N) * Ho * Wo < (1LL << 31), "upsample_ce_lovasz: %d x %d x %d pixels exceed 2^31",
+               N, Ho, Wo);
+  int r = check_dice(zoom, Wo, 0.f, 0.f, ce_weight);
+  if (r) return r;
+  const int S = per_image ? N * C : C;
+  const long long L = per_image ? static_cast<long long>(Ho) * Wo : static_cast<long long>(N) * Ho * Wo;
+  return semseg_segsort_u32_pairs_workspace_bytes(S, L) < 0 ? SEMSEG_E_INVALID : SEMSEG_OK;
+}
+
+// Forward workspace, in 4-byte words (8-byte aligned base): sorted keys [S][L] at 0, payloads [S][L] at S*L, the sort's
+// second key / payload buffers, the sort workspace, the target histogram [N][C+1], skip[S], G[S], w[S] (fp64), the fg
+// tile counts [S][nt], the fp64 tile partials [S][nt], then the CE partials (2 per forward CTA).
+struct LovaszWs {
+  int S, nt;
+  long long L, sort, hist, skip, g, w, fgcnt, partial, ce, total;
+  LovaszWs(int N, int Ho, int Wo, int C, int zoom, int per_image) {
+    S = per_image ? N * C : C;
+    L = per_image ? static_cast<long long>(Ho) * Wo : static_cast<long long>(N) * Ho * Wo;
+    nt = static_cast<int>((L + kLovTile - 1) / kLovTile);
+    const long long SL = static_cast<long long>(S) * L;
+    auto even = [](long long v) { return (v + 1) & ~1LL; };
+    sort = even(4 * SL);
+    hist = sort + even(semseg_segsort_u32_pairs_workspace_bytes(S, L) / 4);
+    skip = hist + static_cast<long long>(N) * (C + 1);
+    g = skip + S;
+    w = even(g + S);
+    fgcnt = w + 2LL * S;
+    partial = even(fgcnt + static_cast<long long>(S) * nt);
+    ce = partial + 2LL * S * nt;
+    total = ce + 2LL * fwd_ctas(N, (Ho - 1) / zoom + 1, Wo);
+  }
+};
+
+template <int Z>
+static int launch_lovasz_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                             int Wo, int ignore_index, int classes_all, int per_image, float ce_weight,
+                             float* workspace, float* loss_out, int64_t* argmax, float* lse, float* gamma,
+                             cudaStream_t stream) {
+  const LovaszWs ws(N, Ho, Wo, C, Z, per_image);
+  const long long SL = static_cast<long long>(ws.S) * ws.L;
+  const long long P = static_cast<long long>(N) * Ho * Wo;
+  unsigned* keys = reinterpret_cast<unsigned*>(workspace);
+  unsigned* vals = keys + SL;
+  int* hist = reinterpret_cast<int*>(workspace + ws.hist);
+  int* skip = reinterpret_cast<int*>(workspace + ws.skip);
+  int* seg_g = reinterpret_cast<int*>(workspace + ws.g);
+  double* seg_w = reinterpret_cast<double*>(workspace + ws.w);
+  unsigned* fgcnt = reinterpret_cast<unsigned*>(workspace + ws.fgcnt);
+  double* partial = reinterpret_cast<double*>(workspace + ws.partial);
+  float* ce = workspace + ws.ce;
+  const long long* tgt = reinterpret_cast<const long long*>(target);
+  int r = launch_fwd_kernel<Z, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ce, argmax, lse,
+                                      nullptr, nullptr, stream);
+  if (r) return r;
+  SB_CUDA(cudaMemsetAsync(hist, 0, sizeof(int) * N * (C + 1), stream));
+  lovasz_target_hist_kernel<<<dim3(cdiv(Ho * Wo, kLovTile), N), 256, 0, stream>>>(tgt, Ho * Wo, C, ignore_index, hist);
+  SB_LAUNCHED();
+  lovasz_segments_kernel<<<1, kMaxClasses, 0, stream>>>(hist, N, C, classes_all, per_image, skip, seg_g, seg_w);
+  SB_LAUNCHED();
+  SB_CUDA(cudaMemsetAsync(gamma, 0, sizeof(float) * P * C, stream));
+  const int Cs = C | 1;
+  const size_t smem = (static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs + C) * sizeof(float);
+  constexpr size_t kMaxSmem =
+      (static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) + kMaxClasses) * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    r = opt_in_smem(lovasz_key_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  lovasz_key_kernel<Z><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, tgt, Ho, Wo, ignore_index, lse, per_image, skip, keys, vals);
+  SB_LAUNCHED();
+  r = semseg_segsort_u32_pairs(keys, vals, keys + 2 * SL, keys + 3 * SL, ws.S, ws.L, skip, workspace + ws.sort,
+                               stream);
+  if (r) return r;
+  const int ctas = ws.S * ws.nt;
+  const int Li = static_cast<int>(ws.L);
+  lovasz_fgcount_kernel<<<ctas, kLovThreads, 0, stream>>>(vals, Li, ws.nt, skip, fgcnt);
+  SB_LAUNCHED();
+  lovasz_fgscan_kernel<<<ws.S, kLovThreads, 0, stream>>>(fgcnt, ws.nt, skip);
+  SB_LAUNCHED();
+  lovasz_grad_kernel<<<ctas, kLovThreads, 0, stream>>>(keys, vals, Li, ws.nt, C, per_image, skip, seg_g, seg_w, fgcnt,
+                                                       gamma, partial);
+  SB_LAUNCHED();
+  lovasz_loss_kernel<<<1, 256, 0, stream>>>(ce, fwd_ctas(N, h, Wo), partial, ws.S, ws.nt, skip, seg_w, ce_weight,
+                                            loss_out, gamma + P * C);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+// Backward workspace: T2 [N][h][2][w][C] of the rows kernel, then the Gamma map [N][Ho][Wo] (the Dice backward's).
+template <int Z>
+static int launch_lovasz_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                             int Wo, int ignore_index, const float* lse, const float* gamma, const float* grad_out,
+                             float* workspace, float* dlogits, cudaStream_t stream) {
+  float* gmap = workspace + 2LL * N * h * w * C;
+  const long long P = static_cast<long long>(N) * Ho * Wo;
+  const long long* tgt = reinterpret_cast<const long long*>(target);
+  lovasz_gamma_sum_kernel<Z><<<static_cast<unsigned>((P + 7) / 8), 256, 0, stream>>>(
+      logits, pitch, N, h, w, C, tgt, Ho, Wo, ignore_index, lse, gamma, gmap);
+  SB_LAUNCHED();
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(DicePix);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(lovasz_rows_kernel<Z>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  lovasz_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(logits, pitch, N, h, w, C, tgt, Ho, Wo, ignore_index,
+                                                               lse, gmap, gamma, workspace);
+  SB_LAUNCHED();
+  // gamma[P*C + 1] = 1: the plain cols kernel's count, so dlogits = grad_out[0] * T2 sums
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, gamma + P * C, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_lovasz_workspace_floats(int N, int Ho, int Wo, int C, int zoom,
+                                                                int per_image) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_lovasz: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && C > 0 && C <= kMaxClasses, "upsample_ce_lovasz: bad sizes");
+  int r = check_lovasz(N, Ho, Wo, C, zoom, 0, per_image, 0.f);
+  if (r) return r;
+  return LovaszWs(N, Ho, Wo, C, zoom, per_image).total;
+}
+
+extern "C" int semseg_upsample_ce_lovasz_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                             const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                             int classes_all, int per_image, float ce_weight, float* workspace,
+                                             float* loss_out, int64_t* argmax, float* lse, float* gamma,
+                                             void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_lovasz(N, Ho, Wo, C, zoom, classes_all, per_image, ce_weight);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && gamma, "upsample_ce_lovasz_fwd: null output");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0,
+               "upsample_ce_lovasz_fwd: workspace not 8-byte aligned");
+  switch (zoom) {
+    case 1: return launch_lovasz_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, classes_all,
+                                        per_image, ce_weight, workspace, loss_out, argmax, lse, gamma, stream);
+    case 2: return launch_lovasz_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, classes_all,
+                                        per_image, ce_weight, workspace, loss_out, argmax, lse, gamma, stream);
+    case 4: return launch_lovasz_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, classes_all,
+                                        per_image, ce_weight, workspace, loss_out, argmax, lse, gamma, stream);
+    default: return launch_lovasz_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, classes_all,
+                                         per_image, ce_weight, workspace, loss_out, argmax, lse, gamma, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_lovasz_bwd_workspace_floats(int N, int Ho, int Wo, int w, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_lovasz: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && w > 0 && C > 0, "upsample_ce_lovasz: bad sizes");
+  return 2LL * N * ((Ho - 1) / zoom + 1) * w * C + static_cast<long long>(N) * Ho * Wo;
+}
+
+extern "C" int semseg_upsample_ce_lovasz_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                             const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                             const float* lse, const float* gamma, const float* grad_out,
+                                             float* workspace, float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_lovasz(N, Ho, Wo, C, zoom, 0, 0, 0.f);
+  if (r) return r;
+  SB_CHECK_ARG(lse && gamma && grad_out && workspace && dlogits, "upsample_ce_lovasz_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_lovasz_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, gamma, grad_out,
+                                        workspace, dlogits, stream);
+    case 2: return launch_lovasz_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, gamma, grad_out,
+                                        workspace, dlogits, stream);
+    case 4: return launch_lovasz_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, gamma, grad_out,
+                                        workspace, dlogits, stream);
+    default: return launch_lovasz_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, gamma,
+                                         grad_out, workspace, dlogits, stream);
   }
 }
 

@@ -602,6 +602,27 @@ class _UpsampleCEDice(torch.autograd.Function):
         return dl, None, None, None, None, None, None
 
 
+class _UpsampleCELovasz(torch.autograd.Function):
+    """The fused tail with losses.LovaszSoftmaxLoss, plus ce_weight * CE. The forward keeps the per pixel-class
+    Lovász gradient weights (gamma, 4 C bytes per output pixel) it scattered from the sorted segments; the sort's
+    buffers are released when it returns."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, classes_all, per_image, ce_weight):
+        info, amax, lse, gamma = ops.upsample_ce_lovasz_fwd(logits, target, ignore_index, classes_all, per_image,
+                                                            ce_weight, zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, gamma)
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, gamma = ctx.saved_tensors
+        dl = ops.upsample_ce_lovasz_bwd(logits, target, ctx.ignore_index, lse, gamma, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None, None
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""
@@ -621,8 +642,9 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     label_smoothing), losses.OhemCrossEntropyLoss (with or without class weights) and losses.DiceLoss, at every zoom
     factor of the model (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits. The
     weighted / smoothed forms need the target on a CUDA device and class weights as a contiguous fp32 [classes] tensor
-    on that device; any other weight, another reduction, and any subclass keep the ATen tail. DiceLoss also needs the
-    target no wider than its kernels stage (2389 columns at zoom 8).
+    on that device; any other weight, another reduction, and any subclass keep the ATen tail. DiceLoss and
+    losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage (2389 columns at zoom 8), and the
+    Lovász loss fewer than 2^31 target pixels.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is nn.CrossEntropyLoss:
         eps = getattr(criterion, 'label_smoothing', 0.0)
@@ -632,6 +654,11 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     elif type(criterion) is losses.DiceLoss:
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
+    elif type(criterion) is losses.LovaszSoftmaxLoss:
+        # the Lovász rows kernel stages the Dice words; its sort payloads hold a pixel index in 31 bits
+        ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
+              _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES and
+              target.numel() < 2 ** 31)
     else:
         ok = type(criterion) is losses.OhemCrossEntropyLoss
     if not (ok and zoom_factor in (1, 2, 4, 8)
@@ -653,7 +680,11 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None):
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
     weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
-    with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index). The default criterion runs the plain kernels."""
+    with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index); with a losses.LovaszSoftmaxLoss, its
+    Lovász-Softmax (+ CE) loss. The default criterion runs the plain kernels."""
+    if isinstance(criterion, losses.LovaszSoftmaxLoss):
+        return _UpsampleCELovasz.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                       criterion.classes == 'all', bool(criterion.per_image), criterion.ce_weight)
     if isinstance(criterion, losses.DiceLoss):
         return _UpsampleCEDice.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.smooth,
                                      criterion.eps, criterion.ce_weight)

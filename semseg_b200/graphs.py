@@ -18,8 +18,8 @@ step counter incremented inside the graph — csrc/bn.cu st_ll / ld_ll) and drop
 Limits (same as torch.cuda.make_graphed_callables): a second training forward before the backward of the first one
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
-cross-entropy with or without class weights and label smoothing, OHEM cross-entropy and the Dice loss) are not captured
-(such models simply stay eager).
+cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss and the Lovász-Softmax
+loss) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -271,12 +271,13 @@ def train_step(model, impl, x, y):
     bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
     # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
     # the criterion's options are launch arguments baked into the graph: a changed thresh, ignore_index,
-    # label_smoothing or Dice smooth / eps / ce_weight captures anew, and so does a replaced class-weight tensor (its
-    # address is baked in); an in-place edit of the weights needs no capture, the kernels read them at every replay
+    # label_smoothing, Dice smooth / eps / ce_weight or Lovász classes / per_image captures anew, and so does a replaced
+    # class-weight tensor (its address is baked in); an in-place edit of the weights needs no capture, the kernels read
+    # them at every replay
     crit = getattr(model, "criterion", None)
     crit_key = (type(crit),) + tuple(getattr(crit, a, None) for a in ("ignore_index", "thresh", "min_kept",
                                                                       "label_smoothing", "reduction", "smooth", "eps",
-                                                                      "ce_weight"))
+                                                                      "ce_weight", "classes", "per_image"))
     cw = getattr(crit, "weight", None)
     crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),

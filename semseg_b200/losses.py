@@ -4,7 +4,7 @@ OhemCrossEntropyLoss is online hard-pixel mining: only the pixels the network is
 the network's fused tail (functional.upsample_ce) it runs inside the same kernels as the default loss, graphed at every
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
-runs the same way.
+and LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, run the same way.
 """
 import math
 
@@ -133,6 +133,67 @@ class DiceLoss(nn.Module):
                                % (logits.device, target.device))
         if logits.dtype != torch.float32 or target.dtype != torch.int64:
             raise TypeError("DiceLoss: fp32 logits and int64 target expected, got %s and %s" %
+                            (logits.dtype, target.dtype))
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+class LovaszSoftmaxLoss(nn.Module):
+    """Lovász-Softmax loss (Berman, Triki, Blaschko, CVPR 2018), the standard surrogate for mIoU, optionally plus
+    cross-entropy, for logits [N, C, H, W] and target [N, H, W]:
+
+        valid    = target != ignore_index and 0 <= target < C     (other out-of-range targets are skipped)
+        p        = softmax(logits) over C
+        segment  = one class over every valid pixel of the call, or one (image, class) pair with per_image
+        fg_i     = [target_i = c],  e_i = |fg_i - p_ic|,  G = sum fg_i                         per segment
+        sort the valid pixels by e descending, ties by flat pixel index (torch.sort(stable=True) over Berman's order)
+        J_k      = 1 - (G - A_k) / (G + B_k),  J_0 = 0   (A_k, B_k: fg / bg pixels among the first k)
+        loss_seg = sum_k e_(k) (J_k - J_{k-1})
+        loss     = mean of loss_seg over the considered segments + ce_weight * CE
+
+    classes='present' considers the segments with G > 0; classes='all' every class (an absent class scores
+    max_i p_ic). per_image=True averages each image's segments and then the N images; an image with no valid pixel adds 0
+    and still counts in 1/N. CE is the mean cross-entropy over the valid pixels. With no valid pixel the loss is 0 and
+    every gradient is 0. The counts are integers and J is float64, so the loss stays exact past 2^24 pixels per segment.
+    Under DistributedDataParallel each rank computes its own loss. The gradient is autograd's with the sort order held
+    fixed (torch's |x| backward: a pixel with e = 0 gets no Lovász gradient).
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels with an on-device segmented
+    radix sort, graphed at every zoom factor; called as a module (validate()) it runs their zoom-1 form on an NHWC copy
+    of the logits. CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback. The forward needs
+    about 16 C bytes per output pixel of transient workspace and keeps 4 C bytes per output pixel for the backward."""
+
+    def __init__(self, ignore_index=255, classes='present', per_image=False, ce_weight=0.0):
+        super(LovaszSoftmaxLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        if not isinstance(classes, str):
+            raise TypeError("classes must be 'present' or 'all', got %r" % (classes,))
+        if classes not in ('present', 'all'):
+            raise ValueError("classes must be 'present' or 'all', got %r" % (classes,))
+        if not isinstance(per_image, bool):
+            raise TypeError("per_image must be a bool, got %r" % (per_image,))
+        self.ignore_index = ignore_index
+        self.classes = classes
+        self.per_image = per_image
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+
+    def extra_repr(self):
+        return "ignore_index=%d, classes=%r, per_image=%s, ce_weight=%g" % (self.ignore_index, self.classes,
+                                                                            self.per_image, self.ce_weight)
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        if logits.dim() != 4 or target.dim() != 3 or target.shape != logits.shape[:1] + logits.shape[2:]:
+            raise ValueError("LovaszSoftmaxLoss: logits [N, C, H, W] and target [N, H, W] expected, got %s and %s" %
+                             (tuple(logits.shape), tuple(target.shape)))
+        if logits.shape[1] > 256:
+            raise ValueError("LovaszSoftmaxLoss: at most 256 classes (got %d); no fallback" % logits.shape[1])
+        if not (logits.is_cuda and target.is_cuda):
+            raise RuntimeError("LovaszSoftmaxLoss runs on the native CUDA kernels only (no CPU fallback); got %s, %s"
+                               % (logits.device, target.device))
+        if logits.dtype != torch.float32 or target.dtype != torch.int64:
+            raise TypeError("LovaszSoftmaxLoss: fp32 logits and int64 target expected, got %s and %s" %
                             (logits.dtype, target.dtype))
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
         return loss

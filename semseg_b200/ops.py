@@ -841,6 +841,71 @@ def upsample_ce_dice_bwd(logits, target, ignore_index, lse, table, grad_out, zoo
     return dl
 
 
+def upsample_ce_lovasz_fwd(logits, target, ignore_index, classes_all, per_image, ce_weight, want_argmax=True, zoom=8,
+                           return_workspace=False):
+    """Lovász-Softmax loss (+ ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract) ->
+    (loss_info [2] = (loss, valid count), argmax, lse, gamma [N*H*W*C + 2]); with return_workspace also the forward
+    workspace, whose first 2 S L words are the sorted keys and payloads of every considered segment."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_lovasz_workspace_floats(n, ho, wo, c, int(zoom), int(bool(per_image))))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_lovasz_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    gamma = torch.empty((n * ho * wo * c + 2,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse = torch.empty((n, ho, wo), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_upsample_ce_lovasz_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                 int(zoom), int(ignore_index), int(bool(classes_all)),
+                                                 int(bool(per_image)), float(ce_weight), _ptr(ws), _ptr(info),
+                                                 _ptr(amax), _ptr(lse), _ptr(gamma), _stream()),
+               "semseg_upsample_ce_lovasz_fwd")
+    if return_workspace:
+        return info, amax, lse, gamma, ws
+    return info, amax, lse, gamma
+
+
+def upsample_ce_lovasz_bwd(logits, target, ignore_index, lse, gamma, grad_out, zoom=8):
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_lovasz_bwd_workspace_floats(n, ho, wo, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_lovasz_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_lovasz_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                 int(zoom), int(ignore_index), _ptr(lse), _ptr(gamma), _ptr(g),
+                                                 _ptr(ws), _ptr(dl), _stream()),
+               "semseg_upsample_ce_lovasz_bwd")
+    return dl
+
+
+def segsort_u32_pairs(keys, vals, skip=None):
+    """Stable sort of each row of the int32 [S, L] CUDA tensors `keys` / `vals` (uint32 bit patterns) by key, in place;
+    rows whose int32 `skip` [S] entry is non-zero are left untouched."""
+    _require_cuda(keys, vals)
+    lib = _lib.load()
+    assert keys.dtype == vals.dtype == torch.int32 and keys.shape == vals.shape and keys.dim() == 2
+    assert keys.is_contiguous() and vals.is_contiguous()
+    s, l = keys.shape
+    nb = int(lib.semseg_segsort_u32_pairs_workspace_bytes(s, l))
+    _lib.check(0 if nb >= 0 else nb, "semseg_segsort_u32_pairs_workspace_bytes")
+    ws = torch.empty((nb,), dtype=torch.uint8, device=keys.device)
+    ka, va = torch.empty_like(keys), torch.empty_like(vals)
+    if skip is not None:
+        assert skip.dtype == torch.int32 and skip.is_contiguous() and skip.numel() == s
+    _lib.check(lib.semseg_segsort_u32_pairs(_ptr(keys), _ptr(vals), _ptr(ka), _ptr(va), s, l, _ptr(skip), _ptr(ws),
+                                            _stream()),
+               "semseg_segsort_u32_pairs")
+    return keys, vals
+
+
 # ------------------------------------------------------------------------------------------------ sliding-window evaluation
 def window_scores(logits, flip, out):
     """fp32 NHWC logits [G (+G mirrored crops when flip), h, w, C] -> flip-averaged softmax scores written into `out`,
