@@ -24,6 +24,7 @@
  *                               semseg_upsample_ce_dice_*: soft Dice loss, alone or plus cross-entropy.
  *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
+ *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -517,6 +518,28 @@ long long semseg_upsample_ce_lovasz_bwd_workspace_floats(int N, int Ho, int Wo, 
 int semseg_upsample_ce_lovasz_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                                   int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* gamma,
                                   const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Pixel-wise knowledge distillation (semseg_b200/losses.py DistillationLoss) on the same fused upsample at zoom `zoom`:
+ * student and teacher are fp32 NHWC [N,h,w,C] maps, each with its own pitch (>= C), both upsampled as the zoom forward
+ * upsamples (zoom 1: the maps themselves). With T = temperature > 0, p = softmax(s/T), q = softmax(t/T) per output pixel
+ * and P = N*Ho*Wo (every pixel; there is no target):
+ *   KL = (1/P) sum_pix sum_c q_c (log q_c - log p_c),  log p_c = (s_c - max s)/T - log sum_c' exp((s_c' - max s)/T)
+ * so s = t gives a KL and a gradient of exactly 0. The backward stages 8 bytes per pixel: Wo <= 2560 at zoom 8.
+ *   fwd: kl_out[0] = KL, kl_out[1] = P; lse fp32 [N,Ho,Wo,2] = (lse(s/T), lse(t/T)) per pixel, keep it for the backward;
+ *        workspace: semseg_upsample_kd_workspace_floats() floats.
+ *   bwd: ADDS grad_out[0] * kd_weight * T * (p_c - q_c) / P, the gradient of kd_weight * T^2 * KL with respect to the
+ *        student map, into dlogits fp32 [N,h,w,C] (dense), which the caller has filled (e.g. with the cross-entropy
+ *        gradient); the teacher gets no gradient. workspace: semseg_upsample_kd_bwd_workspace_floats() floats.
+ * Both reject a bad shape, zoom, temperature, kd_weight, pitch, width or null pointer before any CUDA call; the workspace
+ * functions return -1 for a zoom outside {1, 2, 4, 8} or a bad size. No host synchronisation (graph-capturable), no
+ * atomics: deterministic. */
+long long semseg_upsample_kd_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_kd_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                           int C, int Ho, int Wo, int zoom, float temperature, float* workspace, float* kl_out,
+                           float* lse, void* stream);
+long long semseg_upsample_kd_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_kd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                           int C, int Ho, int Wo, int zoom, float temperature, float kd_weight, const float* lse,
+                           const float* grad_out, float* workspace, float* dlogits, void* stream);
 /* Segmented stable radix sort (csrc/segsort.cu): S segments of L (uint32 key, uint32 payload) pairs, [S][L], each sorted
  * in place by key ascending, equal keys in input order. keys_alt / vals_alt: scratch of the same size. skip: NULL, or
  * int [S] on the device, a non-zero entry leaves that segment untouched. workspace:

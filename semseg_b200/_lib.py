@@ -205,6 +205,12 @@ SIGNATURES = {
     "semseg_upsample_ce_lovasz_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_lovasz_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                               c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_kd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_kd_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f,
+                                       c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_kd_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_kd_bwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f,
+                                       c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_segsort_u32_pairs_workspace_bytes": (c_ll, [c_int, c_ll]),
     "semseg_segsort_u32_pairs": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_ll, c_vp, c_vp, c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),

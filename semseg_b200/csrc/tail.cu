@@ -1294,6 +1294,258 @@ lovasz_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, in
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- distillation
+// Pixel-wise knowledge distillation from a frozen teacher: the student logits s and the teacher logits t, both upsampled
+// xZ exactly as the cross-entropy forward upsamples (Z = 1: the maps themselves), T the temperature, every pixel of
+// every image (no target), P pixels in all:
+//   log p_c = (s_c - m_s)/T - log Z_s,  Z_s = sum_c exp((s_c - m_s)/T),  m_s = max_c s_c     (log q_c likewise from t)
+//   KL = (1/P) sum_pix sum_c q_c (log q_c - log p_c),   dKL/ds_c = (p_c - q_c) / (T P)
+// Each log-probability is formed from its own shifted logit, never as a difference of two large sums, so s = t gives
+// log q_c - log p_c = 0 bit for bit: a KL and a gradient of exactly 0.
+//   forward : one CTA per (kKdCols output columns, interval row, image), the node rows of both maps staged side by side,
+//             three class passes per pixel (max; the two sums of exp; the KL terms: three MUFU per pixel-class), fp32
+//             within the CTA, one (sum KL, pixels) partial per CTA and the plain fp64 reduce; (lse_s/T, lse_t/T) saved per
+//             pixel. 64 columns at Z <= 2, so that two maps of 256 classes fit in shared memory.
+//   backward: the rows layout of upsample_ce_bwd_rows_kernel (one thread per class, both maps' node values in
+//             registers, (lse_s/T, lse_t/T) log2(e) staged per pixel, two MUFU per pixel-class), then a cols kernel that
+//             ADDS grad_out[0] kd_weight T / P times the adjoint into dlogits, which already holds the CE gradient.
+template <int Z>
+struct KdGeom {
+  static constexpr int kCols = Z <= 2 ? 64 : 128;   // output columns per forward CTA
+  static constexpr int kNodes = kCols / Z + 1;
+};
+
+template <int Z>
+__global__ void __launch_bounds__(KdGeom<Z>::kCols)
+upsample_kd_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* __restrict__ tl, int pitch_t, int N, int h,
+                       int w, int C, int Cs, int Ho, int Wo, float inv_t, float* __restrict__ partial,
+                       float2* __restrict__ lse_out) {
+  using G = Zoom<Z>;
+  constexpr int kCols = KdGeom<Z>::kCols, kNodes = KdGeom<Z>::kNodes;
+  extern __shared__ float S[];  // [2 maps: student, teacher][kNodeRows][kNodes][Cs]
+  __shared__ float red_kl[kCols / 32];
+  __shared__ float red_cnt[kCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kNodes, w - j_base);
+  const int tid = threadIdx.x;
+  const int map_floats = G::kNodeRows * kNodes * Cs;
+  for (int idx = tid; idx < 2 * G::kNodeRows * nj * C; idx += kCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = (node / nj) % G::kNodeRows, map = node / (nj * G::kNodeRows);
+    const size_t src = (static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj);
+    S[map * map_floats + (rr * kNodes + jj) * Cs + c] = map ? tl[src * pitch_t + c] : sl[src * pitch_s + c];
+  }
+  __syncthreads();
+  float kl_sum = 0.f, cnt = 0.f;
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* As = S + (j0 - j_base) * Cs;   // student nodes (i0, j0), (i0, j1), (i1, j0), (i1, j1)
+    const float* Bs = S + (j1 - j_base) * Cs;
+    const float* Cs_ = As + kNodes * Cs;
+    const float* Ds = Bs + kNodes * Cs;
+    const float* At = As + map_floats;           // teacher nodes
+    const float* Bt = Bs + map_floats;
+    const float* Ct = Cs_ + map_floats;
+    const float* Dt = Ds + map_floats;
+    const float k2 = inv_t * kLog2e;
+    float ms[Z], mt[Z], zs[Z], zt[Z], kl[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      ms[r] = -INFINITY;
+      mt[r] = -INFINITY;
+      zs[r] = 0.f;
+      zt[r] = 0.f;
+      kl[r] = 0.f;
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float ts = Z == 1 ? As[c] : l0w * As[c] + l1w * Bs[c];
+      const float bs = Z == 1 ? 0.f : l0w * Cs_[c] + l1w * Ds[c];
+      const float tt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
+      const float bt = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        ms[r] = fmaxf(ms[r], row_lerp<Z>(ts, bs, r));
+        mt[r] = fmaxf(mt[r], row_lerp<Z>(tt, bt, r));
+      }
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float ts = Z == 1 ? As[c] : l0w * As[c] + l1w * Bs[c];
+      const float bs = Z == 1 ? 0.f : l0w * Cs_[c] + l1w * Ds[c];
+      const float tt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
+      const float bt = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        zs[r] += ex2_approx((row_lerp<Z>(ts, bs, r) - ms[r]) * k2);
+        zt[r] += ex2_approx((row_lerp<Z>(tt, bt, r) - mt[r]) * k2);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      zs[r] = logf(zs[r]);   // log Z_s, log Z_t from here on
+      zt[r] = logf(zt[r]);
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float ts = Z == 1 ? As[c] : l0w * As[c] + l1w * Bs[c];
+      const float bs = Z == 1 ? 0.f : l0w * Cs_[c] + l1w * Ds[c];
+      const float tt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
+      const float bt = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float lp = (row_lerp<Z>(ts, bs, r) - ms[r]) * inv_t - zs[r];
+        const float lq = (row_lerp<Z>(tt, bt, r) - mt[r]) * inv_t - zt[r];
+        kl[r] = fmaf(ex2_approx(lq * kLog2e), lq - lp, kl[r]);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+        lse_out[pix] = make_float2(fmaf(ms[r], inv_t, zs[r]), fmaf(mt[r], inv_t, zt[r]));
+        kl_sum += kl[r];
+        cnt += 1.f;
+      }
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    kl_sum += __shfl_xor_sync(0xffffffffu, kl_sum, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((tid & 31) == 0) {
+    red_kl[tid >> 5] = kl_sum;
+    red_cnt[tid >> 5] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float l = 0.f, k = 0.f;
+    for (int i = 0; i < kCols / 32; ++i) {
+      l += red_kl[i];
+      k += red_cnt[i];
+    }
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[2 * b] = l;
+    partial[2 * b + 1] = k;
+  }
+}
+
+// One interval (Z columns of Z rows; fewer at the last node row / column when !kFull) of the distillation rows kernel
+// for class c: acc = the (left, right) x (top, bottom node row) sums of p_c - q_c, as in upsample_ce_bwd_rows_kernel.
+template <int Z, bool kFull>
+__device__ __forceinline__ void kd_interval(const float2* s, int Wo, int xb, int rows, int nx, float k2, float a,
+                                            float b, float cc, float d, float at, float bt, float ct, float dt,
+                                            float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    const float topt = l0w * at + l1w * bt;
+    const float bott = l0w * ct + l1w * dt;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const float2 l2 = s[r * Wo + xb + k];
+      const float p = ex2_approx(fmaf(row_lerp<Z>(top, bot, r), k2, -l2.x));
+      const float q = ex2_approx(fmaf(row_lerp<Z>(topt, bott, r), k2, -l2.y));
+      const float g = p - q;
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+// One CTA per (low-res interval row i0, image), one thread per class; out = T2[n][i0][2][w][C] of sum (p_c - q_c).
+template <int Z>
+__global__ void __launch_bounds__(256)
+upsample_kd_bwd_rows_kernel(const float* __restrict__ sl, int pitch_s, const float* __restrict__ tl, int pitch_t, int N,
+                            int h, int w, int C, int Ho, int Wo, float inv_t, const float2* __restrict__ lse,
+                            float* __restrict__ T2) {
+  extern __shared__ float2 s_kpix[];  // [Z][Wo]: (lse_s/T, lse_t/T) * log2(e)
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const float2 l = lse[rowbase + x];
+      s_kpix[r * Wo + x] = make_float2(l.x * kLog2e, l.y * kLog2e);
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const float k2 = inv_t * kLog2e;
+  const float* S0 = sl + (static_cast<size_t>(n) * h + i0) * w * pitch_s + c;
+  const float* S1 = sl + (static_cast<size_t>(n) * h + i1) * w * pitch_s + c;
+  const float* U0 = tl + (static_cast<size_t>(n) * h + i0) * w * pitch_t + c;
+  const float* U1 = tl + (static_cast<size_t>(n) * h + i1) * w * pitch_t + c;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  const int j1 = min(1, w - 1);
+  float a = S0[0], cc = S1[0], at = U0[0], ct = U1[0];   // left node column of the current interval
+  float nb = S0[static_cast<size_t>(j1) * pitch_s], nd = S1[static_cast<size_t>(j1) * pitch_s];
+  float nbt = U0[static_cast<size_t>(j1) * pitch_t], ndt = U1[static_cast<size_t>(j1) * pitch_t];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd, bt = nbt, dt = ndt;
+    const int jn = min(j0 + 2, w - 1);
+    nb = S0[static_cast<size_t>(jn) * pitch_s];
+    nd = S1[static_cast<size_t>(jn) * pitch_s];
+    nbt = U0[static_cast<size_t>(jn) * pitch_t];
+    ndt = U1[static_cast<size_t>(jn) * pitch_t];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      kd_interval<Z, true>(s_kpix, Wo, xb, rows, nx, k2, a, b, cc, d, at, bt, ct, dt, acc);
+    } else {
+      kd_interval<Z, false>(s_kpix, Wo, xb, rows, nx, k2, a, b, cc, d, at, bt, ct, dt, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+    at = bt;
+    ct = dt;
+  }
+}
+
+// dlogits[i] += grad_out[0] * scale * (T2[i][0] + T2[i-1][1]): the cols step of upsample_ce_bwd_cols_kernel, adding to
+// the gradient already in dlogits instead of writing it.
+__global__ void __launch_bounds__(256)
+upsample_kd_bwd_cols_kernel(const float* __restrict__ T2, int N, int h, int w, int C, float scale,
+                            const float* __restrict__ grad_out, float* __restrict__ dlogits) {
+  const int i = blockIdx.x, n = blockIdx.y;
+  const float gs = grad_out[0] * scale;
+  const int wc = w * C;
+  const float* own = T2 + ((static_cast<size_t>(n) * h + i) * 2 + 0) * wc;
+  const float* prev = i > 0 ? T2 + ((static_cast<size_t>(n) * h + (i - 1)) * 2 + 1) * wc : nullptr;
+  float* out = dlogits + (static_cast<size_t>(n) * h + i) * wc;
+  for (int idx = threadIdx.x; idx < wc; idx += blockDim.x) {
+    float acc = own[idx];
+    if (prev) acc += prev[idx];
+    out[idx] = fmaf(acc, gs, out[idx]);
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -1978,6 +2230,132 @@ extern "C" int semseg_upsample_ce_lovasz_bwd(const float* logits, int pitch, int
                                         workspace, dlogits, stream);
     default: return launch_lovasz_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, gamma,
                                          grad_out, workspace, dlogits, stream);
+  }
+}
+
+// Knowledge distillation at zoom factor `zoom` (student and teacher maps upsampled alike). The backward stages one
+// 8-byte word per pixel of the interval's Z output rows, as the plain backward does: Wo <= 2560 at zoom 8.
+static int check_kd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w, int C,
+                    int Ho, int Wo, int zoom, float temperature) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_kd: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(student && teacher, "upsample_kd: null pointer");
+  SB_CHECK_ARG(N > 0 && h > 1 && w > 1 && C > 1 && C <= kMaxClasses, "upsample_kd: bad sizes (C<=%d)", kMaxClasses);
+  SB_CHECK_ARG(pitch_s >= C && pitch_t >= C, "upsample_kd: pitch %d / %d below C = %d", pitch_s, pitch_t, C);
+  SB_CHECK_ARG(Ho == zoom * (h - 1) + 1 && Wo == zoom * (w - 1) + 1,
+               "upsample_kd: needs Ho=%d(h-1)+1, Wo=%d(w-1)+1 (got %dx%d -> %dx%d)", zoom, zoom, h, w, Ho, Wo);
+  SB_CHECK_ARG(std::isfinite(temperature) && temperature > 0.f, "upsample_kd: temperature %g is not finite and > 0",
+               temperature);
+  const size_t max_wo = kBwdSmemMax / (static_cast<size_t>(zoom) * sizeof(float2));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_kd: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int kd_fwd_ctas(int N, int h, int Wo) { return cdiv(Wo, KdGeom<Z>::kCols) * h * N; }
+
+static long long kd_fwd_partials(int N, int h, int Wo, int zoom) {
+  const int cols = zoom <= 2 ? KdGeom<1>::kCols : KdGeom<8>::kCols;
+  return 2LL * N * h * cdiv(Wo, cols);
+}
+
+template <int Z>
+static int launch_kd_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                         int C, int Ho, int Wo, float temperature, float* workspace, float* kl_out, float* lse,
+                         cudaStream_t stream) {
+  using K = KdGeom<Z>;
+  const int Cs = C | 1;
+  // two maps of 256 classes: 133 KB at Z = 1 (65 node columns), 136 KB at Z = 2 and 4 (2 x 33), 70 KB at Z = 8
+  constexpr size_t kMaxSmem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_kd_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_kd_fwd_kernel<Z><<<dim3(cdiv(Wo, K::kCols), h, N), K::kCols, smem, stream>>>(
+      student, pitch_s, teacher, pitch_t, N, h, w, C, Cs, Ho, Wo, 1.f / temperature, workspace,
+      reinterpret_cast<float2*>(lse));
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, kd_fwd_ctas<Z>(N, h, Wo), kl_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_kd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                         int C, int Ho, int Wo, float temperature, float kd_weight, const float* lse,
+                         const float* grad_out, float* workspace, float* dlogits, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(float2);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_kd_bwd_rows_kernel<Z>, attr_set, static_cast<int>(kBwdSmemMax));
+    if (r) return r;
+  }
+  upsample_kd_bwd_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(
+      student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, 1.f / temperature, reinterpret_cast<const float2*>(lse),
+      workspace);
+  SB_LAUNCHED();
+  // d(kd_weight T^2 KL)/ds_c = kd_weight T (p_c - q_c) / P
+  const double P = static_cast<double>(N) * Ho * Wo;
+  const float scale = static_cast<float>(static_cast<double>(kd_weight) * temperature / P);
+  upsample_kd_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, scale, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_kd_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_kd: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0, "upsample_kd: bad sizes");
+  return kd_fwd_partials(N, (Ho - 1) / zoom + 1, Wo, zoom);   // (sum KL, pixels) per forward CTA
+}
+
+extern "C" int semseg_upsample_kd_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N,
+                                      int h, int w, int C, int Ho, int Wo, int zoom, float temperature,
+                                      float* workspace, float* kl_out, float* lse, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_kd(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, zoom, temperature);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && kl_out && lse, "upsample_kd_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_kd_fwd<1>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, workspace,
+                                    kl_out, lse, stream);
+    case 2: return launch_kd_fwd<2>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, workspace,
+                                    kl_out, lse, stream);
+    case 4: return launch_kd_fwd<4>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, workspace,
+                                    kl_out, lse, stream);
+    default: return launch_kd_fwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, workspace,
+                                     kl_out, lse, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_kd_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_kd: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && w > 0 && C > 0, "upsample_kd: bad sizes");
+  return 2LL * N * ((Ho - 1) / zoom + 1) * w * C;  // T2[N][h][2][w][C]
+}
+
+extern "C" int semseg_upsample_kd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N,
+                                      int h, int w, int C, int Ho, int Wo, int zoom, float temperature,
+                                      float kd_weight, const float* lse, const float* grad_out, float* workspace,
+                                      float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_kd(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, zoom, temperature);
+  if (r) return r;
+  SB_CHECK_ARG(std::isfinite(kd_weight) && kd_weight >= 0.f, "upsample_kd_bwd: kd_weight %g is not finite and >= 0",
+               kd_weight);
+  SB_CHECK_ARG(lse && grad_out && workspace && dlogits, "upsample_kd_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_kd_bwd<1>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, kd_weight,
+                                    lse, grad_out, workspace, dlogits, stream);
+    case 2: return launch_kd_bwd<2>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, kd_weight,
+                                    lse, grad_out, workspace, dlogits, stream);
+    case 4: return launch_kd_bwd<4>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, kd_weight,
+                                    lse, grad_out, workspace, dlogits, stream);
+    default: return launch_kd_bwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, kd_weight,
+                                     lse, grad_out, workspace, dlogits, stream);
   }
 }
 

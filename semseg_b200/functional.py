@@ -623,6 +623,30 @@ class _UpsampleCELovasz(torch.autograd.Function):
         return dl, None, None, None, None, None, None
 
 
+class _UpsampleCEKD(torch.autograd.Function):
+    """The fused tail with losses.DistillationLoss: ce_weight * CE (the plain forward, at zoom `zoom`) plus
+    kd_weight * T^2 * KL(teacher || student) (the distillation forward, at zoom `kd_zoom`: the model's zoom, or 1 on the
+    1/8-resolution maps). The backward writes the CE gradient and the distillation kernels add theirs into the same
+    buffer. The teacher map is a constant: it gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, teacher_logits, target, ignore_index, zoom, kd_zoom, temperature, kd_weight, ce_weight):
+        info, amax, lse = ops.upsample_ce_fwd(logits, target, ignore_index, zoom=zoom)
+        kl, lse_kd = ops.upsample_kd_fwd(logits, teacher_logits, temperature, zoom=kd_zoom)
+        ctx.save_for_backward(logits, teacher_logits, target, lse, info, lse_kd)
+        ctx.cfg = (ignore_index, zoom, kd_zoom, temperature, kd_weight, ce_weight)
+        ctx.mark_non_differentiable(amax)
+        return torch.add(info[0] * ce_weight, kl[0], alpha=kd_weight * temperature * temperature), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, teacher_logits, target, lse, info, lse_kd = ctx.saved_tensors
+        ignore_index, zoom, kd_zoom, temperature, kd_weight, ce_weight = ctx.cfg
+        dl = ops.upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_loss * ce_weight, zoom=zoom)
+        ops.upsample_kd_bwd(logits, teacher_logits, temperature, kd_weight, lse_kd, grad_loss, dl, zoom=kd_zoom)
+        return dl, None, None, None, None, None, None, None, None
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""
@@ -644,9 +668,11 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     weighted / smoothed forms need the target on a CUDA device and class weights as a contiguous fp32 [classes] tensor
     on that device; any other weight, another reduction, and any subclass keep the ATen tail. DiceLoss and
     losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage (2389 columns at zoom 8), and the
-    Lovász loss fewer than 2^31 target pixels.
+    Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain form's conditions.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
-    if type(criterion) is nn.CrossEntropyLoss:
+    if type(criterion) is losses.DistillationLoss:
+        ok = True
+    elif type(criterion) is nn.CrossEntropyLoss:
         eps = getattr(criterion, 'label_smoothing', 0.0)
         plain = criterion.weight is None and eps == 0.0
         ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
@@ -676,12 +702,18 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     return target.shape[1] == zoom_factor * (h - 1) + 1 and target.shape[2] == zoom_factor * (w - 1) + 1
 
 
-def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None):
+def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_logits=None):
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
     weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
     with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index); with a losses.LovaszSoftmaxLoss, its
-    Lovász-Softmax (+ CE) loss. The default criterion runs the plain kernels."""
+    Lovász-Softmax (+ CE) loss; with a losses.DistillationLoss and the teacher's fp32 NHWC logits `teacher_logits`
+    (the student's shape), its distillation loss (without them: the plain mean CE, the loss of the aux head). The
+    default criterion runs the plain kernels."""
+    if isinstance(criterion, losses.DistillationLoss) and teacher_logits is not None:
+        kd_zoom = 1 if criterion.at == 'logits' else int(zoom)
+        return _UpsampleCEKD.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
+                                   int(zoom), kd_zoom, criterion.temperature, criterion.kd_weight, criterion.ce_weight)
     if isinstance(criterion, losses.LovaszSoftmaxLoss):
         return _UpsampleCELovasz.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
                                        criterion.classes == 'all', bool(criterion.per_image), criterion.ce_weight)

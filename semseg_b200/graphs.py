@@ -18,8 +18,9 @@ step counter incremented inside the graph — csrc/bn.cu st_ll / ld_ll) and drop
 Limits (same as torch.cuda.make_graphed_callables): a second training forward before the backward of the first one
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
-cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss and the Lovász-Softmax
-loss) are not captured (such models simply stay eager).
+cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
+loss and the distillation loss, whose teacher forward is captured with the step) are not captured (such models simply
+stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -250,9 +251,19 @@ def _capture(model, impl, st, x, y):
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
     del proxies, x_in, x_leaf
-    # the graphs reference the persistent weight slabs: keep their owner alive as long as the graphs
+    # the graphs reference the persistent weight slabs: keep their owner alive as long as the graphs (a distillation
+    # teacher's slabs are its convs' own packs, filled by the eager warm-up calls; the teacher is kept with them)
     st.keep = model.__dict__.get("_sb_pack_plan")
+    teacher = _teacher(getattr(model, "criterion", None))
+    if teacher is not None:
+        st.keep = (st.keep, teacher, [m.__dict__.get("_sb_conv_plan") for m in teacher.modules()])
     torch.cuda.synchronize()
+
+
+def _teacher(crit):
+    """The teacher network a losses.DistillationLoss criterion runs inside the step, else None."""
+    from . import losses
+    return crit.teacher if isinstance(crit, losses.DistillationLoss) else None
 
 
 def train_step(model, impl, x, y):
@@ -280,6 +291,15 @@ def train_step(model, impl, x, y):
                                                                       "ce_weight", "classes", "per_image"))
     cw = getattr(crit, "weight", None)
     crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
+    teacher = _teacher(crit)
+    if teacher is not None:
+        # a distillation teacher runs inside the forward graph: its identity, the addresses and versions of its
+        # parameters and buffers (an in-place edit of a weight bumps the version, so the step is captured again with
+        # the edit rather than replayed stale), its BatchNorm modes and the options of the KL term are baked in too
+        crit_key += (id(teacher), tuple((t.data_ptr(), t._version) for t in teacher.parameters()),
+                     tuple((t.data_ptr(), t._version) for t in teacher.buffers()),
+                     tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)),
+                     crit.temperature, crit.kd_weight, crit.at)
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
            dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad,
            crit_key)

@@ -4,7 +4,8 @@ OhemCrossEntropyLoss is online hard-pixel mining: only the pixels the network is
 the network's fused tail (functional.upsample_ce) it runs inside the same kernels as the default loss, graphed at every
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
-and LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, run the same way.
+and LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, run the same way. DistillationLoss adds a
+pixel-wise distillation term from a frozen teacher network that the student's training forward runs.
 """
 import math
 
@@ -135,6 +136,120 @@ class DiceLoss(nn.Module):
             raise TypeError("DiceLoss: fp32 logits and int64 target expected, got %s and %s" %
                             (logits.dtype, target.dtype))
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+def _check_native_logits(name, logits, target):
+    if logits.dim() != 4 or target.dim() != 3 or target.shape != logits.shape[:1] + logits.shape[2:]:
+        raise ValueError("%s: logits [N, C, H, W] and target [N, H, W] expected, got %s and %s" %
+                         (name, tuple(logits.shape), tuple(target.shape)))
+    if logits.shape[1] > 256:
+        raise ValueError("%s: at most 256 classes (got %d); no fallback" % (name, logits.shape[1]))
+    if not (logits.is_cuda and target.is_cuda):
+        raise RuntimeError("%s runs on the native CUDA kernels only (no CPU fallback); got %s, %s"
+                           % (name, logits.device, target.device))
+    if logits.dtype != torch.float32 or target.dtype != torch.int64:
+        raise TypeError("%s: fp32 logits and int64 target expected, got %s and %s" % (name, logits.dtype, target.dtype))
+
+
+class DistillationLoss(nn.Module):
+    """Pixel-wise knowledge distillation from a frozen teacher network, plus cross-entropy. With s, t the student and
+    teacher logits at the KD resolution, T the temperature, p = softmax(s/T) and q = softmax(t/T) over the classes and P
+    the number of pixels at the KD resolution over all images of the call:
+
+        KL   = (1/P) sum_pixels sum_c q_c (log q_c - log p_c)        (every pixel; the target plays no part)
+        main = ce_weight * CE(student xZ, target; ignore_index, mean over valid pixels) + kd_weight * T^2 * KL
+        aux  = plain CE of the aux head (ignore_index); the teacher has no aux counterpart, ce_weight does not scale it
+        d main / d s_c at the KD resolution, KD part = kd_weight * T * (p_c - q_c) / P
+
+    at='output': s and t after the same bilinear xZ upsample (align_corners) that the CE term uses, i.e. at the target's
+    size; at='logits': the raw 1/8-resolution maps (as structured KD / CIRKD distil them). "Valid" is as in the other
+    criteria: target != ignore_index and 0 <= target < C. Under DistributedDataParallel each rank holds its own teacher
+    and averages over its own pixels.
+
+    `teacher` is a PSPNet or PSANet of this package, in eval mode, on the input's device, with the student's number of
+    classes; the user moves it there. It is held, not owned: it is not a submodule, so it stays out of the student's
+    state_dict, modules(), .cuda() / .to(), convert_sync_batchnorm and DDP's buffer broadcast. It runs inside the
+    student's training forward, before the student's stem, under torch.no_grad() in the student's precision mode, on the
+    folded eval kernels; its parameters, running statistics and training flag are never modified, and no gradient
+    reaches it or, through it, the input (with x.requires_grad, x.grad is the student's).
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, teacher forward and KL
+    term graphed at every zoom factor. Called as a module, forward(logits, target, teacher_logits=None) takes NCHW logits
+    at the target size: without teacher_logits it returns the student's mean cross-entropy (the validation loss
+    validate() logs), with them (the same shape) `main` computed at that size. It runs the zoom-1 kernels on NHWC copies.
+    CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
+
+    def __init__(self, teacher, temperature=1.0, kd_weight=1.0, ce_weight=1.0, ignore_index=255, at='output'):
+        super(DistillationLoss, self).__init__()
+        from .pspnet import PSPNet
+        from .psanet import PSANet
+        if not isinstance(teacher, (PSPNet, PSANet)):
+            raise TypeError("teacher must be a semseg_b200 PSPNet or PSANet, got %s" % type(teacher).__name__)
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        if not isinstance(at, str):
+            raise TypeError("at must be 'output' or 'logits', got %r" % (at,))
+        if at not in ('output', 'logits'):
+            raise ValueError("at must be 'output' or 'logits', got %r" % (at,))
+        temperature = _non_negative("temperature", temperature)
+        if temperature <= 0.0:
+            raise ValueError("temperature must be > 0, got %r" % temperature)
+        self.temperature = temperature
+        self.kd_weight = _non_negative("kd_weight", kd_weight)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+        self.ignore_index = ignore_index
+        self.at = at
+        self.__dict__['_teacher'] = teacher      # held outside the module tree (see the class docstring)
+
+    @property
+    def teacher(self):
+        return self.__dict__['_teacher']
+
+    def __setattr__(self, name, value):
+        # nn.Module.__setattr__ would register a module value as a child, past the read-only property
+        if name in ('teacher', '_teacher'):
+            raise AttributeError("DistillationLoss: the teacher is fixed at construction; build a new criterion")
+        super(DistillationLoss, self).__setattr__(name, value)
+
+    def extra_repr(self):
+        return "teacher=%s, temperature=%g, kd_weight=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
+            type(self.teacher).__name__, self.temperature, self.kd_weight, self.ce_weight, self.ignore_index, self.at)
+
+    def run_teacher(self, x, classes):
+        """The teacher's detached fp32 NHWC 1/8-resolution logits of the input batch `x` (NCHW), for a student with
+        `classes` classes."""
+        from . import functional as SF
+        teacher = self.teacher
+        # the network and every layer whose mode changes the forward (the teacher's own criterion, a module that the
+        # networks' default argument shares with every other network, does not take part)
+        if teacher.training or any(m.training for m in teacher.modules()
+                                   if isinstance(m, (nn.modules.batchnorm._BatchNorm, nn.modules.dropout._DropoutNd))):
+            raise RuntimeError("DistillationLoss: the teacher must be in eval mode (call teacher.eval())")
+        dev = next(teacher.parameters()).device
+        if dev != x.device:
+            raise RuntimeError("DistillationLoss: the teacher is on %s, the input on %s (move the teacher yourself)" %
+                               (dev, x.device))
+        tc = teacher.cls[4].out_channels
+        if tc != classes:
+            raise ValueError("DistillationLoss: the teacher has %d classes, the student %d" % (tc, classes))
+        with torch.no_grad(), SF.network_mode(False, False):
+            return teacher._eval_logits_nhwc(x.detach())
+
+    def forward(self, logits, target, teacher_logits=None):
+        from . import functional as SF
+        _check_native_logits("DistillationLoss", logits, target)
+        s = logits.permute(0, 2, 3, 1).contiguous()
+        if teacher_logits is None:
+            loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1)
+            return loss
+        if teacher_logits.shape != logits.shape or teacher_logits.dtype != torch.float32 or \
+                teacher_logits.device != logits.device:
+            raise ValueError("DistillationLoss: teacher_logits must be fp32 %s on %s like the logits, got %s %s on %s" %
+                             (tuple(logits.shape), logits.device, teacher_logits.dtype, tuple(teacher_logits.shape),
+                              teacher_logits.device))
+        t = teacher_logits.detach().permute(0, 2, 3, 1).contiguous()
+        loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self, teacher_logits=t)
         return loss
 
 

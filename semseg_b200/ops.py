@@ -886,6 +886,56 @@ def upsample_ce_lovasz_bwd(logits, target, ignore_index, lse, gamma, grad_out, z
     return dl
 
 
+def _kd_map_meta(x):
+    """(N, h, w, C, pitch) of an fp32 NHWC logit map whose pixels may be padded (a channel slice of a wider buffer)."""
+    assert x.dtype == torch.float32 and x.dim() == 4 and x.stride(-1) == 1
+    n, h, w, c = x.shape
+    pitch = x.stride(2)
+    assert x.stride(1) == w * pitch and x.stride(0) == h * x.stride(1), "logits must be pixel-contiguous"
+    return n, h, w, c, pitch
+
+
+def upsample_kd_fwd(student, teacher, temperature, zoom=8):
+    """Pixel-wise distillation term on the fused tail (include/semseg_b200.h states the contract): student / teacher
+    fp32 NHWC [N,h,w,C] maps (each with its own pixel pitch), both upsampled xzoom -> (kl_info [2] = (KL, P),
+    lse [N,Ho,Wo,2] = (lse(s/T), lse(t/T)) per pixel)."""
+    _require_cuda(student, teacher)
+    lib = _lib.load()
+    n, h, w, c, ps = _kd_map_meta(student)
+    shape_t = _kd_map_meta(teacher)
+    assert shape_t[:4] == (n, h, w, c), "student and teacher maps differ in shape"
+    ho, wo = int(zoom) * (h - 1) + 1, int(zoom) * (w - 1) + 1
+    nws = int(lib.semseg_upsample_kd_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_kd_workspace_floats")
+    dev = student.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    lse = torch.empty((n, ho, wo, 2), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_upsample_kd_fwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c, ho, wo, int(zoom),
+                                          float(temperature), _ptr(ws), _ptr(info), _ptr(lse), _stream()),
+               "semseg_upsample_kd_fwd")
+    return info, lse
+
+
+def upsample_kd_bwd(student, teacher, temperature, kd_weight, lse, grad_out, dlogits, zoom=8):
+    """dlogits (fp32 [N,h,w,C], dense, already holding a gradient) += grad_out * d(kd_weight T^2 KL)/d student, in
+    place; returns dlogits."""
+    lib = _lib.load()
+    n, h, w, c, ps = _kd_map_meta(student)
+    pt = _kd_map_meta(teacher)[4]
+    assert dlogits.shape == (n, h, w, c) and dlogits.dtype == torch.float32 and dlogits.is_contiguous()
+    ho, wo = int(zoom) * (h - 1) + 1, int(zoom) * (w - 1) + 1
+    nws = int(lib.semseg_upsample_kd_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_kd_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=student.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_kd_bwd(_ptr(student), ps, _ptr(teacher), pt, n, h, w, c, ho, wo, int(zoom),
+                                          float(temperature), float(kd_weight), _ptr(lse), _ptr(g), _ptr(ws),
+                                          _ptr(dlogits), _stream()),
+               "semseg_upsample_kd_bwd")
+    return dlogits
+
+
 def segsort_u32_pairs(keys, vals, skip=None):
     """Stable sort of each row of the int32 [S, L] CUDA tensors `keys` / `vals` (uint32 bit patterns) by key, in place;
     rows whose int32 `skip` [S] entry is non-zero are left untouched."""

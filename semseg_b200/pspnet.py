@@ -8,6 +8,7 @@ import torch.nn.functional as F
 
 from . import functional as SF
 from . import graphs
+from . import losses
 from . import ops
 from . import p2p
 from . import resnet as models
@@ -136,6 +137,10 @@ class _SegNet(nn.Module):
         if self.training and torch.is_grad_enabled():
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
+        t_logits = None
+        if self.training and y is not None and isinstance(self.criterion, losses.DistillationLoss):
+            # the frozen teacher first: its activations are transient before the student's saved ones exist
+            t_logits = self.criterion.run_teacher(x, self.cls[4].out_channels)
         logits, t_aux = self._logits_nhwc(x)
 
         if self.training:
@@ -143,13 +148,16 @@ class _SegNet(nn.Module):
             if SF.fused_tail_supported(self.criterion, logits, y, self.zoom_factor):
                 # upsample + cross-entropy + argmax fused: [N, classes, H, W] never exists (model/pspnet.py:94-103)
                 main_loss, pred = SF.upsample_ce(logits, y, self.criterion.ignore_index, self.zoom_factor,
-                                                 criterion=self.criterion)
+                                                 criterion=self.criterion, teacher_logits=t_logits)
                 aux_loss, _ = SF.upsample_ce(aux_logits, y, self.criterion.ignore_index, self.zoom_factor,
                                              criterion=self.criterion)
                 return pred, main_loss, aux_loss
             x = upsample_logits(logits, (h, w), self.zoom_factor)
             aux = upsample_logits(aux_logits, (h, w), self.zoom_factor)
-            main_loss = self.criterion(x, y)
+            if t_logits is not None:
+                main_loss = self.criterion(x, y, teacher_logits=upsample_logits(t_logits, (h, w), self.zoom_factor))
+            else:
+                main_loss = self.criterion(x, y)
             aux_loss = self.criterion(aux, y)
             return x.max(1)[1], main_loss, aux_loss
         else:
