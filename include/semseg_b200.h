@@ -22,6 +22,7 @@
  *                               semseg_upsample_ce_ohem_*: the same with an OHEM cross-entropy criterion.
  *                               semseg_upsample_ce_{,ohem_}weighted_*: class weights / label smoothing.
  *                               semseg_upsample_ce_dice_*: soft Dice loss, alone or plus cross-entropy.
+ *                               semseg_upsample_ce_focal_*: softmax focal loss, with or without class weights.
  *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
  *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
@@ -486,6 +487,31 @@ long long semseg_upsample_ce_dice_bwd_workspace_floats(int N, int Ho, int Wo, in
 int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                                 int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* table,
                                 const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Softmax focal loss (Lin et al., ICCV 2017; semseg_b200/losses.py FocalLoss) on the same fused upsample at zoom
+ * `zoom`. class_weight fp32 [C] on the device (NULL = all ones; read at every launch, so a CUDA graph sees in-place
+ * edits), gamma finite and >= 0. Per valid pixel (target != ignore_index, 0 <= target < C), with p = softmax(v),
+ * q = 1 - p_t and nll = -log p_t:
+ *   l = w_t q^gamma nll,   loss = sum over valid pixels of l / n_valid   (the pixel count, not sum w_t),
+ *   dl/dv_c = w_t M (p_c - [c = t]),   M = q^gamma + gamma p_t q^(gamma-1) nll,
+ * with torch.pow's 0^0 = 1 (at q = 0: l = 0, M = 1 when gamma = 0 and 0 otherwise); loss 0 and an exactly zero gradient
+ * when no pixel is valid. q = (sum_{c != t} e_c) / (sum_c e_c), so it keeps its relative accuracy as p_t -> 1. The
+ * backward's staged rows take 12 bytes per pixel: the Dice width limit, Wo <= 229376 / (12 zoom), 2389 at zoom 8.
+ *   fwd: loss_out[0] = loss, loss_out[1] = n_valid; argmax (or NULL) and lse as the zoom forward's (the same bits);
+ *        mod fp32 [N,Ho,Wo] = w_t M per pixel, 0 where the pixel is not valid (kept for the backward); workspace:
+ *        semseg_upsample_ce_focal_workspace_floats() floats (the zoom forward's).
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits from the forward's lse, mod and loss_out; workspace:
+ *        semseg_upsample_ce_focal_bwd_workspace_floats() floats (the zoom backward's).
+ * Both reject a bad shape, zoom, gamma, width, alignment or null output before any CUDA call. */
+long long semseg_upsample_ce_focal_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_ce_focal_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                 int Ho, int Wo, int zoom, int ignore_index, const float* class_weight, float gamma,
+                                 float* workspace, float* loss_out, int64_t* argmax, float* lse, float* mod,
+                                 void* stream);
+long long semseg_upsample_ce_focal_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_focal_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                 int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* mod,
+                                 const float* loss_info, const float* grad_out, float* workspace, float* dlogits,
+                                 void* stream);
 /* Lovász-Softmax loss (Berman et al., CVPR 2018), alone or plus cross-entropy (semseg_b200/losses.py
  * LovaszSoftmaxLoss), on the same fused upsample at zoom `zoom`. p = softmax(v) as the Dice passes compute it. A segment
  * is one class over every valid pixel of the call (per_image = 0, S = C segments of L = N*Ho*Wo pixels) or one (image,

@@ -199,6 +199,12 @@ SIGNATURES = {
     "semseg_upsample_ce_dice_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_dice_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_focal_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_focal_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                             c_vp, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_focal_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_focal_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_upsample_ce_lovasz_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_lovasz_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                               c_int, c_int, c_int, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

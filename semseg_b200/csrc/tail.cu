@@ -38,6 +38,9 @@
 // The Lovász-Softmax loss, alone or plus cross-entropy, runs the plain forward instance, a key pass, the segmented stable
 // radix sort of csrc/segsort.cu and its own scan and gradient kernels (see "Lovász-Softmax" below); no existing
 // instance changes.
+//
+// The softmax focal loss, with or without class weights, runs sibling forward and rows kernels (see "focal loss" below)
+// with the plain reduce and cols kernels; no existing instance changes.
 #include <cmath>
 
 #include "host_common.h"
@@ -1546,6 +1549,242 @@ upsample_kd_bwd_cols_kernel(const float* __restrict__ T2, int N, int h, int w, i
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- focal loss
+// Softmax focal loss (Lin et al., ICCV 2017) with optional class weights. Per valid pixel, with p = softmax(v),
+// q = 1 - p_t and nll = -log p_t:
+//   l = w_t q^gamma nll,   loss = sum l / n_valid,
+//   dl/dv_c = w_t M (p_c - [c = t]),   M = q^gamma + gamma p_t q^(gamma-1) nll = q^gamma (1 + gamma p_t nll / q)
+// with torch.pow's 0^0 = 1: at q = 0, l = 0 and M = [gamma = 0]. The forward is the plain forward plus, per pixel, the
+// modulator w_t M (0 where the pixel is not valid) kept for the backward; the backward is the plain one with every
+// pixel's term scaled by its modulator, then the plain cols kernel with 1 / n_valid.
+// Operation order (q and nll keep their relative accuracy as p_t -> 1): the second class pass sums, next to the plain
+// S = sum_c e_c (e_c = ex2((v_c - m) log2e); lse = m + log S is the plain forward's bits), S_o = sum_{c != t} e_c with
+// the target's term skipped, not subtracted. Then q = S_o / S, p_t = e_t / S, nll = log1p(S_o / e_t) (lse - v_t once e_t
+// has underflowed) and q^gamma = ex2(gamma lg2 q): one MUFU pair per pixel.
+__device__ __forceinline__ float lg2_approx(float x) {
+  float y;
+  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+constexpr float kFocalMinEt = 1e-30f;   // below this S_o / e_t may overflow: nll = lse - v_t, large and well conditioned
+
+template <int Z>
+__global__ void __launch_bounds__(kFwdCols)
+upsample_ce_focal_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
+                             const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                             const float* __restrict__ class_weight, float gamma, float* __restrict__ partial,
+                             long long* __restrict__ argmax_out, float* __restrict__ lse_out,
+                             float* __restrict__ mod_out) {
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs] as in upsample_ce_fwd_kernel
+  __shared__ float red_loss[kFwdCols / 32];
+  __shared__ float red_cnt[kFwdCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kFwdNodes, w - j_base);
+  const int tid = threadIdx.x;
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * kFwdNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
+  }
+  __syncthreads();
+  float loss = 0.f, cnt = 0.f;
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* A = S + (j0 - j_base) * Cs;
+    const float* B = S + (j1 - j_base) * Cs;
+    const float* Cc = A + kFwdNodes * Cs;
+    const float* D = B + kFwdNodes * Cs;
+    float m[Z], sum[Z], so[Z];   // so: S_o, the sum without the target's term
+    int am[Z], tc[Z];            // tc: target class, -1 = not valid
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      m[r] = -INFINITY;
+      am[r] = 0;
+      sum[r] = 0.f;
+      so[r] = 0.f;
+      tc[r] = -1;
+      if (r < rows) {
+        const long long t = target[(static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x];
+        if (t != ignore_index && t >= 0 && t < C) tc[r] = static_cast<int>(t);
+      }
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        if (v > m[r]) {
+          m[r] = v;
+          am[r] = c;
+        }
+      }
+    }
+    float m2[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) m2[r] = m[r] * kLog2e;
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        const float e = ex2_approx(fmaf(v, kLog2e, -m2[r]));
+        sum[r] += e;
+        so[r] += c == tc[r] ? 0.f : e;
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+        const float lse = m[r] + __logf(sum[r]);
+        if (argmax_out) argmax_out[pix] = am[r];
+        lse_out[pix] = lse;
+        float mod = 0.f;
+        if (tc[r] >= 0) {
+          const int t = tc[r];
+          const float top = Z == 1 ? A[t] : l0w * A[t] + l1w * B[t];
+          const float bot = Z == 1 ? 0.f : l0w * Cc[t] + l1w * D[t];
+          const float vt = row_lerp<Z>(top, bot, r);
+          const float et = ex2_approx(fmaf(vt, kLog2e, -m2[r]));
+          const float q = so[r] / sum[r];
+          const float nll = et > kFocalMinEt ? log1pf(so[r] / et) : lse - vt;
+          const float wt = class_weight ? class_weight[t] : 1.f;
+          float qg, M;   // q^gamma and the modulator, torch.pow's 0^0 = 1
+          if (q > 0.f) {
+            qg = ex2_approx(gamma * lg2_approx(q));
+            M = qg * fmaf(gamma * (et / sum[r]), nll / q, 1.f);
+          } else {
+            qg = M = gamma == 0.f ? 1.f : 0.f;
+          }
+          loss += wt * qg * nll;
+          cnt += 1.f;
+          mod = wt * M;
+        }
+        mod_out[pix] = mod;
+      }
+    }
+  }
+  // deterministic block reduction -> one (sum of l, valid count) partial per CTA, as upsample_ce_fwd_kernel
+  for (int o = 16; o > 0; o >>= 1) {
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((tid & 31) == 0) {
+    red_loss[tid >> 5] = loss;
+    red_cnt[tid >> 5] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float l = 0.f, k = 0.f;
+    for (int i = 0; i < kFwdCols / 32; ++i) {
+      l += red_loss[i];
+      k += red_cnt[i];
+    }
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[2 * b] = l;
+    partial[2 * b + 1] = k;
+  }
+}
+
+// One interval of the focal rows kernel for class c: g = modulator (p_c - [c = t]), folded as in
+// upsample_ce_bwd_rows_kernel. DicePix::g holds the pixel's modulator.
+template <int Z, bool kFull>
+__device__ __forceinline__ void focal_interval(const DicePix* s, int Wo, int xb, int rows, int nx, int c, float a,
+                                               float b, float cc, float d, float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const DicePix pi = s[r * Wo + xb + k];
+      if (pi.t < 0) continue;  // warp-uniform
+      const float v = row_lerp<Z>(top, bot, r);
+      const float p = ex2_approx(fmaf(v, kLog2e, -pi.lse2));
+      const float g = pi.g * (p - (c == pi.t ? 1.f : 0.f));
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+// Rows layout of upsample_ce_bwd_rows_kernel with the Dice rows kernel's 12-byte pixel word (lse, target, modulator);
+// a pixel whose modulator is 0 (not valid, a zero-weight class, q = 0) is staged as ignored: its gradient is exactly 0.
+template <int Z>
+__global__ void __launch_bounds__(256)
+upsample_ce_focal_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
+                              const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                              const float* __restrict__ lse, const float* __restrict__ mod, float* __restrict__ T2) {
+  extern __shared__ DicePix s_dpix[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const long long t = target[rowbase + x];
+      DicePix pi;
+      pi.g = mod[rowbase + x];
+      pi.t = (t == ignore_index || t < 0 || t >= C || pi.g == 0.f) ? -1 : static_cast<int>(t);
+      pi.lse2 = lse[rowbase + x] * kLog2e;
+      s_dpix[r * Wo + x] = pi;
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
+  const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  float a = L0[0], cc = L1[0];
+  float nb = L0[static_cast<size_t>(min(1, w - 1)) * pitch], nd = L1[static_cast<size_t>(min(1, w - 1)) * pitch];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd;
+    const int jn = min(j0 + 2, w - 1);
+    nb = L0[static_cast<size_t>(jn) * pitch];
+    nd = L1[static_cast<size_t>(jn) * pitch];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      focal_interval<Z, true>(s_dpix, Wo, xb, rows, nx, c, a, b, cc, d, acc);
+    } else {
+      focal_interval<Z, false>(s_dpix, Wo, xb, rows, nx, c, a, b, cc, d, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -2046,6 +2285,113 @@ extern "C" int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N
                                       workspace, dlogits, stream);
     default: return launch_dice_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
                                        workspace, dlogits, stream);
+  }
+}
+
+// Focal loss at zoom factor `zoom`: its own forward and rows kernels, the plain reduce and cols kernels. The rows kernel
+// stages the Dice rows kernel's 12-byte words: the Dice width limit. class_weight NULL = all ones.
+static int check_focal(int zoom, int Wo, float gamma, const void* class_weight, const void* mod) {
+  SB_CHECK_ARG(std::isfinite(gamma) && gamma >= 0.f, "upsample_ce_focal: gamma %g is not finite and >= 0", gamma);
+  SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(class_weight) | reinterpret_cast<uintptr_t>(mod)) & 3) == 0,
+               "upsample_ce_focal: class_weight or modulator map not 4-byte aligned");
+  const size_t max_wo = kDiceSmemMax / (static_cast<size_t>(zoom) * sizeof(DicePix));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_ce_focal: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_focal_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                            int Wo, int ignore_index, const float* class_weight, float gamma, float* workspace,
+                            float* loss_out, int64_t* argmax, float* lse, float* mod, cudaStream_t stream) {
+  const int Cs = C | 1;
+  constexpr size_t kMaxSmem =
+      static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_focal_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_ce_focal_fwd_kernel<Z><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, class_weight,
+      gamma, workspace, reinterpret_cast<long long*>(argmax), lse, mod);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_focal_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                            int Wo, int ignore_index, const float* lse, const float* mod, const float* loss_info,
+                            const float* grad_out, float* workspace, float* dlogits, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(DicePix);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_focal_rows_kernel<Z>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  upsample_ce_focal_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, mod, workspace);
+  SB_LAUNCHED();
+  // loss_info[1] = n_valid: the plain cols kernel's 1 / count
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_focal_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  return semseg_upsample_ce_zoom_workspace_floats(N, Ho, Wo, zoom);
+}
+
+extern "C" int semseg_upsample_ce_focal_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                            const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                            const float* class_weight, float gamma, float* workspace,
+                                            float* loss_out, int64_t* argmax, float* lse, float* mod, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_focal(zoom, Wo, gamma, class_weight, mod);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && mod, "upsample_ce_focal_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_focal_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, class_weight, gamma,
+                                       workspace, loss_out, argmax, lse, mod, stream);
+    case 2: return launch_focal_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, class_weight, gamma,
+                                       workspace, loss_out, argmax, lse, mod, stream);
+    case 4: return launch_focal_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, class_weight, gamma,
+                                       workspace, loss_out, argmax, lse, mod, stream);
+    default: return launch_focal_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, class_weight, gamma,
+                                        workspace, loss_out, argmax, lse, mod, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_focal_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_ce_focal_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                            const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                            const float* lse, const float* mod, const float* loss_info,
+                                            const float* grad_out, float* workspace, float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_focal(zoom, Wo, 0.f, nullptr, mod);
+  if (r) return r;
+  SB_CHECK_ARG(lse && mod && loss_info && grad_out && workspace && dlogits, "upsample_ce_focal_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_focal_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, mod, loss_info,
+                                       grad_out, workspace, dlogits, stream);
+    case 2: return launch_focal_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, mod, loss_info,
+                                       grad_out, workspace, dlogits, stream);
+    case 4: return launch_focal_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, mod, loss_info,
+                                       grad_out, workspace, dlogits, stream);
+    default: return launch_focal_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, mod, loss_info,
+                                        grad_out, workspace, dlogits, stream);
   }
 }
 

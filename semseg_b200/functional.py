@@ -602,6 +602,26 @@ class _UpsampleCEDice(torch.autograd.Function):
         return dl, None, None, None, None, None, None
 
 
+class _UpsampleCEFocal(torch.autograd.Function):
+    """The fused tail with losses.FocalLoss: the mean over the valid pixels of w_t (1 - p_t)^gamma nll. The forward
+    keeps each pixel's gradient modulator; the backward is the plain one scaled per pixel. The class weights are read
+    on the device at every launch (a CUDA-graph replay sees in-place edits) and get no gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, gamma, weight=None):
+        info, amax, lse, mod = ops.upsample_ce_focal_fwd(logits, target, ignore_index, weight, gamma, zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, mod, info)
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, mod, info = ctx.saved_tensors
+        dl = ops.upsample_ce_focal_bwd(logits, target, ctx.ignore_index, lse, mod, info, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None
+
+
 class _UpsampleCELovasz(torch.autograd.Function):
     """The fused tail with losses.LovaszSoftmaxLoss, plus ce_weight * CE. The forward keeps the per pixel-class
     Lovász gradient weights (gamma, 4 C bytes per output pixel) it scattered from the sorted segments; the sort's
@@ -663,12 +683,13 @@ _DICE_PIXEL_BYTES, _DICE_STAGE_BYTES = 12, 224 * 1024
 
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     """The fused kernel implements exactly nn.CrossEntropyLoss(weight, ignore_index=k, reduction='mean',
-    label_smoothing), losses.OhemCrossEntropyLoss (with or without class weights) and losses.DiceLoss, at every zoom
-    factor of the model (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of the 1/8-resolution logits. The
-    weighted / smoothed forms need the target on a CUDA device and class weights as a contiguous fp32 [classes] tensor
-    on that device; any other weight, another reduction, and any subclass keep the ATen tail. DiceLoss and
-    losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage (2389 columns at zoom 8), and the
-    Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain form's conditions.
+    label_smoothing), losses.OhemCrossEntropyLoss and losses.FocalLoss (each with or without class weights) and
+    losses.DiceLoss, at every zoom factor of the model (1, 2, 4, 8) with the target at the zoomed size zoom*(h'-1)+1 of
+    the 1/8-resolution logits. The weighted / smoothed forms need the target on a CUDA device and class weights as a
+    contiguous fp32 [classes] tensor on that device; any other weight, another reduction, and any subclass keep the
+    ATen tail. DiceLoss, FocalLoss and losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage
+    (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
+    form's conditions.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
         ok = True
@@ -677,7 +698,7 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         plain = criterion.weight is None and eps == 0.0
         ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
               (plain or (target is not None and target.is_cuda)))
-    elif type(criterion) is losses.DiceLoss:
+    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss):     # the focal rows kernel stages the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     elif type(criterion) is losses.LovaszSoftmaxLoss:
@@ -707,7 +728,8 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
     weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
     with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index); with a losses.LovaszSoftmaxLoss, its
-    Lovász-Softmax (+ CE) loss; with a losses.DistillationLoss and the teacher's fp32 NHWC logits `teacher_logits`
+    Lovász-Softmax (+ CE) loss; with a losses.FocalLoss, its focal loss (its own ignore_index, gamma and class
+    weights); with a losses.DistillationLoss and the teacher's fp32 NHWC logits `teacher_logits`
     (the student's shape), its distillation loss (without them: the plain mean CE, the loss of the aux head). The
     default criterion runs the plain kernels."""
     if isinstance(criterion, losses.DistillationLoss) and teacher_logits is not None:
@@ -717,6 +739,12 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     if isinstance(criterion, losses.LovaszSoftmaxLoss):
         return _UpsampleCELovasz.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
                                        criterion.classes == 'all', bool(criterion.per_image), criterion.ce_weight)
+    if isinstance(criterion, losses.FocalLoss):
+        if criterion.weight is None:
+            return _UpsampleCEFocal.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                          criterion.gamma)
+        return _UpsampleCEFocal.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.gamma,
+                                      criterion.weight)
     if isinstance(criterion, losses.DiceLoss):
         return _UpsampleCEDice.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.smooth,
                                      criterion.eps, criterion.ce_weight)

@@ -19,8 +19,8 @@ Limits (same as torch.cuda.make_graphed_callables): a second training forward be
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
-loss and the distillation loss, whose teacher forward is captured with the step) are not captured (such models simply
-stay eager).
+loss, the focal loss and the distillation loss, whose teacher forward is captured with the step) are not captured (such
+models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -282,13 +282,13 @@ def train_step(model, impl, x, y):
     bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
     # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
     # the criterion's options are launch arguments baked into the graph: a changed thresh, ignore_index,
-    # label_smoothing, Dice smooth / eps / ce_weight or Lovász classes / per_image captures anew, and so does a replaced
-    # class-weight tensor (its address is baked in); an in-place edit of the weights needs no capture, the kernels read
-    # them at every replay
+    # label_smoothing, Dice smooth / eps / ce_weight, Lovász classes / per_image or focal gamma captures anew, and so
+    # does a replaced class-weight tensor (its address is baked in); an in-place edit of the weights needs no capture,
+    # the kernels read them at every replay
     crit = getattr(model, "criterion", None)
     crit_key = (type(crit),) + tuple(getattr(crit, a, None) for a in ("ignore_index", "thresh", "min_kept",
                                                                       "label_smoothing", "reduction", "smooth", "eps",
-                                                                      "ce_weight", "classes", "per_image"))
+                                                                      "ce_weight", "classes", "per_image", "gamma"))
     cw = getattr(crit, "weight", None)
     crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
     teacher = _teacher(crit)

@@ -4,7 +4,8 @@ OhemCrossEntropyLoss is online hard-pixel mining: only the pixels the network is
 the network's fused tail (functional.upsample_ce) it runs inside the same kernels as the default loss, graphed at every
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
-and LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, run the same way. DistillationLoss adds a
+LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and FocalLoss, the softmax focal loss with
+optional class weights, run the same way. DistillationLoss adds a
 pixel-wise distillation term from a frozen teacher network that the student's training forward runs.
 """
 import math
@@ -150,6 +151,56 @@ def _check_native_logits(name, logits, target):
                            % (name, logits.device, target.device))
     if logits.dtype != torch.float32 or target.dtype != torch.int64:
         raise TypeError("%s: fp32 logits and int64 target expected, got %s and %s" % (name, logits.dtype, target.dtype))
+
+
+class FocalLoss(nn.Module):
+    """Softmax focal loss (Lin et al., ICCV 2017), for logits [N, C, H, W] and target [N, H, W]:
+
+        valid = target != ignore_index and 0 <= target < C     (other out-of-range targets are skipped)
+        p     = softmax(logits) over C,  p_t = p[target],  q = 1 - p_t,  nll = -log p_t
+        l     = w_t * q^gamma * nll                             per valid pixel (w_t = 1 without `weight`)
+        loss  = sum of l over the valid pixels / n_valid
+
+    The mean is over the valid pixel count, not over the sum of the weights: a zero-weight class lowers the loss and
+    leaves the denominator alone. q^gamma follows torch.pow (0^0 = 1), so gamma = 0 is the (weighted) cross-entropy
+    summed and divided by n_valid; gamma is any finite float >= 0. With no valid pixel the loss is 0 and every gradient
+    is 0. Under DistributedDataParallel each rank averages over its own pixels.
+
+    `weight` is a 1-D float tensor of one weight per class, registered as a buffer like nn.CrossEntropyLoss's (moved by
+    .cuda() / .to(), saved in the state_dict; without it there is no buffer). It gets no gradient. The native tail needs
+    it contiguous fp32 on the logits' device and reads it on the device at every launch.
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, graphed at every zoom
+    factor; called as a module (validate()) it runs their zoom-1 form on an NHWC copy of the logits. CUDA fp32 logits
+    with at most 256 classes only: there is no CPU or library fallback."""
+
+    def __init__(self, gamma=2.0, weight=None, ignore_index=255):
+        super(FocalLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        if weight is not None:
+            if not torch.is_tensor(weight) or not weight.is_floating_point():
+                raise TypeError("weight must be a floating-point tensor or None, got %r" % (weight,))
+            if weight.dim() != 1 or weight.numel() == 0:
+                raise ValueError("weight must be 1-D with one entry per class, got shape %s" % (tuple(weight.shape),))
+        self.gamma = _non_negative("gamma", gamma)
+        self.ignore_index = ignore_index
+        self.register_buffer("weight", weight)
+
+    def extra_repr(self):
+        s = "gamma=%g, ignore_index=%d" % (self.gamma, self.ignore_index)
+        return s if self.weight is None else s + ", weight=[%d]" % self.weight.numel()
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        _check_native_logits("FocalLoss", logits, target)
+        w = self.weight
+        if w is not None and not (w.numel() == logits.shape[1] and w.dtype == torch.float32 and w.is_contiguous()
+                                  and w.device == logits.device):
+            raise ValueError("FocalLoss: weight must be contiguous fp32 [%d] on %s (no fallback), got %s [%d] on %s" %
+                             (logits.shape[1], logits.device, w.dtype, w.numel(), w.device))
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
 
 
 class DistillationLoss(nn.Module):

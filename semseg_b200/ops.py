@@ -841,6 +841,47 @@ def upsample_ce_dice_bwd(logits, target, ignore_index, lse, table, grad_out, zoo
     return dl
 
 
+def upsample_ce_focal_fwd(logits, target, ignore_index, weight, gamma, want_argmax=True, zoom=8):
+    """Softmax focal loss on the fused tail (include/semseg_b200.h states the contract); arguments as upsample_ce_fwd
+    plus `weight` (fp32 [C] or None = all ones) and `gamma` >= 0 -> (loss_info [2] = (loss, valid count), argmax, lse,
+    mod). mod fp32 [N,Ho,Wo]: each pixel's gradient modulator w_t * M, 0 where the pixel is not valid."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    _check_class_weight(weight, logits)
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_focal_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_focal_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse, mod = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
+    _lib.check(lib.semseg_upsample_ce_focal_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                int(zoom), int(ignore_index), _ptr(weight), float(gamma), _ptr(ws),
+                                                _ptr(info), _ptr(amax), _ptr(lse), _ptr(mod), _stream()),
+               "semseg_upsample_ce_focal_fwd")
+    return info, amax, lse, mod
+
+
+def upsample_ce_focal_bwd(logits, target, ignore_index, lse, mod, info, grad_out, zoom=8):
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_focal_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_focal_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_focal_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                int(zoom), int(ignore_index), _ptr(lse), _ptr(mod), _ptr(info), _ptr(g),
+                                                _ptr(ws), _ptr(dl), _stream()),
+               "semseg_upsample_ce_focal_bwd")
+    return dl
+
+
 def upsample_ce_lovasz_fwd(logits, target, ignore_index, classes_all, per_image, ce_weight, want_argmax=True, zoom=8,
                            return_workspace=False):
     """Lovász-Softmax loss (+ ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract) ->
