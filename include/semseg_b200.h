@@ -26,6 +26,7 @@
  *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
  *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
+ *                               semseg_upsample_pl_*: confidence-masked pseudo-labels from a teacher's logits.
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -566,6 +567,28 @@ long long semseg_upsample_kd_bwd_workspace_floats(int N, int Ho, int w, int C, i
 int semseg_upsample_kd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
                            int C, int Ho, int Wo, int zoom, float temperature, float kd_weight, const float* lse,
                            const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Confidence-masked pseudo-label cross-entropy (semseg_b200/losses.py PseudoLabelLoss) on the same fused upsample at
+ * zoom `zoom`: student and teacher fp32 NHWC [N,h,w,C] maps, each with its own pitch (>= C), both upsampled as the zoom
+ * forward upsamples. Per output pixel, L = {0 <= target < C, target != ignore_index}, U = {target == ignore_index},
+ * yhat = argmax_c t_c (first maximum), conf = 1 / sum_c exp(t_c - t_yhat):
+ *   loss = ce_weight (1/|L|) sum_L (lse(s) - s_target) + pl_weight (1/|U|) sum_{U, conf >= threshold} (lse(s) - s_yhat)
+ * A term whose set is empty is 0 with a zero gradient; other out-of-range targets belong to neither set. threshold is
+ * any finite float (<= 0: every U pixel, > 1: none), pl_weight / ce_weight finite and >= 0.
+ *   fwd: loss_out fp32 [6] = (CE mean over L, |L|, PL sum / |U|, |U|, 0, 1), so loss = ce_weight loss_out[0] +
+ *        pl_weight loss_out[2]; argmax (or NULL) and lse as the zoom forward's (the same bits); eff_target int64
+ *        [N,Ho,Wo] = target on L, yhat on confident U, -1 elsewhere; weight fp32 [N,Ho,Wo] = ce_weight/|L| on L,
+ *        pl_weight/|U| on confident U, 0 elsewhere. workspace: semseg_upsample_pl_workspace_floats() floats, 8-byte
+ *        aligned.
+ *   bwd: semseg_upsample_ce_focal_bwd(student, ..., eff_target, ..., ignore_index = -1, lse, mod = weight,
+ *        loss_info = loss_out + 4, ...) gives grad_out[0] * dloss/dstudent = sum_p weight_p (p_c - [c = eff_p]).
+ * Wo has the Dice limit (2389 at zoom 8). A bad shape, zoom, pitch, option, width, alignment or null pointer is rejected
+ * before any CUDA call; the workspace function returns -1 for a bad zoom or size. No host synchronisation; the counts
+ * are integer atomics and the sums fixed-order: deterministic. */
+long long semseg_upsample_pl_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_pl_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                           int C, const int64_t* target, int Ho, int Wo, int zoom, int ignore_index, float threshold,
+                           float pl_weight, float ce_weight, float* workspace, float* loss_out, int64_t* argmax,
+                           float* lse, int64_t* eff_target, float* weight, void* stream);
 /* Segmented stable radix sort (csrc/segsort.cu): S segments of L (uint32 key, uint32 payload) pairs, [S][L], each sorted
  * in place by key ascending, equal keys in input order. keys_alt / vals_alt: scratch of the same size. skip: NULL, or
  * int [S] on the device, a non-zero entry leaves that segment untouched. workspace:
@@ -633,6 +656,26 @@ typedef struct semseg_sgd_hyper {
 int semseg_sgd_chunk_elems(void);
 int semseg_sgd_multi(const semseg_sgd_item* items_dev, const void* grad_ptrs_dev, int n_items, int n_chunks,
                      const semseg_sgd_hyper* hyper, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Exponential moving average of a model's weights (semseg_b200/optim.py ModelEMA) over every tensor in one launch, on
+ * semseg_sgd_multi's table layout (an item's chunks are consecutive blocks of semseg_sgd_chunk_elems() elements,
+ * items_dev sorted by chunk0, 8-byte aligned). kind SEMSEG_EMA_LERP_F32: shadow <- lerp(shadow, source, 1 - decay) on
+ * fp32, in torch.lerp's two-branch form (weight < 0.5: e + weight (w - e); else w - (w - e) (1 - weight)), so the bits
+ * equal torch._foreach_lerp_(shadow, source, 1 - decay); decay 0 copies, decay 1 leaves the shadow as it is.
+ * kind SEMSEG_EMA_COPY_I64: the n int64 elements are copied (BatchNorm's num_batches_tracked). Element-wise and
+ * deterministic; a null table, counts <= 0, decay outside [0, 1] or a misaligned table is rejected before any CUDA call.
+ */
+#define SEMSEG_EMA_LERP_F32 0
+#define SEMSEG_EMA_COPY_I64 1
+typedef struct semseg_ema_item {
+  void* shadow;
+  const void* source;
+  long long n;
+  int kind;
+  int chunk0;
+} semseg_ema_item;
+int semseg_ema_multi(const semseg_ema_item* items_dev, int n_items, int n_chunks, double decay, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Training-batch augmentation: tool/train.py:194-201's RandScale -> RandRotate -> RandomGaussianBlur ->

@@ -38,6 +38,14 @@ class SgdItem(ctypes.Structure):
                 ("reserved", c_i32)]
 
 
+EMA_LERP_F32, EMA_COPY_I64 = 0, 1        # semseg_ema_item.kind
+
+
+class EmaItem(ctypes.Structure):
+    """struct semseg_ema_item (include/semseg_b200.h)."""
+    _fields_ = [("shadow", c_vp), ("source", c_vp), ("n", c_ll), ("kind", c_i32), ("chunk0", c_i32)]
+
+
 class SgdHyper(ctypes.Structure):
     """struct semseg_sgd_hyper (include/semseg_b200.h)."""
     _fields_ = [("lr", c_f * 16), ("momentum", c_f * 16), ("weight_decay", c_f * 16), ("dampening", c_f * 16),
@@ -122,6 +130,7 @@ SIGNATURES = {
     "semseg_pack_weights_multi": (c_int, [c_vp, c_int, c_int, c_int, c_vp]),
     "semseg_sgd_chunk_elems": (c_int, []),
     "semseg_sgd_multi": (c_int, [c_vp, c_vp, c_int, c_int, ctypes.POINTER(SgdHyper), c_vp]),
+    "semseg_ema_multi": (c_int, [c_vp, c_int, c_int, ctypes.c_double, c_vp]),
     "semseg_iou_hist": (c_int, [c_vp, c_vp, ctypes.c_longlong, c_int, ctypes.c_longlong, c_int, c_vp, c_vp]),
     "semseg_im2col3x3s2": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_stem_dgrad3x3s2": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int,
@@ -217,6 +226,9 @@ SIGNATURES = {
     "semseg_upsample_kd_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_kd_bwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f,
                                        c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_pl_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_pl_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
+                                       c_int, c_f, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_segsort_u32_pairs_workspace_bytes": (c_ll, [c_int, c_ll]),
     "semseg_segsort_u32_pairs": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_ll, c_vp, c_vp, c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),

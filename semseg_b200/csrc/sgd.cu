@@ -65,7 +65,70 @@ sgd_multi_kernel(const semseg_sgd_item* __restrict__ items, const unsigned long 
   }
 }
 
+// Exponential moving average of a model's weights (semseg_b200/optim.py ModelEMA) in one launch, on the item-table and
+// chunk layout of sgd_multi_kernel. fp32 items: e <- lerp(e, w, weight), weight = 1 - decay, in the two-branch form of
+// torch.lerp (ATen's Lerp.h), so the result is the bits torch._foreach_lerp_(shadow, source, 1 - decay) gives:
+//   weight < 0.5: e + weight (w - e)      else: w - (w - e) (1 - weight)
+// (weight 1, decay 0, is an exact copy; weight 0 leaves e as it is). int64 items are copied. Element-wise, no atomics.
+__device__ __forceinline__ float ema_lerp(float e, float w, float weight) {
+  return fabsf(weight) < 0.5f ? fmaf(weight, w - e, e) : fmaf(-(w - e), 1.f - weight, w);
+}
+
+__global__ void __launch_bounds__(256)
+ema_multi_kernel(const semseg_ema_item* __restrict__ items, int n_items, float weight) {
+  __shared__ int s_item;
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = n_items - 1;
+    const int b = static_cast<int>(blockIdx.x);
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (items[mid].chunk0 <= b) lo = mid; else hi = mid - 1;
+    }
+    s_item = lo;
+  }
+  __syncthreads();
+  const semseg_ema_item it = items[s_item];
+  const long long base = static_cast<long long>(static_cast<int>(blockIdx.x) - it.chunk0) * kSgdChunk;
+  const long long end = min(base + kSgdChunk, it.n);
+  if (it.kind == SEMSEG_EMA_COPY_I64) {
+    long long* __restrict__ e = static_cast<long long*>(it.shadow);
+    const long long* __restrict__ w = static_cast<const long long*>(it.source);
+    for (long long i = base + threadIdx.x; i < end; i += blockDim.x) e[i] = w[i];
+    return;
+  }
+  float* __restrict__ e = static_cast<float*>(it.shadow);
+  const float* __restrict__ w = static_cast<const float*>(it.source);
+  const bool vec = ((reinterpret_cast<uintptr_t>(e) | reinterpret_cast<uintptr_t>(w)) & 15) == 0;
+  long long tail = base;
+  if (vec) {
+    for (long long i = base + 4LL * threadIdx.x; i + 3 < end; i += 4LL * blockDim.x) {
+      float4 a = *reinterpret_cast<const float4*>(e + i);
+      const float4 b = *reinterpret_cast<const float4*>(w + i);
+      a.x = ema_lerp(a.x, b.x, weight);
+      a.y = ema_lerp(a.y, b.y, weight);
+      a.z = ema_lerp(a.z, b.z, weight);
+      a.w = ema_lerp(a.w, b.w, weight);
+      *reinterpret_cast<float4*>(e + i) = a;
+    }
+    tail = base + ((end - base) & ~3LL);
+  }
+  for (long long i = tail + threadIdx.x; i < end; i += blockDim.x) e[i] = ema_lerp(e[i], w[i], weight);
+}
+
 }  // namespace sb
+
+extern "C" int semseg_ema_multi(const semseg_ema_item* items_dev, int n_items, int n_chunks, double decay,
+                                void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SB_CHECK_ARG(items_dev, "ema_multi: null item table");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(items_dev) & 7) == 0, "ema_multi: item table not 8-byte aligned");
+  SB_CHECK_ARG(n_items > 0 && n_chunks > 0, "ema_multi: bad counts (%d items, %d chunks)", n_items, n_chunks);
+  SB_CHECK_ARG(decay >= 0.0 && decay <= 1.0, "ema_multi: decay %g outside [0, 1]", decay);
+  sb::ema_multi_kernel<<<static_cast<unsigned>(n_chunks), 256, 0, stream>>>(items_dev, n_items,
+                                                                            static_cast<float>(1.0 - decay));
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
 
 extern "C" int semseg_sgd_chunk_elems(void) { return sb::kSgdChunk; }
 

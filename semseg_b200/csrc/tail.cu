@@ -41,6 +41,10 @@
 //
 // The softmax focal loss, with or without class weights, runs sibling forward and rows kernels (see "focal loss" below)
 // with the plain reduce and cols kernels; no existing instance changes.
+//
+// Confidence-masked pseudo-labels from a teacher's logits run a count pass and a two-map forward (see "pseudo-labels"
+// below); their backward is the focal backward on the forward's effective targets and weights. No existing instance
+// changes.
 #include <cmath>
 
 #include "host_common.h"
@@ -1785,6 +1789,180 @@ upsample_ce_focal_rows_kernel(const float* __restrict__ logits, int pitch, int N
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- pseudo-labels
+// Confidence-masked pseudo-label cross-entropy from a teacher (FixMatch / UniMatch self-training), with s and t the
+// student and teacher maps after the same xZ upsample:
+//   L = {target in [0, C), target != ignore_index},  U = {target == ignore_index}
+//   yhat = argmax_c t_c (first maximum),  conf = 1 / sum_c exp(t_c - t_yhat)
+//   loss = ce_weight (1/|L|) sum_L (lse - s_target) + pl_weight (1/|U|) sum_{U, conf >= threshold} (lse - s_yhat)
+// Both terms are CE against a per-pixel "effective target" with a per-pixel weight, so the gradient is
+// w_p (p_c - [c = y_p]): the focal backward (rows kernel staging (lse, target, modulator), plain cols kernel with a
+// count of 1) run on the forward's effective-target and weight maps. The weights need |L| and |U| before the forward
+// writes them: a count pass over the target runs first (integer atomics: the counts do not depend on their order).
+//   count  : |L|, |U| as uint64 into the workspace; also writes loss_out[4] = 0, loss_out[5] = 1 (the cols count).
+//   forward: the distillation forward's geometry (both maps' node rows staged), the student's max / argmax / lse with the
+//            plain forward's operations (the plain tail's bits), the teacher's max / argmax / sum of exp in the same
+//            passes; per pixel the effective target (target on L, yhat on confident U, -1 otherwise) and weight
+//            (ce_weight/|L|, pl_weight/|U|, 0); (sum CE over L, |L|) and (sum PL, |U|) per CTA, each reduced in fp64 by
+//            the plain reduce kernel.
+__global__ void __launch_bounds__(256)
+upsample_pl_count_kernel(const long long* __restrict__ target, long long M, int C, int ignore_index,
+                         unsigned long long* __restrict__ counts, float* __restrict__ loss_out) {
+  unsigned nl = 0, nu = 0;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < M;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long t = target[i];
+    if (t == ignore_index) ++nu;
+    else if (t >= 0 && t < C) ++nl;
+  }
+  nl = __reduce_add_sync(0xffffffffu, nl);
+  nu = __reduce_add_sync(0xffffffffu, nu);
+  if ((threadIdx.x & 31) == 0) {
+    if (nl) atomicAdd(&counts[0], static_cast<unsigned long long>(nl));
+    if (nu) atomicAdd(&counts[1], static_cast<unsigned long long>(nu));
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    loss_out[4] = 0.f;
+    loss_out[5] = 1.f;
+  }
+}
+
+template <int Z>
+__global__ void __launch_bounds__(KdGeom<Z>::kCols)
+upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* __restrict__ tl, int pitch_t, int N, int h,
+                       int w, int C, int Cs, const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                       float threshold, float pl_weight, float ce_weight, const unsigned long long* __restrict__ counts,
+                       float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out,
+                       long long* __restrict__ eff_out, float* __restrict__ wt_out) {
+  using G = Zoom<Z>;
+  constexpr int kCols = KdGeom<Z>::kCols, kNodes = KdGeom<Z>::kNodes;
+  extern __shared__ float S[];  // [2 maps: student, teacher][kNodeRows][kNodes][Cs], as upsample_kd_fwd_kernel
+  __shared__ float red[4][kCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kNodes, w - j_base);
+  const int tid = threadIdx.x;
+  const int map_floats = G::kNodeRows * kNodes * Cs;
+  for (int idx = tid; idx < 2 * G::kNodeRows * nj * C; idx += kCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = (node / nj) % G::kNodeRows, map = node / (nj * G::kNodeRows);
+    const size_t src = (static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj);
+    S[map * map_floats + (rr * kNodes + jj) * Cs + c] = map ? tl[src * pitch_t + c] : sl[src * pitch_s + c];
+  }
+  __syncthreads();
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};   // sum CE over L, |L|, sum PL over confident U, |U|
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* A = S + (j0 - j_base) * Cs;   // student nodes (i0, j0), (i0, j1), (i1, j0), (i1, j1)
+    const float* B = S + (j1 - j_base) * Cs;
+    const float* Cc = A + kNodes * Cs;
+    const float* D = B + kNodes * Cs;
+    const float* At = A + map_floats;          // teacher nodes
+    const float* Bt = B + map_floats;
+    const float* Ct = Cc + map_floats;
+    const float* Dt = D + map_floats;
+    float ms[Z], mt[Z], zs[Z], zt[Z];
+    int as[Z], at[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      ms[r] = mt[r] = -INFINITY;
+      as[r] = at[r] = 0;
+      zs[r] = zt[r] = 0.f;
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+      const float topt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
+      const float bott = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        if (v > ms[r]) {
+          ms[r] = v;
+          as[r] = c;
+        }
+        const float u = row_lerp<Z>(topt, bott, r);
+        if (u > mt[r]) {
+          mt[r] = u;
+          at[r] = c;
+        }
+      }
+    }
+    float m2[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) m2[r] = ms[r] * kLog2e;
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+      const float topt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
+      const float bott = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        zs[r] += ex2_approx(fmaf(row_lerp<Z>(top, bot, r), kLog2e, -m2[r]));   // the plain forward's sum
+        zt[r] += ex2_approx((row_lerp<Z>(topt, bott, r) - mt[r]) * kLog2e);    // yhat's term is exactly 1
+      }
+    }
+    const unsigned long long nl = counts[0], nu = counts[1];
+    const float wl = nl ? ce_weight / static_cast<float>(nl) : 0.f;
+    const float wu = nu ? pl_weight / static_cast<float>(nu) : 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+        const long long t = target[pix];
+        const float lse = ms[r] + __logf(zs[r]);
+        if (argmax_out) argmax_out[pix] = as[r];
+        lse_out[pix] = lse;
+        int y = -1;
+        float wt = 0.f;
+        if (t == ignore_index) {
+          acc[3] += 1.f;
+          if (1.f / zt[r] >= threshold) {
+            y = at[r];
+            wt = wu;
+          }
+        } else if (t >= 0 && t < C) {
+          y = static_cast<int>(t);
+          wt = wl;
+          acc[1] += 1.f;
+        }
+        if (y >= 0) {
+          const float top = Z == 1 ? A[y] : l0w * A[y] + l1w * B[y];
+          const float bot = Z == 1 ? 0.f : l0w * Cc[y] + l1w * D[y];
+          acc[t == ignore_index ? 2 : 0] += lse - row_lerp<Z>(top, bot, r);
+        }
+        eff_out[pix] = y;
+        wt_out[pix] = wt;
+      }
+    }
+  }
+  // deterministic block reduction -> (sum CE, |L|) and (sum PL, |U|) per CTA, each laid out as the plain partials
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
+  }
+  if ((tid & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) red[k][tid >> 5] = acc[k];
+  }
+  __syncthreads();
+  if (tid < 4) {
+    float s = 0.f;
+    for (int i = 0; i < kCols / 32; ++i) s += red[tid][i];
+    const size_t nb = static_cast<size_t>(gridDim.x) * gridDim.y * gridDim.z;
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[(tid >> 1) * 2 * nb + 2 * b + (tid & 1)] = s;
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -2702,6 +2880,97 @@ extern "C" int semseg_upsample_kd_bwd(const float* student, int pitch_s, const f
                                     lse, grad_out, workspace, dlogits, stream);
     default: return launch_kd_bwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, kd_weight,
                                      lse, grad_out, workspace, dlogits, stream);
+  }
+}
+
+// Pseudo-label cross-entropy at zoom factor `zoom`: the count pass, the two-map forward and the plain reduce; the
+// backward is semseg_upsample_ce_focal_bwd on the effective targets and weights, so Wo has the Dice limit.
+// Workspace: the two uint64 counts (4 floats), then 2 x (value, count) partials per forward CTA.
+static int check_pl(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w, int C,
+                    const void* target, int Ho, int Wo, int zoom, float threshold, float pl_weight, float ce_weight) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_pl: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(student && teacher && target, "upsample_pl: null pointer");
+  SB_CHECK_ARG(N > 0 && h > 1 && w > 1 && C > 1 && C <= kMaxClasses, "upsample_pl: bad sizes (C<=%d)", kMaxClasses);
+  SB_CHECK_ARG(pitch_s >= C && pitch_t >= C, "upsample_pl: pitch %d / %d below C = %d", pitch_s, pitch_t, C);
+  SB_CHECK_ARG(Ho == zoom * (h - 1) + 1 && Wo == zoom * (w - 1) + 1,
+               "upsample_pl: needs Ho=%d(h-1)+1, Wo=%d(w-1)+1 (got %dx%d -> %dx%d)", zoom, zoom, h, w, Ho, Wo);
+  SB_CHECK_ARG(std::isfinite(threshold), "upsample_pl: threshold %g is not finite", threshold);
+  SB_CHECK_ARG(std::isfinite(pl_weight) && pl_weight >= 0.f, "upsample_pl: pl_weight %g is not finite and >= 0",
+               pl_weight);
+  SB_CHECK_ARG(std::isfinite(ce_weight) && ce_weight >= 0.f, "upsample_pl: ce_weight %g is not finite and >= 0",
+               ce_weight);
+  const size_t max_wo = kDiceSmemMax / (static_cast<size_t>(zoom) * sizeof(DicePix));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_pl: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_pl_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                         int C, const int64_t* target, int Ho, int Wo, int ignore_index, float threshold,
+                         float pl_weight, float ce_weight, float* workspace, float* loss_out, int64_t* argmax,
+                         float* lse, int64_t* eff, float* wt, cudaStream_t stream) {
+  using K = KdGeom<Z>;
+  unsigned long long* counts = reinterpret_cast<unsigned long long*>(workspace);
+  float* partial = workspace + 4;
+  const int ctas = kd_fwd_ctas<Z>(N, h, Wo);
+  const long long M = static_cast<long long>(N) * Ho * Wo;
+  SB_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(unsigned long long), stream));
+  const int count_ctas = static_cast<int>(std::min<long long>((M + 255) / 256, 4LL * num_sms()));
+  upsample_pl_count_kernel<<<count_ctas, 256, 0, stream>>>(reinterpret_cast<const long long*>(target), M, C,
+                                                           ignore_index, counts, loss_out);
+  SB_LAUNCHED();
+  const int Cs = C | 1;
+  constexpr size_t kMaxSmem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_pl_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_pl_fwd_kernel<Z><<<dim3(cdiv(Wo, K::kCols), h, N), K::kCols, smem, stream>>>(
+      student, pitch_s, teacher, pitch_t, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo,
+      ignore_index, threshold, pl_weight, ce_weight, counts, partial, reinterpret_cast<long long*>(argmax), lse,
+      reinterpret_cast<long long*>(eff), wt);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(partial, ctas, loss_out);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(partial + 2LL * ctas, ctas, loss_out + 2);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_pl_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_pl: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0, "upsample_pl: bad sizes");
+  return 4 + 2 * kd_fwd_partials(N, (Ho - 1) / zoom + 1, Wo, zoom);
+}
+
+extern "C" int semseg_upsample_pl_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N,
+                                      int h, int w, int C, const int64_t* target, int Ho, int Wo, int zoom,
+                                      int ignore_index, float threshold, float pl_weight, float ce_weight,
+                                      float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                      int64_t* eff_target, float* weight, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_pl(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, zoom, threshold, pl_weight,
+                   ce_weight);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && eff_target && weight, "upsample_pl_fwd: null output");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "upsample_pl_fwd: workspace not 8-byte aligned");
+  switch (zoom) {
+    case 1: return launch_pl_fwd<1>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                    threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                    weight, stream);
+    case 2: return launch_pl_fwd<2>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                    threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                    weight, stream);
+    case 4: return launch_pl_fwd<4>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                    threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                    weight, stream);
+    default: return launch_pl_fwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                     threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                     weight, stream);
   }
 }
 

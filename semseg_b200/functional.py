@@ -71,23 +71,24 @@ def _is_patch_conv(conv):
             and conv.in_channels <= 3 and conv.groups == 1)
 
 
-def prepack(model, force=False):
+def prepack(model, force=False, dgrad=True):
     """Refresh the operand slabs of every native conv of `model` in one launch when its weights changed (call at the top
     of a training forward; force=True while the step is being captured into a CUDA graph, so that the re-pack is part
-    of every replay). Convs keep working without it: `packed` re-packs each conv through its own one-conv plan."""
+    of every replay). Convs keep working without it: `packed` re-packs each conv through its own one-conv plan.
+    dgrad=False packs the forward slabs only (a network that runs forward only, such as a mean teacher)."""
     convs = [m for m in model.modules() if isinstance(m, nn.Conv2d) and m.weight.is_cuda and
              m.weight.dtype == torch.float32 and m.weight.is_contiguous() and m.kernel_size[0] == m.kernel_size[1] and
              m.kernel_size[0] * m.kernel_size[1] <= ops.MAX_TAPS]
     if not convs:
         return
     split = precision.split_enabled()
-    keys = [(c.weight._version, c.weight.data_ptr(), True, split) for c in convs]
+    keys = [(c.weight._version, c.weight.data_ptr(), dgrad, split) for c in convs]
     if not force and all(c.__dict__.get("_sb_pack", (None,))[0] == k for c, k in zip(convs, keys)):
         return                                            # nothing changed since the last pack
     plan = model.__dict__.get("_sb_pack_plan")
     weights = [c.weight.detach() for c in convs]
-    if plan is None or not plan.valid_for(weights, split):
-        plan = ops.WeightPackPlan(weights, split, patches=[_is_patch_conv(c) for c in convs])
+    if plan is None or not plan.valid_for(weights, split) or (dgrad and plan.packs[0].wd is None):
+        plan = ops.WeightPackPlan(weights, split, dgrad=dgrad, patches=[_is_patch_conv(c) for c in convs])
         model.__dict__["_sb_pack_plan"] = plan
     plan.refresh()
     for c, k, pw in zip(convs, keys, plan.packs):
@@ -667,6 +668,28 @@ class _UpsampleCEKD(torch.autograd.Function):
         return dl, None, None, None, None, None, None, None, None
 
 
+class _UpsampleCEPL(torch.autograd.Function):
+    """The fused tail with losses.PseudoLabelLoss: ce_weight * CE over the labelled pixels plus pl_weight * the
+    confidence-masked pseudo-label CE over the unlabelled ones. The forward keeps each pixel's effective target and
+    weight; the backward is the focal backward on them (w_p (p_c - [c = y_p]), the plain cols kernel with a count of 1).
+    The teacher map is a constant: it gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, teacher_logits, target, ignore_index, zoom, threshold, pl_weight, ce_weight):
+        info, amax, lse, eff, wt = ops.upsample_pl_fwd(logits, teacher_logits, target, ignore_index, threshold,
+                                                       pl_weight, ce_weight, zoom=zoom)
+        ctx.save_for_backward(logits, eff, lse, wt, info)
+        ctx.zoom = zoom
+        ctx.mark_non_differentiable(amax)
+        return torch.add(info[0] * ce_weight, info[2], alpha=pl_weight), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, eff, lse, wt, info = ctx.saved_tensors
+        dl = ops.upsample_ce_focal_bwd(logits, eff, -1, lse, wt, info[4:], grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None, None, None
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""
@@ -689,7 +712,7 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     contiguous fp32 [classes] tensor on that device; any other weight, another reduction, and any subclass keep the
     ATen tail. DiceLoss, FocalLoss and losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
-    form's conditions.
+    form's conditions; losses.PseudoLabelLoss, whose backward is the focal one, the Dice width limit.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
         ok = True
@@ -698,7 +721,8 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         plain = criterion.weight is None and eps == 0.0
         ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
               (plain or (target is not None and target.is_cuda)))
-    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss):     # the focal rows kernel stages the Dice words
+    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss, losses.PseudoLabelLoss):
+        # the focal rows kernel (the pseudo-label backward too) stages the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     elif type(criterion) is losses.LovaszSoftmaxLoss:
@@ -730,12 +754,15 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index); with a losses.LovaszSoftmaxLoss, its
     Lovász-Softmax (+ CE) loss; with a losses.FocalLoss, its focal loss (its own ignore_index, gamma and class
     weights); with a losses.DistillationLoss and the teacher's fp32 NHWC logits `teacher_logits`
-    (the student's shape), its distillation loss (without them: the plain mean CE, the loss of the aux head). The
-    default criterion runs the plain kernels."""
+    (the student's shape), its distillation loss, and with a losses.PseudoLabelLoss and them its pseudo-label loss
+    (without them: the plain mean CE, the loss of the aux head). The default criterion runs the plain kernels."""
     if isinstance(criterion, losses.DistillationLoss) and teacher_logits is not None:
         kd_zoom = 1 if criterion.at == 'logits' else int(zoom)
         return _UpsampleCEKD.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
                                    int(zoom), kd_zoom, criterion.temperature, criterion.kd_weight, criterion.ce_weight)
+    if isinstance(criterion, losses.PseudoLabelLoss) and teacher_logits is not None:
+        return _UpsampleCEPL.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
+                                   int(zoom), criterion.threshold, criterion.pl_weight, criterion.ce_weight)
     if isinstance(criterion, losses.LovaszSoftmaxLoss):
         return _UpsampleCELovasz.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
                                        criterion.classes == 'all', bool(criterion.per_image), criterion.ce_weight)

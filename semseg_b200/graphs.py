@@ -19,8 +19,8 @@ Limits (same as torch.cuda.make_graphed_callables): a second training forward be
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
-loss, the focal loss and the distillation loss, whose teacher forward is captured with the step) are not captured (such
-models simply stay eager).
+loss, the focal loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
+mean teacher's re-pack included) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -256,14 +256,17 @@ def _capture(model, impl, st, x, y):
     st.keep = model.__dict__.get("_sb_pack_plan")
     teacher = _teacher(getattr(model, "criterion", None))
     if teacher is not None:
-        st.keep = (st.keep, teacher, [m.__dict__.get("_sb_conv_plan") for m in teacher.modules()])
+        # a mean teacher's slabs are its whole-model plan's, re-packed inside the captured step
+        st.keep = (st.keep, teacher, teacher.__dict__.get("_sb_pack_plan"),
+                   [m.__dict__.get("_sb_conv_plan") for m in teacher.modules()])
     torch.cuda.synchronize()
 
 
 def _teacher(crit):
-    """The teacher network a losses.DistillationLoss criterion runs inside the step, else None."""
+    """The teacher network a losses.DistillationLoss or losses.PseudoLabelLoss criterion runs inside the step, else
+    None."""
     from . import losses
-    return crit.teacher if isinstance(crit, losses.DistillationLoss) else None
+    return crit.teacher if isinstance(crit, losses._TeacherLoss) else None
 
 
 def train_step(model, impl, x, y):
@@ -293,13 +296,18 @@ def train_step(model, impl, x, y):
     crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
     teacher = _teacher(crit)
     if teacher is not None:
-        # a distillation teacher runs inside the forward graph: its identity, the addresses and versions of its
-        # parameters and buffers (an in-place edit of a weight bumps the version, so the step is captured again with
-        # the edit rather than replayed stale), its BatchNorm modes and the options of the KL term are baked in too
-        crit_key += (id(teacher), tuple((t.data_ptr(), t._version) for t in teacher.parameters()),
-                     tuple((t.data_ptr(), t._version) for t in teacher.buffers()),
-                     tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)),
-                     crit.temperature, crit.kd_weight, crit.at)
+        # a teacher runs inside the forward graph: its identity, the addresses and versions of its parameters and
+        # buffers (an in-place edit of a frozen teacher's weight bumps the version, so the step is captured again with
+        # the edit rather than replayed stale), its BatchNorm modes and the options of the KL / pseudo-label term are
+        # baked in too. A ModelEMA shadow changes every step: its key holds the addresses only, because the captured
+        # step re-packs its slabs and folds its BatchNorm statistics at every replay (losses._TeacherLoss.run_teacher)
+        if getattr(teacher, "_sb_ema_shadow", False):
+            tkey = lambda ts: tuple(t.data_ptr() for t in ts)                          # noqa: E731
+        else:
+            tkey = lambda ts: tuple((t.data_ptr(), t._version) for t in ts)            # noqa: E731
+        crit_key += (id(teacher), tkey(teacher.parameters()), tkey(teacher.buffers()),
+                     tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
+        crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight"))
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
            dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad,
            crit_key)

@@ -6,7 +6,9 @@ zoom factor; called as a module (validate(), or the network's tail when the fuse
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
 LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and FocalLoss, the softmax focal loss with
 optional class weights, run the same way. DistillationLoss adds a
-pixel-wise distillation term from a frozen teacher network that the student's training forward runs.
+pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
+confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
+optim.ModelEMA.
 """
 import math
 
@@ -203,8 +205,78 @@ class FocalLoss(nn.Module):
         return loss
 
 
-class DistillationLoss(nn.Module):
-    """Pixel-wise knowledge distillation from a frozen teacher network, plus cross-entropy. With s, t the student and
+class _TeacherLoss(nn.Module):
+    """What the criteria that learn from a teacher network share: the teacher, held outside the module tree, and
+    `run_teacher`, its forward inside the student's training forward.
+
+    `teacher` is a PSPNet or PSANet of this package, in eval mode, on the input's device, with the student's number of
+    classes: a frozen network, or the `module` of an optim.ModelEMA (a mean teacher). It is held, not owned: it is not a
+    submodule, so it stays out of the student's state_dict, modules(), .cuda() / .to(), convert_sync_batchnorm and DDP's
+    buffer broadcast. It runs inside the student's training forward, before the student's stem, under torch.no_grad() in
+    the student's precision mode, on the folded eval kernels; the criterion never modifies its parameters, running
+    statistics or training flag, and no gradient reaches it or, through it, the input (with x.requires_grad, x.grad is
+    the student's). A ModelEMA shadow changes after every `ema.update`: its operand slabs are re-packed at the top of
+    every teacher forward (in one launch, part of the captured training step), and the graphed step is keyed on its
+    tensors' addresses, not their versions, so it is captured once and replays each step with the current shadow."""
+
+    def __init__(self, teacher, ignore_index):
+        super(_TeacherLoss, self).__init__()
+        from .pspnet import PSPNet
+        from .psanet import PSANet
+        if not isinstance(teacher, (PSPNet, PSANet)):
+            raise TypeError("teacher must be a semseg_b200 PSPNet or PSANet, got %s" % type(teacher).__name__)
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        self.ignore_index = ignore_index
+        self.__dict__['_teacher'] = teacher      # held outside the module tree (see the class docstring)
+
+    @property
+    def teacher(self):
+        return self.__dict__['_teacher']
+
+    def __setattr__(self, name, value):
+        # nn.Module.__setattr__ would register a module value as a child, past the read-only property
+        if name in ('teacher', '_teacher'):
+            raise AttributeError("%s: the teacher is fixed at construction; build a new criterion" %
+                                 type(self).__name__)
+        super(_TeacherLoss, self).__setattr__(name, value)
+
+    def run_teacher(self, x, classes):
+        """The teacher's detached fp32 NHWC 1/8-resolution logits of the input batch `x` (NCHW), for a student with
+        `classes` classes."""
+        from . import functional as SF
+        from . import graphs
+        name = type(self).__name__
+        teacher = self.teacher
+        # the network and every layer whose mode changes the forward (the teacher's own criterion, a module that the
+        # networks' default argument shares with every other network, does not take part)
+        if teacher.training or any(m.training for m in teacher.modules()
+                                   if isinstance(m, (nn.modules.batchnorm._BatchNorm, nn.modules.dropout._DropoutNd))):
+            raise RuntimeError("%s: the teacher must be in eval mode (call teacher.eval())" % name)
+        dev = next(teacher.parameters()).device
+        if dev != x.device:
+            raise RuntimeError("%s: the teacher is on %s, the input on %s (move the teacher yourself)" %
+                               (name, dev, x.device))
+        tc = teacher.cls[4].out_channels
+        if tc != classes:
+            raise ValueError("%s: the teacher has %d classes, the student %d" % (name, tc, classes))
+        if getattr(teacher, "_sb_ema_shadow", False):
+            # a mean teacher changes every step: its slabs are re-packed here, inside the captured step while capturing
+            SF.prepack(teacher, force=graphs.capturing(), dgrad=False)
+        with torch.no_grad(), SF.network_mode(False, False):
+            return teacher._eval_logits_nhwc(x.detach())
+
+    def _teacher_logits_nhwc(self, logits, teacher_logits):
+        if teacher_logits.shape != logits.shape or teacher_logits.dtype != torch.float32 or \
+                teacher_logits.device != logits.device:
+            raise ValueError("%s: teacher_logits must be fp32 %s on %s like the logits, got %s %s on %s" %
+                             (type(self).__name__, tuple(logits.shape), logits.device, teacher_logits.dtype,
+                              tuple(teacher_logits.shape), teacher_logits.device))
+        return teacher_logits.detach().permute(0, 2, 3, 1).contiguous()
+
+
+class DistillationLoss(_TeacherLoss):
+    """Pixel-wise knowledge distillation from a teacher network, plus cross-entropy. With s, t the student and
     teacher logits at the KD resolution, T the temperature, p = softmax(s/T) and q = softmax(t/T) over the classes and P
     the number of pixels at the KD resolution over all images of the call:
 
@@ -218,12 +290,8 @@ class DistillationLoss(nn.Module):
     criteria: target != ignore_index and 0 <= target < C. Under DistributedDataParallel each rank holds its own teacher
     and averages over its own pixels.
 
-    `teacher` is a PSPNet or PSANet of this package, in eval mode, on the input's device, with the student's number of
-    classes; the user moves it there. It is held, not owned: it is not a submodule, so it stays out of the student's
-    state_dict, modules(), .cuda() / .to(), convert_sync_batchnorm and DDP's buffer broadcast. It runs inside the
-    student's training forward, before the student's stem, under torch.no_grad() in the student's precision mode, on the
-    folded eval kernels; its parameters, running statistics and training flag are never modified, and no gradient
-    reaches it or, through it, the input (with x.requires_grad, x.grad is the student's).
+    `teacher` is a frozen PSPNet or PSANet of this package or the `module` of an optim.ModelEMA, with the rules of
+    _TeacherLoss (eval mode, the input's device, the student's classes; held outside the module tree; never modified).
 
     With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, teacher forward and KL
     term graphed at every zoom factor. Called as a module, forward(logits, target, teacher_logits=None) takes NCHW logits
@@ -232,13 +300,7 @@ class DistillationLoss(nn.Module):
     CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
 
     def __init__(self, teacher, temperature=1.0, kd_weight=1.0, ce_weight=1.0, ignore_index=255, at='output'):
-        super(DistillationLoss, self).__init__()
-        from .pspnet import PSPNet
-        from .psanet import PSANet
-        if not isinstance(teacher, (PSPNet, PSANet)):
-            raise TypeError("teacher must be a semseg_b200 PSPNet or PSANet, got %s" % type(teacher).__name__)
-        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
-            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        super(DistillationLoss, self).__init__(teacher, ignore_index)
         if not isinstance(at, str):
             raise TypeError("at must be 'output' or 'logits', got %r" % (at,))
         if at not in ('output', 'logits'):
@@ -249,43 +311,11 @@ class DistillationLoss(nn.Module):
         self.temperature = temperature
         self.kd_weight = _non_negative("kd_weight", kd_weight)
         self.ce_weight = _non_negative("ce_weight", ce_weight)
-        self.ignore_index = ignore_index
         self.at = at
-        self.__dict__['_teacher'] = teacher      # held outside the module tree (see the class docstring)
-
-    @property
-    def teacher(self):
-        return self.__dict__['_teacher']
-
-    def __setattr__(self, name, value):
-        # nn.Module.__setattr__ would register a module value as a child, past the read-only property
-        if name in ('teacher', '_teacher'):
-            raise AttributeError("DistillationLoss: the teacher is fixed at construction; build a new criterion")
-        super(DistillationLoss, self).__setattr__(name, value)
 
     def extra_repr(self):
         return "teacher=%s, temperature=%g, kd_weight=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
             type(self.teacher).__name__, self.temperature, self.kd_weight, self.ce_weight, self.ignore_index, self.at)
-
-    def run_teacher(self, x, classes):
-        """The teacher's detached fp32 NHWC 1/8-resolution logits of the input batch `x` (NCHW), for a student with
-        `classes` classes."""
-        from . import functional as SF
-        teacher = self.teacher
-        # the network and every layer whose mode changes the forward (the teacher's own criterion, a module that the
-        # networks' default argument shares with every other network, does not take part)
-        if teacher.training or any(m.training for m in teacher.modules()
-                                   if isinstance(m, (nn.modules.batchnorm._BatchNorm, nn.modules.dropout._DropoutNd))):
-            raise RuntimeError("DistillationLoss: the teacher must be in eval mode (call teacher.eval())")
-        dev = next(teacher.parameters()).device
-        if dev != x.device:
-            raise RuntimeError("DistillationLoss: the teacher is on %s, the input on %s (move the teacher yourself)" %
-                               (dev, x.device))
-        tc = teacher.cls[4].out_channels
-        if tc != classes:
-            raise ValueError("DistillationLoss: the teacher has %d classes, the student %d" % (tc, classes))
-        with torch.no_grad(), SF.network_mode(False, False):
-            return teacher._eval_logits_nhwc(x.detach())
 
     def forward(self, logits, target, teacher_logits=None):
         from . import functional as SF
@@ -294,12 +324,60 @@ class DistillationLoss(nn.Module):
         if teacher_logits is None:
             loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1)
             return loss
-        if teacher_logits.shape != logits.shape or teacher_logits.dtype != torch.float32 or \
-                teacher_logits.device != logits.device:
-            raise ValueError("DistillationLoss: teacher_logits must be fp32 %s on %s like the logits, got %s %s on %s" %
-                             (tuple(logits.shape), logits.device, teacher_logits.dtype, tuple(teacher_logits.shape),
-                              teacher_logits.device))
-        t = teacher_logits.detach().permute(0, 2, 3, 1).contiguous()
+        t = self._teacher_logits_nhwc(logits, teacher_logits)
+        loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self, teacher_logits=t)
+        return loss
+
+
+class PseudoLabelLoss(_TeacherLoss):
+    """Confidence-masked pseudo-label cross-entropy from a teacher network (the self-training loss of FixMatch-style
+    segmentation, UniMatch and U2PL), plus cross-entropy on the labelled pixels. With s, t the student and teacher
+    logits after the same bilinear xZ upsample (align_corners) that the CE term uses, per output pixel:
+
+        L    = {target in [0, C), target != ignore_index}       labelled pixels
+        U    = {target == ignore_index}                          unlabelled pixels (an unlabelled image: all ignore)
+        yhat = argmax_c t_c (first maximum, as torch.argmax),    conf = softmax(t)_yhat = 1 / sum_c exp(t_c - t_yhat)
+        main = ce_weight (1/|L|) sum_L (lse(s) - s_target) + pl_weight (1/|U|) sum_{U, conf >= threshold} (lse(s) - s_yhat)
+        aux  = plain CE of the aux head on L (ce_weight does not scale it)
+
+    The pseudo-label term is averaged over |U|, every unlabelled pixel, not over the confident ones: UniMatch's
+    normalisation, so that a teacher that grows more confident does not change the weight of each pixel. A term whose set
+    is empty is 0 with an exactly zero gradient; a target outside [0, C) that is not ignore_index belongs to neither set.
+    threshold 0 (or below) trains on every unlabelled pixel, a threshold above 1 on none. The mask and yhat are
+    constants: no gradient flows through the teacher. Under DistributedDataParallel each rank averages over its own
+    pixels.
+
+    `teacher` is a frozen PSPNet or PSANet of this package or the `module` of an optim.ModelEMA (a mean teacher), with
+    the rules of _TeacherLoss. It sees the student's input batch.
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, teacher forward included,
+    graphed at every zoom factor. Called as a module, forward(logits, target, teacher_logits=None) takes NCHW logits at the
+    target size: without teacher_logits it returns the mean cross-entropy over L (the validation loss validate() logs),
+    with them (the same shape) `main` computed at that size. CUDA fp32 logits with at most 256 classes only: there is no
+    CPU or library fallback."""
+
+    def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255):
+        super(PseudoLabelLoss, self).__init__(teacher, ignore_index)
+        if isinstance(threshold, bool) or not isinstance(threshold, (int, float)):
+            raise TypeError("threshold must be a number, got %r" % (threshold,))
+        if not math.isfinite(threshold):
+            raise ValueError("threshold must be finite, got %r" % threshold)
+        self.threshold = float(threshold)
+        self.pl_weight = _non_negative("pl_weight", pl_weight)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+
+    def extra_repr(self):
+        return "teacher=%s, threshold=%g, pl_weight=%g, ce_weight=%g, ignore_index=%d" % (
+            type(self.teacher).__name__, self.threshold, self.pl_weight, self.ce_weight, self.ignore_index)
+
+    def forward(self, logits, target, teacher_logits=None):
+        from . import functional as SF
+        _check_native_logits("PseudoLabelLoss", logits, target)
+        s = logits.permute(0, 2, 3, 1).contiguous()
+        if teacher_logits is None:
+            loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1)
+            return loss
+        t = self._teacher_logits_nhwc(logits, teacher_logits)
         loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self, teacher_logits=t)
         return loss
 

@@ -977,6 +977,43 @@ def upsample_kd_bwd(student, teacher, temperature, kd_weight, lse, grad_out, dlo
     return dlogits
 
 
+def upsample_pl_fwd(student, teacher, target, ignore_index, threshold, pl_weight, ce_weight, want_argmax=True,
+                    zoom=8):
+    """Confidence-masked pseudo-label cross-entropy on the fused tail (include/semseg_b200.h states the contract):
+    student / teacher fp32 NHWC [N,h,w,C] maps (each with its own pixel pitch), target int64 [N,Ho,Wo] ->
+    (loss_info [6] = (CE mean over L, |L|, PL sum / |U|, |U|, 0, 1), argmax, lse, effective target int64 [N,Ho,Wo],
+    weight fp32 [N,Ho,Wo]). The backward is upsample_ce_focal_bwd(student, eff, -1, lse, weight, loss_info[4:], ...)."""
+    _require_cuda(student, teacher, target)
+    lib = _lib.load()
+    n, h, w, c, ps = _kd_map_meta(student)
+    shape_t = _kd_map_meta(teacher)
+    assert shape_t[:4] == (n, h, w, c), "student and teacher maps differ in shape"
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_pl_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_pl_workspace_floats")
+    dev = student.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((6,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    eff = torch.empty((n, ho, wo), dtype=torch.int64, device=dev)
+    lse, wt = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
+    _lib.check(lib.semseg_upsample_pl_fwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c, _ptr(target), ho,
+                                          wo, int(zoom), int(ignore_index), float(threshold), float(pl_weight),
+                                          float(ce_weight), _ptr(ws), _ptr(info), _ptr(amax), _ptr(lse), _ptr(eff),
+                                          _ptr(wt), _stream()),
+               "semseg_upsample_pl_fwd")
+    return info, amax, lse, eff, wt
+
+
+def ema_multi(items_dev, n_items, n_chunks, decay):
+    """shadow <- lerp(shadow, source, 1 - decay) for every fp32 item, int64 items copied, in one launch
+    (include/semseg_b200.h semseg_ema_multi); `items_dev` is a device uint8 tensor holding the item table."""
+    lib = _lib.load()
+    _lib.check(lib.semseg_ema_multi(_ptr(items_dev), int(n_items), int(n_chunks), float(decay), _stream()),
+               "semseg_ema_multi")
+
+
 def segsort_u32_pairs(keys, vals, skip=None):
     """Stable sort of each row of the int32 [S, L] CUDA tensors `keys` / `vals` (uint32 bit patterns) by key, in place;
     rows whose int32 `skip` [S] entry is non-zero are left untouched."""

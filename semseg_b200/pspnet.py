@@ -138,8 +138,9 @@ class _SegNet(nn.Module):
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
         t_logits = None
-        if self.training and y is not None and isinstance(self.criterion, losses.DistillationLoss):
-            # the frozen teacher first: its activations are transient before the student's saved ones exist
+        if self.training and y is not None and isinstance(self.criterion, losses._TeacherLoss):
+            # the teacher first (distillation, pseudo-labels): its activations are transient before the student's saved
+            # ones exist
             t_logits = self.criterion.run_teacher(x, self.cls[4].out_channels)
         logits, t_aux = self._logits_nhwc(x)
 
