@@ -589,6 +589,44 @@ int semseg_upsample_pl_fwd(const float* student, int pitch_s, const float* teach
                            int C, const int64_t* target, int Ho, int Wo, int zoom, int ignore_index, float threshold,
                            float pl_weight, float ce_weight, float* workspace, float* loss_out, int64_t* argmax,
                            float* lse, int64_t* eff_target, float* weight, void* stream);
+/* The mixed form (CutMix / ClassMix, semseg_b200/losses.py MixPseudoLabelLoss): semseg_upsample_pl_fwd with the teacher
+ * of each output pixel (n, i, j) taken from image n's map or its partner (n + 1) mod N's, as mix_mask uint8
+ * [N, 8(h-1)+1, 8(w-1)+1] (semseg_mix_apply's mask on the input grid) says at input pixel (i 8/zoom, j 8/zoom). Per
+ * pixel, yhat and conf are the bits semseg_upsample_pl_fwd computes for that teacher image; target is the mixed target.
+ * The same workspace, outputs, backward and checks, and a null mask is rejected. */
+int semseg_upsample_pl_mix_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h,
+                               int w, int C, const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                               float threshold, float pl_weight, float ce_weight, const uint8_t* mix_mask,
+                               float* workspace, float* loss_out, int64_t* argmax, float* lse, int64_t* eff_target,
+                               float* weight, void* stream);
+/* Mixed-sample masks and batches (csrc/mix.cu) for mean-teacher training. Image n is mixed with its partner
+ * pi(n) = (n + 1) mod N; uniforms fp32 [N, ustride] hold u0 (apply), u1 (area), u2 (ratio), u3 (row), u4 (column) and,
+ * for ClassMix, class priorities u[n, 5 + c]; image n is mixed iff (double) u0 < p.
+ *   mix_argmax_x8: teacher fp32 NHWC [N,h,w,C] (pitch >= C, C <= 256) -> argmax uint8 [N, 8(h-1)+1, 8(w-1)+1], the
+ *                  first maximum after the x8 bilinear (align_corners) upsample, bit-equal to semseg_upsample_pl_fwd's
+ *                  yhat at zoom 8; present uint32 [N, 8]: the classes that occur in each image's argmax, as bits.
+ *   mix_select   : selected uint32 [N, 8] = the ceil(k/2) of each image's k present classes with the smallest
+ *                  (u[n, 5 + c], c), lexicographically (ustride >= 5 + C).
+ *   mix_apply    : M (mask uint8 [N,H,W], 1 = from the partner), x_mixed fp32 NCHW [N,Cin,H,W] = M ? x[pi(n)] : x[n],
+ *                  y_mixed int64 [N,Ho,Wo] = y[pi(n)] where M at input pixel (i 8/zoom, j 8/zoom), else y[n]
+ *                  (H-1, W-1 multiples of 8, Ho = zoom(H-1)/8 + 1). M = 0 on an image that is not mixed; else
+ *                  SEMSEG_MIX_CUTMIX: M = 1 on rows [y0, y0+bh) and columns [x0, x0+bw), in fp64 with every operation
+ *                    correctly rounded: a = ((area_lo + (area_hi - area_lo) u1) H) W, rho = ratio_lo + (ratio_hi -
+ *                    ratio_lo) u2, bw = min(W, max(1, floor(sqrt(a / rho)))), bh = min(H, max(1, floor(sqrt(a rho)))),
+ *                    x0 = min(W - bw, floor(u4 (W - bw + 1))), y0 = min(H - bh, floor(u3 (H - bh + 1)));
+ *                  SEMSEG_MIX_CLASSMIX: M = 1 where argmax[pi(n)] is in selected[pi(n)].
+ *                  p in [0, 1], 0 < area_lo <= area_hi <= 1, 0 < ratio_lo <= ratio_hi; the outputs may not alias x, y.
+ * Bad arguments are rejected before any CUDA call. No host synchronisation; deterministic. */
+#define SEMSEG_MIX_CUTMIX 0
+#define SEMSEG_MIX_CLASSMIX 1
+int semseg_mix_argmax_x8(const float* teacher, int pitch, int N, int h, int w, int C, uint8_t* argmax,
+                         uint32_t* present, void* stream);
+int semseg_mix_select(const float* uniforms, int ustride, const uint32_t* present, int N, int C, uint32_t* selected,
+                      void* stream);
+int semseg_mix_apply(int mode, const float* x, int N, int Cin, int H, int W, const int64_t* y, int Ho, int Wo, int zoom,
+                     const float* uniforms, int ustride, double p, double area_lo, double area_hi, double ratio_lo,
+                     double ratio_hi, const uint8_t* argmax, const uint32_t* selected, uint8_t* mask,
+                     float* x_mixed, int64_t* y_mixed, void* stream);
 /* Segmented stable radix sort (csrc/segsort.cu): S segments of L (uint32 key, uint32 payload) pairs, [S][L], each sorted
  * in place by key ascending, equal keys in input order. keys_alt / vals_alt: scratch of the same size. skip: NULL, or
  * int [S] on the device, a non-zero entry leaves that segment untouched. workspace:

@@ -229,6 +229,14 @@ SIGNATURES = {
     "semseg_upsample_pl_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
     "semseg_upsample_pl_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                        c_int, c_f, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_pl_mix_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,
+                                           c_int, c_int, c_f, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                           c_vp]),
+    "semseg_mix_argmax_x8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
+    "semseg_mix_select": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_vp, c_vp]),
+    "semseg_mix_apply": (c_int, [c_int, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp, c_int,
+                                 ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
+                                 c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_segsort_u32_pairs_workspace_bytes": (c_ll, [c_int, c_ll]),
     "semseg_segsort_u32_pairs": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_ll, c_vp, c_vp, c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),

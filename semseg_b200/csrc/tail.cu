@@ -1827,16 +1827,23 @@ upsample_pl_count_kernel(const long long* __restrict__ target, long long M, int 
   }
 }
 
-template <int Z>
+// kMix (CutMix / ClassMix, losses.MixPseudoLabelLoss): the teacher of an output pixel is image n's map or its partner
+// (n + 1) mod N's, as the uint8 mix mask [N, 8(h-1)+1, 8(w-1)+1] on the input grid says at the pixel's input position
+// (Z i, Z j) * 8/Z (the grids nest under align_corners). The partner's node rows are staged as a third map and each
+// output row picks its teacher with the same operations, so a pixel's (yhat, conf) are the bits the plain instance
+// computes for its teacher image. The mask argument comes last: the kMix = false instances keep their parameter layout.
+template <int Z, bool kMix = false>
 __global__ void __launch_bounds__(KdGeom<Z>::kCols)
 upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* __restrict__ tl, int pitch_t, int N, int h,
                        int w, int C, int Cs, const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                        float threshold, float pl_weight, float ce_weight, const unsigned long long* __restrict__ counts,
                        float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out,
-                       long long* __restrict__ eff_out, float* __restrict__ wt_out) {
+                       long long* __restrict__ eff_out, float* __restrict__ wt_out,
+                       const unsigned char* __restrict__ mix_mask = nullptr) {
   using G = Zoom<Z>;
   constexpr int kCols = KdGeom<Z>::kCols, kNodes = KdGeom<Z>::kNodes;
-  extern __shared__ float S[];  // [2 maps: student, teacher][kNodeRows][kNodes][Cs], as upsample_kd_fwd_kernel
+  constexpr int kMaps = kMix ? 3 : 2;
+  extern __shared__ float S[];  // [kMaps: student, teacher, partner's teacher][kNodeRows][kNodes][Cs]
   __shared__ float red[4][kCols / 32];
   const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kCols;
   const int i1 = min(i0 + 1, h - 1);
@@ -1844,11 +1851,12 @@ upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* _
   const int nj = min(kNodes, w - j_base);
   const int tid = threadIdx.x;
   const int map_floats = G::kNodeRows * kNodes * Cs;
-  for (int idx = tid; idx < 2 * G::kNodeRows * nj * C; idx += kCols) {
+  const int pn = kMix ? (n + 1 == N ? 0 : n + 1) : n;
+  for (int idx = tid; idx < kMaps * G::kNodeRows * nj * C; idx += kCols) {
     const int c = idx % C;
     const int node = idx / C;
     const int jj = node % nj, rr = (node / nj) % G::kNodeRows, map = node / (nj * G::kNodeRows);
-    const size_t src = (static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj);
+    const size_t src = (static_cast<size_t>(kMix && map == 2 ? pn : n) * h + (rr ? i1 : i0)) * w + (j_base + jj);
     S[map * map_floats + (rr * kNodes + jj) * Cs + c] = map ? tl[src * pitch_t + c] : sl[src * pitch_s + c];
   }
   __syncthreads();
@@ -1867,6 +1875,19 @@ upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* _
     const float* Bt = B + map_floats;
     const float* Ct = Cc + map_floats;
     const float* Dt = D + map_floats;
+    const float* Ap = At + map_floats;         // kMix: the partner's teacher nodes
+    const float* Bp = Bt + map_floats;
+    const float* Cp = Ct + map_floats;
+    const float* Dp = Dt + map_floats;
+    unsigned sel = 0;                          // kMix: bit r set -> output row r takes the partner's teacher
+    if constexpr (kMix) {
+      const int H = 8 * (h - 1) + 1, W = 8 * (w - 1) + 1;
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        if (r < rows && mix_mask[(static_cast<size_t>(n) * H + (Z * i0 + r) * (8 / Z)) * W + x * (8 / Z)])
+          sel |= 1u << r;
+      }
+    }
     float ms[Z], mt[Z], zs[Z], zt[Z];
     int as[Z], at[Z];
 #pragma unroll
@@ -1881,6 +1902,11 @@ upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* _
       const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
       const float topt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
       const float bott = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+      float topp = 0.f, botp = 0.f;
+      if constexpr (kMix) {
+        topp = Z == 1 ? Ap[c] : l0w * Ap[c] + l1w * Bp[c];
+        botp = Z == 1 ? 0.f : l0w * Cp[c] + l1w * Dp[c];
+      }
 #pragma unroll
       for (int r = 0; r < Z; ++r) {
         const float v = row_lerp<Z>(top, bot, r);
@@ -1888,7 +1914,7 @@ upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* _
           ms[r] = v;
           as[r] = c;
         }
-        const float u = row_lerp<Z>(topt, bott, r);
+        const float u = kMix && ((sel >> r) & 1u) ? row_lerp<Z>(topp, botp, r) : row_lerp<Z>(topt, bott, r);
         if (u > mt[r]) {
           mt[r] = u;
           at[r] = c;
@@ -1904,10 +1930,16 @@ upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* _
       const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
       const float topt = Z == 1 ? At[c] : l0w * At[c] + l1w * Bt[c];
       const float bott = Z == 1 ? 0.f : l0w * Ct[c] + l1w * Dt[c];
+      float topp = 0.f, botp = 0.f;
+      if constexpr (kMix) {
+        topp = Z == 1 ? Ap[c] : l0w * Ap[c] + l1w * Bp[c];
+        botp = Z == 1 ? 0.f : l0w * Cp[c] + l1w * Dp[c];
+      }
 #pragma unroll
       for (int r = 0; r < Z; ++r) {
         zs[r] += ex2_approx(fmaf(row_lerp<Z>(top, bot, r), kLog2e, -m2[r]));   // the plain forward's sum
-        zt[r] += ex2_approx((row_lerp<Z>(topt, bott, r) - mt[r]) * kLog2e);    // yhat's term is exactly 1
+        const float u = kMix && ((sel >> r) & 1u) ? row_lerp<Z>(topp, botp, r) : row_lerp<Z>(topt, bott, r);
+        zt[r] += ex2_approx((u - mt[r]) * kLog2e);                               // yhat's term is exactly 1
       }
     }
     const unsigned long long nl = counts[0], nu = counts[1];
@@ -2906,11 +2938,12 @@ static int check_pl(const float* student, int pitch_s, const float* teacher, int
   return SEMSEG_OK;
 }
 
-template <int Z>
+template <int Z, bool kMix = false>
 static int launch_pl_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
                          int C, const int64_t* target, int Ho, int Wo, int ignore_index, float threshold,
                          float pl_weight, float ce_weight, float* workspace, float* loss_out, int64_t* argmax,
-                         float* lse, int64_t* eff, float* wt, cudaStream_t stream) {
+                         float* lse, int64_t* eff, float* wt, cudaStream_t stream,
+                         const uint8_t* mix_mask = nullptr) {
   using K = KdGeom<Z>;
   unsigned long long* counts = reinterpret_cast<unsigned long long*>(workspace);
   float* partial = workspace + 4;
@@ -2922,17 +2955,18 @@ static int launch_pl_fwd(const float* student, int pitch_s, const float* teacher
                                                            ignore_index, counts, loss_out);
   SB_LAUNCHED();
   const int Cs = C | 1;
-  constexpr size_t kMaxSmem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * (kMaxClasses | 1) * sizeof(float);
-  const size_t smem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * Cs * sizeof(float);
+  constexpr unsigned long long kMaps = kMix ? 3 : 2;    // kMix: the partner's teacher rows as a third map
+  constexpr size_t kMaxSmem = kMaps * Zoom<Z>::kNodeRows * K::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = kMaps * Zoom<Z>::kNodeRows * K::kNodes * Cs * sizeof(float);
   static std::atomic<bool> attr_set[64];
   if (smem > kSmemDefault) {
-    int r = opt_in_smem(upsample_pl_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    int r = opt_in_smem(upsample_pl_fwd_kernel<Z, kMix>, attr_set, static_cast<int>(kMaxSmem));
     if (r) return r;
   }
-  upsample_pl_fwd_kernel<Z><<<dim3(cdiv(Wo, K::kCols), h, N), K::kCols, smem, stream>>>(
+  upsample_pl_fwd_kernel<Z, kMix><<<dim3(cdiv(Wo, K::kCols), h, N), K::kCols, smem, stream>>>(
       student, pitch_s, teacher, pitch_t, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo,
       ignore_index, threshold, pl_weight, ce_weight, counts, partial, reinterpret_cast<long long*>(argmax), lse,
-      reinterpret_cast<long long*>(eff), wt);
+      reinterpret_cast<long long*>(eff), wt, mix_mask);
   SB_LAUNCHED();
   upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(partial, ctas, loss_out);
   SB_LAUNCHED();
@@ -2971,6 +3005,36 @@ extern "C" int semseg_upsample_pl_fwd(const float* student, int pitch_s, const f
     default: return launch_pl_fwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
                                      threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
                                      weight, stream);
+  }
+}
+
+// The mixed form (CutMix / ClassMix): semseg_upsample_pl_fwd with each output pixel's teacher taken from image n or its
+// partner (n + 1) mod N by the input-grid mix mask; the same workspace.
+extern "C" int semseg_upsample_pl_mix_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N,
+                                          int h, int w, int C, const int64_t* target, int Ho, int Wo, int zoom,
+                                          int ignore_index, float threshold, float pl_weight, float ce_weight,
+                                          const uint8_t* mix_mask, float* workspace, float* loss_out, int64_t* argmax,
+                                          float* lse, int64_t* eff_target, float* weight, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_pl(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, zoom, threshold, pl_weight,
+                   ce_weight);
+  if (r) return r;
+  SB_CHECK_ARG(mix_mask, "upsample_pl_mix_fwd: null mix mask");
+  SB_CHECK_ARG(workspace && loss_out && lse && eff_target && weight, "upsample_pl_mix_fwd: null output");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "upsample_pl_mix_fwd: workspace not 8-byte aligned");
+  switch (zoom) {
+    case 1: return launch_pl_fwd<1, true>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                          threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                          weight, stream, mix_mask);
+    case 2: return launch_pl_fwd<2, true>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                          threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                          weight, stream, mix_mask);
+    case 4: return launch_pl_fwd<4, true>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo, ignore_index,
+                                          threshold, pl_weight, ce_weight, workspace, loss_out, argmax, lse, eff_target,
+                                          weight, stream, mix_mask);
+    default: return launch_pl_fwd<8, true>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo,
+                                           ignore_index, threshold, pl_weight, ce_weight, workspace, loss_out, argmax,
+                                           lse, eff_target, weight, stream, mix_mask);
   }
 }
 

@@ -690,6 +690,25 @@ class _UpsampleCEPL(torch.autograd.Function):
         return dl, None, None, None, None, None, None, None
 
 
+class _UpsampleCEPLMix(_UpsampleCEPL):
+    """The fused tail with losses.MixPseudoLabelLoss: _UpsampleCEPL on the mixed target, each output pixel's teacher
+    image n or its partner (n + 1) mod N as the input-grid mix mask says (ops.upsample_pl_fwd's mixed form). The
+    backward is _UpsampleCEPL's, on the effective targets and weights."""
+
+    @staticmethod
+    def forward(ctx, logits, teacher_logits, target, ignore_index, zoom, threshold, pl_weight, ce_weight, mix_mask):
+        info, amax, lse, eff, wt = ops.upsample_pl_fwd(logits, teacher_logits, target, ignore_index, threshold,
+                                                       pl_weight, ce_weight, zoom=zoom, mix_mask=mix_mask)
+        ctx.save_for_backward(logits, eff, lse, wt, info)
+        ctx.zoom = zoom
+        ctx.mark_non_differentiable(amax)
+        return torch.add(info[0] * ce_weight, info[2], alpha=pl_weight), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, grad_amax):
+        return _UpsampleCEPL.backward(ctx, grad_loss, grad_amax) + (None,)
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""
@@ -712,7 +731,8 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     contiguous fp32 [classes] tensor on that device; any other weight, another reduction, and any subclass keep the
     ATen tail. DiceLoss, FocalLoss and losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
-    form's conditions; losses.PseudoLabelLoss, whose backward is the focal one, the Dice width limit.
+    form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, the Dice
+    width limit.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
         ok = True
@@ -721,7 +741,7 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         plain = criterion.weight is None and eps == 0.0
         ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
               (plain or (target is not None and target.is_cuda)))
-    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss, losses.PseudoLabelLoss):
+    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss, losses.PseudoLabelLoss, losses.MixPseudoLabelLoss):
         # the focal rows kernel (the pseudo-label backward too) stages the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
@@ -747,7 +767,7 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     return target.shape[1] == zoom_factor * (h - 1) + 1 and target.shape[2] == zoom_factor * (w - 1) + 1
 
 
-def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_logits=None):
+def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_logits=None, mix_mask=None):
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
     weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
@@ -755,7 +775,13 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     Lovász-Softmax (+ CE) loss; with a losses.FocalLoss, its focal loss (its own ignore_index, gamma and class
     weights); with a losses.DistillationLoss and the teacher's fp32 NHWC logits `teacher_logits`
     (the student's shape), its distillation loss, and with a losses.PseudoLabelLoss and them its pseudo-label loss
-    (without them: the plain mean CE, the loss of the aux head). The default criterion runs the plain kernels."""
+    (without them: the plain mean CE, the loss of the aux head). With a losses.MixPseudoLabelLoss, the teacher's logits
+    of the unmixed batch and the mix mask `mix_mask` (ops.mix_apply's), the mixed pseudo-label loss on the mixed target;
+    without the mask it is a losses.PseudoLabelLoss. The default criterion runs the plain kernels."""
+    if type(criterion) is losses.MixPseudoLabelLoss and teacher_logits is not None and mix_mask is not None:
+        return _UpsampleCEPLMix.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
+                                      int(zoom), criterion.threshold, criterion.pl_weight, criterion.ce_weight,
+                                      mix_mask)
     if isinstance(criterion, losses.DistillationLoss) and teacher_logits is not None:
         kd_zoom = 1 if criterion.at == 'logits' else int(zoom)
         return _UpsampleCEKD.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,

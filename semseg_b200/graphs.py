@@ -20,7 +20,7 @@ overwrites the first one's saved activations — gradient accumulation over seve
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
 loss, the focal loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
-mean teacher's re-pack included) are not captured (such models simply stay eager).
+mean teacher's re-pack included, and the CutMix / ClassMix pseudo-label loss, its draws and mixing included) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -61,10 +61,12 @@ def note_boundary(t):
 
 class _Step:
     __slots__ = ("key", "calls", "failed", "fwd", "bwd", "bwd2", "x", "y", "pred", "main", "aux", "g_main", "g_aux",
-                 "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot")
+                 "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot", "mix",
+                 "mix_crit")
 
     def __init__(self, key):
         self.key, self.calls, self.failed, self.fwd, self.dx_slot = key, 0, False, None, False
+        self.mix = self.mix_crit = None
 
 
 def _set_grad_outputs(st, g_main, g_aux):
@@ -108,6 +110,7 @@ class _Replay(torch.autograd.Function):
         st.x.copy_(x, non_blocking=True)
         st.y.copy_(y, non_blocking=True)
         st.fwd.replay()
+        _point_mix(st)
         ctx.st = st
         pred, main, aux = st.pred.detach(), st.main.detach(), st.aux.detach()
         ctx.mark_non_differentiable(pred)
@@ -119,6 +122,13 @@ class _Replay(torch.autograd.Function):
         _set_grad_outputs(st, g_main, g_aux)
         st.bwd.replay()
         return _with_dx(st, _fresh(st.grads))
+
+
+def _point_mix(st):
+    """A losses.MixPseudoLabelLoss criterion's last_mix() is the replayed step's: its mask, mixed target and uniforms
+    are that step's static tensors (each captured input shape has its own)."""
+    if st.mix_crit is not None:
+        st.mix_crit._mix_state = st.mix
 
 
 def _with_dx(st, gs):
@@ -138,6 +148,7 @@ class _ReplayHead(torch.autograd.Function):
         st.x.copy_(x, non_blocking=True)
         st.y.copy_(y, non_blocking=True)
         st.fwd.replay()
+        _point_mix(st)
         ctx.st = st
         return st.t_mid.detach()
 
@@ -248,6 +259,10 @@ def _capture(model, impl, st, x, y):
         for mod, name, prm in slots:
             mod._parameters[name] = prm
     st.launches = _lib.launch_count() - l0          # native kernels per replayed step (forward + backward graphs)
+    crit = getattr(model, "criterion", None)
+    if getattr(crit, "_mix_state", None) is not None:
+        # the mix the captured forward wrote: static tensors of the graph's pool, refreshed by every replay
+        st.mix, st.mix_crit = crit._mix_state, crit
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
     del proxies, x_in, x_leaf
@@ -307,7 +322,8 @@ def train_step(model, impl, x, y):
             tkey = lambda ts: tuple((t.data_ptr(), t._version) for t in ts)            # noqa: E731
         crit_key += (id(teacher), tkey(teacher.parameters()), tkey(teacher.buffers()),
                      tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
-        crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight"))
+        crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight",
+                                                             "mix", "p", "area", "ratio"))
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
            dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad,
            crit_key)

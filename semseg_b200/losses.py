@@ -8,7 +8,8 @@ LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and Foc
 optional class weights, run the same way. DistillationLoss adds a
 pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
-optim.ModelEMA.
+optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
+batch, the student learns on the mixed one.
 """
 import math
 
@@ -380,6 +381,106 @@ class PseudoLabelLoss(_TeacherLoss):
         t = self._teacher_logits_nhwc(logits, teacher_logits)
         loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self, teacher_logits=t)
         return loss
+
+
+def _range_pair(name, v, upper):
+    if not isinstance(v, (tuple, list)) or len(v) != 2 or \
+            any(isinstance(a, bool) or not isinstance(a, (int, float)) for a in v):
+        raise TypeError("%s must be a pair of numbers (lo, hi), got %r" % (name, v))
+    lo, hi = float(v[0]), float(v[1])
+    if not (math.isfinite(lo) and math.isfinite(hi) and 0.0 < lo <= hi <= upper):
+        raise ValueError("%s must satisfy 0 < lo <= hi%s, got %r" % (name, " <= %g" % upper if upper < math.inf else "",
+                                                                    v))
+    return lo, hi
+
+
+class MixPseudoLabelLoss(PseudoLabelLoss):
+    """PseudoLabelLoss with mixed-sample perturbation: CutMix (French et al., BMVC 2020, the CutMix-Seg recipe; the box
+    of UniMatch) or ClassMix (Olsson et al., WACV 2021; DACS). The teacher labels the clean batch, the student learns
+    those labels, mixed the same way, on the mixed batch. Per training forward of a PSPNet / PSANet with this criterion,
+    with input x [N,3,H,W] and target y [N,Ho,Wo]:
+
+        u    = torch.rand(N, 5 [+ C for ClassMix]) on the device's default CUDA generator, before the teacher forward
+               (graph-safe like Dropout2d: seeded runs reproduce, a graphed step equals the eager one); image n is mixed
+               iff u[n, 0] < p, with its partner pi(n) = (n + 1) mod N (N = 1: itself, so mixing changes nothing)
+        M    = the mask on the input grid, 1 where a pixel comes from the partner:
+               'cutmix'  : one box per mixed image, area (area_lo + (area_hi - area_lo) u1) H W and aspect ratio
+                           ratio_lo + (ratio_hi - ratio_lo) u2, placed by u3 (row) and u4 (column); computed in fp64
+                           as include/semseg_b200.h semseg_mix_apply states (UniMatch's box without its retry loop)
+               'classmix': A[m] = the teacher's argmax of image m after the x8 upsample to the input grid; the ceil(k/2)
+                           of its k present classes with the smallest (u[m, 5 + c], c) are pasted: M(n) = 1 where
+                           A[pi(n)] is one of them (at most 256 classes)
+        x_m  = M ? x[pi(n)] : x[n]                        y_m = the same mix of y at the target pixels' input positions
+        main = PseudoLabelLoss's main of (student(x_m), y_m), each pixel's pseudo-label and confidence from the teacher
+               of its source image (the teacher runs on the unmixed x)
+        aux  = plain CE of the aux head on y_m;  pred = the student's argmax on x_m
+
+    `p` in [0, 1] (UniMatch: 0.5), `area` = (lo, hi) with 0 < lo <= hi <= 1, `ratio` = (lo, hi) with 0 < lo <= hi; the
+    other arguments and the teacher's rules are PseudoLabelLoss's. Labelled and unlabelled images share the batch: an
+    unlabelled image has an all-ignore_index target, and the mixed target carries each pixel's own label or ignore.
+
+    `last_mix()` returns {'mask': uint8 [N,H,W], 'target': y_m, 'uniforms': u} of the latest training forward, graphed
+    or eager, as views that stay valid until the next forward. The trainer's logged training mIoU compares `pred` with
+    the unmixed target; score against last_mix()['target'] instead. There is no gradient through the mixing: an input
+    with requires_grad raises. Called as a module, forward(logits, target, teacher_logits=None) is PseudoLabelLoss's.
+
+    With the network's fused tail the mixing, the mixed pseudo-label loss and the teacher forward run on native kernels
+    (csrc/mix.cu and csrc/tail.cu), graphed at every zoom factor; where the fused tail does not apply (a target wider
+    than its kernels stage), the mixing stays native and the teacher's upsampled maps are mixed with torch.where. Under
+    DistributedDataParallel each rank mixes its own batch (multi-GPU runs have not been made)."""
+
+    def __init__(self, teacher, mix='cutmix', p=0.5, area=(0.02, 0.4), ratio=(0.3, 1 / 0.3), threshold=0.95,
+                 pl_weight=1.0, ce_weight=1.0, ignore_index=255):
+        super(MixPseudoLabelLoss, self).__init__(teacher, threshold, pl_weight, ce_weight, ignore_index)
+        if not isinstance(mix, str):
+            raise TypeError("mix must be 'cutmix' or 'classmix', got %r" % (mix,))
+        if mix not in ('cutmix', 'classmix'):
+            raise ValueError("mix must be 'cutmix' or 'classmix', got %r" % (mix,))
+        p = _non_negative("p", p)
+        if p > 1.0:
+            raise ValueError("p must lie in [0, 1], got %r" % p)
+        self.mix = mix
+        self.p = p
+        self.area = _range_pair("area", area, 1.0)
+        self.ratio = _range_pair("ratio", ratio, math.inf)
+        self._mix_state = None
+
+    def extra_repr(self):
+        return "teacher=%s, mix=%r, p=%g, area=(%g, %g), ratio=(%g, %g), threshold=%g, pl_weight=%g, ce_weight=%g, " \
+               "ignore_index=%d" % (type(self.teacher).__name__, self.mix, self.p, self.area[0], self.area[1],
+                                    self.ratio[0], self.ratio[1], self.threshold, self.pl_weight, self.ce_weight,
+                                    self.ignore_index)
+
+    def last_mix(self):
+        """{'mask', 'target', 'uniforms'} of the latest training forward (None before the first one)."""
+        return None if self._mix_state is None else dict(self._mix_state)
+
+    def draw(self, x, classes):
+        """The forward's uniforms, drawn before the teacher runs: [N, 5] (CutMix) or [N, 5 + classes] (ClassMix)."""
+        name = type(self).__name__
+        if x.requires_grad:
+            raise RuntimeError("%s: there is no gradient through the mixing; the input must not require grad" % name)
+        if not x.is_cuda or x.dtype != torch.float32 or x.dim() != 4:
+            raise TypeError("%s: the input must be a CUDA fp32 [N, C, H, W] tensor, got %s %s on %s" %
+                            (name, x.dtype, tuple(x.shape), x.device))
+        if self.mix == 'classmix' and classes > 256:
+            raise ValueError("%s: ClassMix needs at most 256 classes, got %d" % (name, classes))
+        return torch.rand((x.shape[0], 5 + (classes if self.mix == 'classmix' else 0)), device=x.device)
+
+    def mix_batch(self, x, y, u, t_logits, zoom):
+        """(x_m, y_m, mask) from the input, target, `draw`'s uniforms and the teacher's NHWC logits of the unmixed
+        input; remembered for last_mix()."""
+        from . import ops
+        if y.dtype != torch.int64:
+            raise TypeError("%s: int64 target expected, got %s" % (type(self).__name__, y.dtype))
+        amap = sel = None
+        if self.mix == 'classmix':
+            amap, present = ops.mix_argmax_x8(t_logits)
+            sel = ops.mix_select(u, present, t_logits.shape[-1])
+        mask, xm, ym = ops.mix_apply(self.mix, x.contiguous(), y.contiguous(), u, self.p, self.area, self.ratio,
+                                     zoom, amap, sel)
+        self._mix_state = {'mask': mask, 'target': ym, 'uniforms': u}
+        return xm, ym, mask
 
 
 class LovaszSoftmaxLoss(nn.Module):

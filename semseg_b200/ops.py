@@ -978,12 +978,14 @@ def upsample_kd_bwd(student, teacher, temperature, kd_weight, lse, grad_out, dlo
 
 
 def upsample_pl_fwd(student, teacher, target, ignore_index, threshold, pl_weight, ce_weight, want_argmax=True,
-                    zoom=8):
+                    zoom=8, mix_mask=None):
     """Confidence-masked pseudo-label cross-entropy on the fused tail (include/semseg_b200.h states the contract):
     student / teacher fp32 NHWC [N,h,w,C] maps (each with its own pixel pitch), target int64 [N,Ho,Wo] ->
     (loss_info [6] = (CE mean over L, |L|, PL sum / |U|, |U|, 0, 1), argmax, lse, effective target int64 [N,Ho,Wo],
-    weight fp32 [N,Ho,Wo]). The backward is upsample_ce_focal_bwd(student, eff, -1, lse, weight, loss_info[4:], ...)."""
-    _require_cuda(student, teacher, target)
+    weight fp32 [N,Ho,Wo]). The backward is upsample_ce_focal_bwd(student, eff, -1, lse, weight, loss_info[4:], ...).
+    mix_mask (uint8 [N, 8(h-1)+1, 8(w-1)+1], mix_apply's mask): the mixed form, each pixel's teacher image n or
+    (n + 1) mod N as the mask says (semseg_upsample_pl_mix_fwd)."""
+    _require_cuda(student, teacher, target, mix_mask)
     lib = _lib.load()
     n, h, w, c, ps = _kd_map_meta(student)
     shape_t = _kd_map_meta(teacher)
@@ -998,12 +1000,78 @@ def upsample_pl_fwd(student, teacher, target, ignore_index, threshold, pl_weight
     amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
     eff = torch.empty((n, ho, wo), dtype=torch.int64, device=dev)
     lse, wt = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
-    _lib.check(lib.semseg_upsample_pl_fwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c, _ptr(target), ho,
-                                          wo, int(zoom), int(ignore_index), float(threshold), float(pl_weight),
-                                          float(ce_weight), _ptr(ws), _ptr(info), _ptr(amax), _ptr(lse), _ptr(eff),
-                                          _ptr(wt), _stream()),
-               "semseg_upsample_pl_fwd")
+    if mix_mask is None:
+        _lib.check(lib.semseg_upsample_pl_fwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c, _ptr(target),
+                                              ho, wo, int(zoom), int(ignore_index), float(threshold), float(pl_weight),
+                                              float(ce_weight), _ptr(ws), _ptr(info), _ptr(amax), _ptr(lse), _ptr(eff),
+                                              _ptr(wt), _stream()),
+                   "semseg_upsample_pl_fwd")
+    else:
+        assert mix_mask.dtype == torch.uint8 and mix_mask.is_contiguous()
+        assert tuple(mix_mask.shape) == (n, 8 * (h - 1) + 1, 8 * (w - 1) + 1), "mix mask is not on the input grid"
+        _lib.check(lib.semseg_upsample_pl_mix_fwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c,
+                                                  _ptr(target), ho, wo, int(zoom), int(ignore_index), float(threshold),
+                                                  float(pl_weight), float(ce_weight), _ptr(mix_mask), _ptr(ws),
+                                                  _ptr(info), _ptr(amax), _ptr(lse), _ptr(eff), _ptr(wt), _stream()),
+                   "semseg_upsample_pl_mix_fwd")
     return info, amax, lse, eff, wt
+
+
+MIX_MODES = {'cutmix': 0, 'classmix': 1}      # SEMSEG_MIX_CUTMIX, SEMSEG_MIX_CLASSMIX
+
+
+def mix_argmax_x8(teacher):
+    """The teacher's argmax after the x8 bilinear (align_corners) upsample (include/semseg_b200.h
+    semseg_mix_argmax_x8): fp32 NHWC [N,h,w,C] (padded pitch allowed) -> (argmax uint8 [N, 8(h-1)+1, 8(w-1)+1],
+    present int32 [N, 8]: the classes that occur in each image, as 256 bits)."""
+    _require_cuda(teacher)
+    lib = _lib.load()
+    n, h, w, c, pitch = _kd_map_meta(teacher)
+    amap = torch.empty((n, 8 * (h - 1) + 1, 8 * (w - 1) + 1), dtype=torch.uint8, device=teacher.device)
+    present = torch.empty((n, 8), dtype=torch.int32, device=teacher.device)
+    _lib.check(lib.semseg_mix_argmax_x8(_ptr(teacher), pitch, n, h, w, c, _ptr(amap), _ptr(present), _stream()),
+               "semseg_mix_argmax_x8")
+    return amap, present
+
+
+def mix_select(uniforms, present, classes):
+    """ClassMix's class sets (semseg_mix_select): uniforms fp32 [N, >= 5 + classes], present int32 [N, 8] -> selected
+    int32 [N, 8], the ceil(k/2) present classes of each image with the smallest (u[n, 5 + c], c), as bits."""
+    _require_cuda(uniforms, present)
+    lib = _lib.load()
+    assert uniforms.dtype == torch.float32 and uniforms.dim() == 2 and uniforms.stride(1) == 1
+    assert present.dtype == torch.int32 and present.is_contiguous() and present.shape == (uniforms.shape[0], 8)
+    sel = torch.empty_like(present)
+    _lib.check(lib.semseg_mix_select(_ptr(uniforms), uniforms.stride(0), _ptr(present), uniforms.shape[0],
+                                     int(classes), _ptr(sel), _stream()),
+               "semseg_mix_select")
+    return sel
+
+
+def mix_apply(mode, x, y, uniforms, p, area, ratio, zoom, amap=None, selected=None):
+    """The mixed batch (semseg_mix_apply): x fp32 NCHW [N,Cin,H,W], y int64 [N,Ho,Wo], uniforms fp32 [N, >= 5] ->
+    (mask uint8 [N,H,W], x_mixed, y_mixed). mode 'cutmix' or 'classmix' (the latter with mix_argmax_x8's argmax and
+    mix_select's selection); p, area = (lo, hi), ratio = (lo, hi) as losses.MixPseudoLabelLoss takes them."""
+    _require_cuda(x, y, uniforms, amap, selected)
+    lib = _lib.load()
+    assert x.dtype == torch.float32 and x.dim() == 4 and x.is_contiguous()
+    assert y.dtype == torch.int64 and y.dim() == 3 and y.is_contiguous()
+    assert uniforms.dtype == torch.float32 and uniforms.dim() == 2 and uniforms.stride(1) == 1
+    n, cin, hh, ww = x.shape
+    assert y.shape[0] == n and uniforms.shape[0] == n, "input, target and uniforms differ in batch size"
+    if mode == 'classmix':
+        assert amap is not None and amap.dtype == torch.uint8 and amap.is_contiguous() and amap.shape == (n, hh, ww)
+        assert selected is not None and selected.dtype == torch.int32 and selected.is_contiguous() and \
+            selected.shape == (n, 8)
+    mask = torch.empty((n, hh, ww), dtype=torch.uint8, device=x.device)
+    xm = torch.empty_like(x)
+    ym = torch.empty_like(y)
+    _lib.check(lib.semseg_mix_apply(MIX_MODES[mode], _ptr(x), n, cin, hh, ww, _ptr(y), y.shape[1], y.shape[2],
+                                    int(zoom), _ptr(uniforms), uniforms.stride(0), float(p), float(area[0]),
+                                    float(area[1]), float(ratio[0]), float(ratio[1]), _ptr(amap), _ptr(selected),
+                                    _ptr(mask), _ptr(xm), _ptr(ym), _stream()),
+               "semseg_mix_apply")
+    return mask, xm, ym
 
 
 def ema_multi(items_dev, n_items, n_chunks, decay):

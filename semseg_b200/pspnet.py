@@ -137,11 +137,16 @@ class _SegNet(nn.Module):
         if self.training and torch.is_grad_enabled():
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
-        t_logits = None
+        t_logits = mix_mask = None
         if self.training and y is not None and isinstance(self.criterion, losses._TeacherLoss):
+            classes = self.cls[4].out_channels
+            mixing = isinstance(self.criterion, losses.MixPseudoLabelLoss)
+            u = self.criterion.draw(x, classes) if mixing else None      # the draws come before the teacher forward
             # the teacher first (distillation, pseudo-labels): its activations are transient before the student's saved
-            # ones exist
-            t_logits = self.criterion.run_teacher(x, self.cls[4].out_channels)
+            # ones exist. It sees the unmixed batch; the student and both heads' losses see the mixed one
+            t_logits = self.criterion.run_teacher(x, classes)
+            if mixing:
+                x, y, mix_mask = self.criterion.mix_batch(x, y, u, t_logits, self.zoom_factor)
         logits, t_aux = self._logits_nhwc(x)
 
         if self.training:
@@ -149,14 +154,19 @@ class _SegNet(nn.Module):
             if SF.fused_tail_supported(self.criterion, logits, y, self.zoom_factor):
                 # upsample + cross-entropy + argmax fused: [N, classes, H, W] never exists (model/pspnet.py:94-103)
                 main_loss, pred = SF.upsample_ce(logits, y, self.criterion.ignore_index, self.zoom_factor,
-                                                 criterion=self.criterion, teacher_logits=t_logits)
+                                                 criterion=self.criterion, teacher_logits=t_logits, mix_mask=mix_mask)
                 aux_loss, _ = SF.upsample_ce(aux_logits, y, self.criterion.ignore_index, self.zoom_factor,
                                              criterion=self.criterion)
                 return pred, main_loss, aux_loss
             x = upsample_logits(logits, (h, w), self.zoom_factor)
             aux = upsample_logits(aux_logits, (h, w), self.zoom_factor)
             if t_logits is not None:
-                main_loss = self.criterion(x, y, teacher_logits=upsample_logits(t_logits, (h, w), self.zoom_factor))
+                t_up = upsample_logits(t_logits, (h, w), self.zoom_factor)
+                if mix_mask is not None:
+                    # each target pixel's teacher map is its source image's: the mask read at the target grid
+                    s = 8 // self.zoom_factor
+                    t_up = torch.where(mix_mask[:, ::s, ::s].unsqueeze(1).bool(), t_up.roll(-1, 0), t_up)
+                main_loss = self.criterion(x, y, teacher_logits=t_up)
             else:
                 main_loss = self.criterion(x, y)
             aux_loss = self.criterion(aux, y)
