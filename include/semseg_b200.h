@@ -662,7 +662,8 @@ int semseg_window_resize_add(const double* canvas, int C, int Hi, int Wi, double
  * Step glue: per-class intersection / union / target areas (util/util.py:55-67, called at tool/train.py:286,375).
  *   counts int32 [3][K] (zeroed by the call): [0] = #(pred == target == k), [1] = #(pred == k) with pred forced to
  *   ignore_index where target == ignore_index, [2] = #(target == k); union = [1] + [2] - [0].
- *   write_back != 0 also stores the masked prediction (the reference masks `output` in place).
+ *   write_back != 0 also stores the masked prediction (the reference masks `output` in place). 1 <= K <= 4096; n == 0
+ *   (pred and target may then be null) gives zero counts.
  */
 int semseg_iou_hist(void* pred_i64, const void* target_i64, long long n, int K, long long ignore_index, int write_back,
                     int* counts, void* stream);
@@ -671,8 +672,10 @@ int semseg_iou_hist(void* pred_i64, const void* target_i64, long long n, int K, 
  * torch.optim.SGD (momentum, dampening, weight decay, nesterov; tool/train.py:140,274-276) over every parameter tensor in
  * one launch. items_dev: device array sorted by chunk0 (an item's chunks are consecutive blocks of
  * semseg_sgd_chunk_elems() elements); grad_ptrs_dev: device array of n_items gradient pointers (0 = no gradient this
- * step: the parameter is skipped); hyper: per-group hyper-parameters, passed by value. `first` != 0 initialises the
- * momentum buffer with the (decayed) gradient, as torch does on a parameter's first step.
+ * step: the parameter is skipped); hyper: per-group hyper-parameters, passed by value, with nesterov a bit mask (bit g:
+ * group g uses Nesterov momentum). `first` != 0 initialises the momentum buffer with the (decayed) gradient, as torch
+ * does on a parameter's first step with a gradient under a non-zero momentum. In a group whose momentum is 0 the buffer
+ * is neither read nor written (it may be null), as torch leaves it.
  */
 #define SEMSEG_SGD_MAX_GROUPS 16
 typedef struct semseg_sgd_item {

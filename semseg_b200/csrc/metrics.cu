@@ -40,7 +40,9 @@ __global__ void __launch_bounds__(256) iou_hist_kernel(long long* __restrict__ p
 extern "C" int semseg_iou_hist(void* pred, const void* target, long long n, int K, long long ignore_index,
                                int write_back, int* counts, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(pred && target && counts && n >= 0 && K > 0 && K <= 4096, "iou_hist: bad args (K=%d)", K);
+  // an empty batch (n == 0, whose tensors may have no storage) gives zero counts, as the reference's histc does
+  SB_CHECK_ARG(counts && n >= 0 && K > 0 && K <= 4096 && (n == 0 || (pred && target)),
+               "iou_hist: bad args (n=%lld, K=%d)", n, K);
   SB_CUDA(cudaMemsetAsync(counts, 0, sizeof(int) * 3 * K, stream));
   if (n == 0) return SEMSEG_OK;
   long long blocks = (n + 256 * 8 - 1) / (256 * 8);

@@ -1,9 +1,11 @@
 // Multi-tensor SGD with momentum and weight decay in ONE launch (SURVEY.md §8 f4; torch.optim.SGD as configured at
 // tool/train.py:140,274-276 runs ~33 foreach kernels over the 161 parameter tensors):
 //   g' = g + wd * w;   buf = first ? g' : momentum * buf + (1 - dampening) * g';   w -= lr * (nesterov ? g' + momentum*buf : buf)
+// and, in a group whose momentum is 0, w -= lr * g' without reading or writing the buffer (torch leaves it as it is).
 // Hyper-parameters are per parameter GROUP (the trainer rewrites the 8 group learning rates every iteration,
-// tool/train.py:299-304) and travel by value in the launch parameters; tensors are described by a device-resident item
-// table (built once) plus a device array of gradient pointers (gradients are fresh tensors every step).
+// tool/train.py:299-304; nesterov is bit `group` of h.nesterov) and travel by value in the launch parameters; tensors
+// are described by a device-resident item table (built once) plus a device array of gradient pointers (gradients are
+// fresh tensors every step).
 #include "host_common.h"
 
 namespace sb {
@@ -28,40 +30,39 @@ sgd_multi_kernel(const semseg_sgd_item* __restrict__ items, const unsigned long 
   const float* __restrict__ g = reinterpret_cast<const float*>(grads[s_item]);
   if (g == nullptr) return;                      // parameter without a gradient this step (torch skips it too)
   const float lr = h.lr[it.group], mom = h.momentum[it.group], wd = h.weight_decay[it.group], damp = h.dampening[it.group];
+  const bool nesterov = (h.nesterov >> it.group) & 1;
+  const bool use_buf = mom != 0.f;               // without momentum the buffer (possibly none: buf == 0) is not touched
+  const bool read_buf = use_buf && !it.first;
   const long long base = static_cast<long long>(static_cast<int>(blockIdx.x) - it.chunk0) * kSgdChunk;
   const long long end = min(base + kSgdChunk, it.n);
   auto upd = [&](float w, float gg, float b) -> float2 {
     gg = fmaf(wd, w, gg);
+    if (!use_buf) return make_float2(w - lr * gg, b);
     b = it.first ? gg : fmaf(mom, b, (1.f - damp) * gg);
-    const float step = h.nesterov ? fmaf(mom, b, gg) : (mom != 0.f ? b : gg);
+    const float step = nesterov ? fmaf(mom, b, gg) : b;
     return make_float2(w - lr * step, b);
   };
   const bool vec = ((reinterpret_cast<uintptr_t>(it.w) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(it.buf)) & 15) == 0;
+  long long tail = base;
   if (vec) {
     for (long long i = base + 4LL * threadIdx.x; i + 3 < end; i += 4LL * blockDim.x) {
       float4 w = *reinterpret_cast<const float4*>(it.w + i);
       const float4 gg = *reinterpret_cast<const float4*>(g + i);
-      float4 b = it.first ? make_float4(0, 0, 0, 0) : *reinterpret_cast<const float4*>(it.buf + i);
+      float4 b = read_buf ? *reinterpret_cast<const float4*>(it.buf + i) : make_float4(0, 0, 0, 0);
       float2 r;
       r = upd(w.x, gg.x, b.x); w.x = r.x; b.x = r.y;
       r = upd(w.y, gg.y, b.y); w.y = r.x; b.y = r.y;
       r = upd(w.z, gg.z, b.z); w.z = r.x; b.z = r.y;
       r = upd(w.w, gg.w, b.w); w.w = r.x; b.w = r.y;
       *reinterpret_cast<float4*>(it.w + i) = w;
-      *reinterpret_cast<float4*>(it.buf + i) = b;
+      if (use_buf) *reinterpret_cast<float4*>(it.buf + i) = b;
     }
-    const long long tail = base + ((end - base) & ~3LL);
-    for (long long i = tail + threadIdx.x; i < end; i += blockDim.x) {
-      const float2 r = upd(it.w[i], g[i], it.first ? 0.f : it.buf[i]);
-      it.w[i] = r.x;
-      it.buf[i] = r.y;
-    }
-  } else {
-    for (long long i = base + threadIdx.x; i < end; i += blockDim.x) {
-      const float2 r = upd(it.w[i], g[i], it.first ? 0.f : it.buf[i]);
-      it.w[i] = r.x;
-      it.buf[i] = r.y;
-    }
+    tail = base + ((end - base) & ~3LL);
+  }
+  for (long long i = tail + threadIdx.x; i < end; i += blockDim.x) {
+    const float2 r = upd(it.w[i], g[i], read_buf ? it.buf[i] : 0.f);
+    it.w[i] = r.x;
+    if (use_buf) it.buf[i] = r.y;
   }
 }
 

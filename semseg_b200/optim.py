@@ -2,8 +2,10 @@
 for every parameter tensor in ONE kernel launch (csrc/sgd.cu) instead of ~33 foreach launches (SURVEY.md §8 f4).
 
 Drop-in for `torch.optim.SGD(params_list, lr=..., momentum=..., weight_decay=...)` at tool/train.py:140 (same constructor
-arguments, same param_groups — the trainer's per-iteration `optimizer.param_groups[i]['lr'] = ...` keeps working — and the
-same state_dict layout: state[p] = {'momentum_buffer': tensor}, so checkpoints move between the two classes).
+arguments, same param_groups — the trainer's per-iteration `optimizer.param_groups[i]['lr'] = ...` keeps working, and
+momentum, dampening, weight decay and nesterov are honoured per group — and the same state_dict layout: state[p] =
+{'momentum_buffer': tensor} once p has taken a step with a gradient under a non-zero momentum, which starts the buffer
+from that gradient, so checkpoints move between the two classes).
 fp32 CUDA parameters only; the conv operand slabs are refreshed by the model's own one-launch re-pack at the next forward
 (semseg_b200.functional.prepack), which notices the update through `bump_versions`.
 """
@@ -25,24 +27,22 @@ class FusedSGD(torch.optim.Optimizer):
             raise ValueError("FusedSGD supports up to 16 parameter groups")
         self._table = None
 
-    def _build(self, plist, device):
+    def _buffer(self, p):
+        st = self.state.get(p)
+        return st.get("momentum_buffer") if st else None
+
+    def _build(self, plist, first, key, device):
         chunk = int(_lib.load().semseg_sgd_chunk_elems())
         items = (_lib.SgdItem * len(plist))()
         c0 = 0
         for k, (gi, p) in enumerate(plist):
-            st = self.state[p]
-            first = "momentum_buffer" not in st or st["momentum_buffer"] is None
-            if first:
-                st["momentum_buffer"] = torch.empty_like(p, memory_format=torch.preserve_format)
             it = items[k]
-            it.w, it.buf, it.n = p.data_ptr(), st["momentum_buffer"].data_ptr(), p.numel()
-            it.group, it.chunk0, it.first = gi, c0, int(first)
+            it.w, it.buf, it.n = p.data_ptr(), key[k][1], p.numel()
+            it.group, it.chunk0, it.first = gi, c0, int(first[k])
             c0 += (p.numel() + chunk - 1) // chunk
         dev = torch.frombuffer(bytearray(bytes(items)), dtype=torch.uint8).to(device)
         dev_ptrs = torch.zeros((len(plist),), dtype=torch.int64, device=device)
-        key = tuple((p.data_ptr(), self.state[p]["momentum_buffer"].data_ptr()) for _, p in plist)
-        any_first = any(items[k].first for k in range(len(plist)))
-        return dict(items=dev, n=len(plist), chunks=c0, dev_ptrs=dev_ptrs, last_ptrs=None, key=key, any_first=any_first)
+        return dict(items=dev, n=len(plist), chunks=c0, dev_ptrs=dev_ptrs, last_ptrs=None, key=key)
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -56,36 +56,40 @@ class FusedSGD(torch.optim.Optimizer):
         for _, p in plist:
             if not (p.is_cuda and p.dtype == torch.float32 and p.is_contiguous()):
                 raise _lib.SemsegError("FusedSGD needs contiguous fp32 CUDA parameters (no CPU fallback)")
-        t = self._table
-        key = tuple((p.data_ptr(), self.state[p]["momentum_buffer"].data_ptr()
-                     if self.state[p].get("momentum_buffer") is not None else 0) for _, p in plist)
-        if t is None or t["key"] != key or t["any_first"]:
-            t = self._table = self._build(plist, plist[0][1].device)
-        ptrs = []
-        for _, p in plist:
+        h = _lib.SgdHyper()
+        for gi, g in enumerate(self.param_groups):
+            h.lr[gi], h.momentum[gi] = float(g["lr"]), float(g["momentum"])
+            h.weight_decay[gi], h.dampening[gi] = float(g["weight_decay"]), float(g["dampening"])
+            h.nesterov |= int(bool(g["nesterov"])) << gi
+        ptrs, first, key = [], [], []
+        for gi, p in plist:
             g = p.grad
             if g is not None and not (g.is_cuda and g.dtype == torch.float32 and g.is_contiguous()):
                 g = p.grad = g.contiguous().float()
             ptrs.append(g.data_ptr() if g is not None else 0)
+            b = self._buffer(p)
+            # like torch.optim.SGD, a parameter gets its momentum buffer on its first step with a gradient under a
+            # non-zero momentum (the kernel's fp32 value), and the buffer starts from that gradient
+            first.append(b is None and g is not None and h.momentum[gi] != 0)
+            if first[-1]:
+                b = self.state[p]["momentum_buffer"] = torch.empty_like(p, memory_format=torch.preserve_format)
+            key.append((p.data_ptr(), b.data_ptr() if b is not None else 0))
+        t = self._table
+        if t is None or t["key"] != key or any(first):
+            t = self._table = self._build(plist, first, key, plist[0][1].device)
         if ptrs != t["last_ptrs"]:
             # Upload the gradient pointer table only when it changed, from a FRESH pinned buffer each time: the copy is
             # asynchronous, so a reused staging buffer could be overwritten by the next step's pointers before this
             # step's copy has run (torch's pinned-memory allocator keeps a freed block alive until its copy completed).
             t["dev_ptrs"].copy_(torch.tensor(ptrs, dtype=torch.int64).pin_memory(), non_blocking=True)
             t["last_ptrs"] = ptrs
-        h = _lib.SgdHyper()
-        for gi, g in enumerate(self.param_groups):
-            h.lr[gi], h.momentum[gi] = float(g["lr"]), float(g["momentum"])
-            h.weight_decay[gi], h.dampening[gi] = float(g["weight_decay"]), float(g["dampening"])
-        h.nesterov = int(bool(self.param_groups[0]["nesterov"]))
         lib = _lib.load()
         _lib.check(lib.semseg_sgd_multi(ctypes.c_void_p(t["items"].data_ptr()), ctypes.c_void_p(t["dev_ptrs"].data_ptr()),
                                         t["n"], t["chunks"], ctypes.byref(h), _stream()), "semseg_sgd_multi")
         # the raw update does not touch the autograd version counters; the conv operand caches are keyed on them
         _bump_versions([p for _, p in plist if p.grad is not None])
-        if t["any_first"]:
-            t["any_first"] = False
-            self._table = None       # rebuild once with first = 0
+        if any(first):
+            self._table = None       # rebuild once with these first flags cleared
         return loss
 
 

@@ -78,10 +78,12 @@ def test_ema_decay_one_is_a_no_op_and_reruns_are_bit_identical():
     assert all(torch.equal(x, y) for x, y in zip(_tensors(a.module), _tensors(b.module)))
 
 
+@pytest.mark.parametrize("decay", [0.0, 0.25, 0.5, 0.75, 0.999])
 @pytest.mark.parametrize("offset", [0, 1, 3])
-def test_ema_kernel_odd_lengths_and_misaligned_tails(offset):
+def test_ema_kernel_odd_lengths_and_misaligned_tails(offset, decay):
     """Raw item tables: lengths 1 .. 2 chunks + 5 at element offsets that break the 16-byte alignment (scalar path) or
-    keep it, int64 items between them."""
+    keep it, int64 items between them. Both branches of torch.lerp's form: weight 1 - decay below 0.5 (decay 0.75,
+    0.999) and from 0.5 up (decay 0.5, 0.25, and 0: the first two updates of a min(decay, 1 - 1/(t+1)) ramp)."""
     from semseg_b200 import ops
     from semseg_b200.optim import ema_table
     g = torch.Generator(device="cuda").manual_seed(offset)
@@ -96,11 +98,11 @@ def test_ema_kernel_odd_lengths_and_misaligned_tails(offset):
             e = torch.randn((n + offset,), device="cuda", generator=g)[offset:]
             w = torch.randn((n + offset,), device="cuda", generator=g)[offset:]
             r = e.clone()
-            torch._foreach_lerp_([r], [w], 1 - 0.75)
+            torch._foreach_lerp_([r], [w], 1 - decay)
             refs.append(r)
         pairs.append((e, w))
     items, n_items, chunks = ema_table(pairs)
-    ops.ema_multi(items, n_items, chunks, 0.75)
+    ops.ema_multi(items, n_items, chunks, decay)
     for (e, _), r in zip(pairs, refs):
         assert torch.equal(e, r)
 
