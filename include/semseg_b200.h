@@ -33,6 +33,7 @@
  *                               (tool/test.py:163-176) and the per-scale resize into the running total
  *                               (tool/test.py:177, 202).
  *   - semseg_augment          : tool/train.py:194-212's transform chains (util/transform.py), one launch per batch.
+ *   - semseg_strong_augment   : the strong (colour jitter, grayscale, blur) student view of mean-teacher training.
  *
  * Activations are NHWC bf16 in HBM; "pitch" arguments are the distance between consecutive pixels in
  * elements (>= channels; lets a kernel read/write a channel slice of a wider concat buffer).
@@ -627,6 +628,29 @@ int semseg_mix_apply(int mode, const float* x, int N, int Cin, int H, int W, con
                      const float* uniforms, int ustride, double p, double area_lo, double area_hi, double ratio_lo,
                      double ratio_hi, const uint8_t* argmax, const uint32_t* selected, uint8_t* mask,
                      float* x_mixed, int64_t* y_mixed, void* stream);
+/* The strong view of mean-teacher training (csrc/strong.cu, semseg_b200/augment.py StrongAugment): colour jitter,
+ * grayscale and Gaussian blur of x fp32 NCHW [N,3,H,W] (normalised) -> out (same shape, not aliasing x). Image n uses
+ * uniforms u[n, 0..11] (fp32 [N, ustride], ustride >= 12); a comparison "u < p" is made as (double) u < p. Per image:
+ *   1. v = clamp((x std_c + mean_c) / 255, 0, 1) in fp32. This and every later step run only when at least one operation
+ *      below applies; an image with none applied is copied bit for bit.
+ *   2. Colour jitter iff u0 < p_jitter. Factors in fp64, rounded once to fp32: brightness b = lo + (hi - lo) u1 with
+ *      [lo, hi] = [max(0, 1 - B), 1 + B], contrast c by u2 and saturation s by u3 alike, hue h = -H + 2H u4. An operation
+ *      of strength 0 is skipped. Order: ascending (u5..u8, index). torchvision.transforms.v2.functional's float forms:
+ *      brightness clamp(b v); contrast clamp(c v + (1 - c) m), m = the image mean of gray(v) at that point of the chain;
+ *      saturation clamp(s v + (1 - s) gray(v)); hue _rgb2hsv, h <- (h + hue) mod 1, _hsv2rgb.
+ *      gray = 0.2989 r + 0.587 g + 0.114 b.
+ *   3. Grayscale iff u9 < p_gray: every channel becomes gray(v).
+ *   4. Blur iff u10 < p_blur: sigma = fp32(sigma_lo + (sigma_hi - sigma_lo) u11) (fp64, rounded once),
+ *      r = min(ceil(3 sigma), ceil(3 sigma_hi)), taps exp(-k^2 / 2 sigma^2), k = -r..r, normalised; separable, with
+ *      reflect-101 borders (the edge pixel is not repeated): torchvision's gaussian_blur(v, [2r+1]*2, [sigma]*2).
+ *   5. out = (255 v - mean_c) / std_c.
+ * workspace: N ceil(H/32) ceil(W/32) floats (per-tile partial sums of the contrast mean). Strengths finite >= 0 with
+ * hue <= 0.5, probabilities in [0, 1], 0 < sigma_lo <= sigma_hi <= 5, std > 0, H and W > ceil(3 sigma_hi). Two launches,
+ * fixed geometry, no atomics, deterministic, no host synchronisation. Bad arguments are rejected before any CUDA call. */
+int semseg_strong_augment(const float* x, int N, int C, int H, int W, const float* uniforms, int ustride,
+                          double brightness, double contrast, double saturation, double hue, double p_jitter,
+                          double p_gray, double p_blur, double sigma_lo, double sigma_hi, const float* mean3,
+                          const float* std3, float* workspace, float* out, void* stream);
 /* Segmented stable radix sort (csrc/segsort.cu): S segments of L (uint32 key, uint32 payload) pairs, [S][L], each sorted
  * in place by key ascending, equal keys in input order. keys_alt / vals_alt: scratch of the same size. skip: NULL, or
  * int [S] on the device, a non-zero entry leaves that segment untouched. workspace:

@@ -237,6 +237,8 @@ SIGNATURES = {
     "semseg_mix_apply": (c_int, [c_int, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp, c_int,
                                  ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double, ctypes.c_double,
                                  c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_strong_augment": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_int] + [ctypes.c_double] * 9 +
+                              [c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_segsort_u32_pairs_workspace_bytes": (c_ll, [c_int, c_ll]),
     "semseg_segsort_u32_pairs": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_ll, c_vp, c_vp, c_vp]),
     "semseg_window_scores": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),

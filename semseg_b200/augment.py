@@ -13,6 +13,9 @@ in cv2's 10-bit fixed point about (w/2, h/2) with border mean / ignore_label, 5x
 borders, horizontal flip, padding (mean / ignore_label, half leading) and crop, then (x - mean) / std in fp32.
 Random draws happen in the calling process, from `rng` (default: the `random` module): a DataLoader worker's
 `random.seed` no longer affects augmentation.
+
+`StrongAugment` is the strong view of mean-teacher training (colour jitter, grayscale, Gaussian blur of an already
+normalised batch, csrc/strong.cu), drawn on the device and made inside the student's forward.
 """
 import collections.abc
 import ctypes
@@ -25,8 +28,8 @@ import torch
 
 from . import _lib, ops
 
-__all__ = ["AugParams", "AugBatch", "ToUint8", "collate", "TrainAugment", "ValAugment", "resized_size",
-           "rotation_inverse"]
+__all__ = ["AugParams", "AugBatch", "ToUint8", "collate", "TrainAugment", "ValAugment", "StrongAugment",
+           "resized_size", "rotation_inverse"]
 
 AugParams = collections.namedtuple("AugParams", "fx fy angle blur flip h_off w_off")
 AugParams.__doc__ = """One sample's draws: resize factors, rotation angle in degrees (None: not rotated), blur and flip
@@ -256,3 +259,114 @@ class ValAugment(_Augment):
         if not isinstance(batch, AugBatch):
             batch = collate(batch)
         return self.apply(batch, self.draw_params(batch.sizes()))
+
+
+def _number(name, v):
+    if isinstance(v, bool) or not isinstance(v, numbers.Real):
+        raise TypeError("%s must be a number, got %r" % (name, v))
+    v = float(v)
+    if not math.isfinite(v):
+        raise ValueError("%s must be finite, got %r" % (name, v))
+    return v
+
+
+class StrongAugment:
+    """The strong view of weak-to-strong mean-teacher training (FixMatch, UniMatch, U2PL, CutMix-Seg): colour jitter,
+    random grayscale and Gaussian blur of a normalised fp32 NCHW batch on the GPU, in two launches of csrc/strong.cu,
+    without a host synchronisation (so it runs inside a captured training step). The defaults are UniMatch's strong
+    pipeline; `mean` / `std` are the normalisation the batch carries (the trainer's, tool/train.py:189-192), and the view
+    is computed on the de-normalised image. Give it to a teacher criterion (losses.DistillationLoss, PseudoLabelLoss,
+    MixPseudoLabelLoss: `strong=`) and the teacher sees the batch while the student sees its strong view.
+
+    Each image n has its own uniforms u[n, 0..11], one torch.rand(N, 12) on the device's default CUDA generator (`draw`).
+    Per image (include/semseg_b200.h semseg_strong_augment states it exactly):
+
+        v      = clamp((x std_c + mean_c) / 255, 0, 1)       only when some operation applies; else x is copied bit for bit
+        jitter iff u0 < p_jitter: factors b in [max(0, 1 - brightness), 1 + brightness] by u1, contrast c by u2,
+               saturation s by u3 alike, hue in [-hue, hue] by u4 (each lo + (hi - lo) u in fp64, rounded once to fp32);
+               a strength of 0 skips its operation (torchvision's None); the order is ascending (u5..u8, index) in
+               place of torchvision's randperm(4). Each is torchvision.transforms.v2.functional's float form:
+               brightness clamp(b v), contrast clamp(c v + (1 - c) mean(gray(v))), saturation clamp(s v + (1 - s)
+               gray(v)), hue through torchvision's HSV conversion; gray = 0.2989 r + 0.587 g + 0.114 b
+        gray   iff u9 < p_gray: every channel becomes gray(v)
+        blur   iff u10 < p_blur: sigma = sigma_lo + (sigma_hi - sigma_lo) u11, r = ceil(3 sigma), the true Gaussian of
+               torchvision's gaussian_blur(v, [2r+1]*2, [sigma]*2) with reflect padding. UniMatch blurs with PIL's box
+               approximation of a Gaussian; this is the exact one. PIL's uint8 rounding between operations is not
+               reproduced either: the chain stays in fp32.
+        x_s    = (255 v - mean_c) / std_c
+
+    The operations move no pixel, so labels stay valid. There is no gradient through the view: an input with
+    requires_grad raises. `strong(x, u=None)` -> the view (u = strong.draw(x) when None), a new tensor; the input is a
+    CUDA fp32 [N, 3, H, W] tensor with H, W > ceil(3 sigma_hi). Under DistributedDataParallel each rank draws its own
+    view (multi-GPU runs have not been made)."""
+
+    def __init__(self, brightness=0.5, contrast=0.5, saturation=0.5, hue=0.25, p_jitter=0.8, p_gray=0.2, p_blur=0.5,
+                 sigma=(0.1, 2.0), mean=(0.485 * 255, 0.456 * 255, 0.406 * 255),
+                 std=(0.229 * 255, 0.224 * 255, 0.225 * 255)):
+        for name, v in (("brightness", brightness), ("contrast", contrast), ("saturation", saturation), ("hue", hue)):
+            v = _number(name, v)
+            if v < 0.0:
+                raise ValueError("%s must be >= 0, got %r" % (name, v))
+            setattr(self, name, v)
+        if self.hue > 0.5:
+            raise ValueError("hue must be <= 0.5, got %r" % self.hue)
+        for name, v in (("p_jitter", p_jitter), ("p_gray", p_gray), ("p_blur", p_blur)):
+            v = _number(name, v)
+            if not 0.0 <= v <= 1.0:
+                raise ValueError("%s must lie in [0, 1], got %r" % (name, v))
+            setattr(self, name, v)
+        if not isinstance(sigma, (tuple, list)) or len(sigma) != 2:
+            raise TypeError("sigma must be a pair (lo, hi), got %r" % (sigma,))
+        lo, hi = _number("sigma", sigma[0]), _number("sigma", sigma[1])
+        if not 0.0 < lo <= hi <= 5.0:
+            raise ValueError("sigma must satisfy 0 < lo <= hi <= 5, got %r" % (sigma,))
+        self.sigma = (lo, hi)
+        for name, v in (("mean", mean), ("std", std)):
+            if not isinstance(v, (tuple, list)) or len(v) != 3:
+                raise ValueError("%s must hold 3 numbers, got %r" % (name, v))
+            setattr(self, name, tuple(_number(name, c) for c in v))
+        if any(s <= 0.0 for s in self.std):
+            raise ValueError("std must be > 0, got %r" % (self.std,))
+
+    def key(self):
+        """The options as a tuple: what a captured training step bakes in."""
+        return (self.brightness, self.contrast, self.saturation, self.hue, self.p_jitter, self.p_gray, self.p_blur,
+                self.sigma, self.mean, self.std)
+
+    def extra_repr(self):
+        return "brightness=%g, contrast=%g, saturation=%g, hue=%g, p_jitter=%g, p_gray=%g, p_blur=%g, sigma=(%g, %g)" \
+               ", mean=(%g, %g, %g), std=(%g, %g, %g)" % ((self.brightness, self.contrast, self.saturation, self.hue,
+                                                           self.p_jitter, self.p_gray, self.p_blur) + self.sigma +
+                                                          self.mean + self.std)
+
+    def __repr__(self):
+        return "StrongAugment(%s)" % self.extra_repr()
+
+    def _check(self, x):
+        if not torch.is_tensor(x):
+            raise TypeError("StrongAugment: the input must be a tensor, got %s" % type(x).__name__)
+        if x.requires_grad:
+            raise RuntimeError("StrongAugment: there is no gradient through the strong view; the input must not "
+                               "require grad")
+        if not x.is_cuda or x.dtype != torch.float32 or x.dim() != 4 or x.shape[1] != 3:
+            raise TypeError("StrongAugment: the input must be a CUDA fp32 [N, 3, H, W] tensor, got %s %s on %s" %
+                            (x.dtype, tuple(x.shape), x.device))
+        r = math.ceil(3.0 * self.sigma[1])
+        if x.shape[2] <= r or x.shape[3] <= r:
+            raise ValueError("StrongAugment: a %dx%d image needs H, W > ceil(3 sigma_hi) = %d" % (x.shape[2], x.shape[3],
+                                                                                                  r))
+
+    def draw(self, x):
+        """The uniforms of one view of `x`: fp32 [N, 12] from torch.rand on x's device."""
+        self._check(x)
+        return torch.rand((x.shape[0], 12), device=x.device)
+
+    def __call__(self, x, u=None):
+        self._check(x)
+        if u is None:
+            u = self.draw(x)
+        if not (torch.is_tensor(u) and u.dtype == torch.float32 and u.device == x.device and u.dim() == 2 and
+                u.shape[0] == x.shape[0] and u.shape[1] >= 12 and u.stride(1) == 1):
+            raise ValueError("StrongAugment: uniforms must be fp32 [%d, >= 12] on %s" % (x.shape[0], x.device))
+        return ops.strong_augment(x.contiguous(), u, self.brightness, self.contrast, self.saturation, self.hue,
+                                  self.p_jitter, self.p_gray, self.p_blur, self.sigma, self.mean, self.std)

@@ -20,7 +20,8 @@ overwrites the first one's saved activations — gradient accumulation over seve
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
 loss, the focal loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
-mean teacher's re-pack included, and the CutMix / ClassMix pseudo-label loss, its draws and mixing included) are not captured (such models simply stay eager).
+mean teacher's re-pack included, and the CutMix / ClassMix pseudo-label loss, its draws and mixing included, with or
+without a strong view of the student's input) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -62,11 +63,11 @@ def note_boundary(t):
 class _Step:
     __slots__ = ("key", "calls", "failed", "fwd", "bwd", "bwd2", "x", "y", "pred", "main", "aux", "g_main", "g_aux",
                  "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot", "mix",
-                 "mix_crit")
+                 "mix_crit", "strong", "strong_crit")
 
     def __init__(self, key):
         self.key, self.calls, self.failed, self.fwd, self.dx_slot = key, 0, False, None, False
-        self.mix = self.mix_crit = None
+        self.mix = self.mix_crit = self.strong = self.strong_crit = None
 
 
 def _set_grad_outputs(st, g_main, g_aux):
@@ -126,9 +127,11 @@ class _Replay(torch.autograd.Function):
 
 def _point_mix(st):
     """A losses.MixPseudoLabelLoss criterion's last_mix() is the replayed step's: its mask, mixed target and uniforms
-    are that step's static tensors (each captured input shape has its own)."""
+    are that step's static tensors (each captured input shape has its own). So is a teacher criterion's last_strong()."""
     if st.mix_crit is not None:
         st.mix_crit._mix_state = st.mix
+    if st.strong_crit is not None:
+        st.strong_crit._strong_state = st.strong
 
 
 def _with_dx(st, gs):
@@ -263,6 +266,9 @@ def _capture(model, impl, st, x, y):
     if getattr(crit, "_mix_state", None) is not None:
         # the mix the captured forward wrote: static tensors of the graph's pool, refreshed by every replay
         st.mix, st.mix_crit = crit._mix_state, crit
+    if getattr(crit, "strong", None) is not None:
+        # likewise the strong view and its uniforms
+        st.strong, st.strong_crit = crit._strong_state, crit
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
     del proxies, x_in, x_leaf
@@ -324,6 +330,8 @@ def train_step(model, impl, x, y):
                      tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
         crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight",
                                                              "mix", "p", "area", "ratio"))
+        if crit.strong is not None:
+            crit_key += ("strong",) + crit.strong.key()    # the strong view's options are launch arguments too
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
            dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad,
            crit_key)

@@ -9,7 +9,8 @@ optional class weights, run the same way. DistillationLoss adds a
 pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
 optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
-batch, the student learns on the mixed one.
+batch, the student learns on the mixed one. Each of the three teacher criteria takes `strong=` (augment.StrongAugment):
+the student then learns on a strongly perturbed view of the batch the teacher sees.
 """
 import math
 
@@ -218,17 +219,29 @@ class _TeacherLoss(nn.Module):
     statistics or training flag, and no gradient reaches it or, through it, the input (with x.requires_grad, x.grad is
     the student's). A ModelEMA shadow changes after every `ema.update`: its operand slabs are re-packed at the top of
     every teacher forward (in one launch, part of the captured training step), and the graphed step is keyed on its
-    tensors' addresses, not their versions, so it is captured once and replays each step with the current shadow."""
+    tensors' addresses, not their versions, so it is captured once and replays each step with the current shadow.
 
-    def __init__(self, teacher, ignore_index):
+    `strong` (an augment.StrongAugment, default None) gives the student a strong view of the batch: per training forward
+    its uniforms are drawn after any mix draw and before the teacher forward, the teacher runs on the batch, and the
+    student, both heads' losses and any mixing see the view (the targets are unchanged: the view moves no pixel).
+    `last_strong()` returns {'image': the view before any mixing, 'uniforms': its draws} of the latest training forward,
+    graphed or eager, as views that stay valid until the next forward. There is no gradient through the view: an input
+    with requires_grad raises. strong=None changes nothing."""
+
+    def __init__(self, teacher, ignore_index, strong=None):
         super(_TeacherLoss, self).__init__()
+        from .augment import StrongAugment
         from .pspnet import PSPNet
         from .psanet import PSANet
         if not isinstance(teacher, (PSPNet, PSANet)):
             raise TypeError("teacher must be a semseg_b200 PSPNet or PSANet, got %s" % type(teacher).__name__)
         if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
             raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        if strong is not None and not isinstance(strong, StrongAugment):
+            raise TypeError("strong must be an augment.StrongAugment or None, got %s" % type(strong).__name__)
         self.ignore_index = ignore_index
+        self.strong = strong
+        self._strong_state = None
         self.__dict__['_teacher'] = teacher      # held outside the module tree (see the class docstring)
 
     @property
@@ -241,6 +254,20 @@ class _TeacherLoss(nn.Module):
             raise AttributeError("%s: the teacher is fixed at construction; build a new criterion" %
                                  type(self).__name__)
         super(_TeacherLoss, self).__setattr__(name, value)
+
+    def _strong_repr(self):
+        return "" if self.strong is None else ", strong=%r" % (self.strong,)
+
+    def last_strong(self):
+        """{'image', 'uniforms'} of the latest training forward's strong view (None before the first one, or without
+        `strong`)."""
+        return None if self._strong_state is None else dict(self._strong_state)
+
+    def strong_view(self, x, u):
+        """The student's view of `x` from `strong.draw`'s uniforms `u`; remembered for last_strong()."""
+        xs = self.strong(x, u)
+        self._strong_state = {'image': xs, 'uniforms': u}
+        return xs
 
     def run_teacher(self, x, classes):
         """The teacher's detached fp32 NHWC 1/8-resolution logits of the input batch `x` (NCHW), for a student with
@@ -300,8 +327,9 @@ class DistillationLoss(_TeacherLoss):
     validate() logs), with them (the same shape) `main` computed at that size. It runs the zoom-1 kernels on NHWC copies.
     CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
 
-    def __init__(self, teacher, temperature=1.0, kd_weight=1.0, ce_weight=1.0, ignore_index=255, at='output'):
-        super(DistillationLoss, self).__init__(teacher, ignore_index)
+    def __init__(self, teacher, temperature=1.0, kd_weight=1.0, ce_weight=1.0, ignore_index=255, at='output',
+                 strong=None):
+        super(DistillationLoss, self).__init__(teacher, ignore_index, strong)
         if not isinstance(at, str):
             raise TypeError("at must be 'output' or 'logits', got %r" % (at,))
         if at not in ('output', 'logits'):
@@ -316,7 +344,8 @@ class DistillationLoss(_TeacherLoss):
 
     def extra_repr(self):
         return "teacher=%s, temperature=%g, kd_weight=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
-            type(self.teacher).__name__, self.temperature, self.kd_weight, self.ce_weight, self.ignore_index, self.at)
+            type(self.teacher).__name__, self.temperature, self.kd_weight, self.ce_weight, self.ignore_index,
+            self.at) + self._strong_repr()
 
     def forward(self, logits, target, teacher_logits=None):
         from . import functional as SF
@@ -357,8 +386,8 @@ class PseudoLabelLoss(_TeacherLoss):
     with them (the same shape) `main` computed at that size. CUDA fp32 logits with at most 256 classes only: there is no
     CPU or library fallback."""
 
-    def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255):
-        super(PseudoLabelLoss, self).__init__(teacher, ignore_index)
+    def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None):
+        super(PseudoLabelLoss, self).__init__(teacher, ignore_index, strong)
         if isinstance(threshold, bool) or not isinstance(threshold, (int, float)):
             raise TypeError("threshold must be a number, got %r" % (threshold,))
         if not math.isfinite(threshold):
@@ -369,7 +398,8 @@ class PseudoLabelLoss(_TeacherLoss):
 
     def extra_repr(self):
         return "teacher=%s, threshold=%g, pl_weight=%g, ce_weight=%g, ignore_index=%d" % (
-            type(self.teacher).__name__, self.threshold, self.pl_weight, self.ce_weight, self.ignore_index)
+            type(self.teacher).__name__, self.threshold, self.pl_weight, self.ce_weight,
+            self.ignore_index) + self._strong_repr()
 
     def forward(self, logits, target, teacher_logits=None):
         from . import functional as SF
@@ -430,8 +460,8 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
     DistributedDataParallel each rank mixes its own batch (multi-GPU runs have not been made)."""
 
     def __init__(self, teacher, mix='cutmix', p=0.5, area=(0.02, 0.4), ratio=(0.3, 1 / 0.3), threshold=0.95,
-                 pl_weight=1.0, ce_weight=1.0, ignore_index=255):
-        super(MixPseudoLabelLoss, self).__init__(teacher, threshold, pl_weight, ce_weight, ignore_index)
+                 pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None):
+        super(MixPseudoLabelLoss, self).__init__(teacher, threshold, pl_weight, ce_weight, ignore_index, strong)
         if not isinstance(mix, str):
             raise TypeError("mix must be 'cutmix' or 'classmix', got %r" % (mix,))
         if mix not in ('cutmix', 'classmix'):
@@ -449,7 +479,7 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
         return "teacher=%s, mix=%r, p=%g, area=(%g, %g), ratio=(%g, %g), threshold=%g, pl_weight=%g, ce_weight=%g, " \
                "ignore_index=%d" % (type(self.teacher).__name__, self.mix, self.p, self.area[0], self.area[1],
                                     self.ratio[0], self.ratio[1], self.threshold, self.pl_weight, self.ce_weight,
-                                    self.ignore_index)
+                                    self.ignore_index) + self._strong_repr()
 
     def last_mix(self):
         """{'mask', 'target', 'uniforms'} of the latest training forward (None before the first one)."""

@@ -1277,3 +1277,26 @@ def augment(data, descs, descs_dev, crop_h, crop_w, mean, std, ignore_label):
     _lib.check(lib.semseg_augment(_ptr(data), data.numel(), descs, _ptr(descs_dev), n, crop_h, crop_w, m3, s3,
                                   ignore_label, _ptr(img), _ptr(lab), _stream()), "semseg_augment")
     return img, lab
+
+
+STRONG_TILE = 32          # csrc/strong.cu kStrongTile: one contrast partial per (32x32 tile, image)
+
+
+def strong_augment(x, uniforms, brightness, contrast, saturation, hue, p_jitter, p_gray, p_blur, sigma, mean, std):
+    """The strong view (semseg_strong_augment): x fp32 NCHW [N,3,H,W] (normalised), uniforms fp32 [N, >= 12] -> the
+    view, a new tensor of x's shape. sigma = (lo, hi); mean / std: 3 numbers each, the normalisation of x."""
+    _require_cuda(x, uniforms)
+    lib = _lib.load()
+    assert x.dtype == torch.float32 and x.dim() == 4 and x.is_contiguous()
+    assert uniforms.dtype == torch.float32 and uniforms.dim() == 2 and uniforms.stride(1) == 1
+    n, c, hh, ww = x.shape
+    assert uniforms.shape[0] == n, "input and uniforms differ in batch size"
+    out = torch.empty_like(x)
+    ws = torch.empty((n * -(-hh // STRONG_TILE) * -(-ww // STRONG_TILE),), dtype=torch.float32, device=x.device)
+    m3, s3 = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
+    _lib.check(lib.semseg_strong_augment(_ptr(x), n, c, hh, ww, _ptr(uniforms), uniforms.stride(0), float(brightness),
+                                         float(contrast), float(saturation), float(hue), float(p_jitter),
+                                         float(p_gray), float(p_blur), float(sigma[0]), float(sigma[1]), m3, s3,
+                                         _ptr(ws), _ptr(out), _stream()),
+               "semseg_strong_augment")
+    return out

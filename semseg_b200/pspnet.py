@@ -142,9 +142,13 @@ class _SegNet(nn.Module):
             classes = self.cls[4].out_channels
             mixing = isinstance(self.criterion, losses.MixPseudoLabelLoss)
             u = self.criterion.draw(x, classes) if mixing else None      # the draws come before the teacher forward
+            strong = self.criterion.strong
+            u_s = strong.draw(x) if strong is not None else None
             # the teacher first (distillation, pseudo-labels): its activations are transient before the student's saved
-            # ones exist. It sees the unmixed batch; the student and both heads' losses see the mixed one
+            # ones exist. It sees the batch; the student and both heads' losses see its strong view, mixed
             t_logits = self.criterion.run_teacher(x, classes)
+            if strong is not None:
+                x = self.criterion.strong_view(x, u_s)
             if mixing:
                 x, y, mix_mask = self.criterion.mix_batch(x, y, u, t_logits, self.zoom_factor)
         logits, t_aux = self._logits_nhwc(x)
