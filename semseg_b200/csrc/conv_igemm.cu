@@ -85,8 +85,19 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     m_tile = item / p.n_tiles;
   };
 
+  auto tile_origin = [&](int m_tile, int& img, int& h0, int& w0) {   // image and first pixel of a pixel tile
+    const int tiles_per_img = p.tiles_h * p.tiles_w;
+    img = m_tile / tiles_per_img;
+    const int rem = m_tile - img * tiles_per_img;
+    h0 = (rem / p.tiles_w) * p.bh;
+    w0 = (rem % p.tiles_w) * p.bw;
+  };
+
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // aligned by an offset from smem_raw (not through an integer), so that the compiler still knows every pointer below
+  // is in shared memory: the epilogue's staging stores and statistics loads become st.shared / ld.shared with 32-bit
+  // addresses instead of generic accesses with 64-bit address arithmetic
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* stage_base = smem;
   uint8_t* out_stage = smem + kStages * kStageBytes;  // 2 x 16 KB
   uint8_t* misc = out_stage + 2 * kStageOutBytes;
@@ -171,11 +182,35 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     int it = 0;
     int store_buf = 0;
     float acc[kAcc];
+    constexpr int kChunks = BLOCK_N / 64;
+    const bool stats = p.stats_partial != nullptr && p.epi_mode == SEMSEG_EPI_RAW;
+    // running sum and sum of squares of this thread's statistics column in every chunk, and the running pixel count
+    // of its 32 rows (the same for every chunk), added to the CTA's statistics row in global memory only when the
+    // CTA's next item is in another channel tile (or there is none)
+    float st_acc[kChunks][2], st_n = 0.f;
+#pragma unroll
+    for (int ch = 0; ch < kChunks; ++ch) st_acc[ch][0] = st_acc[ch][1] = 0.f;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       int m_tile, n_tile, k_slice, kblk0, kblk1;
       decode_item(item, m_tile, n_tile, k_slice);
       slice_range(k_slice, kblk0, kblk1);
       const int num_kb = (kblk1 - kblk0) * nseg;
+      if (p.epi_mode == SEMSEG_EPI_AFFINE && p.residual != nullptr && (lane & 3) < kChunks) {
+        // pull the tile's residual into L2 while the main loop runs (the epilogue reads it chunk by chunk): lane & 3
+        // picks the 128-byte line (one 64-column chunk) of each of the thread's two pixel rows
+        const int c = n_tile * BLOCK_N + 64 * (lane & 3);
+        int img, h0, w0;
+        tile_origin(m_tile, img, h0, w0);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int r = r_base + 8 * i, hi = r / p.bw, wi = r - hi * p.bw;
+          if (c < p.Cout && r < p.bh * p.bw && h0 + hi < p.H && w0 + wi < p.W) {
+            const long long ro = ((static_cast<long long>(img) * p.H + (h0 + hi)) * p.W + (w0 + wi)) * p.res_pitch + c;
+            prefetch_l2(p.residual + ro);
+            if (kSplit) prefetch_l2(p.residual_lo + ro);
+          }
+        }
+      }
       // ---- main loop: one wgmma batch (K = 64) per stage; a stage is released once the next batch was issued and
       // the one reading it has completed
       int prev_s = -1;
@@ -206,11 +241,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
 
       // ---- epilogue
-      const int tiles_per_img = p.tiles_h * p.tiles_w;
-      const int img = m_tile / tiles_per_img;
-      const int rem = m_tile - img * tiles_per_img;
-      const int h0 = (rem / p.tiles_w) * p.bh;
-      const int w0 = (rem % p.tiles_w) * p.bw;
+      int img, h0, w0;
+      tile_origin(m_tile, img, h0, w0);
       const int n0 = n_tile * BLOCK_N;
       auto row_ok = [&](int r) {
         const int hi = r / p.bw, wi = r - (r / p.bw) * p.bw;
@@ -227,7 +259,6 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         rv[i] = row_ok(r_base + 8 * i);
         pix[i] = row_pix(r_base + 8 * i);
       }
-      constexpr int kChunks = BLOCK_N / 64;
 #pragma unroll
       for (int ch = 0; ch < kChunks; ++ch) {
         const int c0 = n0 + ch * 64;  // first output channel of this chunk
@@ -323,63 +354,57 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (kSplit) tma_store_4d(&tmC_lo, obuf + kStageOutBytes, c0, w0, h0, img);
           tma_store_commit();
         }
-        if (p.stats_partial != nullptr && p.epi_mode == SEMSEG_EPI_RAW && wg == (ch & 1)) {
-          // Per-column statistics of the bf16 values just staged (exactly what BN-apply will read back). Warp g of the
-          // warpgroup whose turn it is reduces pixel rows [32g, 32g + 32), lane = column pair (one 4-byte word,
-          // conflict-free), one pass of sum and sum of squares, then a read-modify-write of the CTA's statistics row g
-          // in global memory: no cross-warp traffic, fixed order -> deterministic.
+        if (stats) {
+          // Per-column statistics of the bf16 values just staged (exactly what BN-apply will read back). Warp g of
+          // warpgroup w reduces pixel rows [32g, 32g + 32) of the chunk's columns [32w, 32w + 32), lane = column (two
+          // lanes per 4-byte word: conflict-free), one pass of sum and sum of squares in row order, added to the
+          // thread's registers: no cross-warp traffic, fixed order -> deterministic. A row outside the image adds
+          // +0.f: neither sum is ever -0.f, so that leaves its bits as skipping the row would, and the 32 loads need
+          // no branches and can all be in flight together.
           const int g = wq;
-          float* st_dst = p.stats_partial + (static_cast<size_t>(blockIdx.x) * 4 + g) * 3 * p.Cout + c0 + 2 * lane;
-          float st_old[6];
-          st_old[0] = st_dst[0];
-          st_old[1] = st_dst[1];
-          st_old[2] = st_dst[p.Cout];
-          st_old[3] = st_dst[p.Cout + 1];
-          st_old[4] = st_dst[2 * p.Cout];
-          st_old[5] = st_dst[2 * p.Cout + 1];
           const uint32_t row_msk = __ballot_sync(0xffffffffu, row_ok(g * 32 + lane));
-          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-          const uint8_t* base = obuf + (lane & 3) * 4;
-          const int chunk16 = lane >> 2;
-          auto add_row = [&](int rr, int sw) {  // sw = rr & 7 (the row's swizzle phase)
-            float2 f = __bfloat1622float2(
-                *reinterpret_cast<const __nv_bfloat162*>(base + rr * 128 + ((chunk16 ^ sw) << 4)));
-            if constexpr (kSplit) {
-              const float2 fl = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(
-                  base + kStageOutBytes + rr * 128 + ((chunk16 ^ sw) << 4)));
-              f.x += fl.x;
-              f.y += fl.y;
-            }
-            s0 += f.x;
-            s1 += f.y;
-            q0 = fmaf(f.x, f.x, q0);
-            q1 = fmaf(f.y, f.y, q1);
-          };
-          if ((row_msk & (row_msk + 1u)) == 0u) {
-            // valid rows are a prefix of the warp's 32 (always, unless the box is clipped by the right image edge):
-            // whole groups of 8 rows run without per-row predicates, the swizzle phase is a compile-time constant
-            const int nr = __popc(row_msk);
-            const int nfull = nr >> 3;
-            for (int b8 = 0; b8 < nfull; ++b8) {
-              const int rr0 = g * 32 + b8 * 8;
+          float sm = 0.f, sq = 0.f;
+          const int col = 32 * wg + lane;
+          const uint8_t* base = obuf + g * 32 * 128 + (col & 7) * 2;
+          const int chunk16 = col >> 3;
 #pragma unroll
-              for (int k = 0; k < 8; ++k) add_row(rr0 + k, k);
-            }
-            for (int r = nfull * 8; r < nr; ++r) add_row(g * 32 + r, r & 7);
-          } else {
-#pragma unroll
-            for (int r = 0; r < 32; ++r)
-              if ((row_msk >> r) & 1u) add_row(g * 32 + r, r & 7);
+          for (int r = 0; r < 32; ++r) {   // (32g + r) & 7 = r & 7: the row's swizzle phase
+            const uint8_t* src = base + r * 128 + ((chunk16 ^ (r & 7)) << 4);
+            float f = __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(src));
+            if constexpr (kSplit) f += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(src + kStageOutBytes));
+            f = ((row_msk >> r) & 1u) ? f : 0.f;
+            sm += f;
+            sq = fmaf(f, f, sq);
           }
-          const float nt = static_cast<float>(__popc(row_msk));
-          st_dst[0] = st_old[0] + s0;
-          st_dst[1] = st_old[1] + s1;
-          st_dst[p.Cout] = st_old[2] + q0;
-          st_dst[p.Cout + 1] = st_old[3] + q1;
-          st_dst[2 * p.Cout] = st_old[4] + nt;
-          st_dst[2 * p.Cout + 1] = st_old[5] + nt;
+          st_acc[ch][0] += sm;
+          st_acc[ch][1] += sq;
+          if (ch == 0) st_n += static_cast<float>(__popc(row_msk));   // integer-valued: exact
         }
         store_buf ^= 1;
+      }
+      // Flush: one read-modify-write of the CTA's statistics row g when the next item is in another channel tile. A
+      // CTA's items step by gridDim.x, so its consecutive items either always share the channel tile (then the
+      // registers hold the sum over all its tiles, added to the zeroed row once) or never do (then they hold one
+      // tile's sum): either way the fp32 additions are those of a per-tile update of the row, in the same order.
+      const int next = item + gridDim.x;
+      if (stats && (next >= num_items || (next / p.k_slices) % p.n_tiles != n_tile)) {
+        float* st_dst = p.stats_partial + (static_cast<size_t>(blockIdx.x) * 4 + wq) * 3 * p.Cout + n0 + 32 * wg + lane;
+        float old[kChunks][3];
+#pragma unroll
+        for (int ch = 0; ch < kChunks; ++ch)   // all loads first: one global round trip per flush
+          if (n0 + ch * 64 < p.Cout)
+#pragma unroll
+            for (int v = 0; v < 3; ++v) old[ch][v] = st_dst[ch * 64 + v * p.Cout];
+#pragma unroll
+        for (int ch = 0; ch < kChunks; ++ch) {
+          if (n0 + ch * 64 < p.Cout) {
+            st_dst[ch * 64] = old[ch][0] + st_acc[ch][0];
+            st_dst[ch * 64 + p.Cout] = old[ch][1] + st_acc[ch][1];
+            st_dst[ch * 64 + 2 * p.Cout] = old[ch][2] + st_n;
+          }
+          st_acc[ch][0] = st_acc[ch][1] = 0.f;
+        }
+        st_n = 0.f;
       }
     }
     if (ct == 0) tma_store_wait_all<0>();
