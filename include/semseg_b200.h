@@ -22,6 +22,7 @@
  *                               semseg_upsample_ce_ohem_*: the same with an OHEM cross-entropy criterion.
  *                               semseg_upsample_ce_{,ohem_}weighted_*: class weights / label smoothing.
  *                               semseg_upsample_ce_dice_*: soft Dice loss, alone or plus cross-entropy.
+ *                               semseg_upsample_ce_rmi_*: RMI loss with its BCE term, optionally plus cross-entropy.
  *                               semseg_upsample_ce_focal_*: softmax focal loss, with or without class weights.
  *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
@@ -489,6 +490,43 @@ long long semseg_upsample_ce_dice_bwd_workspace_floats(int N, int Ho, int Wo, in
 int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
                                 int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* table,
                                 const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Region Mutual Information loss (Zhao, Wang, Cai, NeurIPS 2019; semseg_b200/losses.py RMILoss) with its sigmoid BCE
+ * term and optionally cross-entropy, on the same fused upsample at zoom `zoom`, in the authors' default configuration
+ * (average pooling 4, radius 3, lambda_way 1, clip 1e-6: fixed). For the upsampled logits z and the target t:
+ *   v = [t != ignore_index and 0 <= t < C],  y_c = [t = c] v,  s_c = sigmoid(z_c),  q_c = s_c v + 1e-6
+ *   BCE = sum_{pixels, c} v (softplus(z_c) - y_c z_c) / (n_valid + 1)
+ *   Y, Q = 4x4 average pools (stride 4, no padding) of y, q: [N][C][Hp][Wp], Hp = Ho / 4, Wp = Wo / 4 (floor)
+ *   a_k, b_k = the 3x3 neighbourhoods (row-major (dy, dx)) of pooled cell k = (i, j), i < Hp-2, j < Wp-2, of Y and Q;
+ *   K = (Hp-2)(Wp-2); centred a~, b~ (fp64): S_aa, S_bb, S_ab = sum_k a~a~', b~b~', a~b~' (9x9, not divided by K)
+ *   P = S_bb + pos_alpha I,  A = S_aa - S_ab P^-1 S_ab',  r[n,c] = 1/2 log det(A + pos_alpha I)   (Cholesky)
+ *   RMI = sum_c ((1/N) sum_n r[n,c]) / 9,   loss = bce_weight BCE + (1 - bce_weight) RMI + ce_weight CE
+ * CE = mean over the valid pixels of lse - z_t (0 with none). 0 <= bce_weight <= 1, pos_alpha finite > 0, ce_weight
+ * finite >= 0, Ho and Wo >= 12. The backward's rows kernel stages 8 bytes per pixel: Wo <= 229376 / (8 zoom), i.e.
+ * 3584 at zoom 8; wider targets are rejected before any launch.
+ *   fwd: loss_out fp32 [5] = (loss, n_valid, BCE, RMI, CE); argmax (or NULL) and lse as the zoom forward's (the same
+ *        bits); pooled fp32 [2][N][C][Hp][Wp] = Y then Q (kept for the backward: 2 N C Hp Wp floats, 268 MB at
+ *        16 x 150 x 473^2); table fp32 [semseg_upsample_ce_rmi_table_floats()] = per (n, c) a 184-float record
+ *        (T [9][18] = [G_ab' | 2 G_bb] row-major, mean a [9], mean b [9], r, 3 zeros), then 4 scalars for the backward
+ *        (ce_weight / n_valid, 1, bce_weight / (n_valid + 1), (1 - bce_weight) / (144 N)); written on the device:
+ *        graph-capturable. workspace: semseg_upsample_ce_rmi_workspace_floats() floats, 8-byte aligned: the raw fp64
+ *        moment sums [N*C][189] first (sum a[9], sum b[9], a a' upper triangle row-major [45], b b' the same [45],
+ *        a b' [9][9]), then r fp64 [N*C], then the CE and BCE partials.
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits from the forward's lse, pooled maps and table, with
+ *        G_ab = -M S_ab P^-1, G_bb = 1/2 P^-1 S_ab' M S_ab P^-1, M = (A + pos_alpha I)^-1; workspace:
+ *        semseg_upsample_ce_rmi_bwd_workspace_floats() floats (the transpose-upsample rows, then dr/dQ [N][C][Hp][Wp]).
+ * Both reject a bad shape, zoom, option, width, null pointer or misalignment before any CUDA call; the workspace
+ * functions return -1 for a zoom outside {1, 2, 4, 8}. */
+long long semseg_upsample_ce_rmi_workspace_floats(int N, int Ho, int Wo, int C, int zoom);
+long long semseg_upsample_ce_rmi_table_floats(int N, int C);
+int semseg_upsample_ce_rmi_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                               int Ho, int Wo, int zoom, int ignore_index, float bce_weight, float pos_alpha,
+                               float ce_weight, float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                               float* pooled, float* table, void* stream);
+long long semseg_upsample_ce_rmi_bwd_workspace_floats(int N, int Ho, int Wo, int w, int C, int zoom);
+int semseg_upsample_ce_rmi_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                               int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* pooled,
+                               const float* table, const float* grad_out, float* workspace, float* dlogits,
+                               void* stream);
 /* Softmax focal loss (Lin et al., ICCV 2017; semseg_b200/losses.py FocalLoss) on the same fused upsample at zoom
  * `zoom`. class_weight fp32 [C] on the device (NULL = all ones; read at every launch, so a CUDA graph sees in-place
  * edits), gamma finite and >= 0. Per valid pixel (target != ignore_index, 0 <= target < C), with p = softmax(v),

@@ -208,6 +208,13 @@ SIGNATURES = {
     "semseg_upsample_ce_dice_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_dice_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_rmi_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_rmi_table_floats": (c_ll, [c_int, c_int]),
+    "semseg_upsample_ce_rmi_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                           c_f, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_rmi_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_rmi_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                           c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_upsample_ce_focal_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_focal_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                              c_vp, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),

@@ -39,6 +39,9 @@
 // radix sort of csrc/segsort.cu and its own scan and gradient kernels (see "Lovász-Softmax" below); no existing
 // instance changes.
 //
+// The RMI loss with its BCE term, optionally plus cross-entropy, runs the plain forward instance and its own pool, moment,
+// algebra and gradient kernels (see "RMI" below); no existing instance changes.
+//
 // The softmax focal loss, with or without class weights, runs sibling forward and rows kernels (see "focal loss" below)
 // with the plain reduce and cols kernels; no existing instance changes.
 //
@@ -1995,6 +1998,484 @@ upsample_pl_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* _
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- RMI
+// Region Mutual Information loss (Zhao, Wang, Cai, NeurIPS 2019) with its sigmoid BCE term and ce_weight * CE, in the
+// authors' default configuration, fixed here: average pooling 4 (stride 4, no padding), radius 3, lambda_way 1, clip
+// 1e-6. With v = [t valid], y_c = [t = c] v, s = sigmoid(z), q = s v + 1e-6, Y / Q the 4x4 average pools of y / q
+// (Hp = Ho / 4, Wp = Wo / 4), a_k / b_k the 3x3 neighbourhoods of pooled cell k of Y / Q (K = (Hp-2)(Wp-2)), centred:
+//   S_aa, S_bb, S_ab = sums over k of a~a~', b~b~', a~b~'    P = S_bb + alpha I    A = S_aa - S_ab P^-1 S_ab'
+//   r[n,c] = 1/2 log det(A + alpha I),   RMI = sum_{n,c} r / (9N),   BCE = sum v (softplus(z) - y z) / (n_valid + 1)
+//   loss = bce_weight BCE + (1 - bce_weight) RMI + ce_weight CE
+// Backward, M = (A + alpha I)^-1, X = S_ab P^-1: G_ab = -M X, G_bb = 1/2 X' M X, dr/db_k = G_ab' a~_k + 2 G_bb b~_k,
+// dr/dQ[cell] = sum over the 9 offsets d with k = cell - d in range of (dr/db_k)[d], and per valid pixel
+//   dL/dz_c = (1 - bce_weight)/(9N) [pooled] s(1-s)/16 dr/dQ + bce_weight (s - y_c)/(n_valid + 1) + ce_weight/n_valid (p_c - y_c)
+// Chain:
+//   forward : the plain forward instance (lse, argmax, CE partials); rmi_pool (the upsampled logits of a band of whole
+//             pooled rows, one thread per output column: the pooled Y and Q maps and BCE partials, the 16 values of a
+//             cell summed in registers and over 4 lanes in a fixed order); rmi_moments (one CTA per (n, c) and moment
+//             group, fp64 sums over the cells, a fixed-order tree); rmi_algebra (one thread per (n, c), the 9x9 fp64
+//             Cholesky algebra: r and the [G_ab' | 2 G_bb] table); rmi_loss (one CTA, fp64, fixed order).
+//   backward: rmi_dq (dr/dQ per pooled cell from the table and the pooled maps), the rows kernel (one thread per class,
+//             (lse, t) staged per pixel, the pixel terms above), then the plain cols kernel.
+// No float atomics, no host synchronisation.
+constexpr float kRmiClip = 1e-6f;
+constexpr int kRmiMoments = 189;   // sum Y[9], sum Q[9], YY upper triangle [45], QQ upper triangle [45], YQ [9][9]
+constexpr int kRmiRec = 184;       // table record per (n, c): T[9][18] = [G_ab' | 2 G_bb], mean Y[9], mean Q[9], r, pad
+constexpr int kRmiRecUsed = 181;
+constexpr int kRmiGroups = 5;      // moment groups: Y (sums, YY), Q (sums, QQ), YQ rows 0-2, 3-5, 6-8
+constexpr float kLn2 = 0.6931471805599453f;
+
+// A CTA of the pool kernel: whole pooled rows (4 output rows; 8, one interval, at Z = 8) and kCols output columns.
+template <int Z>
+struct RmiBand {
+  static constexpr int kRows = Z < 4 ? 4 : Z;
+  static constexpr int kCols = Z == 1 ? 32 : Z == 2 ? 64 : 128;
+  static constexpr int kNodeRows = Z == 1 ? 4 : kRows / Z + 1;
+  static constexpr int kNodes = kCols / Z + 1;
+};
+
+// e = exp(-|v|), rr = 1 / (1 + e): sigmoid(v) = (v >= 0 ? 1 : e) rr, sigmoid'(v) = e rr^2, softplus(v) = max(v, 0) + log(1 + e)
+__device__ __forceinline__ float rmi_exp_neg_abs(float v) { return ex2_approx(-fabsf(v) * kLog2e); }
+
+template <int Z>
+__global__ void __launch_bounds__(RmiBand<Z>::kCols)
+rmi_pool_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
+                const long long* __restrict__ target, int Ho, int Wo, int ignore_index, float* __restrict__ pooled,
+                float* __restrict__ partial) {
+  using G = Zoom<Z>;
+  using B = RmiBand<Z>;
+  constexpr int kPr = B::kRows / 4;   // pooled rows per band
+  extern __shared__ float S[];        // [kNodeRows][kNodes][Cs]
+  __shared__ float red[B::kCols / 32];
+  const int n = blockIdx.z, y0 = blockIdx.y * B::kRows, x0 = blockIdx.x * B::kCols;
+  const int ib = y0 >> G::kShift;
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(B::kNodes, w - j_base);
+  const int tid = threadIdx.x;
+  for (int idx = tid; idx < B::kNodeRows * nj * C; idx += B::kCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * B::kNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + min(ib + rr, h - 1)) * w + (j_base + jj)) * pitch + c];
+  }
+  __syncthreads();
+  const int Hp = Ho >> 2, Wp = Wo >> 2;
+  const int x = x0 + tid;
+  const int xs = min(x, Wo - 1);   // lanes past the image compute a real column; their cells are never written
+  const int j0 = xs >> G::kShift;
+  const int j1 = min(j0 + 1, w - 1);
+  const float l1w = static_cast<float>(xs & G::kMask) * G::kStep, l0w = 1.f - l1w;
+  const float* A = S + (j0 - j_base) * Cs;
+  const float* Bn = S + (j1 - j_base) * Cs;
+  int tg[B::kRows];   // target class per row, -1 where not valid
+#pragma unroll
+  for (int r = 0; r < B::kRows; ++r) {
+    tg[r] = -1;
+    if (x < Wo && y0 + r < Ho) {
+      const long long t = target[(static_cast<size_t>(n) * Ho + (y0 + r)) * Wo + x];
+      if (t != ignore_index && t >= 0 && t < C) tg[r] = static_cast<int>(t);
+    }
+  }
+  const int pc = x >> 2;
+  const bool writer = (tid & 3) == 0 && pc < Wp;
+  float bce = 0.f;
+  for (int c = 0; c < C; ++c) {
+    float hv[B::kNodeRows];
+#pragma unroll
+    for (int k = 0; k < B::kNodeRows; ++k) {
+      hv[k] = Z == 1 ? A[k * B::kNodes * Cs + c] : l0w * A[k * B::kNodes * Cs + c] + l1w * Bn[k * B::kNodes * Cs + c];
+    }
+    float qs[kPr], ys[kPr];
+#pragma unroll
+    for (int p = 0; p < kPr; ++p) qs[p] = ys[p] = 0.f;
+#pragma unroll
+    for (int r = 0; r < B::kRows; ++r) {
+      float v;
+      if constexpr (Z == 1) {
+        v = hv[r];
+      } else {
+        v = row_lerp<Z>(hv[r >> G::kShift], hv[(r >> G::kShift) + 1], r & G::kMask);
+      }
+      float q = kRmiClip;
+      if (tg[r] >= 0) {
+        const float e = rmi_exp_neg_abs(v);
+        const float rr = __fdividef(1.f, 1.f + e);
+        q += (v >= 0.f ? 1.f : e) * rr;
+        bce += fmaxf(v, 0.f) + kLn2 * lg2_approx(1.f + e) - (tg[r] == c ? v : 0.f);
+        if (tg[r] == c) ys[r >> 2] += 1.f;
+      }
+      qs[r >> 2] += q;
+    }
+#pragma unroll
+    for (int p = 0; p < kPr; ++p) {
+      qs[p] += __shfl_xor_sync(0xffffffffu, qs[p], 1);
+      qs[p] += __shfl_xor_sync(0xffffffffu, qs[p], 2);
+      ys[p] += __shfl_xor_sync(0xffffffffu, ys[p], 1);
+      ys[p] += __shfl_xor_sync(0xffffffffu, ys[p], 2);
+      const int pr = (y0 >> 2) + p;
+      if (writer && pr < Hp) {
+        const size_t cell = static_cast<size_t>(pr) * Wp + pc;
+        const size_t plane = static_cast<size_t>(Hp) * Wp;
+        pooled[(static_cast<size_t>(n) * C + c) * plane + cell] = ys[p] * (1.f / 16.f);
+        pooled[((static_cast<size_t>(N) + n) * C + c) * plane + cell] = qs[p] * (1.f / 16.f);
+      }
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) bce += __shfl_xor_sync(0xffffffffu, bce, o);
+  if ((tid & 31) == 0) red[tid >> 5] = bce;
+  __syncthreads();
+  if (tid == 0) {
+    float s = 0.f;
+    for (int i = 0; i < B::kCols / 32; ++i) s += red[i];
+    partial[(static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = s;
+  }
+}
+
+// One CTA per (n, c) and moment group g: g = 0 / 1 the sums and upper-triangle products of the Y / Q neighbourhoods,
+// g = 2..4 the Y x Q products of neighbourhood rows 3(g-2)..3(g-2)+2. Each thread sums its cells (stride 256) in fp64
+// (the fp32 products are exact), then a fixed xor tree per warp and the 8 warps in order. Raw, uncentred sums.
+__global__ void __launch_bounds__(256)
+rmi_moments_kernel(const float* __restrict__ pooled, int NC, int Hp, int Wp, double* __restrict__ mom) {
+  const int nc = blockIdx.x, g = blockIdx.y;
+  const size_t plane = static_cast<size_t>(Hp) * Wp;
+  const float* Y = pooled + static_cast<size_t>(nc) * plane;
+  const float* Q = pooled + (static_cast<size_t>(NC) + nc) * plane;
+  const int Wk = Wp - 2, K = (Hp - 2) * Wk;
+  double acc[54];
+#pragma unroll
+  for (int m = 0; m < 54; ++m) acc[m] = 0.0;
+  if (g < 2) {
+    const float* M = g == 0 ? Y : Q;
+    for (int k = threadIdx.x; k < K; k += 256) {
+      const float* P = M + static_cast<size_t>(k / Wk) * Wp + k % Wk;
+      double a[9];
+#pragma unroll
+      for (int d = 0; d < 9; ++d) a[d] = P[(d / 3) * Wp + d % 3];
+      int idx = 9;
+#pragma unroll
+      for (int d1 = 0; d1 < 9; ++d1) {
+        acc[d1] += a[d1];
+#pragma unroll
+        for (int d2 = d1; d2 < 9; ++d2) {
+          acc[idx] = fma(a[d1], a[d2], acc[idx]);
+          ++idx;
+        }
+      }
+    }
+  } else {
+    const int dy = g - 2;
+    for (int k = threadIdx.x; k < K; k += 256) {
+      const size_t base = static_cast<size_t>(k / Wk) * Wp + k % Wk;
+      double a[3], b[9];
+#pragma unroll
+      for (int d = 0; d < 3; ++d) a[d] = Y[base + dy * Wp + d];
+#pragma unroll
+      for (int d = 0; d < 9; ++d) b[d] = Q[base + (d / 3) * Wp + d % 3];
+#pragma unroll
+      for (int d1 = 0; d1 < 3; ++d1) {
+#pragma unroll
+        for (int d2 = 0; d2 < 9; ++d2) acc[d1 * 9 + d2] = fma(a[d1], b[d2], acc[d1 * 9 + d2]);
+      }
+    }
+  }
+  __shared__ double red[8][54];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int m = 0; m < 54; ++m) {
+    double v = acc[m];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) red[warp][m] = v;
+  }
+  __syncthreads();
+  const int cnt = g < 2 ? 54 : 27;
+  if (threadIdx.x < cnt) {
+    const int m = threadIdx.x;
+    double s = 0.0;
+    for (int i = 0; i < 8; ++i) s += red[i][m];
+    int o;
+    if (g < 2) {
+      o = m < 9 ? 9 * g + m : 18 + 45 * g + (m - 9);
+    } else {
+      o = 108 + 27 * (g - 2) + m;
+    }
+    mom[static_cast<size_t>(nc) * kRmiMoments + o] = s;
+  }
+}
+
+// In-place lower Cholesky factor of the symmetric 9x9 matrix a (row-major; the upper triangle is left stale).
+__device__ __forceinline__ void rmi_chol9(double* a) {
+  for (int j = 0; j < 9; ++j) {
+    double d = a[j * 9 + j];
+    for (int k = 0; k < j; ++k) d -= a[j * 9 + k] * a[j * 9 + k];
+    d = sqrt(d);
+    a[j * 9 + j] = d;
+    for (int i = j + 1; i < 9; ++i) {
+      double s = a[i * 9 + j];
+      for (int k = 0; k < j; ++k) s -= a[i * 9 + k] * a[j * 9 + k];
+      a[i * 9 + j] = s / d;
+    }
+  }
+}
+
+// x = (L L')^-1 b for the lower Cholesky factor L of rmi_chol9.
+__device__ __forceinline__ void rmi_solve9(const double* L, const double* b, double* x) {
+  for (int i = 0; i < 9; ++i) {
+    double s = b[i];
+    for (int k = 0; k < i; ++k) s -= L[i * 9 + k] * x[k];
+    x[i] = s / L[i * 9 + i];
+  }
+  for (int i = 8; i >= 0; --i) {
+    double s = x[i];
+    for (int k = i + 1; k < 9; ++k) s -= L[k * 9 + i] * x[k];
+    x[i] = s / L[i * 9 + i];
+  }
+}
+
+// One thread per (n, c): the centred 9x9 moments from the raw sums, the Cholesky algebra in fp64, r into rterm and the
+// table record (fp32): T[d][e] = G_ab'[d][e], T[d][9 + e] = 2 G_bb[d][e], mean Y, mean Q, r.
+__global__ void __launch_bounds__(64)
+rmi_algebra_kernel(const double* __restrict__ mom, int NC, int K, float alpha, float* __restrict__ table,
+                   double* __restrict__ rterm) {
+  const int nc = blockIdx.x * 64 + threadIdx.x;
+  if (nc >= NC) return;
+  const double* m = mom + static_cast<size_t>(nc) * kRmiMoments;
+  const double invK = 1.0 / K, al = alpha;
+  double Saa[81], P[81], Sab[81], X[81], MX[81];
+  int ia = 18, ib = 63;
+  for (int d1 = 0; d1 < 9; ++d1) {
+    for (int d2 = d1; d2 < 9; ++d2) {
+      Saa[d1 * 9 + d2] = Saa[d2 * 9 + d1] = m[ia++] - m[d1] * m[d2] * invK;
+      P[d1 * 9 + d2] = P[d2 * 9 + d1] = m[ib++] - m[9 + d1] * m[9 + d2] * invK + (d1 == d2 ? al : 0.0);
+    }
+    for (int d2 = 0; d2 < 9; ++d2) Sab[d1 * 9 + d2] = m[108 + d1 * 9 + d2] - m[d1] * m[9 + d2] * invK;
+  }
+  rmi_chol9(P);
+  for (int d = 0; d < 9; ++d) rmi_solve9(P, Sab + d * 9, X + d * 9);   // X = S_ab P^-1 (P symmetric)
+  double* Am = Saa;                                                  // A + alpha I, in place of S_aa
+  for (int i = 0; i < 9; ++i) {
+    for (int j = i; j < 9; ++j) {
+      double s = Saa[i * 9 + j];
+      for (int e = 0; e < 9; ++e) s -= X[i * 9 + e] * Sab[j * 9 + e];
+      Am[i * 9 + j] = Am[j * 9 + i] = s + (i == j ? al : 0.0);
+    }
+  }
+  rmi_chol9(Am);
+  double r = 0.0;
+  for (int i = 0; i < 9; ++i) r += log(Am[i * 9 + i]);
+  double col[9], sol[9];
+  for (int e = 0; e < 9; ++e) {   // MX = (A + alpha I)^-1 X, column by column
+    for (int i = 0; i < 9; ++i) col[i] = X[i * 9 + e];
+    rmi_solve9(Am, col, sol);
+    for (int i = 0; i < 9; ++i) MX[i * 9 + e] = sol[i];
+  }
+  float* T = table + static_cast<size_t>(nc) * kRmiRec;
+  for (int d = 0; d < 9; ++d) {
+    for (int e = 0; e < 9; ++e) {
+      double gbb = 0.0;
+      for (int i = 0; i < 9; ++i) gbb += X[i * 9 + d] * MX[i * 9 + e];
+      T[d * 18 + e] = static_cast<float>(-MX[e * 9 + d]);
+      T[d * 18 + 9 + e] = static_cast<float>(gbb);
+    }
+    T[162 + d] = static_cast<float>(m[d] * invK);
+    T[171 + d] = static_cast<float>(m[9 + d] * invK);
+  }
+  T[180] = static_cast<float>(r);
+  for (int i = kRmiRecUsed; i < kRmiRec; ++i) T[i] = 0.f;
+  rterm[nc] = r;
+}
+
+// One CTA: CE, BCE and sum r in fp64, fixed order -> loss_out = (loss, n_valid, BCE, RMI, CE) and the backward's
+// scalars sc = (ce_weight / n_valid, 1, bce_weight / (n_valid + 1), (1 - bce_weight) / (144 N)).
+__global__ void __launch_bounds__(256)
+rmi_loss_kernel(const float* __restrict__ ce_partial, int nce, const float* __restrict__ bce_partial, int nbce,
+                const double* __restrict__ rterm, int NC, int N, float bce_weight, float ce_weight,
+                float* __restrict__ loss_out, float* __restrict__ sc) {
+  __shared__ double red[4][256];
+  double l = 0.0, k = 0.0, b = 0.0, r = 0.0;
+  for (int i = threadIdx.x; i < nce; i += 256) {
+    l += ce_partial[2 * i];
+    k += ce_partial[2 * i + 1];
+  }
+  for (int i = threadIdx.x; i < nbce; i += 256) b += bce_partial[i];
+  for (int i = threadIdx.x; i < NC; i += 256) r += rterm[i];
+  red[0][threadIdx.x] = l;
+  red[1][threadIdx.x] = k;
+  red[2][threadIdx.x] = b;
+  red[3][threadIdx.x] = r;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) red[j][threadIdx.x] += red[j][threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const double nv = red[1][0];
+    const double ce = nv > 0.0 ? red[0][0] / nv : 0.0;
+    const double bce = red[2][0] / (nv + 1.0);
+    const double rmi = red[3][0] / (9.0 * N);
+    const double bw = bce_weight;
+    loss_out[0] = static_cast<float>(bw * bce + (1.0 - bw) * rmi + static_cast<double>(ce_weight) * ce);
+    loss_out[1] = static_cast<float>(nv);
+    loss_out[2] = static_cast<float>(bce);
+    loss_out[3] = static_cast<float>(rmi);
+    loss_out[4] = static_cast<float>(ce);
+    sc[0] = nv > 0.0 ? static_cast<float>(ce_weight / nv) : 0.f;
+    sc[1] = 1.f;
+    sc[2] = static_cast<float>(bw / (nv + 1.0));
+    sc[3] = static_cast<float>((1.0 - bw) / (144.0 * N));
+  }
+}
+
+// dr/dQ per pooled cell: one thread per cell of one (n, c) (blockIdx.x), the 5x5 patch of Y and Q around the cell in
+// registers, the table record in shared memory; sum over the neighbourhoods k = cell - d that exist.
+__global__ void __launch_bounds__(256)
+rmi_dq_kernel(const float* __restrict__ pooled, int NC, int Hp, int Wp, const float* __restrict__ table,
+              float* __restrict__ dq) {
+  __shared__ float s_t[kRmiRecUsed];
+  const int nc = blockIdx.x;
+  for (int i = threadIdx.x; i < kRmiRecUsed; i += 256) s_t[i] = table[static_cast<size_t>(nc) * kRmiRec + i];
+  __syncthreads();
+  const int cell = blockIdx.y * 256 + threadIdx.x;
+  if (cell >= Hp * Wp) return;
+  const size_t plane = static_cast<size_t>(Hp) * Wp;
+  const float* Y = pooled + static_cast<size_t>(nc) * plane;
+  const float* Q = pooled + (static_cast<size_t>(NC) + nc) * plane;
+  const int i = cell / Wp, j = cell % Wp;
+  float yv[25], qv[25];
+#pragma unroll
+  for (int p = 0; p < 25; ++p) {
+    const int yi = i + p / 5 - 2, xj = j + p % 5 - 2;
+    const bool in = yi >= 0 && yi < Hp && xj >= 0 && xj < Wp;
+    yv[p] = in ? Y[static_cast<size_t>(yi) * Wp + xj] : 0.f;
+    qv[p] = in ? Q[static_cast<size_t>(yi) * Wp + xj] : 0.f;
+  }
+  float g = 0.f;
+#pragma unroll
+  for (int d = 0; d < 9; ++d) {
+    const int ki = i - d / 3, kj = j - d % 3;
+    if (ki < 0 || ki >= Hp - 2 || kj < 0 || kj >= Wp - 2) continue;
+#pragma unroll
+    for (int e = 0; e < 9; ++e) {
+      const int p = (e / 3 - d / 3 + 2) * 5 + (e % 3 - d % 3 + 2);
+      g = fmaf(s_t[d * 18 + e], yv[p] - s_t[162 + e], g);
+      g = fmaf(s_t[d * 18 + 9 + e], qv[p] - s_t[171 + e], g);
+    }
+  }
+  dq[static_cast<size_t>(nc) * plane + cell] = g;
+}
+
+// One interval of the RMI rows kernel for class c: the (left, right) x (top, bottom node row) gradient sums as in
+// upsample_ce_bwd_rows_kernel, of the pixel terms in the RMI comment above.
+// The interval's Z x Z pixels lie in kRmiCells x kRmiCells pooled cells (Z = 8: 2 x 2; Z <= 4: one, since y0 and xb are
+// multiples of Z): their kr dr/dQ are loaded once per interval, 0 for cells outside the pooled map.
+template <int Z>
+constexpr int kRmiCells = Z == 8 ? 2 : 1;
+
+template <int Z, bool kFull>
+__device__ __forceinline__ void rmi_interval(const PixInfo* s, int Wo, int xb, int y0, int rows, int nx, int c,
+                                             float a, float b, float cc, float d, const float* __restrict__ dqc,
+                                             int Hp, int Wp, float kce, float kbce, float kr, float* acc) {
+  using G = Zoom<Z>;
+  constexpr int kCells = kRmiCells<Z>;
+  float dqv[kCells][kCells];
+#pragma unroll
+  for (int u = 0; u < kCells; ++u) {
+#pragma unroll
+    for (int v = 0; v < kCells; ++v) {
+      const int cy = (y0 >> 2) + u, cx = (xb >> 2) + v;
+      dqv[u][v] = cy < Hp && cx < Wp ? kr * __ldg(dqc + static_cast<size_t>(cy) * Wp + cx) : 0.f;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const PixInfo pi = s[r * Wo + xb + k];
+      if (pi.t < 0) continue;  // warp-uniform
+      const float v = row_lerp<Z>(top, bot, r);
+      const float p = ex2_approx(fmaf(v, kLog2e, -pi.lse2));
+      const float e = rmi_exp_neg_abs(v);
+      const float rr = __fdividef(1.f, 1.f + e);
+      const float sg = (v >= 0.f ? 1.f : e) * rr;
+      const float yc = c == pi.t ? 1.f : 0.f;
+      float g = fmaf(kce, p - yc, kbce * (sg - yc));
+      g = fmaf(e * rr * rr, dqv[kCells == 2 ? r >> 2 : 0][kCells == 2 ? k >> 2 : 0], g);
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+// Rows layout of upsample_ce_bwd_rows_kernel (one CTA per (interval row, image), one thread per class, (lse, t) of the
+// interval's Z output rows staged per pixel): T2 of the RMI + BCE + CE gradient; dq = dr/dQ, sc = the loss scalars.
+template <int Z>
+__global__ void __launch_bounds__(256)
+upsample_ce_rmi_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
+                            const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                            const float* __restrict__ lse, const float* __restrict__ dq, const float* __restrict__ sc,
+                            float* __restrict__ T2) {
+  extern __shared__ PixInfo s_rpix[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const long long t = target[rowbase + x];
+      PixInfo pi;
+      pi.t = (t == ignore_index || t < 0 || t >= C) ? -1 : static_cast<int>(t);
+      pi.lse2 = lse[rowbase + x] * kLog2e;
+      s_rpix[r * Wo + x] = pi;
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const float kce = sc[0], kbce = sc[2], kr = sc[3];
+  const int Hp = Ho >> 2, Wp = Wo >> 2;
+  const float* dqc = dq + (static_cast<size_t>(n) * C + c) * Hp * Wp;
+  const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
+  const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  float a = L0[0], cc = L1[0];
+  float nb = L0[static_cast<size_t>(min(1, w - 1)) * pitch], nd = L1[static_cast<size_t>(min(1, w - 1)) * pitch];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd;
+    const int jn = min(j0 + 2, w - 1);
+    nb = L0[static_cast<size_t>(jn) * pitch];
+    nd = L1[static_cast<size_t>(jn) * pitch];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      rmi_interval<Z, true>(s_rpix, Wo, xb, Z * i0, rows, nx, c, a, b, cc, d, dqc, Hp, Wp, kce, kbce, kr, acc);
+    } else {
+      rmi_interval<Z, false>(s_rpix, Wo, xb, Z * i0, rows, nx, c, a, b, cc, d, dqc, Hp, Wp, kce, kbce, kr, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -2495,6 +2976,171 @@ extern "C" int semseg_upsample_ce_dice_bwd(const float* logits, int pitch, int N
                                       workspace, dlogits, stream);
     default: return launch_dice_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, table, grad_out,
                                        workspace, dlogits, stream);
+  }
+}
+
+// RMI loss (+ bce_weight * BCE + ce_weight * CE) at zoom factor `zoom`. The rows kernel stages 8-byte (lse, target)
+// words of the interval's Z output rows in at most 224 KB of shared memory: Wo <= 3584 at zoom 8.
+constexpr size_t kRmiSmemMax = 224 * 1024;
+
+static int check_rmi(int Ho, int Wo, int zoom, float bce_weight, float pos_alpha, float ce_weight) {
+  SB_CHECK_ARG(Ho >= 12 && Wo >= 12, "upsample_ce_rmi: target %dx%d is smaller than 12x12 (3x3 pooled cells)", Ho, Wo);
+  SB_CHECK_ARG(bce_weight >= 0.f && bce_weight <= 1.f, "upsample_ce_rmi: bce_weight %g is not in [0, 1]", bce_weight);
+  SB_CHECK_ARG(std::isfinite(pos_alpha) && pos_alpha > 0.f, "upsample_ce_rmi: pos_alpha %g is not finite and > 0",
+               pos_alpha);
+  SB_CHECK_ARG(std::isfinite(ce_weight) && ce_weight >= 0.f, "upsample_ce_rmi: ce_weight %g is not finite and >= 0",
+               ce_weight);
+  const size_t max_wo = kRmiSmemMax / (static_cast<size_t>(zoom) * sizeof(PixInfo));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_ce_rmi: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  SB_CHECK_ARG(cdiv((Ho / 4) * (Wo / 4), 256) <= 65535, "upsample_ce_rmi: target %dx%d has too many pooled cells", Ho,
+               Wo);
+  return SEMSEG_OK;
+}
+
+static int rmi_pool_ctas(int N, int Ho, int Wo, int zoom) {
+  const int rows = zoom < 4 ? 4 : zoom, cols = zoom == 1 ? 32 : zoom == 2 ? 64 : 128;
+  return cdiv(Wo, cols) * cdiv(Ho, rows) * N;
+}
+
+// Forward workspace (8-byte aligned): the raw moments fp64 [N*C][189], r fp64 [N*C], then the CE partials (2 per
+// forward CTA) and the BCE partials (1 per pool CTA).
+static long long rmi_ws_floats(int N, int Ho, int Wo, int C, int zoom) {
+  const long long nc = static_cast<long long>(N) * C;
+  return 2LL * nc * (kRmiMoments + 1) + 2LL * fwd_ctas(N, (Ho - 1) / zoom + 1, Wo) + rmi_pool_ctas(N, Ho, Wo, zoom);
+}
+
+template <int Z>
+static int launch_rmi_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                          int Wo, int ignore_index, float bce_weight, float pos_alpha, float ce_weight,
+                          float* workspace, float* loss_out, int64_t* argmax, float* lse, float* pooled, float* table,
+                          cudaStream_t stream) {
+  using B = RmiBand<Z>;
+  const int NC = N * C, Hp = Ho / 4, Wp = Wo / 4;
+  double* mom = reinterpret_cast<double*>(workspace);
+  double* rterm = mom + static_cast<size_t>(NC) * kRmiMoments;
+  float* ce_part = reinterpret_cast<float*>(rterm + NC);
+  const int ctas = fwd_ctas(N, h, Wo);
+  float* bce_part = ce_part + 2LL * ctas;
+  int r = launch_fwd_kernel<Z, false>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ce_part, argmax, lse,
+                                      nullptr, nullptr, stream);
+  if (r) return r;
+  const int Cs = C | 1;
+  const size_t smem = static_cast<size_t>(B::kNodeRows) * B::kNodes * Cs * sizeof(float);
+  constexpr size_t kMaxSmem = static_cast<size_t>(B::kNodeRows) * B::kNodes * (kMaxClasses | 1) * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    r = opt_in_smem(rmi_pool_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  const dim3 pgrid(cdiv(Wo, B::kCols), cdiv(Ho, B::kRows), N);
+  rmi_pool_kernel<Z><<<pgrid, B::kCols, smem, stream>>>(logits, pitch, N, h, w, C, Cs,
+                                                        reinterpret_cast<const long long*>(target), Ho, Wo,
+                                                        ignore_index, pooled, bce_part);
+  SB_LAUNCHED();
+  rmi_moments_kernel<<<dim3(NC, kRmiGroups), 256, 0, stream>>>(pooled, NC, Hp, Wp, mom);
+  SB_LAUNCHED();
+  rmi_algebra_kernel<<<cdiv(NC, 64), 64, 0, stream>>>(mom, NC, (Hp - 2) * (Wp - 2), pos_alpha, table, rterm);
+  SB_LAUNCHED();
+  rmi_loss_kernel<<<1, 256, 0, stream>>>(ce_part, ctas, bce_part, static_cast<int>(pgrid.x * pgrid.y * pgrid.z), rterm,
+                                         NC, N, bce_weight, ce_weight, loss_out,
+                                         table + static_cast<size_t>(NC) * kRmiRec);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+// Backward workspace: T2 [N][h][2][w][C] of the rows kernel, then dr/dQ [N][C][Hp][Wp].
+template <int Z>
+static int launch_rmi_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                          int Wo, int ignore_index, const float* lse, const float* pooled, const float* table,
+                          const float* grad_out, float* workspace, float* dlogits, cudaStream_t stream) {
+  const int NC = N * C, Hp = Ho / 4, Wp = Wo / 4;
+  float* dq = workspace + 2LL * N * h * w * C;
+  const float* sc = table + static_cast<size_t>(NC) * kRmiRec;
+  rmi_dq_kernel<<<dim3(NC, cdiv(Hp * Wp, 256)), 256, 0, stream>>>(pooled, NC, Hp, Wp, table, dq);
+  SB_LAUNCHED();
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(PixInfo);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_rmi_rows_kernel<Z>, attr_set, static_cast<int>(kRmiSmemMax));
+    if (r) return r;
+  }
+  upsample_ce_rmi_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, dq, sc,
+      workspace);
+  SB_LAUNCHED();
+  // sc[1] = 1: the plain cols kernel's count, so dlogits = grad_out[0] * T2 sums
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, sc, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_rmi_workspace_floats(int N, int Ho, int Wo, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_rmi: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && C > 0, "upsample_ce_rmi: bad sizes");
+  return rmi_ws_floats(N, Ho, Wo, C, zoom);
+}
+
+extern "C" long long semseg_upsample_ce_rmi_table_floats(int N, int C) {
+  SB_CHECK_ARG(N > 0 && C > 0, "upsample_ce_rmi: bad sizes");
+  return static_cast<long long>(N) * C * kRmiRec + 4;
+}
+
+extern "C" int semseg_upsample_ce_rmi_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                          const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                          float bce_weight, float pos_alpha, float ce_weight, float* workspace,
+                                          float* loss_out, int64_t* argmax, float* lse, float* pooled, float* table,
+                                          void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_rmi(Ho, Wo, zoom, bce_weight, pos_alpha, ce_weight);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && pooled && table, "upsample_ce_rmi_fwd: null output");
+  SB_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "upsample_ce_rmi_fwd: workspace not 8-byte aligned");
+  SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(pooled) | reinterpret_cast<uintptr_t>(table)) & 3) == 0,
+               "upsample_ce_rmi_fwd: pooled or table not 4-byte aligned");
+  switch (zoom) {
+    case 1: return launch_rmi_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, bce_weight, pos_alpha,
+                                     ce_weight, workspace, loss_out, argmax, lse, pooled, table, stream);
+    case 2: return launch_rmi_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, bce_weight, pos_alpha,
+                                     ce_weight, workspace, loss_out, argmax, lse, pooled, table, stream);
+    case 4: return launch_rmi_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, bce_weight, pos_alpha,
+                                     ce_weight, workspace, loss_out, argmax, lse, pooled, table, stream);
+    default: return launch_rmi_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, bce_weight, pos_alpha,
+                                      ce_weight, workspace, loss_out, argmax, lse, pooled, table, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_rmi_bwd_workspace_floats(int N, int Ho, int Wo, int w, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_rmi: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && w > 0 && C > 0, "upsample_ce_rmi: bad sizes");
+  return 2LL * N * ((Ho - 1) / zoom + 1) * w * C + static_cast<long long>(N) * C * (Ho / 4) * (Wo / 4);
+}
+
+extern "C" int semseg_upsample_ce_rmi_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                          const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                          const float* lse, const float* pooled, const float* table,
+                                          const float* grad_out, float* workspace, float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_rmi(Ho, Wo, zoom, 0.f, 1.f, 0.f);
+  if (r) return r;
+  SB_CHECK_ARG(lse && pooled && table && grad_out && workspace && dlogits, "upsample_ce_rmi_bwd: null pointer");
+  SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(pooled) | reinterpret_cast<uintptr_t>(table)) & 3) == 0,
+               "upsample_ce_rmi_bwd: pooled or table not 4-byte aligned");
+  switch (zoom) {
+    case 1: return launch_rmi_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, pooled, table,
+                                     grad_out, workspace, dlogits, stream);
+    case 2: return launch_rmi_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, pooled, table,
+                                     grad_out, workspace, dlogits, stream);
+    case 4: return launch_rmi_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, pooled, table,
+                                     grad_out, workspace, dlogits, stream);
+    default: return launch_rmi_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, pooled, table,
+                                      grad_out, workspace, dlogits, stream);
   }
 }
 

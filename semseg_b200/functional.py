@@ -709,6 +709,26 @@ class _UpsampleCEPLMix(_UpsampleCEPL):
         return _UpsampleCEPL.backward(ctx, grad_loss, grad_amax) + (None,)
 
 
+class _UpsampleCERMI(torch.autograd.Function):
+    """The fused tail with losses.RMILoss: RMI + BCE (+ CE) over the call. The forward keeps the pooled Y / Q maps and
+    the per-(image, class) gradient table it computed on the device; the backward needs nothing else from the host."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, bce_weight, pos_alpha, ce_weight):
+        info, amax, lse, pooled, table = ops.upsample_ce_rmi_fwd(logits, target, ignore_index, bce_weight, pos_alpha,
+                                                                 ce_weight, zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, pooled, table)
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, pooled, table = ctx.saved_tensors
+        dl = ops.upsample_ce_rmi_bwd(logits, target, ctx.ignore_index, lse, pooled, table, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None, None
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""
@@ -721,6 +741,9 @@ def _class_weight_supported(weight, target, classes):
 # The Dice rows kernels stage 12 bytes per pixel of an interval's Z output rows in at most 224 KB of shared memory
 # (csrc/tail.cu kDiceSmemMax): Wo <= 2389 at zoom 8.
 _DICE_PIXEL_BYTES, _DICE_STAGE_BYTES = 12, 224 * 1024
+# The RMI rows kernel stages 8 bytes per pixel in the same 224 KB (Wo <= 3584 at zoom 8); RMI needs a target of at least
+# 12 x 12, three pooled cells each way.
+_RMI_PIXEL_BYTES, _RMI_MIN_SIZE = 8, 12
 
 
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
@@ -732,7 +755,8 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     ATen tail. DiceLoss, FocalLoss and losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
     form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, the Dice
-    width limit.
+    width limit. losses.RMILoss needs a target of at least 12 x 12 and no wider than its rows kernel stages (3584 columns
+    at zoom 8).
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
         ok = True
@@ -745,6 +769,10 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         # the focal rows kernel (the pseudo-label backward too) stages the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
+    elif type(criterion) is losses.RMILoss:
+        ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
+              target.shape[1] >= _RMI_MIN_SIZE and target.shape[2] >= _RMI_MIN_SIZE and
+              _RMI_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     elif type(criterion) is losses.LovaszSoftmaxLoss:
         # the Lovász rows kernel stages the Dice words; its sort payloads hold a pixel index in 31 bits
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
@@ -771,7 +799,8 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
     weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
-    with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index); with a losses.LovaszSoftmaxLoss, its
+    with a losses.DiceLoss, its Dice (+ CE) loss (its own ignore_index); with a losses.RMILoss, its RMI + BCE (+ CE)
+    loss; with a losses.LovaszSoftmaxLoss, its
     Lovász-Softmax (+ CE) loss; with a losses.FocalLoss, its focal loss (its own ignore_index, gamma and class
     weights); with a losses.DistillationLoss and the teacher's fp32 NHWC logits `teacher_logits`
     (the student's shape), its distillation loss, and with a losses.PseudoLabelLoss and them its pseudo-label loss
@@ -798,6 +827,9 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
                                           criterion.gamma)
         return _UpsampleCEFocal.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.gamma,
                                       criterion.weight)
+    if isinstance(criterion, losses.RMILoss):
+        return _UpsampleCERMI.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.bce_weight,
+                                    criterion.pos_alpha, criterion.ce_weight)
     if isinstance(criterion, losses.DiceLoss):
         return _UpsampleCEDice.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.smooth,
                                      criterion.eps, criterion.ce_weight)

@@ -19,7 +19,7 @@ Limits (same as torch.cuda.make_graphed_callables): a second training forward be
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
-loss, the focal loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
+loss, the focal loss, the RMI loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
 mean teacher's re-pack included, and the CutMix / ClassMix pseudo-label loss, its draws and mixing included, with or
 without a strong view of the student's input) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
@@ -306,13 +306,15 @@ def train_step(model, impl, x, y):
     bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
     # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
     # the criterion's options are launch arguments baked into the graph: a changed thresh, ignore_index,
-    # label_smoothing, Dice smooth / eps / ce_weight, Lovász classes / per_image or focal gamma captures anew, and so
+    # label_smoothing, Dice smooth / eps / ce_weight, Lovász classes / per_image, focal gamma or RMI bce_weight /
+    # pos_alpha captures anew, and so
     # does a replaced class-weight tensor (its address is baked in); an in-place edit of the weights needs no capture,
     # the kernels read them at every replay
     crit = getattr(model, "criterion", None)
     crit_key = (type(crit),) + tuple(getattr(crit, a, None) for a in ("ignore_index", "thresh", "min_kept",
                                                                       "label_smoothing", "reduction", "smooth", "eps",
-                                                                      "ce_weight", "classes", "per_image", "gamma"))
+                                                                      "ce_weight", "classes", "per_image", "gamma",
+                                                                      "bce_weight", "pos_alpha"))
     cw = getattr(crit, "weight", None)
     crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
     teacher = _teacher(crit)

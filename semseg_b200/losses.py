@@ -5,7 +5,7 @@ the network's fused tail (functional.upsample_ce) it runs inside the same kernel
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
 LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and FocalLoss, the softmax focal loss with
-optional class weights, run the same way. DistillationLoss adds a
+optional class weights, run the same way, and so does RMILoss, the Region Mutual Information loss with its BCE term. DistillationLoss adds a
 pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
 optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
@@ -570,5 +570,61 @@ class LovaszSoftmaxLoss(nn.Module):
         if logits.dtype != torch.float32 or target.dtype != torch.int64:
             raise TypeError("LovaszSoftmaxLoss: fp32 logits and int64 target expected, got %s and %s" %
                             (logits.dtype, target.dtype))
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+class RMILoss(nn.Module):
+    """Region Mutual Information loss (Zhao, Wang, Cai, "Region Mutual Information Loss for Semantic Segmentation",
+    NeurIPS 2019) with its sigmoid BCE term, optionally plus cross-entropy, for logits z [N, C, H, W] and target
+    t [N, H, W]:
+
+        v      = t != ignore_index and 0 <= t < C          (other targets are not valid, as in DiceLoss)
+        y_c    = [t = c] v,  s_c = sigmoid(z_c),  q_c = s_c v + 1e-6
+        BCE    = sum over pixels and classes of v (softplus(z_c) - y_c z_c) / (n_valid + 1)
+        Y, Q   = avg_pool(y, 4, stride 4), avg_pool(q, 4, stride 4)     (Hp = H // 4, Wp = W // 4, no padding)
+        a_k, b_k = the 3x3 neighbourhoods of pooled cell k of Y and Q (9-vectors), K = (Hp - 2)(Wp - 2) of them
+        S_aa, S_bb, S_ab = sums over k of the centred a a', b b', a b'   (float64, 9x9)
+        r[n,c] = 1/2 log det(S_aa - S_ab (S_bb + pos_alpha I)^-1 S_ab' + pos_alpha I)
+        RMI    = sum over c of (mean over n of r[n,c]) / 9
+        loss   = bce_weight * BCE + (1 - bce_weight) * RMI + ce_weight * CE
+
+    CE is the mean cross-entropy over the valid pixels. The sums run over the pixels of the call (per rank under
+    DistributedDataParallel). Pixels in the last H mod 4 rows and W mod 4 columns reach BCE and CE but not RMI. With no
+    valid pixel BCE is 0, r = 9/2 log(pos_alpha) and every gradient is 0. This is the authors' released code in its
+    default configuration; its pooling (average, 4), radius (3), lambda_way (1) and clip (1e-6) are fixed, which lets
+    the kernels specialise on them.
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, graphed at every zoom
+    factor, without the full-resolution logits; called as a module (validate()) it runs their zoom-1 form on an NHWC
+    copy of the logits. H and W must be at least 12 (three pooled cells). CUDA fp32 logits with at most 256 classes
+    only: there is no CPU or library fallback. The forward keeps 8 C bytes per pooled cell (the pooled Y and Q maps) for
+    the backward."""
+
+    def __init__(self, ignore_index=255, bce_weight=0.5, pos_alpha=5e-4, ce_weight=0.0):
+        super(RMILoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        bce_weight = _non_negative("bce_weight", bce_weight)
+        if bce_weight > 1.0:
+            raise ValueError("bce_weight must lie in [0, 1], got %r" % bce_weight)
+        pos_alpha = _non_negative("pos_alpha", pos_alpha)
+        if pos_alpha <= 0.0:
+            raise ValueError("pos_alpha must be > 0, got %r" % pos_alpha)
+        self.ignore_index = ignore_index
+        self.bce_weight = bce_weight
+        self.pos_alpha = pos_alpha
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+
+    def extra_repr(self):
+        return "ignore_index=%d, bce_weight=%g, pos_alpha=%g, ce_weight=%g" % (self.ignore_index, self.bce_weight,
+                                                                              self.pos_alpha, self.ce_weight)
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        if logits.dim() == 4 and (logits.shape[2] < 12 or logits.shape[3] < 12):
+            raise ValueError("RMILoss: H and W must be at least 12 (three 4x4 pooled cells), got %dx%d" %
+                             (logits.shape[2], logits.shape[3]))
+        _check_native_logits("RMILoss", logits, target)
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
         return loss

@@ -1102,6 +1102,56 @@ def segsort_u32_pairs(keys, vals, skip=None):
     return keys, vals
 
 
+def upsample_ce_rmi_fwd(logits, target, ignore_index, bce_weight, pos_alpha, ce_weight, want_argmax=True, zoom=8,
+                        workspace=None):
+    """RMI loss (+ bce_weight * BCE + ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract);
+    arguments as upsample_ce_fwd plus the RMI options -> (loss_info [5] = (loss, valid count, BCE, RMI, CE), argmax,
+    lse, pooled [2, N, C, Ho/4, Wo/4] = (Y, Q), table [N*C*184 + 4]: per (n, c) [G_ab' | 2 G_bb], the means and r,
+    then the backward's scalars). `workspace` (fp32, at least semseg_upsample_ce_rmi_workspace_floats, 8-byte aligned)
+    lets a caller read the raw fp64 moment sums the kernels leave at its start."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_rmi_workspace_floats(n, ho, wo, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_rmi_workspace_floats")
+    ntab = int(lib.semseg_upsample_ce_rmi_table_floats(n, c))
+    _lib.check(0 if ntab >= 0 else ntab, "semseg_upsample_ce_rmi_table_floats")
+    dev = logits.device
+    if workspace is None:
+        workspace = torch.empty((nws,), dtype=torch.float32, device=dev)
+    assert workspace.dtype == torch.float32 and workspace.numel() >= nws and workspace.is_contiguous()
+    info = torch.empty((5,), dtype=torch.float32, device=dev)
+    table = torch.empty((ntab,), dtype=torch.float32, device=dev)
+    pooled = torch.empty((2, n, c, ho // 4, wo // 4), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse = torch.empty((n, ho, wo), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_upsample_ce_rmi_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                              int(zoom), int(ignore_index), float(bce_weight), float(pos_alpha),
+                                              float(ce_weight), _ptr(workspace), _ptr(info), _ptr(amax), _ptr(lse),
+                                              _ptr(pooled), _ptr(table), _stream()),
+               "semseg_upsample_ce_rmi_fwd")
+    return info, amax, lse, pooled, table
+
+
+def upsample_ce_rmi_bwd(logits, target, ignore_index, lse, pooled, table, grad_out, zoom=8):
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_rmi_bwd_workspace_floats(n, ho, wo, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_rmi_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_rmi_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                              int(zoom), int(ignore_index), _ptr(lse), _ptr(pooled), _ptr(table),
+                                              _ptr(g), _ptr(ws), _ptr(dl), _stream()),
+               "semseg_upsample_ce_rmi_bwd")
+    return dl
+
+
 # ------------------------------------------------------------------------------------------------ sliding-window evaluation
 def window_scores(logits, flip, out):
     """fp32 NHWC logits [G (+G mirrored crops when flip), h, w, C] -> flip-averaged softmax scores written into `out`,
