@@ -334,6 +334,16 @@ int semseg_add_act(const void* a, const void* a_lo, int a_pitch, const void* b, 
  * (model/pspnet.py:68,76) and its backward. */
 int semseg_scale_nc(const void* x, const void* x_lo, int x_pitch, const float* scale, void* out, void* out_lo,
                     int out_pitch, int N, int HW, int C, void* stream);
+/* Feature perturbation (UniMatch's FP stream). Fork: x holds N images [N][HW][x_pitch], out 2N [2N][HW][out_pitch];
+ * out[n] = x[n] and out[N + n] = x[n] * scale[n*C + c], each computed in fp32 from x (hi + lo) and stored by the
+ * activation store, so the second half is bit-equal to semseg_scale_nc(x, scale) and scale = 1 gives equal halves.
+ * Fold (its backward): d holds 2N images, out N; out[n] = d[n] + scale[n*C + c] * d[N + n] in fp32 (product and sum
+ * each rounded to nearest, no fma), rounded once to the activation form. Both: C % 8 == 0, pitches multiples of 8 and
+ * at least C, 16-byte aligned bases and scale, one storage form (plain or split) for input and output. */
+int semseg_fp_fork(const void* x, const void* x_lo, int x_pitch, const float* scale, void* out, void* out_lo,
+                   int out_pitch, int N, int HW, int C, void* stream);
+int semseg_fp_fold(const void* d, const void* d_lo, int d_pitch, const float* scale, void* out, void* out_lo,
+                   int out_pitch, int N, int HW, int C, void* stream);
 /* fp32 rows [M][in_pitch] (C columns used) -> activation rows [M][out_pitch], columns C..Cp-1 zero (Cp % 8 == 0). */
 int semseg_f32_to_act(const float* in, int in_pitch, void* out, void* out_lo, int out_pitch, long long M, int C,
                       int Cp, void* stream);

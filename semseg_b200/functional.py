@@ -846,6 +846,17 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     return _UpsampleCE.apply(logits, target.contiguous(), ignore_index, int(zoom))
 
 
+def upsample_fp(logits, target, zoom, criterion, teacher_logits, mix_mask=None):
+    """The feature-perturbation term of a losses.PseudoLabelLoss (or MixPseudoLabelLoss, with the mix mask) whose
+    fp_weight > 0: fp_weight * its pseudo-label term on the perturbed stream's fp32 NHWC logits, with no labelled term.
+    It is the pseudo-label tail of upsample_ce with ce_weight 0 and pl_weight = fp_weight -> (loss, argmax)."""
+    args = (logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index, int(zoom), criterion.threshold,
+            criterion.fp_weight, 0.0)
+    if mix_mask is not None:
+        return _UpsampleCEPLMix.apply(*args, mix_mask)
+    return _UpsampleCEPL.apply(*args)
+
+
 # ------------------------------------------------------------------------------------------------ pyramid pooling
 class _PPMLink:
     """Carries the identity-branch gradient of x from the concat node to the pooling node of one PPM invocation.
@@ -1076,6 +1087,27 @@ class _ScaleNC(torch.autograd.Function):
     def backward(ctx, dy):
         (scale,) = ctx.saved_tensors
         return ops.scale_nc(dy if dy.is_contiguous() else dy.contiguous(), scale), None
+
+
+class _FPFork(torch.autograd.Function):
+    """x [N] -> cat(x, x * scale) [2N] (UniMatch's feature-perturbation batch) in one native launch. The backward is the
+    fold kernel alone, d[:N] + scale * d[N:] rounded once: autograd never sums the two halves (as in _Fork, a split-aware
+    sum, here with the scale in the same fp32 expression). No gradient reaches the scale."""
+
+    @staticmethod
+    def forward(ctx, x, scale):
+        ctx.save_for_backward(scale)
+        return ops.fp_fork(x, scale)
+
+    @staticmethod
+    def backward(ctx, d):
+        (scale,) = ctx.saved_tensors
+        return ops.fp_fold(d if d.is_contiguous() else d.contiguous(), scale), None
+
+
+def fp_fork(x, scale):
+    """cat(x, x * scale[n, c]) along the batch of an N-image activation (scale fp32 [N, C]); differentiable in x."""
+    return _FPFork.apply(x, scale)
 
 
 def dropout2d_nhwc(x, p, training):

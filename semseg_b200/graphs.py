@@ -20,8 +20,8 @@ overwrites the first one's saved activations — gradient accumulation over seve
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
 loss, the focal loss, the RMI loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
-mean teacher's re-pack included, and the CutMix / ClassMix pseudo-label loss, its draws and mixing included, with or
-without a strong view of the student's input) are not captured (such models simply stay eager).
+mean teacher's re-pack included, the pseudo-label losses' feature-perturbation stream, and the CutMix / ClassMix
+pseudo-label loss, its draws and mixing included, with or without a strong view of the student's input) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -63,11 +63,11 @@ def note_boundary(t):
 class _Step:
     __slots__ = ("key", "calls", "failed", "fwd", "bwd", "bwd2", "x", "y", "pred", "main", "aux", "g_main", "g_aux",
                  "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot", "mix",
-                 "mix_crit", "strong", "strong_crit")
+                 "mix_crit", "strong", "strong_crit", "fp", "fp_crit")
 
     def __init__(self, key):
         self.key, self.calls, self.failed, self.fwd, self.dx_slot = key, 0, False, None, False
-        self.mix = self.mix_crit = self.strong = self.strong_crit = None
+        self.mix = self.mix_crit = self.strong = self.strong_crit = self.fp = self.fp_crit = None
 
 
 def _set_grad_outputs(st, g_main, g_aux):
@@ -127,11 +127,14 @@ class _Replay(torch.autograd.Function):
 
 def _point_mix(st):
     """A losses.MixPseudoLabelLoss criterion's last_mix() is the replayed step's: its mask, mixed target and uniforms
-    are that step's static tensors (each captured input shape has its own). So is a teacher criterion's last_strong()."""
+    are that step's static tensors (each captured input shape has its own). So are a teacher criterion's last_strong()
+    and a pseudo-label criterion's last_fp()."""
     if st.mix_crit is not None:
         st.mix_crit._mix_state = st.mix
     if st.strong_crit is not None:
         st.strong_crit._strong_state = st.strong
+    if st.fp_crit is not None:
+        st.fp_crit._fp_state = st.fp
 
 
 def _with_dx(st, gs):
@@ -269,6 +272,9 @@ def _capture(model, impl, st, x, y):
     if getattr(crit, "strong", None) is not None:
         # likewise the strong view and its uniforms
         st.strong, st.strong_crit = crit._strong_state, crit
+    if getattr(crit, "fp_weight", 0.0) > 0.0:
+        # and the feature perturbation's uniforms and scale
+        st.fp, st.fp_crit = crit._fp_state, crit
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
     del proxies, x_in, x_leaf
@@ -331,7 +337,7 @@ def train_step(model, impl, x, y):
         crit_key += (id(teacher), tkey(teacher.parameters()), tkey(teacher.buffers()),
                      tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
         crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight",
-                                                             "mix", "p", "area", "ratio"))
+                                                             "fp_weight", "fp_dropout", "mix", "p", "area", "ratio"))
         if crit.strong is not None:
             crit_key += ("strong",) + crit.strong.key()    # the strong view's options are launch arguments too
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),

@@ -10,7 +10,9 @@ pixel-wise distillation term from a teacher network that the student's training 
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
 optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
 batch, the student learns on the mixed one. Each of the three teacher criteria takes `strong=` (augment.StrongAugment):
-the student then learns on a strongly perturbed view of the batch the teacher sees.
+the student then learns on a strongly perturbed view of the batch the teacher sees. The two pseudo-label criteria take
+`fp_weight=` too: UniMatch's feature perturbation, a second pass of the context module and classifier on the student's
+channel-dropped layer4 features that learns the same pseudo-labels.
 """
 import math
 
@@ -384,9 +386,31 @@ class PseudoLabelLoss(_TeacherLoss):
     graphed at every zoom factor. Called as a module, forward(logits, target, teacher_logits=None) takes NCHW logits at the
     target size: without teacher_logits it returns the mean cross-entropy over L (the validation loss validate() logs),
     with them (the same shape) `main` computed at that size. CUDA fp32 logits with at most 256 classes only: there is no
-    CPU or library fallback."""
+    CPU or library fallback.
 
-    def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None):
+    `fp_weight` > 0 adds UniMatch's feature perturbation (Yang et al., CVPR 2023, its "FP" stream): the context module
+    and classifier run a second time on the student's layer4 features after a channel dropout, and that prediction learns
+    the same pseudo-labels. Per training forward of a PSPNet / PSANet, with f the student's layer4 output (of whatever
+    the student sees: its strong view, mixed):
+
+        u    = torch.rand(N, 2048) on the default CUDA generator, after the mix and strong draws, before the teacher
+        s    = [u < 1 - fp_dropout] / (1 - fp_dropout)        per (image, channel); fp_dropout = 0 gives s = 1
+        the context module and cls run once on cat(f, f * s) (2N images: every BatchNorm there takes batch statistics
+        over the 2N, running statistics are updated once; cls's Dropout2d draws for all 2N) -> s_main, s_fp
+        main = the main above of s_main + fp_weight (1/|U|) sum_{U, conf >= threshold} (lse(s_fp) - s_fp[yhat])
+        aux, pred: unchanged (of the aux head and of s_main)
+
+    U, yhat and conf are the pseudo-label term's (with mixing: the mixed target and the teacher map of each pixel's
+    source image); labelled pixels get no FP term. The gradient reaching f is d[:N] + s * d[N:]; none flows through s or
+    the teacher. `last_fp()` returns {'uniforms': u, 'scale': s} of the latest training forward, graphed or eager (None
+    before the first one, and with fp_weight 0). fp_weight = 0 (the default) runs no draw and no second stream: the
+    forward is the one without the option. validate(), eval mode and the teacher's forward never run the stream.
+    UniMatch's (loss_x + 0.5 loss_s + 0.5 loss_fp) / 2 with one strong stream is ce_weight=0.5, pl_weight=0.25,
+    fp_weight=0.25. Under DistributedDataParallel SyncBatchNorm sees 2N images per rank in the context module and cls
+    (multi-GPU runs have not been made)."""
+
+    def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None,
+                 fp_weight=0.0, fp_dropout=0.5):
         super(PseudoLabelLoss, self).__init__(teacher, ignore_index, strong)
         if isinstance(threshold, bool) or not isinstance(threshold, (int, float)):
             raise TypeError("threshold must be a number, got %r" % (threshold,))
@@ -395,11 +419,42 @@ class PseudoLabelLoss(_TeacherLoss):
         self.threshold = float(threshold)
         self.pl_weight = _non_negative("pl_weight", pl_weight)
         self.ce_weight = _non_negative("ce_weight", ce_weight)
+        self.fp_weight = _non_negative("fp_weight", fp_weight)
+        self.fp_dropout = _non_negative("fp_dropout", fp_dropout)
+        if self.fp_dropout >= 1.0:
+            raise ValueError("fp_dropout must lie in [0, 1), got %r" % fp_dropout)
+        self._fp_state = None
+
+    def _fp_repr(self):
+        return ", fp_weight=%g, fp_dropout=%g" % (self.fp_weight, self.fp_dropout)
 
     def extra_repr(self):
         return "teacher=%s, threshold=%g, pl_weight=%g, ce_weight=%g, ignore_index=%d" % (
             type(self.teacher).__name__, self.threshold, self.pl_weight, self.ce_weight,
-            self.ignore_index) + self._strong_repr()
+            self.ignore_index) + self._fp_repr() + self._strong_repr()
+
+    def last_fp(self):
+        """{'uniforms', 'scale'} of the latest training forward's feature perturbation (None before the first one, or
+        with fp_weight 0)."""
+        return None if self._fp_state is None else dict(self._fp_state)
+
+    def fp_draw(self, x, channels):
+        """The per-(image, channel) factor s [N, channels] of the feature-perturbation stream from fresh uniforms of
+        the default CUDA generator; remembered for last_fp()."""
+        u = torch.rand((x.shape[0], channels), device=x.device)
+        keep = 1.0 - self.fp_dropout
+        s = (u < keep).float().div_(keep)
+        self._fp_state = {'uniforms': u, 'scale': s}
+        return s
+
+    def fp_loss(self, logits, target, teacher_logits):
+        """The feature-perturbation term alone, module form: fp_weight * the pseudo-label term of the perturbed stream's
+        NCHW logits at the target size, with the teacher's logits of the same shape."""
+        from . import functional as SF
+        _check_native_logits(type(self).__name__, logits, target)
+        t = self._teacher_logits_nhwc(logits, teacher_logits)
+        loss, _ = SF.upsample_fp(logits.permute(0, 2, 3, 1).contiguous(), target, 1, self, t)
+        return loss
 
     def forward(self, logits, target, teacher_logits=None):
         from . import functional as SF
@@ -446,7 +501,8 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
         aux  = plain CE of the aux head on y_m;  pred = the student's argmax on x_m
 
     `p` in [0, 1] (UniMatch: 0.5), `area` = (lo, hi) with 0 < lo <= hi <= 1, `ratio` = (lo, hi) with 0 < lo <= hi; the
-    other arguments and the teacher's rules are PseudoLabelLoss's. Labelled and unlabelled images share the batch: an
+    other arguments (fp_weight and fp_dropout included: the feature-perturbation stream runs on the mixed batch's
+    features) and the teacher's rules are PseudoLabelLoss's. Labelled and unlabelled images share the batch: an
     unlabelled image has an all-ignore_index target, and the mixed target carries each pixel's own label or ignore.
 
     `last_mix()` returns {'mask': uint8 [N,H,W], 'target': y_m, 'uniforms': u} of the latest training forward, graphed
@@ -460,8 +516,9 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
     DistributedDataParallel each rank mixes its own batch (multi-GPU runs have not been made)."""
 
     def __init__(self, teacher, mix='cutmix', p=0.5, area=(0.02, 0.4), ratio=(0.3, 1 / 0.3), threshold=0.95,
-                 pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None):
-        super(MixPseudoLabelLoss, self).__init__(teacher, threshold, pl_weight, ce_weight, ignore_index, strong)
+                 pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None, fp_weight=0.0, fp_dropout=0.5):
+        super(MixPseudoLabelLoss, self).__init__(teacher, threshold, pl_weight, ce_weight, ignore_index, strong,
+                                                 fp_weight, fp_dropout)
         if not isinstance(mix, str):
             raise TypeError("mix must be 'cutmix' or 'classmix', got %r" % (mix,))
         if mix not in ('cutmix', 'classmix'):
@@ -479,7 +536,7 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
         return "teacher=%s, mix=%r, p=%g, area=(%g, %g), ratio=(%g, %g), threshold=%g, pl_weight=%g, ce_weight=%g, " \
                "ignore_index=%d" % (type(self.teacher).__name__, self.mix, self.p, self.area[0], self.area[1],
                                     self.ratio[0], self.ratio[1], self.threshold, self.pl_weight, self.ce_weight,
-                                    self.ignore_index) + self._strong_repr()
+                                    self.ignore_index) + self._fp_repr() + self._strong_repr()
 
     def last_mix(self):
         """{'mask', 'target', 'uniforms'} of the latest training forward (None before the first one)."""

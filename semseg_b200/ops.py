@@ -633,6 +633,31 @@ def scale_nc(x, scale):
     return out
 
 
+def fp_fork(x, scale):
+    """Feature-perturbation fork of an N-image activation: the 2N-image cat(x, scale_nc(x, scale)) in x's storage form,
+    from one read of x (scale fp32 [N, C])."""
+    lib = _lib.load()
+    n, h, w, c, xp = _nhwc_meta(x)
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == n * c
+    out = empty_act((2 * n, h, w, c), is_split(x), x.device)
+    _lib.check(lib.semseg_fp_fork(_ptr(x), _lo(x), xp, _ptr(scale), _ptr(out), _lo(out), c, n, h * w, c, _stream()),
+               "semseg_fp_fork")
+    return out
+
+
+def fp_fold(d, scale):
+    """The fork's backward: d[:N] + scale * d[N:] of a 2N-image activation gradient, in fp32, rounded once."""
+    lib = _lib.load()
+    n2, h, w, c, dp = _nhwc_meta(d)
+    assert n2 % 2 == 0, "the fold takes a 2N-image gradient"
+    n = n2 // 2
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == n * c
+    out = empty_act((n, h, w, c), is_split(d), d.device)
+    _lib.check(lib.semseg_fp_fold(_ptr(d), _lo(d), dp, _ptr(scale), _ptr(out), _lo(out), c, n, h * w, c, _stream()),
+               "semseg_fp_fold")
+    return out
+
+
 def f32_to_act(x, split, pad_to=8):
     """fp32 NHWC [N,H,W,C] (channel-contiguous, any pixel pitch) -> activation [N,H,W,Cp], Cp = C rounded up to
     `pad_to`, padding zero filled."""

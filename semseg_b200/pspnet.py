@@ -137,13 +137,15 @@ class _SegNet(nn.Module):
         if self.training and torch.is_grad_enabled():
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
-        t_logits = mix_mask = None
+        t_logits = mix_mask = fp_scale = None
         if self.training and y is not None and isinstance(self.criterion, losses._TeacherLoss):
             classes = self.cls[4].out_channels
             mixing = isinstance(self.criterion, losses.MixPseudoLabelLoss)
             u = self.criterion.draw(x, classes) if mixing else None      # the draws come before the teacher forward
             strong = self.criterion.strong
             u_s = strong.draw(x) if strong is not None else None
+            if getattr(self.criterion, "fp_weight", 0.0) > 0.0:
+                fp_scale = self.criterion.fp_draw(x, self.layer4[-1].conv3.out_channels)
             # the teacher first (distillation, pseudo-labels): its activations are transient before the student's saved
             # ones exist. It sees the batch; the student and both heads' losses see its strong view, mixed
             t_logits = self.criterion.run_teacher(x, classes)
@@ -151,7 +153,12 @@ class _SegNet(nn.Module):
                 x = self.criterion.strong_view(x, u_s)
             if mixing:
                 x, y, mix_mask = self.criterion.mix_batch(x, y, u, t_logits, self.zoom_factor)
-        logits, t_aux = self._logits_nhwc(x)
+        if fp_scale is None:
+            logits, t_aux = self._logits_nhwc(x)
+            fp_logits = None
+        else:
+            both, t_aux = self._logits_nhwc(x, fp_scale)
+            logits, fp_logits = both.chunk(2)            # the clean and the perturbed stream's logits
 
         if self.training:
             aux_logits = head_forward_nhwc(self.aux, t_aux)
@@ -159,6 +166,9 @@ class _SegNet(nn.Module):
                 # upsample + cross-entropy + argmax fused: [N, classes, H, W] never exists (model/pspnet.py:94-103)
                 main_loss, pred = SF.upsample_ce(logits, y, self.criterion.ignore_index, self.zoom_factor,
                                                  criterion=self.criterion, teacher_logits=t_logits, mix_mask=mix_mask)
+                if fp_logits is not None:
+                    main_loss = main_loss + SF.upsample_fp(fp_logits, y, self.zoom_factor, self.criterion, t_logits,
+                                                           mix_mask)[0]
                 aux_loss, _ = SF.upsample_ce(aux_logits, y, self.criterion.ignore_index, self.zoom_factor,
                                              criterion=self.criterion)
                 return pred, main_loss, aux_loss
@@ -171,6 +181,9 @@ class _SegNet(nn.Module):
                     s = 8 // self.zoom_factor
                     t_up = torch.where(mix_mask[:, ::s, ::s].unsqueeze(1).bool(), t_up.roll(-1, 0), t_up)
                 main_loss = self.criterion(x, y, teacher_logits=t_up)
+                if fp_logits is not None:
+                    main_loss = main_loss + self.criterion.fp_loss(upsample_logits(fp_logits, (h, w), self.zoom_factor),
+                                                                   y, t_up)
             else:
                 main_loss = self.criterion(x, y)
             aux_loss = self.criterion(aux, y)
@@ -181,9 +194,11 @@ class _SegNet(nn.Module):
                 x = F.interpolate(x, size=(h, w), mode='bilinear', align_corners=True)
             return x
 
-    def _logits_nhwc(self, x):
+    def _logits_nhwc(self, x, fp_scale=None):
         """fp32 NHWC classifier logits [N, h', w', classes] before the final upsample, and in training mode layer3's
-        output for the aux head (None in eval mode)."""
+        output for the aux head (None in eval mode). With `fp_scale` (fp32 [N, 2048], the feature-perturbation factor of
+        losses.PseudoLabelLoss) the context module and cls run on cat(f, f * fp_scale) of layer4's output f: logits
+        [2N, h', w', classes], the clean stream first."""
         t = self.layer0.forward_nchw(x)          # x.grad, when asked for, straight from the stem dgrad kernel
         t = self.layer1.forward_nhwc(t)
         t = graphs.note_boundary(self.layer2.forward_nhwc(t))     # where a captured backward is cut in two
@@ -192,6 +207,8 @@ class _SegNet(nn.Module):
         if self.training:       # layer3's output feeds layer4 and the aux head: explicit fan-out (native gradient add)
             t_tmp, t_aux = SF.fork(t_tmp, 2)
         t = self.layer4.forward_nhwc(t_tmp)
+        if fp_scale is not None:
+            t = SF.fp_fork(t, fp_scale)
         return head_forward_nhwc(self.cls, self._context_nhwc(t)), t_aux
 
     def _eval_logits_nhwc(self, x):
