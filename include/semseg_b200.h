@@ -344,6 +344,14 @@ int semseg_fp_fork(const void* x, const void* x_lo, int x_pitch, const float* sc
                    int out_pitch, int N, int HW, int C, void* stream);
 int semseg_fp_fold(const void* d, const void* d_lo, int d_pitch, const float* scale, void* out, void* out_lo,
                    int out_pitch, int N, int HW, int C, void* stream);
+/* The same with the first N of M >= N images perturbed (UniMatch's two strong streams, the first one perturbed).
+ * Fork: x holds M images, out M + N; out[m] = x[m] and out[M + n] = x[n] * scale[n*C + c] for n < N. Fold: d holds
+ * M + N images, out M; out[m] = d[m], plus scale[n*C + c] * d[M + n] for n < N, in the arithmetic above, rounded once.
+ * The other rules are the ones above; M = N gives semseg_fp_fork / semseg_fp_fold's results bit for bit. */
+int semseg_fp_fork_prefix(const void* x, const void* x_lo, int x_pitch, const float* scale, void* out, void* out_lo,
+                          int out_pitch, int M, int N, int HW, int C, void* stream);
+int semseg_fp_fold_prefix(const void* d, const void* d_lo, int d_pitch, const float* scale, void* out, void* out_lo,
+                          int out_pitch, int M, int N, int HW, int C, void* stream);
 /* fp32 rows [M][in_pitch] (C columns used) -> activation rows [M][out_pitch], columns C..Cp-1 zero (Cp % 8 == 0). */
 int semseg_f32_to_act(const float* in, int in_pitch, void* out, void* out_lo, int out_pitch, long long M, int C,
                       int Cp, void* stream);

@@ -159,6 +159,8 @@ SIGNATURES = {
     "semseg_scale_nc": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp]),
     "semseg_fp_fork": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp]),
     "semseg_fp_fold": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp]),
+    "semseg_fp_fork_prefix": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
+    "semseg_fp_fold_prefix": (c_int, [c_vp, c_vp, c_int, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp]),
     "semseg_f32_to_act": (c_int, [c_vp, c_int, c_vp, c_vp, c_int, c_ll, c_int, c_int, c_vp]),
     "semseg_act_to_f32": (c_int, [c_vp, c_vp, c_int, c_vp, c_int, c_ll, c_int, c_vp]),
     "semseg_maxpool3x3s2_fwd": (c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_int, c_vp]),

@@ -356,10 +356,10 @@ class StrongAugment:
             raise ValueError("StrongAugment: a %dx%d image needs H, W > ceil(3 sigma_hi) = %d" % (x.shape[2], x.shape[3],
                                                                                                   r))
 
-    def draw(self, x):
-        """The uniforms of one view of `x`: fp32 [N, 12] from torch.rand on x's device."""
+    def draw(self, x, views=1):
+        """The uniforms of `views` views of `x`: fp32 [views * N, 12] from one torch.rand on x's device, view-major."""
         self._check(x)
-        return torch.rand((x.shape[0], 12), device=x.device)
+        return torch.rand((views * x.shape[0], 12), device=x.device)
 
     def __call__(self, x, u=None):
         self._check(x)

@@ -715,16 +715,17 @@ __global__ void scale_nc_kernel(const __nv_bfloat16* __restrict__ x, const __nv_
   }
 }
 
-// Feature-perturbation fork: x [N, HW, C] -> out [2N, HW, C] with out[n] = x[n] and out[N + n] = x[n] * s[n, c]. The
-// second half is scale_nc's arithmetic (bit-equal to scale_nc(x, s)); the first half is stored through the same
-// act_st8, so s = 1 gives two bit-equal halves in either storage form.
+// Feature-perturbation fork: x [M, HW, C] -> out [M + N, HW, C] with out[m] = x[m] and out[M + n] = x[n] * s[n, c] for
+// the first N <= M images (M = N: UniMatch's FP batch; M = 2N: its two strong streams, the first one perturbed). The
+// perturbed part is scale_nc's arithmetic (bit-equal to scale_nc(x[:N], s)); the copy is stored through the same
+// act_st8, so s = 1 gives bit-equal copies in either storage form.
 template <bool S>
 __global__ void fp_fork_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ x_lo, int x_pitch,
                                const float* __restrict__ s, __nv_bfloat16* __restrict__ out,
-                               __nv_bfloat16* __restrict__ out_lo, int out_pitch, int N, long long HW, int C) {
+                               __nv_bfloat16* __restrict__ out_lo, int out_pitch, int M, int N, long long HW, int C) {
   const int groups = C >> 3;
-  const long long half = static_cast<long long>(N) * HW;
-  const long long total = half * groups;
+  const long long first = static_cast<long long>(M) * HW;
+  const long long total = first * groups;
   for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long p = idx / groups;
@@ -733,38 +734,43 @@ __global__ void fp_fork_kernel(const __nv_bfloat16* __restrict__ x, const __nv_b
     float f[8];
     act_ld8<S>(x, x_lo, p * x_pitch + c0, f);
     act_st8<S>(out, out_lo, p * out_pitch + c0, f);
-    const float4 s0 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0);
-    const float4 s1 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0 + 4);
-    f[0] *= s0.x; f[1] *= s0.y; f[2] *= s0.z; f[3] *= s0.w;
-    f[4] *= s1.x; f[5] *= s1.y; f[6] *= s1.z; f[7] *= s1.w;
-    act_st8<S>(out, out_lo, (p + half) * out_pitch + c0, f);
+    if (n < N) {
+      const float4 s0 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0);
+      const float4 s1 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0 + 4);
+      f[0] *= s0.x; f[1] *= s0.y; f[2] *= s0.z; f[3] *= s0.w;
+      f[4] *= s1.x; f[5] *= s1.y; f[6] *= s1.z; f[7] *= s1.w;
+      act_st8<S>(out, out_lo, (p + first) * out_pitch + c0, f);
+    }
   }
 }
 
-// Its backward: out[n] = d[n] + s[n, c] * d[N + n], in fp32 (the product and the sum each rounded to nearest, never
-// contracted to an fma) and rounded once to the activation form.
+// Its backward: out[m] = d[m], plus s[n, c] * d[M + n] for the first N images, in fp32 (the product and the sum each
+// rounded to nearest, never contracted to an fma) and rounded once to the activation form.
 template <bool S>
 __global__ void fp_fold_kernel(const __nv_bfloat16* __restrict__ d, const __nv_bfloat16* __restrict__ d_lo, int d_pitch,
                                const float* __restrict__ s, __nv_bfloat16* __restrict__ out,
-                               __nv_bfloat16* __restrict__ out_lo, int out_pitch, int N, long long HW, int C) {
+                               __nv_bfloat16* __restrict__ out_lo, int out_pitch, int M, int N, long long HW, int C) {
   const int groups = C >> 3;
-  const long long half = static_cast<long long>(N) * HW;
-  const long long total = half * groups;
+  const long long first = static_cast<long long>(M) * HW;
+  const long long total = first * groups;
   for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
        idx += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long p = idx / groups;
     const int c0 = static_cast<int>(idx - p * groups) << 3;
     const int n = static_cast<int>(p / HW);
     const Raw8<S> ra = act_ldraw<S>(d, d_lo, p * d_pitch + c0);
-    const Raw8<S> rb = act_ldraw<S>(d, d_lo, (p + half) * d_pitch + c0);
-    const float4 s0 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0);
-    const float4 s1 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0 + 4);
-    const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-    float a[8], b[8];
+    float a[8];
     act_unpack<S>(ra, a);
-    act_unpack<S>(rb, b);
+    if (n < N) {
+      const Raw8<S> rb = act_ldraw<S>(d, d_lo, (p + first) * d_pitch + c0);
+      const float4 s0 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0);
+      const float4 s1 = *reinterpret_cast<const float4*>(s + static_cast<size_t>(n) * C + c0 + 4);
+      const float sv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+      float b[8];
+      act_unpack<S>(rb, b);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) a[q] = __fadd_rn(a[q], __fmul_rn(sv[q], b[q]));
+      for (int q = 0; q < 8; ++q) a[q] = __fadd_rn(a[q], __fmul_rn(sv[q], b[q]));
+    }
     act_st8<S>(out, out_lo, p * out_pitch + c0, a);
   }
 }
@@ -1170,12 +1176,14 @@ extern "C" int semseg_scale_nc(const void* x, const void* x_lo, int x_pitch, con
   return SEMSEG_OK;
 }
 
-// The fork and the fold share their argument rules: `x` holds N images (fork) or 2N (fold), `out` the other count.
+// The fork and the fold share their argument rules: the fork's `x` holds M images and `out` M + N, the fold's the
+// other way round; the first N <= M images are the perturbed ones.
 static int check_fp_args(const char* fn, const void* x, const void* x_lo, int x_pitch, const float* scale,
-                         const void* out, const void* out_lo, int out_pitch, int N, int HW, int C) {
+                         const void* out, const void* out_lo, int out_pitch, int M, int N, int HW, int C) {
   SB_CHECK_ARG(x && scale && out, "%s: null x, scale or out", fn);
   SB_CHECK_ARG(N > 0 && HW > 0 && C > 0 && C % 8 == 0, "%s: need N, HW, C > 0 and C %% 8 == 0 (N %d, HW %d, C %d)", fn,
                N, HW, C);
+  SB_CHECK_ARG(M >= N, "%s: need M >= N (M %d, N %d)", fn, M, N);
   SB_CHECK_ARG(x_pitch >= C && x_pitch % 8 == 0 && out_pitch >= C && out_pitch % 8 == 0,
                "%s: pitches must be multiples of 8 and at least C (x %d, out %d, C %d)", fn, x_pitch, out_pitch, C);
   SB_CHECK_ARG((out_lo != nullptr) == (x_lo != nullptr), "%s: input and output must use the same storage form", fn);
@@ -1183,28 +1191,48 @@ static int check_fp_args(const char* fn, const void* x, const void* x_lo, int x_
   return check_vec_acts(fn, C, {{x, x_lo, x_pitch}, {out, out_lo, out_pitch}});
 }
 
-extern "C" int semseg_fp_fork(const void* x, const void* x_lo, int x_pitch, const float* scale, void* out, void* out_lo,
-                              int out_pitch, int N, int HW, int C, void* stream_) {
+static int fp_fork_launch(const char* fn, const void* x, const void* x_lo, int x_pitch, const float* scale, void* out,
+                          void* out_lo, int out_pitch, int M, int N, int HW, int C, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (const int r = check_fp_args("fp_fork", x, x_lo, x_pitch, scale, out, out_lo, out_pitch, N, HW, C)) return r;
-  const long long total = static_cast<long long>(N) * HW * (C / 8);
+  if (const int r = check_fp_args(fn, x, x_lo, x_pitch, scale, out, out_lo, out_pitch, M, N, HW, C)) return r;
+  const long long total = static_cast<long long>(M) * HW * (C / 8);
   SB_ACT_DISPATCH(x_lo != nullptr, fp_fork_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                                        static_cast<const bf16*>(x), static_cast<const bf16*>(x_lo), x_pitch, scale,
-                                       static_cast<bf16*>(out), static_cast<bf16*>(out_lo), out_pitch, N, HW, C));
+                                       static_cast<bf16*>(out), static_cast<bf16*>(out_lo), out_pitch, M, N, HW, C));
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
 
-extern "C" int semseg_fp_fold(const void* d, const void* d_lo, int d_pitch, const float* scale, void* out, void* out_lo,
-                              int out_pitch, int N, int HW, int C, void* stream_) {
+static int fp_fold_launch(const char* fn, const void* d, const void* d_lo, int d_pitch, const float* scale, void* out,
+                          void* out_lo, int out_pitch, int M, int N, int HW, int C, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (const int r = check_fp_args("fp_fold", d, d_lo, d_pitch, scale, out, out_lo, out_pitch, N, HW, C)) return r;
-  const long long total = static_cast<long long>(N) * HW * (C / 8);
+  if (const int r = check_fp_args(fn, d, d_lo, d_pitch, scale, out, out_lo, out_pitch, M, N, HW, C)) return r;
+  const long long total = static_cast<long long>(M) * HW * (C / 8);
   SB_ACT_DISPATCH(d_lo != nullptr, fp_fold_kernel<kS><<<ew_grid(total, 256), 256, 0, stream>>>(
                                        static_cast<const bf16*>(d), static_cast<const bf16*>(d_lo), d_pitch, scale,
-                                       static_cast<bf16*>(out), static_cast<bf16*>(out_lo), out_pitch, N, HW, C));
+                                       static_cast<bf16*>(out), static_cast<bf16*>(out_lo), out_pitch, M, N, HW, C));
   SB_LAUNCHED();
   return SEMSEG_OK;
+}
+
+extern "C" int semseg_fp_fork(const void* x, const void* x_lo, int x_pitch, const float* scale, void* out, void* out_lo,
+                              int out_pitch, int N, int HW, int C, void* stream) {
+  return fp_fork_launch("fp_fork", x, x_lo, x_pitch, scale, out, out_lo, out_pitch, N, N, HW, C, stream);
+}
+
+extern "C" int semseg_fp_fold(const void* d, const void* d_lo, int d_pitch, const float* scale, void* out, void* out_lo,
+                              int out_pitch, int N, int HW, int C, void* stream) {
+  return fp_fold_launch("fp_fold", d, d_lo, d_pitch, scale, out, out_lo, out_pitch, N, N, HW, C, stream);
+}
+
+extern "C" int semseg_fp_fork_prefix(const void* x, const void* x_lo, int x_pitch, const float* scale, void* out,
+                                     void* out_lo, int out_pitch, int M, int N, int HW, int C, void* stream) {
+  return fp_fork_launch("fp_fork_prefix", x, x_lo, x_pitch, scale, out, out_lo, out_pitch, M, N, HW, C, stream);
+}
+
+extern "C" int semseg_fp_fold_prefix(const void* d, const void* d_lo, int d_pitch, const float* scale, void* out,
+                                     void* out_lo, int out_pitch, int M, int N, int HW, int C, void* stream) {
+  return fp_fold_launch("fp_fold_prefix", d, d_lo, d_pitch, scale, out, out_lo, out_pitch, M, N, HW, C, stream);
 }
 
 static int splitk_chunk_rows(int M) {

@@ -1090,23 +1090,27 @@ class _ScaleNC(torch.autograd.Function):
 
 
 class _FPFork(torch.autograd.Function):
-    """x [N] -> cat(x, x * scale) [2N] (UniMatch's feature-perturbation batch) in one native launch. The backward is the
-    fold kernel alone, d[:N] + scale * d[N:] rounded once: autograd never sums the two halves (as in _Fork, a split-aware
-    sum, here with the scale in the same fp32 expression). No gradient reaches the scale."""
+    """x [M] -> cat(x, x[:N] * scale) [M + N] (UniMatch's feature-perturbation batch; M > N when the first N images are
+    one stream of several) in one native launch. The backward is the fold kernel alone, d[:M] with scale * d[M:] added
+    to its first N images, rounded once: autograd never sums the two parts (as in _Fork, a split-aware sum, here with the
+    scale in the same fp32 expression). No gradient reaches the scale. M = N runs the plain fork and fold."""
 
     @staticmethod
     def forward(ctx, x, scale):
         ctx.save_for_backward(scale)
-        return ops.fp_fork(x, scale)
+        ctx.prefix = x.shape[-4] != scale.shape[0]
+        return ops.fp_fork_prefix(x, scale) if ctx.prefix else ops.fp_fork(x, scale)
 
     @staticmethod
     def backward(ctx, d):
         (scale,) = ctx.saved_tensors
-        return ops.fp_fold(d if d.is_contiguous() else d.contiguous(), scale), None
+        d = d if d.is_contiguous() else d.contiguous()
+        return (ops.fp_fold_prefix(d, scale) if ctx.prefix else ops.fp_fold(d, scale)), None
 
 
 def fp_fork(x, scale):
-    """cat(x, x * scale[n, c]) along the batch of an N-image activation (scale fp32 [N, C]); differentiable in x."""
+    """cat(x, x[:N] * scale[n, c]) along the batch of an M-image activation (scale fp32 [N, C], N <= M); differentiable
+    in x."""
     return _FPFork.apply(x, scale)
 
 

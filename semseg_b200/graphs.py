@@ -20,7 +20,7 @@ overwrites the first one's saved activations — gradient accumulation over seve
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
 loss, the focal loss, the RMI loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
-mean teacher's re-pack included, the pseudo-label losses' feature-perturbation stream, and the CutMix / ClassMix
+mean teacher's re-pack included, the pseudo-label losses' feature-perturbation stream and second strong stream, and the CutMix / ClassMix
 pseudo-label loss, its draws and mixing included, with or without a strong view of the student's input) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
@@ -338,6 +338,8 @@ def train_step(model, impl, x, y):
                      tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
         crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight",
                                                              "fp_weight", "fp_dropout", "mix", "p", "area", "ratio"))
+        if getattr(crit, "streams", 1) != 1:
+            crit_key += ("streams", crit.streams)          # a 2N-image student: other shapes and launches
         if crit.strong is not None:
             crit_key += ("strong",) + crit.strong.key()    # the strong view's options are launch arguments too
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),

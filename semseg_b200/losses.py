@@ -12,7 +12,8 @@ optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or Clas
 batch, the student learns on the mixed one. Each of the three teacher criteria takes `strong=` (augment.StrongAugment):
 the student then learns on a strongly perturbed view of the batch the teacher sees. The two pseudo-label criteria take
 `fp_weight=` too: UniMatch's feature perturbation, a second pass of the context module and classifier on the student's
-channel-dropped layer4 features that learns the same pseudo-labels.
+channel-dropped layer4 features that learns the same pseudo-labels, and `streams=2`: UniMatch's dual-stream
+perturbation, two strong views of every image, each with its own draws, in one student pass.
 """
 import math
 
@@ -407,10 +408,39 @@ class PseudoLabelLoss(_TeacherLoss):
     forward is the one without the option. validate(), eval mode and the teacher's forward never run the stream.
     UniMatch's (loss_x + 0.5 loss_s + 0.5 loss_fp) / 2 with one strong stream is ce_weight=0.5, pl_weight=0.25,
     fp_weight=0.25. Under DistributedDataParallel SyncBatchNorm sees 2N images per rank in the context module and cls
-    (multi-GPU runs have not been made)."""
+    (multi-GPU runs have not been made).
+
+    `streams=2` is UniMatch's dual-stream perturbation: every image gets two strong views, each with its own draws, and
+    both learn the same pseudo-labels. It needs `strong` (two views without it would be the same images; the CutMix /
+    ClassMix criterion takes it without, its two mixes differ). Per training forward of a PSPNet / PSANet with input x
+    [N,3,H,W] and target y, rows [0, N) of every [2N, .] draw belonging to stream 1 and rows [N, 2N) to stream 2:
+
+        draws  in the one-stream order on the default CUDA generator, before the teacher: the mix uniforms
+               torch.rand(2N, 5 [+ C]) (MixPseudoLabelLoss), the strong uniforms torch.rand(2N, 12), the FP uniforms
+               torch.rand(N, 2048) (fp_weight > 0)
+        teacher once, on the unmixed x (N images)
+        view_k = mix_k(strong_k(x)), y_k = mix_k(y): each stream's strong view from its own uniform rows, each stream
+                 mixed within itself (image n's partner is that stream's view of image (n + 1) mod N; ClassMix takes the
+                 one teacher argmax and selects classes from the stream's own rows); without mixing y_k = y
+        the whole student runs once on cat(view_1, view_2) (2N images: every BatchNorm takes statistics over the 2N,
+        SyncBatchNorm 2N per rank; cls's Dropout2d draws for all 2N). With fp_weight > 0 only stream 1's layer4 features
+        f_1 are perturbed: the context module and cls run on cat(f_1, f_2, f_1 * s) (3N images), one FP term
+        main   = (main_1 + main_2) / 2 + fp_weight * FP,  main_k the main above of stream k's logits, y_k and teacher maps
+                 (with mixing, of each pixel's source image), FP the term above on stream 1's logits, mask and target
+        aux    = (aux_1 + aux_2) / 2;  pred = stream 1's argmax [N]
+
+    With this, UniMatch's full loss (loss_x + 0.25 loss_s1 + 0.25 loss_s2 + 0.5 loss_fp) / 2 is ce_weight=0.5,
+    pl_weight=0.25, fp_weight=0.25, the weights of the one-stream recipe. The accessors are stream-major: last_strong()
+    holds 'image' [2N,3,H,W] and 'uniforms' [2N,12], MixPseudoLabelLoss.last_mix() 'mask' [2N,H,W], 'target'
+    [2N,Ho,Wo] and 'uniforms' [2N, .]; last_fp() stays [N, 2048]. The student's activations are those of a 2N-image
+    batch. streams=1 (the default) is the one-stream forward. Eval mode, validate(), the teacher's forward and the
+    module form forward(logits, target, teacher_logits) are single-stream."""
+
+    # two streams are two different views only through the strong view's draws (a mix criterion's boxes differ too)
+    _streams_need_strong = True
 
     def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None,
-                 fp_weight=0.0, fp_dropout=0.5):
+                 fp_weight=0.0, fp_dropout=0.5, streams=1):
         super(PseudoLabelLoss, self).__init__(teacher, ignore_index, strong)
         if isinstance(threshold, bool) or not isinstance(threshold, (int, float)):
             raise TypeError("threshold must be a number, got %r" % (threshold,))
@@ -423,10 +453,29 @@ class PseudoLabelLoss(_TeacherLoss):
         self.fp_dropout = _non_negative("fp_dropout", fp_dropout)
         if self.fp_dropout >= 1.0:
             raise ValueError("fp_dropout must lie in [0, 1), got %r" % fp_dropout)
+        if isinstance(streams, bool):
+            raise TypeError("streams must be the int 1 or 2, got %r" % (streams,))
+        if not (isinstance(streams, int) and streams in (1, 2)):
+            raise ValueError("streams must be the int 1 or 2, got %r" % (streams,))
+        if streams == 2 and strong is None and self._streams_need_strong:
+            raise ValueError("%s: streams=2 needs a strong view (strong=None would give two identical streams)" %
+                             type(self).__name__)
+        self.streams = streams
         self._fp_state = None
 
     def _fp_repr(self):
-        return ", fp_weight=%g, fp_dropout=%g" % (self.fp_weight, self.fp_dropout)
+        return ", fp_weight=%g, fp_dropout=%g" % (self.fp_weight, self.fp_dropout) + \
+            (", streams=2" if self.streams == 2 else "")
+
+    def strong_streams(self, x, u):
+        """The student's views of `x` from the strong uniforms `u` [streams * N, 12], stream-major: each stream's view
+        from its own rows, concatenated along the batch; remembered for last_strong()."""
+        if self.streams == 1:
+            return self.strong_view(x, u)
+        n = x.shape[0]
+        xs = torch.cat([self.strong(x, u[k * n:(k + 1) * n]) for k in range(self.streams)])
+        self._strong_state = {'image': xs, 'uniforms': u}
+        return xs
 
     def extra_repr(self):
         return "teacher=%s, threshold=%g, pl_weight=%g, ce_weight=%g, ignore_index=%d" % (
@@ -513,12 +562,18 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
     With the network's fused tail the mixing, the mixed pseudo-label loss and the teacher forward run on native kernels
     (csrc/mix.cu and csrc/tail.cu), graphed at every zoom factor; where the fused tail does not apply (a target wider
     than its kernels stage), the mixing stays native and the teacher's upsampled maps are mixed with torch.where. Under
-    DistributedDataParallel each rank mixes its own batch (multi-GPU runs have not been made)."""
+    DistributedDataParallel each rank mixes its own batch (multi-GPU runs have not been made).
+
+    `streams=2` (PseudoLabelLoss's dual-stream perturbation) needs no strong view here: each stream mixes within itself
+    from its own uniform rows, so the two streams differ by their boxes or class sets."""
+
+    _streams_need_strong = False
 
     def __init__(self, teacher, mix='cutmix', p=0.5, area=(0.02, 0.4), ratio=(0.3, 1 / 0.3), threshold=0.95,
-                 pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None, fp_weight=0.0, fp_dropout=0.5):
+                 pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None, fp_weight=0.0, fp_dropout=0.5,
+                 streams=1):
         super(MixPseudoLabelLoss, self).__init__(teacher, threshold, pl_weight, ce_weight, ignore_index, strong,
-                                                 fp_weight, fp_dropout)
+                                                 fp_weight, fp_dropout, streams)
         if not isinstance(mix, str):
             raise TypeError("mix must be 'cutmix' or 'classmix', got %r" % (mix,))
         if mix not in ('cutmix', 'classmix'):
@@ -543,7 +598,8 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
         return None if self._mix_state is None else dict(self._mix_state)
 
     def draw(self, x, classes):
-        """The forward's uniforms, drawn before the teacher runs: [N, 5] (CutMix) or [N, 5 + classes] (ClassMix)."""
+        """The forward's uniforms, drawn before the teacher runs: [streams * N, 5] (CutMix) or [streams * N,
+        5 + classes] (ClassMix), stream-major."""
         name = type(self).__name__
         if x.requires_grad:
             raise RuntimeError("%s: there is no gradient through the mixing; the input must not require grad" % name)
@@ -552,20 +608,30 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
                             (name, x.dtype, tuple(x.shape), x.device))
         if self.mix == 'classmix' and classes > 256:
             raise ValueError("%s: ClassMix needs at most 256 classes, got %d" % (name, classes))
-        return torch.rand((x.shape[0], 5 + (classes if self.mix == 'classmix' else 0)), device=x.device)
+        return torch.rand((self.streams * x.shape[0], 5 + (classes if self.mix == 'classmix' else 0)),
+                          device=x.device)
 
     def mix_batch(self, x, y, u, t_logits, zoom):
         """(x_m, y_m, mask) from the input, target, `draw`'s uniforms and the teacher's NHWC logits of the unmixed
-        input; remembered for last_mix()."""
+        input; remembered for last_mix(). With two streams `x` holds both streams' views ([2N], or the N images
+        themselves for both without a strong view) and each stream is mixed within itself from its own uniform rows:
+        x_m, y_m and the mask are [2N], stream-major."""
         from . import ops
         if y.dtype != torch.int64:
             raise TypeError("%s: int64 target expected, got %s" % (type(self).__name__, y.dtype))
-        amap = sel = None
+        n = y.shape[0]
+        x, y = x.contiguous(), y.contiguous()
+        amap = present = None
         if self.mix == 'classmix':
             amap, present = ops.mix_argmax_x8(t_logits)
-            sel = ops.mix_select(u, present, t_logits.shape[-1])
-        mask, xm, ym = ops.mix_apply(self.mix, x.contiguous(), y.contiguous(), u, self.p, self.area, self.ratio,
-                                     zoom, amap, sel)
+        outs = []
+        for k in range(self.streams):
+            rows = slice(k * n, (k + 1) * n)
+            u_k = u[rows]
+            sel = ops.mix_select(u_k, present, t_logits.shape[-1]) if amap is not None else None
+            outs.append(ops.mix_apply(self.mix, x[rows] if x.shape[0] > n else x, y, u_k, self.p, self.area,
+                                      self.ratio, zoom, amap, sel))
+        mask, xm, ym = outs[0] if len(outs) == 1 else (torch.cat(t) for t in zip(*outs))
         self._mix_state = {'mask': mask, 'target': ym, 'uniforms': u}
         return xm, ym, mask
 

@@ -658,6 +658,36 @@ def fp_fold(d, scale):
     return out
 
 
+def fp_fork_prefix(x, scale):
+    """Feature-perturbation fork of an M-image activation whose first N images are perturbed (scale fp32 [N, C],
+    N <= M): the (M + N)-image cat(x, scale_nc(x[:N], scale)) in x's storage form, from one read of x. M = N is fp_fork's
+    result bit for bit."""
+    lib = _lib.load()
+    m, h, w, c, xp = _nhwc_meta(x)
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.dim() == 2 and scale.shape[1] == c
+    n = scale.shape[0]
+    out = empty_act((m + n, h, w, c), is_split(x), x.device)
+    _lib.check(lib.semseg_fp_fork_prefix(_ptr(x), _lo(x), xp, _ptr(scale), _ptr(out), _lo(out), c, m, n, h * w, c,
+                                         _stream()),
+               "semseg_fp_fork_prefix")
+    return out
+
+
+def fp_fold_prefix(d, scale):
+    """fp_fork_prefix's backward: d[:M] with scale * d[M:] added to its first N images, of an (M + N)-image activation
+    gradient (scale fp32 [N, C]), in fp32, rounded once. M = N is fp_fold's result bit for bit."""
+    lib = _lib.load()
+    mn, h, w, c, dp = _nhwc_meta(d)
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.dim() == 2 and scale.shape[1] == c
+    n = scale.shape[0]
+    m = mn - n
+    out = empty_act((m, h, w, c), is_split(d), d.device)
+    _lib.check(lib.semseg_fp_fold_prefix(_ptr(d), _lo(d), dp, _ptr(scale), _ptr(out), _lo(out), c, m, n, h * w, c,
+                                         _stream()),
+               "semseg_fp_fold_prefix")
+    return out
+
+
 def f32_to_act(x, split, pad_to=8):
     """fp32 NHWC [N,H,W,C] (channel-contiguous, any pixel pitch) -> activation [N,H,W,Cp], Cp = C rounded up to
     `pad_to`, padding zero filled."""

@@ -60,6 +60,16 @@ def upsample_logits(logits_nhwc, size, zoom_factor):
     return x
 
 
+def _chunks(t, k):
+    """`t` split into k equal chunks along the batch (k = 1: the tensor itself, no view)."""
+    return t.chunk(k) if k > 1 else (t,)
+
+
+def _stream_mean(terms):
+    """The mean of the per-stream losses (one stream: its loss itself, no extra kernel)."""
+    return terms[0] if len(terms) == 1 else sum(terms[1:], terms[0]) / len(terms)
+
+
 class _SegNet(nn.Module):
     """The network body PSPNet and PSANet share (model/pspnet.py:29-105, model/psanet.py:101-179): the dilated ResNet,
     a context module between layer4 and `cls`, the `cls` / `aux` heads and the forward. `context` is None or
@@ -138,67 +148,77 @@ class _SegNet(nn.Module):
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
         t_logits = mix_mask = fp_scale = None
+        streams = 1
         if self.training and y is not None and isinstance(self.criterion, losses._TeacherLoss):
             classes = self.cls[4].out_channels
             mixing = isinstance(self.criterion, losses.MixPseudoLabelLoss)
+            streams = getattr(self.criterion, "streams", 1)
             u = self.criterion.draw(x, classes) if mixing else None      # the draws come before the teacher forward
             strong = self.criterion.strong
-            u_s = strong.draw(x) if strong is not None else None
+            u_s = None if strong is None else strong.draw(x) if streams == 1 else strong.draw(x, streams)
             if getattr(self.criterion, "fp_weight", 0.0) > 0.0:
                 fp_scale = self.criterion.fp_draw(x, self.layer4[-1].conv3.out_channels)
             # the teacher first (distillation, pseudo-labels): its activations are transient before the student's saved
             # ones exist. It sees the batch; the student and both heads' losses see its strong view, mixed
             t_logits = self.criterion.run_teacher(x, classes)
             if strong is not None:
-                x = self.criterion.strong_view(x, u_s)
+                x = self.criterion.strong_streams(x, u_s) if streams > 1 else self.criterion.strong_view(x, u_s)
             if mixing:
                 x, y, mix_mask = self.criterion.mix_batch(x, y, u, t_logits, self.zoom_factor)
-        if fp_scale is None:
-            logits, t_aux = self._logits_nhwc(x)
-            fp_logits = None
-        else:
-            both, t_aux = self._logits_nhwc(x, fp_scale)
-            logits, fp_logits = both.chunk(2)            # the clean and the perturbed stream's logits
+        # the student's batch: `streams` views of the N images, stream-major, and with the FP stream stream 1's
+        # perturbed copy after them. Each stream's logits, aux logits, target and mix mask are a contiguous N-image chunk
+        # without the FP stream the call is the one-argument form it always was (subclasses and wrappers override it)
+        out, t_aux = self._logits_nhwc(x) if fp_scale is None else self._logits_nhwc(x, fp_scale)
+        logits = _chunks(out, streams + (fp_scale is not None))
+        fp_logits = logits[streams] if fp_scale is not None else None
 
         if self.training:
-            aux_logits = head_forward_nhwc(self.aux, t_aux)
-            if SF.fused_tail_supported(self.criterion, logits, y, self.zoom_factor):
-                # upsample + cross-entropy + argmax fused: [N, classes, H, W] never exists (model/pspnet.py:94-103)
-                main_loss, pred = SF.upsample_ce(logits, y, self.criterion.ignore_index, self.zoom_factor,
-                                                 criterion=self.criterion, teacher_logits=t_logits, mix_mask=mix_mask)
+            aux_logits = _chunks(head_forward_nhwc(self.aux, t_aux), streams)
+            ys = _chunks(y, streams) if mix_mask is not None else (y,) * streams      # the mixed target is [2N]
+            masks = _chunks(mix_mask, streams) if mix_mask is not None else (None,) * streams
+            if SF.fused_tail_supported(self.criterion, logits[0], y, self.zoom_factor):
+                # upsample + cross-entropy + argmax fused: [N, classes, H, W] never exists (model/pspnet.py:94-103);
+                # one call per stream: each has its own target, mask and normalisers, and the one teacher map
+                mains, preds = zip(*(SF.upsample_ce(logits[k], ys[k], self.criterion.ignore_index, self.zoom_factor,
+                                                    criterion=self.criterion, teacher_logits=t_logits,
+                                                    mix_mask=masks[k]) for k in range(streams)))
+                main_loss = _stream_mean(mains)
                 if fp_logits is not None:
-                    main_loss = main_loss + SF.upsample_fp(fp_logits, y, self.zoom_factor, self.criterion, t_logits,
-                                                           mix_mask)[0]
-                aux_loss, _ = SF.upsample_ce(aux_logits, y, self.criterion.ignore_index, self.zoom_factor,
-                                             criterion=self.criterion)
-                return pred, main_loss, aux_loss
-            x = upsample_logits(logits, (h, w), self.zoom_factor)
-            aux = upsample_logits(aux_logits, (h, w), self.zoom_factor)
+                    main_loss = main_loss + SF.upsample_fp(fp_logits, ys[0], self.zoom_factor, self.criterion,
+                                                           t_logits, masks[0])[0]
+                aux_loss = _stream_mean([SF.upsample_ce(a, y_k, self.criterion.ignore_index, self.zoom_factor,
+                                                        criterion=self.criterion)[0] for a, y_k in zip(aux_logits, ys)])
+                return preds[0], main_loss, aux_loss
+            ups = [upsample_logits(v, (h, w), self.zoom_factor) for v in logits[:streams]]
+            aux_ups = [upsample_logits(v, (h, w), self.zoom_factor) for v in aux_logits]
             if t_logits is not None:
                 t_up = upsample_logits(t_logits, (h, w), self.zoom_factor)
+                t_ups = [t_up] * streams
                 if mix_mask is not None:
                     # each target pixel's teacher map is its source image's: the mask read at the target grid
                     s = 8 // self.zoom_factor
-                    t_up = torch.where(mix_mask[:, ::s, ::s].unsqueeze(1).bool(), t_up.roll(-1, 0), t_up)
-                main_loss = self.criterion(x, y, teacher_logits=t_up)
+                    t_ups = [torch.where(m[:, ::s, ::s].unsqueeze(1).bool(), t_up.roll(-1, 0), t_up) for m in masks]
+                main_loss = _stream_mean([self.criterion(v, y_k, teacher_logits=t_k)
+                                          for v, y_k, t_k in zip(ups, ys, t_ups)])
                 if fp_logits is not None:
                     main_loss = main_loss + self.criterion.fp_loss(upsample_logits(fp_logits, (h, w), self.zoom_factor),
-                                                                   y, t_up)
+                                                                   ys[0], t_ups[0])
             else:
-                main_loss = self.criterion(x, y)
-            aux_loss = self.criterion(aux, y)
-            return x.max(1)[1], main_loss, aux_loss
+                main_loss = self.criterion(ups[0], y)
+            aux_loss = _stream_mean([self.criterion(a, y_k) for a, y_k in zip(aux_ups, ys)])
+            return ups[0].max(1)[1], main_loss, aux_loss
         else:
-            x = ops.nhwc_f32_to_nchw(logits) if not logits.requires_grad else logits.permute(0, 3, 1, 2).contiguous()
+            x = logits[0]
+            x = ops.nhwc_f32_to_nchw(x) if not x.requires_grad else x.permute(0, 3, 1, 2).contiguous()
             if self.zoom_factor != 1:
                 x = F.interpolate(x, size=(h, w), mode='bilinear', align_corners=True)
             return x
 
     def _logits_nhwc(self, x, fp_scale=None):
-        """fp32 NHWC classifier logits [N, h', w', classes] before the final upsample, and in training mode layer3's
-        output for the aux head (None in eval mode). With `fp_scale` (fp32 [N, 2048], the feature-perturbation factor of
-        losses.PseudoLabelLoss) the context module and cls run on cat(f, f * fp_scale) of layer4's output f: logits
-        [2N, h', w', classes], the clean stream first."""
+        """fp32 NHWC classifier logits [M, h', w', classes] of an M-image batch before the final upsample, and in
+        training mode layer3's output for the aux head (None in eval mode). With `fp_scale` (fp32 [N, 2048], N <= M, the
+        feature-perturbation factor of losses.PseudoLabelLoss) the context module and cls run on cat(f, f[:N] *
+        fp_scale) of layer4's output f: logits [M + N, h', w', classes], the unperturbed images first."""
         t = self.layer0.forward_nchw(x)          # x.grad, when asked for, straight from the stem dgrad kernel
         t = self.layer1.forward_nhwc(t)
         t = graphs.note_boundary(self.layer2.forward_nhwc(t))     # where a captured backward is cut in two
