@@ -624,6 +624,35 @@ long long semseg_upsample_kd_bwd_workspace_floats(int N, int Ho, int w, int C, i
 int semseg_upsample_kd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
                            int C, int Ho, int Wo, int zoom, float temperature, float kd_weight, const float* lse,
                            const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Cross-image relational distillation (semseg_b200/losses.py DistillationLoss relation_weight; CIRKD's mini-batch
+ * pixel-to-pixel term). Features are NHWC bf16 [B,h,w,C] activations (lo == NULL: plain; else the split form), C = 512.
+ *   nodes:     node (a,b) of image n max-pools rows [p a, min(p a + p, h)) x columns [p b, min(p b + p, w)) per channel
+ *              (max_pool2d(p, p, ceil_mode=True)); M = ceil(h/p) ceil(w/p), 1 <= p <= 16. Each node is divided by its
+ *              fp32 L2 norm (Sigma x^2 in a fixed order); a node with norm < 1e-12 is the zero vector. Written as the bf16
+ *              operand nodes [B,M,512] (dense, 16-byte aligned), plus nodes_lo (bf16(v - hi)) when non-NULL. With argmax
+ *              (uint8 [B,M,512], 16-byte aligned) and inv_norm (fp32 [B,M]) it also saves the window offset
+ *              (row-major, first maximum) of every (node, channel) maximum and 1/|x| (0 for a zero node).
+ *   kl_fwd:    with X_i, Y_i the student / teacher nodes of image i and tau = temperature > 0,
+ *              S_ij = X_i X_j^T / tau, T_ij = Y_i Y_j^T / tau, P = row-softmax(S), Q = row-softmax(T),
+ *              loss[0] = tau^2 / (B^2 M) sum_{i,j} sum_rows KL(Q_ij,row || P_ij,row)     (all ordered pairs)
+ *              lse fp32 [B,B,M,2] = (lse of the row of S_ij, of T_ij) per (i, j, row): keep it for the backward.
+ *              workspace: semseg_relation_workspace_floats(B, M) floats, 8-byte aligned. Both node sets share one form.
+ *   kl_bwd:    dnodes fp32 [B,M,512] = grad_out[0] d loss / d X (the student nodes; the teacher gets none), written.
+ *   nodes_bwd: dfeat [B,h,w,512] (its own form and pitch) = the gradient of the features through the normalisation and
+ *              the saved maxima; every element is written (zero off the maxima and for zero nodes).
+ * Every entry point rejects a null pointer, a bad shape, C != 512, a pool outside [1, 16], a bad temperature, a pitch
+ * that is not a multiple of 8 or below C, or a misaligned pointer before any CUDA call. No host synchronisation
+ * (graph-capturable), no atomics: deterministic. semseg_relation_workspace_floats returns -1 for a bad size. */
+int semseg_relation_nodes(const void* feat, const void* feat_lo, int pitch, int B, int h, int w, int C, int pool,
+                          void* nodes, void* nodes_lo, unsigned char* argmax, float* inv_norm, void* stream);
+long long semseg_relation_workspace_floats(int B, int M);
+int semseg_relation_kl_fwd(const void* xs, const void* xs_lo, const void* xt, const void* xt_lo, int B, int M, int C,
+                           float temperature, float* workspace, float* lse, float* loss, void* stream);
+int semseg_relation_kl_bwd(const void* xs, const void* xs_lo, const void* xt, const void* xt_lo, int B, int M, int C,
+                           float temperature, const float* lse, const float* grad_out, float* dnodes, void* stream);
+int semseg_relation_nodes_bwd(const void* feat, const void* feat_lo, int pitch, int B, int h, int w, int C, int pool,
+                              const unsigned char* argmax, const float* inv_norm, const float* dnodes, void* dfeat,
+                              void* dfeat_lo, int dfeat_pitch, void* stream);
 /* Confidence-masked pseudo-label cross-entropy (semseg_b200/losses.py PseudoLabelLoss) on the same fused upsample at
  * zoom `zoom`: student and teacher fp32 NHWC [N,h,w,C] maps, each with its own pitch (>= C), both upsampled as the zoom
  * forward upsamples. Per output pixel, L = {0 <= target < C, target != ignore_index}, U = {target == ignore_index},

@@ -237,7 +237,14 @@ SIGNATURES = {
     "semseg_upsample_kd_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_kd_bwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f,
                                        c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
-    "semseg_upsample_pl_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_relation_nodes": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
+                                      c_vp]),
+    "semseg_relation_workspace_floats": (c_ll, [c_int, c_int]),
+    "semseg_relation_kl_fwd": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_relation_kl_bwd": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, c_f, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_relation_nodes_bwd": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp,
+                                          c_vp, c_vp, c_int, c_vp]),
+    "semseg_upsample_pl_workspace_floats":(c_ll, [c_int, c_int, c_int, c_int]),
     "semseg_upsample_pl_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                        c_int, c_f, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_upsample_pl_mix_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,

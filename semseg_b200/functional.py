@@ -729,6 +729,43 @@ class _UpsampleCERMI(torch.autograd.Function):
         return dl, None, None, None, None, None, None
 
 
+class _RelationKD(torch.autograd.Function):
+    """losses.DistillationLoss's relation term R of the student's and the teacher's cls[2] features (csrc/relation.cu):
+    the forward forms both networks' nodes and the fused KL, the backward recomputes the similarity tiles from the saved
+    log-sum-exps and routes the node gradient through the normalisation to each window's maximum. The teacher's
+    features are a constant: they get no gradient."""
+
+    @staticmethod
+    def forward(ctx, f_s, f_t, temperature, pool):
+        split = ops.is_split(f_s)
+        xs, arg, inv = ops.relation_nodes(f_s, pool, split, student=True)
+        xt = ops.relation_nodes(f_t, pool, split)[0]
+        loss, lse = ops.relation_kl_fwd(xs, xt, temperature)
+        ctx.save_for_backward(f_s, xs, xt, arg, inv, lse)
+        ctx.cfg = (temperature, pool)
+        return loss.view(())
+
+    @staticmethod
+    def backward(ctx, grad):
+        f_s, xs, xt, arg, inv, lse = ctx.saved_tensors
+        temperature, pool = ctx.cfg
+        dn = ops.relation_kl_bwd(xs, xt, temperature, lse, grad)
+        return ops.relation_nodes_bwd(f_s, pool, arg, inv, dn), None, None, None
+
+
+def relation_kd(f_s, f_t, temperature, pool):
+    """CIRKD's mini-batch pixel-to-pixel relation term (losses.DistillationLoss states it) of NHWC activations
+    f_s, f_t [B,h,w,512] -> fp32 scalar, differentiable in f_s. There is no fallback: another width, a pool outside
+    [1, 16] or mismatched shapes raise."""
+    if tuple(f_s.shape[-4:]) != tuple(f_t.shape[-4:]):
+        raise ValueError("relation_kd: the student's features %s and the teacher's %s differ in shape" %
+                         (tuple(f_s.shape[-4:]), tuple(f_t.shape[-4:])))
+    if f_s.shape[-1] != ops.RELATION_C:
+        raise ValueError("relation_kd: the relation kernels take %d channels, got %d (no fallback)" %
+                         (ops.RELATION_C, f_s.shape[-1]))
+    return _RelationKD.apply(f_s, f_t.detach(), float(temperature), int(pool))
+
+
 def _class_weight_supported(weight, target, classes):
     """Class weights the fused kernels read: None, or a contiguous 1-D fp32 tensor on the target's CUDA device (of
     length `classes` when that is known)."""

@@ -63,11 +63,12 @@ def note_boundary(t):
 class _Step:
     __slots__ = ("key", "calls", "failed", "fwd", "bwd", "bwd2", "x", "y", "pred", "main", "aux", "g_main", "g_aux",
                  "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot", "mix",
-                 "mix_crit", "strong", "strong_crit", "fp", "fp_crit")
+                 "mix_crit", "strong", "strong_crit", "fp", "fp_crit", "rel", "rel_crit")
 
     def __init__(self, key):
         self.key, self.calls, self.failed, self.fwd, self.dx_slot = key, 0, False, None, False
         self.mix = self.mix_crit = self.strong = self.strong_crit = self.fp = self.fp_crit = None
+        self.rel = self.rel_crit = None
 
 
 def _set_grad_outputs(st, g_main, g_aux):
@@ -128,13 +129,15 @@ class _Replay(torch.autograd.Function):
 def _point_mix(st):
     """A losses.MixPseudoLabelLoss criterion's last_mix() is the replayed step's: its mask, mixed target and uniforms
     are that step's static tensors (each captured input shape has its own). So are a teacher criterion's last_strong()
-    and a pseudo-label criterion's last_fp()."""
+    and a pseudo-label criterion's last_fp(), and a distillation criterion's last_relation()."""
     if st.mix_crit is not None:
         st.mix_crit._mix_state = st.mix
     if st.strong_crit is not None:
         st.strong_crit._strong_state = st.strong
     if st.fp_crit is not None:
         st.fp_crit._fp_state = st.fp
+    if st.rel_crit is not None:
+        st.rel_crit._relation_state = st.rel
 
 
 def _with_dx(st, gs):
@@ -275,6 +278,9 @@ def _capture(model, impl, st, x, y):
     if getattr(crit, "fp_weight", 0.0) > 0.0:
         # and the feature perturbation's uniforms and scale
         st.fp, st.fp_crit = crit._fp_state, crit
+    if getattr(crit, "relation_weight", 0.0) > 0.0:
+        # and the relation term's features and loss
+        st.rel, st.rel_crit = crit._relation_state, crit
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
     del proxies, x_in, x_leaf
@@ -338,6 +344,9 @@ def train_step(model, impl, x, y):
                      tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
         crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight",
                                                              "fp_weight", "fp_dropout", "mix", "p", "area", "ratio"))
+        if getattr(crit, "relation_weight", 0.0) > 0.0:
+            # the relation term's kernels and arguments; at weight 0 the key is the one without the option
+            crit_key += ("relation", crit.relation_weight, crit.relation_temperature, crit.relation_pool)
         if getattr(crit, "streams", 1) != 1:
             crit_key += ("streams", crit.streams)          # a 2N-image student: other shapes and launches
         if crit.strong is not None:

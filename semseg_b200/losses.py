@@ -272,9 +272,9 @@ class _TeacherLoss(nn.Module):
         self._strong_state = {'image': xs, 'uniforms': u}
         return xs
 
-    def run_teacher(self, x, classes):
+    def run_teacher(self, x, classes, feature=False):
         """The teacher's detached fp32 NHWC 1/8-resolution logits of the input batch `x` (NCHW), for a student with
-        `classes` classes."""
+        `classes` classes; with `feature`, (logits, its cls[2] output [N, h', w', 512]) of the same eval forward."""
         from . import functional as SF
         from . import graphs
         name = type(self).__name__
@@ -295,6 +295,9 @@ class _TeacherLoss(nn.Module):
             # a mean teacher changes every step: its slabs are re-packed here, inside the captured step while capturing
             SF.prepack(teacher, force=graphs.capturing(), dgrad=False)
         with torch.no_grad(), SF.network_mode(False, False):
+            if feature:
+                logits, f, _ = teacher._logits_nhwc(x.detach(), relation=True)
+                return logits, f
             return teacher._eval_logits_nhwc(x.detach())
 
     def _teacher_logits_nhwc(self, logits, teacher_logits):
@@ -328,10 +331,31 @@ class DistillationLoss(_TeacherLoss):
     term graphed at every zoom factor. Called as a module, forward(logits, target, teacher_logits=None) takes NCHW logits
     at the target size: without teacher_logits it returns the student's mean cross-entropy (the validation loss
     validate() logs), with them (the same shape) `main` computed at that size. It runs the zoom-1 kernels on NHWC copies.
-    CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
+    CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback.
+
+    `relation_weight` > 0 adds CIRKD's mini-batch pixel-to-pixel relation term (Yang et al., "Cross-Image Relational
+    Knowledge Distillation for Semantic Segmentation", CVPR 2022), in the network's training forward only. With f_s the
+    student's cls[2] output (3x3 conv, BN, ReLU, before the dropout) and f_t the same point of the teacher's eval
+    forward, both [B, h', w', 512]:
+
+        nodes  X_i, Y_i [M, 512] of image i: max_pool2d(f, p, p, ceil_mode=True) per channel (p = relation_pool,
+               M = ceil(h'/p) ceil(w'/p)), each divided by its L2 norm (a node of norm < 1e-12 is the zero vector and
+               gets no gradient); rounded once to the precision mode's operand form (bf16, or hi + lo in bf16x3)
+        S_ij = X_i X_j^T / tau,  T_ij = Y_i Y_j^T / tau,  P = row-softmax(S), Q = row-softmax(T)  (tau =
+               relation_temperature; the softmax runs over the M nodes of image j)
+        R    = tau^2 / (B^2 M) sum over all ordered image pairs (i, j), i = j included, of sum_rows KL(Q_ij,row || P_ij,row)
+        main = the main above + relation_weight * R
+
+    B is the student's batch (per rank under DistributedDataParallel: each rank relates its own images; multi-GPU runs
+    have not been made). The teacher gets no gradient; the student's gradient reaches cls[2] beside the dropout's.
+    `aux`, `pred` and the pixel term are unchanged. On the native kernels of csrc/relation.cu, graphed with the step;
+    neither [B M, B M] map is stored. `last_relation()` returns {'student': f_s, 'teacher': f_t, 'loss': R} of the
+    latest training forward, graphed or eager (None before the first one, or with relation_weight 0).
+    relation_weight = 0 (the default) runs none of it: the step is the one without the option. The module form
+    forward(logits, target, teacher_logits) has no features, so it never has the relation term."""
 
     def __init__(self, teacher, temperature=1.0, kd_weight=1.0, ce_weight=1.0, ignore_index=255, at='output',
-                 strong=None):
+                 strong=None, relation_weight=0.0, relation_temperature=1.0, relation_pool=2):
         super(DistillationLoss, self).__init__(teacher, ignore_index, strong)
         if not isinstance(at, str):
             raise TypeError("at must be 'output' or 'logits', got %r" % (at,))
@@ -344,11 +368,41 @@ class DistillationLoss(_TeacherLoss):
         self.kd_weight = _non_negative("kd_weight", kd_weight)
         self.ce_weight = _non_negative("ce_weight", ce_weight)
         self.at = at
+        self.relation_weight = _non_negative("relation_weight", relation_weight)
+        relation_temperature = _non_negative("relation_temperature", relation_temperature)
+        if relation_temperature <= 0.0:
+            raise ValueError("relation_temperature must be > 0, got %r" % relation_temperature)
+        self.relation_temperature = relation_temperature
+        if isinstance(relation_pool, bool) or not isinstance(relation_pool, int):
+            raise TypeError("relation_pool must be an int, got %r" % (relation_pool,))
+        if not 1 <= relation_pool <= 16:
+            raise ValueError("relation_pool must lie in [1, 16], got %r" % relation_pool)
+        self.relation_pool = relation_pool
+        self._relation_state = None
 
     def extra_repr(self):
-        return "teacher=%s, temperature=%g, kd_weight=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
-            type(self.teacher).__name__, self.temperature, self.kd_weight, self.ce_weight, self.ignore_index,
-            self.at) + self._strong_repr()
+        s = "teacher=%s, temperature=%g, kd_weight=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
+            type(self.teacher).__name__, self.temperature, self.kd_weight, self.ce_weight, self.ignore_index, self.at)
+        if self.relation_weight > 0.0:
+            s += ", relation_weight=%g, relation_temperature=%g, relation_pool=%d" % (
+                self.relation_weight, self.relation_temperature, self.relation_pool)
+        return s + self._strong_repr()
+
+    def last_relation(self):
+        """{'student', 'teacher', 'loss'} of the latest training forward's relation term (None before the first one,
+        or with relation_weight 0)."""
+        return None if self._relation_state is None else dict(self._relation_state)
+
+    def relation(self, f_s, f_t):
+        """R of the student's and the teacher's cls[2] features (unweighted; differentiable in f_s); remembered for
+        last_relation()."""
+        from . import functional as SF
+        if tuple(f_s.shape[-4:]) != tuple(f_t.shape[-4:]):
+            raise ValueError("DistillationLoss: the student's relation features %s and the teacher's %s differ in "
+                             "shape (channels or grid)" % (tuple(f_s.shape[-4:]), tuple(f_t.shape[-4:])))
+        r = SF.relation_kd(f_s, f_t, self.relation_temperature, self.relation_pool)
+        self._relation_state = {'student': f_s.detach(), 'teacher': f_t.detach(), 'loss': r.detach()}
+        return r
 
     def forward(self, logits, target, teacher_logits=None):
         from . import functional as SF

@@ -1032,6 +1032,86 @@ def upsample_kd_bwd(student, teacher, temperature, kd_weight, lse, grad_out, dlo
     return dlogits
 
 
+RELATION_C = 512          # csrc/relation.cu kRlC: the feature width the relation kernels are specialised to
+
+
+def relation_grid(h, w, pool):
+    """Nodes per image of an h x w feature map pooled p x p in ceil mode."""
+    return ((h + pool - 1) // pool) * ((w + pool - 1) // pool)
+
+
+def _lo_nodes(t):
+    """Pointer to the lo plane of split relation nodes [2,B,M,C], NULL for plain ones [B,M,C]."""
+    return ctypes.c_void_p(t[1].data_ptr()) if t.dim() == 4 else ctypes.c_void_p(0)
+
+
+def relation_nodes(feat, pool, split, student=False):
+    """Relation nodes of a [B,h,w,512] activation (either storage form; include/semseg_b200.h states the contract) ->
+    (nodes bf16 [B,M,512], or [2,B,M,512] hi / lo planes when `split`; with `student` also the window offsets uint8
+    [B,M,512] and 1/|x| fp32 [B,M], else None, None)."""
+    _require_cuda(feat)
+    lib = _lib.load()
+    b, h, w, c, pitch = _nhwc_meta(feat)
+    m = relation_grid(h, w, pool)
+    dev = feat.device
+    nodes = torch.empty(((2,) if split else ()) + (b, m, c), dtype=torch.bfloat16, device=dev)
+    arg = inv = None
+    if student:
+        arg = torch.empty((b, m, c), dtype=torch.uint8, device=dev)
+        inv = torch.empty((b, m), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_relation_nodes(_ptr(feat), _lo(feat), pitch, b, h, w, c, int(pool), _ptr(nodes),
+                                         _lo_nodes(nodes), _ptr(arg), _ptr(inv), _stream()), "semseg_relation_nodes")
+    return nodes, arg, inv
+
+
+def _relation_kl_meta(xs, xt):
+    assert xs.shape == xt.shape and xs.dtype == xt.dtype == torch.bfloat16 and xs.is_contiguous() and \
+        xt.is_contiguous(), "student and teacher nodes differ"
+    return xs.shape[-3], xs.shape[-2], xs.shape[-1]
+
+
+def relation_kl_fwd(xs, xt, temperature):
+    """The relation KL of student / teacher nodes (relation_nodes') -> (loss [1] = tau^2/(B^2 M) sum KL,
+    lse fp32 [B,B,M,2])."""
+    _require_cuda(xs, xt)
+    lib = _lib.load()
+    b, m, c = _relation_kl_meta(xs, xt)
+    nws = int(lib.semseg_relation_workspace_floats(b, m))
+    _lib.check(0 if nws >= 0 else nws, "semseg_relation_workspace_floats")
+    dev = xs.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    lse = torch.empty((b, b, m, 2), dtype=torch.float32, device=dev)
+    loss = torch.empty((1,), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_relation_kl_fwd(_ptr(xs), _lo_nodes(xs), _ptr(xt), _lo_nodes(xt), b, m, c, float(temperature),
+                                          _ptr(ws), _ptr(lse), _ptr(loss), _stream()), "semseg_relation_kl_fwd")
+    return loss, lse
+
+
+def relation_kl_bwd(xs, xt, temperature, lse, grad_out):
+    """grad_out * d loss / d (student nodes) -> fp32 [B,M,512]."""
+    lib = _lib.load()
+    b, m, c = _relation_kl_meta(xs, xt)
+    assert lse.shape == (b, b, m, 2) and lse.dtype == torch.float32 and lse.is_contiguous()
+    dn = torch.empty((b, m, c), dtype=torch.float32, device=xs.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_relation_kl_bwd(_ptr(xs), _lo_nodes(xs), _ptr(xt), _lo_nodes(xt), b, m, c, float(temperature),
+                                          _ptr(lse), _ptr(g), _ptr(dn), _stream()), "semseg_relation_kl_bwd")
+    return dn
+
+
+def relation_nodes_bwd(feat, pool, arg, inv, dnodes):
+    """The gradient of the features `feat` [B,h,w,512] from the nodes' fp32 gradient, through the normalisation and the
+    saved window maxima, in feat's storage form."""
+    lib = _lib.load()
+    b, h, w, c, pitch = _nhwc_meta(feat)
+    assert dnodes.dtype == torch.float32 and dnodes.is_contiguous() and dnodes.shape == (b, relation_grid(h, w, pool), c)
+    df = empty_act((b, h, w, c), is_split(feat), feat.device)
+    _lib.check(lib.semseg_relation_nodes_bwd(_ptr(feat), _lo(feat), pitch, b, h, w, c, int(pool), _ptr(arg), _ptr(inv),
+                                             _ptr(dnodes), _ptr(df), _lo(df), c, _stream()),
+               "semseg_relation_nodes_bwd")
+    return df
+
+
 def upsample_pl_fwd(student, teacher, target, ignore_index, threshold, pl_weight, ce_weight, want_argmax=True,
                     zoom=8, mix_mask=None):
     """Confidence-masked pseudo-label cross-entropy on the fused tail (include/semseg_b200.h states the contract):

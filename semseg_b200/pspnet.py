@@ -45,11 +45,17 @@ class PPM(nn.Module):
         return SF.to_nchw_f32(self.forward_nhwc(SF.to_nhwc_bf16(x)))
 
 
-def head_forward_nhwc(head, t):
-    """cls / aux head: 3x3 conv + BN + ReLU + Dropout2d + 1x1 conv with bias -> fp32 NHWC logits."""
+def head_forward_nhwc(head, t, feature=False):
+    """cls / aux head: 3x3 conv + BN + ReLU + Dropout2d + 1x1 conv with bias -> fp32 NHWC logits. With `feature`:
+    (logits, the ReLU output before the dropout), the feature a second consumer (the relation term) reads; the two
+    gradients meet in a split-aware fork."""
     t = SF.conv_bn_act(t, head[0], head[1], relu=True)
+    f = None
+    if feature:
+        t, f = SF.fork(t, 2)
     t = SF.dropout2d_nhwc(t, head[3].p, head[3].training)
-    return SF.conv_bias_f32(t, head[4])
+    out = SF.conv_bias_f32(t, head[4])
+    return (out, f) if feature else out
 
 
 def upsample_logits(logits_nhwc, size, zoom_factor):
@@ -147,8 +153,9 @@ class _SegNet(nn.Module):
         if self.training and torch.is_grad_enabled():
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
-        t_logits = mix_mask = fp_scale = None
+        t_logits = mix_mask = fp_scale = t_feat = None
         streams = 1
+        relation = False
         if self.training and y is not None and isinstance(self.criterion, losses._TeacherLoss):
             classes = self.cls[4].out_channels
             mixing = isinstance(self.criterion, losses.MixPseudoLabelLoss)
@@ -160,7 +167,11 @@ class _SegNet(nn.Module):
                 fp_scale = self.criterion.fp_draw(x, self.layer4[-1].conv3.out_channels)
             # the teacher first (distillation, pseudo-labels): its activations are transient before the student's saved
             # ones exist. It sees the batch; the student and both heads' losses see its strong view, mixed
-            t_logits = self.criterion.run_teacher(x, classes)
+            relation = getattr(self.criterion, "relation_weight", 0.0) > 0.0
+            if relation:
+                t_logits, t_feat = self.criterion.run_teacher(x, classes, feature=True)
+            else:
+                t_logits = self.criterion.run_teacher(x, classes)
             if strong is not None:
                 x = self.criterion.strong_streams(x, u_s) if streams > 1 else self.criterion.strong_view(x, u_s)
             if mixing:
@@ -168,7 +179,10 @@ class _SegNet(nn.Module):
         # the student's batch: `streams` views of the N images, stream-major, and with the FP stream stream 1's
         # perturbed copy after them. Each stream's logits, aux logits, target and mix mask are a contiguous N-image chunk
         # without the FP stream the call is the one-argument form it always was (subclasses and wrappers override it)
-        out, t_aux = self._logits_nhwc(x) if fp_scale is None else self._logits_nhwc(x, fp_scale)
+        if relation:
+            out, f_s, t_aux = self._logits_nhwc(x, relation=True)
+        else:
+            out, t_aux = self._logits_nhwc(x) if fp_scale is None else self._logits_nhwc(x, fp_scale)
         logits = _chunks(out, streams + (fp_scale is not None))
         fp_logits = logits[streams] if fp_scale is not None else None
 
@@ -188,6 +202,8 @@ class _SegNet(nn.Module):
                                                            t_logits, masks[0])[0]
                 aux_loss = _stream_mean([SF.upsample_ce(a, y_k, self.criterion.ignore_index, self.zoom_factor,
                                                         criterion=self.criterion)[0] for a, y_k in zip(aux_logits, ys)])
+                if relation:
+                    main_loss = main_loss + self.criterion.relation_weight * self.criterion.relation(f_s, t_feat)
                 return preds[0], main_loss, aux_loss
             ups = [upsample_logits(v, (h, w), self.zoom_factor) for v in logits[:streams]]
             aux_ups = [upsample_logits(v, (h, w), self.zoom_factor) for v in aux_logits]
@@ -206,6 +222,8 @@ class _SegNet(nn.Module):
             else:
                 main_loss = self.criterion(ups[0], y)
             aux_loss = _stream_mean([self.criterion(a, y_k) for a, y_k in zip(aux_ups, ys)])
+            if relation:
+                main_loss = main_loss + self.criterion.relation_weight * self.criterion.relation(f_s, t_feat)
             return ups[0].max(1)[1], main_loss, aux_loss
         else:
             x = logits[0]
@@ -214,11 +232,13 @@ class _SegNet(nn.Module):
                 x = F.interpolate(x, size=(h, w), mode='bilinear', align_corners=True)
             return x
 
-    def _logits_nhwc(self, x, fp_scale=None):
+    def _logits_nhwc(self, x, fp_scale=None, relation=False):
         """fp32 NHWC classifier logits [M, h', w', classes] of an M-image batch before the final upsample, and in
         training mode layer3's output for the aux head (None in eval mode). With `fp_scale` (fp32 [N, 2048], N <= M, the
         feature-perturbation factor of losses.PseudoLabelLoss) the context module and cls run on cat(f, f[:N] *
-        fp_scale) of layer4's output f: logits [M + N, h', w', classes], the unperturbed images first."""
+        fp_scale) of layer4's output f: logits [M + N, h', w', classes], the unperturbed images first. With `relation`
+        a third value follows: cls[2]'s output [M, h', w', 512] before the dropout (losses.DistillationLoss's relation
+        term)."""
         t = self.layer0.forward_nchw(x)          # x.grad, when asked for, straight from the stem dgrad kernel
         t = self.layer1.forward_nhwc(t)
         t = graphs.note_boundary(self.layer2.forward_nhwc(t))     # where a captured backward is cut in two
@@ -229,6 +249,8 @@ class _SegNet(nn.Module):
         t = self.layer4.forward_nhwc(t_tmp)
         if fp_scale is not None:
             t = SF.fp_fork(t, fp_scale)
+        if relation:
+            return head_forward_nhwc(self.cls, self._context_nhwc(t), feature=True) + (t_aux,)
         return head_forward_nhwc(self.cls, self._context_nhwc(t)), t_aux
 
     def _eval_logits_nhwc(self, x):
