@@ -28,6 +28,7 @@
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
  *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
  *                               semseg_upsample_pl_*: confidence-masked pseudo-labels from a teacher's logits.
+ *                               semseg_upsample_ce_entropy_*: entropy minimisation, plus cross-entropy.
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -685,6 +686,35 @@ int semseg_upsample_pl_mix_fwd(const float* student, int pitch_s, const float* t
                                float threshold, float pl_weight, float ce_weight, const uint8_t* mix_mask,
                                float* workspace, float* loss_out, int64_t* argmax, float* lse, int64_t* eff_target,
                                float* weight, void* stream);
+/* Entropy minimisation plus cross-entropy (TENT, ADVENT's MinEnt, entropy regularisation; semseg_b200/losses.py
+ * EntropyLoss) on the same fused upsample at zoom `zoom`. Per output pixel, with s the upsampled logits,
+ * L = {0 <= target < C, target != ignore_index}, U = {target == ignore_index}, p = softmax(s), lse = logsumexp(s) and
+ * H = lse - sum_c p_c s_c (natural log):
+ *   loss = ce_weight (1/|L|) sum_L (lse - s_target) + ent_weight (1/|U|) sum_U H
+ *   dloss/ds_c = ce_weight/|L| (p_c - [c = t]) on L,   -ent_weight/|U| p_c (s_c - lse + H) = ent_weight/|U| p_c (mu - s_c)
+ *   on U, with mu = sum_c p_c s_c the softmax-expected logit.
+ * A term whose set is empty is 0 with an exactly zero gradient; other out-of-range targets belong to neither set. With
+ * m the pixel's max (at class a), S_o = sum_{c != a} exp(s_c - m), S = 1 + S_o and D = sum_c exp(s_c - m) (s_c - m) <= 0:
+ * H = log1p(S_o) - D / S (finite, >= 0 and relatively accurate however far the logits saturate) and mu = m + D / S
+ * (= s_c exactly for constant logits: a zero gradient).
+ *   fwd: loss_out fp32 [6] = (CE mean over L, |L|, H mean over U, |U|, 0, 1), so loss = ce_weight loss_out[0] +
+ *        ent_weight loss_out[2]; argmax (or NULL) and lse as the zoom forward's (the same bits); mu fp32 [N,Ho,Wo] per
+ *        pixel (kept for the backward); workspace: semseg_upsample_ce_entropy_workspace_floats() floats.
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits from the forward's lse, mu and loss_out (|L|, |U|);
+ *        ent_weight / ce_weight finite and >= 0; workspace: semseg_upsample_ce_entropy_bwd_workspace_floats() floats.
+ * The backward's staged rows take 12 bytes per pixel: the Dice width limit, Wo <= 229376 / (12 zoom), 2389 at zoom 8;
+ * both directions reject a wider target. A bad shape, zoom, pitch, weight, width, alignment or null pointer is rejected
+ * before any CUDA call; the workspace functions return -1 for a bad zoom or size. No atomics, no host synchronisation:
+ * deterministic. */
+long long semseg_upsample_ce_entropy_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_ce_entropy_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                   int Ho, int Wo, int zoom, int ignore_index, float* workspace, float* loss_out,
+                                   int64_t* argmax, float* lse, float* mu, void* stream);
+long long semseg_upsample_ce_entropy_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_entropy_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                   int Ho, int Wo, int zoom, int ignore_index, float ent_weight, float ce_weight,
+                                   const float* lse, const float* mu, const float* loss_info, const float* grad_out,
+                                   float* workspace, float* dlogits, void* stream);
 /* Mixed-sample masks and batches (csrc/mix.cu) for mean-teacher training. Image n is mixed with its partner
  * pi(n) = (n + 1) mod N; uniforms fp32 [N, ustride] hold u0 (apply), u1 (area), u2 (ratio), u3 (row), u4 (column) and,
  * for ClassMix, class priorities u[n, 5 + c]; image n is mixed iff (double) u0 < p.

@@ -48,6 +48,9 @@
 // Confidence-masked pseudo-labels from a teacher's logits run a count pass and a two-map forward (see "pseudo-labels"
 // below); their backward is the focal backward on the forward's effective targets and weights. No existing instance
 // changes.
+//
+// Entropy minimisation plus cross-entropy (TENT / MinEnt) runs sibling forward and rows kernels (see "entropy" below)
+// with the plain reduce and cols kernels; no existing instance changes.
 #include <cmath>
 
 #include "host_common.h"
@@ -2476,6 +2479,243 @@ upsample_ce_rmi_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- entropy
+// Entropy minimisation (TENT, ADVENT's MinEnt, entropy regularisation) plus cross-entropy, with s the logits after the
+// xZ upsample:
+//   L = {target in [0, C), target != ignore_index},  U = {target == ignore_index}
+//   p = softmax(s),  lse = logsumexp(s),  H = lse - sum_c p_c s_c = -sum_c p_c log p_c
+//   loss = ce_weight (1/|L|) sum_L (lse - s_target) + ent_weight (1/|U|) sum_U H
+//   dloss/ds_c = ce_weight/|L| (p_c - [c = t]) on L,   -ent_weight/|U| p_c (s_c - lse + H) on U
+// and s_c - lse + H = s_c - mu with mu = sum_c p_c s_c, the softmax-expected logit.
+// forward : the plain forward's two class passes (lse and argmax are the plain tail's bits); the second pass also sums,
+//           with e_c = exp(s_c - m) (m: the pixel's max, at class a), S_o = sum_{c != a} e_c with a's term skipped, not
+//           subtracted, and D = sum_c e_c (s_c - m) <= 0. With S = 1 + S_o (a's term exactly 1): mu = m + D / S and
+//           H = log1p(S_o) - D / S, two non-negative terms. So H is >= 0, finite, and keeps its relative accuracy when
+//           the logits saturate (a term whose e_c underflowed adds exactly 0; log S is not a rounded log near 1). Per
+//           pixel lse and mu are written; per CTA (sum CE over L, |L|) and (sum H over U, |U|), each reduced in fp64 by
+//           the plain reduce kernel, as the pseudo-label forward does. Constant logits give D = 0 and mu = s_c exactly.
+// backward: the rows kernel stages (lse, class or U marker, mu) per pixel, the Dice 12-byte word, and reads |L| and |U|
+//           from the forward's loss words for the two per-pixel weights; the plain cols kernel with a count of 1.
+// loss_out: [0] CE mean over L, [1] |L|, [2] H mean over U, [3] |U|, [4] 0, [5] 1 (the cols kernel's count).
+constexpr int kEntNone = -1;   // staged target of a pixel with no term (or whose term has weight 0)
+constexpr int kEntU = -2;      // staged target of an unlabelled pixel
+
+template <int Z>
+__global__ void __launch_bounds__(kFwdCols)
+upsample_ce_entropy_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
+                               const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                               float* __restrict__ partial, float* __restrict__ loss_out,
+                               long long* __restrict__ argmax_out, float* __restrict__ lse_out,
+                               float* __restrict__ mu_out) {
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs] as in upsample_ce_fwd_kernel
+  __shared__ float red[4][kFwdCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kFwdNodes, w - j_base);
+  const int tid = threadIdx.x;
+  if ((blockIdx.x | blockIdx.y | blockIdx.z) == 0 && tid == 0) {
+    loss_out[4] = 0.f;
+    loss_out[5] = 1.f;
+  }
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * kFwdNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
+  }
+  __syncthreads();
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};   // sum CE over L, |L|, sum H over U, |U|
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* A = S + (j0 - j_base) * Cs;
+    const float* B = S + (j1 - j_base) * Cs;
+    const float* Cc = A + kFwdNodes * Cs;
+    const float* D = B + kFwdNodes * Cs;
+    float m[Z], sum[Z], so[Z], sd[Z];   // so: S_o = sum_{c != argmax} e_c; sd: D = sum_c e_c (s_c - m) <= 0
+    int am[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      m[r] = -INFINITY;
+      am[r] = 0;
+      sum[r] = 0.f;
+      so[r] = 0.f;
+      sd[r] = 0.f;
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        if (v > m[r]) {
+          m[r] = v;
+          am[r] = c;
+        }
+      }
+    }
+    float m2[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) m2[r] = m[r] * kLog2e;
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        const float e = ex2_approx(fmaf(v, kLog2e, -m2[r]));   // the plain forward's sum
+        sum[r] += e;
+        so[r] += c == am[r] ? 0.f : e;
+        sd[r] = fmaf(e, v - m[r], sd[r]);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+        const long long t = target[pix];
+        const float lse = m[r] + __logf(sum[r]);
+        const float dm = sd[r] / (1.f + so[r]);   // D / S with the argmax's term taken as exactly 1
+        if (argmax_out) argmax_out[pix] = am[r];
+        lse_out[pix] = lse;
+        mu_out[pix] = m[r] + dm;
+        if (t == ignore_index) {
+          const float H = log1pf(so[r]) - dm;
+          acc[2] += H;
+          acc[3] += 1.f;
+        } else if (t >= 0 && t < C) {
+          const int tc = static_cast<int>(t);
+          const float top = Z == 1 ? A[tc] : l0w * A[tc] + l1w * B[tc];
+          const float bot = Z == 1 ? 0.f : l0w * Cc[tc] + l1w * D[tc];
+          acc[0] += lse - row_lerp<Z>(top, bot, r);
+          acc[1] += 1.f;
+        }
+      }
+    }
+  }
+  // deterministic block reduction -> (sum CE, |L|) and (sum H, |U|) per CTA, each laid out as the plain partials
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    for (int o = 16; o > 0; o >>= 1) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], o);
+  }
+  if ((tid & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) red[k][tid >> 5] = acc[k];
+  }
+  __syncthreads();
+  if (tid < 4) {
+    float s = 0.f;
+    for (int i = 0; i < kFwdCols / 32; ++i) s += red[tid][i];
+    const size_t nb = static_cast<size_t>(gridDim.x) * gridDim.y * gridDim.z;
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[(tid >> 1) * 2 * nb + 2 * b + (tid & 1)] = s;
+  }
+}
+
+// One interval of the entropy rows kernel for class c, folded as in upsample_ce_bwd_rows_kernel. DicePix::t is the
+// target class on L, kEntU on U; DicePix::g holds mu.
+template <int Z, bool kFull>
+__device__ __forceinline__ void entropy_interval(const DicePix* s, int Wo, int xb, int rows, int nx, int c, float a,
+                                                 float b, float cc, float d, float wl, float wu, float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const DicePix pi = s[r * Wo + xb + k];
+      if (pi.t == kEntNone) continue;  // warp-uniform
+      const float v = row_lerp<Z>(top, bot, r);
+      const float p = ex2_approx(fmaf(v, kLog2e, -pi.lse2));
+      const float g = pi.t >= 0 ? wl * (p - (c == pi.t ? 1.f : 0.f)) : wu * p * (pi.g - v);
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+// Rows layout of upsample_ce_bwd_rows_kernel with the Dice rows kernel's 12-byte pixel word (lse, target / kEntU, mu).
+// The weights ce_weight / |L| and ent_weight / |U| come from the forward's loss words (0 for an empty set); a pixel
+// whose term has weight 0 is staged as kEntNone: its gradient is exactly 0.
+template <int Z>
+__global__ void __launch_bounds__(256)
+upsample_ce_entropy_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
+                                const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
+                                float ent_weight, float ce_weight, const float* __restrict__ lse,
+                                const float* __restrict__ mu, const float* __restrict__ loss_info,
+                                float* __restrict__ T2) {
+  extern __shared__ DicePix s_dpix[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  const float nl = loss_info[1], nu = loss_info[3];
+  const float wl = nl > 0.f ? ce_weight / nl : 0.f;
+  const float wu = nu > 0.f ? ent_weight / nu : 0.f;
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const long long t = target[rowbase + x];
+      DicePix pi;
+      if (t == ignore_index) {
+        pi.t = wu != 0.f ? kEntU : kEntNone;
+      } else {
+        pi.t = (t >= 0 && t < C && wl != 0.f) ? static_cast<int>(t) : kEntNone;
+      }
+      pi.g = mu[rowbase + x];
+      pi.lse2 = lse[rowbase + x] * kLog2e;
+      s_dpix[r * Wo + x] = pi;
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
+  const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  float a = L0[0], cc = L1[0];
+  float nb = L0[static_cast<size_t>(min(1, w - 1)) * pitch], nd = L1[static_cast<size_t>(min(1, w - 1)) * pitch];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd;
+    const int jn = min(j0 + 2, w - 1);
+    nb = L0[static_cast<size_t>(jn) * pitch];
+    nd = L1[static_cast<size_t>(jn) * pitch];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      entropy_interval<Z, true>(s_dpix, Wo, xb, rows, nx, c, a, b, cc, d, wl, wu, acc);
+    } else {
+      entropy_interval<Z, false>(s_dpix, Wo, xb, rows, nx, c, a, b, cc, d, wl, wu, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -3681,6 +3921,126 @@ extern "C" int semseg_upsample_pl_mix_fwd(const float* student, int pitch_s, con
     default: return launch_pl_fwd<8, true>(student, pitch_s, teacher, pitch_t, N, h, w, C, target, Ho, Wo,
                                            ignore_index, threshold, pl_weight, ce_weight, workspace, loss_out, argmax,
                                            lse, eff_target, weight, stream, mix_mask);
+  }
+}
+
+// Entropy (+ CE) at zoom factor `zoom`: its own forward and rows kernels, the plain reduce (twice) and cols kernels. The
+// rows kernel stages the Dice rows kernel's 12-byte words: the Dice width limit, checked by both directions.
+// Forward workspace: 2 x (value, count) partials per forward CTA.
+static int check_entropy(int zoom, int Wo, const void* lse, const void* mu) {
+  SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(lse) | reinterpret_cast<uintptr_t>(mu)) & 3) == 0,
+               "upsample_ce_entropy: lse or mu map not 4-byte aligned");
+  const size_t max_wo = kDiceSmemMax / (static_cast<size_t>(zoom) * sizeof(DicePix));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_ce_entropy: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_entropy_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                              int Ho, int Wo, int ignore_index, float* workspace, float* loss_out, int64_t* argmax,
+                              float* lse, float* mu, cudaStream_t stream) {
+  const int Cs = C | 1;
+  const int ctas = fwd_ctas(N, h, Wo);
+  constexpr size_t kMaxSmem =
+      static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_entropy_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_ce_entropy_fwd_kernel<Z><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, workspace,
+      loss_out, reinterpret_cast<long long*>(argmax), lse, mu);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, ctas, loss_out);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace + 2LL * ctas, ctas, loss_out + 2);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_entropy_bwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                              int Ho, int Wo, int ignore_index, float ent_weight, float ce_weight, const float* lse,
+                              const float* mu, const float* loss_info, const float* grad_out, float* workspace,
+                              float* dlogits, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(DicePix);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_entropy_rows_kernel<Z>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  upsample_ce_entropy_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, ent_weight,
+      ce_weight, lse, mu, loss_info, workspace);
+  SB_LAUNCHED();
+  // loss_info[5] = 1: the per-pixel weights are in T2 already
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info + 4, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_entropy_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_entropy: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0, "upsample_ce_entropy: bad sizes");
+  return 2 * semseg_upsample_ce_zoom_workspace_floats(N, Ho, Wo, zoom);
+}
+
+extern "C" int semseg_upsample_ce_entropy_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                              const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                              float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                              float* mu, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_entropy(zoom, Wo, lse, mu);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && mu, "upsample_ce_entropy_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_entropy_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                         argmax, lse, mu, stream);
+    case 2: return launch_entropy_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                         argmax, lse, mu, stream);
+    case 4: return launch_entropy_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace, loss_out,
+                                         argmax, lse, mu, stream);
+    default: return launch_entropy_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, workspace,
+                                          loss_out, argmax, lse, mu, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_entropy_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_ce_entropy: zoom %d is not one of 1, 2, 4, 8", zoom);
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_ce_entropy_bwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                              const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                              float ent_weight, float ce_weight, const float* lse, const float* mu,
+                                              const float* loss_info, const float* grad_out, float* workspace,
+                                              float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_entropy(zoom, Wo, lse, mu);
+  if (r) return r;
+  SB_CHECK_ARG(std::isfinite(ent_weight) && ent_weight >= 0.f,
+               "upsample_ce_entropy: ent_weight %g is not finite and >= 0", ent_weight);
+  SB_CHECK_ARG(std::isfinite(ce_weight) && ce_weight >= 0.f,
+               "upsample_ce_entropy: ce_weight %g is not finite and >= 0", ce_weight);
+  SB_CHECK_ARG(lse && mu && loss_info && grad_out && workspace && dlogits, "upsample_ce_entropy_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_entropy_bwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ent_weight,
+                                         ce_weight, lse, mu, loss_info, grad_out, workspace, dlogits, stream);
+    case 2: return launch_entropy_bwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ent_weight,
+                                         ce_weight, lse, mu, loss_info, grad_out, workspace, dlogits, stream);
+    case 4: return launch_entropy_bwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ent_weight,
+                                         ce_weight, lse, mu, loss_info, grad_out, workspace, dlogits, stream);
+    default: return launch_entropy_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ent_weight,
+                                          ce_weight, lse, mu, loss_info, grad_out, workspace, dlogits, stream);
   }
 }
 

@@ -623,6 +623,28 @@ class _UpsampleCEFocal(torch.autograd.Function):
         return dl, None, None, None, None, None
 
 
+class _UpsampleCEEntropy(torch.autograd.Function):
+    """The fused tail with losses.EntropyLoss: ce_weight * CE over the labelled pixels plus ent_weight * the mean
+    softmax entropy over the unlabelled ones. The forward keeps each pixel's lse and expected logit; the backward
+    weighs the two sets with the forward's counts on the device."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, ent_weight, ce_weight):
+        info, amax, lse, mu = ops.upsample_ce_entropy_fwd(logits, target, ignore_index, zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, mu, info)
+        ctx.cfg = (ignore_index, zoom, ent_weight, ce_weight)
+        ctx.mark_non_differentiable(amax)
+        return torch.add(info[0] * ce_weight, info[2], alpha=ent_weight), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, mu, info = ctx.saved_tensors
+        ignore_index, zoom, ent_weight, ce_weight = ctx.cfg
+        dl = ops.upsample_ce_entropy_bwd(logits, target, ignore_index, ent_weight, ce_weight, lse, mu, info, grad_loss,
+                                         zoom=zoom)
+        return dl, None, None, None, None, None
+
+
 class _UpsampleCELovasz(torch.autograd.Function):
     """The fused tail with losses.LovaszSoftmaxLoss, plus ce_weight * CE. The forward keeps the per pixel-class
     Lovász gradient weights (gamma, 4 C bytes per output pixel) it scattered from the sorted segments; the sort's
@@ -791,8 +813,9 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     contiguous fp32 [classes] tensor on that device; any other weight, another reduction, and any subclass keep the
     ATen tail. DiceLoss, FocalLoss and losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
-    form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, the Dice
-    width limit. losses.RMILoss needs a target of at least 12 x 12 and no wider than its rows kernel stages (3584 columns
+    form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
+    losses.EntropyLoss, whose rows kernel stages the same words, the Dice width limit. losses.RMILoss needs a target of
+    at least 12 x 12 and no wider than its rows kernel stages (3584 columns
     at zoom 8).
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
@@ -802,8 +825,9 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         plain = criterion.weight is None and eps == 0.0
         ok = (criterion.reduction == 'mean' and 0.0 <= eps <= 1.0 and
               (plain or (target is not None and target.is_cuda)))
-    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss, losses.PseudoLabelLoss, losses.MixPseudoLabelLoss):
-        # the focal rows kernel (the pseudo-label backward too) stages the Dice words
+    elif type(criterion) in (losses.DiceLoss, losses.FocalLoss, losses.PseudoLabelLoss, losses.MixPseudoLabelLoss,
+                             losses.EntropyLoss):
+        # the focal rows kernel (the pseudo-label backward too) and the entropy rows kernel stage the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     elif type(criterion) is losses.RMILoss:
@@ -843,7 +867,9 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     (the student's shape), its distillation loss, and with a losses.PseudoLabelLoss and them its pseudo-label loss
     (without them: the plain mean CE, the loss of the aux head). With a losses.MixPseudoLabelLoss, the teacher's logits
     of the unmixed batch and the mix mask `mix_mask` (ops.mix_apply's), the mixed pseudo-label loss on the mixed target;
-    without the mask it is a losses.PseudoLabelLoss. The default criterion runs the plain kernels."""
+    without the mask it is a losses.PseudoLabelLoss. With a losses.EntropyLoss, its ce_weight * CE over the labelled
+    pixels plus ent_weight * mean entropy over the unlabelled ones (its own ignore_index); the networks score their aux
+    head with the plain form. The default criterion runs the plain kernels."""
     if type(criterion) is losses.MixPseudoLabelLoss and teacher_logits is not None and mix_mask is not None:
         return _UpsampleCEPLMix.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
                                       int(zoom), criterion.threshold, criterion.pl_weight, criterion.ce_weight,
@@ -855,6 +881,9 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     if isinstance(criterion, losses.PseudoLabelLoss) and teacher_logits is not None:
         return _UpsampleCEPL.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
                                    int(zoom), criterion.threshold, criterion.pl_weight, criterion.ce_weight)
+    if isinstance(criterion, losses.EntropyLoss):
+        return _UpsampleCEEntropy.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                        criterion.ent_weight, criterion.ce_weight)
     if isinstance(criterion, losses.LovaszSoftmaxLoss):
         return _UpsampleCELovasz.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
                                        criterion.classes == 'all', bool(criterion.per_image), criterion.ce_weight)

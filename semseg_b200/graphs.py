@@ -19,7 +19,7 @@ Limits (same as torch.cuda.make_graphed_callables): a second training forward be
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
 The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
 cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
-loss, the focal loss, the RMI loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
+loss, the focal loss, the RMI loss, the entropy loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
 mean teacher's re-pack included, the pseudo-label losses' feature-perturbation stream and second strong stream, and the CutMix / ClassMix
 pseudo-label loss, its draws and mixing included, with or without a strong view of the student's input) are not captured (such models simply stay eager).
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
@@ -316,17 +316,19 @@ def train_step(model, impl, x, y):
     # BatchNorm modes (batch statistics or frozen) decide which kernels the step runs: freezing or unfreezing a layer
     # after a capture must capture again, not replay the old step
     bn_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm))
+    # likewise the heads' Dropout2d modes: a dropout switched to eval mode (adapt.Tent) runs no mask kernel
+    drop_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.Dropout2d))
     # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
     # the criterion's options are launch arguments baked into the graph: a changed thresh, ignore_index,
-    # label_smoothing, Dice smooth / eps / ce_weight, Lovász classes / per_image, focal gamma or RMI bce_weight /
-    # pos_alpha captures anew, and so
+    # label_smoothing, Dice smooth / eps / ce_weight, Lovász classes / per_image, focal gamma, RMI bce_weight /
+    # pos_alpha or entropy ent_weight captures anew, and so
     # does a replaced class-weight tensor (its address is baked in); an in-place edit of the weights needs no capture,
     # the kernels read them at every replay
     crit = getattr(model, "criterion", None)
     crit_key = (type(crit),) + tuple(getattr(crit, a, None) for a in ("ignore_index", "thresh", "min_kept",
                                                                       "label_smoothing", "reduction", "smooth", "eps",
                                                                       "ce_weight", "classes", "per_image", "gamma",
-                                                                      "bce_weight", "pos_alpha"))
+                                                                      "bce_weight", "pos_alpha", "ent_weight"))
     cw = getattr(crit, "weight", None)
     crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
     teacher = _teacher(crit)
@@ -352,8 +354,8 @@ def train_step(model, impl, x, y):
         if crit.strong is not None:
             crit_key += ("strong",) + crit.strong.key()    # the strong view's options are launch arguments too
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
-           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, x.requires_grad,
-           crit_key)
+           dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, drop_modes,
+           x.requires_grad, crit_key)
     if x.requires_grad and x.dtype != torch.float32:
         return None                           # the captured input gradient is handed out in the parameters' fp32 buffer
     st = steps.get(key)

@@ -5,7 +5,9 @@ the network's fused tail (functional.upsample_ce) it runs inside the same kernel
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
 LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and FocalLoss, the softmax focal loss with
-optional class weights, run the same way, and so does RMILoss, the Region Mutual Information loss with its BCE term. DistillationLoss adds a
+optional class weights, run the same way, and so do RMILoss, the Region Mutual Information loss with its BCE term, and
+EntropyLoss, entropy minimisation on the unlabelled pixels plus cross-entropy on the labelled ones (TENT's objective,
+adapt.Tent). DistillationLoss adds a
 pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
 optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
@@ -207,6 +209,53 @@ class FocalLoss(nn.Module):
             raise ValueError("FocalLoss: weight must be contiguous fp32 [%d] on %s (no fallback), got %s [%d] on %s" %
                              (logits.shape[1], logits.device, w.dtype, w.numel(), w.device))
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+class EntropyLoss(nn.Module):
+    """Entropy minimisation plus cross-entropy: the test-time objective of TENT (Wang et al., ICLR 2021; adapt.Tent),
+    ADVENT's MinEnt loss (Vu et al., CVPR 2019) and the entropy regulariser of semi-supervised training (Grandvalet &
+    Bengio, NeurIPS 2004): entropy on the unlabelled pixels, cross-entropy on the labelled ones. With s the logits after
+    the network's bilinear xZ upsample (align_corners), per output pixel:
+
+        L    = {target in [0, C), target != ignore_index}       labelled pixels
+        U    = {target == ignore_index}                          unlabelled pixels (an unlabelled image: all ignore)
+        p    = softmax(s),  lse = logsumexp(s),  H = lse - sum_c p_c s_c       (= -sum_c p_c log p_c, natural log)
+        main = ce_weight (1/|L|) sum_L (lse - s_target) + ent_weight (1/|U|) sum_U H
+        aux  = plain CE of the aux head on L (ce_weight does not scale it)
+        pred = argmax of s
+
+    A term whose set is empty is 0 with an exactly zero gradient; a target outside [0, C) that is not ignore_index
+    belongs to neither set. ADVENT's normalised entropy, H / log C, is ent_weight = w / log(C). Under
+    DistributedDataParallel each rank averages over its own pixels.
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, graphed at every zoom
+    factor; called as a module, forward(logits, target) takes NCHW logits at the target size and returns `main`, on the
+    zoom-1 form of the kernels on an NHWC copy (validate() logs it). CUDA fp32 logits with at most 256 classes only:
+    there is no CPU or library fallback."""
+
+    def __init__(self, ignore_index=255, ent_weight=1.0, ce_weight=1.0):
+        super(EntropyLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        self.ignore_index = ignore_index
+        self.ent_weight = _non_negative("ent_weight", ent_weight)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+
+    def extra_repr(self):
+        return "ignore_index=%d, ent_weight=%g, ce_weight=%g" % (self.ignore_index, self.ent_weight, self.ce_weight)
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        _check_native_logits("EntropyLoss", logits, target)
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+    def aux_loss(self, logits, target):
+        """The aux head's loss, module form: the plain mean cross-entropy over L of NCHW logits at the target size."""
+        from . import functional as SF
+        _check_native_logits("EntropyLoss", logits, target)
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1)
         return loss
 
 

@@ -937,6 +937,50 @@ def upsample_ce_focal_bwd(logits, target, ignore_index, lse, mod, info, grad_out
     return dl
 
 
+def upsample_ce_entropy_fwd(logits, target, ignore_index, want_argmax=True, zoom=8):
+    """Entropy minimisation plus cross-entropy on the fused tail (include/semseg_b200.h states the contract); arguments as
+    upsample_ce_fwd -> (loss_info [6] = (CE mean over L, |L|, H mean over U, |U|, 0, 1), argmax, lse, mu). mu fp32
+    [N,Ho,Wo]: each pixel's softmax-expected logit sum_c p_c s_c, kept for the backward. The loss is ce_weight * loss_info[0] + ent_weight *
+    loss_info[2]; the weights enter at the backward."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_entropy_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_entropy_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((6,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse, mu = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
+    _lib.check(lib.semseg_upsample_ce_entropy_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                  int(zoom), int(ignore_index), _ptr(ws), _ptr(info), _ptr(amax),
+                                                  _ptr(lse), _ptr(mu), _stream()),
+               "semseg_upsample_ce_entropy_fwd")
+    return info, amax, lse, mu
+
+
+def upsample_ce_entropy_bwd(logits, target, ignore_index, ent_weight, ce_weight, lse, mu, info, grad_out, zoom=8):
+    """grad_out[0] * d(ce_weight * info[0] + ent_weight * info[2]) / dlogits -> fp32 [N,h,w,C], from the forward's lse,
+    mu and info."""
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_entropy_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_entropy_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_entropy_bwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                  int(zoom), int(ignore_index), float(ent_weight), float(ce_weight),
+                                                  _ptr(lse), _ptr(mu), _ptr(info), _ptr(g), _ptr(ws), _ptr(dl),
+                                                  _stream()),
+               "semseg_upsample_ce_entropy_bwd")
+    return dl
+
+
 def upsample_ce_lovasz_fwd(logits, target, ignore_index, classes_all, per_image, ce_weight, want_argmax=True, zoom=8,
                            return_workspace=False):
     """Lovász-Softmax loss (+ ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract) ->

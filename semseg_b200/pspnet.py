@@ -187,6 +187,8 @@ class _SegNet(nn.Module):
         fp_logits = logits[streams] if fp_scale is not None else None
 
         if self.training:
+            # losses.EntropyLoss scores the aux head with the plain cross-entropy over the labelled pixels
+            entropy = isinstance(self.criterion, losses.EntropyLoss)
             aux_logits = _chunks(head_forward_nhwc(self.aux, t_aux), streams)
             ys = _chunks(y, streams) if mix_mask is not None else (y,) * streams      # the mixed target is [2N]
             masks = _chunks(mix_mask, streams) if mix_mask is not None else (None,) * streams
@@ -200,8 +202,9 @@ class _SegNet(nn.Module):
                 if fp_logits is not None:
                     main_loss = main_loss + SF.upsample_fp(fp_logits, ys[0], self.zoom_factor, self.criterion,
                                                            t_logits, masks[0])[0]
+                aux_crit = None if entropy else self.criterion
                 aux_loss = _stream_mean([SF.upsample_ce(a, y_k, self.criterion.ignore_index, self.zoom_factor,
-                                                        criterion=self.criterion)[0] for a, y_k in zip(aux_logits, ys)])
+                                                        criterion=aux_crit)[0] for a, y_k in zip(aux_logits, ys)])
                 if relation:
                     main_loss = main_loss + self.criterion.relation_weight * self.criterion.relation(f_s, t_feat)
                 return preds[0], main_loss, aux_loss
@@ -221,7 +224,8 @@ class _SegNet(nn.Module):
                                                                    ys[0], t_ups[0])
             else:
                 main_loss = self.criterion(ups[0], y)
-            aux_loss = _stream_mean([self.criterion(a, y_k) for a, y_k in zip(aux_ups, ys)])
+            aux_fn = self.criterion.aux_loss if entropy else self.criterion
+            aux_loss = _stream_mean([aux_fn(a, y_k) for a, y_k in zip(aux_ups, ys)])
             if relation:
                 main_loss = main_loss + self.criterion.relation_weight * self.criterion.relation(f_s, t_feat)
             return ups[0].max(1)[1], main_loss, aux_loss
