@@ -29,6 +29,7 @@
  *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
  *                               semseg_upsample_pl_*: confidence-masked pseudo-labels from a teacher's logits.
  *                               semseg_upsample_ce_entropy_*: entropy minimisation, plus cross-entropy.
+ *                               semseg_gated_crf_*: the Gated CRF loss's pairwise term (csrc/crf.cu).
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -715,6 +716,35 @@ int semseg_upsample_ce_entropy_bwd(const float* logits, int pitch, int N, int h,
                                    int Ho, int Wo, int zoom, int ignore_index, float ent_weight, float ce_weight,
                                    const float* lse, const float* mu, const float* loss_info, const float* grad_out,
                                    float* workspace, float* dlogits, void* stream);
+/* Gated CRF loss (Obukhov et al., 2019; semseg_b200/losses.py GatedCRFLoss), the pairwise term, on the loss grid
+ * Hg x Wg = zoom (h-1)+1 x zoom (w-1)+1 of the fp32 NHWC logits [N,h,w,pitch] (zoom 1: the logits grid itself; zoom
+ * > 1: the tail's bilinear xZ upsample, align_corners). The image is fp32 NCHW [N,3,H,W], normalised as
+ * (rgb255 - mean) / std, with H = istride (Hg-1)+1 and W = istride (Wg-1)+1: grid pixel (y, x) takes its colour
+ * rgb = (image[.., istride y, istride x] std + mean) / 255. With p_i = softmax over the classes at grid pixel i,
+ * W(i) the (2 radius+1)^2 window around i without i and without pixels outside the grid, and positions in grid units:
+ *   k_ij = exp(-|pos_i - pos_j|^2 / (2 sigma_xy^2) - |rgb_i - rgb_j|^2 / (2 sigma_rgb^2))
+ *   G_ic = sum_{j in W(i)} k_ij p_jc,   S_i = sum_c p_ic G_ic,   CRF = (1/P) sum_i sum_{j in W(i)} k_ij (1 - p_i.p_j)
+ *   dCRF/ds_ic = -(2/P) p_ic (G_ic - S_i),   P = N Hg Wg.
+ *   fwd: lse fp32 [N,Hg,Wg], the per-pixel logsumexp on the grid: the zoom forward's lse (input), or, with compute_lse
+ *        (zoom 1 only), written here; s_out fp32 [N,Hg,Wg] = S (kept for the backward); loss_out fp32 [2] = (CRF, P)
+ *        through the tail's fp64 reduce; workspace: semseg_gated_crf_workspace_floats() floats (2 per 16x16 tile).
+ *   bwd: ADDS grad_out[0] * crf_weight * dCRF/dlogits into dlogits fp32 [N,h,w,C] (written before, e.g. by the
+ *        cross-entropy backward); workspace: semseg_gated_crf_bwd_workspace_floats() floats, 0 at zoom 1, else
+ *        N C Wg (Hg + h): the per-class output-resolution terms [N,Hg,Wg,C] and their row adjoint [N,h,Wg,C] (21
+ *        classes at 16 x 473^2, zoom 8: 0.34 GB; 150 classes: 2.4 GB).
+ * Limits: C <= 256, radius in [1, 8], sigmas finite and > 0, mean finite, std finite and > 0, crf_weight finite and
+ * >= 0, Hg <= 65535 * 16; any grid width. A bad argument is rejected before any CUDA call; the workspace functions return
+ * -1 for a bad zoom or size. No atomics, no host synchronisation: deterministic, and graph-capturable. */
+long long semseg_gated_crf_workspace_floats(int N, int h, int w, int zoom);
+int semseg_gated_crf_fwd(const float* logits, int pitch, int N, int h, int w, int C, int zoom, float* lse,
+                         int compute_lse, const float* image, int H, int W, int istride, int radius, float sigma_xy,
+                         float sigma_rgb, float mean0, float mean1, float mean2, float std0, float std1, float std2,
+                         float* workspace, float* s_out, float* loss_out, void* stream);
+long long semseg_gated_crf_bwd_workspace_floats(int N, int h, int w, int C, int zoom);
+int semseg_gated_crf_bwd(const float* logits, int pitch, int N, int h, int w, int C, int zoom, const float* lse,
+                         const float* image, int H, int W, int istride, int radius, float sigma_xy, float sigma_rgb,
+                         float mean0, float mean1, float mean2, float std0, float std1, float std2, const float* s_in,
+                         float crf_weight, const float* grad_out, float* workspace, float* dlogits, void* stream);
 /* Mixed-sample masks and batches (csrc/mix.cu) for mean-teacher training. Image n is mixed with its partner
  * pi(n) = (n + 1) mod N; uniforms fp32 [N, ustride] hold u0 (apply), u1 (area), u2 (ratio), u3 (row), u4 (column) and,
  * for ClassMix, class priorities u[n, 5 + c]; image n is mixed iff (double) u0 < p.

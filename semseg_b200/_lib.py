@@ -256,6 +256,12 @@ SIGNATURES = {
     "semseg_upsample_ce_entropy_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_entropy_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                                c_int, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_gated_crf_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_gated_crf_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int,
+                                     c_int, c_int, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_gated_crf_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_gated_crf_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int,
+                                     c_int, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_vp, c_f, c_vp, c_vp, c_vp, c_vp]),
     "semseg_mix_argmax_x8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "semseg_mix_select": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_vp, c_vp]),
     "semseg_mix_apply": (c_int, [c_int, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp, c_int,

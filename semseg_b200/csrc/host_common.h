@@ -53,6 +53,10 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
 // Pixel box (bh x bw <= max_pixels) maximising tile utilisation of an H x W map.
 void choose_box(int H, int W, int max_pixels, int* bh, int* bw);
 
+// The fused tail's fixed-order fp64 reduce of (sum, count) partial pairs (csrc/tail.cu): loss_out[0] = sum / max(count,
+// 1), loss_out[1] = count.
+int launch_mean_reduce(const float* partial, int nblocks, float* loss_out, cudaStream_t stream);
+
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
 // An activation operand of a kernel that accesses it in vector pieces (act_ld8 / act_st8, uint4, uint2): hi and lo

@@ -281,6 +281,13 @@ __global__ void upsample_ce_reduce_kernel(const float* __restrict__ partial, int
   }
 }
 
+// The reduce above for the other translation units (csrc/crf.cu): loss_out[0] = sum / count, loss_out[1] = count.
+int launch_mean_reduce(const float* partial, int nblocks, float* loss_out, cudaStream_t stream) {
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(partial, nblocks, loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------- OHEM selection
 // The k-th smallest p_t over the valid pixels, exactly: a radix select over the fp32 bit patterns (non-negative floats
 // order like their uint32 patterns), four passes of 8 bits from the top. Each pass histograms the digit of the pixels

@@ -645,6 +645,58 @@ class _UpsampleCEEntropy(torch.autograd.Function):
         return dl, None, None, None, None, None
 
 
+def _crf_cfg(crit):
+    return crit.radius, crit.sigma_xy, crit.sigma_rgb, crit.mean, crit.std
+
+
+class _UpsampleCECRF(torch.autograd.Function):
+    """The fused tail with losses.GatedCRFLoss: ce_weight * CE (the plain forward and backward, unchanged) plus
+    crf_weight * the Gated CRF term on the grid of zoom `crf_zoom` (the tail's own at='output', 1 at 'logits'), with the
+    image sampled at stride `istride`. The CRF forward keeps S per grid pixel; its backward adds into the CE gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, target, image, ignore_index, zoom, crf_zoom, istride, crf_weight, ce_weight, cfg):
+        info, amax, lse = ops.upsample_ce_fwd(logits, target, ignore_index, zoom=zoom)
+        cinfo, s, crf_lse = ops.gated_crf_fwd(logits, lse if crf_zoom == zoom else None, image, crf_zoom, istride,
+                                              *cfg)
+        ctx.save_for_backward(logits, target, image, lse, info, crf_lse, s)
+        ctx.cfg = (ignore_index, zoom, crf_zoom, istride, crf_weight, ce_weight, cfg)
+        ctx.mark_non_differentiable(amax)
+        return torch.add(info[0] * ce_weight, cinfo[0], alpha=crf_weight), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, image, lse, info, crf_lse, s = ctx.saved_tensors
+        ignore_index, zoom, crf_zoom, istride, crf_weight, ce_weight, cfg = ctx.cfg
+        dl = ops.upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_loss * ce_weight, zoom=zoom)
+        ops.gated_crf_bwd(logits, crf_lse, image, s, crf_weight, grad_loss, dl, crf_zoom, istride, *cfg)
+        return dl, None, None, None, None, None, None, None, None, None
+
+
+class _GatedCRF(torch.autograd.Function):
+    """The Gated CRF term alone (unweighted) on the grid of fp32 NHWC logits, the image at the same grid (zoom 1)."""
+
+    @staticmethod
+    def forward(ctx, logits, image, cfg):
+        cinfo, s, lse = ops.gated_crf_fwd(logits, None, image, 1, 1, *cfg)
+        ctx.save_for_backward(logits, image, lse, s)
+        ctx.cfg = cfg
+        return cinfo[0].clone()
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        logits, image, lse, s = ctx.saved_tensors
+        dl = torch.zeros_like(logits, memory_format=torch.contiguous_format)
+        ops.gated_crf_bwd(logits, lse, image, s, 1.0, grad_loss, dl, 1, 1, *ctx.cfg)
+        return dl, None, None
+
+
+def gated_crf(logits, image, criterion):
+    """The unweighted Gated CRF term of losses.GatedCRFLoss `criterion` on the grid of fp32 NHWC logits [N,H,W,C], the
+    NCHW fp32 image [N,3,H,W] on the same grid (a constant: it gets no gradient)."""
+    return _GatedCRF.apply(logits, image.detach().contiguous(), _crf_cfg(criterion))
+
+
 class _UpsampleCELovasz(torch.autograd.Function):
     """The fused tail with losses.LovaszSoftmaxLoss, plus ce_weight * CE. The forward keeps the per pixel-class
     Lovász gradient weights (gamma, 4 C bytes per output pixel) it scattered from the sorted segments; the sort's
@@ -803,6 +855,8 @@ _DICE_PIXEL_BYTES, _DICE_STAGE_BYTES = 12, 224 * 1024
 # The RMI rows kernel stages 8 bytes per pixel in the same 224 KB (Wo <= 3584 at zoom 8); RMI needs a target of at least
 # 12 x 12, three pooled cells each way.
 _RMI_PIXEL_BYTES, _RMI_MIN_SIZE = 8, 12
+# The plain backward rows kernel stages 8 bytes per pixel of an interval's Z output rows in 160 KB (Wo <= 2560 at zoom 8).
+_CRF_CE_PIXEL_BYTES, _CRF_CE_STAGE_BYTES = 8, 160 * 1024
 
 
 def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
@@ -816,7 +870,8 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
     losses.EntropyLoss, whose rows kernel stages the same words, the Dice width limit. losses.RMILoss needs a target of
     at least 12 x 12 and no wider than its rows kernel stages (3584 columns
-    at zoom 8).
+    at zoom 8). losses.GatedCRFLoss needs the target no wider than the plain backward stages (2560 columns at zoom 8);
+    its classes (<= 256, checked here with the logits), radius and sigmas are in the kernels' limits by construction.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
         ok = True
@@ -830,6 +885,11 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         # the focal rows kernel (the pseudo-label backward too) and the entropy rows kernel stage the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
+    elif type(criterion) is losses.GatedCRFLoss:
+        # the cross-entropy part is the plain tail's, whose backward stages 8 bytes per pixel of Z rows in 160 KB; the
+        # CRF kernels take any width (csrc/crf.cu), and the criterion keeps radius, classes and sigmas in their limits
+        ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
+              _CRF_CE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _CRF_CE_STAGE_BYTES)
     elif type(criterion) is losses.RMILoss:
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               target.shape[1] >= _RMI_MIN_SIZE and target.shape[2] >= _RMI_MIN_SIZE and
@@ -856,7 +916,8 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     return target.shape[1] == zoom_factor * (h - 1) + 1 and target.shape[2] == zoom_factor * (w - 1) + 1
 
 
-def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_logits=None, mix_mask=None):
+def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_logits=None, mix_mask=None,
+                image=None, image_stride=None):
     """-> (mean CE loss scalar, argmax int64 [N,H,W]); H = zoom*(h-1)+1, W = zoom*(w-1)+1. With a
     losses.OhemCrossEntropyLoss `criterion`, the loss is its OHEM cross-entropy (its own ignore_index and class
     weights); with an nn.CrossEntropyLoss that has class weights or label smoothing, its weighted / smoothed mean;
@@ -869,7 +930,22 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     of the unmixed batch and the mix mask `mix_mask` (ops.mix_apply's), the mixed pseudo-label loss on the mixed target;
     without the mask it is a losses.PseudoLabelLoss. With a losses.EntropyLoss, its ce_weight * CE over the labelled
     pixels plus ent_weight * mean entropy over the unlabelled ones (its own ignore_index); the networks score their aux
-    head with the plain form. The default criterion runs the plain kernels."""
+    head with the plain form. With a losses.GatedCRFLoss and the network's fp32 NCHW input `image` (a constant),
+    ce_weight * CE plus crf_weight * its Gated CRF term; `image_stride` is the image's pixel stride on the loss grid
+    (default: 8 / zoom at at='output', 8 at at='logits'); without an image a positive crf_weight raises. The default
+    criterion runs the plain kernels."""
+    if isinstance(criterion, losses.GatedCRFLoss):
+        if criterion.crf_weight == 0.0:
+            # no CRF kernel: the plain step, bit for bit when ce_weight is 1
+            loss, amax = _UpsampleCE.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom))
+            return (loss if criterion.ce_weight == 1.0 else loss * criterion.ce_weight), amax
+        if image is None:
+            raise ValueError("GatedCRFLoss with crf_weight > 0 needs the image on the fused tail")
+        out = criterion.at == 'output'
+        istride = image_stride if image_stride is not None else (8 // int(zoom) if out else 8)
+        return _UpsampleCECRF.apply(logits, target.contiguous(), image.detach().contiguous(), criterion.ignore_index,
+                                    int(zoom), int(zoom) if out else 1, int(istride), criterion.crf_weight,
+                                    criterion.ce_weight, _crf_cfg(criterion))
     if type(criterion) is losses.MixPseudoLabelLoss and teacher_logits is not None and mix_mask is not None:
         return _UpsampleCEPLMix.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
                                       int(zoom), criterion.threshold, criterion.pl_weight, criterion.ce_weight,

@@ -5,9 +5,10 @@ the network's fused tail (functional.upsample_ce) it runs inside the same kernel
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
 LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and FocalLoss, the softmax focal loss with
-optional class weights, run the same way, and so do RMILoss, the Region Mutual Information loss with its BCE term, and
+optional class weights, run the same way, and so do RMILoss, the Region Mutual Information loss with its BCE term,
 EntropyLoss, entropy minimisation on the unlabelled pixels plus cross-entropy on the labelled ones (TENT's objective,
-adapt.Tent). DistillationLoss adds a
+adapt.Tent), and GatedCRFLoss, cross-entropy plus the Gated CRF pairwise term for scribble- and point-supervised
+training. DistillationLoss adds a
 pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
 optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
@@ -257,6 +258,123 @@ class EntropyLoss(nn.Module):
         _check_native_logits("EntropyLoss", logits, target)
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1)
         return loss
+
+
+_IMAGENET_MEAN = (0.485 * 255, 0.456 * 255, 0.406 * 255)
+_IMAGENET_STD = (0.229 * 255, 0.224 * 255, 0.225 * 255)
+
+
+def _triple(name, v, positive):
+    try:
+        t = tuple(v)
+    except TypeError:
+        raise TypeError("%s must be three numbers, got %r" % (name, v)) from None
+    if len(t) != 3 or any(isinstance(a, bool) or not isinstance(a, (int, float)) for a in t):
+        raise TypeError("%s must be three numbers, got %r" % (name, v))
+    t = tuple(float(a) for a in t)
+    if not all(math.isfinite(a) and (a > 0.0 or not positive) for a in t):
+        raise ValueError("%s must be finite%s, got %r" % (name, " and > 0" if positive else "", v))
+    return t
+
+
+class GatedCRFLoss(nn.Module):
+    """Cross-entropy on the labelled pixels plus the Gated CRF loss (Obukhov et al., "Gated CRF Loss for Weakly
+    Supervised Semantic Image Segmentation", 2019), the pairwise term of scribble-, click- and point-supervised
+    training: the target is mostly ignore_index, and the term pulls neighbouring pixels of similar colour towards the
+    same class. It is a local-window relaxation of the DenseCRF loss of Tang et al. (ECCV 2018) with the Potts model.
+
+    The loss grid:
+        at='output': the target grid Ho = Z (h' - 1) + 1, on the logits upsampled xZ (align_corners), as the CE term;
+        at='logits': the raw 1/8-resolution grid h' x w'.
+    rgb_i is the network input x (normalised NCHW fp32) point-sampled at the grid points and un-normalised as
+    (x std + mean) / 255; the grid aligns with the input under align_corners, so the sampling stride is 8 / Z
+    (at='output') or 8 (at='logits'), which equals F.interpolate(..., align_corners=True). With p_i = softmax(s_i) over
+    the classes, positions (row, col) in grid units and W(i) the (2 radius + 1)^2 window around i without i itself and
+    without pixels outside the image:
+
+        k_ij = exp(-|pos_i - pos_j|^2 / (2 sigma_xy^2) - |rgb_i - rgb_j|^2 / (2 sigma_rgb^2))     (symmetric)
+        CRF  = (1/P) sum_n sum_i sum_{j in W(i)} k_ij (1 - sum_c p_ic p_jc),   P = grid pixels of the call (per rank)
+        main = ce_weight CE + crf_weight CRF,  CE the mean over the labelled pixels (0 <= target < C, not ignore_index)
+        aux  = the aux head's plain CE on the labelled pixels;  pred = argmax
+        dCRF/ds_ic = -(2/P) p_ic (G_ic - S_i),  G_ic = sum_{j in W(i)} k_ij p_jc,  S_i = sum_c p_ic G_ic
+
+    The image gate is a constant: with x.requires_grad, x.grad is the network path's gradient only. The published code
+    differs in one place: it zero-pads the features, so out-of-image neighbours get a non-zero k; their p is zero, so
+    that only adds a constant to the loss value, and the gradient is the same. Crop padding takes part as the mean
+    colour (the published code's source / destination masks are not implemented). crf_weight = 0 runs no CRF kernel:
+    the step is the nn.CrossEntropyLoss(ignore_index) step.
+
+    With the network's fused tail (functional.upsample_ce, which the network hands its input batch) it runs on the
+    tail's kernels and csrc/crf.cu, graphed at every zoom factor. Called as a module, forward(logits, target, image)
+    takes NCHW logits at the target size and the NCHW image at that size and returns `main` on that grid (the zoom-1
+    kernels on NHWC copies); without `image` it returns the plain mean CE, which validate() logs. CUDA fp32 only, at
+    most 256 classes, radius 1 to 8: there is no CPU or library fallback."""
+
+    def __init__(self, ignore_index=255, crf_weight=0.1, ce_weight=1.0, radius=5, sigma_xy=6.0, sigma_rgb=0.1,
+                 mean=_IMAGENET_MEAN, std=_IMAGENET_STD, at='output'):
+        super(GatedCRFLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        self.ignore_index = ignore_index
+        self.crf_weight = _non_negative("crf_weight", crf_weight)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+        if isinstance(radius, bool) or not isinstance(radius, int):
+            raise TypeError("radius must be an int, got %r" % (radius,))
+        if not 1 <= radius <= 8:
+            raise ValueError("radius must be in [1, 8], got %d" % radius)
+        self.radius = radius
+        for name, v in (("sigma_xy", sigma_xy), ("sigma_rgb", sigma_rgb)):
+            if isinstance(v, bool) or not isinstance(v, (int, float)):
+                raise TypeError("%s must be a number, got %r" % (name, v))
+            if not (math.isfinite(v) and v > 0):
+                raise ValueError("%s must be finite and > 0, got %r" % (name, v))
+        self.sigma_xy, self.sigma_rgb = float(sigma_xy), float(sigma_rgb)
+        self.mean = _triple("mean", mean, False)
+        self.std = _triple("std", std, True)
+        if at not in ('output', 'logits'):
+            raise ValueError("at must be 'output' or 'logits', got %r" % (at,))
+        self.at = at
+
+    def extra_repr(self):
+        return ("ignore_index=%d, crf_weight=%g, ce_weight=%g, radius=%d, sigma_xy=%g, sigma_rgb=%g, at=%r" %
+                (self.ignore_index, self.crf_weight, self.ce_weight, self.radius, self.sigma_xy, self.sigma_rgb,
+                 self.at))
+
+    def _check_image(self, image, n, hg, wg):
+        if not (torch.is_tensor(image) and image.dim() == 4 and tuple(image.shape) == (n, 3, hg, wg)):
+            raise ValueError("GatedCRFLoss: image [%d, 3, %d, %d] expected, got %s" %
+                             (n, hg, wg, tuple(image.shape) if torch.is_tensor(image) else type(image).__name__))
+        if not image.is_cuda or image.dtype != torch.float32:
+            raise TypeError("GatedCRFLoss: a CUDA fp32 image expected, got %s on %s" % (image.dtype, image.device))
+
+    def forward(self, logits, target, image=None):
+        from . import functional as SF
+        _check_native_logits("GatedCRFLoss", logits, target)
+        nhwc = logits.permute(0, 2, 3, 1).contiguous()
+        if image is None:
+            loss, _ = SF.upsample_ce(nhwc, target, self.ignore_index, 1)
+            return loss
+        self._check_image(image, logits.shape[0], logits.shape[2], logits.shape[3])
+        loss, _ = SF.upsample_ce(nhwc, target, self.ignore_index, 1, criterion=self, image=image, image_stride=1)
+        return loss
+
+    def aux_loss(self, logits, target):
+        """The aux head's loss, module form: the plain mean cross-entropy of NCHW logits at the target size."""
+        from . import functional as SF
+        _check_native_logits("GatedCRFLoss", logits, target)
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1)
+        return loss
+
+    def crf_term(self, logits, image):
+        """CRF alone (not weighted) on the grid of NCHW fp32 logits [N, C, H, W], with the image [N, 3, H, W] on the
+        same grid: the zoom-1 kernels on NHWC copies. The networks' ATen tail uses it."""
+        from . import functional as SF
+        if not (logits.dim() == 4 and logits.is_cuda and logits.dtype == torch.float32):
+            raise TypeError("GatedCRFLoss: CUDA fp32 NCHW logits expected")
+        if logits.shape[1] > 256:
+            raise ValueError("GatedCRFLoss: at most 256 classes (got %d); no fallback" % logits.shape[1])
+        self._check_image(image, logits.shape[0], logits.shape[2], logits.shape[3])
+        return SF.gated_crf(logits.permute(0, 2, 3, 1).contiguous(), image, self)
 
 
 class _TeacherLoss(nn.Module):

@@ -981,6 +981,62 @@ def upsample_ce_entropy_bwd(logits, target, ignore_index, ent_weight, ce_weight,
     return dl
 
 
+def _crf_image_args(image, hg, wg, istride):
+    """The NCHW fp32 image operand of the Gated CRF kernels: [N, 3, istride (hg-1)+1, istride (wg-1)+1], contiguous."""
+    assert image.dtype == torch.float32 and image.dim() == 4 and image.shape[1] == 3 and image.is_contiguous()
+    return _ptr(image), image.shape[2], image.shape[3], int(istride)
+
+
+def gated_crf_fwd(logits, lse, image, zoom, istride, radius, sigma_xy, sigma_rgb, mean, std):
+    """The Gated CRF pairwise term (include/semseg_b200.h states the contract) on the grid zoom*(h-1)+1 x zoom*(w-1)+1 of
+    the fp32 NHWC logits [N,h,w,C]: -> (info [2] = (CRF, P), S [N,Hg,Wg], lse). `lse` is the grid's per-pixel
+    logsumexp (the zoom forward's), or None at zoom 1: computed here. `image` fp32 NCHW at stride `istride` of the
+    grid; `mean` / `std` three numbers each (the image's normalisation)."""
+    _require_cuda(logits, image)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    n, h, w, c = logits.shape
+    zoom = int(zoom)
+    hg, wg = zoom * (h - 1) + 1, zoom * (w - 1) + 1
+    dev = logits.device
+    nws = int(lib.semseg_gated_crf_workspace_floats(n, h, w, zoom))
+    _lib.check(0 if nws >= 0 else nws, "semseg_gated_crf_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    compute_lse = lse is None
+    if compute_lse:
+        lse = torch.empty((n, hg, wg), dtype=torch.float32, device=dev)
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (n, hg, wg)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    s = torch.empty((n, hg, wg), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_gated_crf_fwd(_ptr(logits), logits.stride(2), n, h, w, c, zoom, _ptr(lse), int(compute_lse),
+                                        *_crf_image_args(image, hg, wg, istride), int(radius), float(sigma_xy),
+                                        float(sigma_rgb), *(float(v) for v in mean), *(float(v) for v in std),
+                                        _ptr(ws), _ptr(s), _ptr(info), _stream()),
+               "semseg_gated_crf_fwd")
+    return info, s, lse
+
+
+def gated_crf_bwd(logits, lse, image, s, crf_weight, grad_out, dlogits, zoom, istride, radius, sigma_xy, sigma_rgb,
+                  mean, std):
+    """Adds grad_out[0] * crf_weight * dCRF/dlogits into dlogits (fp32 [N,h,w,C], contiguous) in place, from the
+    forward's lse and S."""
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    zoom = int(zoom)
+    hg, wg = zoom * (h - 1) + 1, zoom * (w - 1) + 1
+    assert dlogits.dtype == torch.float32 and dlogits.is_contiguous() and tuple(dlogits.shape) == (n, h, w, c)
+    nws = int(lib.semseg_gated_crf_bwd_workspace_floats(n, h, w, c, zoom))
+    _lib.check(0 if nws >= 0 else nws, "semseg_gated_crf_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_gated_crf_bwd(_ptr(logits), logits.stride(2), n, h, w, c, zoom, _ptr(lse),
+                                        *_crf_image_args(image, hg, wg, istride), int(radius), float(sigma_xy),
+                                        float(sigma_rgb), *(float(v) for v in mean), *(float(v) for v in std), _ptr(s),
+                                        float(crf_weight), _ptr(g), _ptr(ws), _ptr(dlogits), _stream()),
+               "semseg_gated_crf_bwd")
+    return dlogits
+
+
 def upsample_ce_lovasz_fwd(logits, target, ignore_index, classes_all, per_image, ce_weight, want_argmax=True, zoom=8,
                            return_workspace=False):
     """Lovász-Softmax loss (+ ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract) ->

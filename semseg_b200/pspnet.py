@@ -187,8 +187,10 @@ class _SegNet(nn.Module):
         fp_logits = logits[streams] if fp_scale is not None else None
 
         if self.training:
-            # losses.EntropyLoss scores the aux head with the plain cross-entropy over the labelled pixels
-            entropy = isinstance(self.criterion, losses.EntropyLoss)
+            # losses.EntropyLoss and losses.GatedCRFLoss score the aux head with the plain cross-entropy over the
+            # labelled pixels; the Gated CRF term reads the input batch
+            plain_aux = isinstance(self.criterion, (losses.EntropyLoss, losses.GatedCRFLoss))
+            crf = isinstance(self.criterion, losses.GatedCRFLoss)
             aux_logits = _chunks(head_forward_nhwc(self.aux, t_aux), streams)
             ys = _chunks(y, streams) if mix_mask is not None else (y,) * streams      # the mixed target is [2N]
             masks = _chunks(mix_mask, streams) if mix_mask is not None else (None,) * streams
@@ -197,12 +199,13 @@ class _SegNet(nn.Module):
                 # one call per stream: each has its own target, mask and normalisers, and the one teacher map
                 mains, preds = zip(*(SF.upsample_ce(logits[k], ys[k], self.criterion.ignore_index, self.zoom_factor,
                                                     criterion=self.criterion, teacher_logits=t_logits,
-                                                    mix_mask=masks[k]) for k in range(streams)))
+                                                    mix_mask=masks[k], image=x if crf else None)
+                                     for k in range(streams)))
                 main_loss = _stream_mean(mains)
                 if fp_logits is not None:
                     main_loss = main_loss + SF.upsample_fp(fp_logits, ys[0], self.zoom_factor, self.criterion,
                                                            t_logits, masks[0])[0]
-                aux_crit = None if entropy else self.criterion
+                aux_crit = None if plain_aux else self.criterion
                 aux_loss = _stream_mean([SF.upsample_ce(a, y_k, self.criterion.ignore_index, self.zoom_factor,
                                                         criterion=aux_crit)[0] for a, y_k in zip(aux_logits, ys)])
                 if relation:
@@ -222,9 +225,20 @@ class _SegNet(nn.Module):
                 if fp_logits is not None:
                     main_loss = main_loss + self.criterion.fp_loss(upsample_logits(fp_logits, (h, w), self.zoom_factor),
                                                                    ys[0], t_ups[0])
+            elif crf:
+                # the same loss on the ATen tail: plain CE on the upsampled logits, the CRF term through the module's
+                # kernels on its grid (the upsampled or the raw logits) and the input sampled at that grid's stride
+                c = self.criterion
+                main_loss = c(ups[0], y)
+                if c.ce_weight != 1.0:
+                    main_loss = main_loss * c.ce_weight
+                if c.crf_weight > 0.0:
+                    grid, s = ((ups[0], 8 // self.zoom_factor) if c.at == 'output' else
+                               (logits[0].permute(0, 3, 1, 2), 8))
+                    main_loss = main_loss + c.crf_weight * c.crf_term(grid, x[:, :, ::s, ::s])
             else:
                 main_loss = self.criterion(ups[0], y)
-            aux_fn = self.criterion.aux_loss if entropy else self.criterion
+            aux_fn = self.criterion.aux_loss if plain_aux else self.criterion
             aux_loss = _stream_mean([aux_fn(a, y_k) for a, y_k in zip(aux_ups, ys)])
             if relation:
                 main_loss = main_loss + self.criterion.relation_weight * self.criterion.relation(f_s, t_feat)
