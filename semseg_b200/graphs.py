@@ -17,11 +17,9 @@ step counter incremented inside the graph — csrc/bn.cu st_ll / ld_ll) and drop
 
 Limits (same as torch.cuda.make_graphed_callables): a second training forward before the backward of the first one
 overwrites the first one's saved activations — gradient accumulation over several forwards needs SEMSEG_B200_GRAPH=0.
-The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported:
-cross-entropy with or without class weights and label smoothing, OHEM cross-entropy, the Dice loss, the Lovász-Softmax
-loss, the focal loss, the RMI loss, the entropy loss, the Gated CRF loss, the distillation and the pseudo-label losses, whose teacher forward is captured with the step, a
-mean teacher's re-pack included, the pseudo-label losses' feature-perturbation stream and second strong stream, and the CutMix / ClassMix
-pseudo-label loss, its draws and mixing included, with or without a strong view of the student's input) are not captured (such models simply stay eager).
+The NCCL fallback of the SyncBN exchange and criteria the fused tail does not implement (functional.fused_tail_supported)
+are not captured (such models simply stay eager). With a teacher criterion the teacher forward (a mean teacher's
+re-pack included), the draws, the strong view, the mixing and the extra student streams are captured with the step.
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
 import os
@@ -30,7 +28,7 @@ import warnings
 import torch
 import torch.distributed as dist
 
-from . import precision
+from . import losses, precision
 
 WARMUP_CALLS = 3          # eager calls with an unchanged key before capturing
 MAX_GRAPHS = 4            # captured input shapes per model (each keeps a private activation pool); others stay eager
@@ -62,13 +60,11 @@ def note_boundary(t):
 
 class _Step:
     __slots__ = ("key", "calls", "failed", "fwd", "bwd", "bwd2", "x", "y", "pred", "main", "aux", "g_main", "g_aux",
-                 "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot", "mix",
-                 "mix_crit", "strong", "strong_crit", "fp", "fp_crit", "rel", "rel_crit")
+                 "grads", "grads2", "t_mid", "d_mid", "n_tail", "params", "pool", "keep", "launches", "dx_slot", "crit",
+                 "last")
 
     def __init__(self, key):
         self.key, self.calls, self.failed, self.fwd, self.dx_slot = key, 0, False, None, False
-        self.mix = self.mix_crit = self.strong = self.strong_crit = self.fp = self.fp_crit = None
-        self.rel = self.rel_crit = None
 
 
 def _set_grad_outputs(st, g_main, g_aux):
@@ -109,10 +105,7 @@ class _Replay(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, st, x, y, *params):
-        st.x.copy_(x, non_blocking=True)
-        st.y.copy_(y, non_blocking=True)
-        st.fwd.replay()
-        _point_mix(st)
+        _replay_forward(st, x, y)
         ctx.st = st
         pred, main, aux = st.pred.detach(), st.main.detach(), st.aux.detach()
         ctx.mark_non_differentiable(pred)
@@ -126,18 +119,15 @@ class _Replay(torch.autograd.Function):
         return _with_dx(st, _fresh(st.grads))
 
 
-def _point_mix(st):
-    """A losses.MixPseudoLabelLoss criterion's last_mix() is the replayed step's: its mask, mixed target and uniforms
-    are that step's static tensors (each captured input shape has its own). So are a teacher criterion's last_strong()
-    and a pseudo-label criterion's last_fp(), and a distillation criterion's last_relation()."""
-    if st.mix_crit is not None:
-        st.mix_crit._mix_state = st.mix
-    if st.strong_crit is not None:
-        st.strong_crit._strong_state = st.strong
-    if st.fp_crit is not None:
-        st.fp_crit._fp_state = st.fp
-    if st.rel_crit is not None:
-        st.rel_crit._relation_state = st.rel
+def _replay_forward(st, x, y):
+    """The forward graph replayed on `x`, `y`. A teacher criterion's last_mix(), last_strong(), last_fp() and
+    last_relation() are then the replayed step's: the records its captured forward wrote, static tensors of that step
+    (each captured input shape has its own), are put back."""
+    st.x.copy_(x, non_blocking=True)
+    st.y.copy_(y, non_blocking=True)
+    st.fwd.replay()
+    if st.last:
+        st.crit._last.update(st.last)
 
 
 def _with_dx(st, gs):
@@ -154,10 +144,7 @@ class _ReplayHead(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, st, x, y, *params_head):
-        st.x.copy_(x, non_blocking=True)
-        st.y.copy_(y, non_blocking=True)
-        st.fwd.replay()
-        _point_mix(st)
+        _replay_forward(st, x, y)
         ctx.st = st
         return st.t_mid.detach()
 
@@ -220,6 +207,11 @@ def _capture(model, impl, st, x, y):
     torch.cuda.synchronize()
     st.pool = torch.cuda.graph_pool_handle()
     st.fwd, st.bwd, st.bwd2 = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph(), None
+    crit = getattr(model, "criterion", None)
+    last = getattr(crit, "_last", {})
+    # the records' identities only: holding the eager step's records would keep their tensors alive through the capture
+    # (a forward writes each record as a new dict while the old one still exists, so the ids cannot repeat)
+    before = {k: id(v) for k, v in last.items()}
     l0 = _lib.launch_count()
     global _boundary
     _capturing, _boundary = True, None
@@ -268,38 +260,20 @@ def _capture(model, impl, st, x, y):
         for mod, name, prm in slots:
             mod._parameters[name] = prm
     st.launches = _lib.launch_count() - l0          # native kernels per replayed step (forward + backward graphs)
-    crit = getattr(model, "criterion", None)
-    if getattr(crit, "_mix_state", None) is not None:
-        # the mix the captured forward wrote: static tensors of the graph's pool, refreshed by every replay
-        st.mix, st.mix_crit = crit._mix_state, crit
-    if getattr(crit, "strong", None) is not None:
-        # likewise the strong view and its uniforms
-        st.strong, st.strong_crit = crit._strong_state, crit
-    if getattr(crit, "fp_weight", 0.0) > 0.0:
-        # and the feature perturbation's uniforms and scale
-        st.fp, st.fp_crit = crit._fp_state, crit
-    if getattr(crit, "relation_weight", 0.0) > 0.0:
-        # and the relation term's features and loss
-        st.rel, st.rel_crit = crit._relation_state, crit
+    # the last-step records the captured forward wrote: static tensors of the graph's pool, refreshed by every replay
+    st.crit, st.last = crit, {k: v for k, v in last.items() if before.get(k) != id(v)}
     # drop the autograd graph built during capture; the static outputs live on in the graphs' private memory pool
     st.pred, st.main, st.aux = st.pred.detach(), st.main.detach(), st.aux.detach()
     del proxies, x_in, x_leaf
     # the graphs reference the persistent weight slabs: keep their owner alive as long as the graphs (a distillation
     # teacher's slabs are its convs' own packs, filled by the eager warm-up calls; the teacher is kept with them)
     st.keep = model.__dict__.get("_sb_pack_plan")
-    teacher = _teacher(getattr(model, "criterion", None))
+    teacher = getattr(crit, "teacher", None)      # a distillation or pseudo-label criterion's
     if teacher is not None:
         # a mean teacher's slabs are its whole-model plan's, re-packed inside the captured step
         st.keep = (st.keep, teacher, teacher.__dict__.get("_sb_pack_plan"),
                    [m.__dict__.get("_sb_conv_plan") for m in teacher.modules()])
     torch.cuda.synchronize()
-
-
-def _teacher(crit):
-    """The teacher network a losses.DistillationLoss or losses.PseudoLabelLoss criterion runs inside the step, else
-    None."""
-    from . import losses
-    return crit.teacher if isinstance(crit, losses._TeacherLoss) else None
 
 
 def train_step(model, impl, x, y):
@@ -319,42 +293,8 @@ def train_step(model, impl, x, y):
     # likewise the heads' Dropout2d modes: a dropout switched to eval mode (adapt.Tent) runs no mask kernel
     drop_modes = tuple(m.training for m in model.modules() if isinstance(m, torch.nn.Dropout2d))
     # an input that needs a gradient runs other kernels (the phase-form stem conv, its dgrad): a capture of its own
-    # the criterion's options are launch arguments baked into the graph: a changed thresh, ignore_index,
-    # label_smoothing, Dice smooth / eps / ce_weight, Lovász classes / per_image, focal gamma, RMI bce_weight /
-    # pos_alpha, entropy ent_weight or Gated CRF crf_weight / radius / sigmas / at / mean / std captures anew, and so
-    # does a replaced class-weight tensor (its address is baked in); an in-place edit of the weights needs no capture,
-    # the kernels read them at every replay
-    crit = getattr(model, "criterion", None)
-    crit_key = (type(crit),) + tuple(getattr(crit, a, None) for a in ("ignore_index", "thresh", "min_kept",
-                                                                      "label_smoothing", "reduction", "smooth", "eps",
-                                                                      "ce_weight", "classes", "per_image", "gamma",
-                                                                      "bce_weight", "pos_alpha", "ent_weight",
-                                                                      "crf_weight", "radius", "sigma_xy", "sigma_rgb",
-                                                                      "at", "mean", "std"))
-    cw = getattr(crit, "weight", None)
-    crit_key += (cw.data_ptr(), cw.numel()) if torch.is_tensor(cw) else (None,)
-    teacher = _teacher(crit)
-    if teacher is not None:
-        # a teacher runs inside the forward graph: its identity, the addresses and versions of its parameters and
-        # buffers (an in-place edit of a frozen teacher's weight bumps the version, so the step is captured again with
-        # the edit rather than replayed stale), its BatchNorm modes and the options of the KL / pseudo-label term are
-        # baked in too. A ModelEMA shadow changes every step: its key holds the addresses only, because the captured
-        # step re-packs its slabs and folds its BatchNorm statistics at every replay (losses._TeacherLoss.run_teacher)
-        if getattr(teacher, "_sb_ema_shadow", False):
-            tkey = lambda ts: tuple(t.data_ptr() for t in ts)                          # noqa: E731
-        else:
-            tkey = lambda ts: tuple((t.data_ptr(), t._version) for t in ts)            # noqa: E731
-        crit_key += (id(teacher), tkey(teacher.parameters()), tkey(teacher.buffers()),
-                     tuple(m.training for m in teacher.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)))
-        crit_key += tuple(getattr(crit, a, None) for a in ("temperature", "kd_weight", "at", "threshold", "pl_weight",
-                                                             "fp_weight", "fp_dropout", "mix", "p", "area", "ratio"))
-        if getattr(crit, "relation_weight", 0.0) > 0.0:
-            # the relation term's kernels and arguments; at weight 0 the key is the one without the option
-            crit_key += ("relation", crit.relation_weight, crit.relation_temperature, crit.relation_pool)
-        if getattr(crit, "streams", 1) != 1:
-            crit_key += ("streams", crit.streams)          # a 2N-image student: other shapes and launches
-        if crit.strong is not None:
-            crit_key += ("strong",) + crit.strong.key()    # the strong view's options are launch arguments too
+    # the criterion's options are launch arguments baked into the graphs: each criterion declares its own
+    crit_key = losses.graph_key(getattr(model, "criterion", None))
     key = (tuple(x.shape), x.dtype, tuple(y.shape), y.dtype, x.device.index, precision.get_mode(), len(ptrs), hash(ptrs),
            dist.get_world_size() if (dist.is_available() and dist.is_initialized()) else 1, bn_modes, drop_modes,
            x.requires_grad, crit_key)

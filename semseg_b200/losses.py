@@ -47,6 +47,9 @@ class OhemCrossEntropyLoss(nn.Module):
 
     CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
 
+    # the options a captured training step bakes in as launch arguments (graph_key)
+    graph_options = ("ignore_index", "thresh", "min_kept")
+
     def __init__(self, ignore_index=255, thresh=0.7, min_kept=100000, weight=None):
         super(OhemCrossEntropyLoss, self).__init__()
         if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
@@ -120,6 +123,8 @@ class DiceLoss(nn.Module):
     factor; called as a module (validate()) it runs their zoom-1 form on an NHWC copy of the logits. CUDA fp32 logits
     with at most 256 classes only: there is no CPU or library fallback."""
 
+    graph_options = ("ignore_index", "smooth", "eps", "ce_weight")
+
     def __init__(self, ignore_index=255, smooth=0.0, eps=1e-7, ce_weight=0.0):
         super(DiceLoss, self).__init__()
         if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
@@ -184,6 +189,8 @@ class FocalLoss(nn.Module):
     factor; called as a module (validate()) it runs their zoom-1 form on an NHWC copy of the logits. CUDA fp32 logits
     with at most 256 classes only: there is no CPU or library fallback."""
 
+    graph_options = ("ignore_index", "gamma")
+
     def __init__(self, gamma=2.0, weight=None, ignore_index=255):
         super(FocalLoss, self).__init__()
         if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
@@ -234,6 +241,8 @@ class EntropyLoss(nn.Module):
     factor; called as a module, forward(logits, target) takes NCHW logits at the target size and returns `main`, on the
     zoom-1 form of the kernels on an NHWC copy (validate() logs it). CUDA fp32 logits with at most 256 classes only:
     there is no CPU or library fallback."""
+
+    graph_options = ("ignore_index", "ent_weight", "ce_weight")
 
     def __init__(self, ignore_index=255, ent_weight=1.0, ce_weight=1.0):
         super(EntropyLoss, self).__init__()
@@ -309,6 +318,8 @@ class GatedCRFLoss(nn.Module):
     takes NCHW logits at the target size and the NCHW image at that size and returns `main` on that grid (the zoom-1
     kernels on NHWC copies); without `image` it returns the plain mean CE, which validate() logs. CUDA fp32 only, at
     most 256 classes, radius 1 to 8: there is no CPU or library fallback."""
+
+    graph_options = ("ignore_index", "crf_weight", "ce_weight", "radius", "sigma_xy", "sigma_rgb", "at", "mean", "std")
 
     def __init__(self, ignore_index=255, crf_weight=0.1, ce_weight=1.0, radius=5, sigma_xy=6.0, sigma_rgb=0.1,
                  mean=_IMAGENET_MEAN, std=_IMAGENET_STD, at='output'):
@@ -398,6 +409,8 @@ class _TeacherLoss(nn.Module):
     graphed or eager, as views that stay valid until the next forward. There is no gradient through the view: an input
     with requires_grad raises. strong=None changes nothing."""
 
+    graph_options = ("ignore_index",)
+
     def __init__(self, teacher, ignore_index, strong=None):
         super(_TeacherLoss, self).__init__()
         from .augment import StrongAugment
@@ -411,7 +424,7 @@ class _TeacherLoss(nn.Module):
             raise TypeError("strong must be an augment.StrongAugment or None, got %s" % type(strong).__name__)
         self.ignore_index = ignore_index
         self.strong = strong
-        self._strong_state = None
+        self._last = {}      # last_strong(), last_fp(), last_mix(), last_relation(); put back by a graphed replay
         self.__dict__['_teacher'] = teacher      # held outside the module tree (see the class docstring)
 
     @property
@@ -428,16 +441,35 @@ class _TeacherLoss(nn.Module):
     def _strong_repr(self):
         return "" if self.strong is None else ", strong=%r" % (self.strong,)
 
+    def _last_record(self, name):
+        r = self._last.get(name)
+        return None if r is None else dict(r)
+
     def last_strong(self):
         """{'image', 'uniforms'} of the latest training forward's strong view (None before the first one, or without
         `strong`)."""
-        return None if self._strong_state is None else dict(self._strong_state)
+        return self._last_record('strong')
 
     def strong_view(self, x, u):
         """The student's view of `x` from `strong.draw`'s uniforms `u`; remembered for last_strong()."""
         xs = self.strong(x, u)
-        self._strong_state = {'image': xs, 'uniforms': u}
+        self._last['strong'] = {'image': xs, 'uniforms': u}
         return xs
+
+    def _teacher_key(self):
+        """The teacher's part of graph_key. The teacher runs inside the captured forward: its identity, the addresses
+        and versions of its parameters and buffers (an in-place edit of a frozen teacher's weight bumps the version, so
+        the step is captured again with the edit rather than replayed stale), its BatchNorm modes and the strong view's
+        options are baked in. A ModelEMA shadow changes every step: its key holds the addresses only, because the
+        captured step re-packs its slabs and folds its BatchNorm statistics at every replay (run_teacher)."""
+        teacher = self.teacher
+        if getattr(teacher, "_sb_ema_shadow", False):
+            tkey = lambda ts: tuple(t.data_ptr() for t in ts)                          # noqa: E731
+        else:
+            tkey = lambda ts: tuple((t.data_ptr(), t._version) for t in ts)            # noqa: E731
+        key = (id(teacher), tkey(teacher.parameters()), tkey(teacher.buffers()),
+               tuple(m.training for m in teacher.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)))
+        return key if self.strong is None else key + ("strong",) + self.strong.key()
 
     def run_teacher(self, x, classes, feature=False):
         """The teacher's detached fp32 NHWC 1/8-resolution logits of the input batch `x` (NCHW), for a student with
@@ -521,6 +553,12 @@ class DistillationLoss(_TeacherLoss):
     relation_weight = 0 (the default) runs none of it: the step is the one without the option. The module form
     forward(logits, target, teacher_logits) has no features, so it never has the relation term."""
 
+    @property
+    def graph_options(self):
+        # the relation term's options are launch arguments only when it runs: at weight 0 the key is the one without
+        kd = _TeacherLoss.graph_options + ("temperature", "kd_weight", "ce_weight", "at")
+        return kd + ("relation_weight", "relation_temperature", "relation_pool") if self.relation_weight > 0.0 else kd
+
     def __init__(self, teacher, temperature=1.0, kd_weight=1.0, ce_weight=1.0, ignore_index=255, at='output',
                  strong=None, relation_weight=0.0, relation_temperature=1.0, relation_pool=2):
         super(DistillationLoss, self).__init__(teacher, ignore_index, strong)
@@ -545,7 +583,6 @@ class DistillationLoss(_TeacherLoss):
         if not 1 <= relation_pool <= 16:
             raise ValueError("relation_pool must lie in [1, 16], got %r" % relation_pool)
         self.relation_pool = relation_pool
-        self._relation_state = None
 
     def extra_repr(self):
         s = "teacher=%s, temperature=%g, kd_weight=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
@@ -558,7 +595,7 @@ class DistillationLoss(_TeacherLoss):
     def last_relation(self):
         """{'student', 'teacher', 'loss'} of the latest training forward's relation term (None before the first one,
         or with relation_weight 0)."""
-        return None if self._relation_state is None else dict(self._relation_state)
+        return self._last_record('relation')
 
     def relation(self, f_s, f_t):
         """R of the student's and the teacher's cls[2] features (unweighted; differentiable in f_s); remembered for
@@ -568,7 +605,7 @@ class DistillationLoss(_TeacherLoss):
             raise ValueError("DistillationLoss: the student's relation features %s and the teacher's %s differ in "
                              "shape (channels or grid)" % (tuple(f_s.shape[-4:]), tuple(f_t.shape[-4:])))
         r = SF.relation_kd(f_s, f_t, self.relation_temperature, self.relation_pool)
-        self._relation_state = {'student': f_s.detach(), 'teacher': f_t.detach(), 'loss': r.detach()}
+        self._last['relation'] = {'student': f_s.detach(), 'teacher': f_t.detach(), 'loss': r.detach()}
         return r
 
     def forward(self, logits, target, teacher_logits=None):
@@ -659,6 +696,8 @@ class PseudoLabelLoss(_TeacherLoss):
 
     # two streams are two different views only through the strong view's draws (a mix criterion's boxes differ too)
     _streams_need_strong = True
+    graph_options = _TeacherLoss.graph_options + ("threshold", "pl_weight", "ce_weight", "fp_weight", "fp_dropout",
+                                                  "streams")
 
     def __init__(self, teacher, threshold=0.95, pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None,
                  fp_weight=0.0, fp_dropout=0.5, streams=1):
@@ -682,7 +721,6 @@ class PseudoLabelLoss(_TeacherLoss):
             raise ValueError("%s: streams=2 needs a strong view (strong=None would give two identical streams)" %
                              type(self).__name__)
         self.streams = streams
-        self._fp_state = None
 
     def _fp_repr(self):
         return ", fp_weight=%g, fp_dropout=%g" % (self.fp_weight, self.fp_dropout) + \
@@ -695,7 +733,7 @@ class PseudoLabelLoss(_TeacherLoss):
             return self.strong_view(x, u)
         n = x.shape[0]
         xs = torch.cat([self.strong(x, u[k * n:(k + 1) * n]) for k in range(self.streams)])
-        self._strong_state = {'image': xs, 'uniforms': u}
+        self._last['strong'] = {'image': xs, 'uniforms': u}
         return xs
 
     def extra_repr(self):
@@ -706,7 +744,7 @@ class PseudoLabelLoss(_TeacherLoss):
     def last_fp(self):
         """{'uniforms', 'scale'} of the latest training forward's feature perturbation (None before the first one, or
         with fp_weight 0)."""
-        return None if self._fp_state is None else dict(self._fp_state)
+        return self._last_record('fp')
 
     def fp_draw(self, x, channels):
         """The per-(image, channel) factor s [N, channels] of the feature-perturbation stream from fresh uniforms of
@@ -714,7 +752,7 @@ class PseudoLabelLoss(_TeacherLoss):
         u = torch.rand((x.shape[0], channels), device=x.device)
         keep = 1.0 - self.fp_dropout
         s = (u < keep).float().div_(keep)
-        self._fp_state = {'uniforms': u, 'scale': s}
+        self._last['fp'] = {'uniforms': u, 'scale': s}
         return s
 
     def fp_loss(self, logits, target, teacher_logits):
@@ -789,6 +827,7 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
     from its own uniform rows, so the two streams differ by their boxes or class sets."""
 
     _streams_need_strong = False
+    graph_options = PseudoLabelLoss.graph_options + ("mix", "p", "area", "ratio")
 
     def __init__(self, teacher, mix='cutmix', p=0.5, area=(0.02, 0.4), ratio=(0.3, 1 / 0.3), threshold=0.95,
                  pl_weight=1.0, ce_weight=1.0, ignore_index=255, strong=None, fp_weight=0.0, fp_dropout=0.5,
@@ -806,7 +845,6 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
         self.p = p
         self.area = _range_pair("area", area, 1.0)
         self.ratio = _range_pair("ratio", ratio, math.inf)
-        self._mix_state = None
 
     def extra_repr(self):
         return "teacher=%s, mix=%r, p=%g, area=(%g, %g), ratio=(%g, %g), threshold=%g, pl_weight=%g, ce_weight=%g, " \
@@ -816,7 +854,7 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
 
     def last_mix(self):
         """{'mask', 'target', 'uniforms'} of the latest training forward (None before the first one)."""
-        return None if self._mix_state is None else dict(self._mix_state)
+        return self._last_record('mix')
 
     def draw(self, x, classes):
         """The forward's uniforms, drawn before the teacher runs: [streams * N, 5] (CutMix) or [streams * N,
@@ -853,7 +891,7 @@ class MixPseudoLabelLoss(PseudoLabelLoss):
             outs.append(ops.mix_apply(self.mix, x[rows] if x.shape[0] > n else x, y, u_k, self.p, self.area,
                                       self.ratio, zoom, amap, sel))
         mask, xm, ym = outs[0] if len(outs) == 1 else (torch.cat(t) for t in zip(*outs))
-        self._mix_state = {'mask': mask, 'target': ym, 'uniforms': u}
+        self._last['mix'] = {'mask': mask, 'target': ym, 'uniforms': u}
         return xm, ym, mask
 
 
@@ -881,6 +919,8 @@ class LovaszSoftmaxLoss(nn.Module):
     radix sort, graphed at every zoom factor; called as a module (validate()) it runs their zoom-1 form on an NHWC copy
     of the logits. CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback. The forward needs
     about 16 C bytes per output pixel of transient workspace and keeps 4 C bytes per output pixel for the backward."""
+
+    graph_options = ("ignore_index", "classes", "per_image", "ce_weight")
 
     def __init__(self, ignore_index=255, classes='present', per_image=False, ce_weight=0.0):
         super(LovaszSoftmaxLoss, self).__init__()
@@ -945,6 +985,8 @@ class RMILoss(nn.Module):
     only: there is no CPU or library fallback. The forward keeps 8 C bytes per pooled cell (the pooled Y and Q maps) for
     the backward."""
 
+    graph_options = ("ignore_index", "bce_weight", "pos_alpha", "ce_weight")
+
     def __init__(self, ignore_index=255, bce_weight=0.5, pos_alpha=5e-4, ce_weight=0.0):
         super(RMILoss, self).__init__()
         if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
@@ -972,3 +1014,19 @@ class RMILoss(nn.Module):
         _check_native_logits("RMILoss", logits, target)
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
         return loss
+
+
+def graph_key(criterion):
+    """The criterion's part of the key of a captured training step (graphs.train_step). Its options are launch arguments
+    baked into the step's graphs, so each criterion class declares them in `graph_options` (nn.CrossEntropyLoss's are
+    ignore_index, label_smoothing and reduction) and a changed option captures anew. The class weights enter as the
+    tensor's address and length: the kernels read them at every replay, so an in-place edit needs no capture, but a
+    replaced tensor does. A teacher criterion adds its teacher's part (_TeacherLoss._teacher_key)."""
+    names = ("ignore_index", "label_smoothing", "reduction") if type(criterion) is nn.CrossEntropyLoss else \
+        criterion.graph_options
+    key = (type(criterion),) + tuple(getattr(criterion, a) for a in names)
+    w = getattr(criterion, "weight", None)
+    key += (w.data_ptr(), w.numel()) if torch.is_tensor(w) else (None,)
+    if isinstance(criterion, _TeacherLoss):
+        key += criterion._teacher_key()
+    return key

@@ -1,6 +1,6 @@
 """CPU tier for the dual-stream perturbation of losses.PseudoLabelLoss / MixPseudoLabelLoss (streams=2): option
-validation and repr, the option in the captured step's key, the prefix fork / fold entry points' argument checks, and
-the oracle of tests/dual_oracle.py against float64 autograd of its definition."""
+validation and repr, the prefix fork / fold entry points' argument checks, and the oracle of tests/dual_oracle.py
+against float64 autograd of its definition."""
 import ctypes
 
 import pytest
@@ -62,51 +62,6 @@ def test_strong_draw_takes_views():
     s = StrongAugment()
     with pytest.raises(TypeError):
         s.draw(torch.zeros((2, 3, 17, 17)), 2)          # a CPU input: refused before torch.rand
-
-
-# ------------------------------------------------------------------------------------------------ graph key
-def test_streams_enter_the_graph_key(nets, monkeypatch):
-    """streams=2 is a new captured step; streams=1 keeps the key of a criterion built without the option."""
-    from semseg_b200 import graphs
-    keys = []
-
-    class _Stop(Exception):
-        pass
-
-    def fake_step(key):
-        keys.append(key)
-        raise _Stop
-
-    monkeypatch.setattr(graphs, "_Step", fake_step)
-    monkeypatch.setattr(graphs, "enabled", lambda: True)
-    student, teacher = nets
-    x = torch.zeros((1, 3, 17, 17))
-    y = torch.zeros((1, 17, 17), dtype=torch.int64)
-
-    class _X:
-        """A stand-in input that passes train_step's device test."""
-        is_cuda, shape, dtype, requires_grad = True, x.shape, x.dtype, False
-        device = torch.device("cuda", 0)
-
-    strong = StrongAugment()
-    variants = [dict(strong=strong), dict(strong=strong, streams=1), dict(strong=strong, streams=2),
-                dict(strong=strong, streams=2, fp_weight=0.5), dict(strong=strong, fp_weight=0.5)]
-    old = student.__dict__.get("criterion")
-    try:
-        for cls in (PseudoLabelLoss, MixPseudoLabelLoss):
-            start = len(keys)
-            for kw in variants:
-                student.criterion = cls(teacher, **kw)
-                student.__dict__.pop("_sb_graph_steps", None)
-                with pytest.raises(_Stop):
-                    graphs.train_step(student, None, _X(), y)
-            crit_keys = [k[-1] for k in keys[start:]]
-            assert crit_keys[0] == crit_keys[1], cls                 # streams=1 is the default's key
-            assert len(set(crit_keys)) == len(variants) - 1, cls
-            assert crit_keys[2] != crit_keys[0] and crit_keys[3] != crit_keys[4], cls
-    finally:
-        if old is not None:
-            student.criterion = old
 
 
 # ------------------------------------------------------------------------------------------------ C-ABI validation

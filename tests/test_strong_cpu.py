@@ -1,7 +1,7 @@
 """CPU tier: the strong view of mean-teacher training (augment.StrongAugment, csrc/strong.cu) — the float64 oracle
 against torchvision.transforms.v2.functional (each operation, all 24 orders, hue at +-0.5, saturation 0, blur at sigma
 0.1, 2 and 5), the per-image parameters at their edges, the argument checks of StrongAugment, of the three teacher
-criteria and of the C entry point, and the view's options in the graph key."""
+criteria and of the C entry point."""
 import ctypes
 import itertools
 import math
@@ -212,53 +212,3 @@ def test_strong_entry_point_validates():
     assert _call(H=6) == -1 and b"ceil(3 sigma_hi) = 6" in _err()
     assert _call(W=6) == -1 and b"ceil(3 sigma_hi) = 6" in _err()
     assert _call(H=15, W=40, shi=5.0) == -1 and b"= 15" in _err()
-
-
-# ------------------------------------------------------------------------------------------------ graph key
-def test_strong_options_enter_the_graph_key(nets, monkeypatch):
-    """Each option of the strong view is part of the captured step's key; without a view the key is the criterion's."""
-    from semseg_b200 import graphs
-    keys = []
-
-    class _Stop(Exception):
-        pass
-
-    def fake_step(key):
-        keys.append(key)
-        raise _Stop
-
-    monkeypatch.setattr(graphs, "_Step", fake_step)
-    monkeypatch.setattr(graphs, "enabled", lambda: True)
-    student, teacher = nets
-    x = torch.zeros((1, 3, 17, 17))
-    y = torch.zeros((1, 17, 17), dtype=torch.int64)
-
-    class _X:
-        """A stand-in input that passes train_step's device test."""
-        is_cuda, shape, dtype, requires_grad = True, x.shape, x.dtype, False
-        device = torch.device("cuda", 0)
-
-    variants = [None, dict(), dict(brightness=0.4), dict(contrast=0.4), dict(saturation=0.4), dict(hue=0.2),
-                dict(p_jitter=0.7), dict(p_gray=0.1), dict(p_blur=0.4), dict(sigma=(0.2, 2.0)), dict(sigma=(0.1, 3.0)),
-                dict(mean=(1.0, 2.0, 3.0)), dict(std=(50.0, 60.0, 70.0))]
-    old = student.__dict__.get("criterion")
-    try:
-        for cls in (PseudoLabelLoss, MixPseudoLabelLoss, DistillationLoss):
-            start = len(keys)
-            for kw in variants:
-                student.criterion = cls(teacher, strong=None if kw is None else StrongAugment(**kw))
-                student.__dict__.pop("_sb_graph_steps", None)
-                with pytest.raises(_Stop):
-                    graphs.train_step(student, None, _X(), y)
-            crit_keys = [k[-1] for k in keys[start:]]
-            assert len(set(crit_keys)) == len(variants), cls
-            # without a view the key is exactly the criterion's own
-            plain = cls(teacher)
-            student.criterion = plain
-            student.__dict__.pop("_sb_graph_steps", None)
-            with pytest.raises(_Stop):
-                graphs.train_step(student, None, _X(), y)
-            assert keys[-1][-1] == crit_keys[0] and "strong" not in keys[-1][-1]
-    finally:
-        if old is not None:
-            student.criterion = old

@@ -72,7 +72,7 @@ class TorchMix(MixPseudoLabelLoss):
         xm = torch.where(mask.unsqueeze(1), x.roll(-1, 0), x)
         s = 8 // zoom
         ym = torch.where(mask[:, ::s, ::s], y.roll(-1, 0), y)
-        self._mix_state = {'mask': mask.to(torch.uint8), 'target': ym, 'uniforms': u}
+        self._last['mix'] = {'mask': mask.to(torch.uint8), 'target': ym, 'uniforms': u}
         return xm, ym, mask.to(torch.uint8)
 
 
