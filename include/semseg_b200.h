@@ -30,6 +30,7 @@
  *                               semseg_upsample_pl_*: confidence-masked pseudo-labels from a teacher's logits.
  *                               semseg_upsample_ce_entropy_*: entropy minimisation, plus cross-entropy.
  *                               semseg_gated_crf_*: the Gated CRF loss's pairwise term (csrc/crf.cu).
+ *                               semseg_abl_*: the Active Boundary Loss term (csrc/boundary.cu).
  *   - semseg_window_*         : the post-network steps of sliding-window evaluation (tool/test.py:122-178): the eval
  *                               logit upsample (model/pspnet.py:95, tool/test.py:138), softmax and flip averaging
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
@@ -745,6 +746,42 @@ int semseg_gated_crf_bwd(const float* logits, int pitch, int N, int h, int w, in
                          const float* image, int H, int W, int istride, int radius, float sigma_xy, float sigma_rgb,
                          float mean0, float mean1, float mean2, float std0, float std1, float std2, const float* s_in,
                          float crf_weight, const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Active Boundary Loss (Wang et al., AAAI 2022; semseg_b200/losses.py ActiveBoundaryLoss), the boundary term, on the
+ * loss grid Hg x Wg = zoom (h-1)+1 x zoom (w-1)+1 of the fp32 NHWC logits [N,h,w,pitch] (zoom 1: the logits grid
+ * itself; zoom > 1: the tail's bilinear xZ upsample, align_corners), with the target int64 [N,Hg,Wg]. Per image, with
+ * p = softmax of the grid logits s and KL(a|b) = sum_c a_c (log a_c - log b_c):
+ *   GT boundary: t(y,x) != t(y+1,x), t(y,x) != t(y,x+1) or t(y,x) == ignore_index;
+ *   D = fp32(max(sqrt(e) - 1, 0)), e the exact squared distance to the image's nearest GT-boundary pixel (+inf on an
+ *     image without one: it selects nothing);
+ *   k(y,x) = KL(p_yx | p_y+1,x) + KL(p_yx | p_y,x+1) (0 past the last row / column); t_0 = 1e-5, t_j+1 = 1.2 t_j in
+ *     fp64, compared as fp32; j* = the smallest j < 256 with #(k > t_j) <= max_n_ratio Hg Wg over the call (255 if
+ *     none); B(p) = some pixel of p's 3x3 neighbourhood has k > t_j*;
+ *   neighbours n_0..n_7 at (+1,0) (-1,0) (0,-1) (0,+1) (-1,+1) (+1,+1) (-1,-1) (+1,-1), 8 = p itself; dir(p) = the
+ *     first argmin of D over the nine (out-of-image: +inf); p is selected if B(p), dir != 8 and D(p) is finite;
+ *   z_j = KL(p_nj | p) (an out-of-image n_j replicates the edge), y_dir = 1 - label_smoothing, y_j = label_smoothing
+ *     / 8 elsewhere, l = -sum_j y_j log softmax(z)_j, w = min(D, max_clip_dist) / max_clip_dist;
+ *   ABL = (1/M) sum over the M selected pixels of w l (0 when M = 0); dz_j/ds_p,c = p_c - p_nj,c (n_j detached).
+ *   fwd: lse fp32 [N,Hg,Wg], the grid's per-pixel logsumexp (the zoom forward's); state: semseg_abl_workspace_floats
+ *        (pass 0) floats, kept for the backward, P = N Hg Wg, in 4-byte words: D fp32 [P] at 0, k fp32 [P] at P, w dl/dz
+ *        fp32 [P][8] at 2P (written for the selected pixels), code uint8 [P] at 10P (dir | B << 4 | selected << 5; dir
+ *        15 on an image without a GT boundary), the level histogram int32 [257] at 10P + ceil(P/4), then j* int32 and
+ *        the bits of t_j*, then the per-tile partials (16 x 473^2 images: 0.15 GB); loss_out fp32 [2] = (ABL, M)
+ *        through the tail's fp64 reduce.
+ *   bwd: ADDS grad_out[0] * abl_weight * dABL/dlogits into dlogits fp32 [N,h,w,C] (written before, e.g. by the
+ *        cross-entropy backward), from the forward's lse, state and loss_out (loss_info); workspace:
+ *        semseg_abl_workspace_floats (pass 1) floats, 0 at zoom 1, else N C Wg (Hg + h), the output-resolution
+ *        gradient and its row adjoint (21 classes at 16 x 473^2, zoom 8: 0.34 GB; 150 classes: 2.4 GB).
+ * Limits: C <= 256, N <= 65535, Hg <= 65535 * 16, max_n_ratio in [0, 1], max_clip_dist finite and > 0,
+ * label_smoothing in [0, 1], abl_weight finite and >= 0. A bad argument is rejected before any CUDA call; the
+ * workspace function returns -1 for a bad zoom, size or pass. The histogram counts with integer atomics; no other
+ * atomics, no host synchronisation: deterministic, and graph-capturable. */
+long long semseg_abl_workspace_floats(int N, int h, int w, int C, int zoom, int pass);
+int semseg_abl_fwd(const float* logits, int pitch, int N, int h, int w, int C, int zoom, const float* lse,
+                   const void* target_i64, long long ignore_index, double max_n_ratio, float max_clip_dist,
+                   float label_smoothing, float* state, float* loss_out, void* stream);
+int semseg_abl_bwd(const float* logits, int pitch, int N, int h, int w, int C, int zoom, const float* lse,
+                   const float* state, const float* loss_info, float abl_weight, const float* grad_out,
+                   float* workspace, float* dlogits, void* stream);
 /* Mixed-sample masks and batches (csrc/mix.cu) for mean-teacher training. Image n is mixed with its partner
  * pi(n) = (n + 1) mod N; uniforms fp32 [N, ustride] hold u0 (apply), u1 (area), u2 (ratio), u3 (row), u4 (column) and,
  * for ClassMix, class priorities u[n, 5 + c]; image n is mixed iff (double) u0 < p.
@@ -836,6 +873,16 @@ int semseg_window_resize_add(const double* canvas, int C, int Hi, int Wi, double
  */
 int semseg_iou_hist(void* pred_i64, const void* target_i64, long long n, int K, long long ignore_index, int write_back,
                     int* counts, void* stream);
+/* Boundary IoU (Cheng et al., CVPR 2021; semseg_b200/metrics.py boundaryIoUGPU) of pred and target int64 [N,H,W]:
+ *   a pixel of label c lies in its map's band if its (2d+1)^2 window holds another label or reaches outside the image
+ *   (the per-class mask padded by 1 and 3x3-eroded d times, subtracted from the mask); in the target ignore_index is a
+ *   label of its own. Over the pixels whose target is not ignore_index, counts int32 [3][K] (zeroed by the call):
+ *   [0] = #(pred == target == k, both in band), [1] = #(pred == k in band), [2] = #(target == k in band); union =
+ *   [1] + [2] - [0]. Labels outside [0, K) are not counted; labels are compared saturated to int32.
+ *   workspace: 4 N H W int32 (the row-window minima and maxima of both maps). 1 <= K <= 4096, d >= 1.
+ */
+int semseg_boundary_iou_hist(const void* pred_i64, const void* target_i64, int N, int H, int W, int K,
+                             long long ignore_index, int d, int* workspace, int* counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * torch.optim.SGD (momentum, dampening, weight decay, nesterov; tool/train.py:140,274-276) over every parameter tensor in

@@ -132,6 +132,7 @@ SIGNATURES = {
     "semseg_sgd_multi": (c_int, [c_vp, c_vp, c_int, c_int, ctypes.POINTER(SgdHyper), c_vp]),
     "semseg_ema_multi": (c_int, [c_vp, c_int, c_int, ctypes.c_double, c_vp]),
     "semseg_iou_hist": (c_int, [c_vp, c_vp, ctypes.c_longlong, c_int, ctypes.c_longlong, c_int, c_vp, c_vp]),
+    "semseg_boundary_iou_hist": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_ll, c_int, c_vp, c_vp, c_vp]),
     "semseg_im2col3x3s2": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_stem_dgrad3x3s2": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int,
                                        c_vp, c_vp]),
@@ -262,6 +263,11 @@ SIGNATURES = {
     "semseg_gated_crf_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_gated_crf_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int,
                                      c_int, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_f, c_vp, c_f, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_abl_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
+    "semseg_abl_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_ll, ctypes.c_double, c_f,
+                               c_f, c_vp, c_vp, c_vp]),
+    "semseg_abl_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_f, c_vp, c_vp,
+                               c_vp, c_vp]),
     "semseg_mix_argmax_x8": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "semseg_mix_select": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_vp, c_vp]),
     "semseg_mix_apply": (c_int, [c_int, c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_vp, c_int,

@@ -284,6 +284,19 @@ gated_crf_adjoint_cols_kernel(const float* __restrict__ T, int N, int h, int w, 
   dlogits[i] += acc;
 }
 
+// The two adjoint passes above, for the other translation units too (csrc/boundary.cu).
+int launch_bilinear_adjoint(const float* D, float* T, int N, int h, int w, int Hg, int Wg, int C, int zoom,
+                            float* dlogits, cudaStream_t stream) {
+  const long long rows = static_cast<long long>(N) * h * Wg * C, cols = static_cast<long long>(N) * h * w * C;
+  gated_crf_adjoint_rows_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, stream>>>(D, N, h, Hg, Wg, C,
+                                                                                              zoom, T);
+  SB_LAUNCHED();
+  gated_crf_adjoint_cols_kernel<<<static_cast<unsigned>((cols + 255) / 256), 256, 0, stream>>>(T, N, h, w, Wg, C,
+                                                                                              zoom, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -457,13 +470,6 @@ extern "C" int semseg_gated_crf_bwd(const float* logits, int pitch, int N, int h
     default: r = launch_crf_bwd<32>(g, s_in, scale, grad_out, out, acc, stream); break;
   }
   if (r || zoom == 1) return r;
-  float* T = workspace + static_cast<long long>(N) * g.Hg * g.Wg * C;
-  const long long rows = static_cast<long long>(N) * h * g.Wg * C, cols = static_cast<long long>(N) * h * w * C;
-  gated_crf_adjoint_rows_kernel<<<static_cast<unsigned>((rows + 255) / 256), 256, 0, stream>>>(workspace, N, h, g.Hg,
-                                                                                              g.Wg, C, zoom, T);
-  SB_LAUNCHED();
-  gated_crf_adjoint_cols_kernel<<<static_cast<unsigned>((cols + 255) / 256), 256, 0, stream>>>(T, N, h, w, g.Wg, C,
-                                                                                              zoom, dlogits);
-  SB_LAUNCHED();
-  return SEMSEG_OK;
+  return launch_bilinear_adjoint(workspace, workspace + static_cast<long long>(N) * g.Hg * g.Wg * C, N, h, w, g.Hg,
+                                 g.Wg, C, zoom, dlogits, stream);
 }

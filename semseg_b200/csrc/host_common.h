@@ -57,6 +57,11 @@ void choose_box(int H, int W, int max_pixels, int* bh, int* bw);
 // 1), loss_out[1] = count.
 int launch_mean_reduce(const float* partial, int nblocks, float* loss_out, cudaStream_t stream);
 
+// The bilinear adjoint of the tail's xZ upsample (csrc/crf.cu): dlogits [N,h,w,C] += the fold of the output-resolution
+// gradient D [N,Hg,Wg,C], a rows pass into T [N,h,Wg,C], then a cols pass.
+int launch_bilinear_adjoint(const float* D, float* T, int N, int h, int w, int Hg, int Wg, int C, int zoom,
+                            float* dlogits, cudaStream_t stream);
+
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
 // An activation operand of a kernel that accesses it in vector pieces (act_ld8 / act_st8, uint4, uint2): hi and lo

@@ -697,6 +697,33 @@ def gated_crf(logits, image, criterion):
     return _GatedCRF.apply(logits, image.detach().contiguous(), _crf_cfg(criterion))
 
 
+def _abl_cfg(crit):
+    return crit.max_n_ratio, crit.max_clip_dist, crit.label_smoothing
+
+
+class _UpsampleCEABL(torch.autograd.Function):
+    """The fused tail with losses.ActiveBoundaryLoss: ce_weight * CE (the plain forward and backward, unchanged) plus
+    abl_weight * the ABL term on the tail's output grid. The ABL forward keeps its state (distance map, selection and
+    w dl/dz per selected pixel); its backward adds into the CE gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, abl_weight, ce_weight, cfg):
+        info, amax, lse = ops.upsample_ce_fwd(logits, target, ignore_index, zoom=zoom)
+        ainfo, state = ops.abl_fwd(logits, lse, target, ignore_index, zoom, *cfg)
+        ctx.save_for_backward(logits, target, lse, info, ainfo, state)
+        ctx.cfg = (ignore_index, zoom, abl_weight, ce_weight)
+        ctx.mark_non_differentiable(amax)
+        return torch.add(info[0] * ce_weight, ainfo[0], alpha=abl_weight), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, info, ainfo, state = ctx.saved_tensors
+        ignore_index, zoom, abl_weight, ce_weight = ctx.cfg
+        dl = ops.upsample_ce_bwd(logits, target, ignore_index, lse, info, grad_loss * ce_weight, zoom=zoom)
+        ops.abl_bwd(logits, lse, state, ainfo, abl_weight, grad_loss, dl, zoom)
+        return dl, None, None, None, None, None, None
+
+
 class _UpsampleCELovasz(torch.autograd.Function):
     """The fused tail with losses.LovaszSoftmaxLoss, plus ce_weight * CE. The forward keeps the per pixel-class
     Lovász gradient weights (gamma, 4 C bytes per output pixel) it scattered from the sorted segments; the sort's
@@ -870,8 +897,9 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
     losses.EntropyLoss, whose rows kernel stages the same words, the Dice width limit. losses.RMILoss needs a target of
     at least 12 x 12 and no wider than its rows kernel stages (3584 columns
-    at zoom 8). losses.GatedCRFLoss needs the target no wider than the plain backward stages (2560 columns at zoom 8);
-    its classes (<= 256, checked here with the logits), radius and sigmas are in the kernels' limits by construction.
+    at zoom 8). losses.GatedCRFLoss and losses.ActiveBoundaryLoss need the target no wider than the plain backward
+    stages (2560 columns at zoom 8); their classes (<= 256, checked here with the logits) and options are in the
+    kernels' limits by construction.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
     if type(criterion) is losses.DistillationLoss:
         ok = True
@@ -885,9 +913,10 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         # the focal rows kernel (the pseudo-label backward too) and the entropy rows kernel stage the Dice words
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
-    elif type(criterion) is losses.GatedCRFLoss:
+    elif type(criterion) in (losses.GatedCRFLoss, losses.ActiveBoundaryLoss):
         # the cross-entropy part is the plain tail's, whose backward stages 8 bytes per pixel of Z rows in 160 KB; the
-        # CRF kernels take any width (csrc/crf.cu), and the criterion keeps radius, classes and sigmas in their limits
+        # CRF and ABL kernels take any width (csrc/crf.cu, csrc/boundary.cu), and the criteria keep their options in
+        # the kernels' limits
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _CRF_CE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _CRF_CE_STAGE_BYTES)
     elif type(criterion) is losses.RMILoss:
@@ -932,8 +961,16 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     pixels plus ent_weight * mean entropy over the unlabelled ones (its own ignore_index); the networks score their aux
     head with the plain form. With a losses.GatedCRFLoss and the network's fp32 NCHW input `image` (a constant),
     ce_weight * CE plus crf_weight * its Gated CRF term; `image_stride` is the image's pixel stride on the loss grid
-    (default: 8 / zoom at at='output', 8 at at='logits'); without an image a positive crf_weight raises. The default
+    (default: 8 / zoom at at='output', 8 at at='logits'); without an image a positive crf_weight raises. With a
+    losses.ActiveBoundaryLoss, ce_weight * CE plus abl_weight * its boundary term on the output grid. The default
     criterion runs the plain kernels."""
+    if isinstance(criterion, losses.ActiveBoundaryLoss):
+        if criterion.abl_weight == 0.0:
+            # no ABL kernel: the plain step, bit for bit when ce_weight is 1
+            loss, amax = _UpsampleCE.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom))
+            return (loss if criterion.ce_weight == 1.0 else loss * criterion.ce_weight), amax
+        return _UpsampleCEABL.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                    criterion.abl_weight, criterion.ce_weight, _abl_cfg(criterion))
     if isinstance(criterion, losses.GatedCRFLoss):
         if criterion.crf_weight == 0.0:
             # no CRF kernel: the plain step, bit for bit when ce_weight is 1

@@ -8,7 +8,8 @@ LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and Foc
 optional class weights, run the same way, and so do RMILoss, the Region Mutual Information loss with its BCE term,
 EntropyLoss, entropy minimisation on the unlabelled pixels plus cross-entropy on the labelled ones (TENT's objective,
 adapt.Tent), and GatedCRFLoss, cross-entropy plus the Gated CRF pairwise term for scribble- and point-supervised
-training. DistillationLoss adds a
+training, and ActiveBoundaryLoss, cross-entropy plus the Active Boundary Loss that moves predicted boundaries towards
+the ground truth's. DistillationLoss adds a
 pixel-wise distillation term from a teacher network that the student's training forward runs, and PseudoLabelLoss a
 confidence-masked pseudo-label term on the unlabelled pixels; the teacher is a frozen network or the mean teacher of an
 optim.ModelEMA. MixPseudoLabelLoss is that pseudo-label loss with CutMix or ClassMix: the teacher labels the clean
@@ -386,6 +387,79 @@ class GatedCRFLoss(nn.Module):
             raise ValueError("GatedCRFLoss: at most 256 classes (got %d); no fallback" % logits.shape[1])
         self._check_image(image, logits.shape[0], logits.shape[2], logits.shape[3])
         return SF.gated_crf(logits.permute(0, 2, 3, 1).contiguous(), image, self)
+
+
+class ActiveBoundaryLoss(nn.Module):
+    """Cross-entropy plus the Active Boundary Loss (Wang et al., "Active Boundary Loss for Semantic Segmentation", AAAI
+    2022): it moves the predicted boundaries, where neighbouring class distributions diverge, towards the ground
+    truth's, which networks that predict at 1/8 resolution and upsample bilinearly blur. On the loss grid (the target
+    grid, the logits upsampled xZ, align_corners), with p = softmax and KL(a|b) = sum_c a_c (log a_c - log b_c), per
+    rank over the N images of the call:
+
+        GT boundary  t(y,x) != t(y+1,x), t(y,x) != t(y,x+1), or t(y,x) == ignore_index
+        D(p)         max(sqrt(e) - 1, 0), e the exact squared distance to the image's nearest GT-boundary pixel
+        k(y,x)       KL(p_yx | p_y+1,x) + KL(p_yx | p_y,x+1)           (a term is 0 past the last row / column)
+        j*           the smallest j < 256 with #(k > t_j) <= max_n_ratio Hg Wg over the call, t_j = 1e-5 1.2^j
+        B(p)         some pixel of p's 3x3 neighbourhood has k > t_j*
+        dir(p)       the first argmin of D over the 8 neighbours (+1,0) (-1,0) (0,-1) (0,+1) (-1,+1) (+1,+1) (-1,-1)
+                     (+1,-1) and p itself (index 8; out-of-image neighbours: +inf)
+        selected     B(p), dir(p) != 8 and p's image has a GT boundary; M of them
+        z_j          KL(p_nj | p), the neighbour's distribution detached (an out-of-image n_j replicates the edge)
+        l(p)         -sum_j y_j log softmax(z)_j, y_dir = 1 - label_smoothing, y_j = label_smoothing / 8 elsewhere
+        w(p)         min(D(p), max_clip_dist) / max_clip_dist
+        main         ce_weight CE + abl_weight (1/M) sum_selected w l,  CE the mean over the labelled pixels
+        aux          the aux head's plain CE;  pred = argmax
+
+    The published code differs where it is undefined or host-bound: ABL is 0 with a zero gradient when M = 0 (it
+    returns None there), an image without a GT boundary selects nothing (its scipy distance map is meaningless), the
+    threshold search is a histogram on the device instead of a host loop, and the direction targets' smoothing weights
+    are kept as published (they sum to 1 - label_smoothing / 8). The selection, directions and weights are constants:
+    the gradient flows through the centre distribution of each z_j only. abl_weight = 0 runs no ABL kernel: the step is
+    the nn.CrossEntropyLoss(ignore_index) step.
+
+    With the network's fused tail (functional.upsample_ce) it runs on the tail's kernels and csrc/boundary.cu, graphed
+    at every zoom factor: the distance transform, the threshold search and the selection never leave the device.
+    Called as a module, forward(logits, target) takes NCHW logits at the target size and returns `main` (the zoom-1
+    kernels on an NHWC copy), which the networks' ATen tail and validate() use. CUDA fp32 only, at most 256 classes:
+    there is no CPU or library fallback."""
+
+    graph_options = ("ignore_index", "abl_weight", "ce_weight", "label_smoothing", "max_n_ratio", "max_clip_dist")
+
+    def __init__(self, ignore_index=255, abl_weight=1.0, ce_weight=1.0, label_smoothing=0.2, max_n_ratio=0.01,
+                 max_clip_dist=20.0):
+        super(ActiveBoundaryLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        self.ignore_index = ignore_index
+        self.abl_weight = _non_negative("abl_weight", abl_weight)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+        self.label_smoothing = _non_negative("label_smoothing", label_smoothing)
+        if self.label_smoothing > 1.0:
+            raise ValueError("label_smoothing must lie in [0, 1], got %r" % (label_smoothing,))
+        self.max_n_ratio = _non_negative("max_n_ratio", max_n_ratio)
+        if self.max_n_ratio > 1.0:
+            raise ValueError("max_n_ratio must lie in [0, 1], got %r" % (max_n_ratio,))
+        self.max_clip_dist = _non_negative("max_clip_dist", max_clip_dist)
+        if self.max_clip_dist == 0.0:
+            raise ValueError("max_clip_dist must be > 0, got %r" % (max_clip_dist,))
+
+    def extra_repr(self):
+        return ("ignore_index=%d, abl_weight=%g, ce_weight=%g, label_smoothing=%g, max_n_ratio=%g, max_clip_dist=%g" %
+                (self.ignore_index, self.abl_weight, self.ce_weight, self.label_smoothing, self.max_n_ratio,
+                 self.max_clip_dist))
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        _check_native_logits("ActiveBoundaryLoss", logits, target)
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+    def aux_loss(self, logits, target):
+        """The aux head's loss, module form: the plain mean cross-entropy of NCHW logits at the target size."""
+        from . import functional as SF
+        _check_native_logits("ActiveBoundaryLoss", logits, target)
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1)
+        return loss
 
 
 class _TeacherLoss(nn.Module):

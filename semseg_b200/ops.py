@@ -1037,6 +1037,76 @@ def gated_crf_bwd(logits, lse, image, s, crf_weight, grad_out, dlogits, zoom, is
     return dlogits
 
 
+def abl_fwd(logits, lse, target, ignore_index, zoom, max_n_ratio, max_clip_dist, label_smoothing):
+    """The Active Boundary Loss term (include/semseg_b200.h states the contract) on the grid zoom*(h-1)+1 x zoom*(w-1)+1
+    of the fp32 NHWC logits [N,h,w,C], target int64 [N,Hg,Wg], `lse` the grid's per-pixel logsumexp (the zoom
+    forward's): -> (info [2] = (ABL, M), state). `state` is the flat forward state the backward reads; abl_maps views
+    its maps."""
+    _require_cuda(logits, lse, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    n, h, w, c = logits.shape
+    zoom = int(zoom)
+    hg, wg = zoom * (h - 1) + 1, zoom * (w - 1) + 1
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (n, hg, wg)
+    assert target.dtype == torch.int64 and target.is_contiguous() and tuple(target.shape) == (n, hg, wg)
+    nws = int(lib.semseg_abl_workspace_floats(n, h, w, c, zoom, 0))
+    _lib.check(0 if nws >= 0 else nws, "semseg_abl_workspace_floats")
+    state = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    info = torch.empty((2,), dtype=torch.float32, device=logits.device)
+    _lib.check(lib.semseg_abl_fwd(_ptr(logits), logits.stride(2), n, h, w, c, zoom, _ptr(lse), _ptr(target),
+                                  int(ignore_index), float(max_n_ratio), float(max_clip_dist), float(label_smoothing),
+                                  _ptr(state), _ptr(info), _stream()),
+               "semseg_abl_fwd")
+    return info, state
+
+
+def abl_maps(state, n, hg, wg):
+    """Views of the forward state of abl_fwd on an [n, hg, wg] grid: D, k (fp32), w dl/dz (fp32 [.., 8], valid at the
+    selected pixels), code (uint8: dir | B << 4 | selected << 5) and j* (int32 [1])."""
+    p = n * hg * wg
+    code_words = (p + 3) // 4
+    ints = state.view(torch.int32)
+    return {"D": state[:p].view(n, hg, wg), "k": state[p:2 * p].view(n, hg, wg),
+            "wg": state[2 * p:10 * p].view(n, hg, wg, 8),
+            "code": state[10 * p:10 * p + code_words].view(torch.uint8)[:p].view(n, hg, wg),
+            "jstar": ints[10 * p + code_words + 257:10 * p + code_words + 258]}
+
+
+def abl_bwd(logits, lse, state, info, abl_weight, grad_out, dlogits, zoom):
+    """Adds grad_out[0] * abl_weight * dABL/dlogits into dlogits (fp32 [N,h,w,C], contiguous) in place, from the
+    forward's lse, state and info."""
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    zoom = int(zoom)
+    assert dlogits.dtype == torch.float32 and dlogits.is_contiguous() and tuple(dlogits.shape) == (n, h, w, c)
+    nws = int(lib.semseg_abl_workspace_floats(n, h, w, c, zoom, 1))
+    _lib.check(0 if nws >= 0 else nws, "semseg_abl_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_abl_bwd(_ptr(logits), logits.stride(2), n, h, w, c, zoom, _ptr(lse), _ptr(state), _ptr(info),
+                                  float(abl_weight), _ptr(g), _ptr(ws), _ptr(dlogits), _stream()),
+               "semseg_abl_bwd")
+    return dlogits
+
+
+def boundary_iou_hist(output, target, K, ignore_index, d):
+    """Boundary IoU counts of int64 [N,H,W] maps with band width d: -> int32 [3, K] = (intersection, |output band|,
+    |target band|) per class."""
+    _require_cuda(output, target)
+    assert output.dtype == torch.int64 and target.dtype == torch.int64 and output.dim() == 3
+    assert output.shape == target.shape
+    lib = _lib.load()
+    n, h, w = output.shape
+    out, tgt = output.contiguous(), target.contiguous()
+    ws = torch.empty((4 * n * h * w,), dtype=torch.int32, device=output.device)
+    counts = torch.empty((3, int(K)), dtype=torch.int32, device=output.device)
+    _lib.check(lib.semseg_boundary_iou_hist(_ptr(out), _ptr(tgt), n, h, w, int(K), int(ignore_index), int(d), _ptr(ws),
+                                            _ptr(counts), _stream()),
+               "semseg_boundary_iou_hist")
+    return counts
+
+
 def upsample_ce_lovasz_fwd(logits, target, ignore_index, classes_all, per_image, ce_weight, want_argmax=True, zoom=8,
                            return_workspace=False):
     """Lovász-Softmax loss (+ ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract) ->

@@ -187,9 +187,9 @@ class _SegNet(nn.Module):
         fp_logits = logits[streams] if fp_scale is not None else None
 
         if self.training:
-            # losses.EntropyLoss and losses.GatedCRFLoss score the aux head with the plain cross-entropy over the
-            # labelled pixels; the Gated CRF term reads the input batch
-            plain_aux = isinstance(self.criterion, (losses.EntropyLoss, losses.GatedCRFLoss))
+            # losses.EntropyLoss, losses.GatedCRFLoss and losses.ActiveBoundaryLoss score the aux head with the plain
+            # cross-entropy over the labelled pixels; the Gated CRF term reads the input batch
+            plain_aux = isinstance(self.criterion, (losses.EntropyLoss, losses.GatedCRFLoss, losses.ActiveBoundaryLoss))
             crf = isinstance(self.criterion, losses.GatedCRFLoss)
             aux_logits = _chunks(head_forward_nhwc(self.aux, t_aux), streams)
             ys = _chunks(y, streams) if mix_mask is not None else (y,) * streams      # the mixed target is [2N]
