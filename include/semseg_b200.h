@@ -36,6 +36,8 @@
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
  *                               (tool/test.py:163-176) and the per-scale resize into the running total
  *                               (tool/test.py:177, 202).
+ *   - semseg_densecrf_*       : dense CRF refinement of the evaluation scores (pydensecrf's DenseCRF2D with a Gaussian
+ *                               and a bilateral Potts kernel), on a device permutohedral lattice.
  *   - semseg_augment          : tool/train.py:194-212's transform chains (util/transform.py), one launch per batch.
  *   - semseg_strong_augment   : the strong (colour jitter, grayscale, blur) student view of mean-teacher training.
  *
@@ -863,6 +865,44 @@ int semseg_window_accumulate(const float* scores, int C, int crop_h, int crop_w,
                              int nx, int full_h, int full_w, int top, int left, int img_h, int img_w, double* canvas,
                              void* stream);
 int semseg_window_resize_add(const double* canvas, int C, int Hi, int Wi, double* total, int Ho, int Wo, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Dense CRF refinement of one image (Krähenbühl & Koltun 2011; semseg_b200/densecrf.py DenseCRF; csrc/densecrf.cu):
+ * Potts mean field with a smoothness kernel exp(-|p_i - p_j|^2 / 2 pos_xy_std^2) (d = 2) and an appearance kernel
+ * exp(-|p_i - p_j|^2 / 2 bi_xy_std^2 - |I_i - I_j|^2 / 2 bi_rgb_std^2) (d = 5), each on a permutohedral lattice and
+ * symmetrically normalised: K~ v = n * K (n * v), n = (K 1 + 1e-20)^-1/2. Pixel i = y W + x has position (x, y) and
+ * colour I_i = image[i][0..2], clamped to [0, 255].
+ *   lattice_bytes : size of the lattice buffer of an H x W image; both lattices at their worst case V = N (d+1) plus the
+ *                   build's scratch, about 700 bytes per pixel (1.5 GB at 2048 x 1024).
+ *   build         : image fp32 HWC [H][W][3] -> lattice. The first two int32 of the lattice are then V_s and V_a, the
+ *                   vertex counts, read back once to size the value buffers. Lattice keys pack the d stored coordinates
+ *                   into 64 bits with per-coordinate widths from their range (image size and standard deviations); a
+ *                   configuration that needs more than 64 bits, or a coordinate range beyond +-2^52, is rejected.
+ *                   0 < H W, 6 H W < 2^31.
+ *   values_floats : values workspace of meanfield / filter = 2 (V_s + V_a) C floats (two [V][C] buffers per kernel).
+ *   meanfield     : prob fp32 [H W][C] (class-contiguous) -> Q fp32 [H W][C]: Q0 = softmax(log max(prob, clip)), then
+ *                   `iterations` times Q <- softmax(log max(prob, clip) + pos_weight K~_s Q + bi_weight K~_a Q). A
+ *                   kernel of weight 0 is skipped. FLT_MIN <= clip < 1 (the log is taken in fp32), weights finite
+ *                   and >= 0, iterations >= 0.
+ *   filter        : out fp32 [H W][C] = K~ in for kernel 0 (smoothness) or 1 (appearance).
+ *   keys          : out int32 [V][d] = the vertex keys of kernel 0 or 1 (the first d lattice coordinates, in key order),
+ *                   given the standard deviations of the build.
+ * V_s / V_a passed to meanfield, filter and keys are the build's. Deterministic (no float atomics, every result
+ * written once); the build reads nothing back to the host. Bad arguments (empty images, non-finite or non-positive
+ * standard deviations, negative or non-finite weights, iterations < 0, clip outside [FLT_MIN, 1), key overflow, null
+ * pointers) are rejected before any CUDA call.
+ */
+long long semseg_densecrf_lattice_bytes(int H, int W);
+int semseg_densecrf_build(const float* image, int H, int W, double pos_xy_std, double bi_xy_std, double bi_rgb_std,
+                          void* lattice, void* stream);
+long long semseg_densecrf_values_floats(int H, int W, int Vs, int Va, int C);
+int semseg_densecrf_meanfield(const void* lattice, int H, int W, int Vs, int Va, const float* prob, int C, double clip,
+                              int iterations, double pos_weight, double bi_weight, float* values, float* Q,
+                              void* stream);
+int semseg_densecrf_filter(const void* lattice, int H, int W, int Vs, int Va, int kernel, const float* in, int C,
+                           float* values, float* out, void* stream);
+int semseg_densecrf_keys(const void* lattice, int H, int W, int Vs, int Va, int kernel, double pos_xy_std,
+                         double bi_xy_std, double bi_rgb_std, int* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Step glue: per-class intersection / union / target areas (util/util.py:55-67, called at tool/train.py:286,375).

@@ -18,6 +18,7 @@ c_i32 = ctypes.c_int32
 c_vp = ctypes.c_void_p
 c_f = ctypes.c_float
 c_ll = ctypes.c_longlong
+c_d = ctypes.c_double
 I9 = c_i32 * MAX_TAPS
 
 
@@ -281,6 +282,13 @@ SIGNATURES = {
     "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_window_resize_add": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    "semseg_densecrf_lattice_bytes": (c_ll, [c_int, c_int]),
+    "semseg_densecrf_build": (c_int, [c_vp, c_int, c_int, c_d, c_d, c_d, c_vp, c_vp]),
+    "semseg_densecrf_values_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_densecrf_meanfield": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_d, c_int, c_d, c_d, c_vp,
+                                          c_vp, c_vp]),
+    "semseg_densecrf_filter": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_vp, c_vp, c_vp]),
+    "semseg_densecrf_keys": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_d, c_d, c_d, c_vp, c_vp]),
     "semseg_augment": (c_int, [c_vp, c_ll, ctypes.POINTER(AugmentDesc), c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int,
                                c_vp, c_vp, c_vp]),
 }

@@ -79,7 +79,14 @@ def _native_net(model, classes, crop_h, crop_w, device):
 class SlidingWindowPredictor:
     """model: eval-mode network mapping [B, 3, crop_h, crop_w] -> [B, classes, h', w'] logits."""
 
-    def __init__(self, model, classes, crop_h, crop_w, mean, std=None, stride_rate=2 / 3, flip=True, max_batch=32):
+    def __init__(self, model, classes, crop_h, crop_w, mean, std=None, stride_rate=2 / 3, flip=True, max_batch=32,
+                 crf=None):
+        """crf: None, or a densecrf.DenseCRF run on the scale-averaged scores before the argmax (both finishes); the
+        returned scores are then its marginals."""
+        from .densecrf import DenseCRF
+        if crf is not None and not isinstance(crf, DenseCRF):
+            raise TypeError("SlidingWindowPredictor: crf must be None or a DenseCRF, got %s" % type(crf).__name__)
+        self.crf = crf
         self.model, self.classes = model, int(classes)
         self.crop_h, self.crop_w = int(crop_h), int(crop_w)
         self.mean = [float(m) for m in mean]
@@ -181,7 +188,9 @@ class SlidingWindowPredictor:
         exact=True  : every step as in the reference (host cv2 resize of each scale's score map, numpy accumulation):
                       bit-identical to the serial procedure, but the host works on [h, w, classes] float64 arrays.
         exact=False : score maps are resized, summed over the scales and arg-maxed on the device; only the result
-                      crosses PCIe (the argmax, plus the scores when return_scores)."""
+                      crosses PCIe (the argmax, plus the scores when return_scores).
+        With a `crf`, the scale-averaged scores are refined by it on the device before the argmax, in both finishes,
+        and the scores returned are its marginals (float64 [h, w, classes])."""
         h, w = image.shape[:2]
         total = np.zeros((h, w, self.classes), dtype=np.float64) if exact else \
             torch.zeros((self.classes, h, w), dtype=torch.float64, device=self.device)
@@ -196,6 +205,12 @@ class SlidingWindowPredictor:
             else:
                 total += self.scale_on_device(resized, h, w)
         total /= len(scales)
+        if self.crf is not None:
+            # the CRF works on class-contiguous fp32 scores on the device; exact=True sends its host total there once
+            scores = torch.from_numpy(total).to(self.device) if exact else total.permute(1, 2, 0)
+            q = self.crf.refine_hwc(image, scores.float().contiguous())
+            amax = q.argmax(2).cpu().numpy()
+            return (q.double().cpu().numpy() if exact or return_scores else None), amax
         if exact:
             return total, np.argmax(total, axis=2)
         amax = total.argmax(0).cpu().numpy()

@@ -1407,6 +1407,76 @@ def segsort_u32_pairs(keys, vals, skip=None):
     return keys, vals
 
 
+def densecrf_build(image, pos_xy_std, bi_xy_std, bi_rgb_std):
+    """Both permutohedral lattices (smoothness, appearance) of one fp32 HWC [H, W, 3] CUDA image in 0..255 ->
+    (lattice uint8 buffer, (V_s, V_a)); the vertex counts are the one host read of the build."""
+    _require_cuda(image)
+    assert image.dtype == torch.float32 and image.dim() == 3 and image.shape[2] == 3
+    lib = _lib.load()
+    h, w = int(image.shape[0]), int(image.shape[1])
+    nb = int(lib.semseg_densecrf_lattice_bytes(h, w))
+    _lib.check(0 if nb >= 0 else nb, "semseg_densecrf_lattice_bytes")
+    img = image.contiguous()
+    lattice = torch.empty((nb,), dtype=torch.uint8, device=image.device)
+    _lib.check(lib.semseg_densecrf_build(_ptr(img), h, w, float(pos_xy_std), float(bi_xy_std), float(bi_rgb_std),
+                                         _ptr(lattice), _stream()),
+               "semseg_densecrf_build")
+    vs, va = (int(v) for v in lattice[:8].view(torch.int32).cpu())
+    return lattice, (vs, va)
+
+
+def _densecrf_values(h, w, V, C, device):
+    lib = _lib.load()
+    nf = int(lib.semseg_densecrf_values_floats(h, w, V[0], V[1], C))
+    _lib.check(0 if nf >= 0 else nf, "semseg_densecrf_values_floats")
+    return torch.empty((nf,), dtype=torch.float32, device=device)
+
+
+def densecrf_meanfield(lattice, hw, V, prob, clip, iterations, pos_weight, bi_weight):
+    """Mean-field marginals fp32 [H*W, C] of the class-contiguous fp32 probabilities `prob` [H*W, C] on the lattices of
+    densecrf_build (include/semseg_b200.h states the contract)."""
+    _require_cuda(lattice, prob)
+    assert prob.dtype == torch.float32 and prob.dim() == 2 and prob.is_contiguous()
+    h, w = hw
+    C = int(prob.shape[1])
+    lib = _lib.load()
+    values = _densecrf_values(h, w, V, C, prob.device)
+    Q = torch.empty_like(prob)
+    _lib.check(lib.semseg_densecrf_meanfield(_ptr(lattice), h, w, V[0], V[1], _ptr(prob), C, float(clip),
+                                             int(iterations), float(pos_weight), float(bi_weight), _ptr(values), _ptr(Q),
+                                             _stream()),
+               "semseg_densecrf_meanfield")
+    return Q
+
+
+def densecrf_filter(lattice, hw, V, kernel, values_in):
+    """The normalised filter K~ of kernel 0 (smoothness) or 1 (appearance) applied to fp32 [H*W, C] values."""
+    _require_cuda(lattice, values_in)
+    assert values_in.dtype == torch.float32 and values_in.dim() == 2 and values_in.is_contiguous()
+    h, w = hw
+    C = int(values_in.shape[1])
+    lib = _lib.load()
+    values = _densecrf_values(h, w, V, C, values_in.device)
+    out = torch.empty_like(values_in)
+    _lib.check(lib.semseg_densecrf_filter(_ptr(lattice), h, w, V[0], V[1], int(kernel), _ptr(values_in), C,
+                                          _ptr(values), _ptr(out), _stream()),
+               "semseg_densecrf_filter")
+    return out
+
+
+def densecrf_keys(lattice, hw, V, kernel, pos_xy_std, bi_xy_std, bi_rgb_std):
+    """The unpacked vertex keys int32 [V, d] (in key order) of kernel 0 (d = 2) or 1 (d = 5) of a densecrf_build."""
+    _require_cuda(lattice)
+    h, w = hw
+    d = 2 if kernel == 0 else 5
+    lib = _lib.load()
+    out = torch.empty((V[int(kernel)], d), dtype=torch.int32, device=lattice.device)
+    _lib.check(lib.semseg_densecrf_keys(_ptr(lattice), h, w, V[0], V[1], int(kernel), float(pos_xy_std),
+                                        float(bi_xy_std), float(bi_rgb_std), _ptr(out), _stream()),
+               "semseg_densecrf_keys")
+    return out
+
+
 def upsample_ce_rmi_fwd(logits, target, ignore_index, bce_weight, pos_alpha, ce_weight, want_argmax=True, zoom=8,
                         workspace=None):
     """RMI loss (+ bce_weight * BCE + ce_weight * CE) on the fused tail (include/semseg_b200.h states the contract);
