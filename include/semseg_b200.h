@@ -36,6 +36,8 @@
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
  *                               (tool/test.py:163-176) and the per-scale resize into the running total
  *                               (tool/test.py:177, 202).
+ *   - semseg_anomaly_*        : anomaly segmentation on the evaluation scores (max-logit, energy, standardized
+ *                               max-logit) and its AUROC / AP / FPR95, with semseg_window_scores_stats.
  *   - semseg_densecrf_*       : dense CRF refinement of the evaluation scores (pydensecrf's DenseCRF2D with a Gaussian
  *                               and a bilateral Potts kernel), on a device permutohedral lattice.
  *   - semseg_augment          : tool/train.py:194-212's transform chains (util/transform.py), one launch per batch.
@@ -865,6 +867,48 @@ int semseg_window_accumulate(const float* scores, int C, int crop_h, int crop_w,
                              int nx, int full_h, int full_w, int top, int left, int img_h, int img_w, double* canvas,
                              void* stream);
 int semseg_window_resize_add(const double* canvas, int C, int Hi, int Wi, double* total, int Ho, int Wo, void* stream);
+/* window_scores_stats: window_scores with the same arguments, writing out fp32 [G, C + 2, crop_h, crop_w]: channels
+ * 0..C-1 bit-identical to window_scores', then ML = max_c v and LSE = max + log(sum_c exp(v - max)) of the same
+ * upsampled logits v, each flip-averaged as (a + a_mirror) * 0.5 when flip. window_accumulate and window_resize_add
+ * take the C + 2 channels unchanged. */
+int semseg_window_scores_stats(const float* logits, int pitch, int G, int h, int w, int C, int flip, float* out,
+                               int crop_h, int crop_w, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Anomaly segmentation (semseg_b200/anomaly.py; csrc/anomaly.cu). No host synchronisation, no float atomics:
+ * deterministic. Bad arguments (null pointers, sizes, options) are rejected before any CUDA call; the workspace
+ * queries return -1 for bad sizes.
+ *   class_moments : pred int64 [P] (the argmax), ml fp64 [P] (the ML plane) -> moments fp64 [3][C] += (sum ML,
+ *                   sum ML^2, pixel count) per class c = pred; predictions outside [0, C) are not counted.
+ *                   workspace: class_moments_workspace_bytes(P, C) = 24 C ceil(P / 2048) bytes. 1 <= C <= 4096.
+ *   sml           : standardized max-logit of one H x W image: S = (ml - mean[pred]) / std[pred] (mean, std: fp64 [C]
+ *                   on the device; a prediction outside [0, C) gives NaN), then boundary_iterations Jacobi suppression
+ *                   steps i at width r_i = boundary_width - i floor(boundary_width / boundary_iterations): a pixel whose
+ *                   (2 r_i + 1)^2 window, clipped to the image, holds another prediction takes the mean of S over the
+ *                   non-boundary pixels of its clipped 3x3 neighbourhood (kept if there are none); then
+ *                   T = sum g S(p + d (a, b)) / sum g over the taps inside the image, a, b in [-k/2, k/2],
+ *                   g = exp(-(a^2 + b^2) / 2 sigma^2), d = smooth_dilation; out fp32 [H, W] = -T. fp64 throughout.
+ *                   1 <= smooth_kernel <= 63 odd, sigma finite > 0, dilation >= 1, boundary_width >= 1 when
+ *                   boundary_iterations > 0. workspace: sml_workspace_bytes(H, W) = 40 H W bytes.
+ *   metrics       : score fp32 [n], label [n] (uint8 when label_bytes = 1, int64 when 8; 1 = anomaly, 0 = inlier,
+ *                   ignore_index = void) -> out fp64 [3] = (AUROC, AP, FPR95), info int64 [3] = (positives, negatives,
+ *                   error bits: 1 = a label other than 0, 1, ignore_index; 2 = a non-finite score on a non-void pixel).
+ *                   Non-void pixels sorted by score descending, equal scores (-0.0 = +0.0) one group g with cumulative
+ *                   TP_g, FP_g: AUROC = sum_g (FP_g - FP_g-1)(TP_g-1 + TP_g) / 2PN (Mann-Whitney, ties 1/2),
+ *                   AP = sum_g (TP_g - TP_g-1) / P * TP_g / (TP_g + FP_g), FPR95 = FP_g / N at the first g with
+ *                   TP_g >= 0.95 P. NaN without positives or without negatives. 0 < n < 2^31.
+ *                   workspace: metrics_workspace_bytes(n), about 16 n bytes.
+ */
+long long semseg_anomaly_class_moments_workspace_bytes(long long P, int C);
+int semseg_anomaly_class_moments(const long long* pred, const double* ml, long long P, int C, void* workspace,
+                                 double* moments, void* stream);
+long long semseg_anomaly_sml_workspace_bytes(int H, int W);
+int semseg_anomaly_sml(const double* ml, const long long* pred, int H, int W, int C, const double* mean,
+                       const double* std, int boundary_width, int boundary_iterations, int smooth_kernel,
+                       double smooth_sigma, int smooth_dilation, void* workspace, float* out, void* stream);
+long long semseg_anomaly_metrics_workspace_bytes(long long n);
+int semseg_anomaly_metrics(const float* score, const void* label, int label_bytes, long long n,
+                           long long ignore_index, void* workspace, double* out, long long* info, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Dense CRF refinement of one image (Krähenbühl & Koltun 2011; semseg_b200/densecrf.py DenseCRF; csrc/densecrf.cu):

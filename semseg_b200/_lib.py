@@ -282,6 +282,14 @@ SIGNATURES = {
     "semseg_window_accumulate": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_vp, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_window_resize_add": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    "semseg_window_scores_stats": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    "semseg_anomaly_class_moments_workspace_bytes": (c_ll, [c_ll, c_int]),
+    "semseg_anomaly_class_moments": (c_int, [c_vp, c_vp, c_ll, c_int, c_vp, c_vp, c_vp]),
+    "semseg_anomaly_sml_workspace_bytes": (c_ll, [c_int, c_int]),
+    "semseg_anomaly_sml": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int, c_int, c_int, c_d, c_int, c_vp,
+                                   c_vp, c_vp]),
+    "semseg_anomaly_metrics_workspace_bytes": (c_ll, [c_ll]),
+    "semseg_anomaly_metrics": (c_int, [c_vp, c_vp, c_int, c_ll, c_ll, c_vp, c_vp, c_vp, c_vp]),
     "semseg_densecrf_lattice_bytes": (c_ll, [c_int, c_int]),
     "semseg_densecrf_build": (c_int, [c_vp, c_int, c_int, c_d, c_d, c_d, c_vp, c_vp]),
     "semseg_densecrf_values_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),

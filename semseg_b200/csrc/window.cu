@@ -15,6 +15,12 @@
 // because the xZ grid nests in the x8 grid (align_corners), the xZ result is bilinear on each of its cells, and bilinear
 // interpolation of a bilinear function is exact. The two differ only by fp32 rounding.
 //
+// semseg_window_scores_stats: the same kernel (template flag kStats) writing C + 2 channels per crop: the C scores with
+// unchanged arithmetic, then ML = max_c v and LSE = max + log(sum exp(v - max)) of the same upsampled logits, from the
+// max and the sum of passes 1 and 2 (the log is taken before the sum is replaced by its reciprocal), flip-averaged as
+// (a + a_mirror) * 0.5. The anomaly scores of semseg_b200/anomaly.py are defined on them; the accumulation and the
+// resize below are class-count agnostic and carry the two extra channels unchanged.
+//
 // semseg_window_accumulate: a gather. Every pixel of the un-padded canvas sums in fp64 the scores of the crops that
 // cover it in grid (row-major) order, starting from 0.0, and divides by their count: the same fp64 operations in the
 // same order as `canvas[:, win] += scores[k]` over the grid followed by `canvas /= hits`, so the result is bit-identical.
@@ -42,7 +48,8 @@ __device__ __forceinline__ float lerp_aten(float l0, float a, float l1, float b)
 // and an IEEE division per score would cost a slow-path call and register spills). (exp2 of v*log2e - max*log2e, as the training tail does, would cost
 // an error proportional to |max| instead of |v - max|: ~1e-4 in the scores of a network with logits in the thousands.)
 // Shared memory: [image (original, mirror)][node row (i0, i1)][kScoreNodes][Cs], Cs odd (distinct banks per node).
-template <bool kFlip>
+// kStats: `out` holds C + 2 channels per crop, the last two ML and LSE (see the file comment).
+template <bool kFlip, bool kStats>
 __global__ void __launch_bounds__(kScoreCols)
 window_scores_kernel(const float* __restrict__ logits, int pitch, int G, int h, int w, int C, int Cs, int Ho, int Wo,
                      float* __restrict__ out) {
@@ -115,13 +122,29 @@ window_scores_kernel(const float* __restrict__ logits, int pitch, int G, int h, 
       }
     }
   }
+  const size_t plane = static_cast<size_t>(Ho) * Wo;
+  const int Co = kStats ? C + 2 : C;   // channels per crop in `out`
+  float* o = out + static_cast<size_t>(g) * Co * plane + static_cast<size_t>(8 * i0) * Wo + x;
+  if constexpr (kStats) {
+    float* oml = o + static_cast<size_t>(C) * plane;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      float ml = mx[0][r], lse = mx[0][r] + logf(sum[0][r]);
+      if (kFlip) {
+        ml = (ml + mx[1][r]) * 0.5f;
+        lse = (lse + (mx[1][r] + logf(sum[1][r]))) * 0.5f;
+      }
+      if (r < rows) {
+        oml[static_cast<size_t>(r) * Wo] = ml;
+        oml[plane + static_cast<size_t>(r) * Wo] = lse;
+      }
+    }
+  }
 #pragma unroll
   for (int im = 0; im < kImages; ++im)
 #pragma unroll
     for (int r = 0; r < 8; ++r) sum[im][r] = __fdividef(1.f, sum[im][r]);   // sum in [1, C]: now its reciprocal
   // pass 3: scores
-  const size_t plane = static_cast<size_t>(Ho) * Wo;
-  float* o = out + static_cast<size_t>(g) * C * plane + static_cast<size_t>(8 * i0) * Wo + x;
 #pragma unroll 2
   for (int c = 0; c < C; ++c) {
     float p[8];
@@ -220,25 +243,39 @@ window_resize_add_kernel(const double* __restrict__ canvas, int C, int Hi, int W
 
 using namespace sb;
 
-extern "C" int semseg_window_scores(const float* logits, int pitch, int G, int h, int w, int C, int flip, float* out,
-                                    int crop_h, int crop_w, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  SB_CHECK_ARG(logits && out, "window_scores: null pointer");
+template <bool kStats>
+static int window_scores(const char* fn, const float* logits, int pitch, int G, int h, int w, int C, int flip,
+                         float* out, int crop_h, int crop_w, cudaStream_t stream) {
+  SB_CHECK_ARG(logits && out, "%s: null pointer", fn);
   SB_CHECK_ARG(G > 0 && h > 1 && w > 1 && h <= 65535 && G <= 65535 && C > 0 && C <= kWinMaxClasses && pitch >= C &&
                    (flip == 0 || flip == 1),
-               "window_scores: bad sizes (G=%d h=%d w=%d C=%d pitch=%d flip=%d; C<=%d, pitch>=C)", G, h, w, C, pitch,
-               flip, kWinMaxClasses);
+               "%s: bad sizes (G=%d h=%d w=%d C=%d pitch=%d flip=%d; C<=%d, pitch>=C)", fn, G, h, w, C, pitch, flip,
+               kWinMaxClasses);
   SB_CHECK_ARG(crop_h == 8 * (h - 1) + 1 && crop_w == 8 * (w - 1) + 1,
-               "window_scores: crop must be 8(h-1)+1 x 8(w-1)+1 of the %dx%d logits (got %dx%d)", h, w, crop_h, crop_w);
+               "%s: crop must be 8(h-1)+1 x 8(w-1)+1 of the %dx%d logits (got %dx%d)", fn, h, w, crop_h, crop_w);
   const int Cs = C | 1;
   const size_t smem = static_cast<size_t>(flip ? 2 : 1) * 2 * kScoreNodes * Cs * sizeof(float);  // <= 41 KB
   dim3 grid(cdiv(crop_w, kScoreCols), h, G);
   if (flip)
-    window_scores_kernel<true><<<grid, kScoreCols, smem, stream>>>(logits, pitch, G, h, w, C, Cs, crop_h, crop_w, out);
+    window_scores_kernel<true, kStats><<<grid, kScoreCols, smem, stream>>>(logits, pitch, G, h, w, C, Cs, crop_h,
+                                                                           crop_w, out);
   else
-    window_scores_kernel<false><<<grid, kScoreCols, smem, stream>>>(logits, pitch, G, h, w, C, Cs, crop_h, crop_w, out);
+    window_scores_kernel<false, kStats><<<grid, kScoreCols, smem, stream>>>(logits, pitch, G, h, w, C, Cs, crop_h,
+                                                                            crop_w, out);
   SB_LAUNCHED();
   return SEMSEG_OK;
+}
+
+extern "C" int semseg_window_scores(const float* logits, int pitch, int G, int h, int w, int C, int flip, float* out,
+                                    int crop_h, int crop_w, void* stream) {
+  return window_scores<false>("window_scores", logits, pitch, G, h, w, C, flip, out, crop_h, crop_w,
+                              static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int semseg_window_scores_stats(const float* logits, int pitch, int G, int h, int w, int C, int flip,
+                                          float* out, int crop_h, int crop_w, void* stream) {
+  return window_scores<true>("window_scores_stats", logits, pitch, G, h, w, C, flip, out, crop_h, crop_w,
+                             static_cast<cudaStream_t>(stream));
 }
 
 // Origins must start at 0, ascend strictly, end at extent - crop and leave no gap (every pixel covered).

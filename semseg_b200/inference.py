@@ -23,6 +23,10 @@ accumulation / normalisation by the overlap count stay on the device. Two ways t
     to the crop. The native kernel upsamples the 1/8-resolution logits x8 straight to the crop instead. The two are
     equal up to fp32 rounding: the xZ grid nests in the x8 grid (align_corners), the xZ result is bilinear on every
     cell of its grid, and bilinear interpolation reproduces a bilinear function exactly.
+With an `anomaly` scorer (anomaly.AnomalyScorer) the exact=False finishes carry two more channels through the same
+steps: the flip-averaged max logit (ML) and logsumexp (LSE) of each crop's upsampled logits (csrc/window.cu's
+stats variant of the scores kernel, or torch amax / logsumexp in the ATen finish). The C score channels and the argmax
+are the same bits as without a scorer; the scorer turns ML, LSE or the scores into a per-pixel anomaly map.
 `net_process` / `scale_process` keep the reference's signatures and return types (and the exact arithmetic);
 `SlidingWindowPredictor` is the object form that also covers the per-image scale loop.
 
@@ -80,13 +84,21 @@ class SlidingWindowPredictor:
     """model: eval-mode network mapping [B, 3, crop_h, crop_w] -> [B, classes, h', w'] logits."""
 
     def __init__(self, model, classes, crop_h, crop_w, mean, std=None, stride_rate=2 / 3, flip=True, max_batch=32,
-                 crf=None):
+                 crf=None, anomaly=None):
         """crf: None, or a densecrf.DenseCRF run on the scale-averaged scores before the argmax (both finishes); the
-        returned scores are then its marginals."""
+        returned scores are then its marginals.
+        anomaly: None, or an anomaly.AnomalyScorer; __call__ then also returns its fp32 [h, w] CUDA anomaly map
+        (exact=False only; not together with crf)."""
+        from .anomaly import AnomalyScorer
         from .densecrf import DenseCRF
         if crf is not None and not isinstance(crf, DenseCRF):
             raise TypeError("SlidingWindowPredictor: crf must be None or a DenseCRF, got %s" % type(crf).__name__)
-        self.crf = crf
+        if anomaly is not None and not isinstance(anomaly, AnomalyScorer):
+            raise TypeError("SlidingWindowPredictor: anomaly must be None or an AnomalyScorer, got %s"
+                            % type(anomaly).__name__)
+        if crf is not None and anomaly is not None:
+            raise ValueError("SlidingWindowPredictor: crf and anomaly cannot be combined")
+        self.crf, self.anomaly = crf, anomaly
         self.model, self.classes = model, int(classes)
         self.crop_h, self.crop_w = int(crop_h), int(crop_w)
         self.mean = [float(m) for m in mean]
@@ -107,20 +119,21 @@ class SlidingWindowPredictor:
             t = t / torch.tensor(self.std, dtype=torch.float32, device=self.device).view(3, 1, 1)
         return t.contiguous()
 
-    def _scores(self, crops, net=None):
+    def _scores(self, crops, net=None, stats=False):
         """[G, 3, ch, cw] normalised crops -> [G, classes, ch, cw] flip-averaged softmax scores (fp32). With `net` (see
         _native_net) the scores kernel writes each batch's scores straight into the result from the 1/8-resolution
-        logits."""
+        logits. With `stats` two more channels follow the scores: the flip-averaged max and logsumexp over the classes
+        of the upsampled logits."""
         per_call = self.max_batch // 2 if self.flip else self.max_batch
         if net is not None:
-            out = torch.empty((crops.shape[0], self.classes) + tuple(crops.shape[2:]), dtype=torch.float32,
-                              device=crops.device)
+            out = torch.empty((crops.shape[0], self.classes + (2 if stats else 0)) + tuple(crops.shape[2:]),
+                              dtype=torch.float32, device=crops.device)
             with torch.no_grad():
                 for g0 in range(0, crops.shape[0], per_call):
                     part = crops[g0:g0 + per_call]
                     logits = net._eval_logits_nhwc(torch.cat([part, part.flip(3)], 0) if self.flip else part)
                     self.forward_calls += 1
-                    ops.window_scores(logits, self.flip, out[g0:g0 + part.shape[0]])
+                    ops.window_scores(logits, self.flip, out[g0:g0 + part.shape[0]], stats)
             return out
         outs = []
         with torch.no_grad():
@@ -132,14 +145,21 @@ class SlidingWindowPredictor:
                 if logits.shape[2:] != batch.shape[2:]:
                     logits = F.interpolate(logits, tuple(batch.shape[2:]), mode="bilinear", align_corners=True)
                 prob = F.softmax(logits.float(), dim=1)
+                if stats:
+                    lf = logits.float()
+                    extra = torch.stack([lf.amax(1), torch.logsumexp(lf, 1)], 1)
                 if self.flip:
                     n = part.shape[0]
                     prob = (prob[:n] + prob[n:].flip(3)) / 2
+                    if stats:
+                        extra = (extra[:n] + extra[n:].flip(3)) * 0.5
+                if stats:
+                    prob = torch.cat([prob, extra], 1)
                 outs.append(prob)
         return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
 
     # ------------------------------------------------------------------------------------------- one scale
-    def _scale_canvas(self, image, net=None):
+    def _scale_canvas(self, image, net=None, stats=False):
         """Overlap-normalised scores of one rescaled image, un-padded: float64 [classes, img_h, img_w] on the device
         (tool/test.py:148-176: padding, crop grid, accumulation in grid order, division by the crop count). With `net`
         the scores and the accumulation run on the native kernels (contiguous result, same bits as the loop)."""
@@ -155,10 +175,10 @@ class SlidingWindowPredictor:
         windows = [(y0, x0) for y0 in ys for x0 in xs]
         x = self._normalised(image)
         crops = torch.stack([x[:, y0:y0 + ch, x0:x0 + cw] for y0, x0 in windows], 0)
-        scores = self._scores(crops, net)
+        scores = self._scores(crops, net, stats)
         if net is not None:
             return ops.window_accumulate(scores, ys, xs, (full_h, full_w), top, left, (img_h, img_w))
-        canvas = torch.zeros((self.classes, full_h, full_w), dtype=torch.float64, device=self.device)
+        canvas = torch.zeros((scores.shape[1], full_h, full_w), dtype=torch.float64, device=self.device)
         hits = np.zeros((full_h, full_w), dtype=np.float64)
         for k, (y0, x0) in enumerate(windows):          # grid order = the reference's accumulation order
             canvas[:, y0:y0 + ch, x0:x0 + cw] += scores[k]
@@ -173,14 +193,30 @@ class SlidingWindowPredictor:
         host = self._scale_canvas(image).permute(1, 2, 0).contiguous().cpu().numpy()
         return cv2.resize(host, (out_w, out_h), interpolation=cv2.INTER_LINEAR)
 
-    def scale_on_device(self, image, out_h, out_w):
+    def scale_on_device(self, image, out_h, out_w, stats=False):
         """Same scores as `scale`, float64 [classes, out_h, out_w], resized on the device (bilinear, half-pixel centres,
         no anti-aliasing = cv2.INTER_LINEAR's sampling; cv2 rounds its interpolation weights to fp32, so the two agree
         to ~1e-7, not bit for bit)."""
-        canvas = self._scale_canvas(image)
+        canvas = self._scale_canvas(image, stats=stats)
         return F.interpolate(canvas[None], size=(out_h, out_w), mode="bilinear", align_corners=False)[0]
 
     # ------------------------------------------------------------------------------------------- one image
+    def _stats_total(self, image, base_size, scales):
+        """The exact=False finish with the two statistics channels: (total fp64 [classes + 2, h, w] on the device, the
+        scale average of the scores, ML and LSE; argmax int64 [h, w] of its score channels)."""
+        h, w = image.shape[:2]
+        total = torch.zeros((self.classes + 2, h, w), dtype=torch.float64, device=self.device)
+        net = _native_net(self.model, self.classes, self.crop_h, self.crop_w, self.device)
+        for s in scales:
+            new_h, new_w = scaled_size(h, w, round(s * base_size))
+            resized = cv2.resize(image, (new_w, new_h), interpolation=cv2.INTER_LINEAR)
+            if net is not None:
+                ops.window_resize_add(self._scale_canvas(resized, net, stats=True), total)
+            else:
+                total += self.scale_on_device(resized, h, w, stats=True)
+        total /= len(scales)
+        return total, total[:self.classes].argmax(0)
+
     def __call__(self, image, base_size, scales, exact=False, return_scores=True):
         """(scores float64 [h, w, classes] or None, argmax int64 [h, w]) of a float32 HWC image: the body of the
         evaluation loop, tool/test.py:186-199.
@@ -190,7 +226,16 @@ class SlidingWindowPredictor:
         exact=False : score maps are resized, summed over the scales and arg-maxed on the device; only the result
                       crosses PCIe (the argmax, plus the scores when return_scores).
         With a `crf`, the scale-averaged scores are refined by it on the device before the argmax, in both finishes,
-        and the scores returned are its marginals (float64 [h, w, classes])."""
+        and the scores returned are its marginals (float64 [h, w, classes]).
+        With an `anomaly` scorer the result is (scores, argmax, anomaly map fp32 [h, w] on the device); scores and
+        argmax are the same bits as without it. exact=True raises ValueError then."""
+        if self.anomaly is not None:
+            if exact:
+                raise ValueError("SlidingWindowPredictor: exact=True does not support an anomaly scorer")
+            total, pred = self._stats_total(image, base_size, scales)
+            amap = self.anomaly.score_map(total, pred)
+            scores = total[:self.classes].permute(1, 2, 0).contiguous().cpu().numpy() if return_scores else None
+            return scores, pred.cpu().numpy(), amap
         h, w = image.shape[:2]
         total = np.zeros((h, w, self.classes), dtype=np.float64) if exact else \
             torch.zeros((self.classes, h, w), dtype=torch.float64, device=self.device)

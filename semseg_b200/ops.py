@@ -1528,9 +1528,11 @@ def upsample_ce_rmi_bwd(logits, target, ignore_index, lse, pooled, table, grad_o
 
 
 # ------------------------------------------------------------------------------------------------ sliding-window evaluation
-def window_scores(logits, flip, out):
+def window_scores(logits, flip, out, stats=False):
     """fp32 NHWC logits [G (+G mirrored crops when flip), h, w, C] -> flip-averaged softmax scores written into `out`,
-    a contiguous fp32 [G, C, 8(h-1)+1, 8(w-1)+1] tensor (typically a slice of a scale's score buffer)."""
+    a contiguous fp32 [G, C, 8(h-1)+1, 8(w-1)+1] tensor (typically a slice of a scale's score buffer). With `stats`
+    (semseg_window_scores_stats) `out` has C + 2 channels: the same scores, then the flip-averaged max logit and
+    logsumexp of the upsampled logits."""
     _require_cuda(logits, out)
     lib = _lib.load()
     assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(3) == 1
@@ -1539,9 +1541,12 @@ def window_scores(logits, flip, out):
     assert logits.stride(1) == w * pitch and logits.stride(0) == h * logits.stride(1), "logits must be pixel-contiguous"
     g = n // 2 if flip else n
     assert not flip or n % 2 == 0, "flip needs the crops followed by their mirrors"
-    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and tuple(out.shape[:2]) == (g, c)
-    _lib.check(lib.semseg_window_scores(_ptr(logits), pitch, g, h, w, c, int(bool(flip)), _ptr(out), out.shape[2],
-                                        out.shape[3], _stream()), "semseg_window_scores")
+    co = c + 2 if stats else c
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and tuple(out.shape[:2]) == (g, co)
+    fn, name = ((lib.semseg_window_scores_stats, "semseg_window_scores_stats") if stats else
+                (lib.semseg_window_scores, "semseg_window_scores"))
+    _lib.check(fn(_ptr(logits), pitch, g, h, w, c, int(bool(flip)), _ptr(out), out.shape[2], out.shape[3], _stream()),
+               name)
     return out
 
 
@@ -1578,6 +1583,64 @@ def window_resize_add(canvas, total):
     _lib.check(lib.semseg_window_resize_add(_ptr(canvas), c, hi, wi, _ptr(total), ho, wo, _stream()),
                "semseg_window_resize_add")
     return total
+
+
+# ------------------------------------------------------------------------------------------------ anomaly segmentation
+def anomaly_class_moments(pred, ml, moments):
+    """moments fp64 [3, C] += per-class (sum ML, sum ML^2, count) of the int64 prediction `pred` and the fp64 ML plane
+    `ml` (same shape); in place, deterministic."""
+    _require_cuda(pred, ml, moments)
+    assert pred.dtype == torch.int64 and ml.dtype == torch.float64 and moments.dtype == torch.float64
+    assert pred.is_contiguous() and ml.is_contiguous() and moments.is_contiguous() and pred.shape == ml.shape
+    assert moments.dim() == 2 and moments.shape[0] == 3
+    lib = _lib.load()
+    p, c = pred.numel(), int(moments.shape[1])
+    nb = int(lib.semseg_anomaly_class_moments_workspace_bytes(p, c))
+    _lib.check(0 if nb >= 0 else nb, "semseg_anomaly_class_moments_workspace_bytes")
+    ws = torch.empty((nb,), dtype=torch.uint8, device=pred.device)
+    _lib.check(lib.semseg_anomaly_class_moments(_ptr(pred), _ptr(ml), p, c, _ptr(ws), _ptr(moments), _stream()),
+               "semseg_anomaly_class_moments")
+    return moments
+
+
+def anomaly_sml(ml, pred, mean, std, boundary_width, boundary_iterations, smooth_kernel, smooth_sigma,
+                smooth_dilation):
+    """Standardized max-logit map fp32 [H, W] (higher = more anomalous) of the fp64 ML plane and the int64 prediction
+    [H, W], with the per-class fp64 `mean` / `std` [C] on the device (include/semseg_b200.h states the contract)."""
+    _require_cuda(ml, pred, mean, std)
+    assert ml.dtype == torch.float64 and pred.dtype == torch.int64 and ml.dim() == 2 and ml.shape == pred.shape
+    assert mean.dtype == std.dtype == torch.float64 and mean.dim() == 1 and mean.shape == std.shape
+    ml, pred, mean, std = ml.contiguous(), pred.contiguous(), mean.contiguous(), std.contiguous()
+    lib = _lib.load()
+    h, w = (int(v) for v in ml.shape)
+    nb = int(lib.semseg_anomaly_sml_workspace_bytes(h, w))
+    _lib.check(0 if nb >= 0 else nb, "semseg_anomaly_sml_workspace_bytes")
+    ws = torch.empty((nb,), dtype=torch.uint8, device=ml.device)
+    out = torch.empty((h, w), dtype=torch.float32, device=ml.device)
+    _lib.check(lib.semseg_anomaly_sml(_ptr(ml), _ptr(pred), h, w, int(mean.numel()), _ptr(mean), _ptr(std),
+                                      int(boundary_width), int(boundary_iterations), int(smooth_kernel),
+                                      float(smooth_sigma), int(smooth_dilation), _ptr(ws), _ptr(out), _stream()),
+               "semseg_anomaly_sml")
+    return out
+
+
+def anomaly_metrics(score, label, ignore_index):
+    """(out fp64 [3] = (AUROC, AP, FPR95), info int64 [3] = (positives, negatives, error bits)) on the device, of the
+    fp32 scores and the uint8 / int64 labels (1-D, same length) -> include/semseg_b200.h semseg_anomaly_metrics."""
+    _require_cuda(score, label)
+    assert score.dtype == torch.float32 and score.dim() == 1 and score.is_contiguous()
+    assert label.dtype in (torch.uint8, torch.int64) and label.shape == score.shape and label.is_contiguous()
+    lib = _lib.load()
+    n = score.numel()
+    nb = int(lib.semseg_anomaly_metrics_workspace_bytes(n))
+    _lib.check(0 if nb >= 0 else nb, "semseg_anomaly_metrics_workspace_bytes")
+    ws = torch.empty((nb,), dtype=torch.uint8, device=score.device)
+    out = torch.empty((3,), dtype=torch.float64, device=score.device)
+    info = torch.empty((3,), dtype=torch.int64, device=score.device)
+    _lib.check(lib.semseg_anomaly_metrics(_ptr(score), _ptr(label), label.element_size(), n, int(ignore_index),
+                                          _ptr(ws), _ptr(out), _ptr(info), _stream()),
+               "semseg_anomaly_metrics")
+    return out, info
 
 
 # ------------------------------------------------------------------------------------------------ pyramid pooling
