@@ -171,6 +171,17 @@ typedef struct semseg_conv_desc {
    * semseg_conv_splitk_finish). */
   int32_t k_slices;
   int64_t slice_stride;
+  /* e4m3 operand mode (eval convs of semseg_b200/fp8.py; e4m3 = 1, or 2 for the unpromoted accumulation that
+   * tools/probe_accum.py measures against it): x is e4m3 NHWC [Nin,Hin,Win,x_pitch] bytes and w an
+   * e4m3 slab [n_wtaps][w_rows][w_cols] (semseg_fp8_pack_weights); a K block is 128 channels and (e4m3 = 1) the
+   * tensor-core partial of every K block is added into the fp32 accumulator (promotion). AFFINE epilogue only, which writes y (bf16, may be
+   * NULL) and / or y8: e4m3 NHWC [N,H,W,y8_pitch] bytes of sat_e4m3(v * y8_qscale), v the bf16 epilogue's fp32 value.
+   * Dequantisation (s_x * s_w[c]) is folded into scale[c] by the caller. Requires Cin % 128 == 0, Cout % 64 == 0, x_pitch,
+   * w_cols, y8_pitch multiples of 16 (bytes), and no split operands, K slicing or statistics. */
+  int32_t e4m3;
+  void* y8;
+  int32_t y8_pitch;
+  float y8_qscale;
 } semseg_conv_desc;
 
 /* Number of K slices such that one slice holds at most max_kblocks K blocks (64-channel block x tap). */
@@ -233,6 +244,23 @@ typedef struct semseg_pack_item {
   int split; /* != 0: lo slabs follow the hi slabs (wf + taps*Cout*cols_f, wd + taps*Cin*cols_d, wp + Cout*32) */
 } semseg_pack_item;
 int semseg_pack_weights_multi(const semseg_pack_item* items_dev, int n_items, int n_tiles, int max_taps, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * FP8 (e4m3) eval support (csrc/fp8.cu). One quantisation formula throughout: q = sat_e4m3(v * qscale) with
+ * qscale = 448 / amax computed in fp32, round to nearest even, saturating to +-448 (NaN stays NaN).
+ *   semseg_fp8_quantize: bf16 NHWC x [M pixels][x_pitch] -> e4m3 y [M][y_pitch], C channels, q(x * qscale).
+ *   semseg_fp8_amax    : amax_bits[0] = max(amax_bits[0], max |x| as fp32 bits) over a bf16 NHWC tensor; |x| bit
+ *                        patterns order as integers, so the running maximum over calls is exact and order-free.
+ *                        NaN inputs are ignored.
+ *   semseg_fp8_pack_weights: fp32 OIHW w [Cout][Cin][taps] -> e4m3 slab wf [taps][Cout][Cin] = q(w) with the
+ *                        per-output-channel qscale = 448 / amax_c, and the dequantisation scale scale_w[c] = amax_c / 448
+ *                        (amax_c = max |w| of output channel c; an all-zero channel uses amax_c = 448).
+ *                        Cin % 16 == 0; one launch per conv, at freeze time.
+ * Pitches are in elements; C % 16 == 0, pitches multiples of 16. */
+int semseg_fp8_quantize(const void* x, int x_pitch, void* y, int y_pitch, long long M, int C, float qscale,
+                        void* stream);
+int semseg_fp8_amax(const void* x, int x_pitch, long long M, int C, unsigned int* amax_bits, void* stream);
+int semseg_fp8_pack_weights(const float* w, int Cout, int Cin, int taps, void* wf, float* scale_w, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Layout conversion at the module boundary.

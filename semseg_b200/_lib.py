@@ -74,6 +74,7 @@ class ConvDesc(ctypes.Structure):
         ("x_lo", c_vp), ("y_lo", c_vp), ("residual_lo", c_vp),
         ("w_split", c_i32),
         ("k_slices", c_i32), ("slice_stride", ctypes.c_int64),
+        ("e4m3", c_i32), ("y8", c_vp), ("y8_pitch", c_i32), ("y8_qscale", c_f),
     ]
 
 
@@ -129,6 +130,9 @@ SIGNATURES = {
     "semseg_conv_wgrad": (c_int, [ctypes.POINTER(WgradDesc), c_vp]),
     "semseg_wgrad_reduce": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_vp, c_int, c_vp]),
     "semseg_pack_weights_multi": (c_int, [c_vp, c_int, c_int, c_int, c_vp]),
+    "semseg_fp8_quantize": (c_int, [c_vp, c_int, c_vp, c_int, c_ll, c_int, c_f, c_vp]),
+    "semseg_fp8_amax": (c_int, [c_vp, c_int, c_ll, c_int, c_vp, c_vp]),
+    "semseg_fp8_pack_weights": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_vp, c_vp]),
     "semseg_sgd_chunk_elems": (c_int, []),
     "semseg_sgd_multi": (c_int, [c_vp, c_vp, c_int, c_int, ctypes.POINTER(SgdHyper), c_vp]),
     "semseg_ema_multi": (c_int, [c_vp, c_int, c_int, ctypes.c_double, c_vp]),

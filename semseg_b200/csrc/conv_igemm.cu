@@ -61,13 +61,25 @@ struct ConvKParams {
   float* out_f32;
   int out_pitch;
   float* stats_partial;  // [gridDim.x * 4][3][Cout]: per 32 pixel rows of the tile (sum, sum of squares, count)
+  // e4m3 operand mode (kFp8): which outputs the AFFINE epilogue writes, and the factor its e4m3 output is multiplied by
+  // before the saturating round (1 / s_out, where s_out is the consumer's dequantisation scale)
+  int out_bf16, out_e4m3;
+  float y8_qscale;
 };
 
+// kFp8 (e4m3 operand mode, eval only): x and w are e4m3 bytes, a K block is 128 channels (still one 128-byte swizzle
+// span, so the stage bytes, TMA boxes and barrier ring are those of bf16) and takes four m64nNk32 e4m3 wgmmas. With
+// kPromote each stage accumulates into a fresh register tile that is then added into the fp32 master accumulator (the
+// FP8 tensor-core accumulation loses precision over long K, measured in DESIGN §4), so BLOCK_N <= 128; without it the
+// wgmmas accumulate straight into acc like bf16 (kept for that measurement). The AFFINE epilogue writes the bf16 output,
+// an e4m3 copy of it scaled by y8_qscale (staged in the second buffer with a 64-byte swizzle, TMA store through the
+// tmC_lo slot), or both.
+//
 // kSplit (bf16x3 operand mode, activations stored as hi/lo bf16 planes — act.cuh): every K block is issued three times,
 // (x_hi, w_hi), (x_lo, w_hi), (x_hi, w_lo), into the same fp32 accumulator; the producer just picks the hi or lo
 // tensor map per segment, the MMA loop is unchanged. The epilogue splits its fp32 result into (hi, lo) again and stores
 // both planes (two staging tiles, two TMA stores); BatchNorm statistics are taken from hi + lo.
-template <int BLOCK_N, bool kSplit>
+template <int BLOCK_N, bool kSplit, bool kFp8, bool kPromote>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmA_lo,
@@ -77,6 +89,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   constexpr int kStages = Cfg::kStages;
   constexpr int kStageBytes = Cfg::kStageBytes;
   constexpr int kAcc = BLOCK_N / 2;   // fp32 accumulator registers per thread
+  constexpr int kKElems = kFp8 ? 2 * kBlockK : kBlockK;   // channels per K block (128 bytes either way)
+  static_assert(!(kSplit && kFp8), "bf16x3 and e4m3 operand modes are exclusive");
   const int num_items = p.num_m_tiles * p.n_tiles * p.k_slices;
   auto decode_item = [&](int item, int& m_tile, int& n_tile, int& k_slice) {
     k_slice = item % p.k_slices;
@@ -164,10 +178,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           uint8_t* a_dst = stage_base + s * kStageBytes;
           uint8_t* b_dst = a_dst + kATileBytes;
           mbar_expect_tx(&full_bar[s], stage_tx);
-          tma_load_4d(a_dst, mA, &full_bar[s], cb * kBlockK, w0 + p.dw[t], h0 + p.dh[t],
+          tma_load_4d(a_dst, mA, &full_bar[s], cb * kKElems, w0 + p.dw[t], h0 + p.dh[t],
                       img * p.img_mul + p.img_add[t]);
           // 3-D weights [taps][rows][cols]: coordinates (k, row, tap)
-          tma_load_3d(b_dst, mB, &full_bar[s], cb * kBlockK, n0, p.wtap[t]);
+          tma_load_3d(b_dst, mB, &full_bar[s], cb * kKElems, n0, p.wtap[t]);
         }
       }
     }
@@ -183,7 +197,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     int store_buf = 0;
     float acc[kAcc];
     constexpr int kChunks = BLOCK_N / 64;
-    const bool stats = p.stats_partial != nullptr && p.epi_mode == SEMSEG_EPI_RAW;
+    const bool stats = !kFp8 && p.stats_partial != nullptr && p.epi_mode == SEMSEG_EPI_RAW;
     // running sum and sum of squares of this thread's statistics column in every chunk, and the running pixel count
     // of its 32 rows (the same for every chunk), added to the CTA's statistics row in global memory only when the
     // CTA's next item is in another channel tile (or there is none)
@@ -216,6 +230,32 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       int prev_s = -1;
 #pragma unroll
       for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+      if constexpr (kFp8 && kPromote) {
+        // promoted accumulation: each stage's four wgmmas start a fresh tile, which is added into acc in fp32 once they
+        // completed; the other warpgroup's wgmmas keep the tensor core busy meanwhile
+        float part[kAcc];
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int s = it % kStages;
+          const uint32_t par = (it / kStages) & 1;
+          mbar_wait(&full_bar[s], par);
+          const uint32_t a_addr = smem_u32(stage_base + s * kStageBytes) + static_cast<uint32_t>(wg * 64 * 128);
+          const uint32_t b_addr = smem_u32(stage_base + s * kStageBytes + kATileBytes);
+          const uint64_t adesc = make_wgmma_desc_sw128(a_addr, 16, 1024);
+          const uint64_t bdesc = make_wgmma_desc_sw128(b_addr, 16, 1024);
+          wgmma_fence_operand(part);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k)   // advance 32 bytes (32 e4m3) along K inside the 128-byte swizzle span
+            wgmma_e4m3<BLOCK_N>(part, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
+                                k > 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_operand(part);
+          mbar_arrive(&empty_bar[s]);
+#pragma unroll
+          for (int i = 0; i < kAcc; ++i) acc[i] += part[i];
+        }
+      } else {
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const int s = it % kStages;
         const uint32_t par = (it / kStages) & 1;
@@ -228,8 +268,12 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kBlockK / 16; ++k)   // advance 32 bytes (16 bf16) along K inside the 128-byte swizzle span
-          wgmma_bf16<BLOCK_N, 0, 0>(acc, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
-                                    (kb > 0 || k > 0) ? 1u : 0u);
+          if constexpr (kFp8)   // (32 e4m3 per step)
+            wgmma_e4m3<BLOCK_N>(acc, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
+                                (kb > 0 || k > 0) ? 1u : 0u);
+          else
+            wgmma_bf16<BLOCK_N, 0, 0>(acc, adesc + static_cast<uint64_t>(k * 2), bdesc + static_cast<uint64_t>(k * 2),
+                                      (kb > 0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<1>();
         wgmma_fence_operand(acc);
@@ -239,6 +283,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>();
       wgmma_fence_operand(acc);
       if (prev_s >= 0) mbar_arrive(&empty_bar[prev_s]);
+      }
 
       // ---- epilogue
       int img, h0, w0;
@@ -329,8 +374,10 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
         // registers -> bf16 -> 128B-swizzled staging tile (row = pixel, 64 channels = 128 bytes); the two staging
         // buffers are used alternately (split storage: buffer 0 = hi plane tile, buffer 1 = lo plane tile)
-        uint8_t* obuf = out_stage + (kSplit ? 0 : store_buf) * kStageOutBytes;
-        if (ct == 0) tma_store_wait_read<(kSplit ? 0 : 1)>();  // the store(s) that last read the buffer(s) drained
+        // (kFp8: buffer 0 = bf16 tile, buffer 1 = e4m3 tile [row][64 bytes] with the 64-byte swizzle: 16-byte chunk
+        // c of row r at chunk c ^ ((r >> 1) & 3), so the 8 rows of a warp's stores hit 8 distinct bank groups)
+        uint8_t* obuf = out_stage + ((kSplit || kFp8) ? 0 : store_buf) * kStageOutBytes;
+        if (ct == 0) tma_store_wait_read<((kSplit || kFp8) ? 0 : 1)>();  // the store(s) that last read the buffer(s) drained
         named_bar_sync(1, kConsumerThreads);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -338,6 +385,15 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           for (int i = 0; i < 2; ++i) {
             const int r = r_base + 8 * i;
             const float v0 = a[4 * j + 2 * i], v1 = a[4 * j + 2 * i + 1];
+            if constexpr (kFp8) {
+              if (p.out_bf16)
+                *reinterpret_cast<uint32_t*>(obuf + r * 128 + ((j ^ (r & 7)) << 4) + cq * 2) = pack_bf16x2(v0, v1);
+              if (p.out_e4m3)
+                *reinterpret_cast<uint16_t*>(obuf + kStageOutBytes + r * 64 + ((((j >> 1) ^ (r >> 1)) & 3) << 4) +
+                                             8 * (j & 1) + cq) =
+                    pack_e4m3x2(v0 * p.y8_qscale, v1 * p.y8_qscale);
+              continue;
+            }
             const uint32_t h = pack_bf16x2(v0, v1);
             const int off = r * 128 + ((j ^ (r & 7)) << 4) + cq * 2;
             *reinterpret_cast<uint32_t*>(obuf + off) = h;
@@ -350,8 +406,13 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         fence_proxy_async_smem();
         named_bar_sync(1, kConsumerThreads);
         if (ct == 0) {
-          tma_store_4d(&tmC, obuf, c0, w0, h0, img);
-          if (kSplit) tma_store_4d(&tmC_lo, obuf + kStageOutBytes, c0, w0, h0, img);
+          if constexpr (kFp8) {
+            if (p.out_bf16) tma_store_4d(&tmC, obuf, c0, w0, h0, img);
+            if (p.out_e4m3) tma_store_4d(&tmC_lo, obuf + kStageOutBytes, c0, w0, h0, img);
+          } else {
+            tma_store_4d(&tmC, obuf, c0, w0, h0, img);
+            if (kSplit) tma_store_4d(&tmC_lo, obuf + kStageOutBytes, c0, w0, h0, img);
+          }
           tma_store_commit();
         }
         if (stats) {
@@ -430,18 +491,35 @@ static int launch_conv(const ConvMaps& tm, const ConvKParams& kp, bool split, in
   int dev = 0;
   SB_CUDA(cudaGetDevice(&dev));
   if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
-    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  Cfg::kSmemBytes));
-    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  Cfg::kSmemBytes));
     if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
   }
   if (split)
-    conv_igemm_kernel<BLOCK_N, true><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(tm.a, tm.b, tm.c, tm.a_lo,
-                                                                                      tm.b_lo, tm.c_lo, kp);
+    conv_igemm_kernel<BLOCK_N, true, false, false><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(
+        tm.a, tm.b, tm.c, tm.a_lo, tm.b_lo, tm.c_lo, kp);
   else
-    conv_igemm_kernel<BLOCK_N, false><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(tm.a, tm.b, tm.c, tm.a_lo,
-                                                                                       tm.b_lo, tm.c_lo, kp);
+    conv_igemm_kernel<BLOCK_N, false, false, false><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(
+        tm.a, tm.b, tm.c, tm.a_lo, tm.b_lo, tm.c_lo, kp);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int BLOCK_N, bool kPromote>
+static int launch_conv_e4m3(const ConvMaps& tm, const ConvKParams& kp, int grid, cudaStream_t stream) {
+  using Cfg = ConvCfg<BLOCK_N>;
+  static std::atomic<bool> attr_set[64];
+  int dev = 0;
+  SB_CUDA(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64 || !attr_set[dev].load(std::memory_order_acquire)) {
+    SB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BLOCK_N, false, true, kPromote>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 Cfg::kSmemBytes));
+    if (dev >= 0 && dev < 64) attr_set[dev].store(true, std::memory_order_release);
+  }
+  conv_igemm_kernel<BLOCK_N, false, true, kPromote><<<grid, kConvThreads, Cfg::kSmemBytes, stream>>>(tm.a, tm.b, tm.c, tm.a_lo,
+                                                                                          tm.b_lo, tm.c_lo, kp);
   SB_LAUNCHED();
   return SEMSEG_OK;
 }
@@ -470,6 +548,98 @@ extern "C" int semseg_conv_stats_rows(int N, int H, int W, int Cout) {
   return 4 * sb::conv_grid(N * sb::cdiv(H, bh) * sb::cdiv(W, bw), sb::cdiv(Cout, conv_block_n(Cout)));
 }
 
+// The e4m3 operand mode (eval convs of semseg_b200/fp8.py): x and w are e4m3 bytes, the AFFINE epilogue writes y (bf16),
+// y8 (e4m3, v * y8_qscale rounded and saturated) or both. Everything the mode does not support is rejected here.
+static int conv_fprop_e4m3(const semseg_conv_desc* d, cudaStream_t stream) {
+  using namespace sb;
+  SB_CHECK_ARG(d->e4m3 == 1 || d->e4m3 == 2, "conv: e4m3 must be 0, 1 (promoted) or 2 (unpromoted), got %d", d->e4m3);
+  SB_CHECK_ARG(d->Cin % 128 == 0, "conv: e4m3 operands need Cin %% 128 == 0 (got %d)", d->Cin);
+  SB_CHECK_ARG(d->Cout % 64 == 0, "conv: e4m3 operands need Cout %% 64 == 0 (got %d)", d->Cout);
+  SB_CHECK_ARG(d->epi_mode == SEMSEG_EPI_AFFINE, "conv: e4m3 operands need the AFFINE epilogue");
+  SB_CHECK_ARG(d->x_lo == nullptr && d->y_lo == nullptr && d->residual_lo == nullptr && d->w_split == 0,
+               "conv: e4m3 operands cannot be split (bf16x3)");
+  SB_CHECK_ARG(d->k_slices <= 1, "conv: e4m3 operands cannot be K-sliced");
+  SB_CHECK_ARG(d->stats_partial == nullptr, "conv: e4m3 operands take no statistics");
+  SB_CHECK_ARG(d->y != nullptr || d->y8 != nullptr, "conv: e4m3 conv without an output (y, y8)");
+  SB_CHECK_ARG(d->x_pitch % 16 == 0 && d->x_pitch >= d->Cin,
+               "conv: e4m3 x_pitch %d must be a multiple of 16 bytes and >= Cin", d->x_pitch);
+  SB_CHECK_ARG(d->w_cols % 16 == 0 && d->w_cols >= d->Cin,
+               "conv: e4m3 w_cols %d must be a multiple of 16 bytes and >= Cin", d->w_cols);
+  SB_CHECK_ARG(d->y == nullptr || (d->y_pitch % 8 == 0 && d->y_pitch >= d->Cout), "conv: bad y_pitch %d", d->y_pitch);
+  SB_CHECK_ARG(d->y8 == nullptr || (d->y8_pitch % 16 == 0 && d->y8_pitch >= d->Cout),
+               "conv: y8_pitch %d must be a multiple of 16 bytes and >= Cout", d->y8_pitch);
+  SB_CHECK_ARG(d->y8 == nullptr || (d->y8_qscale > 0.f && d->y8_qscale < 3.0e38f),
+               "conv: y8_qscale must be finite and > 0");
+  SB_CHECK_ARG(d->residual == nullptr || (d->res_pitch % 8 == 0 && (reinterpret_cast<uintptr_t>(d->residual) & 3) == 0),
+               "conv: res_pitch must be a multiple of 8 and the residual 4-byte aligned");
+  for (int t = 0; t < d->taps; ++t)
+    SB_CHECK_ARG(d->wtap[t] >= 0 && d->wtap[t] < d->n_wtaps, "conv: wtap[%d]=%d out of range", t, d->wtap[t]);
+
+  ConvKParams kp;
+  memset(&kp, 0, sizeof(kp));
+  kp.N = d->N; kp.H = d->H; kp.W = d->W; kp.Cin = d->Cin; kp.Cout = d->Cout; kp.taps = d->taps;
+  choose_box(d->H, d->W, kBlockM, &kp.bh, &kp.bw);
+  kp.tiles_h = cdiv(d->H, kp.bh);
+  kp.tiles_w = cdiv(d->W, kp.bw);
+  kp.num_m_tiles = d->N * kp.tiles_h * kp.tiles_w;
+  kp.k_chunks = d->Cin / 128;
+  for (int t = 0; t < d->taps; ++t) {
+    kp.dh[t] = d->dh[t]; kp.dw[t] = d->dw[t]; kp.wtap[t] = d->wtap[t]; kp.img_add[t] = d->img_add[t];
+  }
+  kp.img_mul = d->img_mul;
+  kp.epi_mode = SEMSEG_EPI_AFFINE; kp.relu = d->relu;
+  kp.scale = d->scale; kp.shift = d->shift;
+  kp.residual = static_cast<const __nv_bfloat16*>(d->residual); kp.res_pitch = d->res_pitch;
+  kp.nseg = 1;
+  kp.out_bf16 = d->y != nullptr;
+  kp.out_e4m3 = d->y8 != nullptr;
+  kp.y8_qscale = d->y8_qscale;
+  const int block_n = d->Cout % 128 == 0 ? 128 : 64;   // <= 128: the promoted accumulation holds two register tiles
+  kp.n_tiles = d->Cout / block_n;
+  kp.k_slices = 1;
+  kp.kb_per_slice = kp.taps * kp.k_chunks;
+  const int grid = conv_grid(kp.num_m_tiles, kp.n_tiles);
+
+  ConvMaps tm;
+  {
+    uint64_t dims[4] = {(uint64_t)d->Cin, (uint64_t)d->Win, (uint64_t)d->Hin, (uint64_t)d->Nin};
+    uint64_t str[3] = {(uint64_t)d->x_pitch, (uint64_t)d->x_pitch * d->Win, (uint64_t)d->x_pitch * d->Win * d->Hin};
+    uint32_t box[4] = {128u, (uint32_t)kp.bw, (uint32_t)kp.bh, 1};
+    int r = encode_tmap_u8(&tm.a, d->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (r) return r;
+    tm.a_lo = tm.a;
+  }
+  {
+    uint64_t dims[3] = {(uint64_t)d->w_cols, (uint64_t)d->w_rows, (uint64_t)d->n_wtaps};
+    uint64_t str[2] = {(uint64_t)d->w_cols, (uint64_t)d->w_cols * d->w_rows};
+    uint32_t box[3] = {128u, (uint32_t)block_n, 1};
+    int r = encode_tmap_u8(&tm.b, d->w, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (r) return r;
+    tm.b_lo = tm.b;
+  }
+  {
+    uint32_t box[4] = {64u, (uint32_t)kp.bw, (uint32_t)kp.bh, 1};
+    int r;
+    if (d->y) {
+      uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N};
+      uint64_t str[3] = {(uint64_t)d->y_pitch * 2, (uint64_t)d->y_pitch * 2 * d->W, (uint64_t)d->y_pitch * 2 * d->W * d->H};
+      if ((r = encode_tmap_bf16(&tm.c, d->y, 4, dims, str, box))) return r;
+    }
+    if (d->y8) {   // the e4m3 staging tile: [row][64 bytes], 64-byte swizzle
+      uint64_t dims[4] = {(uint64_t)d->Cout, (uint64_t)d->W, (uint64_t)d->H, (uint64_t)d->N};
+      uint64_t str[3] = {(uint64_t)d->y8_pitch, (uint64_t)d->y8_pitch * d->W, (uint64_t)d->y8_pitch * d->W * d->H};
+      if ((r = encode_tmap_u8(&tm.c_lo, d->y8, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B))) return r;
+    }
+    if (!d->y) tm.c = tm.c_lo;
+    if (!d->y8) tm.c_lo = tm.c;
+  }
+  if (d->e4m3 == 2)   // unpromoted accumulation: the measurement form of DESIGN §4
+    return block_n == 128 ? launch_conv_e4m3<128, false>(tm, kp, grid, stream)
+                          : launch_conv_e4m3<64, false>(tm, kp, grid, stream);
+  return block_n == 128 ? launch_conv_e4m3<128, true>(tm, kp, grid, stream)
+                        : launch_conv_e4m3<64, true>(tm, kp, grid, stream);
+}
+
 extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
   using namespace sb;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -482,6 +652,8 @@ extern "C" int semseg_conv_fprop(const semseg_conv_desc* d, void* stream_) {
   SB_CHECK_ARG(d->w_cols % 8 == 0 && d->w_cols >= d->Cin, "conv: w_cols %d must be a multiple of 8 and >= Cin",
                d->w_cols);
   SB_CHECK_ARG(d->epi_mode >= 0 && d->epi_mode <= 2, "conv: bad epi_mode");
+  if (d->e4m3) return conv_fprop_e4m3(d, stream);
+  SB_CHECK_ARG(d->y8 == nullptr, "conv: y8 (e4m3 output) needs e4m3 operands");
 
   ConvKParams kp;
   memset(&kp, 0, sizeof(kp));

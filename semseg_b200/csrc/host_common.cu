@@ -53,8 +53,8 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
   return fn;
 }
 
-int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box) {
+static int encode_tmap(CUtensorMap* out, CUtensorMapDataType dtype, CUtensorMapSwizzle swizzle, const void* base,
+                       int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box) {
   auto fn = get_encode();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
@@ -84,8 +84,8 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
     }
   }
   auto encode = [&] {
-    return fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), gd, gs, bx, es,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+    return fn(out, dtype, rank, const_cast<void*>(base), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+              CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   };
   CUresult r = encode();
@@ -102,6 +102,17 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
     return SEMSEG_E_CUDA;
   }
   return SEMSEG_OK;
+}
+
+int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box) {
+  return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, CU_TENSOR_MAP_SWIZZLE_128B, base, rank, dims, strides_bytes,
+                     box);
+}
+
+int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                   const uint32_t* box, CUtensorMapSwizzle swizzle) {
+  return encode_tmap(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, swizzle, base, rank, dims, strides_bytes, box);
 }
 
 void choose_box(int H, int W, int max_pixels, int* bh_out, int* bw_out) {

@@ -50,6 +50,10 @@ int num_sms();
 int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                      const uint64_t* strides_bytes, const uint32_t* box);
 
+// The same for one-byte elements (e4m3 operands: SWIZZLE_128B; the e4m3 epilogue staging tile: SWIZZLE_64B).
+int encode_tmap_u8(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                   const uint32_t* box, CUtensorMapSwizzle swizzle);
+
 // Pixel box (bh x bw <= max_pixels) maximising tile utilisation of an H x W map.
 void choose_box(int H, int W, int max_pixels, int* bh, int* bw);
 

@@ -112,6 +112,19 @@ def network_mode(training, input_grad=True):
         _net.training, _net.input_grad = prev
 
 
+@contextlib.contextmanager
+def fp8_plan(plan):
+    """Runs the enclosed eval forward with `plan` (semseg_b200/fp8.py) consulted by every eval-mode conv + BatchNorm stage
+    on this thread: it runs the stages it covers in FP8 (or, while calibrating, records their input range) and returns
+    None for the others, which take the bf16 path."""
+    prev = getattr(_net, "fp8", None)
+    _net.fp8 = plan
+    try:
+        yield
+    finally:
+        _net.fp8 = prev
+
+
 def network_forward(fn):
     """Decorator of a module's forward(x, ...): the module is the network being run, in its own training mode."""
     @functools.wraps(fn)
@@ -466,6 +479,11 @@ def conv_bn_act(x, conv, bn, relu=True, residual=None, out=None):
     # validate() (tool/train.py:353-359) calls model.eval()(input) without torch.no_grad() and never back-propagates,
     # so the result is returned detached (a later .backward() through it raises torch's usual "does not require grad").
     # A frozen BatchNorm takes this path only when nothing of the stage needs a gradient (see _bn_mode).
+    plan = getattr(_net, "fp8", None)
+    if plan is not None:
+        y = plan.conv_bn_act(x, conv, bn, relu, residual, out)
+        if y is not None:
+            return y
     return cba_forward(x, conv, bn, relu, residual, out, mode="eval")[0]
 
 

@@ -67,8 +67,12 @@ def _model_device(model):
 
 def _native_net(model, classes, crop_h, crop_w, device):
     """The semseg_b200 PSPNet / PSANet behind `model` when its scores can be finished by csrc/window.cu, else None."""
+    from .fp8 import Fp8Eval
     from .psanet import PSANet
     from .pspnet import PSPNet
+    if isinstance(model, Fp8Eval):      # the FP8 forward of its PSPNet / PSANet (semseg_b200/fp8.py)
+        inner = _native_net(model.model, classes, crop_h, crop_w, device)
+        return model if inner is not None else None
     if isinstance(model, torch.nn.DataParallel):
         if len(model.device_ids) > 1:
             return None

@@ -397,6 +397,93 @@ def conv_fprop(x, w3d, cout, taps, *, out=None, epi=EPI_RAW, relu=False, scale=N
     return y, sp
 
 
+# ------------------------------------------------------------------------------------------------ FP8 (e4m3) eval operands
+# e4m3 activations are torch.float8_e4m3fn NHWC tensors [N,H,W,C] holding q = sat_e4m3(v * qscale), qscale = 448 / amax
+# of the calibrated tensor (semseg_b200/fp8.py); the dequantisation scale amax / 448 lives in the consuming conv's folded
+# epilogue scale. Used by the eval-only FP8 forward; the training and bf16 / bf16x3 paths never see them.
+E4M3 = torch.float8_e4m3fn
+
+
+def _e4m3_meta(t):
+    """(N, H, W, C, pitch) of an e4m3 NHWC activation (pitch in bytes = elements)."""
+    assert t.dtype == E4M3 and t.dim() == 4, (t.shape, t.dtype)
+    n, h, w, c = t.shape
+    sn, sh, sw, sc = t.stride()
+    assert sc == 1 and sh == sw * w and sn == sh * h, "NHWC tensor must be pixel-contiguous (stride %s)" % (t.stride(),)
+    return n, h, w, c, sw
+
+
+def fp8_quantize(x, qscale):
+    """bf16 NHWC activation -> e4m3 NHWC activation sat_e4m3(x * qscale) (one launch)."""
+    _require_cuda(x)
+    lib = _lib.load()
+    n, h, w, c, p = _nhwc_meta(x)
+    assert not is_split(x), "FP8 operands are quantised from plain bf16 activations"
+    y = torch.empty((n, h, w, c), dtype=E4M3, device=x.device)
+    _lib.check(lib.semseg_fp8_quantize(_ptr(x), p, _ptr(y), c, n * h * w, c, float(qscale), _stream()),
+               "semseg_fp8_quantize")
+    return y
+
+
+def fp8_amax(x, amax_bits):
+    """amax_bits (int32 [1], read as fp32 bits) = max(amax_bits, max |x|) of a bf16 NHWC activation, on the device."""
+    _require_cuda(x, amax_bits)
+    lib = _lib.load()
+    n, h, w, c, p = _nhwc_meta(x)
+    assert not is_split(x) and amax_bits.dtype == torch.int32
+    _lib.check(lib.semseg_fp8_amax(_ptr(x), p, n * h * w, c, _ptr(amax_bits), _stream()), "semseg_fp8_amax")
+
+
+def fp8_pack_weights(w):
+    """fp32 OIHW conv weight -> (e4m3 slab [taps][Cout][Cin], fp32 dequantisation scales [Cout] = amax_c / 448)."""
+    _require_cuda(w)
+    lib = _lib.load()
+    w = w.detach()
+    w = w if w.is_contiguous() else w.contiguous()
+    assert w.dtype == torch.float32 and w.dim() == 4 and w.shape[2] == w.shape[3]
+    cout, cin, k, _ = w.shape
+    wf = torch.empty((k * k, cout, cin), dtype=E4M3, device=w.device)
+    sw = torch.empty((cout,), dtype=torch.float32, device=w.device)
+    _lib.check(lib.semseg_fp8_pack_weights(_ptr(w), cout, cin, k * k, _ptr(wf), _ptr(sw), _stream()),
+               "semseg_fp8_pack_weights")
+    return wf, sw
+
+
+def conv_fprop_e4m3(x8, wf8, cout, taps, *, scale, shift, relu=False, residual=None, bf16_out=True, y8_qscale=None,
+                    img_add=None, out_nhw=None, promote=True):
+    """The AFFINE conv (act(acc * scale + shift + residual)) of e4m3 `x8` with the e4m3 slab `wf8` [taps][Cout][Cin]:
+    returns (y bf16 NHWC or None, y8 e4m3 NHWC or None); y8 = sat_e4m3(v * y8_qscale) is written when y8_qscale is
+    given, y when bf16_out. `scale` carries the dequantisation (s_x * s_w[c]). promote=False: the unpromoted
+    tensor-core accumulation, for measuring what the promotion buys (tools/probe_accum.py)."""
+    _require_cuda(x8, wf8)
+    lib = _lib.load()
+    nin, hin, win, cin, xp = _e4m3_meta(x8)
+    n, h, w = out_nhw if out_nhw is not None else (nin, hin, win)
+    assert wf8.dtype == E4M3 and wf8.is_contiguous() and wf8.dim() == 3
+    assert bf16_out or y8_qscale is not None
+    d = ConvDesc()
+    d.N, d.H, d.W, d.Cin, d.Cout = n, h, w, cin, cout
+    d.x, d.Nin, d.Hin, d.Win, d.x_pitch = x8.data_ptr(), nin, hin, win, xp
+    d.w, d.n_wtaps, d.w_rows, d.w_cols = wf8.data_ptr(), wf8.shape[0], wf8.shape[1], wf8.shape[2]
+    _fill_taps(d, taps, img_add=img_add)
+    d.epi_mode, d.relu, d.e4m3 = EPI_AFFINE, int(bool(relu)), 1 if promote else 2
+    assert scale.dtype == torch.float32 and shift.dtype == torch.float32 and scale.numel() >= cout
+    d.scale, d.shift = scale.data_ptr(), shift.data_ptr()
+    y = y8 = None
+    if bf16_out:
+        y = torch.empty((n, h, w, cout), dtype=torch.bfloat16, device=x8.device)
+        d.y, d.y_pitch = y.data_ptr(), cout
+    if y8_qscale is not None:
+        y8 = torch.empty((n, h, w, cout), dtype=E4M3, device=x8.device)
+        d.y8, d.y8_pitch, d.y8_qscale = y8.data_ptr(), cout, float(y8_qscale)
+    if residual is not None:
+        rn, rh, rw, rc, rp = _nhwc_meta(residual)
+        assert (rn, rh, rw, rc) == (n, h, w, cout) and not is_split(residual)
+        d.residual, d.res_pitch = residual.data_ptr(), rp
+    _lib.check(lib.semseg_conv_fprop(ctypes.byref(d), _stream()), "semseg_conv_fprop (e4m3)")
+    return y, y8
+
+
 def conv_wgrad(x, dy, cin, cout, taps, grad_out=None, accumulate=False, img_add=None):
     """dW (fp32 OIHW [cout][cin][k][k]) from NHWC bf16 x and dy. The pixel grid is dy's; `x` may be a phase tensor
     (stride-2 convs) addressed through `img_add`."""
