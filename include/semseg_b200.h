@@ -605,6 +605,22 @@ int semseg_upsample_ce_focal_bwd(const float* logits, int pitch, int N, int h, i
                                  int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* mod,
                                  const float* loss_info, const float* grad_out, float* workspace, float* dlogits,
                                  void* stream);
+/* The SegPGD attack loss (Gu et al., ECCV 2022; semseg_b200/adversarial.py) on the same fused upsample at zoom `zoom`.
+ * Per valid pixel j (target != ignore_index, 0 <= target < C), with pred_j the first-maximum argmax of the upsampled
+ * logits computed in the same pass and nll_j = lse_j - v_{j,target} (the plain forward's bits):
+ *   w_j = (1 - lambda) if pred_j == target_j else lambda,   loss = sum_j w_j nll_j / n_valid,
+ * the weights constants (no gradient through the argmax); loss 0 and an exactly zero gradient when no pixel is valid.
+ * lambda finite in [0, 1] (the attack's lambda_t = (t - 1) / (2T) at iteration t = 1..T).
+ *   fwd: loss_out[0] = loss, loss_out[1] = n_valid; argmax (or NULL) and lse as the zoom forward's (the same bits);
+ *        mod fp32 [N,Ho,Wo] = w_j, 0 where the pixel is not valid; workspace: semseg_upsample_ce_zoom_workspace_floats()
+ *        floats.
+ *   bwd: semseg_upsample_ce_focal_bwd(logits, ..., lse, mod, loss_out, ...) gives grad_out[0] * dloss/dlogits
+ *        = grad_out[0] sum_j w_j (p_c - [c = target_j]) / n_valid.
+ * Wo has the focal width limit (2389 at zoom 8). A bad shape, zoom, lambda, width, alignment or null pointer is rejected
+ * before any CUDA call. */
+int semseg_upsample_segpgd_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                               int Ho, int Wo, int zoom, int ignore_index, float lambda, float* workspace,
+                               float* loss_out, int64_t* argmax, float* lse, float* mod, void* stream);
 /* Lovász-Softmax loss (Berman et al., CVPR 2018), alone or plus cross-entropy (semseg_b200/losses.py
  * LovaszSoftmaxLoss), on the same fused upsample at zoom `zoom`. p = softmax(v) as the Dice passes compute it. A segment
  * is one class over every valid pixel of the call (per_image = 0, S = C segments of L = N*Ho*Wo pixels) or one (image,
@@ -1073,6 +1089,30 @@ typedef struct semseg_augment_desc {
 int semseg_augment(const void* data, long long data_bytes, const semseg_augment_desc* desc_host,
                    const semseg_augment_desc* desc_dev, int n, int crop_h, int crop_w, const float* mean3,
                    const float* std3, int ignore_label, float* out_img, long long* out_lab, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * L-infinity PGD / SegPGD attack steps (semseg_b200/adversarial.py) on the network's fp32 NCHW input [N,3,H,W] in the
+ * normalised space it sees. Per channel c, from the attack's eps, alpha and the trainer's mean / std in 0-255 pixel
+ * units, computed on the host in fp64 and rounded to fp32 once:
+ *   step[c] = alpha / std_c,  eps[c] = eps / std_c,  lo[c] = (0 - mean_c) / std_c,  hi[c] = (255 - mean_c) / std_c.
+ * Every operation below is one fp32 round-to-nearest in the order written, without FMA contraction, so the results are
+ * bit-identical to the same formula in torch fp32 (s = sign(g) with sign(0) = 0, as torch.sign):
+ *   semseg_adv_step : v = x + step s;  v = min(max(v, x0 - eps), x0 + eps);  out = min(max(v, lo), hi)
+ *                     (step s is exact; out may be x: the step runs in place)
+ *   semseg_adv_start: out = min(max(min(max(x0 + eps (2u - 1), x0 - eps), x0 + eps), lo), hi)
+ *                     (u: uniforms in [0, 1) of the input's shape, drawn by the caller)
+ * Both reject a null pointer, a tensor that is not 4-byte aligned, a bad shape (3N <= 65535) or constants that are not
+ * finite, a negative step or eps, or lo > hi, before any CUDA call. */
+typedef struct semseg_adv_box {
+  float step[3];
+  float eps[3];
+  float lo[3];
+  float hi[3];
+} semseg_adv_box;
+int semseg_adv_step(const float* x, const float* grad, const float* x0, float* out, int N, int H, int W,
+                    const semseg_adv_box* box, void* stream);
+int semseg_adv_start(const float* x0, const float* u, float* out, int N, int H, int W, const semseg_adv_box* box,
+                     void* stream);
 
 #ifdef __cplusplus
 }

@@ -95,6 +95,11 @@ class WgradDesc(ctypes.Structure):
     ]
 
 
+class AdvBox(ctypes.Structure):
+    """struct semseg_adv_box (include/semseg_b200.h): the attack step's per-channel constants."""
+    _fields_ = [("step", c_f * 3), ("eps", c_f * 3), ("lo", c_f * 3), ("hi", c_f * 3)]
+
+
 class AugmentDesc(ctypes.Structure):
     """struct semseg_augment_desc (include/semseg_b200.h): one sample of semseg_augment."""
     _fields_ = [("img_off", c_ll), ("lab_off", c_ll), ("h", c_i32), ("w", c_i32), ("rh", c_i32), ("rw", c_i32),
@@ -231,6 +236,8 @@ SIGNATURES = {
     "semseg_upsample_ce_focal_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_focal_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                              c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_segpgd_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                           c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_upsample_ce_lovasz_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_lovasz_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int,
                                               c_int, c_int, c_int, c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
@@ -303,6 +310,8 @@ SIGNATURES = {
     "semseg_densecrf_keys": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_d, c_d, c_d, c_vp, c_vp]),
     "semseg_augment": (c_int, [c_vp, c_ll, ctypes.POINTER(AugmentDesc), c_vp, c_int, c_int, c_int, c_vp, c_vp, c_int,
                                c_vp, c_vp, c_vp]),
+    "semseg_adv_step": (c_int, [c_vp, c_vp, c_vp, c_vp, c_int, c_int, c_int, ctypes.POINTER(AdvBox), c_vp]),
+    "semseg_adv_start": (c_int, [c_vp, c_vp, c_vp, c_int, c_int, c_int, ctypes.POINTER(AdvBox), c_vp]),
 }
 
 _lib = None

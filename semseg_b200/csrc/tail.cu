@@ -51,6 +51,9 @@
 //
 // Entropy minimisation plus cross-entropy (TENT / MinEnt) runs sibling forward and rows kernels (see "entropy" below)
 // with the plain reduce and cols kernels; no existing instance changes.
+//
+// The SegPGD attack loss runs a sibling forward kernel with the plain reduce; its backward is the focal backward on the
+// forward's per-pixel weights (see "SegPGD" below). No existing instance changes.
 #include <cmath>
 
 #include "host_common.h"
@@ -1802,6 +1805,123 @@ upsample_ce_focal_rows_kernel(const float* __restrict__ logits, int pitch, int N
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- SegPGD
+// The SegPGD attack loss (Gu et al., ECCV 2022). Per valid pixel (target t in [0, C), t != ignore_index), with pred the
+// first-maximum argmax of the same pass and nll = lse - v_t as the plain forward computes it:
+//   w = (1 - lambda) if pred == t else lambda,   loss = sum w nll / n_valid.
+// The weights are constants (no gradient through the argmax), so dloss/dv_c = w (p_c - [c = t]) / n_valid: the focal
+// backward with the modulator map mod = w (0 where the pixel is not valid). The two class passes are the plain
+// forward's, so lse, the argmax and nll carry the plain kernel's bits.
+template <int Z>
+__global__ void __launch_bounds__(kFwdCols)
+upsample_segpgd_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
+                           const long long* __restrict__ target, int Ho, int Wo, int ignore_index, float lambda,
+                           float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out,
+                           float* __restrict__ mod_out) {
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs] as in upsample_ce_fwd_kernel
+  __shared__ float red_loss[kFwdCols / 32];
+  __shared__ float red_cnt[kFwdCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kFwdNodes, w - j_base);
+  const int tid = threadIdx.x;
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * kFwdNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
+  }
+  __syncthreads();
+  float loss = 0.f, cnt = 0.f;
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* A = S + (j0 - j_base) * Cs;
+    const float* B = S + (j1 - j_base) * Cs;
+    const float* Cc = A + kFwdNodes * Cs;
+    const float* D = B + kFwdNodes * Cs;
+    float m[Z], sum[Z];
+    int am[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      m[r] = -INFINITY;
+      am[r] = 0;
+      sum[r] = 0.f;
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        if (v > m[r]) {
+          m[r] = v;
+          am[r] = c;
+        }
+      }
+    }
+    float m2[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) m2[r] = m[r] * kLog2e;
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) sum[r] += ex2_approx(fmaf(row_lerp<Z>(top, bot, r), kLog2e, -m2[r]));
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+        const long long t = target[pix];
+        const float lse = m[r] + __logf(sum[r]);
+        if (argmax_out) argmax_out[pix] = am[r];
+        lse_out[pix] = lse;
+        float wt = 0.f;
+        if (t != ignore_index && t >= 0 && t < C) {
+          const int tc = static_cast<int>(t);
+          const float top = Z == 1 ? A[tc] : l0w * A[tc] + l1w * B[tc];
+          const float bot = Z == 1 ? 0.f : l0w * Cc[tc] + l1w * D[tc];
+          const float vt = row_lerp<Z>(top, bot, r);
+          wt = am[r] == tc ? 1.f - lambda : lambda;
+          loss += wt * (lse - vt);
+          cnt += 1.f;
+        }
+        mod_out[pix] = wt;
+      }
+    }
+  }
+  // deterministic block reduction -> one (sum of w nll, valid count) partial per CTA, as upsample_ce_fwd_kernel
+  for (int o = 16; o > 0; o >>= 1) {
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((tid & 31) == 0) {
+    red_loss[tid >> 5] = loss;
+    red_cnt[tid >> 5] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float l = 0.f, k = 0.f;
+    for (int i = 0; i < kFwdCols / 32; ++i) {
+      l += red_loss[i];
+      k += red_cnt[i];
+    }
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[2 * b] = l;
+    partial[2 * b + 1] = k;
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------- pseudo-labels
 // Confidence-masked pseudo-label cross-entropy from a teacher (FixMatch / UniMatch self-training), with s and t the
 // student and teacher maps after the same xZ upsample:
@@ -3495,6 +3615,54 @@ extern "C" int semseg_upsample_ce_focal_bwd(const float* logits, int pitch, int 
                                        grad_out, workspace, dlogits, stream);
     default: return launch_focal_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lse, mod, loss_info,
                                         grad_out, workspace, dlogits, stream);
+  }
+}
+
+// SegPGD at zoom factor `zoom`: its own forward kernel, the plain reduce; the backward is semseg_upsample_ce_focal_bwd.
+template <int Z>
+static int launch_segpgd_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                             int Wo, int ignore_index, float lambda, float* workspace, float* loss_out, int64_t* argmax,
+                             float* lse, float* mod, cudaStream_t stream) {
+  const int Cs = C | 1;
+  constexpr size_t kMaxSmem =
+      static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_segpgd_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_segpgd_fwd_kernel<Z><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lambda,
+      workspace, reinterpret_cast<long long*>(argmax), lse, mod);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" int semseg_upsample_segpgd_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                          const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                          float lambda, float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                          float* mod, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  SB_CHECK_ARG(std::isfinite(lambda) && lambda >= 0.f && lambda <= 1.f,
+               "upsample_segpgd_fwd: lambda %g is not in [0, 1]", lambda);
+  // the focal backward's rows kernel stages this map: its width limit and alignment
+  r = check_focal(zoom, Wo, 0.f, nullptr, mod);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && mod, "upsample_segpgd_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_segpgd_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lambda, workspace,
+                                        loss_out, argmax, lse, mod, stream);
+    case 2: return launch_segpgd_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lambda, workspace,
+                                        loss_out, argmax, lse, mod, stream);
+    case 4: return launch_segpgd_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lambda, workspace,
+                                        loss_out, argmax, lse, mod, stream);
+    default: return launch_segpgd_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, lambda, workspace,
+                                         loss_out, argmax, lse, mod, stream);
   }
 }
 

@@ -641,6 +641,31 @@ class _UpsampleCEFocal(torch.autograd.Function):
         return dl, None, None, None, None, None
 
 
+class _UpsampleSegPGD(torch.autograd.Function):
+    """The fused tail with the SegPGD attack loss (adversarial.PGDAttack(kind='segpgd')): the mean over the valid pixels
+    of w nll, w = 1 - lam where the argmax hits the target and lam elsewhere, the weights constants. The forward keeps
+    each pixel's weight; the backward is the focal one with that modulator map."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, lam):
+        info, amax, lse, mod = ops.upsample_segpgd_fwd(logits, target, ignore_index, lam, zoom=zoom)
+        ctx.save_for_backward(logits, target, lse, mod, info)
+        ctx.ignore_index, ctx.zoom = ignore_index, zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, target, lse, mod, info = ctx.saved_tensors
+        dl = ops.upsample_ce_focal_bwd(logits, target, ctx.ignore_index, lse, mod, info, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None
+
+
+def upsample_segpgd(logits, target, ignore_index, zoom, lam):
+    """-> (SegPGD loss scalar, argmax) of fp32 NHWC logits against the zoomed target (see _UpsampleSegPGD)."""
+    return _UpsampleSegPGD.apply(logits, target.contiguous(), int(ignore_index), int(zoom), float(lam))
+
+
 class _UpsampleCEEntropy(torch.autograd.Function):
     """The fused tail with losses.EntropyLoss: ce_weight * CE over the labelled pixels plus ent_weight * the mean
     softmax entropy over the unlabelled ones. The forward keeps each pixel's lse and expected logit; the backward
@@ -912,14 +937,15 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     contiguous fp32 [classes] tensor on that device; any other weight, another reduction, and any subclass keep the
     ATen tail. DiceLoss, FocalLoss and losses.LovaszSoftmaxLoss also need the target no wider than their kernels stage
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
-    form's conditions; losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
+    form's conditions, and so does losses.AdversarialLoss (plain cross-entropy on the attacked batch; the attack checks
+    its own tail's limits); losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
     losses.EntropyLoss, whose rows kernel stages the same words, the Dice width limit. losses.RMILoss needs a target of
     at least 12 x 12 and no wider than its rows kernel stages (3584 columns
     at zoom 8). losses.GatedCRFLoss and losses.ActiveBoundaryLoss need the target no wider than the plain backward
     stages (2560 columns at zoom 8); their classes (<= 256, checked here with the logits) and options are in the
     kernels' limits by construction.
     `logits` fp32 NHWC, or None with the NCHW input size `x_size` (decision before the network has run)."""
-    if type(criterion) is losses.DistillationLoss:
+    if type(criterion) in (losses.DistillationLoss, losses.AdversarialLoss):
         ok = True
     elif type(criterion) is nn.CrossEntropyLoss:
         eps = getattr(criterion, 'label_smoothing', 0.0)

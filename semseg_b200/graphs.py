@@ -22,6 +22,7 @@ are not captured (such models simply stay eager). With a teacher criterion the t
 re-pack included), the draws, the strong view, the mixing and the extra student streams are captured with the step.
 Set SEMSEG_B200_GRAPH=0 to disable; any capture failure also falls back to the eager path (same kernels) with a warning.
 """
+import contextlib
 import os
 import warnings
 
@@ -34,6 +35,7 @@ WARMUP_CALLS = 3          # eager calls with an unchanged key before capturing
 MAX_GRAPHS = 4            # captured input shapes per model (each keeps a private activation pool); others stay eager
 _capturing = False
 _boundary = None          # activation noted by the model during capture: where the backward is cut in two
+_no_boundary = 0          # > 0 inside passes that are not the step's own forward (an adversarial attack's)
 
 
 def enabled():
@@ -53,9 +55,22 @@ def note_boundary(t):
     DDP's bucket hooks: their all-reduce starts) while the second graph still computes, which restores the
     communication / computation overlap a single backward graph would lose."""
     global _boundary
-    if _capturing and t.requires_grad:
+    if _capturing and not _no_boundary and t.requires_grad:
         _boundary = t
     return t
+
+
+@contextlib.contextmanager
+def no_boundary():
+    """Network passes run inside a captured step that are not the step's own forward (the K passes of an adversarial
+    attack, losses.AdversarialLoss): their activations need a gradient too, but the step's backward must not be cut
+    at them."""
+    global _no_boundary
+    _no_boundary += 1
+    try:
+        yield
+    finally:
+        _no_boundary -= 1
 
 
 class _Step:

@@ -17,7 +17,9 @@ batch, the student learns on the mixed one. Each of the three teacher criteria t
 the student then learns on a strongly perturbed view of the batch the teacher sees. The two pseudo-label criteria take
 `fp_weight=` too: UniMatch's feature perturbation, a second pass of the context module and classifier on the student's
 channel-dropped layer4 features that learns the same pseudo-labels, and `streams=2`: UniMatch's dual-stream
-perturbation, two strong views of every image, each with its own draws, in one student pass.
+perturbation, two strong views of every image, each with its own draws, in one student pass. AdversarialLoss is PGD
+adversarial training: an adversarial.PGDAttack runs on the network inside its training forward and both heads learn
+plain cross-entropy on the attacked batch.
 """
 import math
 
@@ -1087,6 +1089,77 @@ class RMILoss(nn.Module):
                              (logits.shape[2], logits.shape[3]))
         _check_native_logits("RMILoss", logits, target)
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+class AdversarialLoss(nn.Module):
+    """PGD adversarial training (Madry et al., ICLR 2018; for PSPNet, DDC-AT, Xu, Zhao & Jia, ICCV 2021): the network
+    learns on adversarial images. Given as the `criterion` of a PSPNet / PSANet, per training forward with input x and
+    target y:
+
+        x_adv = attack(x, y)      the adversarial.PGDAttack `attack`, run on the network itself in eval mode
+        main  = CE(student(x_adv), y),  aux = CE(aux head on x_adv, y)     (plain cross-entropy, ignore_index)
+        pred  = the student's argmax on x_adv
+
+    The attack runs inside the training forward, after the weight re-pack and before the student's stem: every module's
+    own training flag is recorded, the network is put in eval mode (running statistics, no dropout), the same function
+    as PGDAttack.attack runs its K iterations with the parameters as constants (no weight gradient, `.grad` untouched,
+    no buffer changes), and each module's flag is put back (a frozen-BatchNorm recipe keeps its eval layers). With the
+    fused tail the whole step, the attack included, is one captured training step (graphs.train_step). Under
+    DistributedDataParallel each rank attacks its own images (eval BatchNorm exchanges nothing between ranks).
+
+    `last_adv()` returns {'image': x_adv, 'losses': the attack's per-iteration losses, fp32 [steps]} of the latest
+    training forward, graphed or eager, as views that stay valid until the next forward. There is no gradient through
+    the attack to the input: an input with requires_grad raises. Called as a module, forward(logits, target) is the plain
+    cross-entropy (validate() logs it)."""
+
+    graph_options = ("ignore_index", "attack_key")
+
+    def __init__(self, attack, ignore_index=255):
+        super(AdversarialLoss, self).__init__()
+        from .adversarial import PGDAttack
+        if not isinstance(attack, PGDAttack):
+            raise TypeError("attack must be an adversarial.PGDAttack, got %s" % type(attack).__name__)
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        self.attack = attack
+        self.ignore_index = ignore_index
+        self._last = {}      # last_adv(); put back by a graphed replay
+
+    @property
+    def attack_key(self):
+        return self.attack.key()
+
+    def extra_repr(self):
+        return "attack=%r, ignore_index=%d" % (self.attack, self.ignore_index)
+
+    def last_adv(self):
+        """{'image', 'losses'} of the latest training forward's attack (None before the first one)."""
+        r = self._last.get('adv')
+        return None if r is None else dict(r)
+
+    def perturb(self, model, x, y):
+        """x_adv for the training forward of `model` (its operand slabs packed) on (x, y); remembered for last_adv()."""
+        from . import adversarial
+        name = type(self).__name__
+        if x.requires_grad:
+            raise RuntimeError("%s: there is no gradient through the attack; the input must not require grad" % name)
+        adversarial.check_inputs(model, x, y, self.attack.kind, name)
+        flags = [(m, m.training) for m in model.modules()]
+        for m, _ in flags:
+            m.training = False
+        try:
+            x_adv, per_step = adversarial.run(model, self.attack, x, y)
+        finally:
+            for m, f in flags:
+                m.training = f
+        self._last['adv'] = {'image': x_adv, 'losses': per_step}
+        return x_adv
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        _check_native_logits("AdversarialLoss", logits, target)
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1)
         return loss
 
 

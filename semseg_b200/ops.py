@@ -1024,6 +1024,74 @@ def upsample_ce_focal_bwd(logits, target, ignore_index, lse, mod, info, grad_out
     return dl
 
 
+def upsample_segpgd_fwd(logits, target, ignore_index, lam, want_argmax=True, zoom=8):
+    """The SegPGD attack loss on the fused tail (include/semseg_b200.h states the contract); arguments as upsample_ce_fwd
+    plus `lam` in [0, 1] -> (loss_info [2] = (loss, valid count), argmax, lse, mod). mod fp32 [N,Ho,Wo]: each pixel's
+    weight (1 - lam where the argmax hits the target, lam elsewhere), 0 where the pixel is not valid. The backward is
+    upsample_ce_focal_bwd with this map."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_zoom_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_zoom_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse, mod = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
+    _lib.check(lib.semseg_upsample_segpgd_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                              int(zoom), int(ignore_index), float(lam), _ptr(ws), _ptr(info),
+                                              _ptr(amax), _ptr(lse), _ptr(mod), _stream()),
+               "semseg_upsample_segpgd_fwd")
+    return info, amax, lse, mod
+
+
+# ------------------------------------------------------------------------------------------------ attack steps
+def adv_box(eps, alpha, mean, std):
+    """The attack's per-channel constants in the network's normalised space, from eps, alpha and the trainer's mean /
+    std (0-255 pixel units): step = alpha / std, eps / std, the pixel box ((0 - mean) / std, (255 - mean) / std),
+    computed in fp64 (Python floats) and rounded to fp32 once."""
+    box = _lib.AdvBox()
+    for c in range(3):
+        s, m = float(std[c]), float(mean[c])
+        box.step[c], box.eps[c] = float(alpha) / s, float(eps) / s
+        box.lo[c], box.hi[c] = (0.0 - m) / s, (255.0 - m) / s
+    return box
+
+
+def _adv_shape(*ts):
+    _require_cuda(*ts)
+    x = ts[0]
+    for t in ts:
+        if not (t.dtype == torch.float32 and t.is_contiguous() and t.shape == x.shape and t.device == x.device):
+            raise ValueError("semseg_b200: attack step tensors must be contiguous fp32 of one shape on one device, got "
+                             "%s" % [(t.dtype, tuple(t.shape), str(t.device)) for t in ts])
+    if x.dim() != 4 or x.shape[1] != 3:
+        raise ValueError("semseg_b200: attack step needs an [N, 3, H, W] input, got %s" % (tuple(x.shape),))
+    return x.shape[0], x.shape[2], x.shape[3]
+
+
+def adv_step(x, grad, x0, box, out=None):
+    """One projected sign step (semseg_adv_step) -> out (a new tensor, or `out`, which may be `x`)."""
+    out = torch.empty_like(x) if out is None else out
+    n, h, w = _adv_shape(x, grad, x0, out)
+    _lib.check(_lib.load().semseg_adv_step(_ptr(x), _ptr(grad), _ptr(x0), _ptr(out), n, h, w, ctypes.byref(box),
+                                           _stream()), "semseg_adv_step")
+    return out
+
+
+def adv_start(x0, u, box, out=None):
+    """The random start inside the eps-ball and the pixel box (semseg_adv_start) from uniforms `u`."""
+    out = torch.empty_like(x0) if out is None else out
+    n, h, w = _adv_shape(x0, u, out)
+    _lib.check(_lib.load().semseg_adv_start(_ptr(x0), _ptr(u), _ptr(out), n, h, w, ctypes.byref(box), _stream()),
+               "semseg_adv_start")
+    return out
+
+
 def upsample_ce_entropy_fwd(logits, target, ignore_index, want_argmax=True, zoom=8):
     """Entropy minimisation plus cross-entropy on the fused tail (include/semseg_b200.h states the contract); arguments as
     upsample_ce_fwd -> (loss_info [6] = (CE mean over L, |L|, H mean over U, |U|, 0, 1), argmax, lse, mu). mu fp32

@@ -153,6 +153,10 @@ class _SegNet(nn.Module):
         if self.training and torch.is_grad_enabled():
             SF.prepack(self, force=graphs.capturing())   # all conv operand slabs refreshed in one launch
             p2p.begin_step(force=graphs.capturing())     # new SyncBN exchange epoch (device-resident step counter)
+        if self.training and y is not None and isinstance(self.criterion, losses.AdversarialLoss):
+            # PGD adversarial training: the attack runs on this network in eval mode, with the packs just refreshed;
+            # the student and both heads' losses see x_adv
+            x = self.criterion.perturb(self, x, y)
         t_logits = mix_mask = fp_scale = t_feat = None
         streams = 1
         relation = False
