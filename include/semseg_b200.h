@@ -27,6 +27,8 @@
  *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
  *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
+ *                               semseg_upsample_ce_unbiased_*, semseg_upsample_unkd_*: MiB's class-incremental
+ *                               cross-entropy and distillation from the previous step's logits.
  *                               semseg_upsample_pl_*: confidence-masked pseudo-labels from a teacher's logits.
  *                               semseg_upsample_ce_entropy_*: entropy minimisation, plus cross-entropy.
  *                               semseg_gated_crf_*: the Gated CRF loss's pairwise term (csrc/crf.cu).
@@ -675,6 +677,49 @@ long long semseg_upsample_kd_bwd_workspace_floats(int N, int Ho, int w, int C, i
 int semseg_upsample_kd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
                            int C, int Ho, int Wo, int zoom, float temperature, float kd_weight, const float* lse,
                            const float* grad_out, float* workspace, float* dlogits, void* stream);
+/* Class-incremental training (MiB, Cermelli et al., CVPR 2020; semseg_b200/losses.py IncrementalLoss) on the same fused
+ * upsample at zoom `zoom`: a student of C classes, the previous step's network (the teacher) of C_old, 2 <= C_old < C
+ * <= 256. Class 0 is the background, [0, C_old) the old classes, [C_old, C) the new ones; lse_A(x) = log sum_{c in A}
+ * exp(x_c), each subset's sum against its own maximum (a confident new-class pixel labelled background gives a large
+ * finite loss). Both backward rows kernels stage 12 bytes per pixel: the Dice width limit, Wo <= 2389 at zoom 8.
+ * Unbiased cross-entropy, per valid pixel (target != ignore_index, 0 <= target < C):
+ *   l = lse_all(s) - lse_old(s) for target < C_old (old labels count as background), lse_all(s) - s_target otherwise;
+ *   loss = mean over the valid pixels (0 with a zero gradient when there is none);
+ *   dl/ds_c = p_c - [target < C_old][c < C_old] exp(s_c - lse_old) - [target >= C_old][c = target].
+ *   fwd: loss_out[0] = loss, loss_out[1] = n_valid; argmax (or NULL) over all C classes and lse as the zoom forward's;
+ *        lse_old fp32 [N,Ho,Wo] = lse_old(s) per pixel (keep both for the backward); workspace:
+ *        semseg_upsample_ce_unbiased_workspace_floats() floats.
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits; workspace: semseg_upsample_ce_unbiased_bwd_workspace_floats().
+ * Unbiased distillation: the teacher is an fp32 NHWC [N,h,w,C_old] map with its own pitch (>= C_old), upsampled as the
+ * student. With q = softmax(alpha t) over the C_old classes (alpha finite and > 0), B = {0} u [C_old, C), per pixel
+ * (every pixel, no target):
+ *   k = -(1/C_old) [ q_0 (lse_B(s) - lse_all(s)) + sum_{c=1}^{C_old-1} q_c (s_c - lse_all(s)) ],  KD = mean of k over the
+ *   P = N*Ho*Wo pixels;  dKD/ds_c = (p_c - q_0 exp(s_c - lse_B)) / (C_old P) for c in B, (p_c - q_c) / (C_old P) else.
+ *   fwd: loss_out[0] = KD, loss_out[1] = P; lse fp32 [N,Ho,Wo,3] = (lse_all(s), lse_B(s), lse(alpha t)) per pixel, keep
+ *        it for the backward; workspace: semseg_upsample_unkd_workspace_floats() floats.
+ *   bwd: ADDS grad_out[0] * kd_weight * dKD/ds into dlogits fp32 [N,h,w,C] (dense), which the caller has filled (with the
+ *        unbiased cross-entropy gradient); the teacher gets no gradient. workspace:
+ *        semseg_upsample_unkd_bwd_workspace_floats() floats.
+ * All four reject a bad shape, zoom, C_old, alpha, kd_weight, pitch, width or null pointer before any CUDA call; the
+ * workspace functions return -1 for a zoom outside {1, 2, 4, 8} or a bad size. No host synchronisation
+ * (graph-capturable), no atomics: deterministic. */
+long long semseg_upsample_ce_unbiased_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_ce_unbiased_fwd(const float* logits, int pitch, int N, int h, int w, int C, int C_old,
+                                    const int64_t* target, int Ho, int Wo, int zoom, int ignore_index, float* workspace,
+                                    float* loss_out, int64_t* argmax, float* lse, float* lse_old, void* stream);
+long long semseg_upsample_ce_unbiased_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_unbiased_bwd(const float* logits, int pitch, int N, int h, int w, int C, int C_old,
+                                    const int64_t* target, int Ho, int Wo, int zoom, int ignore_index, const float* lse,
+                                    const float* lse_old, const float* loss_info, const float* grad_out,
+                                    float* workspace, float* dlogits, void* stream);
+long long semseg_upsample_unkd_workspace_floats(int N, int Ho, int Wo, int zoom);
+int semseg_upsample_unkd_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                             int C, int C_old, int Ho, int Wo, int zoom, float alpha, float* workspace, float* loss_out,
+                             float* lse, void* stream);
+long long semseg_upsample_unkd_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_unkd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                             int C, int C_old, int Ho, int Wo, int zoom, float alpha, float kd_weight, const float* lse,
+                             const float* grad_out, float* workspace, float* dlogits, void* stream);
 /* Cross-image relational distillation (semseg_b200/losses.py DistillationLoss relation_weight; CIRKD's mini-batch
  * pixel-to-pixel term). Features are NHWC bf16 [B,h,w,C] activations (lo == NULL: plain; else the split form), C = 512.
  *   nodes:     node (a,b) of image n max-pools rows [p a, min(p a + p, h)) x columns [p b, min(p b + p, w)) per channel

@@ -250,6 +250,18 @@ SIGNATURES = {
     "semseg_upsample_kd_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_kd_bwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_f,
                                        c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_unbiased_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_unbiased_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,
+                                                c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_unbiased_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_unbiased_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,
+                                                c_int, c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_unkd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_unkd_fwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                         c_int, c_f, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_unkd_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_unkd_bwd": (c_int, [c_vp, c_int, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                         c_int, c_f, c_f, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_relation_nodes": (c_int, [c_vp, c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp, c_vp, c_vp,
                                       c_vp]),
     "semseg_relation_workspace_floats": (c_ll, [c_int, c_int]),

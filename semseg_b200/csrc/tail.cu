@@ -54,6 +54,10 @@
 //
 // The SegPGD attack loss runs a sibling forward kernel with the plain reduce; its backward is the focal backward on the
 // forward's per-pixel weights (see "SegPGD" below). No existing instance changes.
+//
+// MiB's unbiased cross-entropy is a third compile-time flag of the plain forward and rows kernels, kUnbiased; its unbiased
+// distillation runs sibling kernels of the distillation ones with their cols kernel (see "class-incremental" below). The
+// kUnbiased = false instances are unchanged.
 #include <cmath>
 
 #include "host_common.h"
@@ -116,13 +120,19 @@ __device__ __forceinline__ void stage_class_weights(const float* __restrict__ cl
 // kWeighted without kOhem: the partials are (sum of loss_pix, sum of w_t); the class weights and W are staged after the
 // node rows and the second class pass also sums w_c (m - v_c) per output row (m: the row's max, so no term cancels).
 // kWeighted with kOhem: nll = w_t (lse - v_t). The weighted-only arguments come after the OHEM ones.
-template <int Z, bool kOhem, bool kWeighted = false>
+// kUnbiased (MiB's unbiased cross-entropy, see "class-incremental" below; neither kOhem nor kWeighted): the first pass
+// also keeps the maximum over the old classes [0, c_old), the second their own sum of exp2 against it, and lse_old_out
+// gets lse_old per pixel; a pixel labelled with an old class scores lse - lse_old, one labelled with a new class
+// lse - v_t. Its arguments come last; the other instances do not read them.
+template <int Z, bool kOhem, bool kWeighted = false, bool kUnbiased = false>
 __global__ void __launch_bounds__(kFwdCols)
 upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs,
                        const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                        float* __restrict__ partial, long long* __restrict__ argmax_out, float* __restrict__ lse_out,
                        float* __restrict__ pt_out, float* __restrict__ nll_out,
-                       const float* __restrict__ class_weight = nullptr, float smoothing = 0.f) {
+                       const float* __restrict__ class_weight = nullptr, float smoothing = 0.f, int c_old = 0,
+                       float* __restrict__ lse_old_out = nullptr) {
+  static_assert(!(kUnbiased && (kOhem || kWeighted)), "the unbiased form is plain cross-entropy otherwise");
   using G = Zoom<Z>;
   constexpr int kFwdNodes = G::kNodes;
   constexpr bool kWeightedCE = kWeighted && !kOhem;
@@ -156,12 +166,15 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
     const float* Cc = A + kFwdNodes * Cs;      // node (i1, j0); not staged (and not read) at Z = 1
     const float* D = B + kFwdNodes * Cs;       // node (i1, j1)
     float m[Z], sum[Z];
+    float mo[Z], so[Z];  // kUnbiased: the old classes' own maximum and sum
     int am[Z];
 #pragma unroll
     for (int r = 0; r < Z; ++r) {
       m[r] = -INFINITY;
       am[r] = 0;
       sum[r] = 0.f;
+      mo[r] = 0.f;
+      so[r] = 0.f;
     }
 #pragma unroll 2
     for (int c = 0; c < C; ++c) {
@@ -174,6 +187,12 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
         if (v > m[r]) {
           m[r] = v;
           am[r] = c;
+        }
+      }
+      if constexpr (kUnbiased) {
+        if (c == c_old - 1) {   // classes run in order: the maximum so far is the old classes'
+#pragma unroll
+          for (int r = 0; r < Z; ++r) mo[r] = m[r];
         }
       }
     }
@@ -192,6 +211,9 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
         const float v = row_lerp<Z>(top, bot, r);
         sum[r] += ex2_approx(fmaf(v, kLog2e, -m2[r]));
         if constexpr (kWeightedCE) sw[r] = fmaf(s_w[c], m[r] - v, sw[r]);
+        if constexpr (kUnbiased) {
+          if (c < c_old) so[r] += ex2_approx(fmaf(v, kLog2e, -mo[r] * kLog2e));
+        }
       }
     }
 #pragma unroll
@@ -202,7 +224,15 @@ upsample_ce_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h
         const float lse = m[r] + __logf(sum[r]);
         if (argmax_out) argmax_out[pix] = am[r];
         lse_out[pix] = lse;
-        if (t != ignore_index && t >= 0 && t < C) {
+        float lse_old = 0.f;
+        if constexpr (kUnbiased) {
+          lse_old = mo[r] + __logf(so[r]);
+          lse_old_out[pix] = lse_old;
+        }
+        if (kUnbiased && t != ignore_index && t >= 0 && t < c_old) {
+          loss += lse - lse_old;   // an old-class label counts as background: every old class is the target
+          cnt += 1.f;
+        } else if (t != ignore_index && t >= 0 && t < C) {
           const int tc = static_cast<int>(t);
           const float top = Z == 1 ? A[tc] : l0w * A[tc] + l1w * B[tc];
           const float bot = Z == 1 ? 0.f : l0w * Cc[tc] + l1w * D[tc];
@@ -438,19 +468,23 @@ __device__ __forceinline__ float pix_grad(float p, int c, int t, const float* s_
   }
 }
 
-template <int Z, bool kOhem, bool kWeighted = false>
+// kUnbiased (neither kOhem nor kWeighted): a pixel labelled with an old class (t < c_old) is staged with t = C, which no
+// class matches, and its lse_old * log2(e) in a float array after the pixel words (12 bytes per pixel in all); the old
+// classes' threads subtract exp(v_c - lse_old) from its p_c - [c = t] = p_c.
+template <int Z, bool kOhem, bool kWeighted = false, bool kUnbiased = false>
 __global__ void __launch_bounds__(256)
 upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C,
                             const long long* __restrict__ target, int Ho, int Wo, int ignore_index,
                             const float* __restrict__ lse, float* __restrict__ T2, const float* __restrict__ pt,
                             const float* __restrict__ thr, const float* __restrict__ class_weight = nullptr,
-                            float smoothing = 0.f) {
+                            float smoothing = 0.f, int c_old = 0, const float* __restrict__ lse_old = nullptr) {
   using G = Zoom<Z>;
   extern __shared__ PixInfo s_pix[];  // [Z][Wo]
   const int i0 = blockIdx.x, n = blockIdx.y;
   const int i1 = min(i0 + 1, h - 1);
   const int rows = min(Z, Ho - Z * i0);
   float* s_w = reinterpret_cast<float*>(s_pix + Z * Wo);   // kWeighted: [C] class weights, then W
+  float* s_lso = s_w;                                      // kUnbiased: [Z][Wo] lse_old * log2(e)
   if constexpr (kWeighted) stage_class_weights(class_weight, C, s_w);
   float thr_v = 0.f;
   if constexpr (kOhem) thr_v = thr[0];
@@ -462,6 +496,10 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
       pi.t = (t == ignore_index || t < 0 || t >= C) ? -1 : static_cast<int>(t);
       if constexpr (kOhem) {
         if (!(pt[rowbase + x] < thr_v)) pi.t = -1;
+      }
+      if constexpr (kUnbiased) {
+        if (pi.t >= 0 && pi.t < c_old) pi.t = C;
+        s_lso[r * Wo + x] = lse_old[rowbase + x] * kLog2e;
       }
       pi.lse2 = lse[rowbase + x] * kLog2e;
       s_pix[r * Wo + x] = pi;
@@ -503,8 +541,10 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
           const PixInfo pi = s_pix[r * Wo + xb + k];
           if (pi.t < 0) continue;  // warp-uniform
           const float v = row_lerp<Z>(top, bot, r);
-          const float g =
-              pix_grad<kOhem, kWeighted>(ex2_approx(fmaf(v, kLog2e, -pi.lse2)), c, pi.t, s_w, k1, k2, gam);
+          float g = pix_grad<kOhem, kWeighted>(ex2_approx(fmaf(v, kLog2e, -pi.lse2)), c, pi.t, s_w, k1, k2, gam);
+          if constexpr (kUnbiased) {
+            if (c < c_old && pi.t == C) g -= ex2_approx(fmaf(v, kLog2e, -s_lso[r * Wo + xb + k]));
+          }
           g0 = fmaf(1.f - G::kStep * r, g, g0);
           g1 = fmaf(G::kStep * r, g, g1);
         }
@@ -524,8 +564,10 @@ upsample_ce_bwd_rows_kernel(const float* __restrict__ logits, int pitch, int N, 
           if (pi.t < 0) continue;
           const float l1h = G::kStep * r, l0h = 1.f - l1h;
           const float v = l0h * top + l1h * bot;
-          const float g =
-              pix_grad<kOhem, kWeighted>(ex2_approx(fmaf(v, kLog2e, -pi.lse2)), c, pi.t, s_w, k1, k2, gam);
+          float g = pix_grad<kOhem, kWeighted>(ex2_approx(fmaf(v, kLog2e, -pi.lse2)), c, pi.t, s_w, k1, k2, gam);
+          if constexpr (kUnbiased) {
+            if (c < c_old && pi.t == C) g -= ex2_approx(fmaf(v, kLog2e, -s_lso[r * Wo + xb + k]));
+          }
           g0 = fmaf(l0h, g, g0);
           g1 = fmaf(l1h, g, g1);
         }
@@ -1566,6 +1608,290 @@ upsample_kd_bwd_cols_kernel(const float* __restrict__ T2, int N, int h, int w, i
     float acc = own[idx];
     if (prev) acc += prev[idx];
     out[idx] = fmaf(acc, gs, out[idx]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- class-incremental
+// MiB's background-aware losses (Cermelli et al., CVPR 2020) for a student of C classes and the previous step's network,
+// the teacher, of C_old < C: class 0 is the background, [0, C_old) the old classes, [C_old, C) the new ones, and
+// lse_A(x) = log sum_{c in A} exp(x_c), each subset's sum taken against its own maximum, so a confidently new-class
+// pixel labelled background scores a large finite loss, not inf.
+// Unbiased cross-entropy: the kUnbiased instances of the plain forward and rows kernels (above) with the plain reduce and
+// cols kernels. Per valid pixel, l = lse_all(s) - lse_old(s) for a label t < C_old (an old label counts as background),
+// lse_all(s) - s_t otherwise; dl/ds_c = p_c - [t < C_old][c < C_old] exp(s_c - lse_old) - [t >= C_old][c = t].
+// Unbiased distillation, every pixel (no target), q = softmax(alpha t) over the C_old teacher classes and
+// B = {0} u [C_old, C):
+//   k = -(1/C_old) [ q_0 (lse_B(s) - lse_all(s)) + sum_{c=1}^{C_old-1} q_c (s_c - lse_all(s)) ],   KD = mean of k
+//   dk/ds_c = (p_c - q_0 exp(s_c - lse_B)) / C_old for c in B,   (p_c - q_c) / C_old for 1 <= c < C_old
+//   forward : the distillation forward's layout (KdGeom, both maps' node rows staged side by side; the teacher's C_old
+//             channels at the student's stride), three class passes per pixel (the maxima of s over all classes and
+//             over B and of t; the three sums; the terms), one (sum k, pixels) partial per CTA and the plain fp64
+//             reduce; (lse_all(s), lse_B(s), lse(alpha t)) saved per pixel.
+//   backward: the distillation rows layout with those three words log2(e) staged per pixel (12 bytes: the Dice width
+//             limit), a thread of a class in B reading the teacher's class 0; then the distillation cols kernel, which
+//             ADDS into dlogits.
+struct UnkdPix {
+  float all2, b2, t2;   // lse_all(s), lse_B(s), lse(alpha t), times log2(e)
+};
+
+template <int Z>
+__device__ __forceinline__ void node_pair(const float* A, const float* B, const float* Cc, const float* D, int c,
+                                          float l0w, float l1w, float& top, float& bot) {
+  top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+  bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+}
+
+template <int Z>
+__global__ void __launch_bounds__(KdGeom<Z>::kCols)
+upsample_unkd_fwd_kernel(const float* __restrict__ sl, int pitch_s, const float* __restrict__ tl, int pitch_t, int N,
+                         int h, int w, int C, int c_old, int Cs, int Ho, int Wo, float alpha,
+                         float* __restrict__ partial, float* __restrict__ lse_out) {
+  using G = Zoom<Z>;
+  constexpr int kCols = KdGeom<Z>::kCols, kNodes = KdGeom<Z>::kNodes;
+  extern __shared__ float S[];  // [2 maps: student (C), teacher (c_old)][kNodeRows][kNodes][Cs]
+  __shared__ float red_k[kCols / 32];
+  __shared__ float red_cnt[kCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kNodes, w - j_base);
+  const int tid = threadIdx.x;
+  const int map_floats = G::kNodeRows * kNodes * Cs;
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    const size_t src = (static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj);
+    S[(rr * kNodes + jj) * Cs + c] = sl[src * pitch_s + c];
+  }
+  for (int idx = tid; idx < G::kNodeRows * nj * c_old; idx += kCols) {
+    const int c = idx % c_old;
+    const int node = idx / c_old;
+    const int jj = node % nj, rr = node / nj;
+    const size_t src = (static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj);
+    S[map_floats + (rr * kNodes + jj) * Cs + c] = tl[src * pitch_t + c];
+  }
+  __syncthreads();
+  float k_sum = 0.f, cnt = 0.f;
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* As = S + (j0 - j_base) * Cs;   // student nodes (i0, j0), (i0, j1), (i1, j0), (i1, j1)
+    const float* Bs = S + (j1 - j_base) * Cs;
+    const float* Cs_ = As + kNodes * Cs;
+    const float* Ds = Bs + kNodes * Cs;
+    const float* At = As + map_floats;           // teacher nodes
+    const float* Bt = Bs + map_floats;
+    const float* Ct = Cs_ + map_floats;
+    const float* Dt = Ds + map_floats;
+    const float ka = alpha * kLog2e;
+    float ms[Z], mb[Z], mt[Z], zs[Z], zb[Z], zt[Z], acc[Z];
+    float ts, bs, tt, bt;
+    node_pair<Z>(As, Bs, Cs_, Ds, 0, l0w, l1w, ts, bs);
+    node_pair<Z>(At, Bt, Ct, Dt, 0, l0w, l1w, tt, bt);
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      ms[r] = mb[r] = row_lerp<Z>(ts, bs, r);
+      mt[r] = row_lerp<Z>(tt, bt, r);
+      zs[r] = zb[r] = zt[r] = acc[r] = 0.f;
+    }
+    // pass 1: the maxima (class 0 above; the old classes; the new classes, which are in B)
+#pragma unroll 2
+    for (int c = 1; c < c_old; ++c) {
+      node_pair<Z>(As, Bs, Cs_, Ds, c, l0w, l1w, ts, bs);
+      node_pair<Z>(At, Bt, Ct, Dt, c, l0w, l1w, tt, bt);
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        ms[r] = fmaxf(ms[r], row_lerp<Z>(ts, bs, r));
+        mt[r] = fmaxf(mt[r], row_lerp<Z>(tt, bt, r));
+      }
+    }
+#pragma unroll 2
+    for (int c = c_old; c < C; ++c) {
+      node_pair<Z>(As, Bs, Cs_, Ds, c, l0w, l1w, ts, bs);
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(ts, bs, r);
+        ms[r] = fmaxf(ms[r], v);
+        mb[r] = fmaxf(mb[r], v);
+      }
+    }
+    // pass 2: the sums, each against its own maximum
+    node_pair<Z>(As, Bs, Cs_, Ds, 0, l0w, l1w, ts, bs);
+#pragma unroll
+    for (int r = 0; r < Z; ++r) zb[r] = ex2_approx((row_lerp<Z>(ts, bs, r) - mb[r]) * kLog2e);
+#pragma unroll 2
+    for (int c = 0; c < c_old; ++c) {
+      node_pair<Z>(As, Bs, Cs_, Ds, c, l0w, l1w, ts, bs);
+      node_pair<Z>(At, Bt, Ct, Dt, c, l0w, l1w, tt, bt);
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        zs[r] += ex2_approx((row_lerp<Z>(ts, bs, r) - ms[r]) * kLog2e);
+        zt[r] += ex2_approx((row_lerp<Z>(tt, bt, r) - mt[r]) * ka);
+      }
+    }
+#pragma unroll 2
+    for (int c = c_old; c < C; ++c) {
+      node_pair<Z>(As, Bs, Cs_, Ds, c, l0w, l1w, ts, bs);
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(ts, bs, r);
+        zs[r] += ex2_approx((v - ms[r]) * kLog2e);
+        zb[r] += ex2_approx((v - mb[r]) * kLog2e);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      zs[r] = logf(zs[r]);   // log sums from here on
+      zb[r] = logf(zb[r]);
+      zt[r] = logf(zt[r]);
+    }
+    // pass 3: q_0 (lse_B - lse_all) + sum_{c >= 1} q_c (s_c - lse_all), log q_c = alpha (t_c - m_t) - log z_t
+    node_pair<Z>(At, Bt, Ct, Dt, 0, l0w, l1w, tt, bt);
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      const float q0 = ex2_approx(((row_lerp<Z>(tt, bt, r) - mt[r]) * alpha - zt[r]) * kLog2e);
+      acc[r] = q0 * ((mb[r] - ms[r]) + (zb[r] - zs[r]));
+    }
+#pragma unroll 2
+    for (int c = 1; c < c_old; ++c) {
+      node_pair<Z>(As, Bs, Cs_, Ds, c, l0w, l1w, ts, bs);
+      node_pair<Z>(At, Bt, Ct, Dt, c, l0w, l1w, tt, bt);
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float q = ex2_approx(((row_lerp<Z>(tt, bt, r) - mt[r]) * alpha - zt[r]) * kLog2e);
+        acc[r] = fmaf(q, (row_lerp<Z>(ts, bs, r) - ms[r]) - zs[r], acc[r]);
+      }
+    }
+    const float inv_old = 1.f / static_cast<float>(c_old);
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo + x;
+        lse_out[3 * pix + 0] = ms[r] + zs[r];
+        lse_out[3 * pix + 1] = mb[r] + zb[r];
+        lse_out[3 * pix + 2] = fmaf(mt[r], alpha, zt[r]);
+        k_sum -= acc[r] * inv_old;
+        cnt += 1.f;
+      }
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    k_sum += __shfl_xor_sync(0xffffffffu, k_sum, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((tid & 31) == 0) {
+    red_k[tid >> 5] = k_sum;
+    red_cnt[tid >> 5] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float l = 0.f, k = 0.f;
+    for (int i = 0; i < kCols / 32; ++i) {
+      l += red_k[i];
+      k += red_cnt[i];
+    }
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[2 * b] = l;
+    partial[2 * b + 1] = k;
+  }
+}
+
+// One interval of the unbiased distillation rows kernel for class c (kd_interval's structure): acc = the (left, right) x
+// (top, bottom node row) sums of p_c - q_0 exp(s_c - lse_B) (in_b) or p_c - q_c, the teacher values those of class 0
+// (in_b) or c.
+template <int Z, bool kFull>
+__device__ __forceinline__ void unkd_interval(const UnkdPix* s, int Wo, int xb, int rows, int nx, float ka, bool in_b,
+                                              float a, float b, float cc, float d, float at, float bt, float ct,
+                                              float dt, float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    const float topt = l0w * at + l1w * bt;
+    const float bott = l0w * ct + l1w * dt;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const UnkdPix u = s[r * Wo + xb + k];
+      const float v = row_lerp<Z>(top, bot, r);
+      const float p = ex2_approx(fmaf(v, kLog2e, -u.all2));
+      const float q = ex2_approx(fmaf(row_lerp<Z>(topt, bott, r), ka, -u.t2));
+      const float g = in_b ? fmaf(-q, ex2_approx(fmaf(v, kLog2e, -u.b2)), p) : p - q;
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+// One CTA per (low-res interval row i0, image), one thread per student class; out = T2[n][i0][2][w][C] of C_old dk/ds_c.
+template <int Z>
+__global__ void __launch_bounds__(256)
+upsample_unkd_bwd_rows_kernel(const float* __restrict__ sl, int pitch_s, const float* __restrict__ tl, int pitch_t,
+                              int N, int h, int w, int C, int c_old, int Ho, int Wo, float alpha,
+                              const float* __restrict__ lse, float* __restrict__ T2) {
+  extern __shared__ UnkdPix s_upix[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  for (int r = 0; r < rows; ++r) {
+    const size_t rowbase = (static_cast<size_t>(n) * Ho + (Z * i0 + r)) * Wo;
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const float* l = lse + 3 * (rowbase + x);
+      s_upix[r * Wo + x] = UnkdPix{l[0] * kLog2e, l[1] * kLog2e, l[2] * kLog2e};
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const bool in_b = c == 0 || c >= c_old;
+  const int tc = in_b ? 0 : c;
+  const float ka = alpha * kLog2e;
+  const float* S0 = sl + (static_cast<size_t>(n) * h + i0) * w * pitch_s + c;
+  const float* S1 = sl + (static_cast<size_t>(n) * h + i1) * w * pitch_s + c;
+  const float* U0 = tl + (static_cast<size_t>(n) * h + i0) * w * pitch_t + tc;
+  const float* U1 = tl + (static_cast<size_t>(n) * h + i1) * w * pitch_t + tc;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  const int j1 = min(1, w - 1);
+  float a = S0[0], cc = S1[0], at = U0[0], ct = U1[0];   // left node column of the current interval
+  float nb = S0[static_cast<size_t>(j1) * pitch_s], nd = S1[static_cast<size_t>(j1) * pitch_s];
+  float nbt = U0[static_cast<size_t>(j1) * pitch_t], ndt = U1[static_cast<size_t>(j1) * pitch_t];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd, bt = nbt, dt = ndt;
+    const int jn = min(j0 + 2, w - 1);
+    nb = S0[static_cast<size_t>(jn) * pitch_s];
+    nd = S1[static_cast<size_t>(jn) * pitch_s];
+    nbt = U0[static_cast<size_t>(jn) * pitch_t];
+    ndt = U1[static_cast<size_t>(jn) * pitch_t];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      unkd_interval<Z, true>(s_upix, Wo, xb, rows, nx, ka, in_b, a, b, cc, d, at, bt, ct, dt, acc);
+    } else {
+      unkd_interval<Z, false>(s_upix, Wo, xb, rows, nx, ka, in_b, a, b, cc, d, at, bt, ct, dt, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+    at = bt;
+    ct = dt;
   }
 }
 
@@ -3973,6 +4299,218 @@ extern "C" int semseg_upsample_kd_bwd(const float* student, int pitch_s, const f
                                     lse, grad_out, workspace, dlogits, stream);
     default: return launch_kd_bwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, Ho, Wo, temperature, kd_weight,
                                      lse, grad_out, workspace, dlogits, stream);
+  }
+}
+
+// Class-incremental (MiB) losses at zoom factor `zoom`. Both backward rows kernels stage 12 bytes per pixel of the
+// interval's Z output rows in kDiceSmemMax: the Dice width limit, Wo <= 2389 at zoom 8.
+static int check_incremental(int C, int c_old, int zoom, int Wo) {
+  SB_CHECK_ARG(c_old >= 2 && c_old < C, "upsample_incremental: C_old = %d must lie in [2, C = %d)", c_old, C);
+  const size_t max_wo = kDiceSmemMax / (static_cast<size_t>(zoom) * 12);
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_incremental: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_unbiased_fwd(const float* logits, int pitch, int N, int h, int w, int C, int c_old,
+                               const int64_t* target, int Ho, int Wo, int ignore_index, float* workspace,
+                               float* loss_out, int64_t* argmax, float* lse, float* lse_old, cudaStream_t stream) {
+  const int Cs = C | 1;
+  constexpr size_t kMaxSmem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_fwd_kernel<Z, false, false, true>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_ce_fwd_kernel<Z, false, false, true><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, workspace,
+      reinterpret_cast<long long*>(argmax), lse, nullptr, nullptr, nullptr, 0.f, c_old, lse_old);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_unbiased_bwd(const float* logits, int pitch, int N, int h, int w, int C, int c_old,
+                               const int64_t* target, int Ho, int Wo, int ignore_index, const float* lse,
+                               const float* lse_old, const float* loss_info, const float* grad_out, float* workspace,
+                               float* dlogits, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * (sizeof(PixInfo) + sizeof(float));
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_ce_bwd_rows_kernel<Z, false, false, true>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  upsample_ce_bwd_rows_kernel<Z, false, false, true><<<dim3(h, N), threads, smem, stream>>>(
+      logits, pitch, N, h, w, C, reinterpret_cast<const long long*>(target), Ho, Wo, ignore_index, lse, workspace,
+      nullptr, nullptr, nullptr, 0.f, c_old, lse_old);
+  SB_LAUNCHED();
+  upsample_ce_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_unbiased_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  return semseg_upsample_ce_zoom_workspace_floats(N, Ho, Wo, zoom);
+}
+
+extern "C" int semseg_upsample_ce_unbiased_fwd(const float* logits, int pitch, int N, int h, int w, int C, int c_old,
+                                               const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                               float* workspace, float* loss_out, int64_t* argmax, float* lse,
+                                               float* lse_old, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_incremental(C, c_old, zoom, Wo);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && lse_old, "upsample_ce_unbiased_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_unbiased_fwd<1>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, workspace,
+                                          loss_out, argmax, lse, lse_old, stream);
+    case 2: return launch_unbiased_fwd<2>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, workspace,
+                                          loss_out, argmax, lse, lse_old, stream);
+    case 4: return launch_unbiased_fwd<4>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, workspace,
+                                          loss_out, argmax, lse, lse_old, stream);
+    default: return launch_unbiased_fwd<8>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, workspace,
+                                           loss_out, argmax, lse, lse_old, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_unbiased_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_ce_unbiased_bwd(const float* logits, int pitch, int N, int h, int w, int C, int c_old,
+                                               const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                               const float* lse, const float* lse_old, const float* loss_info,
+                                               const float* grad_out, float* workspace, float* dlogits,
+                                               void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_incremental(C, c_old, zoom, Wo);
+  if (r) return r;
+  SB_CHECK_ARG(lse && lse_old && loss_info && grad_out && dlogits && workspace, "upsample_ce_unbiased_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_unbiased_bwd<1>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, lse, lse_old,
+                                          loss_info, grad_out, workspace, dlogits, stream);
+    case 2: return launch_unbiased_bwd<2>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, lse, lse_old,
+                                          loss_info, grad_out, workspace, dlogits, stream);
+    case 4: return launch_unbiased_bwd<4>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, lse, lse_old,
+                                          loss_info, grad_out, workspace, dlogits, stream);
+    default: return launch_unbiased_bwd<8>(logits, pitch, N, h, w, C, c_old, target, Ho, Wo, ignore_index, lse,
+                                           lse_old, loss_info, grad_out, workspace, dlogits, stream);
+  }
+}
+
+static int check_unkd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w, int C,
+                      int c_old, int Ho, int Wo, int zoom, float alpha) {
+  SB_CHECK_ARG(valid_zoom(zoom), "upsample_unkd: zoom %d is not one of 1, 2, 4, 8", zoom);
+  SB_CHECK_ARG(student && teacher, "upsample_unkd: null pointer");
+  SB_CHECK_ARG(N > 0 && h > 1 && w > 1 && C > 1 && C <= kMaxClasses, "upsample_unkd: bad sizes (C<=%d)", kMaxClasses);
+  SB_CHECK_ARG(pitch_s >= C && pitch_t >= c_old, "upsample_unkd: pitch %d / %d below C = %d / C_old = %d", pitch_s,
+               pitch_t, C, c_old);
+  SB_CHECK_ARG(Ho == zoom * (h - 1) + 1 && Wo == zoom * (w - 1) + 1,
+               "upsample_unkd: needs Ho=%d(h-1)+1, Wo=%d(w-1)+1 (got %dx%d -> %dx%d)", zoom, zoom, h, w, Ho, Wo);
+  SB_CHECK_ARG(std::isfinite(alpha) && alpha > 0.f, "upsample_unkd: alpha %g is not finite and > 0", alpha);
+  return check_incremental(C, c_old, zoom, Wo);
+}
+
+template <int Z>
+static int launch_unkd_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                           int C, int c_old, int Ho, int Wo, float alpha, float* workspace, float* loss_out,
+                           float* lse, cudaStream_t stream) {
+  using K = KdGeom<Z>;
+  const int Cs = C | 1;
+  // the distillation forward's shared memory: two maps at the student's stride
+  constexpr size_t kMaxSmem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = 2ull * Zoom<Z>::kNodeRows * K::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_unkd_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_unkd_fwd_kernel<Z><<<dim3(cdiv(Wo, K::kCols), h, N), K::kCols, smem, stream>>>(
+      student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Cs, Ho, Wo, alpha, workspace, lse);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<<<1, 256, 0, stream>>>(workspace, kd_fwd_ctas<Z>(N, h, Wo), loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_unkd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N, int h, int w,
+                           int C, int c_old, int Ho, int Wo, float alpha, float kd_weight, const float* lse,
+                           const float* grad_out, float* workspace, float* dlogits, cudaStream_t stream) {
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(UnkdPix);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_unkd_bwd_rows_kernel<Z>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  upsample_unkd_bwd_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(student, pitch_s, teacher, pitch_t, N, h, w,
+                                                                          C, c_old, Ho, Wo, alpha, lse, workspace);
+  SB_LAUNCHED();
+  // d(kd_weight KD)/ds_c = kd_weight (C_old dk/ds_c) / (C_old P)
+  const double P = static_cast<double>(N) * Ho * Wo;
+  const float scale = static_cast<float>(static_cast<double>(kd_weight) / (static_cast<double>(c_old) * P));
+  upsample_kd_bwd_cols_kernel<<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, scale, grad_out, dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_unkd_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  return semseg_upsample_kd_workspace_floats(N, Ho, Wo, zoom);
+}
+
+extern "C" int semseg_upsample_unkd_fwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N,
+                                        int h, int w, int C, int c_old, int Ho, int Wo, int zoom, float alpha,
+                                        float* workspace, float* loss_out, float* lse, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_unkd(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, zoom, alpha);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse, "upsample_unkd_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_unkd_fwd<1>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, workspace,
+                                      loss_out, lse, stream);
+    case 2: return launch_unkd_fwd<2>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, workspace,
+                                      loss_out, lse, stream);
+    case 4: return launch_unkd_fwd<4>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, workspace,
+                                      loss_out, lse, stream);
+    default: return launch_unkd_fwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, workspace,
+                                       loss_out, lse, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_unkd_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  return semseg_upsample_kd_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_unkd_bwd(const float* student, int pitch_s, const float* teacher, int pitch_t, int N,
+                                        int h, int w, int C, int c_old, int Ho, int Wo, int zoom, float alpha,
+                                        float kd_weight, const float* lse, const float* grad_out, float* workspace,
+                                        float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_unkd(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, zoom, alpha);
+  if (r) return r;
+  SB_CHECK_ARG(std::isfinite(kd_weight) && kd_weight >= 0.f, "upsample_unkd_bwd: kd_weight %g is not finite and >= 0",
+               kd_weight);
+  SB_CHECK_ARG(lse && grad_out && workspace && dlogits, "upsample_unkd_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_unkd_bwd<1>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, kd_weight,
+                                      lse, grad_out, workspace, dlogits, stream);
+    case 2: return launch_unkd_bwd<2>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, kd_weight,
+                                      lse, grad_out, workspace, dlogits, stream);
+    case 4: return launch_unkd_bwd<4>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha, kd_weight,
+                                      lse, grad_out, workspace, dlogits, stream);
+    default: return launch_unkd_bwd<8>(student, pitch_s, teacher, pitch_t, N, h, w, C, c_old, Ho, Wo, alpha,
+                                       kd_weight, lse, grad_out, workspace, dlogits, stream);
   }
 }
 

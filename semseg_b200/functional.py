@@ -812,6 +812,38 @@ class _UpsampleCEKD(torch.autograd.Function):
         return dl, None, None, None, None, None, None, None, None
 
 
+class _UpsampleCEIncremental(torch.autograd.Function):
+    """The fused tail with losses.IncrementalLoss: ce_weight * the unbiased CE (the kUnbiased forward, at zoom `zoom`)
+    plus, with the previous step's logits `teacher_logits` (C_old classes) and kd_weight > 0, kd_weight * the unbiased
+    distillation (at zoom `kd_zoom`: the model's zoom, or 1 on the 1/8-resolution maps). Without teacher logits it is
+    the unbiased CE alone (the aux head's loss). The backward writes the CE gradient and the distillation kernels add
+    theirs into the same buffer. The teacher map is a constant: it gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, teacher_logits, target, ignore_index, zoom, kd_zoom, c_old, alpha, kd_weight, ce_weight):
+        info, amax, lse, lse_old = ops.upsample_ce_unbiased_fwd(logits, target, ignore_index, c_old, zoom=zoom)
+        kd = teacher_logits is not None and kd_weight > 0.0
+        ctx.mark_non_differentiable(amax)
+        ctx.cfg = (ignore_index, zoom, kd_zoom, c_old, alpha, kd_weight, ce_weight, kd)
+        if not kd:
+            ctx.save_for_backward(logits, target, lse, lse_old, info)
+            return (info[0] if ce_weight == 1.0 else info[0] * ce_weight), amax
+        kd_info, lse_kd = ops.upsample_unkd_fwd(logits, teacher_logits, alpha, zoom=kd_zoom)
+        ctx.save_for_backward(logits, target, lse, lse_old, info, teacher_logits, lse_kd)
+        return torch.add(info[0] * ce_weight, kd_info[0], alpha=kd_weight), amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        ignore_index, zoom, kd_zoom, c_old, alpha, kd_weight, ce_weight, kd = ctx.cfg
+        logits, target, lse, lse_old, info = ctx.saved_tensors[:5]
+        g = grad_loss if ce_weight == 1.0 else grad_loss * ce_weight
+        dl = ops.upsample_ce_unbiased_bwd(logits, target, ignore_index, c_old, lse, lse_old, info, g, zoom=zoom)
+        if kd:
+            teacher_logits, lse_kd = ctx.saved_tensors[5:]
+            ops.upsample_unkd_bwd(logits, teacher_logits, alpha, kd_weight, lse_kd, grad_loss, dl, zoom=kd_zoom)
+        return dl, None, None, None, None, None, None, None, None, None
+
+
 class _UpsampleCEPL(torch.autograd.Function):
     """The fused tail with losses.PseudoLabelLoss: ce_weight * CE over the labelled pixels plus pl_weight * the
     confidence-masked pseudo-label CE over the unlabelled ones. The forward keeps each pixel's effective target and
@@ -939,7 +971,8 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
     form's conditions, and so does losses.AdversarialLoss (plain cross-entropy on the attacked batch; the attack checks
     its own tail's limits); losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
-    losses.EntropyLoss, whose rows kernel stages the same words, the Dice width limit. losses.RMILoss needs a target of
+    losses.EntropyLoss, whose rows kernel stages the same words, and losses.IncrementalLoss, whose unbiased CE and
+    distillation rows kernels stage as many bytes per pixel, the Dice width limit. losses.RMILoss needs a target of
     at least 12 x 12 and no wider than its rows kernel stages (3584 columns
     at zoom 8). losses.GatedCRFLoss and losses.ActiveBoundaryLoss need the target no wider than the plain backward
     stages (2560 columns at zoom 8); their classes (<= 256, checked here with the logits) and options are in the
@@ -963,6 +996,10 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         # the kernels' limits
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _CRF_CE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _CRF_CE_STAGE_BYTES)
+    elif type(criterion) is losses.IncrementalLoss:
+        # the unbiased CE and distillation rows kernels stage 12 bytes per pixel, the Dice words' size, in the same 224 KB
+        ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
+              _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     elif type(criterion) is losses.RMILoss:
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               target.shape[1] >= _RMI_MIN_SIZE and target.shape[2] >= _RMI_MIN_SIZE and
@@ -1006,8 +1043,10 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     head with the plain form. With a losses.GatedCRFLoss and the network's fp32 NCHW input `image` (a constant),
     ce_weight * CE plus crf_weight * its Gated CRF term; `image_stride` is the image's pixel stride on the loss grid
     (default: 8 / zoom at at='output', 8 at at='logits'); without an image a positive crf_weight raises. With a
-    losses.ActiveBoundaryLoss, ce_weight * CE plus abl_weight * its boundary term on the output grid. The default
-    criterion runs the plain kernels."""
+    losses.ActiveBoundaryLoss, ce_weight * CE plus abl_weight * its boundary term on the output grid. With a
+    losses.IncrementalLoss and the previous step's fp32 NHWC logits `teacher_logits` ([N, h, w, C_old]), ce_weight *
+    its unbiased CE plus kd_weight * its unbiased distillation; without them the unbiased CE alone (the aux head's
+    loss). The default criterion runs the plain kernels."""
     if isinstance(criterion, losses.ActiveBoundaryLoss):
         if criterion.abl_weight == 0.0:
             # no ABL kernel: the plain step, bit for bit when ce_weight is 1
@@ -1031,6 +1070,12 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
         return _UpsampleCEPLMix.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,
                                       int(zoom), criterion.threshold, criterion.pl_weight, criterion.ce_weight,
                                       mix_mask)
+    if isinstance(criterion, losses.IncrementalLoss):
+        kd_zoom = 1 if criterion.at == 'logits' else int(zoom)
+        t = None if teacher_logits is None else teacher_logits.detach()
+        ce_weight = 1.0 if t is None else criterion.ce_weight
+        return _UpsampleCEIncremental.apply(logits, t, target.contiguous(), criterion.ignore_index, int(zoom), kd_zoom,
+                                            criterion.c_old, criterion.alpha, criterion.kd_weight, ce_weight)
     if isinstance(criterion, losses.DistillationLoss) and teacher_logits is not None:
         kd_zoom = 1 if criterion.at == 'logits' else int(zoom)
         return _UpsampleCEKD.apply(logits, teacher_logits.detach(), target.contiguous(), criterion.ignore_index,

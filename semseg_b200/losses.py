@@ -19,7 +19,9 @@ the student then learns on a strongly perturbed view of the batch the teacher se
 channel-dropped layer4 features that learns the same pseudo-labels, and `streams=2`: UniMatch's dual-stream
 perturbation, two strong views of every image, each with its own draws, in one student pass. AdversarialLoss is PGD
 adversarial training: an adversarial.PGDAttack runs on the network inside its training forward and both heads learn
-plain cross-entropy on the attacked batch.
+plain cross-entropy on the attacked batch. IncrementalLoss is class-incremental training with MiB's unbiased
+cross-entropy and unbiased distillation from the previous step's network, whose classifier has fewer classes
+(incremental.expand_classifier grows the student's).
 """
 import math
 
@@ -486,6 +488,8 @@ class _TeacherLoss(nn.Module):
     with requires_grad raises. strong=None changes nothing."""
 
     graph_options = ("ignore_index",)
+    # True where the teacher is the previous step of class-incremental training: it has fewer classes than the student
+    _teacher_has_fewer_classes = False
 
     def __init__(self, teacher, ignore_index, strong=None):
         super(_TeacherLoss, self).__init__()
@@ -564,7 +568,11 @@ class _TeacherLoss(nn.Module):
             raise RuntimeError("%s: the teacher is on %s, the input on %s (move the teacher yourself)" %
                                (name, dev, x.device))
         tc = teacher.cls[4].out_channels
-        if tc != classes:
+        if self._teacher_has_fewer_classes:
+            if not tc < classes:
+                raise ValueError("%s: the teacher has %d classes, the student %d; the student must have more" %
+                                 (name, tc, classes))
+        elif tc != classes:
             raise ValueError("%s: the teacher has %d classes, the student %d" % (name, tc, classes))
         if getattr(teacher, "_sb_ema_shadow", False):
             # a mean teacher changes every step: its slabs are re-packed here, inside the captured step while capturing
@@ -692,6 +700,87 @@ class DistillationLoss(_TeacherLoss):
             loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1)
             return loss
         t = self._teacher_logits_nhwc(logits, teacher_logits)
+        loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self, teacher_logits=t)
+        return loss
+
+
+class IncrementalLoss(_TeacherLoss):
+    """Class-incremental training with MiB's background-aware losses (Cermelli et al., "Modeling the Background for
+    Incremental Learning in Semantic Segmentation", CVPR 2020). The teacher is the network of the previous step, with
+    C_old classes; the student is its copy grown to C > C_old classes by incremental.expand_classifier. Class 0 is the
+    background, [0, C_old) the old classes, [C_old, C) the new ones. With s the student's logits, t the teacher's,
+    lse_A(x) = log sum_{c in A} exp(x_c) (each subset's sum against its own maximum) and B = {0} u [C_old, C):
+
+        CE_u : per valid pixel (target != ignore_index, 0 <= target < C), lse_all(s) - lse_old(s) for a target below
+               C_old (the old classes, which step's data labels as background, count as background) and
+               lse_all(s) - s_target otherwise; the mean over the valid pixels (0 with a zero gradient when none is)
+        KD_u : per pixel (every pixel, no target), with q = softmax(alpha * t) over the C_old teacher classes,
+               -(1/C_old) [ q_0 (lse_B(s) - lse_all(s)) + sum_{c=1}^{C_old-1} q_c (s_c - lse_all(s)) ]; the mean
+        main = ce_weight * CE_u + kd_weight * KD_u
+        aux  = CE_u of the aux head (ce_weight does not scale it)
+
+    at='output': KD_u on both maps after the same bilinear xZ upsample (align_corners) that the CE term uses (MiB's
+    choice); at='logits': on the raw 1/8-resolution maps. kd_weight = 0 runs no distillation kernel (MiB's "UNCE only"
+    ablation). The default kd_weight = 10 is MiB's Pascal VOC value; the right value depends on the benchmark (MiB uses
+    100 on ADE20K). Labels of classes the student does not have yet must be remapped to 0 in the data: the criterion
+    does not see them.
+
+    `teacher` is a frozen PSPNet or PSANet of this package with fewer classes than the student (C_old is read from its
+    cls[4]), with the other rules of _TeacherLoss (eval mode, the input's device; held outside the module tree; never
+    modified). Under DistributedDataParallel each rank holds its own teacher and averages over its own pixels.
+
+    With the network's fused tail (functional.upsample_ce) both terms run inside the tail's kernels, teacher forward
+    included, graphed at every zoom factor. Called as a module, forward(logits, target, teacher_logits=None) takes
+    NCHW logits at the target size: without teacher_logits it returns CE_u (the aux head's loss, and the validation
+    loss validate() logs), with them ([N, C_old, H, W]) `main` at that size. It runs the zoom-1 kernels on NHWC copies.
+    CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
+
+    graph_options = _TeacherLoss.graph_options + ("kd_weight", "alpha", "ce_weight", "at")
+    _teacher_has_fewer_classes = True
+
+    def __init__(self, teacher, kd_weight=10.0, alpha=1.0, ce_weight=1.0, ignore_index=255, at='output'):
+        super(IncrementalLoss, self).__init__(teacher, ignore_index)
+        if not isinstance(at, str):
+            raise TypeError("at must be 'output' or 'logits', got %r" % (at,))
+        if at not in ('output', 'logits'):
+            raise ValueError("at must be 'output' or 'logits', got %r" % (at,))
+        alpha = _non_negative("alpha", alpha)
+        if alpha <= 0.0:
+            raise ValueError("alpha must be > 0, got %r" % alpha)
+        self.alpha = alpha
+        self.kd_weight = _non_negative("kd_weight", kd_weight)
+        self.ce_weight = _non_negative("ce_weight", ce_weight)
+        self.at = at
+        if not 2 <= self.c_old < 256:
+            raise ValueError("IncrementalLoss: the teacher has %d classes; it needs 2 to 255" % self.c_old)
+
+    @property
+    def c_old(self):
+        """The teacher's number of classes: the old classes are [0, c_old)."""
+        return self.teacher.cls[4].out_channels
+
+    def extra_repr(self):
+        return "teacher=%s (%d classes), kd_weight=%g, alpha=%g, ce_weight=%g, ignore_index=%d, at=%r" % (
+            type(self.teacher).__name__, self.c_old, self.kd_weight, self.alpha, self.ce_weight, self.ignore_index,
+            self.at)
+
+    def forward(self, logits, target, teacher_logits=None):
+        from . import functional as SF
+        if logits.dim() == 4 and not self.c_old < logits.shape[1]:
+            raise ValueError("IncrementalLoss: the teacher has %d classes, the student %d; the student must have more" %
+                             (self.c_old, logits.shape[1]))
+        _check_native_logits("IncrementalLoss", logits, target)
+        s = logits.permute(0, 2, 3, 1).contiguous()
+        if teacher_logits is None:
+            loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self)
+            return loss
+        want = logits.shape[:1] + (self.c_old,) + logits.shape[2:]
+        if teacher_logits.shape != want or teacher_logits.dtype != torch.float32 or \
+                teacher_logits.device != logits.device:
+            raise ValueError("IncrementalLoss: teacher_logits must be fp32 %s on %s, got %s %s on %s" %
+                             (tuple(want), logits.device, teacher_logits.dtype, tuple(teacher_logits.shape),
+                              teacher_logits.device))
+        t = teacher_logits.detach().permute(0, 2, 3, 1).contiguous()
         loss, _ = SF.upsample_ce(s, target, self.ignore_index, 1, criterion=self, teacher_logits=t)
         return loss
 

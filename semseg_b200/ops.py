@@ -1092,6 +1092,87 @@ def adv_start(x0, u, box, out=None):
     return out
 
 
+def upsample_ce_unbiased_fwd(logits, target, ignore_index, c_old, want_argmax=True, zoom=8):
+    """MiB's unbiased cross-entropy on the fused tail (include/semseg_b200.h states the contract); arguments as
+    upsample_ce_fwd plus the teacher's class count `c_old` -> (loss_info [2] = (loss, n_valid), argmax, lse, lse_old)."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_unbiased_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_unbiased_workspace_floats")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse, lse_old = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
+    _lib.check(lib.semseg_upsample_ce_unbiased_fwd(_ptr(logits), logits.stride(2), n, h, w, c, int(c_old),
+                                                   _ptr(target), ho, wo, int(zoom), int(ignore_index), _ptr(ws),
+                                                   _ptr(info), _ptr(amax), _ptr(lse), _ptr(lse_old), _stream()),
+               "semseg_upsample_ce_unbiased_fwd")
+    return info, amax, lse, lse_old
+
+
+def upsample_ce_unbiased_bwd(logits, target, ignore_index, c_old, lse, lse_old, info, grad_out, zoom=8):
+    """dlogits fp32 [N,h,w,C] (dense) = grad_out * d(unbiased CE)/dlogits from the forward's lse, lse_old and info."""
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_unbiased_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_unbiased_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_unbiased_bwd(_ptr(logits), logits.stride(2), n, h, w, c, int(c_old),
+                                                   _ptr(target), ho, wo, int(zoom), int(ignore_index), _ptr(lse),
+                                                   _ptr(lse_old), _ptr(info), _ptr(g), _ptr(ws), _ptr(dl), _stream()),
+               "semseg_upsample_ce_unbiased_bwd")
+    return dl
+
+
+def upsample_unkd_fwd(student, teacher, alpha, zoom=8):
+    """MiB's unbiased distillation on the fused tail (include/semseg_b200.h states the contract): student fp32 NHWC
+    [N,h,w,C] and teacher [N,h,w,C_old] maps (each with its own pixel pitch), both upsampled xzoom -> (kd_info [2] =
+    (KD, P), lse [N,Ho,Wo,3] = (lse_all(s), lse_B(s), lse(alpha t)) per pixel)."""
+    _require_cuda(student, teacher)
+    lib = _lib.load()
+    n, h, w, c, ps = _kd_map_meta(student)
+    shape_t = _kd_map_meta(teacher)
+    assert shape_t[:3] == (n, h, w), "student and teacher maps differ in shape"
+    ho, wo = int(zoom) * (h - 1) + 1, int(zoom) * (w - 1) + 1
+    nws = int(lib.semseg_upsample_unkd_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_unkd_workspace_floats")
+    dev = student.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    lse = torch.empty((n, ho, wo, 3), dtype=torch.float32, device=dev)
+    _lib.check(lib.semseg_upsample_unkd_fwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c, shape_t[3], ho,
+                                            wo, int(zoom), float(alpha), _ptr(ws), _ptr(info), _ptr(lse), _stream()),
+               "semseg_upsample_unkd_fwd")
+    return info, lse
+
+
+def upsample_unkd_bwd(student, teacher, alpha, kd_weight, lse, grad_out, dlogits, zoom=8):
+    """dlogits (fp32 [N,h,w,C], dense, already holding a gradient) += grad_out * d(kd_weight KD)/d student, in place;
+    returns dlogits."""
+    lib = _lib.load()
+    n, h, w, c, ps = _kd_map_meta(student)
+    shape_t = _kd_map_meta(teacher)
+    assert dlogits.shape == (n, h, w, c) and dlogits.dtype == torch.float32 and dlogits.is_contiguous()
+    ho, wo = int(zoom) * (h - 1) + 1, int(zoom) * (w - 1) + 1
+    nws = int(lib.semseg_upsample_unkd_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_unkd_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=student.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_unkd_bwd(_ptr(student), ps, _ptr(teacher), shape_t[4], n, h, w, c, shape_t[3], ho,
+                                            wo, int(zoom), float(alpha), float(kd_weight), _ptr(lse), _ptr(g),
+                                            _ptr(ws), _ptr(dlogits), _stream()),
+               "semseg_upsample_unkd_bwd")
+    return dlogits
+
+
 def upsample_ce_entropy_fwd(logits, target, ignore_index, want_argmax=True, zoom=8):
     """Entropy minimisation plus cross-entropy on the fused tail (include/semseg_b200.h states the contract); arguments as
     upsample_ce_fwd -> (loss_info [6] = (CE mean over L, |L|, H mean over U, |U|, 0, 1), argmax, lse, mu). mu fp32
