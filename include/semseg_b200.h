@@ -24,6 +24,8 @@
  *                               semseg_upsample_ce_dice_*: soft Dice loss, alone or plus cross-entropy.
  *                               semseg_upsample_ce_rmi_*: RMI loss with its BCE term, optionally plus cross-entropy.
  *                               semseg_upsample_ce_focal_*: softmax focal loss, with or without class weights.
+ *                               semseg_upsample_ce_relax_*: boundary label relaxation, with or without class
+ *                               weights.
  *                               semseg_upsample_ce_lovasz_*: Lovász-Softmax, alone or plus cross-entropy, on
  *                               semseg_segsort_u32_pairs (segmented stable radix sort).
  *                               semseg_upsample_kd_*: pixel-wise distillation from a teacher's logits.
@@ -607,6 +609,33 @@ int semseg_upsample_ce_focal_bwd(const float* logits, int pitch, int N, int h, i
                                  int Ho, int Wo, int zoom, int ignore_index, const float* lse, const float* mod,
                                  const float* loss_info, const float* grad_out, float* workspace, float* dlogits,
                                  void* stream);
+/* Boundary label relaxation (Zhu et al., CVPR 2019; semseg_b200/losses.py BoundaryRelaxationLoss) on the same fused
+ * upsample at zoom `zoom`. class_weight fp32 [C] on the device (NULL = all ones; read at every launch), border in
+ * [0, 4]. A label is valid when it is != ignore_index and in [0, C). For a valid pixel i, S_i is the set of valid labels
+ * in the (2 border + 1)^2 window of the target centred on i, clipped to the image; with p = softmax(v):
+ *   l_i = -log sum_{c in S_i} p_c,   omega_i = (1/|S_i|) sum_{c in S_i} w_c,   loss = sum_i omega_i l_i / D,
+ *   D = sum_i omega_i,   dl_i/dv_c = p_c - [c in S_i] p_c / (1 - R_i),   R_i = sum_{c not in S_i} p_c,
+ * loss 0 and an exactly zero gradient when D = 0. l_i is taken as log1p(e_R / e_S) from the two sums of exp and keeps
+ * its relative accuracy when small; it and its gradient are exactly 0 when S_i holds every class. The backward's
+ * staged rows take 12 bytes per pixel: the Dice width limit, Wo <= 229376 / (12 zoom), 2389 at zoom 8.
+ *   fwd: loss_out[0] = loss, loss_out[1] = D; argmax (or NULL) and lse as the zoom forward's (the same bits); sets int32
+ *        [semseg_upsample_ce_relax_sets_words()] = each pixel's label set (tag, omega, mask words) and lq fp32
+ *        [N,Ho,Wo] = log2(R / (1 - R)) per valid pixel, both kept for the backward; workspace:
+ *        semseg_upsample_ce_relax_workspace_floats() floats (the zoom forward's).
+ *   bwd: dlogits fp32 [N,h,w,C] = grad_out[0] * dloss/dlogits from the forward's lse, sets, lq and loss_out; workspace:
+ *        semseg_upsample_ce_relax_bwd_workspace_floats() floats (the zoom backward's).
+ * Both reject a bad shape, zoom, border, width, alignment or null pointer before any CUDA call; sets_words returns -1
+ * for a bad size. No host synchronisation (graph-capturable), no float atomics: deterministic. */
+long long semseg_upsample_ce_relax_workspace_floats(int N, int Ho, int Wo, int zoom);
+long long semseg_upsample_ce_relax_sets_words(int N, int Ho, int Wo, int C);
+int semseg_upsample_ce_relax_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target,
+                                 int Ho, int Wo, int zoom, int ignore_index, int border, const float* class_weight,
+                                 float* workspace, float* loss_out, int64_t* argmax, float* lse, int32_t* sets,
+                                 float* lq, void* stream);
+long long semseg_upsample_ce_relax_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom);
+int semseg_upsample_ce_relax_bwd(const float* logits, int pitch, int N, int h, int w, int C, int Ho, int Wo, int zoom,
+                                 const float* lse, const int32_t* sets, const float* lq, const float* loss_info,
+                                 const float* grad_out, float* workspace, float* dlogits, void* stream);
 /* The SegPGD attack loss (Gu et al., ECCV 2022; semseg_b200/adversarial.py) on the same fused upsample at zoom `zoom`.
  * Per valid pixel j (target != ignore_index, 0 <= target < C), with pred_j the first-maximum argmax of the upsampled
  * logits computed in the same pass and nll_j = lse_j - v_{j,target} (the plain forward's bits):

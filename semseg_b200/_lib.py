@@ -236,6 +236,13 @@ SIGNATURES = {
     "semseg_upsample_ce_focal_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
     "semseg_upsample_ce_focal_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                              c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_relax_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_relax_sets_words": (c_ll, [c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_relax_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
+                                             c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "semseg_upsample_ce_relax_bwd_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int]),
+    "semseg_upsample_ce_relax_bwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_vp,
+                                             c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_upsample_segpgd_fwd": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_int, c_int,
                                            c_f, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "semseg_upsample_ce_lovasz_workspace_floats": (c_ll, [c_int, c_int, c_int, c_int, c_int, c_int]),

@@ -3169,6 +3169,343 @@ upsample_ce_entropy_rows_kernel(const float* __restrict__ logits, int pitch, int
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- label relaxation
+// Boundary label relaxation (Zhu et al., CVPR 2019). S_i is the set of valid labels (target != ignore_index, in [0, C))
+// in the (2 border + 1)^2 window of the target grid centred on valid pixel i, clipped to the image; w the class weights
+// (all ones when none are given). With p = softmax(v), per valid pixel:
+//   l_i = -log sum_{c in S_i} p_c,   omega_i = (1/|S_i|) sum_{c in S_i} w_c,   loss = sum omega l / D,  D = sum omega
+//   dl_i/dv_c = p_c - [c in S_i] p_c / (1 - R_i),   R_i = sum_{c not in S_i} p_c
+// and loss 0 with an exactly zero gradient when D = 0.
+// Three passes:
+//   sets    : one thread per target pixel scans its window once and writes a tag (-1: not valid; t: interior, S = {t};
+//             kRelaxSet: boundary), omega, and for a boundary pixel its set as a bit mask of ceil(C/32) words. The
+//             window costs (2 border + 1)^2 target reads per pixel, hence the cap kRelaxMaxBorder.
+//   forward : the plain forward's two class passes (lse and argmax keep its bits); the second also sums the set's mass
+//             e_S and its complement e_R (e_c = ex2((v_c - m) log2e)), each term added to one sum, never subtracted. Then
+//             l = log1p(e_R / e_S) (= -log1p(-R), no rounded 1 - R: small losses keep their relative accuracy; 0 when
+//             S holds every class) and q = R / (1 - R) = e_R / e_S is kept as lq = log2 q for the backward. Where e_S
+//             has underflowed, l = lse - lse_S over the set's members and q = expm1(l) = exp(l) in fp32. The partials
+//             (sum omega l, sum omega) go to the weighted-mean reduce.
+//   backward: the rows layout with a 12-byte pixel word (the Dice width limit) holding the two exponent offsets
+//             a = lse log2e - log2 omega and b = a - lq: g = ex2(v log2e - a) = omega p_c outside the set and
+//             g = -ex2(v log2e - b) = -omega p_c q inside it (the in-set term p_c - p_c / (1 - R) without its
+//             cancellation), then the weighted-mean cols kernel. Membership is c == t for an interior pixel and one
+//             warp-uniform mask word (a warp's 32 classes) for a boundary one.
+constexpr int kRelaxSet = 1 << 30;    // tag of a boundary pixel (any value >= kMaxClasses)
+constexpr int kRelaxMaxBorder = 4;
+constexpr int kRelaxThreads = 256;
+
+__global__ void __launch_bounds__(kRelaxThreads)
+upsample_relax_sets_kernel(const long long* __restrict__ target, int N, int Ho, int Wo, int C, int ignore_index,
+                           int border, const float* __restrict__ class_weight, int* __restrict__ tag,
+                           float* __restrict__ omega, unsigned* __restrict__ mask) {
+  __shared__ unsigned s_mask[(kMaxClasses / 32) * kRelaxThreads];   // thread-private: word k at [k][tid]
+  const long long M = static_cast<long long>(N) * Ho * Wo;
+  const long long pix = static_cast<long long>(blockIdx.x) * kRelaxThreads + threadIdx.x;
+  if (pix >= M) return;
+  const long long t = target[pix];
+  if (t == ignore_index || t < 0 || t >= C) {
+    tag[pix] = -1;
+    omega[pix] = 0.f;
+    return;
+  }
+  const int nw = (C + 31) >> 5;
+  const int x = static_cast<int>(pix % Wo);
+  const long long ny = pix / Wo;
+  const int y = static_cast<int>(ny % Ho);
+  const long long* img = target + (ny / Ho) * Ho * Wo;
+  unsigned* sm = s_mask + threadIdx.x;
+  for (int k = 0; k < nw; ++k) sm[k * kRelaxThreads] = 0u;
+  bool interior = true;
+  const int ya = max(y - border, 0), yb = min(y + border, Ho - 1);
+  const int xa = max(x - border, 0), xb = min(x + border, Wo - 1);
+  for (int yy = ya; yy <= yb; ++yy) {
+    for (int xx = xa; xx <= xb; ++xx) {
+      const long long l = img[static_cast<size_t>(yy) * Wo + xx];
+      if (l == ignore_index || l < 0 || l >= C) continue;
+      const int li = static_cast<int>(l);
+      sm[(li >> 5) * kRelaxThreads] |= 1u << (li & 31);
+      interior = interior && l == t;
+    }
+  }
+  const int tc = static_cast<int>(t);
+  if (interior) {
+    tag[pix] = tc;
+    omega[pix] = class_weight ? class_weight[tc] : 1.f;
+    return;
+  }
+  // the weights summed in ascending class order; without weights omega = |S| / |S| = 1 exactly
+  unsigned* mk = mask + pix * nw;
+  float wsum = 0.f;
+  int cnt = 0;
+  for (int k = 0; k < nw; ++k) {
+    unsigned bits = sm[k * kRelaxThreads];
+    mk[k] = bits;
+    cnt += __popc(bits);
+    while (bits) {
+      const int c = 32 * k + __ffs(bits) - 1;
+      bits &= bits - 1;
+      wsum += class_weight ? class_weight[c] : 1.f;
+    }
+  }
+  tag[pix] = kRelaxSet;
+  omega[pix] = wsum / static_cast<float>(cnt);
+}
+
+// Mask word k (classes [32k, 32k + 32)) of a pixel's set from its tag: an interior pixel's is its label's bit.
+__device__ __forceinline__ unsigned relax_word(int tg, const unsigned* __restrict__ mask, size_t pix, int nw, int k) {
+  if (tg == kRelaxSet) return mask[pix * nw + k];
+  return tg >= 0 && (tg >> 5) == k ? 1u << (tg & 31) : 0u;
+}
+
+template <int Z>
+__global__ void __launch_bounds__(kFwdCols)
+upsample_relax_fwd_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Cs, int Ho,
+                          int Wo, const int* __restrict__ tag, const float* __restrict__ omega,
+                          const unsigned* __restrict__ mask, float* __restrict__ partial,
+                          long long* __restrict__ argmax_out, float* __restrict__ lse_out, float* __restrict__ lq_out) {
+  using G = Zoom<Z>;
+  constexpr int kFwdNodes = G::kNodes;
+  extern __shared__ float S[];  // [kNodeRows][kFwdNodes][Cs] as in upsample_ce_fwd_kernel
+  __shared__ float red_loss[kFwdCols / 32];
+  __shared__ float red_cnt[kFwdCols / 32];
+  const int n = blockIdx.z, i0 = blockIdx.y, x0 = blockIdx.x * kFwdCols;
+  const int i1 = min(i0 + 1, h - 1);
+  const int j_base = x0 >> G::kShift;
+  const int nj = min(kFwdNodes, w - j_base);
+  const int tid = threadIdx.x;
+  for (int idx = tid; idx < G::kNodeRows * nj * C; idx += kFwdCols) {
+    const int c = idx % C;
+    const int node = idx / C;
+    const int jj = node % nj, rr = node / nj;
+    S[(rr * kFwdNodes + jj) * Cs + c] =
+        logits[((static_cast<size_t>(n) * h + (rr ? i1 : i0)) * w + (j_base + jj)) * pitch + c];
+  }
+  __syncthreads();
+  float loss = 0.f, cnt = 0.f;
+  const int x = x0 + tid;
+  const int rows = min(Z, Ho - Z * i0);
+  if (x < Wo) {
+    const int j0 = x >> G::kShift;
+    const int j1 = min(j0 + 1, w - 1);
+    const float l1w = static_cast<float>(x & G::kMask) * G::kStep, l0w = 1.f - l1w;
+    const float* A = S + (j0 - j_base) * Cs;
+    const float* B = S + (j1 - j_base) * Cs;
+    const float* Cc = A + kFwdNodes * Cs;
+    const float* D = B + kFwdNodes * Cs;
+    const size_t pix0 = (static_cast<size_t>(n) * Ho + Z * i0) * Wo + x;   // row r: pix0 + r * Wo
+    const int nw = (C + 31) >> 5;
+    float m[Z], sum[Z], er[Z], es[Z];   // er, es: the complement's and the set's sums of e_c
+    int am[Z], tg[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      m[r] = -INFINITY;
+      am[r] = 0;
+      sum[r] = 0.f;
+      er[r] = 0.f;
+      es[r] = 0.f;
+      tg[r] = r < rows ? tag[pix0 + static_cast<size_t>(r) * Wo] : -1;
+    }
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+      const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) {
+        const float v = row_lerp<Z>(top, bot, r);
+        if (v > m[r]) {
+          m[r] = v;
+          am[r] = c;
+        }
+      }
+    }
+    float m2[Z];
+#pragma unroll
+    for (int r = 0; r < Z; ++r) m2[r] = m[r] * kLog2e;
+    for (int k = 0; k < nw; ++k) {
+      unsigned bits[Z];
+#pragma unroll
+      for (int r = 0; r < Z; ++r) bits[r] = relax_word(tg[r], mask, pix0 + static_cast<size_t>(r) * Wo, nw, k);
+      const int c_end = min(C, 32 * k + 32);
+#pragma unroll 2
+      for (int c = 32 * k; c < c_end; ++c) {
+        const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+        const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+#pragma unroll
+        for (int r = 0; r < Z; ++r) {
+          const float v = row_lerp<Z>(top, bot, r);
+          const float e = ex2_approx(fmaf(v, kLog2e, -m2[r]));
+          const bool in = bits[r] & 1u;
+          bits[r] >>= 1;
+          sum[r] += e;
+          er[r] += in ? 0.f : e;
+          es[r] += in ? e : 0.f;
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (r < rows) {
+        const size_t pix = pix0 + static_cast<size_t>(r) * Wo;
+        const float lse = m[r] + __logf(sum[r]);
+        if (argmax_out) argmax_out[pix] = am[r];
+        lse_out[pix] = lse;
+        float lq = 0.f;
+        if (tg[r] >= 0) {
+          float nll;
+          if (es[r] > kFocalMinEt) {
+            const float q = er[r] / es[r];
+            nll = log1pf(q);
+            lq = log2f(q);      // -inf when S holds all the mass: the in-set gradient is exactly 0
+          } else {
+            // lse_S over the set's members, against their own maximum
+            auto member_v = [&](int c) {
+              const float top = Z == 1 ? A[c] : l0w * A[c] + l1w * B[c];
+              const float bot = Z == 1 ? 0.f : l0w * Cc[c] + l1w * D[c];
+              return row_lerp<Z>(top, bot, r);
+            };
+            float ms = -INFINITY, ss = 0.f;
+            for (int k = 0; k < nw; ++k) {
+              for (unsigned b = relax_word(tg[r], mask, pix, nw, k); b; b &= b - 1) {
+                ms = fmaxf(ms, member_v(32 * k + __ffs(b) - 1));
+              }
+            }
+            for (int k = 0; k < nw; ++k) {
+              for (unsigned b = relax_word(tg[r], mask, pix, nw, k); b; b &= b - 1) {
+                ss += __expf(member_v(32 * k + __ffs(b) - 1) - ms);
+              }
+            }
+            nll = lse - (ms + __logf(ss));
+            lq = nll * kLog2e;
+          }
+          const float wgt = omega[pix];
+          loss = fmaf(wgt, nll, loss);
+          cnt += wgt;
+        }
+        lq_out[pix] = lq;
+      }
+    }
+  }
+  // deterministic block reduction -> one (sum of omega l, sum of omega) partial per CTA, as upsample_ce_fwd_kernel
+  for (int o = 16; o > 0; o >>= 1) {
+    loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  }
+  if ((tid & 31) == 0) {
+    red_loss[tid >> 5] = loss;
+    red_cnt[tid >> 5] = cnt;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    float l = 0.f, k = 0.f;
+    for (int i = 0; i < kFwdCols / 32; ++i) {
+      l += red_loss[i];
+      k += red_cnt[i];
+    }
+    const size_t b = (static_cast<size_t>(blockIdx.z) * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+    partial[2 * b] = l;
+    partial[2 * b + 1] = k;
+  }
+}
+
+struct RelaxPix {
+  float a;   // lse log2e - log2 omega: the exponent offset outside the set
+  int t;     // -1: no gradient; the label of an interior pixel; kRelaxSet: a boundary pixel
+  float b;   // a - log2 q: the exponent offset inside the set
+};
+static_assert(sizeof(RelaxPix) == 12, "the relaxation rows kernel stages the Dice words' 12 bytes per pixel");
+
+// One interval of the relaxation rows kernel for class c, folded as in upsample_ce_bwd_rows_kernel. mk_c points at the
+// mask word of class c of pixel 0; pix0 is the interval's first output row's first pixel.
+template <int Z, bool kFull>
+__device__ __forceinline__ void relax_interval(const RelaxPix* s, int Wo, int xb, int rows, int nx, int c,
+                                               const unsigned* __restrict__ mk_c, size_t pix0, int nw, float a,
+                                               float b, float cc, float d, float* acc) {
+  using G = Zoom<Z>;
+#pragma unroll
+  for (int k = 0; k < Z; ++k) {
+    if (!kFull && k >= nx) break;
+    const float l1w = G::kStep * k, l0w = 1.f - l1w;
+    const float top = l0w * a + l1w * b;
+    const float bot = l0w * cc + l1w * d;
+    float g0 = 0.f, g1 = 0.f;
+#pragma unroll
+    for (int r = 0; r < Z; ++r) {
+      if (!kFull && r >= rows) break;
+      const RelaxPix pi = s[r * Wo + xb + k];
+      if (pi.t < 0) continue;  // warp-uniform
+      const bool in = pi.t == kRelaxSet  // warp-uniform; the word is the same for the warp's 32 classes
+                          ? (mk_c[(pix0 + static_cast<size_t>(r) * Wo + xb + k) * nw] >> (c & 31)) & 1u
+                          : c == pi.t;
+      const float v = row_lerp<Z>(top, bot, r);
+      const float e = ex2_approx(fmaf(v, kLog2e, -(in ? pi.b : pi.a)));
+      const float g = in ? -e : e;
+      g0 = fmaf(1.f - G::kStep * r, g, g0);
+      g1 = fmaf(G::kStep * r, g, g1);
+    }
+    acc[0] = fmaf(l0w, g0, acc[0]);
+    acc[1] = fmaf(l1w, g0, acc[1]);
+    acc[2] = fmaf(l0w, g1, acc[2]);
+    acc[3] = fmaf(l1w, g1, acc[3]);
+  }
+}
+
+template <int Z>
+__global__ void __launch_bounds__(256)
+upsample_relax_rows_kernel(const float* __restrict__ logits, int pitch, int N, int h, int w, int C, int Ho, int Wo,
+                           const float* __restrict__ lse, const int* __restrict__ tag, const float* __restrict__ omega,
+                           const unsigned* __restrict__ mask, const float* __restrict__ lq, float* __restrict__ T2) {
+  extern __shared__ RelaxPix s_relax[];  // [Z][Wo]
+  const int i0 = blockIdx.x, n = blockIdx.y;
+  const int i1 = min(i0 + 1, h - 1);
+  const int rows = min(Z, Ho - Z * i0);
+  const size_t pix0 = (static_cast<size_t>(n) * Ho + Z * i0) * Wo;
+  for (int r = 0; r < rows; ++r) {
+    for (int x = threadIdx.x; x < Wo; x += blockDim.x) {
+      const size_t pix = pix0 + static_cast<size_t>(r) * Wo + x;
+      const int tg = tag[pix];
+      const float wgt = omega[pix];
+      RelaxPix pi;
+      pi.t = tg < 0 || wgt == 0.f ? -1 : tg;
+      pi.a = pi.t < 0 ? 0.f : lse[pix] * kLog2e - (wgt == 1.f ? 0.f : log2f(wgt));
+      pi.b = pi.t < 0 ? 0.f : pi.a - lq[pix];
+      s_relax[r * Wo + x] = pi;
+    }
+  }
+  __syncthreads();
+  const int c = threadIdx.x;
+  if (c >= C) return;
+  const int nw = (C + 31) >> 5;
+  const unsigned* mk_c = mask + (c >> 5);
+  const float* L0 = logits + (static_cast<size_t>(n) * h + i0) * w * pitch + c;
+  const float* L1 = logits + (static_cast<size_t>(n) * h + i1) * w * pitch + c;
+  float* T0 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 0) * w * C + c;
+  float* T1 = T2 + ((static_cast<size_t>(n) * h + i0) * 2 + 1) * w * C + c;
+  float a = L0[0], cc = L1[0];
+  float nb = L0[static_cast<size_t>(min(1, w - 1)) * pitch], nd = L1[static_cast<size_t>(min(1, w - 1)) * pitch];
+  float carry0 = 0.f, carry1 = 0.f;
+  for (int j0 = 0; j0 < w; ++j0) {
+    const float b = nb, d = nd;
+    const int jn = min(j0 + 2, w - 1);
+    nb = L0[static_cast<size_t>(jn) * pitch];
+    nd = L1[static_cast<size_t>(jn) * pitch];
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    const int xb = j0 * Z;
+    const int nx = min(Z, Wo - xb);
+    if (rows == Z && nx == Z) {
+      relax_interval<Z, true>(s_relax, Wo, xb, rows, nx, c, mk_c, pix0, nw, a, b, cc, d, acc);
+    } else {
+      relax_interval<Z, false>(s_relax, Wo, xb, rows, nx, c, mk_c, pix0, nw, a, b, cc, d, acc);
+    }
+    T0[static_cast<size_t>(j0) * C] = carry0 + acc[0];
+    T1[static_cast<size_t>(j0) * C] = carry1 + acc[2];
+    carry0 = acc[1];
+    carry1 = acc[3];
+    a = b;
+    cc = d;
+  }
+}
+
 }  // namespace sb
 
 using namespace sb;
@@ -4754,6 +5091,142 @@ extern "C" int semseg_upsample_ce_entropy_bwd(const float* logits, int pitch, in
                                          ce_weight, lse, mu, loss_info, grad_out, workspace, dlogits, stream);
     default: return launch_entropy_bwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, ent_weight,
                                           ce_weight, lse, mu, loss_info, grad_out, workspace, dlogits, stream);
+  }
+}
+
+// Boundary label relaxation at zoom factor `zoom`: the sets pass, its own forward and rows kernels, the weighted-mean
+// reduce and cols kernels. The rows kernel stages 12 bytes per pixel: the Dice width limit, Wo <= 2389 at zoom 8.
+// The per-pixel record `sets` (int32 words, M = N*Ho*Wo): tag[M], omega[M] (fp32), then ceil(C/32) mask words per pixel.
+static int check_relax(int zoom, int Wo, int border, const void* class_weight, const void* sets, const void* lq) {
+  SB_CHECK_ARG(border >= 0 && border <= kRelaxMaxBorder, "upsample_ce_relax: border %d is not in [0, %d]", border,
+               kRelaxMaxBorder);
+  SB_CHECK_ARG(((reinterpret_cast<uintptr_t>(class_weight) | reinterpret_cast<uintptr_t>(sets) |
+                 reinterpret_cast<uintptr_t>(lq)) & 3) == 0,
+               "upsample_ce_relax: class_weight, sets or lq not 4-byte aligned");
+  const size_t max_wo = kDiceSmemMax / (static_cast<size_t>(zoom) * sizeof(RelaxPix));
+  SB_CHECK_ARG(static_cast<size_t>(Wo) <= max_wo,
+               "upsample_ce_relax: output width %d too large for the staged rows (at most %d at zoom %d)", Wo,
+               static_cast<int>(max_wo), zoom);
+  return SEMSEG_OK;
+}
+
+struct RelaxSets {
+  int* tag;
+  float* omega;
+  unsigned* mask;
+};
+
+static RelaxSets relax_sets(int32_t* sets, int N, int Ho, int Wo) {
+  const size_t M = static_cast<size_t>(N) * Ho * Wo;
+  return {reinterpret_cast<int*>(sets), reinterpret_cast<float*>(sets + M), reinterpret_cast<unsigned*>(sets + 2 * M)};
+}
+
+template <int Z>
+static int launch_relax_fwd(const float* logits, int pitch, int N, int h, int w, int C, const int64_t* target, int Ho,
+                            int Wo, int ignore_index, int border, const float* class_weight, float* workspace,
+                            float* loss_out, int64_t* argmax, float* lse, int32_t* sets, float* lq,
+                            cudaStream_t stream) {
+  const RelaxSets rs = relax_sets(sets, N, Ho, Wo);
+  const long long M = static_cast<long long>(N) * Ho * Wo;
+  upsample_relax_sets_kernel<<<static_cast<unsigned>((M + kRelaxThreads - 1) / kRelaxThreads), kRelaxThreads, 0,
+                               stream>>>(reinterpret_cast<const long long*>(target), N, Ho, Wo, C, ignore_index, border,
+                                         class_weight, rs.tag, rs.omega, rs.mask);
+  SB_LAUNCHED();
+  const int Cs = C | 1;
+  constexpr size_t kMaxSmem =
+      static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * (kMaxClasses | 1) * sizeof(float);
+  const size_t smem = static_cast<size_t>(Zoom<Z>::kNodeRows) * Zoom<Z>::kNodes * Cs * sizeof(float);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_relax_fwd_kernel<Z>, attr_set, static_cast<int>(kMaxSmem));
+    if (r) return r;
+  }
+  upsample_relax_fwd_kernel<Z><<<dim3(cdiv(Wo, kFwdCols), h, N), kFwdCols, smem, stream>>>(
+      logits, pitch, N, h, w, C, Cs, Ho, Wo, rs.tag, rs.omega, rs.mask, workspace, reinterpret_cast<long long*>(argmax),
+      lse, lq);
+  SB_LAUNCHED();
+  upsample_ce_reduce_kernel<true><<<1, 256, 0, stream>>>(workspace, fwd_ctas(N, h, Wo), loss_out);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+template <int Z>
+static int launch_relax_bwd(const float* logits, int pitch, int N, int h, int w, int C, int Ho, int Wo,
+                            const float* lse, const int32_t* sets, const float* lq, const float* loss_info,
+                            const float* grad_out, float* workspace, float* dlogits, cudaStream_t stream) {
+  const RelaxSets rs = relax_sets(const_cast<int32_t*>(sets), N, Ho, Wo);
+  const int threads = (C + 31) / 32 * 32;
+  const size_t smem = static_cast<size_t>(Z) * Wo * sizeof(RelaxPix);
+  static std::atomic<bool> attr_set[64];
+  if (smem > kSmemDefault) {
+    int r = opt_in_smem(upsample_relax_rows_kernel<Z>, attr_set, static_cast<int>(kDiceSmemMax));
+    if (r) return r;
+  }
+  upsample_relax_rows_kernel<Z><<<dim3(h, N), threads, smem, stream>>>(logits, pitch, N, h, w, C, Ho, Wo, lse, rs.tag,
+                                                                       rs.omega, rs.mask, lq, workspace);
+  SB_LAUNCHED();
+  // loss_info[1] = D = sum of omega: the weighted cols kernel's 1 / D, 0 when D = 0
+  upsample_ce_bwd_cols_kernel<true><<<dim3(h, N), 256, 0, stream>>>(workspace, N, h, w, C, loss_info, grad_out,
+                                                                    dlogits);
+  SB_LAUNCHED();
+  return SEMSEG_OK;
+}
+
+extern "C" long long semseg_upsample_ce_relax_workspace_floats(int N, int Ho, int Wo, int zoom) {
+  return semseg_upsample_ce_zoom_workspace_floats(N, Ho, Wo, zoom);
+}
+
+extern "C" long long semseg_upsample_ce_relax_sets_words(int N, int Ho, int Wo, int C) {
+  SB_CHECK_ARG(N > 0 && Ho > 0 && Wo > 0 && C > 1 && C <= kMaxClasses, "upsample_ce_relax: bad sizes (C<=%d)",
+               kMaxClasses);
+  return (2LL + (C + 31) / 32) * N * Ho * Wo;
+}
+
+extern "C" int semseg_upsample_ce_relax_fwd(const float* logits, int pitch, int N, int h, int w, int C,
+                                            const int64_t* target, int Ho, int Wo, int zoom, int ignore_index,
+                                            int border, const float* class_weight, float* workspace, float* loss_out,
+                                            int64_t* argmax, float* lse, int32_t* sets, float* lq, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, target, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_relax(zoom, Wo, border, class_weight, sets, lq);
+  if (r) return r;
+  SB_CHECK_ARG(workspace && loss_out && lse && sets && lq, "upsample_ce_relax_fwd: null output");
+  switch (zoom) {
+    case 1: return launch_relax_fwd<1>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, border, class_weight,
+                                       workspace, loss_out, argmax, lse, sets, lq, stream);
+    case 2: return launch_relax_fwd<2>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, border, class_weight,
+                                       workspace, loss_out, argmax, lse, sets, lq, stream);
+    case 4: return launch_relax_fwd<4>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, border, class_weight,
+                                       workspace, loss_out, argmax, lse, sets, lq, stream);
+    default: return launch_relax_fwd<8>(logits, pitch, N, h, w, C, target, Ho, Wo, ignore_index, border, class_weight,
+                                        workspace, loss_out, argmax, lse, sets, lq, stream);
+  }
+}
+
+extern "C" long long semseg_upsample_ce_relax_bwd_workspace_floats(int N, int Ho, int w, int C, int zoom) {
+  return semseg_upsample_ce_zoom_bwd_workspace_floats(N, Ho, w, C, zoom);
+}
+
+extern "C" int semseg_upsample_ce_relax_bwd(const float* logits, int pitch, int N, int h, int w, int C, int Ho, int Wo,
+                                            int zoom, const float* lse, const int32_t* sets, const float* lq,
+                                            const float* loss_info, const float* grad_out, float* workspace,
+                                            float* dlogits, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int r = check_tail(logits, pitch, N, h, w, C, sets, Ho, Wo, zoom);
+  if (r) return r;
+  r = check_relax(zoom, Wo, 0, nullptr, sets, lq);
+  if (r) return r;
+  SB_CHECK_ARG(lse && lq && loss_info && grad_out && workspace && dlogits, "upsample_ce_relax_bwd: null pointer");
+  switch (zoom) {
+    case 1: return launch_relax_bwd<1>(logits, pitch, N, h, w, C, Ho, Wo, lse, sets, lq, loss_info, grad_out,
+                                       workspace, dlogits, stream);
+    case 2: return launch_relax_bwd<2>(logits, pitch, N, h, w, C, Ho, Wo, lse, sets, lq, loss_info, grad_out,
+                                       workspace, dlogits, stream);
+    case 4: return launch_relax_bwd<4>(logits, pitch, N, h, w, C, Ho, Wo, lse, sets, lq, loss_info, grad_out,
+                                       workspace, dlogits, stream);
+    default: return launch_relax_bwd<8>(logits, pitch, N, h, w, C, Ho, Wo, lse, sets, lq, loss_info, grad_out,
+                                        workspace, dlogits, stream);
   }
 }
 

@@ -641,6 +641,26 @@ class _UpsampleCEFocal(torch.autograd.Function):
         return dl, None, None, None, None, None
 
 
+class _UpsampleCERelaxed(torch.autograd.Function):
+    """The fused tail with losses.BoundaryRelaxationLoss at border > 0: the omega-weighted mean of -log of each valid
+    pixel's label-set mass. The forward keeps each pixel's label set and log2(R / (1 - R)); the backward needs nothing
+    else from the host. The class weights are read on the device at every launch and get no gradient."""
+
+    @staticmethod
+    def forward(ctx, logits, target, ignore_index, zoom, border, weight=None):
+        info, amax, lse, sets, lq = ops.upsample_ce_relax_fwd(logits, target, ignore_index, weight, border, zoom=zoom)
+        ctx.save_for_backward(logits, lse, sets, lq, info)
+        ctx.zoom = zoom
+        ctx.mark_non_differentiable(amax)
+        return info[0], amax
+
+    @staticmethod
+    def backward(ctx, grad_loss, _grad_amax):
+        logits, lse, sets, lq, info = ctx.saved_tensors
+        dl = ops.upsample_ce_relax_bwd(logits, lse, sets, lq, info, grad_loss, zoom=ctx.zoom)
+        return dl, None, None, None, None, None
+
+
 class _UpsampleSegPGD(torch.autograd.Function):
     """The fused tail with the SegPGD attack loss (adversarial.PGDAttack(kind='segpgd')): the mean over the valid pixels
     of w nll, w = 1 - lam where the argmax hits the target and lam elsewhere, the weights constants. The forward keeps
@@ -971,8 +991,9 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
     (2389 columns at zoom 8), and the Lovász loss fewer than 2^31 target pixels. losses.DistillationLoss takes the plain
     form's conditions, and so does losses.AdversarialLoss (plain cross-entropy on the attacked batch; the attack checks
     its own tail's limits); losses.PseudoLabelLoss and losses.MixPseudoLabelLoss, whose backward is the focal one, and
-    losses.EntropyLoss, whose rows kernel stages the same words, and losses.IncrementalLoss, whose unbiased CE and
-    distillation rows kernels stage as many bytes per pixel, the Dice width limit. losses.RMILoss needs a target of
+    losses.EntropyLoss, whose rows kernel stages the same words, losses.IncrementalLoss, whose unbiased CE and
+    distillation rows kernels stage as many bytes per pixel, and losses.BoundaryRelaxationLoss (at every border; its
+    class weights as the weighted form's), the Dice width limit. losses.RMILoss needs a target of
     at least 12 x 12 and no wider than its rows kernel stages (3584 columns
     at zoom 8). losses.GatedCRFLoss and losses.ActiveBoundaryLoss need the target no wider than the plain backward
     stages (2560 columns at zoom 8); their classes (<= 256, checked here with the logits) and options are in the
@@ -996,6 +1017,11 @@ def fused_tail_supported(criterion, logits, target, zoom_factor, x_size=None):
         # the kernels' limits
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
               _CRF_CE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _CRF_CE_STAGE_BYTES)
+    elif type(criterion) is losses.BoundaryRelaxationLoss:
+        # the relaxation rows kernel stages 12 bytes per pixel, the Dice words' size, at every border; border 0 runs
+        # the (weighted) cross-entropy kernels, whose limit is wider, and keeps the same decision
+        ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
+              _DICE_PIXEL_BYTES * zoom_factor * target.shape[2] <= _DICE_STAGE_BYTES)
     elif type(criterion) is losses.IncrementalLoss:
         # the unbiased CE and distillation rows kernels stage 12 bytes per pixel, the Dice words' size, in the same 224 KB
         ok = (zoom_factor in (1, 2, 4, 8) and target is not None and target.dim() == 3 and
@@ -1046,7 +1072,9 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
     losses.ActiveBoundaryLoss, ce_weight * CE plus abl_weight * its boundary term on the output grid. With a
     losses.IncrementalLoss and the previous step's fp32 NHWC logits `teacher_logits` ([N, h, w, C_old]), ce_weight *
     its unbiased CE plus kd_weight * its unbiased distillation; without them the unbiased CE alone (the aux head's
-    loss). The default criterion runs the plain kernels."""
+    loss). With a losses.BoundaryRelaxationLoss, its relaxed loss over each pixel's label set (its own ignore_index,
+    border and class weights; border 0 is the (weighted) cross-entropy step). The default criterion runs the plain
+    kernels."""
     if isinstance(criterion, losses.ActiveBoundaryLoss):
         if criterion.abl_weight == 0.0:
             # no ABL kernel: the plain step, bit for bit when ce_weight is 1
@@ -1095,6 +1123,18 @@ def upsample_ce(logits, target, ignore_index, zoom=8, criterion=None, teacher_lo
                                           criterion.gamma)
         return _UpsampleCEFocal.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.gamma,
                                       criterion.weight)
+    if isinstance(criterion, losses.BoundaryRelaxationLoss):
+        w = criterion.weight
+        if criterion.border == 0:
+            # every set is the pixel's own label: the (weighted) cross-entropy step, bit for bit
+            if w is None:
+                return _UpsampleCE.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom))
+            return _UpsampleCEWeighted.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), w, 0.0)
+        if w is None:
+            return _UpsampleCERelaxed.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                            criterion.border)
+        return _UpsampleCERelaxed.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom),
+                                        criterion.border, w)
     if isinstance(criterion, losses.RMILoss):
         return _UpsampleCERMI.apply(logits, target.contiguous(), criterion.ignore_index, int(zoom), criterion.bce_weight,
                                     criterion.pos_alpha, criterion.ce_weight)

@@ -4,8 +4,9 @@ OhemCrossEntropyLoss is online hard-pixel mining: only the pixels the network is
 the network's fused tail (functional.upsample_ce) it runs inside the same kernels as the default loss, graphed at every
 zoom factor; called as a module (validate(), or the network's tail when the fused one does not apply) it runs the
 zoom-1 form of those kernels on an NHWC copy of the logits. DiceLoss, the soft Dice loss alone or plus cross-entropy,
-LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, and FocalLoss, the softmax focal loss with
-optional class weights, run the same way, and so do RMILoss, the Region Mutual Information loss with its BCE term,
+LovaszSoftmaxLoss, the Lovász-Softmax loss alone or plus cross-entropy, FocalLoss, the softmax focal loss with
+optional class weights, and BoundaryRelaxationLoss, cross-entropy against the set of labels near each pixel, run the
+same way, and so do RMILoss, the Region Mutual Information loss with its BCE term,
 EntropyLoss, entropy minimisation on the unlabelled pixels plus cross-entropy on the labelled ones (TENT's objective,
 adapt.Tent), and GatedCRFLoss, cross-entropy plus the Gated CRF pairwise term for scribble- and point-supervised
 training, and ActiveBoundaryLoss, cross-entropy plus the Active Boundary Loss that moves predicted boundaries towards
@@ -221,6 +222,73 @@ class FocalLoss(nn.Module):
                                   and w.device == logits.device):
             raise ValueError("FocalLoss: weight must be contiguous fp32 [%d] on %s (no fallback), got %s [%d] on %s" %
                              (logits.shape[1], logits.device, w.dtype, w.numel(), w.device))
+        loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
+        return loss
+
+
+class BoundaryRelaxationLoss(nn.Module):
+    """Boundary label relaxation (Zhu et al., Improving Semantic Segmentation via Video Propagation and Label
+    Relaxation, CVPR 2019), for logits [N, C, H, W] and target [N, H, W]:
+
+        valid_j = target_j != ignore_index and 0 <= target_j < C
+        S_i     = {target_j : valid_j, j in the (2 border + 1)^2 square centred on i, clipped to the image}  (valid i)
+        p       = softmax(logits) over C
+        l_i     = -log sum_{c in S_i} p_ic
+        omega_i = (1/|S_i|) sum_{c in S_i} w_c                (w = weight, all ones without it)
+        loss    = sum over valid i of omega_i l_i / sum over valid i of omega_i
+
+    With a zero denominator the loss is 0 and every gradient is 0. A pixel whose window holds only its own label scores
+    plain cross-entropy, so border = 0 is exactly nn.CrossEntropyLoss(weight, ignore_index): the fused tail then runs
+    the cross-entropy step itself. The window lies on the target's grid (the fused tail's output grid). Ignored and
+    out-of-range neighbours, and positions outside the image, add no class. Under DistributedDataParallel each rank
+    averages over its own pixels.
+
+    Where this differs from the published NVIDIA code (its ImgWtLossSoftNLL): that code
+    drops every pixel within `border` of an ignored pixel or of the image edge, where this loss keeps those pixels with
+    the smaller set their window gives; and its optional per-image class weighting ("img_wt") is not offered here.
+
+    `border` is an int in [0, 4]: the window's (2 border + 1)^2 target reads per pixel bound the label-set pass's cost.
+    Changing it between steps (the "reduce the border after epoch k" schedule) captures a new training-step graph.
+    `weight` is a 1-D float tensor of one weight per class, registered as a buffer like nn.CrossEntropyLoss's (moved by
+    .cuda() / .to(), saved in the state_dict; without it there is no buffer). It gets no gradient. The native tail needs
+    it contiguous fp32 on the logits' device and reads it on the device at every launch, so in-place edits need no new
+    capture.
+
+    With the network's fused tail (functional.upsample_ce) it runs inside the tail's kernels, graphed at every zoom
+    factor, on both heads; called as a module (validate()) it runs their zoom-1 form on an NHWC copy of the logits.
+    CUDA fp32 logits with at most 256 classes only: there is no CPU or library fallback."""
+
+    graph_options = ("ignore_index", "border")
+
+    def __init__(self, border=1, weight=None, ignore_index=255):
+        super(BoundaryRelaxationLoss, self).__init__()
+        if isinstance(ignore_index, bool) or not isinstance(ignore_index, int):
+            raise TypeError("ignore_index must be an int, got %r" % (ignore_index,))
+        if isinstance(border, bool) or not isinstance(border, int):
+            raise TypeError("border must be an int, got %r" % (border,))
+        if not 0 <= border <= 4:
+            raise ValueError("border must lie in [0, 4], got %d" % border)
+        if weight is not None:
+            if not torch.is_tensor(weight) or not weight.is_floating_point():
+                raise TypeError("weight must be a floating-point tensor or None, got %r" % (weight,))
+            if weight.dim() != 1 or weight.numel() == 0:
+                raise ValueError("weight must be 1-D with one entry per class, got shape %s" % (tuple(weight.shape),))
+        self.border = border
+        self.ignore_index = ignore_index
+        self.register_buffer("weight", weight)
+
+    def extra_repr(self):
+        s = "border=%d, ignore_index=%d" % (self.border, self.ignore_index)
+        return s if self.weight is None else s + ", weight=[%d]" % self.weight.numel()
+
+    def forward(self, logits, target):
+        from . import functional as SF
+        _check_native_logits("BoundaryRelaxationLoss", logits, target)
+        w = self.weight
+        if w is not None and not (w.numel() == logits.shape[1] and w.dtype == torch.float32 and w.is_contiguous()
+                                  and w.device == logits.device):
+            raise ValueError("BoundaryRelaxationLoss: weight must be contiguous fp32 [%d] on %s (no fallback), got %s "
+                             "[%d] on %s" % (logits.shape[1], logits.device, w.dtype, w.numel(), w.device))
         loss, _ = SF.upsample_ce(logits.permute(0, 2, 3, 1).contiguous(), target, self.ignore_index, 1, criterion=self)
         return loss
 

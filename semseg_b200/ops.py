@@ -1024,6 +1024,51 @@ def upsample_ce_focal_bwd(logits, target, ignore_index, lse, mod, info, grad_out
     return dl
 
 
+def upsample_ce_relax_fwd(logits, target, ignore_index, weight, border, want_argmax=True, zoom=8):
+    """Boundary label relaxation on the fused tail (include/semseg_b200.h states the contract); arguments as
+    upsample_ce_fwd plus `weight` (fp32 [C] or None = all ones) and `border` in [0, 4] -> (loss_info [2] = (loss,
+    sum of the pixel weights), argmax, lse, sets, lq). sets int32: each pixel's label set; lq fp32 [N,Ho,Wo]: log2 of
+    R / (1 - R) per valid pixel; both are kept for the backward."""
+    _require_cuda(logits, target)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 4 and logits.stride(-1) == 1
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    _check_class_weight(weight, logits)
+    n, h, w, c = logits.shape
+    _, ho, wo = target.shape
+    nws = int(lib.semseg_upsample_ce_relax_workspace_floats(n, ho, wo, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_relax_workspace_floats")
+    nsets = int(lib.semseg_upsample_ce_relax_sets_words(n, ho, wo, c))
+    _lib.check(0 if nsets >= 0 else nsets, "semseg_upsample_ce_relax_sets_words")
+    dev = logits.device
+    ws = torch.empty((nws,), dtype=torch.float32, device=dev)
+    info = torch.empty((2,), dtype=torch.float32, device=dev)
+    amax = torch.empty((n, ho, wo), dtype=torch.int64, device=dev) if want_argmax else None
+    lse, lq = (torch.empty((n, ho, wo), dtype=torch.float32, device=dev) for _ in range(2))
+    sets = torch.empty((nsets,), dtype=torch.int32, device=dev)
+    _lib.check(lib.semseg_upsample_ce_relax_fwd(_ptr(logits), logits.stride(2), n, h, w, c, _ptr(target), ho, wo,
+                                                int(zoom), int(ignore_index), int(border), _ptr(weight), _ptr(ws),
+                                                _ptr(info), _ptr(amax), _ptr(lse), _ptr(sets), _ptr(lq), _stream()),
+               "semseg_upsample_ce_relax_fwd")
+    return info, amax, lse, sets, lq
+
+
+def upsample_ce_relax_bwd(logits, lse, sets, lq, info, grad_out, zoom=8):
+    lib = _lib.load()
+    n, h, w, c = logits.shape
+    _, ho, wo = lse.shape
+    dl = torch.empty((n, h, w, c), dtype=torch.float32, device=logits.device)
+    nws = int(lib.semseg_upsample_ce_relax_bwd_workspace_floats(n, ho, w, c, int(zoom)))
+    _lib.check(0 if nws >= 0 else nws, "semseg_upsample_ce_relax_bwd_workspace_floats")
+    ws = torch.empty((nws,), dtype=torch.float32, device=logits.device)
+    g = grad_out.reshape(1).float().contiguous()
+    _lib.check(lib.semseg_upsample_ce_relax_bwd(_ptr(logits), logits.stride(2), n, h, w, c, ho, wo, int(zoom),
+                                                _ptr(lse), _ptr(sets), _ptr(lq), _ptr(info), _ptr(g), _ptr(ws),
+                                                _ptr(dl), _stream()),
+               "semseg_upsample_ce_relax_bwd")
+    return dl
+
+
 def upsample_segpgd_fwd(logits, target, ignore_index, lam, want_argmax=True, zoom=8):
     """The SegPGD attack loss on the fused tail (include/semseg_b200.h states the contract); arguments as upsample_ce_fwd
     plus `lam` in [0, 1] -> (loss_info [2] = (loss, valid count), argmax, lse, mod). mod fp32 [N,Ho,Wo]: each pixel's
