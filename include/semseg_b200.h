@@ -40,6 +40,8 @@
  *                               (tool/test.py:139-141), the overlap accumulation and normalisation
  *                               (tool/test.py:163-176) and the per-scale resize into the running total
  *                               (tool/test.py:177, 202).
+ *                               semseg_window_scores_mc: the same scores averaged over Monte Carlo dropout draws,
+ *                               with the mean sample entropy.
  *   - semseg_anomaly_*        : anomaly segmentation on the evaluation scores (max-logit, energy, standardized
  *                               max-logit) and its AUROC / AP / FPR95, with semseg_window_scores_stats.
  *   - semseg_densecrf_*       : dense CRF refinement of the evaluation scores (pydensecrf's DenseCRF2D with a Gaussian
@@ -991,6 +993,16 @@ int semseg_window_resize_add(const double* canvas, int C, int Hi, int Wi, double
  * take the C + 2 channels unchanged. */
 int semseg_window_scores_stats(const float* logits, int pitch, int G, int h, int w, int C, int flip, float* out,
                                int crop_h, int crop_w, void* stream);
+/* window_scores_mc: Monte Carlo dropout scores. logits fp32 [T][G (+G mirrors when flip)][h][w][pitch] (T draws of one
+ * batch's low-resolution logits, each draw laid out as window_scores' input) -> out fp32 [G, C + 1, crop_h, crop_w]:
+ * channels 0..C-1 = (sum_t p_t) * (1/T), p_t draw t's flip-averaged scores with window_scores' arithmetic, summed in draw
+ * order; channel C = the same mean of the flip-averaged sample entropy H_t = log S - sum_c q_c (v_c - max) of the
+ * upsampled logits v (S = sum_c exp(v_c - max), q = the softmax). T = 1 gives score channels bit-identical to
+ * window_scores'. The upsampled logits are never stored; each element of out is written once; no atomics
+ * (deterministic). Same checks as window_scores, plus 1 <= T <= 128. window_accumulate and window_resize_add take the
+ * C + 1 channels unchanged. */
+int semseg_window_scores_mc(const float* logits, int pitch, int T, int G, int h, int w, int C, int flip, float* out,
+                            int crop_h, int crop_w, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Anomaly segmentation (semseg_b200/anomaly.py; csrc/anomaly.cu). No host synchronisation, no float atomics:

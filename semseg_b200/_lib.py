@@ -313,6 +313,8 @@ SIGNATURES = {
                                          c_int, c_int, c_int, c_vp, c_vp]),
     "semseg_window_resize_add": (c_int, [c_vp, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
     "semseg_window_scores_stats": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int, c_vp]),
+    "semseg_window_scores_mc": (c_int, [c_vp, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_vp, c_int, c_int,
+                                        c_vp]),
     "semseg_anomaly_class_moments_workspace_bytes": (c_ll, [c_ll, c_int]),
     "semseg_anomaly_class_moments": (c_int, [c_vp, c_vp, c_ll, c_int, c_vp, c_vp, c_vp]),
     "semseg_anomaly_sml_workspace_bytes": (c_ll, [c_int, c_int]),

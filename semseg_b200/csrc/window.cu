@@ -166,6 +166,136 @@ window_scores_kernel(const float* __restrict__ logits, int pitch, int G, int h, 
   }
 }
 
+constexpr int kMcRows = 2;                       // output rows per CTA (same node interval: 8 is even)
+constexpr int kMcThreads = kScoreCols * kMcRows; // one thread per output pixel
+constexpr int kMcMaxDraws = 128;
+
+// Monte Carlo dropout scores: T draws of a batch's low-resolution logits -> per crop the draw mean of the flip-averaged
+// softmax and of the flip-averaged sample entropy. One CTA per (64 output columns, 2 output rows, crop); a thread owns
+// one output pixel. Per draw the two node rows of each image are staged as in window_scores_kernel, and the three passes
+// over the classes (max, sum of exp, then q = exp(v - max) / sum) use its arithmetic, so each draw's flip-averaged score
+// is the bits window_scores_kernel writes. Pass 3 also forms the sample entropy from the max-shifted logits,
+// H = log S - sum_c q_c (v_c - max), taken as log S - (1/S) sum_c e_c (v_c - max) with e = exp(v - max): both terms
+// are >= 0, so a confident pixel keeps a small H accurate (log-sum-exp minus sum q v would cancel). The running draw
+// sums live in shared memory, [C][kMcThreads] (thread-contiguous: no bank conflicts, no atomics), the entropy sum in a
+// register; every element of `out` is written once, after the last draw, as sum * (1/T) (the sums start from draw 0's
+// value, so T = 1 writes window_scores' bits).
+// Shared memory: the node stage [image][node row][kScoreNodes][Cs], then the accumulators: <= 169 KB at C = 256.
+template <bool kFlip>
+__global__ void __launch_bounds__(kMcThreads)
+window_scores_mc_kernel(const float* __restrict__ logits, int pitch, int T, int G, int h, int w, int C, int Cs, int Ho,
+                        int Wo, float inv_t, float* __restrict__ out) {
+  extern __shared__ float S[];
+  constexpr int kImages = kFlip ? 2 : 1;
+  float* acc = S + kImages * 2 * kScoreNodes * Cs;
+  const int g = blockIdx.z, x0 = blockIdx.x * kScoreCols;
+  const int tid = threadIdx.x;
+  const int x = x0 + (tid % kScoreCols), y = kMcRows * blockIdx.y + tid / kScoreCols;
+  const int i0 = (kMcRows * blockIdx.y) >> 3;     // both rows of the CTA lie in this node interval
+  const int i1 = min(i0 + 1, h - 1);
+  const int x_last = min(x0 + kScoreCols, Wo) - 1;
+  const int jb0 = x0 >> 3;
+  const int jb1 = (Wo - 1 - x_last) >> 3;
+  const bool valid = x < Wo && y < Ho;
+  const int r = y & 7;
+  const float l1h = 0.125f * r, l0h = 1.f - 0.125f * r;
+  const float* P[kImages][4];
+  float l0w[kImages], l1w[kImages];
+#pragma unroll
+  for (int im = 0; im < kImages; ++im) {
+    const int xi = valid ? (im ? Wo - 1 - x : x) : x0;
+    const int jb = im ? jb1 : jb0;
+    const int j0 = xi >> 3, j1 = min(j0 + 1, w - 1);
+    l1w[im] = static_cast<float>(xi & 7) * 0.125f;
+    l0w[im] = 1.f - l1w[im];
+    const float* top = S + (im * 2) * kScoreNodes * Cs;
+    P[im][0] = top + (j0 - jb) * Cs;
+    P[im][1] = top + (j1 - jb) * Cs;
+    P[im][2] = P[im][0] + kScoreNodes * Cs;
+    P[im][3] = P[im][1] + kScoreNodes * Cs;
+  }
+  const size_t draw_stride = static_cast<size_t>(kImages) * G * h * w * pitch;
+  float hsum = 0.f;
+  for (int t = 0; t < T; ++t) {
+    const float* lt = logits + t * draw_stride;
+    __syncthreads();                            // the previous draw's stage is no longer read
+    for (int idx = tid; idx < kImages * 2 * kScoreNodes * C; idx += kMcThreads) {
+      const int c = idx % C;
+      const int node = idx / C;
+      const int jj = node % kScoreNodes, rr = (node / kScoreNodes) & 1, im = node / (2 * kScoreNodes);
+      const int j = (im ? jb1 : jb0) + jj;
+      if (j < w)
+        S[node * Cs + c] =
+            lt[((static_cast<size_t>(im * G + g) * h + (rr ? i1 : i0)) * w + j) * static_cast<size_t>(pitch) + c];
+    }
+    __syncthreads();
+    if (!valid) continue;
+    float mx[kImages], sum[kImages];
+#pragma unroll
+    for (int im = 0; im < kImages; ++im) {
+      mx[im] = -INFINITY;
+      sum[im] = 0.f;
+    }
+    // pass 1: max
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+#pragma unroll
+      for (int im = 0; im < kImages; ++im) {
+        const float top = lerp_aten(l0w[im], P[im][0][c], l1w[im], P[im][1][c]);
+        const float bot = lerp_aten(l0w[im], P[im][2][c], l1w[im], P[im][3][c]);
+        mx[im] = fmaxf(mx[im], lerp_aten(l0h, top, l1h, bot));
+      }
+    }
+    // pass 2: sum of exp(v - max)
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+#pragma unroll
+      for (int im = 0; im < kImages; ++im) {
+        const float top = lerp_aten(l0w[im], P[im][0][c], l1w[im], P[im][1][c]);
+        const float bot = lerp_aten(l0w[im], P[im][2][c], l1w[im], P[im][3][c]);
+        sum[im] += expf(lerp_aten(l0h, top, l1h, bot) - mx[im]);
+      }
+    }
+    float ent[kImages], rs[kImages];
+#pragma unroll
+    for (int im = 0; im < kImages; ++im) {
+      ent[im] = logf(sum[im]);
+      rs[im] = __fdividef(1.f, sum[im]);
+    }
+    // pass 3: scores into the draw sums, and sum_c exp(v - max) (v - max) per image. The flip average is rounded as
+    // the compiler contracts window_scores_kernel's (q + q_mirror) * 0.5: the mirror's product fused into the sum,
+    // fma(e_mirror, 1/S_mirror, q) * 0.5, written out so that it cannot contract otherwise here.
+    float ed[kImages];
+#pragma unroll
+    for (int im = 0; im < kImages; ++im) ed[im] = 0.f;
+#pragma unroll 2
+    for (int c = 0; c < C; ++c) {
+      float e[kImages];
+#pragma unroll
+      for (int im = 0; im < kImages; ++im) {
+        const float top = lerp_aten(l0w[im], P[im][0][c], l1w[im], P[im][1][c]);
+        const float bot = lerp_aten(l0w[im], P[im][2][c], l1w[im], P[im][3][c]);
+        const float d = lerp_aten(l0h, top, l1h, bot) - mx[im];
+        e[im] = expf(d);
+        ed[im] = fmaf(e[im], d, ed[im]);
+      }
+      const float p = kFlip ? fmaf(e[kImages - 1], rs[kImages - 1], __fmul_rn(e[0], rs[0])) * 0.5f
+                            : __fmul_rn(e[0], rs[0]);
+      float* a = acc + c * kMcThreads + tid;
+      *a = t ? *a + p : p;
+    }
+    // H = log S - (1/S) sum_c e_c d_c, both terms >= 0
+    float hs = ent[0] - rs[0] * ed[0];
+    if (kFlip) hs = (hs + (ent[kImages - 1] - rs[kImages - 1] * ed[kImages - 1])) * 0.5f;
+    hsum = t ? hsum + hs : hs;
+  }
+  if (!valid) return;
+  const size_t plane = static_cast<size_t>(Ho) * Wo;
+  float* o = out + static_cast<size_t>(g) * (C + 1) * plane + static_cast<size_t>(y) * Wo + x;
+  for (int c = 0; c < C; ++c) o[c * plane] = acc[c * kMcThreads + tid] * inv_t;
+  o[C * plane] = hsum * inv_t;
+}
+
 // Crop origins of one scale, per axis, ascending; passed by value (2 KB of kernel parameters).
 struct WindowGrid {
   int ny, nx;
@@ -276,6 +406,38 @@ extern "C" int semseg_window_scores_stats(const float* logits, int pitch, int G,
                                           float* out, int crop_h, int crop_w, void* stream) {
   return window_scores<true>("window_scores_stats", logits, pitch, G, h, w, C, flip, out, crop_h, crop_w,
                              static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int semseg_window_scores_mc(const float* logits, int pitch, int T, int G, int h, int w, int C, int flip,
+                                       float* out, int crop_h, int crop_w, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  SB_CHECK_ARG(logits && out, "window_scores_mc: null pointer");
+  SB_CHECK_ARG(T >= 1 && T <= kMcMaxDraws, "window_scores_mc: draws T=%d not in 1..%d", T, kMcMaxDraws);
+  SB_CHECK_ARG(G > 0 && h > 1 && w > 1 && h <= 65535 && G <= 65535 && C > 0 && C <= kWinMaxClasses && pitch >= C &&
+                   (flip == 0 || flip == 1),
+               "window_scores_mc: bad sizes (G=%d h=%d w=%d C=%d pitch=%d flip=%d; C<=%d, pitch>=C)", G, h, w, C, pitch,
+               flip, kWinMaxClasses);
+  SB_CHECK_ARG(crop_h == 8 * (h - 1) + 1 && crop_w == 8 * (w - 1) + 1,
+               "window_scores_mc: crop must be 8(h-1)+1 x 8(w-1)+1 of the %dx%d logits (got %dx%d)", h, w, crop_h,
+               crop_w);
+  const int Cs = C | 1;
+  const size_t smem = (static_cast<size_t>(flip ? 2 : 1) * 2 * kScoreNodes * Cs + static_cast<size_t>(C) * kMcThreads) *
+                      sizeof(float);   // <= 169 KB
+  const float inv_t = 1.f / static_cast<float>(T);
+  dim3 grid(cdiv(crop_w, kScoreCols), cdiv(crop_h, kMcRows), G);
+  if (flip) {
+    SB_CUDA(cudaFuncSetAttribute(window_scores_mc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(smem)));
+    window_scores_mc_kernel<true><<<grid, kMcThreads, smem, stream>>>(logits, pitch, T, G, h, w, C, Cs, crop_h, crop_w,
+                                                                      inv_t, out);
+  } else {
+    SB_CUDA(cudaFuncSetAttribute(window_scores_mc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 static_cast<int>(smem)));
+    window_scores_mc_kernel<false><<<grid, kMcThreads, smem, stream>>>(logits, pitch, T, G, h, w, C, Cs, crop_h,
+                                                                       crop_w, inv_t, out);
+  }
+  SB_LAUNCHED();
+  return SEMSEG_OK;
 }
 
 // Origins must start at 0, ascend strictly, end at extent - crop and leave no gap (every pixel covered).

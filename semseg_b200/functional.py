@@ -528,12 +528,15 @@ class _ConvBiasF32(torch.autograd.Function):
         return dx, dw, db, None
 
 
-def conv_bias_f32(x, conv):
+def conv_bias_f32(x, conv, out=None):
+    """1x1 conv + bias -> fp32 NHWC. `out` (inference only): a pixel-contiguous fp32 [N, H, W, cout] view to write
+    into, e.g. one draw's slice of a larger buffer."""
     assert conv.kernel_size == (1, 1) and conv.stride == (1, 1) and x.shape[-1] % 8 == 0
     if torch.is_grad_enabled() and (x.requires_grad or conv.weight.requires_grad):
+        assert out is None, "conv_bias_f32: out= is for the inference forward"
         return _ConvBiasF32.apply(x, conv.weight, conv.bias, conv)
     pw = packed(conv, need_dgrad=False, split=ops.is_split(x))
-    y, _ = ops.conv_fprop(x, pw.wf, pw.cout, ops.conv_taps(1, 1), epi=EPI_F32, shift=conv.bias)
+    y, _ = ops.conv_fprop(x, pw.wf, pw.cout, ops.conv_taps(1, 1), epi=EPI_F32, shift=conv.bias, out_f32=out)
     return y
 
 
@@ -1422,13 +1425,17 @@ def fp_fork(x, scale):
     return _FPFork.apply(x, scale)
 
 
+def dropout2d_scale(n, c, p, device):
+    """nn.Dropout2d's draw: fp32 [n, c], 0 or 1/(1-p) per (image, channel). dropout2d_nhwc and the Monte Carlo dropout
+    draws of the sliding-window predictor both take it from here, so one seed gives both the same masks."""
+    return torch.empty((n, c), device=device, dtype=torch.float32).bernoulli_(1.0 - p).mul_(1.0 / (1.0 - p))
+
+
 def dropout2d_nhwc(x, p, training):
     """nn.Dropout2d on NHWC: one Bernoulli per (n, c), kept channels scaled by 1/(1-p) (model/pspnet.py:68,76)."""
     if not training or p == 0.0:
         return x
-    n, c = x.shape[-4], x.shape[-1]
-    scale = torch.empty((n, c), device=x.device, dtype=torch.float32).bernoulli_(1.0 - p).mul_(1.0 / (1.0 - p))
-    return _ScaleNC.apply(x, scale)
+    return _ScaleNC.apply(x, dropout2d_scale(x.shape[-4], x.shape[-1], p, x.device))
 
 
 class _MaxPool3x3s2(torch.autograd.Function):

@@ -27,6 +27,13 @@ With an `anomaly` scorer (anomaly.AnomalyScorer) the exact=False finishes carry 
 steps: the flip-averaged max logit (ML) and logsumexp (LSE) of each crop's upsampled logits (csrc/window.cu's
 stats variant of the scores kernel, or torch amax / logsumexp in the ATen finish). The C score channels and the argmax
 are the same bits as without a scorer; the scorer turns ML, LSE or the scores into a per-pixel anomaly map.
+With `mc_draws` = T > 0 the predictor does Monte Carlo dropout (Gal & Ghahramani 2016; Kendall et al. 2017): every
+crop batch is scored under T dropout draws and the exact=False finish carries one more channel, the mean sample entropy
+E[H], through the same accumulation and resize. On the native path the network runs once per batch up to cls[2] and
+each draw is one masked 1x1 classifier (PSPNet._mc_eval_logits_nhwc); csrc/window.cu's MC variant of the scores kernel
+upsamples, soft-maxes, flip-averages and draw-averages them (the [T, 2G, classes, crop, crop] logits never exist).
+Any other model runs T forwards per batch with its dropout modules in training mode and the ATen steps. Both paths
+take the same Dropout2d masks in the same order, so one seed gives both the same draws.
 `net_process` / `scale_process` keep the reference's signatures and return types (and the exact arithmetic);
 `SlidingWindowPredictor` is the object form that also covers the per-image scale loop.
 
@@ -88,13 +95,29 @@ class SlidingWindowPredictor:
     """model: eval-mode network mapping [B, 3, crop_h, crop_w] -> [B, classes, h', w'] logits."""
 
     def __init__(self, model, classes, crop_h, crop_w, mean, std=None, stride_rate=2 / 3, flip=True, max_batch=32,
-                 crf=None, anomaly=None):
+                 crf=None, anomaly=None, mc_draws=0):
         """crf: None, or a densecrf.DenseCRF run on the scale-averaged scores before the argmax (both finishes); the
         returned scores are then its marginals.
         anomaly: None, or an anomaly.AnomalyScorer; __call__ then also returns its fp32 [h, w] CUDA anomaly map
-        (exact=False only; not together with crf)."""
+        (exact=False only; not together with crf).
+        mc_draws: 0 (deterministic), or T in 1..128 Monte Carlo dropout draws per crop; __call__ then returns the
+        predictive mean and an uncertainty map (exact=False only; not with crf, anomaly or an Fp8Eval model; the model
+        must hold a dropout layer with p > 0)."""
         from .anomaly import AnomalyScorer
         from .densecrf import DenseCRF
+        from .fp8 import Fp8Eval
+        if isinstance(mc_draws, bool) or not isinstance(mc_draws, (int, np.integer)):
+            raise TypeError("SlidingWindowPredictor: mc_draws must be an int, got %s" % type(mc_draws).__name__)
+        if not 0 <= int(mc_draws) <= 128:
+            raise ValueError("SlidingWindowPredictor: mc_draws must be in 0..128 (0 = off), got %d" % mc_draws)
+        self.mc_draws = int(mc_draws)
+        if self.mc_draws:
+            if crf is not None or anomaly is not None:
+                raise ValueError("SlidingWindowPredictor: mc_draws cannot be combined with crf or anomaly")
+            if isinstance(model, Fp8Eval):
+                raise ValueError("SlidingWindowPredictor: mc_draws does not support an Fp8Eval model")
+            if not any(isinstance(m, torch.nn.modules.dropout._DropoutNd) and m.p > 0 for m in model.modules()):
+                raise ValueError("SlidingWindowPredictor: mc_draws needs a model with a dropout layer of p > 0")
         if crf is not None and not isinstance(crf, DenseCRF):
             raise TypeError("SlidingWindowPredictor: crf must be None or a DenseCRF, got %s" % type(crf).__name__)
         if anomaly is not None and not isinstance(anomaly, AnomalyScorer):
@@ -123,19 +146,28 @@ class SlidingWindowPredictor:
             t = t / torch.tensor(self.std, dtype=torch.float32, device=self.device).view(3, 1, 1)
         return t.contiguous()
 
-    def _scores(self, crops, net=None, stats=False):
+    def _scores(self, crops, net=None, stats=False, mc=False):
         """[G, 3, ch, cw] normalised crops -> [G, classes, ch, cw] flip-averaged softmax scores (fp32). With `net` (see
         _native_net) the scores kernel writes each batch's scores straight into the result from the 1/8-resolution
         logits. With `stats` two more channels follow the scores: the flip-averaged max and logsumexp over the classes
-        of the upsampled logits."""
+        of the upsampled logits. With `mc` the scores are the mean over self.mc_draws dropout draws and one more
+        channel follows them: the mean flip-averaged sample entropy."""
         per_call = self.max_batch // 2 if self.flip else self.max_batch
+        if mc and net is None:
+            return self._mc_scores_aten(crops, per_call)
         if net is not None:
-            out = torch.empty((crops.shape[0], self.classes + (2 if stats else 0)) + tuple(crops.shape[2:]),
+            out = torch.empty((crops.shape[0], self.classes + (1 if mc else 2 if stats else 0)) + tuple(crops.shape[2:]),
                               dtype=torch.float32, device=crops.device)
             with torch.no_grad():
                 for g0 in range(0, crops.shape[0], per_call):
                     part = crops[g0:g0 + per_call]
-                    logits = net._eval_logits_nhwc(torch.cat([part, part.flip(3)], 0) if self.flip else part)
+                    batch = torch.cat([part, part.flip(3)], 0) if self.flip else part
+                    if mc:
+                        logits = net._mc_eval_logits_nhwc(batch, self.mc_draws)
+                        self.forward_calls += 1
+                        ops.window_scores_mc(logits, self.flip, out[g0:g0 + part.shape[0]])
+                        continue
+                    logits = net._eval_logits_nhwc(batch)
                     self.forward_calls += 1
                     ops.window_scores(logits, self.flip, out[g0:g0 + part.shape[0]], stats)
             return out
@@ -162,8 +194,43 @@ class SlidingWindowPredictor:
                 outs.append(prob)
         return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
 
+    def _mc_scores_aten(self, crops, per_call):
+        """The `mc` scores of _scores for any model: self.mc_draws forwards per batch with every dropout module of the
+        model in training mode (each module's own mode restored afterwards, also on an error), then the ATen steps:
+        upsample, softmax, sample entropy log S - sum_c q_c (v_c - max), flip average, draw mean."""
+        drops = [m for m in self.model.modules() if isinstance(m, torch.nn.modules.dropout._DropoutNd)]
+        modes = [m.training for m in drops]
+        outs = []
+        try:
+            for m in drops:
+                m.train()
+            with torch.no_grad():
+                for g0 in range(0, crops.shape[0], per_call):
+                    part = crops[g0:g0 + per_call]
+                    n = part.shape[0]
+                    batch = torch.cat([part, part.flip(3)], 0) if self.flip else part
+                    acc = None
+                    for _ in range(self.mc_draws):
+                        logits = self.model(batch)
+                        self.forward_calls += 1
+                        if logits.shape[2:] != batch.shape[2:]:
+                            logits = F.interpolate(logits, tuple(batch.shape[2:]), mode="bilinear", align_corners=True)
+                        lf = logits.float()
+                        prob = F.softmax(lf, dim=1)
+                        d = lf - lf.amax(1, keepdim=True)
+                        ent = torch.logsumexp(d, 1) - (prob * d).sum(1)
+                        sample = torch.cat([prob, ent[:, None]], 1)
+                        if self.flip:
+                            sample = (sample[:n] + sample[n:].flip(3)) * 0.5
+                        acc = sample if acc is None else acc + sample
+                    outs.append(acc * (1.0 / self.mc_draws))
+        finally:
+            for m, mode in zip(drops, modes):
+                m.train(mode)
+        return outs[0] if len(outs) == 1 else torch.cat(outs, 0)
+
     # ------------------------------------------------------------------------------------------- one scale
-    def _scale_canvas(self, image, net=None, stats=False):
+    def _scale_canvas(self, image, net=None, stats=False, mc=False):
         """Overlap-normalised scores of one rescaled image, un-padded: float64 [classes, img_h, img_w] on the device
         (tool/test.py:148-176: padding, crop grid, accumulation in grid order, division by the crop count). With `net`
         the scores and the accumulation run on the native kernels (contiguous result, same bits as the loop)."""
@@ -179,7 +246,7 @@ class SlidingWindowPredictor:
         windows = [(y0, x0) for y0 in ys for x0 in xs]
         x = self._normalised(image)
         crops = torch.stack([x[:, y0:y0 + ch, x0:x0 + cw] for y0, x0 in windows], 0)
-        scores = self._scores(crops, net, stats)
+        scores = self._scores(crops, net, stats, mc)
         if net is not None:
             return ops.window_accumulate(scores, ys, xs, (full_h, full_w), top, left, (img_h, img_w))
         canvas = torch.zeros((scores.shape[1], full_h, full_w), dtype=torch.float64, device=self.device)
@@ -197,27 +264,29 @@ class SlidingWindowPredictor:
         host = self._scale_canvas(image).permute(1, 2, 0).contiguous().cpu().numpy()
         return cv2.resize(host, (out_w, out_h), interpolation=cv2.INTER_LINEAR)
 
-    def scale_on_device(self, image, out_h, out_w, stats=False):
+    def scale_on_device(self, image, out_h, out_w, stats=False, mc=False):
         """Same scores as `scale`, float64 [classes, out_h, out_w], resized on the device (bilinear, half-pixel centres,
         no anti-aliasing = cv2.INTER_LINEAR's sampling; cv2 rounds its interpolation weights to fp32, so the two agree
         to ~1e-7, not bit for bit)."""
-        canvas = self._scale_canvas(image, stats=stats)
+        canvas = self._scale_canvas(image, stats=stats, mc=mc)
         return F.interpolate(canvas[None], size=(out_h, out_w), mode="bilinear", align_corners=False)[0]
 
     # ------------------------------------------------------------------------------------------- one image
-    def _stats_total(self, image, base_size, scales):
+    def _stats_total(self, image, base_size, scales, mc=False):
         """The exact=False finish with the two statistics channels: (total fp64 [classes + 2, h, w] on the device, the
-        scale average of the scores, ML and LSE; argmax int64 [h, w] of its score channels)."""
+        scale average of the scores, ML and LSE; argmax int64 [h, w] of its score channels). With `mc` the one MC
+        dropout channel instead: total [classes + 1, h, w], the predictive mean and the mean sample entropy E[H]."""
         h, w = image.shape[:2]
-        total = torch.zeros((self.classes + 2, h, w), dtype=torch.float64, device=self.device)
+        total = torch.zeros((self.classes + (1 if mc else 2), h, w), dtype=torch.float64, device=self.device)
         net = _native_net(self.model, self.classes, self.crop_h, self.crop_w, self.device)
+        stats = not mc
         for s in scales:
             new_h, new_w = scaled_size(h, w, round(s * base_size))
             resized = cv2.resize(image, (new_w, new_h), interpolation=cv2.INTER_LINEAR)
             if net is not None:
-                ops.window_resize_add(self._scale_canvas(resized, net, stats=True), total)
+                ops.window_resize_add(self._scale_canvas(resized, net, stats=stats, mc=mc), total)
             else:
-                total += self.scale_on_device(resized, h, w, stats=True)
+                total += self.scale_on_device(resized, h, w, stats=stats, mc=mc)
         total /= len(scales)
         return total, total[:self.classes].argmax(0)
 
@@ -232,7 +301,23 @@ class SlidingWindowPredictor:
         With a `crf`, the scale-averaged scores are refined by it on the device before the argmax, in both finishes,
         and the scores returned are its marginals (float64 [h, w, classes]).
         With an `anomaly` scorer the result is (scores, argmax, anomaly map fp32 [h, w] on the device); scores and
-        argmax are the same bits as without it. exact=True raises ValueError then."""
+        argmax are the same bits as without it. exact=True raises ValueError then.
+        With mc_draws = T > 0 the result is (scores, argmax, uncertainty): scores the MC predictive mean p_bar (float64
+        [h, w, classes], or None), argmax its argmax, uncertainty fp32 [2, h, w] on the device: channel 0 the predictive
+        entropy H[p_bar] = -sum_c p_bar log p_bar (0 log 0 = 0), channel 1 the mutual information H[p_bar] - E[H[p]]
+        (not clamped), both in nats. Every sample the predictor averages (T draws x the crop and its mirror x the
+        overlapping crops x the scales) enters p_bar and E[H] with the same weight, so the mutual information is the
+        Jensen gap over all of them: zero only where a pixel sees one sample (T = 1, no flip, one crop, one scale).
+        exact=True raises ValueError then."""
+        if self.mc_draws:
+            if exact:
+                raise ValueError("SlidingWindowPredictor: exact=True does not support mc_draws")
+            total, pred = self._stats_total(image, base_size, scales, mc=True)
+            pbar = total[:self.classes]
+            hbar = -torch.special.xlogy(pbar, pbar).sum(0)
+            uncertainty = torch.stack([hbar, hbar - total[self.classes]]).float()
+            scores = pbar.permute(1, 2, 0).contiguous().cpu().numpy() if return_scores else None
+            return scores, pred.cpu().numpy(), uncertainty
         if self.anomaly is not None:
             if exact:
                 raise ValueError("SlidingWindowPredictor: exact=True does not support an anomaly scorer")

@@ -1831,6 +1831,25 @@ def window_scores(logits, flip, out, stats=False):
     return out
 
 
+def window_scores_mc(logits, flip, out):
+    """Monte Carlo dropout scores (semseg_window_scores_mc): fp32 logits [T, G (+G mirrored crops when flip), h, w, C]
+    (each draw pixel-contiguous, channel pitch >= C) -> `out`, a contiguous fp32 [G, C + 1, 8(h-1)+1, 8(w-1)+1] tensor:
+    the draw mean of the flip-averaged softmax scores, then the draw mean of the flip-averaged sample entropy."""
+    _require_cuda(logits, out)
+    lib = _lib.load()
+    assert logits.dtype == torch.float32 and logits.dim() == 5 and logits.stride(4) == 1
+    t, n, h, w, c = logits.shape
+    pitch = logits.stride(3)
+    assert (logits.stride(2) == w * pitch and logits.stride(1) == h * logits.stride(2) and
+            logits.stride(0) == n * logits.stride(1)), "logits must be pixel-contiguous"
+    g = n // 2 if flip else n
+    assert not flip or n % 2 == 0, "flip needs the crops followed by their mirrors"
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 4 and tuple(out.shape[:2]) == (g, c + 1)
+    _lib.check(lib.semseg_window_scores_mc(_ptr(logits), pitch, t, g, h, w, c, int(bool(flip)), _ptr(out),
+                                           out.shape[2], out.shape[3], _stream()), "semseg_window_scores_mc")
+    return out
+
+
 def _int_array(vals):
     return (ctypes.c_int * len(vals))(*[int(v) for v in vals])
 

@@ -281,6 +281,22 @@ class _SegNet(nn.Module):
         assert not self.training, "_eval_logits_nhwc is the eval-mode forward"
         return self._logits_nhwc(x)[0]
 
+    def _mc_eval_logits_nhwc(self, x, draws):
+        """Monte Carlo dropout logits of the eval forward: fp32 NHWC [draws, N, h', w', classes], draw t bit-identical
+        to _eval_logits_nhwc(x) with cls[3] in training mode, the t-th such call under the same RNG state. The network
+        runs once up to cls[2] (the relation feature of _logits_nhwc); each draw takes Dropout2d's [N, 512] mask from
+        SF.dropout2d_scale, as that forward would, and runs the 1x1 classifier into its slice of the result."""
+        assert not self.training, "_mc_eval_logits_nhwc is the eval-mode forward"
+        with torch.no_grad():
+            _, f, _ = self._logits_nhwc(x, relation=True)
+            drop, conv = self.cls[3], self.cls[4]
+            n, h, w, c = (int(v) for v in f.shape[-4:])
+            out = torch.empty((draws, n, h, w, conv.out_channels), dtype=torch.float32, device=x.device)
+            for t in range(draws):
+                ft = f if drop.p == 0.0 else ops.scale_nc(f, SF.dropout2d_scale(n, c, drop.p, f.device))
+                SF.conv_bias_f32(ft, conv, out=out[t])
+        return out
+
 
 class PSPNet(_SegNet):
     def __init__(self, layers=50, bins=(1, 2, 3, 6), dropout=0.1, classes=2, zoom_factor=8, use_ppm=True,
